@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the lightning-pose hot path on B200 (driver contract: see the task statement).
+"""Benchmark of the lightning-pose hot path on H100.
 
 Workload = BASELINE.json configs[1]: ResNet-50 semi-supervised (temporal + PCA losses), synthetic
 384x384 video, 17 keypoints.  One *step* = one pass of the hot path over one batch of synthetic
@@ -39,7 +39,7 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"  # H100 SXM data sheet (dense)
 
 
 class ClockSampler:
@@ -155,15 +155,16 @@ BACKBONE_PARAMS = 23_508_032  # ResNet-50 trunk (SURVEY 8(e): 94.4 MB of fp32 gr
 
 
 class HotPath:
-    # our own kernel launches per step, counted from the committed launch lists (profiles/r02_launches_train_step.csv,
-    # profiles/r02_kineto_step.json); library kernels of torch (a dozen scalar element-wise ops, NCCL) are not counted
-    # per head call: preparation (packs + pads) + k1a + banded layer 2 (one two-pass softmax kernel from 148 frames up) +
+    # our own kernel launches per step, counted from the launch sites of the step's code path; library kernels of torch
+    # (a dozen scalar element-wise ops, NCCL) are not counted
+    # per head call: preparation (packs + pads) + k1a + banded layer 2 (one two-pass softmax kernel from 132 frames up) +
     # decode (warp kernel + queued CTA kernel) = 5;  labeled: + fused targets/MSE + its final reduction (2);
     # unlabeled: + remap + unsupervised losses (2)
     LAUNCHES_FWD = 2 * 5 + 2 + 2
     # unlabeled: unsup bwd, remap bwd, decode windows + dense fallback (4), then per head backward: preparation, plane dots,
-    # G2 front end, wgrad2, dgrad2, wgrad1, dgrad1 = 7, + the window patch pass (1);  labeled: targets/MSE bwd + the same 7
-    LAUNCHES_BWD = (4 + 7 + 1) + (1 + 7) + 1  # + the Adam step
+    # G2 front end, wgrad2, dgrad2, wgrad1, dgrad1 = 7, + the fixed-order sums of dW2, db2, db1, dW1 (4), + the window patch
+    # pass (1);  labeled: targets/MSE bwd + the same 7 + 4
+    LAUNCHES_BWD = (4 + 7 + 4 + 1) + (1 + 7 + 4) + 1  # + the Adam step
 
     def __init__(self, prob, device, fwd_only: bool, world: int = 1, ddp_payload_floats: int = 0, two_streams: bool = True):
         from lightning_pose_b200 import ops
@@ -243,9 +244,23 @@ class HotPath:
             if self.reducer is not None:
                 out = self.reducer.finish_step(scalars)  # head bucket (+ logged scalars) after the backward
                 self.opt.step()
+                self.last_out = out
                 return out
             self.opt.step()
-        return torch.stack(scalars)
+        self.last_out = torch.stack(scalars)
+        return self.last_out
+
+    def dump_outputs(self, out_dir: str, scalars: torch.Tensor) -> None:
+        """What the timed step hands its caller after the last timed step, as float32 .npy files: the four logged loss
+        scalars (total, supervised, temporal, PCA) and the head's parameters (updated by the Adam step) and gradients."""
+        os.makedirs(out_dir, exist_ok=True)
+        arrays = {"losses": scalars}
+        for name, p in self.head.named_parameters():
+            arrays[f"param.{name}"] = p
+            if p.grad is not None:
+                arrays[f"grad.{name}"] = p.grad
+        for name, t in arrays.items():
+            np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 class GraphedStep:
@@ -321,7 +336,7 @@ def time_steps(fn, steps, warmup, barrier=None):
 
 
 class L2Flusher:
-    """Writes a buffer larger than the 126 MB L2 between timed repetitions of a single stage."""
+    """Writes a buffer larger than the L2 (50 MB on an H100) between timed repetitions of a single stage."""
 
     def __init__(self, dev, mib: int = 256):
         self.buf = torch.empty(mib * 2**20 // 4, dtype=torch.float32, device=dev)
@@ -484,6 +499,8 @@ def run_ours(args):
             os.execv(sys.executable, [sys.executable] + sys.argv + ["--no-graph"])
     with ClockSampler(local) as clk:
         ms = time_steps(step_fn, args.steps, args.warmup, barrier)
+    if args.dump_outputs and rank == 0:
+        hp.dump_outputs(args.dump_outputs, step_fn.out if graphed else hp.last_out)
     t = torch.tensor([ms], device=dev)
     if dist:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -569,14 +586,6 @@ def run_ours(args):
         del flat_fn, hp_f, feats_f, prob_f
     # roofline: the stage with the largest measured share of the step
     dom = max(br, key=lambda k: br[k]["ms"])
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as fh:
-            per_frame = json.load(fh).get(dom, {}).get("dram_bytes_per_frame")
-            nfr = {"head_fwd": n_frames, "decode_fwd": n_frames, "head_bwd_unlabeled": n_frames - hp.n_clips * B_LABELED}.get(dom, hp.n_clips * B_LABELED)
-            traffic = per_frame * nfr if per_frame else None  # ncu --set full capture (profiles/), scaled to this launch
-    except Exception:
-        pass
     line = {
         "metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -584,7 +593,7 @@ def run_ours(args):
         "config": {
             "workload": f"BASELINE configs[1] hot path on ResNet-50 features (B,2048,12,12): {args.clips} clips/step/GPU x (16 labeled + 32 unlabeled) frames, "
                         f"K=17, heatmaps 96x96, decode field 384x384; pass = {'forward' if args.fwd_only else 'forward + backward + Adam step on the head (+ gradient all-reduce when N>1)'}",
-            "backward": "all native: loss stack, remap, sparse soft-argmax windows, target+mse, fused softmax-backward/G2 front end, tcgen05 dgrad+wgrad of both transposed convolutions; Adam step on the head parameters: one native launch (lpb_adam_step)",
+            "backward": "all native: loss stack, remap, sparse soft-argmax windows, target+mse, fused softmax-backward/G2 front end, tensor-core dgrad+wgrad of both transposed convolutions; Adam step on the head parameters: one native launch (lpb_adam_step)",
             "frames_per_step_per_gpu": n_frames, "regime": ("trained-like synthetic response (unimodal Gaussian-like heatmaps; planted features + bilinear per-keypoint deconvs, see bench.make_problem); fresh_init_regime = reference initialiser"
                                                                                   if args.regime == "trained" else "fresh init (reference initialiser, flat heatmaps)"),
             "launch": ("whole step replayed from one CUDA graph" if graphed else "eager launches")
@@ -599,7 +608,7 @@ def run_ours(args):
         "gpu_launches": (HotPath.LAUNCHES_FWD + (0 if args.fwd_only else HotPath.LAUNCHES_BWD)) * args.steps,
         "clocks": clk.summary(),
         "roofline": {"bound": "hbm", "kernel": f"{dom}: {br[dom]['what']}", "achieved": br[dom]["gbs"], "peak": pk["hbm_gbs"], "unit": "GB/s",
-                     "frac": br[dom]["gbs"] / pk["hbm_gbs"], "traffic": traffic, "peak_source": pk_src,
+                     "frac": br[dom]["gbs"] / pk["hbm_gbs"], "peak_source": pk_src,
                      "algorithmic_bytes_per_launch": br[dom]["algorithmic_bytes"], "launch_ms": br[dom]["ms"],
                      "selection": "arg-max of the per-stage device times below (each stage timed alone, median of 20 repetitions, L2 flushed before each)"},
         "stages": {k: {"ms": round(v["ms"], 4), "ms_mean": round(v["ms_mean"], 4), "GBps": round(v["gbs"], 1), "frac_hbm": round(v["gbs"] / pk["hbm_gbs"], 4)} for k, v in br.items()},
@@ -688,11 +697,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one returned (loss scalars, updated head parameters and "
+                         "their gradients) as DIR/<name>.npy (float32); the seeded inputs make runs with the same arguments comparable")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--clips", type=int, default=16, help="clips per step per GPU (48 frames each)")
     ap.add_argument("--regime", default="trained", choices=["trained", "fresh"], help="synthetic input regime (see make_problem)")
-    ap.add_argument("--dtype", default="bf16", choices=["f32", "bf16"], help="feature dtype (bf16 = tcgen05 head)")
+    ap.add_argument("--dtype", default="bf16", choices=["f32", "bf16"], help="feature dtype (bf16 = tensor-core head)")
     ap.add_argument("--no-flat", action="store_true", help="skip the secondary fresh-init (flat heatmap) regime")
     ap.add_argument("--fwd-only", action="store_true", help="time the forward pass only (default: full training step)")
     ap.add_argument("--no-cpu-baseline", action="store_true")

@@ -1,11 +1,11 @@
 #!/usr/bin/env bash
-# Build liblpb200.so (hand-written sm_100a CUDA behind a C ABI) in-tree.
+# Build liblpb200.so (hand-written sm_90a CUDA behind a C ABI) in-tree.
 set -euo pipefail
 cd "$(dirname "$0")"
 SRC=lightning_pose_b200/csrc
 OUT=lightning_pose_b200/liblpb200.so
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -O3)
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -O3)
 mkdir -p build
 objs=()
 pids=()

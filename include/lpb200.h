@@ -1,4 +1,4 @@
-/* lpb200 - C-ABI of the B200-native lightning-pose hot path (liblpb200.so, sm_100a only).
+/* lpb200 - C-ABI of the H100-native lightning-pose hot path (liblpb200.so, sm_90a only).
  *
  * Boundary contract
  *   - plain C: device pointers + sizes + a CUDA stream handle (cudaStream_t passed as void*);
@@ -36,7 +36,7 @@ extern "C" {
 /* library / build info -------------------------------------------------------------------- */
 int lpb_version(void);                /* e.g. 100 = 0.1.0 */
 const char* lpb_last_error(void);     /* message of the last failing call on this thread */
-const char* lpb_build_arch(void);     /* "sm_100a" */
+const char* lpb_build_arch(void);     /* "sm_90a" */
 
 /* kernel-variant switches: a bring-up / profiling aid (A/B two implementations of the same stage on the same inputs);
  * every variant computes the same results.  lpb_get_tuning returns -1 for an unknown key. */
@@ -46,14 +46,14 @@ const char* lpb_build_arch(void);     /* "sm_100a" */
 #define LPB_TUNE_DECODE_RING 3          /* 1: soft-argmax planes staged once in shared memory by a bulk-copy ring; 0 (default): warp per plane from global */
 #define LPB_TUNE_K1A_BULK_XS 4          /* 1: the saved operand copy leaves k1a by TMA bulk stores from the operand stage; 0 (default): producer stores */
 #define LPB_TUNE_DECODE_L2_HINTS 5      /* 1 (default): L2 evict_last / evict_first hints on the decode's two sweeps of a plane */
-#define LPB_TUNE_B3A_PREFETCH 6         /* 1 (default): b3a epilogue issues the next item's TMEM loads before storing the current one */
+#define LPB_TUNE_B3A_PREFETCH 6         /* 1 (default): b3a epilogue issues the next item's accumulator blocks before storing the current one */
 #define LPB_TUNE_SOFTMAX_SPLIT 7         /* 1 (default): plane softmax as two launches parallel over (frame, band) when there are fewer frames than SMs, else one per-frame two-pass kernel; 0: never split; 2: always */
 #define LPB_TUNE_DECODE_WARP_CTAS 8     /* > 0: resident CTAs per SM of the warp-per-plane decode are capped (fewer planes in flight than L2 holds); 0: no cap */
 #define LPB_TUNE_DECODE_REVERSE 9       /* 1: the decode walks the planes last-to-first (the producer's most recent writes are still in L2) */
 #define LPB_TUNE_B3A_TMA_STORE 10       /* 1 (default): b3a stages d features in shared memory and a TMA tensor store scatters them to NCHW; 0: direct 16-byte stores */
-#define LPB_TUNE_WGRAD_SWAP 11          /* layer-1 weight gradient: 1: A = features (M = 128 channels), B = gradient rows (N = 80); 2 (default): the same with the gradient rows staged twice, one row apart, side by side along N (N = 160: two shifts per MMA); 0: A = gradient rows */
+#define LPB_TUNE_WGRAD_SWAP 11          /* no effect in this build (accepted for compatibility): the weight gradient has one form */
 #define LPB_TUNE_G2_PATCH 12            /* 1 (default): decode windows enter the gradient rows in a patch pass (one warp per plane) after a look-up-free streaming pass; 0: look-ups fused into the streaming pass */
-#define LPB_TUNE_MMA_TILE_INNER 13      /* 1 (default; measured neutral): k1a issues its MMAs tile-innermost (consecutive MMAs accumulate into different TMEM tiles); 0: tile-outermost */
+#define LPB_TUNE_MMA_TILE_INNER 13      /* no effect in this build (accepted for compatibility): k1a has one MMA order */
 #define LPB_TUNE_DECODE_HINTS 14        /* 1: the fused two-pass softmax emits per-plane decode hints (arg max + largest value outside its 32x32 box) and the decode skips its plane sweeps when they allow; 0 (default): hints never produced (measured: what the decode saves, the issue-bound softmax epilogue pays) */
 #define LPB_TUNE_K1A_XS_COPY 15         /* k1a's saved operand copy: 2 (default): a dedicated extra warp sends each finished operand stage out with TMA bulk stores (the transposers store nothing); 1: streamed out of the finished stage by the transposer threads (whole sectors); 0: each transposer thread stores the rows it produced */
 #define LPB_TUNE_COUNT 16
@@ -156,10 +156,10 @@ int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* stream);
 int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
                       int Cout, float* grad_in, float* grad_w, float* grad_bias, void* stream);
 
-/* bf16 tensor-core path (tcgen05 / TMEM): features bf16 NCHW, fp32 master weights (rounded to bf16 on device, as
+/* bf16 tensor-core path (tensor-core mma): features bf16 NCHW, fp32 master weights (rounded to bf16 on device, as
  * autocast does), fp32 accumulate, fp32 heatmaps.  One-deconv heads (ViT family, heads/heatmap.py:192-193: pass
  * w2 = b2 = NULL, c2 = 0) and two-deconv heads (ResNet family); C % 128 == 0, H*W % 8 == 0, c1, c2 <= 20 (c1 < 20 for
- * two deconvs).  Two kernel families serve it: whole-frame-in-TMEM kernels for two-deconv heads on feature maps up to
+ * two deconvs).  Two kernel families serve it: whole-frame kernels for two-deconv heads on feature maps up to
  * 12x12 ("fast path"), and banded kernels for everything else (one-deconv heads, 16x16 / 24x24 ... maps).
  * lpb_head_bf16_plan reports which one a shape takes: plan[0] = 1 fast path, 0 banded (then saved_xs is REQUIRED by
  * lpb_head_fwd_bf16: it is the pixel-shuffled operand itself); LPB_ERR_UNSUPPORTED if neither fits. */
@@ -181,7 +181,7 @@ int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes);
 
 /* backward of lpb_head_fwd_bf16 (replaces autograd through heatmap.py:203-212 and, fused into its front end,
  * through spatial_softmax2d :211 and run_subpixelmaxima :103-144).  Kernels: gradient front end (G2 writer),
- * layer-2 wgrad, layer-2 dgrad, layer-1 wgrad, layer-1 dgrad + inverse PixelShuffle (all tcgen05).
+ * layer-2 wgrad, layer-2 dgrad, layer-1 wgrad, layer-1 dgrad + inverse PixelShuffle (all tensor-core).
  * The gradient w.r.t. the head OUTPUT [B, c2, 8H, 8W] is the sum of
  *   g_out        dense fp32 gradient (heatmap losses), or NULL
  *   win/win_meta/g_overflow   sparse soft-argmax gradient from lpb_decode_bwd_windows, or NULL/NULL/NULL
@@ -344,8 +344,9 @@ int lpb_unsup_losses_bwd(const float* keypoints, const float* confidences, int64
                          const float* grad_out, float* grad_keypoints, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------
- * UMMA descriptor self-test (tests only): one-CTA GEMM over operands in the library's row layout
- * [kchunk][row][8] bf16; mode 0 = K-major view, 1 = MN-major view; d [128][n] fp32. */
+ * Tensor-core operand self-test (bring-up aid): one-CTA GEMM over operands in the library's row layout
+ * [kchunk][row][8] bf16; mode 0 = K-major view, 1 = MN-major view; d [128][n] fp32.  col_off has no effect
+ * (kept for ABI compatibility). */
 int lpb_selftest_umma(const void* a, int kca, int rows_a, const void* b, int kcb, int rows_b, int mode, int n, int k,
                       int row_shift, int col_off, float* d, void* stream);
 

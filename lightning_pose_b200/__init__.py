@@ -1,4 +1,4 @@
-"""lightning_pose_b200 - B200-native (sm_100a) hot path of lightning-pose.
+"""lightning_pose_b200 - H100-native (sm_90a) hot path of lightning-pose.
 
 Mirrors the reference's module layout for the one path it accelerates, so that
 ``lightning_pose.models.heads.heatmap`` -> ``lightning_pose_b200.models.heads.heatmap`` etc.:

@@ -1,6 +1,6 @@
 """ctypes binding of ``liblpb200.so`` (the C-ABI declared in ``include/lpb200.h``).
 
-The library is hand-written sm_100a CUDA built in-tree by ``build.sh`` /
+The library is hand-written sm_90a CUDA built in-tree by ``build.sh`` /
 ``__graft_entry__.build()``.  There is no CPU implementation behind these symbols: if the shared
 object is missing, importing this module raises, and every wrapper in ``ops.py`` refuses non-CUDA
 tensors.

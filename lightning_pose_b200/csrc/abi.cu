@@ -7,7 +7,7 @@ const char* last_error_cstr();
 
 extern "C" int lpb_version(void) { return 100; }
 extern "C" const char* lpb_last_error(void) { return lpb::last_error_cstr(); }
-extern "C" const char* lpb_build_arch(void) { return "sm_100a"; }
+extern "C" const char* lpb_build_arch(void) { return "sm_90a"; }
 
 // Kernel-variant switches (profiling / bring-up aid; defaults are the measured-best variants).  Process-global, read at
 // launch time only.
@@ -24,9 +24,9 @@ int g_tuning[LPB_TUNE_COUNT] = {
     0,  // LPB_TUNE_DECODE_WARP_CTAS
     0,  // LPB_TUNE_DECODE_REVERSE
     1,  // LPB_TUNE_B3A_TMA_STORE
-    2,  // LPB_TUNE_WGRAD_SWAP (2: swapped + two shifts per MMA along N)
+    2,  // LPB_TUNE_WGRAD_SWAP (no effect)
     1,  // LPB_TUNE_G2_PATCH
-    1,  // LPB_TUNE_MMA_TILE_INNER
+    1,  // LPB_TUNE_MMA_TILE_INNER (no effect)
     0,  // LPB_TUNE_DECODE_HINTS (measured: decode 118 -> 52 us per 512 frames, but the bound costs the softmax epilogue +80 us: net zero)
     2,  // LPB_TUNE_K1A_XS_COPY (2: a dedicated warp sends the finished stage to the saved copy with TMA bulk stores)
 };

@@ -10,7 +10,7 @@
 //   H(x)[block] = L_k x[block] + h_k,   L_k = sum_f T_kf C_kf^T,   h_k = sum_f T_kf cb_kf + tb_k.
 // The recurrence therefore needs no convolution at all: per output frame, keypoint and 2x2 block it is five 4x4
 // matrix-vector steps per direction on the per-frame deconv maps WF[t] = W_f(x_t), WB[t] = W_b(x_t).  Those maps are
-// computed ONCE per frame by the head's tcgen05 GEMM (head_rows_bf16.cu) -- a frame that sits in five overlapping windows
+// computed ONCE per frame by the head's tensor-core GEMM (head_rows_bf16.cu) -- a frame that sits in five overlapping windows
 // of a video sequence is never duplicated (the reference tiles the features 5x, base.py:380-390) -- and the windows are
 // an index table idx[m][s] into them.  HBM-bound: 10 plane reads (mostly L2 hits between neighbouring windows) + 1 write.
 #include <cstdint>
@@ -289,7 +289,7 @@ extern "C" int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes
               "context_gather: bad arguments (odd context length, item size a multiple of 16 bytes)");
   const int64_t total = n * ctx * (item_bytes / 16);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;  // 32 CTAs per SM of an H100 SXM
   context_gather_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint4*>(seq), n, item_bytes / 16, ctx,
                                                                                         static_cast<uint4*>(out));
   LPB_CUDA(cudaGetLastError());

@@ -6,7 +6,7 @@
 //   (x, y) = sum p * (col, row);  conf = sum of the 5x5 window of p around (trunc y, trunc x)
 //   (x, y) -= {0.5, 1.5, 2.5}
 //
-// B200 design (DESIGN.md "K2"): one CTA per plane; the plane is staged ONCE into shared memory by
+// Design (DESIGN.md "K2"): one CTA per plane; the plane is staged ONCE into shared memory by
 // the TMA engine (cp.async.bulk, one copy per row into a zero-padded tile); the 4x-upsampled field
 // is never materialised: field = U_H h U_W^T is evaluated separably in registers (horizontal pass
 // from smem, vertical pass on a sliding register window with the phase-periodic interior weights

@@ -1,4 +1,5 @@
-// bf16 heatmap head on the 5th-gen tensor cores (tcgen05 + TMEM), two-deconv (ResNet-family) heads.
+// bf16 heatmap head on the tensor cores (mma.sync m16n8k16, fp32 accumulators in registers), two-deconv (ResNet-family)
+// heads.
 // Reference: lightning_pose/models/heads/heatmap.py:20-71 (layer stack), :203-212 (forward).
 //
 // Formulation ("4-shift GEMM").  A stride-2 3x3 transposed convolution in gather form:
@@ -8,14 +9,13 @@
 // m = Hi; then the four (dm,dn) shifts are the SAME matrix read from a start address moved by
 // (dm*(Wi+1) + dn) rows, and
 //   D[row, cls*20 + o] = sum_shift A_shift[row, :] . B_shift[cls*20 + o, :]
-// is an ordinary GEMM accumulated in TMEM over 4 shifts x K.  D needs no col2im: row (m,n), class
-// (py,px) IS output pixel (2m+py, 2n+px).  Operands use the K-major no-swizzle UMMA layout with
-// SBO = 128 B, where rows are linear in memory, so a row shift is just a different descriptor start
-// address (tcgen05.cuh).
+// is an ordinary GEMM accumulated over 4 shifts x K.  D needs no col2im: row (m,n), class
+// (py,px) IS output pixel (2m+py, 2n+px).  Operands use the K-major row layout (16-byte rows, linear
+// in memory), so a row shift is just a different ldmatrix start address (mma_sm90.cuh).
 //
 //   k1a: features (NCHW bf16) --[PixelShuffle folded into a transposing producer]--> smem A stages
-//        --tcgen05.mma--> TMEM --epilogue(+bias, ->bf16)--> mid activations in the A layout (global)
-//   k1b: mid (A layout, TMA bulk rows) --tcgen05.mma--> TMEM --epilogue--> two-pass plane softmax
+//        --mma.sync--> registers --epilogue(+bias, ->bf16)--> mid activations in the A layout (global)
+//   k1b: mid (A layout, TMA bulk rows) --mma.sync--> registers --epilogue--> two-pass plane softmax
 //        (pass 0: online max/sum, pass 1: recompute the cheap K=32 GEMM and write normalised fp32)
 #include <cuda_bf16.h>
 
@@ -27,7 +27,7 @@
 #include "head_rows.cuh"
 #include "lpb_common.cuh"
 #include "row_layout.cuh"
-#include "tcgen05.cuh"
+#include "mma_sm90.cuh"
 
 namespace lpb {
 
@@ -145,16 +145,21 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
 }
 
 int launch_head_prep(const PrepJobs& jobs, cudaStream_t s) {
-  head_prep_kernel<<<148 * 2, 256, 0, s>>>(jobs);
+  head_prep_kernel<<<132 * 2, 256, 0, s>>>(jobs);  // two CTAs per SM of an H100 SXM
   return LPB_OK;
 }
 
 // =====================================================================================================
 // k1a: PixelShuffle + first transposed convolution
 // =====================================================================================================
-// warps 0..TW-1 transposers, warp TW MMA issuer (+TMEM owner), warps TW+1..TW+4 epilogue, warp TW+5 TMA loader
+// warps 0..TW-1 transposers, warps TW..TW+CW-1 MMA + epilogue, warp TW+CW TMA loader (+ warp TW+CW+1: saved-copy stores)
+// A CTA works on (frame, tile group) items: the group's K1A_TPG M-tiles of 128 raster rows keep their fp32 accumulators in
+// the MMA warps' registers across all channel stages (warp = one tile's 32-row quarter, 80 columns = 80 registers).
 constexpr int K1A_TW = 4;                      // transposer warps
-constexpr int K1A_THREADS = 32 * (K1A_TW + 6);  // + MMA warp, 4 epilogue warps, TMA loader warp
+constexpr int K1A_TPG = 2;                     // M-tiles per item
+constexpr int K1A_CW = 4 * K1A_TPG;            // MMA warps
+constexpr int K1A_LOADER = K1A_TW + K1A_CW;
+constexpr int K1A_THREADS = 32 * (K1A_TW + K1A_CW + 1);
 constexpr int K1A_ASTAGES = 2;  // K-major operand stages (A + packed weights)
 constexpr int K1A_RSTAGES = 2;  // raw NCHW stages filled by the TMA engine
 constexpr int K1A_MAXPAD = 6;   // pad rows of the saved copy a transposer thread writes per stage (host falls back to head_prep beyond)
@@ -172,8 +177,8 @@ struct K1aParams {
   int backoff;                // idle warps sleep between barrier polls
   int xs_bulk;                // 1: the saved operand copy is written by TMA bulk stores straight from the operand stage
   int xs_pads;                // 1: the block transposers also write the saved copy's pad rows (else head_prep cleared them)
-  int tile_inner;             // 1: MMA issue order (shift, k16, tile) instead of (tile, shift, k16)
   int xs_copy;                // 1: the saved copy is streamed out of the finished operand stage by all transposer threads (coalesced)
+  int ntg;                    // tile groups per frame (items per frame); only group 0 writes the saved copy
   HeadGeom g;
 };
 
@@ -196,9 +201,6 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
   uint64_t* empty = bars + 2;                   // [2] MMAs reading the stage have completed
   uint64_t* raw_full = bars + 4;                // [2] TMA bytes landed
   uint64_t* raw_empty = bars + 6;               // [2] transposers are done with the raw stage
-  uint64_t* tmem_full = bars + 8;
-  uint64_t* tmem_empty = bars + 9;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 10);
   unsigned char* zreg = reinterpret_cast<unsigned char*>(bars) + 128;  // 1 KB of zeros: source of the saved copy's lead rows
   const bool xs_bulk = P.xs && P.xs_bulk;
 
@@ -210,33 +212,36 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&full[s], 32 * K1A_TW + 1);
-      mbar_init(&empty[s], (xs_bulk || XS == 3) ? 2 : 1);  // the MMAs have read the stage (+ the bulk stores of the saved copy have)
+      mbar_init(&empty[s], K1A_CW + ((xs_bulk || XS == 3) ? 1 : 0));  // the MMA warps have read the stage (+ the bulk stores of the saved copy have)
       mbar_init(&raw_full[s], 1);
       mbar_init(&raw_empty[s], 32 * K1A_TW);
     }
-    mbar_init(tmem_full, 1);
-    mbar_init(tmem_empty, 128);
     fence_mbar_init();
   }
-  if (warp == K1A_TW) tc::tmem_alloc(tmem_ptr, 512);
-  fence_proxy_async();  // generic-proxy zero fill -> visible to the async proxy (UMMA operand reads)
-  tc::fence_before_sync();
+  fence_proxy_async();  // generic-proxy zero fill -> visible to the async proxy (bulk stores of the saved copy)
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
 
   const int rows_mid = P.Lmid.rows;
-  int nframes = 0;
-  for (int b = blockIdx.x; b < P.B; b += gridDim.x) ++nframes;
-  const int total_it = nframes * P.nstages;
+  const int nitems = P.B * P.ntg;
+  int nmine = 0;
+  for (int item = blockIdx.x; item < nitems; item += gridDim.x) ++nmine;
+  const int total_it = nmine * P.nstages;
+  // item of pipeline iteration it: frame b, tile group tg (group 0 also writes the saved copy)
+  auto item_of = [&](int it, int& b, int& tg) {
+    const int item = blockIdx.x + (it / P.nstages) * gridDim.x;
+    b = item / P.ntg;
+    tg = item - b * P.ntg;
+  };
 
-  if (warp == K1A_TW + 5) {
+  if (warp == K1A_LOADER) {
     // ================= TMA loader: raw feature slabs run ahead, weights follow the operand slots ====
     if (lane == 0) {
       auto issue_raw = [&](int it) {
         const int r = it % K1A_RSTAGES;
         mbar_wait(&raw_empty[r], ((it / K1A_RSTAGES) & 1) ^ 1);
-        const int b = blockIdx.x + (it / P.nstages) * gridDim.x, st = it % P.nstages;
+        int b, tg;
+        item_of(it, b, tg);
+        const int st = it % P.nstages;
         mbar_expect_tx(&raw_full[r], (uint32_t)raw_bytes);
         bulk_g2s(raw_base + r * raw_bytes, P.feat + ((size_t)b * P.C + (size_t)st * 4 * HB_KSTAGE) * P.HW, (uint32_t)raw_bytes,
                  &raw_full[r]);
@@ -256,19 +261,22 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
           // 256-byte stride were k1a's critical path in training).  The stage is released once the MMAs AND these
           // stores have read it.
           mbar_wait(&full[s], (it / K1A_ASTAGES) & 1);
-          const int b = blockIdx.x + (it / P.nstages) * gridDim.x;
-          unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
-          const unsigned char* As = stage_base + s * stage_bytes;
-          const uint32_t lead_b = (uint32_t)P.Lxs.lead * 16, body_b = (uint32_t)(g.rows + g.P + 1) * 16;
+          int b, tg;
+          item_of(it, b, tg);
+          if (tg == 0) {
+            unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
+            const unsigned char* As = stage_base + s * stage_bytes;
+            const uint32_t lead_b = (uint32_t)P.Lxs.lead * 16, body_b = (uint32_t)(g.rows + g.P + 1) * 16;
 #pragma unroll
-          for (int kc = 0; kc < 4; ++kc) {
-            unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
-            bulk_s2g(dst, zreg, lead_b);
-            bulk_s2g(dst + lead_b, As + (size_t)kc * g.rows_alloc * 16, body_b);
+            for (int kc = 0; kc < 4; ++kc) {
+              unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
+              bulk_s2g(dst, zreg, lead_b);
+              bulk_s2g(dst + lead_b, As + (size_t)kc * g.rows_alloc * 16, body_b);
+            }
+            bulk_commit_group();
+            bulk_wait_group_read0();
           }
-          bulk_commit_group();
-          bulk_wait_group_read0();
-          tc::mbar_arrive(&empty[s]);
+          mbar_arrive(&empty[s]);
         }
       }
       if (xs_bulk) bulk_wait_group0();  // the copies are in global memory before the kernel ends
@@ -289,8 +297,10 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
       unsigned char* As = stage_base + s * stage_bytes;
       unsigned char* xs_st = nullptr;
       if (P.xs && !xs_bulk) {
-        const int b = blockIdx.x + (it / P.nstages) * gridDim.x, st = it % P.nstages;
-        xs_st = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
+        int b, tg;
+        item_of(it, b, tg);
+        const int st = it % P.nstages;
+        if (tg == 0) xs_st = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
       }
       const unsigned short* raw = reinterpret_cast<const unsigned short*>(raw_base + r * raw_bytes);
       for (int pr = warp; pr < npair; pr += K1A_TW) {
@@ -308,8 +318,8 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
         }
       }
       fence_proxy_async();
-      tc::mbar_arrive(&full[s]);
-      tc::mbar_arrive(&raw_empty[r]);
+      mbar_arrive(&full[s]);
+      mbar_arrive(&raw_empty[r]);
     }
   } else if (warp < K1A_TW) {
     // ================= transposers: raw NCHW slab (smem) -> K-major rows, PixelShuffle folded in ======
@@ -368,9 +378,11 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
       unsigned char* As = stage_base + s * stage_bytes;
       unsigned char* xs_st = nullptr;  // this (frame, stage)'s 4 K-chunks of the saved copy
       unsigned char* xs_cp = nullptr;  // copy-out form: the saved copy leaves through the operand stage (below)
-      if (XS != 0 && XS != 3 && P.xs && !xs_bulk) {
-        const int b = blockIdx.x + (it / P.nstages) * gridDim.x, st = it % P.nstages;
-        unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
+      int b_it, tg_it;
+      item_of(it, b_it, tg_it);
+      if (XS != 0 && XS != 3 && P.xs && !xs_bulk && tg_it == 0) {
+        const int st = it % P.nstages;
+        unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b_it * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
         if (XS == 2) xs_cp = slab;
         else xs_st = slab;
       }
@@ -407,8 +419,8 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
           if (k < npd) *reinterpret_cast<uint4*>(xs_st + t_pad[k]) = make_uint4(0, 0, 0, 0);
       }
       fence_proxy_async();
-      tc::mbar_arrive(&full[s]);
-      tc::mbar_arrive(&raw_empty[r]);
+      mbar_arrive(&full[s]);
+      mbar_arrive(&raw_empty[r]);
       if (xs_cp) {
         // Saved copy, copy-out form: the operand stage IS the copy's row layout (halo rows and zero columns included), so
         // once all four transposer warps have written it, the 128 threads stream it out with consecutive 16-byte rows per
@@ -438,96 +450,65 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
         }
       }
     }
-  } else if (XS == 3 && warp == K1A_TW + 6) {
+  } else if (XS == 3 && warp == K1A_LOADER + 1) {
     // ================= store warp: finished operand stage -> saved copy, by TMA bulk stores =========================
     if (lane == 0) {
       const uint32_t lead_b = (uint32_t)P.Lxs.lead * 16, body_b = (uint32_t)(g.rows + g.P + 1) * 16;
       for (int it = 0; it < total_it; ++it) {
         const int s = it % K1A_ASTAGES, st = it % P.nstages;
         mbar_wait(&full[s], (it / K1A_ASTAGES) & 1);
-        const int b = blockIdx.x + (it / P.nstages) * gridDim.x;
-        unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
-        const unsigned char* As = stage_base + s * stage_bytes;
+        int b, tg;
+        item_of(it, b, tg);
+        if (tg == 0) {
+          unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
+          const unsigned char* As = stage_base + s * stage_bytes;
 #pragma unroll
-        for (int kc = 0; kc < 4; ++kc) {
-          unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
-          bulk_s2g(dst, zreg, lead_b);
-          bulk_s2g(dst + lead_b, As + (size_t)kc * g.rows_alloc * 16, body_b);
+          for (int kc = 0; kc < 4; ++kc) {
+            unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
+            bulk_s2g(dst, zreg, lead_b);
+            bulk_s2g(dst + lead_b, As + (size_t)kc * g.rows_alloc * 16, body_b);
+          }
+          bulk_commit_group();
+          bulk_wait_group_read0();
         }
-        bulk_commit_group();
-        bulk_wait_group_read0();
-        tc::mbar_arrive(&empty[s]);
+        mbar_arrive(&empty[s]);
       }
       bulk_wait_group0();  // the copies are in global memory before the kernel ends
     }
-  } else if (warp == K1A_TW) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = tc::make_idesc_bf16_f32(128, HB_NCOLS);
+  } else if (warp < K1A_LOADER) {
+    // ================= MMA warps: tile t = tg * K1A_TPG + tt, accumulator rows [32 q, 32 q + 32) of it, all 80 columns ====
+    // epilogue: (+bias) -> bf16 -> mid activations (A layout); channel c1 of the mid activations is the constant 1 (lets
+    // the next layer fold its bias into the GEMM)
+    const int cw = warp - K1A_TW, q = cw & 3, tt = cw >> 2;
     const uint32_t lbo_a = g.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
     int it = 0;
-    uint32_t fph = 0;
-    for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
-      mbar_wait(tmem_empty, fph ^ 1);
-      tc::fence_after_sync();
+    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+      const int b = item / P.ntg, t = (item - b * P.ntg) * K1A_TPG + tt;
+      const bool active = t < g.tiles;
+      float acc[2][HB_NCOLS / 8][4];
+      mma::zero(acc);
       for (int st = 0; st < P.nstages; ++st, ++it) {
         const int s = it % K1A_ASTAGES;
         mbar_wait(&full[s], (it / K1A_ASTAGES) & 1);
-        tc::fence_after_sync();
-        {  // the whole warp, convergent: one elected lane issues (tc::umma_bf16_e)
+        if (active) {
           const uint32_t a0 = smem_u32(stage_base + s * stage_bytes);
           const uint32_t b0 = a0 + a_stage_bytes;
-          if (P.tile_inner) {
-            // issue order (shift, k16, tile): consecutive MMAs accumulate into different TMEM tiles
 #pragma unroll
-            for (int sh = 0; sh < 4; ++sh) {
-              const int shift_rows = (sh >> 1) * g.P + (sh & 1);
+          for (int sh = 0; sh < 4; ++sh) {
+            const int shift_rows = (sh >> 1) * g.P + (sh & 1);
 #pragma unroll
-              for (int k16 = 0; k16 < 2; ++k16) {
-                const uint64_t bd = tc::make_smem_desc(b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, 128);
-                const uint32_t aa0 = a0 + (2 * k16) * lbo_a + shift_rows * 16;
-                const uint32_t acc = (st | sh | k16) != 0 ? 1u : 0u;
-                for (int t = 0; t < g.tiles; ++t)
-                  tc::umma_bf16_e(tmem_u + t * HB_NCOLS, tc::make_smem_desc(aa0 + t * 2048, lbo_a, 128), bd, idesc, acc);
-              }
-            }
-          } else {
-          for (int t = 0; t < g.tiles; ++t) {
-#pragma unroll
-            for (int sh = 0; sh < 4; ++sh) {
-              const int shift_rows = (sh >> 1) * g.P + (sh & 1);
-#pragma unroll
-              for (int k16 = 0; k16 < 2; ++k16) {
-                const uint32_t aa = a0 + (2 * k16) * lbo_a + (t * 128 + shift_rows) * 16;
-                const uint32_t bb = b0 + (sh * 4 + 2 * k16) * lbo_b;
-                tc::umma_bf16_e(tmem_u + t * HB_NCOLS, tc::make_smem_desc(aa, lbo_a, 128), tc::make_smem_desc(bb, lbo_b, 128),
-                                idesc, (st | sh | k16) != 0 ? 1u : 0u);
-              }
-            }
+            for (int k16 = 0; k16 < 2; ++k16)
+              mma::kstep(acc, a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
           }
-          }
-          tc::umma_commit_e(&empty[s]);
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
       }
-      tc::umma_commit_e(tmem_full);
-      __syncwarp();
-      fph ^= 1;
-    }
-  } else {
-    // ================= epilogue: TMEM -> (+bias) -> bf16 -> mid activations (A layout) =================
-    // channel c1 of the mid activations is the constant 1 (lets the next layer fold its bias into the GEMM)
-    const int q = warp & 3;
-    uint32_t fph = 0;
-    for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
-      mbar_wait_idle(tmem_full, fph, P.backoff);
-      tc::fence_after_sync();
-      for (int t = 0; t < g.tiles; ++t) {
-        float d[HB_NCOLS];
+      if (!active) continue;
+      float d[HB_NCOLS];
 #pragma unroll
-        for (int cc = 0; cc < HB_NCOLS / 16; ++cc)
-          tc::tmem_ld16_async(tmem_base + ((uint32_t)(32 * q) << 16) + t * HB_NCOLS + cc * 16, &d[cc * 16]);
-        tc::tmem_ld_wait();
+      for (int nt = 0; nt < HB_NCOLS / 8; ++nt) mma::rows8(acc, nt, &d[nt * 8], lane);
+      {
         const int row = t * 128 + 32 * q + lane;
         const int m = row / g.P, n = row - m * g.P;
         if (m < g.Hi && n < g.Wi) {
@@ -562,23 +543,17 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
           }
         }
       }
-      tc::fence_before_sync();
-      tc::mbar_arrive(tmem_empty);
-      fph ^= 1;
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == K1A_TW) tc::tmem_dealloc(tmem_base, 512);
 }
 
 // =====================================================================================================
 // k1b: second transposed convolution + plane softmax (two CTAs per SM, half a frame resident at a time)
 // =====================================================================================================
-// warp 0 loader, warp 1 MMA issuer (+TMEM owner), warps 2-9 epilogue: lane quarter q = warp % 4,
-// output-row parity e = (warp - 2) / 4 (classes 2e, 2e+1 = TMEM columns [40e, 40e+40)).
+// warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue: row quarter q = warp % 4 of each 128-row M-tile,
+// output-row parity e = (warp - 2) / 4 (classes 2e, 2e+1 = accumulator columns [40e, 40e+40)).  The whole K (4 shifts x
+// 32 channels) of a half frame is resident, so a warp computes each 16-column block of its rows when its epilogue needs it.
 constexpr int K1B_THREADS = 320;
-constexpr int K1B_TPB = 3;      // M-tiles per batch (3 * 80 = 240 of the CTA's 256 TMEM columns)
 constexpr int K1B_EPI = 256;    // epilogue threads
 
 struct K1bParams {
@@ -603,31 +578,21 @@ __global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + 1;
   uint64_t* b_full = bars + 2;
-  uint64_t* t_full = bars + 3;
-  uint64_t* t_empty = bars + 4;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 5);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < a_bytes / 16; i += K1B_THREADS) reinterpret_cast<uint4*>(As)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     mbar_init(a_full, 1);
-    mbar_init(a_empty, 1);
+    mbar_init(a_empty, K1B_EPI / 32);
     mbar_init(b_full, 1);
-    mbar_init(t_full, 1);
-    mbar_init(t_empty, K1B_EPI);
     fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_ptr, 256);
   fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
 
   const int Hi = 2 * P.Hh, Wi = g.Wi;        // full conv-input image
   const int Ho = 2 * Hi, Wo = 2 * Wi;
   const int npix = Hi * Wi;
-  const int nbatch = (g.tiles + K1B_TPB - 1) / K1B_TPB;
   const int npass = P.final_softmax ? 2 : 1;
   const int nphase = 2 * npass;  // (pass, half)
 
@@ -652,50 +617,16 @@ __global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = tc::make_idesc_bf16_f32(128, HB_NCOLS);
-    const uint32_t lbo_a = g.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
-    const uint32_t a0 = smem_u32(As), b0 = smem_u32(Bs);
-    mbar_wait(b_full, 0);
-    int ph = 0, nb = 0;
-    for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
-      for (int phase = 0; phase < nphase; ++phase, ++ph) {
-        mbar_wait(a_full, ph & 1);
-        tc::fence_after_sync();
-        for (int bt = 0; bt < nbatch; ++bt, ++nb) {
-          mbar_wait(t_empty, (nb & 1) ^ 1);
-          tc::fence_after_sync();
-          if (lane == 0) {
-            for (int tt = 0; tt < K1B_TPB; ++tt) {
-              const int t = bt * K1B_TPB + tt;
-              if (t >= g.tiles) break;
-#pragma unroll
-              for (int sh = 0; sh < 4; ++sh) {
-                const int shift_rows = (sh >> 1) * g.P + (sh & 1);
-#pragma unroll
-                for (int k16 = 0; k16 < 2; ++k16) {
-                  const uint32_t aa = a0 + (2 * k16) * lbo_a + (t * 128 + shift_rows) * 16;
-                  const uint32_t bb = b0 + (sh * 4 + 2 * k16) * lbo_b;
-                  tc::umma_bf16(tmem_base + tt * HB_NCOLS, tc::make_smem_desc(aa, lbo_a, 128),
-                                tc::make_smem_desc(bb, lbo_b, 128), idesc, (sh | k16) != 0 ? 1u : 0u);
-                }
-              }
-            }
-            tc::umma_commit(t_full);
-            if (bt == nbatch - 1) tc::umma_commit(a_empty);  // every read of this half has completed
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else {
+  } else if (warp >= 2) {
     // ================= epilogue =================
     const int q = warp & 3, e = (warp - 2) >> 2;
     const int ew = warp - 2;  // 0..7
     const float L2E = 1.4426950408889634f;
     const size_t plane_stride = (size_t)Ho * Wo;
-    int nb = 0;
+    const uint32_t lbo_a = g.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
+    const uint32_t a0 = smem_u32(As), b0 = smem_u32(Bs);
+    mbar_wait(b_full, 0);
+    int ph = 0;
     for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
       float mx[HB_CLS], sm[HB_CLS];
 #pragma unroll
@@ -706,19 +637,27 @@ __global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const
       for (int phase = 0; phase < nphase; ++phase) {
         const int hf = phase & 1;
         const bool write = (phase >= nphase - 2);
-        for (int bt = 0; bt < nbatch; ++bt, ++nb) {
-          mbar_wait(t_full, nb & 1);
-          tc::fence_after_sync();
-          for (int tt = 0; tt < K1B_TPB; ++tt) {
-            const int t = bt * K1B_TPB + tt;
-            if (t >= g.tiles) break;
-            // columns [40e, 40e+40) = classes (py = e, px = 0|1) of this tile; TMEM loads stay 16-column
-            // aligned: read [32e, 32e+48) and pick with compile-time register indices
+        mbar_wait(a_full, ph & 1);
+        {
+          for (int t = 0; t < g.tiles; ++t) {
+            // columns [40e, 40e+40) = classes (py = e, px = 0|1) of this tile; computed in 16-column blocks [32e, 32e+48)
+            // and picked with compile-time register indices
             float d[48];
 #pragma unroll
-            for (int cc = 0; cc < 3; ++cc)
-              tc::tmem_ld16_async(tmem_base + ((uint32_t)(32 * q) << 16) + tt * HB_NCOLS + 32 * e + cc * 16, &d[cc * 16]);
-            tc::tmem_ld_wait();
+            for (int cc = 0; cc < 3; ++cc) {
+              float acc[2][2][4];
+              mma::zero(acc);
+#pragma unroll
+              for (int sh = 0; sh < 4; ++sh) {
+                const int shift_rows = (sh >> 1) * g.P + (sh & 1);
+#pragma unroll
+                for (int k16 = 0; k16 < 2; ++k16)
+                  mma::kstep(acc, a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
+                             b0 + (sh * 4 + 2 * k16) * lbo_b + (32 * e + 16 * cc) * 16, lbo_b, lane);
+              }
+              mma::rows8(acc, 0, &d[cc * 16], lane);
+              mma::rows8(acc, 1, &d[cc * 16 + 8], lane);
+            }
             const int row = t * 128 + 32 * q + lane;
             const int ml = row / g.P, n = row - ml * g.P;
             const bool valid = (ml < P.Hh) && (n < Wi);
@@ -755,8 +694,9 @@ __global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const
             if (e == 0) planes(std::integral_constant<int, 0>{});
             else planes(std::integral_constant<int, 1>{});
           }
-          tc::fence_before_sync();
-          tc::mbar_arrive(t_empty);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(a_empty);  // this warp's reads of the half are done
+          ++ph;
         }
         if (P.final_softmax && phase == 1) {
           // merge the online-softmax states: lanes -> warp (shuffles) -> 8 epilogue warps (smem)
@@ -787,9 +727,6 @@ __global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const
       }
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 256);
 }
 
 static size_t k1a_smem_bytes(const HeadGeom& g, int HW) {
@@ -810,14 +747,13 @@ __host__ inline HeadGeom make_half_geom(int Hh, int Wi) {
 }  // namespace lpb
 
 // ---- which kernels serve a shape ---------------------------------------------------------------------------
-// fast path (k1a + k1b): two-deconv heads whose whole frame fits the TMEM / shared-memory tiling above;
+// fast path (k1a + k1b): two-deconv heads whose whole frame fits the shared-memory tiling above;
 // generic path (head_rows_bf16.cu): everything else -- one-deconv heads, larger feature maps.
 static bool head_fast_path(int C, int H, int W, int c2, int max_smem) {
   using namespace lpb;
   if (c2 <= 0) return false;
   if (!((W >= 7 || W == 4 || W == 6) && H * W <= 192 && W <= 31)) return false;  // W <= 31: the saved copy's lead rows fit the 1 KB zero source
   const HeadGeom g1 = make_geom(2 * H, 2 * W), g2 = make_half_geom(2 * H, 4 * W);
-  if (g1.tiles * HB_NCOLS > 512) return false;
   return (int64_t)k1a_smem_bytes(g1, H * W) <= max_smem && (int64_t)k1b_smem_bytes(g2) <= max_smem;
 }
 
@@ -826,8 +762,8 @@ static int device_limits(int* max_smem, int* sms) {
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
       cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
     (void)cudaGetLastError();
-    *max_smem = 227 * 1024;  // sm_100a (also what a CPU-only caller sizing buffers should assume)
-    *sms = 148;
+    *max_smem = 227 * 1024;  // sm_90a (also what a CPU-only caller sizing buffers should assume)
+    *sms = 132;
   }
   return 0;
 }
@@ -841,7 +777,7 @@ extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan
   int max_smem, sms;
   device_limits(&max_smem, &sms);
   plan[0] = head_fast_path(C, H, W, c2, max_smem) ? 1 : 0;
-  if (!plan[0] && ((size_t)32 * H * W * 2 > 200 * 1024 || (c2 > 0 ? 4 : 2) * W + 1 > 384)) {
+  if (!plan[0] && ((size_t)32 * H * W * 2 > 200 * 1024 || (c2 > 0 ? 4 : 2) * W + 1 > CR_BAND_ROWS)) {
     set_error("head_bf16_plan: feature map %dx%d too large for this build", H, W);
     return LPB_ERR_UNSUPPORTED;
   }
@@ -982,17 +918,18 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
   pa.row_transposer = g_tuning[LPB_TUNE_K1A_ROW_TRANSPOSER];
   pa.backoff = g_tuning[LPB_TUNE_WAIT_BACKOFF];
   pa.xs_bulk = g_tuning[LPB_TUNE_K1A_BULK_XS];
-  pa.tile_inner = g_tuning[LPB_TUNE_MMA_TILE_INNER];
   pa.xs_copy = (g_tuning[LPB_TUNE_K1A_XS_COPY] && !pa.row_transposer && !pa.xs_bulk) ? 1 : 0;
   pa.xs_pads = k1a_pads ? 1 : 0;
   pa.g = g1;
+  pa.ntg = (g1.tiles + K1A_TPG - 1) / K1A_TPG;
   {
     // compile-time form of the saved copy (see the kernel): none / run-time forms / copy-out
     if (pa.xs_copy && Lxs.lead > 32 * K1A_TW) pa.xs_copy = 0;
     const int form = (!pa.xs || pa.row_transposer || pa.xs_bulk) ? (pa.xs || pa.row_transposer ? 1 : 0) : (g_tuning[LPB_TUNE_K1A_XS_COPY] == 2 ? 3 : (pa.xs_copy ? 2 : 1));
     auto kern = form == 0 ? k1a_shuffle_convt_kernel<0> : (form == 1 ? k1a_shuffle_convt_kernel<1> : (form == 2 ? k1a_shuffle_convt_kernel<2> : k1a_shuffle_convt_kernel<3>));
     LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s1));
-    kern<<<B < sms ? B : sms, K1A_THREADS + (form == 3 ? 32 : 0), s1, s>>>(pa);
+    const int items = B * pa.ntg;
+    kern<<<items < sms ? items : sms, K1A_THREADS + (form == 3 ? 32 : 0), s1, s>>>(pa);
   }
   if (g_tuning[LPB_TUNE_SOFTMAX_EPILOGUE_V2]) {
     // layer 2 on the banded kernel (head_rows_bf16.cu): same GEMM, leaner softmax epilogue

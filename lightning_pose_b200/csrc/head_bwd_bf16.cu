@@ -1,11 +1,11 @@
-// Backward of the bf16 heatmap head on tcgen05 (data gradients), mirroring head_bf16.cu.
+// Backward of the bf16 heatmap head on tensor-core (data gradients), mirroring head_bf16.cu.
 // Reference: autograd of lightning_pose/models/heads/heatmap.py:203-212 (PixelShuffle + 2 x ConvTranspose2d).
 //
 // Gradients travel in the "class-major row layout"  G[b][kchunk = k/8][row = m*Wi + n][8] bf16  with
 // k = cls*20 + o, cls = (py, px): row (m, n) carries, for every output class and channel, the gradient at
 // output pixel (2m+py, 2n+px).  In this layout the data gradient of a stride-2 3x3 transposed convolution
 //   d in[c, m', n'] = sum_{cls, (dm,dn) valid} G[(m'-dm, n'-dn)][(cls, o)] * W[c, o, ky, kx]
-// is again a 4-shift GEMM (negative row shifts of the same smem operand, tcgen05.cuh), K = 80:
+// is again a 4-shift GEMM (negative row shifts of the same smem operand, mma_sm90.cuh), K = 80:
 //   b2d: G2 (48x48 rows)  x W2  -> d mid (48x48 x 17)  written straight into G1 (24x24 rows) for the next stage
 //   b3a: W1 (M = 128 channels) x G1^T -> d Xs[c][row]   un-shuffled in the epilogue into d features (NCHW bf16)
 #include <cuda_bf16.h>
@@ -19,7 +19,7 @@
 
 #include "lpb_common.cuh"
 #include "row_layout.cuh"
-#include "tcgen05.cuh"
+#include "mma_sm90.cuh"
 
 namespace lpb {
 
@@ -324,7 +324,7 @@ static void launch_g2_build(const G2Src& S, int B, int C, int Hi, int Wi, __nv_b
 // =====================================================================================================
 // b2d: data gradient of the second deconv:  G2 -> d mid, emitted as G1 (+ bias gradient of layer 1)
 // =====================================================================================================
-constexpr int B2D_THREADS = 192;  // warp 0 loader, warp 1 MMA, warps 2-5 epilogue
+constexpr int B2D_THREADS = 192;  // warp 0 loader, warp 1 idle, warps 2-5 MMA + epilogue (K of a chunk is resident)
 constexpr int B2D_TILES = 3;       // M-tiles per chunk: R2 = 384 / (Wi + 1) image rows (7 * 49 = 343 raster rows at Wi = 48)
 
 struct B2dParams {
@@ -332,7 +332,7 @@ struct B2dParams {
   const __nv_bfloat16* wpk;   // [4][10][32][8]
   __nv_bfloat16* G1;          // [B][10][L1.rows][8] padded row layout of the (Hi/2 x Wi/2) grid
   RowLayout L2, L1;
-  float* db1;                 // [c1] accumulated with atomics (pre-zeroed)
+  float* db1_part;            // [gridDim.x * 4 MMA warps][GB_CLS]: each warp's bias-gradient sum (reduced in a fixed order)
   int B, Hi, Wi, c1;
   int R2;                     // image rows per chunk
 };
@@ -350,26 +350,17 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + 1;
   uint64_t* w_full = bars + 2;
-  uint64_t* t_full = bars + 3;
-  uint64_t* t_empty = bars + 4;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 5);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   for (int i = tid; i < a_bytes / 16; i += B2D_THREADS) reinterpret_cast<uint4*>(As)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     mbar_init(a_full, 1);
-    mbar_init(a_empty, 1);
+    mbar_init(a_empty, 4);  // one arrival per MMA warp
     mbar_init(w_full, 1);
-    mbar_init(t_full, 1);
-    mbar_init(t_empty, 128);
     fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_ptr, 128);
   fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
   const int B2D_ROWS = P.R2;
   const int nchunk = (Hi + B2D_ROWS - 1) / B2D_ROWS;
 
@@ -395,41 +386,11 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = tc::make_idesc_bf16_f32(128, 32);
+  } else if (warp >= 2) {
+    const int q = warp & 3;
     const uint32_t lbo_a = rows_alloc * 16, lbo_b = 32 * 16;
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
     const uint32_t a0 = smem_u32(As), b0 = smem_u32(Ws);
     mbar_wait(w_full, 0);
-    int it = 0;
-    for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
-      for (int ck = 0; ck < nchunk; ++ck, ++it) {
-        mbar_wait(a_full, it & 1);
-        mbar_wait(t_empty, (it & 1) ^ 1);
-        tc::fence_after_sync();
-        {  // whole warp, convergent; one elected lane issues (tcgen05.cuh)
-          for (int t = 0; t < B2D_TILES; ++t) {
-#pragma unroll
-            for (int sh = 0; sh < 4; ++sh) {
-              const int shift_rows = (sh >> 1) * Pp + (sh & 1);
-#pragma unroll
-              for (int k16 = 0; k16 < GB_K / 16; ++k16) {
-                if (k16 < sh) continue;  // all-zero weight chunks of this shift (see b3a)
-                const uint32_t aa = a0 + (2 * k16) * lbo_a + (LEAD + t * 128 - shift_rows) * 16;
-                const uint32_t bb = b0 + (sh * GB_KC + 2 * k16) * lbo_b;
-                tc::umma_bf16_e(tmem_u + t * 32, tc::make_smem_desc(aa, lbo_a, 128), tc::make_smem_desc(bb, lbo_b, 128), idesc,
-                                (sh | k16) != 0 ? 1u : 0u);
-              }
-            }
-          }
-          tc::umma_commit_e(t_full);
-          tc::umma_commit_e(a_empty);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    const int q = warp & 3;
     float dbs[GB_CLS];
 #pragma unroll
     for (int o = 0; o < GB_CLS; ++o) dbs[o] = 0.f;
@@ -437,13 +398,25 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
     for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
       for (int ck = 0; ck < nchunk; ++ck, ++it) {
         const int y0 = ck * B2D_ROWS, nrow = min(B2D_ROWS, Hi - y0);
-        mbar_wait(t_full, it & 1);
-        tc::fence_after_sync();
+        mbar_wait(a_full, it & 1);
         for (int t = 0; t < B2D_TILES; ++t) {
           float d[32];
+          {
+            float acc[2][4][4];
+            mma::zero(acc);
 #pragma unroll
-          for (int cc = 0; cc < 2; ++cc) tc::tmem_ld16_async(tmem_base + ((uint32_t)(32 * q) << 16) + t * 32 + cc * 16, &d[cc * 16]);
-          tc::tmem_ld_wait();
+            for (int sh = 0; sh < 4; ++sh) {
+              const int shift_rows = (sh >> 1) * Pp + (sh & 1);
+#pragma unroll
+              for (int k16 = 0; k16 < GB_K / 16; ++k16) {
+                if (k16 < sh) continue;  // all-zero weight chunks of this shift (see b3a)
+                mma::kstep(acc, a0 + (2 * k16) * lbo_a + (LEAD + t * 128 + 32 * q - shift_rows) * 16, lbo_a, b0 + (sh * GB_KC + 2 * k16) * lbo_b,
+                           lbo_b, lane);
+              }
+            }
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) mma::rows8(acc, nt, &d[8 * nt], lane);
+          }
           const int row = t * 128 + 32 * q + lane;
           const int ml = row / Pp, n = row - ml * Pp;
           if (ml < nrow && n < Wi) {
@@ -467,26 +440,23 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
             }
           }
         }
-        tc::fence_before_sync();
-        tc::mbar_arrive(t_empty);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(a_empty);
       }
     }
+    float* part = P.db1_part + ((size_t)blockIdx.x * 4 + q) * GB_CLS;
 #pragma unroll
     for (int o = 0; o < GB_CLS; ++o) {
-      if (o >= P.c1) break;
       const float s = warp_sum(dbs[o]);
-      if (lane == 0 && s != 0.f) atomicAdd(P.db1 + o, s);
+      if (lane == 0) part[o] = s;
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 128);
 }
 
 // =====================================================================================================
 // b3a: data gradient of the first deconv + inverse PixelShuffle:  G1 -> d features (NCHW bf16)
 // =====================================================================================================
-constexpr int B3A_THREADS = 320;  // warp 0 loader, warp 1 MMA, warps 2-9 epilogue (lane = channel, two warps per TMEM lane quarter)
+constexpr int B3A_THREADS = 320;  // warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue (lane = channel, two warps per 32-channel quarter)
 
 struct B3aParams {
   const __nv_bfloat16* G1;   // [B][10][L.rows][8] padded row layout
@@ -495,7 +465,7 @@ struct B3aParams {
   __nv_bfloat16* dfeat;      // [B][4*C4][(Hi/2)*(Wi/2)]
   int B, C4, Hi, Wi;         // shuffled-image geometry (Hi = 2H, Wi = 2W)
   int Hh;                    // image rows per band (multiple of 4)
-  int ncols;                 // TMEM columns per band = Hh * (Wi + 1) rounded up to 16 (<= 304; <= 256: double-buffered)
+  int ncols;                 // accumulator columns per band = Hh * (Wi + 1) rounded up to 16 (<= 304)
   int backoff, prefetch;
   int tma_store;             // 1: the epilogue stages bf16 rows in shared memory and a TMA tensor store writes them (below)
 };
@@ -512,8 +482,8 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, const void* 
 __device__ __forceinline__ void bulk_wait_group_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// A frame is processed in bands of Hh image rows (the accumulator of a band, N = Hh * (Wi + 1) pixels, must fit TMEM next
-// to nothing else; the band's gradient rows plus the halo row above are double-buffered in shared memory).
+// A frame is processed in bands of Hh image rows (N = Hh * (Wi + 1) accumulator columns per band; the band's gradient
+// rows plus the halo row above are double-buffered in shared memory).
 template <int WS2>
 __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_constant__ B3aParams P, const __grid_constant__ CUtensorMap TM) {
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -528,39 +498,23 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
   uint64_t* g_full = bars;       // [2]
   uint64_t* g_empty = bars + 2;  // [2]
   uint64_t* w_full = bars + 4;
-  uint64_t* t_full = bars + 5;   // [2]
-  uint64_t* t_empty = bars + 7;  // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 9);
   // staging slices of the TMA store: [ip & 1][pl][128 lanes][4 * WS2 bytes]
   unsigned char* Ss = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(bars + 12) + 127) & ~(uintptr_t)127);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntile = (P.C4 + 127) / 128;
-  // accumulator buffers: two when a band's columns fit twice into the 512 TMEM columns (the MMAs of band i + 1 then
-  // overlap the epilogue of band i), else one
-  const int nbuf = P.ncols <= 256 ? 2 : 1;
   const int mt = blockIdx.x % ntile, slot = blockIdx.x / ntile, nslot = gridDim.x / ntile;
 
   for (int i = tid; i < 2 * g_bytes / 16; i += B3A_THREADS) reinterpret_cast<uint4*>(Gs)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     for (int st = 0; st < 2; ++st) {
       mbar_init(&g_full[st], 1);
-      mbar_init(&g_empty[st], 1);
+      mbar_init(&g_empty[st], 8);  // one arrival per MMA warp
     }
     mbar_init(w_full, 1);
-    for (int st = 0; st < 2; ++st) {
-      mbar_init(&t_full[st], 1);
-      mbar_init(&t_empty[st], 256);
-    }
     fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_ptr, 512);
   fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int n0 = P.ncols > 256 ? 160 : P.ncols;  // first MMA's N; the rest goes into a second MMA
-  const int n1 = P.ncols - n0;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -582,71 +536,51 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
                    P.G1 + (((size_t)b * GB_KC + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, &g_full[st]);
         }
       }
-  } else if (warp == 1) {
-    const uint32_t idesc0 = tc::make_idesc_bf16_f32(128, n0);
-    const uint32_t idesc1 = n1 > 0 ? tc::make_idesc_bf16_f32(128, n1) : 0u;
-    const uint32_t lbo_g = rows_alloc * 16, lbo_w = 128 * 16;
-    const uint32_t w0 = smem_u32(Ws);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    mbar_wait(w_full, 0);
-    int it = 0;
-    for (int b = slot; b < P.B; b += nslot)
-      for (int band = 0; band < nbands; ++band, ++it) {
-        const int st = it & 1;
-        const int tb = it % nbuf, tph = (it / nbuf) & 1;
-        const uint32_t dcol = tmem_u + tb * 256;
-        mbar_wait(&g_full[st], (it >> 1) & 1);
-        mbar_wait(&t_empty[tb], tph ^ 1);
-        tc::fence_after_sync();
-        {  // whole warp, convergent; one elected lane issues (tcgen05.cuh)
-          const uint32_t g0 = smem_u32(Gs + (size_t)st * g_bytes);
-#pragma unroll
-          for (int sh = 0; sh < 4; ++sh) {
-            const int shift_rows = (sh >> 1) * Pp + (sh & 1);
-#pragma unroll
-            for (int k16 = 0; k16 < GB_K / 16; ++k16) {
-              // K = (cls, o), cls = 2 py + px at stride 20: shift (dm, dn) has no tap for classes with py < dm or px < dn,
-              // so its packed weights are zero for k < 20 (dn), k < 40 (dm), k < 60 (both): the 16-wide chunks k16 < sh
-              // are all-zero and their MMAs are skipped (14 of 20 remain)
-              if (k16 < sh) continue;
-              const uint32_t ww = w0 + ((sh * GB_KC + 2 * k16) * 128) * 16;
-              const uint32_t gg = g0 + (2 * k16) * lbo_g + (LEAD - shift_rows) * 16;
-              const uint64_t wd = tc::make_smem_desc(ww, lbo_w, 128);
-              tc::umma_bf16_e(dcol, wd, tc::make_smem_desc(gg, lbo_g, 128), idesc0, (sh | k16) != 0 ? 1u : 0u);
-              if (n1 > 0)
-                tc::umma_bf16_e(dcol + n0, wd, tc::make_smem_desc(gg + n0 * 16, lbo_g, 128), idesc1, (sh | k16) != 0 ? 1u : 0u);
-            }
-          }
-          tc::umma_commit_e(&t_full[tb]);
-          tc::umma_commit_e(&g_empty[st]);
-        }
-        __syncwarp();
-      }
-  } else {
-    // Epilogue.  Thread = shuffled channel c (TMEM lane); shuffled pixel (m, n) = (2i + di, 2j + dj) belongs to source
+  } else if (warp >= 2) {
+    // MMA + epilogue.  The band's whole K (4 shifts x 80) is resident, so a warp computes each 16-pixel block of its 32
+    // channels (accumulator rows) when the epilogue needs it.  Thread = shuffled channel c (accumulator row); shuffled pixel (m, n) = (2i + di, 2j + dj) belongs to source
     // plane 4c + 2di + dj.  A work item is (di, pair of feature rows i, i+1): two accumulator rows m = 2i + di and m + 2,
     // i.e. 2 * WS2 consecutive elements of each of the planes dj = 0, 1 -> aligned 16-byte stores.  The two warps of a
     // lane quarter take alternate items.
     const int q = warp & 3, e = (warp - 2) >> 2;
     const int c = mt * 128 + 32 * q + lane;
     const int HW = (Hi / 2) * WS2;
-    constexpr int NCH = (2 * WS2 + 15) / 16;  // 16-column TMEM loads per accumulator row
+    constexpr int NCH = (2 * WS2 + 15) / 16;  // 16-column blocks per accumulator row
+    const uint32_t lbo_g = rows_alloc * 16, lbo_w = 128 * 16;
+    const uint32_t w0 = smem_u32(Ws);
+    mbar_wait(w_full, 0);
     int it = 0, tma_cnt = 0;
     for (int b = slot; b < P.B; b += nslot)
       for (int band = 0; band < nbands; ++band, ++it) {
-        const int y0 = band * Hh, hb = min(Hh, Hi - y0);
+        const int st = it & 1, y0 = band * Hh, hb = min(Hh, Hi - y0);
         const int npairs = hb / 4;  // feature-row pairs in this band
-        const int tb = it % nbuf, tph = (it / nbuf) & 1;
-        const uint32_t dcol = tmem_base + tb * 256;
-        mbar_wait_idle(&t_full[tb], tph, P.backoff);
-        tc::fence_after_sync();
+        mbar_wait_idle(&g_full[st], (it >> 1) & 1, P.backoff);
+        const uint32_t g0 = smem_u32(Gs + (size_t)st * g_bytes);
         auto issue = [&](int item, float (&buf)[2][NCH * 16]) {
           const int ml = 4 * (item >> 1) + (item & 1);  // first accumulator row of the item within this band
 #pragma unroll
           for (int r = 0; r < 2; ++r)
 #pragma unroll
-            for (int k = 0; k < NCH; ++k)
-              tc::tmem_ld16_async(dcol + ((uint32_t)(32 * q) << 16) + (ml + 2 * r) * Pp + 16 * k, &buf[r][16 * k]);
+            for (int k = 0; k < NCH; ++k) {
+              const int col0 = (ml + 2 * r) * Pp + 16 * k;  // first accumulator column (band pixel) of the block
+              float acc[2][2][4];
+              mma::zero(acc);
+#pragma unroll
+              for (int sh = 0; sh < 4; ++sh) {
+                const int shift_rows = (sh >> 1) * Pp + (sh & 1);
+#pragma unroll
+                for (int k16 = 0; k16 < GB_K / 16; ++k16) {
+                  // K = (cls, o), cls = 2 py + px at stride 20: shift (dm, dn) has no tap for classes with py < dm or px < dn,
+                  // so its packed weights are zero for k < 20 (dn), k < 40 (dm), k < 60 (both): the 16-wide chunks k16 < sh
+                  // are all-zero and skipped (14 of 20 remain)
+                  if (k16 < sh) continue;
+                  mma::kstep(acc, w0 + ((sh * GB_KC + 2 * k16) * 128 + 32 * q) * 16, lbo_w,
+                             g0 + (2 * k16) * lbo_g + (LEAD - shift_rows + col0) * 16, lbo_g, lane);
+                }
+              }
+              mma::rows8(acc, 0, &buf[r][16 * k], lane);
+              mma::rows8(acc, 1, &buf[r][16 * k + 8], lane);
+            }
         };
         auto emit = [&](int item, const float (&v)[2][NCH * 16]) {
           if (c >= P.C4) return;
@@ -684,7 +618,6 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
             unsigned char* sl = Ss + (size_t)(par * 4 + 2 * e) * SLICE + (size_t)(32 * q + lane) * PB;
             if (issuer) bulk_wait_group_read1();  // at most the previous item's stores (the other ip parity) still read smem
             named_bar_sync(1 + e, 128);
-            tc::tmem_ld_wait();
 #pragma unroll
             for (int dj = 0; dj < 2; ++dj) {
 #pragma unroll
@@ -709,16 +642,13 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
             }
           }
         } else if (NCH <= 2 && P.prefetch) {
-          // the TMEM loads of the next item are in flight while the current item is converted and stored (the
-          // epilogue was TMEM-load-latency bound: ~55 % of its stall samples sat behind tcgen05.wait::ld)
+          // the next item's blocks are computed before the current item is converted and stored
           float va[2][NCH * 16], vb[2][NCH * 16];
           if (e < nitems) issue(e, va);
           for (int item = e; item < nitems; item += 4) {
-            tc::tmem_ld_wait();
             if (item + 2 < nitems) issue(item + 2, vb);
             emit(item, va);
             if (item + 2 < nitems) {
-              tc::tmem_ld_wait();
               if (item + 4 < nitems) issue(item + 4, va);
               emit(item + 2, vb);
             }
@@ -727,18 +657,14 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
           for (int item = e; item < nitems; item += 2) {
             float v[2][NCH * 16];
             issue(item, v);
-            tc::tmem_ld_wait();
             emit(item, v);
           }
         }
-        tc::fence_before_sync();
-        tc::mbar_arrive(&t_empty[tb]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&g_empty[st]);  // this warp's reads of the band are done
       }
     if (P.tma_store && q == 0 && lane == 0) bulk_wait_group0();  // the stores have landed before the kernel ends
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 512);
 }
 
 
@@ -746,73 +672,84 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
 // wg: weight gradient of a stride-2 3x3 transposed convolution (both layers)
 // =====================================================================================================
 //   dW[c, o, ky, kx] = sum_{frames, rows} X[row + shift][c] * G[row][(cls, o)]      ((cls, shift) -> tap)
-// a GEMM whose K dimension is the pixel raster.  Both operands are the row layout read TRANSPOSED
-// (MN-major UMMA descriptors, tcgen05.cuh / umma_selftest.cu mode 1): A = G (M = 128 covers the 80 real
-// (cls, o) rows; the descriptor's last 6 K-chunk groups run on into the X stages and fill accumulator lanes
-// 80..127 that nothing reads), B = X at a row offset (the shift), N = this CTA's channel group.
-// The four shifts own four accumulators D_sh[k][c] that stay in TMEM across every (frame, row-chunk) unit of
-// the CTA; one epilogue at the end adds them into dW with atomics.  An all-ones input channel (the bias lane
-// of the mid activations) yields the bias gradient from the same GEMM.
-constexpr int WG_THREADS = 192;  // warp 0 loader, warp 1 MMA, warps 2-5 epilogue
+// a GEMM whose K dimension is the pixel raster.  Both operands are the row layout read TRANSPOSED (ldmatrix .trans,
+// mma_sm90.cuh kstep_mn / umma_selftest.cu mode 1): A = G (M = the 80 (cls, o) rows), B = X at a row offset (the
+// shift), N = this CTA's channel group.  MMA warp w owns shift w % 4 and half w / 4 of the channel group; its
+// accumulators D_sh[k][c] stay in registers across every (frame, row-chunk) unit of the CTA, and one epilogue at the
+// end adds them into dW with atomics.  An all-ones input channel (the bias lane of the mid activations) yields the bias
+// gradient from the same GEMM.
+constexpr int WG_THREADS = 288;  // warp 0 loader, warps 1-8 MMA + epilogue
 
 struct WgParams {
   const __nv_bfloat16* X;     // [B][kcx_total][L.rows][8] padded row layout
   const __nv_bfloat16* G;     // [B][10][L.rows][8]
   RowLayout L;
-  float* dW;                  // [Cin][Cout][3][3], pre-zeroed
-  float* dbias;               // [Cout] or null: taken from input channel ones_c
+  float* part;                // [slots][Cin * Cout * 9 + 4 * Cout]: this slot's dW, then its bias gradient per output class
+  int has_bias;               // 1: the bias gradient is taken from input channel ones_c
   int B, Hi, Wi;
   int R;                      // image rows per unit
   int KR;                     // GEMM-K rows per unit = R*(Wi+1) rounded up to 16
   int XR;                     // X rows per K-chunk in smem (KR + Wi + 2, multiple of 8)
   int kcx, kcx_total;         // K-chunks (8 channels) per CTA group / per frame
   int Cin, Cout, ones_c;
-  int stack;                  // 1: the four shifted copies of X are stacked along N in smem -> one MMA per K step
-                              // (small channel counts: an N = 32 MMA costs as much operand fetch as an N = 128 one)
-  int swap;                   // 1: operands swapped: A = X (M = 128 channels, the shift is A's row offset), B = G (N = 80):
-                              // D_sh[channel][(cls, o)].  An MMA's time goes with N, so 80 columns instead of 128 (of which the
-                              // A = G form wastes the 48 lanes above the 80 real rows) is 0.63x the tensor time.  Needs kcx = 16.
-                              // 2: swapped AND the gradient rows staged twice, the second copy one raster row late, side by side
-                              // along N: B = [G[r] | G[r-1]] (N = 160), so ONE MMA covers the shifts (dm, 0) and (dm, 1) --
-                              // sum_r X[r+s]G[r-1] = sum_r X[r+s+1]G[r] because the rows that enter / leave the sum are pad
-                              // columns (zero).  Below N ~ 144 an MMA's time is its operand fetch whatever N is: half the MMAs.
   int smem_bytes;
 };
 
+// The gradients are summed over the CTAs in a fixed order (per-CTA partials, then reduce_partials_kernel), so that a
+// backward pass gives bit-identical results from run to run.
+constexpr int WG_MAX_CTAS = 132;   // weight-gradient CTAs per layer (one per SM of an H100 SXM; fewer on smaller devices)
+constexpr int B2D_MAX_CTAS = 264;  // b2d CTAs (two per SM)
+__host__ __device__ inline size_t wgrad_part_stride(int Cin, int Cout) { return (size_t)Cin * Cout * 9 + 4 * (size_t)Cout; }
+// weight-gradient channel group (K-chunks of 8 channels per CTA) of a layer with nkc K-chunks of input
+inline int wgrad_kcx(int nkc) { return nkc % 8 == 0 ? 8 : 4; }
+inline int wgrad_max_slots(int nkc) {
+  const int slots = WG_MAX_CTAS / (nkc / wgrad_kcx(nkc));
+  return slots < 1 ? 1 : slots;
+}
+
+// out[i] = sum_{p < nparts} sum_{j < nsub} part[p * stride + j * n + i], in that order (i < n)
+__global__ void __launch_bounds__(256) reduce_partials_kernel(const float* __restrict__ part, int nparts, size_t stride, int nsub, int n,
+                                                              float* __restrict__ out) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int p = 0; p < nparts; ++p)
+      for (int j = 0; j < nsub; ++j) s += part[(size_t)p * stride + (size_t)j * n + i];
+    out[i] = s;
+  }
+}
+static void reduce_partials(const float* part, int nparts, size_t stride, int nsub, int n, float* out, cudaStream_t s) {
+  int blocks = (n + 255) / 256;
+  if (blocks > 4 * WG_MAX_CTAS) blocks = 4 * WG_MAX_CTAS;
+  reduce_partials_kernel<<<blocks, 256, 0, s>>>(part, nparts, stride, nsub, n, out);
+}
+
+// NT = n8 tiles per warp = kcx / 2
+template <int NT>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_constant__ WgParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1, R = P.R, KR = P.KR, XR = P.XR;
-  const int gcp = P.swap == 2 ? 2 : 1;  // copies of the gradient rows per stage
-  const int g_bytes = gcp * GB_KC * KR * 16, x_bytes = (P.stack ? 4 : 1) * P.kcx * XR * 16;
+  const int g_bytes = GB_KC * KR * 16, x_bytes = P.kcx * XR * 16;
   unsigned char* Gs = smem;
   unsigned char* Xs = smem + 2 * g_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + P.smem_bytes - 64);
   uint64_t* full = bars;       // [2]
   uint64_t* empty = bars + 2;  // [2]
-  uint64_t* t_done = bars + 4;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 5);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int N = P.kcx * 8;
   const int ngroups = P.kcx_total / P.kcx;  // kcx_total may include K-chunks beyond the last group (ignored)
   const int grp = blockIdx.x % ngroups, slot = blockIdx.x / ngroups, nslot = gridDim.x / ngroups;
   const int nchunk = Hi / R, nunits = P.B * nchunk;  // R divides Hi (host)
-  const uint32_t ncols = P.swap ? 512u : (4 * N <= 32 ? 32 : (4 * N <= 64 ? 64 : (4 * N <= 128 ? 128 : (4 * N <= 256 ? 256 : 512))));
 
   for (int i = tid; i < (P.smem_bytes - 64) / 16; i += WG_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], WG_THREADS / 32 - 1);  // one arrival per MMA warp
     }
-    mbar_init(t_done, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_ptr, ncols);
   fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == 0) {
     int j = 0;
@@ -820,124 +757,63 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
       const int s = j & 1, b = u / nchunk, y0 = (u - b * nchunk) * R;
       mbar_wait(&empty[s], ((j >> 1) & 1) ^ 1);
       // one copy per K-chunk: R image rows of G; R + 1 rows of X (the row below is the shifts' halo)
-      const uint32_t gbytes = (uint32_t)(R * Pp * 16), xbytes = P.stack ? gbytes : (uint32_t)((R + 1) * Pp * 16);
-      const int nx = (P.stack ? 4 : 1) * P.kcx;  // X copies: stacked mode loads each K-chunk once per shift, pre-shifted
-      if (lane == 0) mbar_expect_tx(&full[s], gcp * GB_KC * gbytes + nx * xbytes);
+      const uint32_t gbytes = (uint32_t)(R * Pp * 16), xbytes = (uint32_t)((R + 1) * Pp * 16);
+      if (lane == 0) mbar_expect_tx(&full[s], GB_KC * gbytes + P.kcx * xbytes);
       __syncwarp();
       const size_t row0 = (size_t)P.L.lead + (size_t)y0 * Pp;
-      if (lane < gcp * GB_KC) {
-        const int cp = lane / GB_KC, kc = lane - cp * GB_KC;  // copy 1 starts one row early: its smem row r holds G[r - 1]
-        bulk_g2s(Gs + (size_t)s * g_bytes + (size_t)lane * KR * 16, P.G + (((size_t)b * GB_KC + kc) * P.L.rows + row0 - cp) * 8, gbytes,
-                 &full[s]);
-      }
-      if (lane < nx) {
-        const int sh = lane / P.kcx, kc = lane - sh * P.kcx;
-        const size_t shift_rows = P.stack ? (size_t)((sh >> 1) * Pp + (sh & 1)) : 0;
+      if (lane < GB_KC)
+        bulk_g2s(Gs + (size_t)s * g_bytes + (size_t)lane * KR * 16, P.G + (((size_t)b * GB_KC + lane) * P.L.rows + row0) * 8, gbytes, &full[s]);
+      if (lane < P.kcx)
         bulk_g2s(Xs + (size_t)s * x_bytes + (size_t)lane * XR * 16,
-                 P.X + (((size_t)b * P.kcx_total + (size_t)grp * P.kcx + kc) * P.L.rows + row0 + shift_rows) * 8, xbytes, &full[s]);
-      }
+                 P.X + (((size_t)b * P.kcx_total + (size_t)grp * P.kcx + lane) * P.L.rows + row0) * 8, xbytes, &full[s]);
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = tc::make_idesc_bf16_f32(128, P.swap ? gcp * GB_K : (P.stack ? 4 * N : N)) | (1u << 15) | (1u << 16);  // both operands MN-major
-    const uint32_t g0 = smem_u32(Gs), x0 = smem_u32(Xs);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
+  } else if (slot < nunits) {
+    const int cw = warp - 1, sh = cw & 3, half = cw >> 2;
+    const int dm = sh >> 1, dn = sh & 1, shift_rows = dm * Pp + dn;
+    const uint32_t g0 = smem_u32(Gs), x0 = smem_u32(Xs) + (uint32_t)(half * NT) * XR * 16;  // n8 tile = one K-chunk of X
+    float acc[GB_K / 16][NT][4];
+    mma::zero(acc);
     int j = 0;
     for (int u = slot; u < nunits; u += nslot, ++j) {
       const int s = j & 1;
       mbar_wait(&full[s], (j >> 1) & 1);
-      tc::fence_after_sync();
-      {  // whole warp, convergent; one elected lane issues (tcgen05.cuh)
-        for (int k16 = 0; k16 < KR / 16; ++k16) {
-          const uint64_t gd = tc::make_smem_desc(g0 + s * g_bytes + k16 * 256, 128, KR * 16);
-          if (P.stack) {
-            tc::umma_bf16_e(tmem_u, gd, tc::make_smem_desc(x0 + s * x_bytes + k16 * 256, 128, XR * 16), idesc, (j | k16) != 0 ? 1u : 0u);
-            continue;
-          }
-          if (P.swap == 2) {  // columns [160 dm, 160 dm + 80) = shift (dm, 0), the next 80 = shift (dm, 1): the same map as swap == 1
-#pragma unroll
-            for (int dm = 0; dm < 2; ++dm)
-              tc::umma_bf16_e(tmem_u + dm * 2 * GB_K, tc::make_smem_desc(x0 + s * x_bytes + (k16 * 16 + dm * Pp) * 16, 128, XR * 16), gd, idesc,
-                            (j | k16) != 0 ? 1u : 0u);
-            continue;
-          }
-#pragma unroll
-          for (int sh = 0; sh < 4; ++sh) {
-            const int shift_rows = (sh >> 1) * Pp + (sh & 1);
-            const uint64_t xd = tc::make_smem_desc(x0 + s * x_bytes + (k16 * 16 + shift_rows) * 16, 128, XR * 16);
-            if (P.swap) tc::umma_bf16_e(tmem_u + sh * GB_K, xd, gd, idesc, (j | k16) != 0 ? 1u : 0u);
-            else tc::umma_bf16_e(tmem_u + sh * N, gd, xd, idesc, (j | k16) != 0 ? 1u : 0u);
-          }
-        }
-        tc::umma_commit_e(&empty[s]);
-      }
+      for (int k16 = 0; k16 < KR / 16; ++k16)
+        mma::kstep_mn(acc, g0 + s * g_bytes + k16 * 256, KR * 16, x0 + s * x_bytes + (k16 * 16 + shift_rows) * 16, XR * 16, lane);
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-    if (j > 0) tc::umma_commit_e(t_done);
-    __syncwarp();
-  } else if (slot < nunits && P.swap) {
-    // swapped form: lane = channel, column = (cls, o) of shift sh
-    const int q = warp & 3;
-    mbar_wait(t_done, 0);
-    tc::fence_after_sync();
-    const int c = grp * N + 32 * q + lane;
-#pragma unroll 1
-    for (int sh = 0; sh < 4; ++sh) {
-      const int dm = sh >> 1, dn = sh & 1;
+    // accumulator (k = 16 mt + g (+8), c = 8 nt + 2 t (+1)) of shift sh -> this slot's partial of dW[c][o][ky][kx]
+    float* part = P.part + (size_t)slot * wgrad_part_stride(P.Cin, P.Cout);
+    const int gq = lane >> 2, tq = lane & 3;
 #pragma unroll
-      for (int k0 = 0; k0 < GB_K; k0 += 16) {
-        float v[16];
-        tc::tmem_ld16(tmem_base + ((uint32_t)(32 * q) << 16) + sh * GB_K + k0, v);
+    for (int mt = 0; mt < GB_K / 16; ++mt)
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int k = k0 + i, cls = k / GB_CLS, o = k - cls * GB_CLS, py = cls >> 1, px = cls & 1;  // compile-time
-          const bool valid = o < P.Cout && !(py == 0 && dm == 1) && !(px == 0 && dn == 1) && c < P.Cin;
-          const int ky = py == 0 ? 1 : (dm ? 0 : 2), kx = px == 0 ? 1 : (dn ? 0 : 2);
-          if (valid) atomicAdd(P.dW + ((size_t)c * P.Cout + o) * 9 + ky * 3 + kx, v[i]);
-        }
-      }
-    }
-  } else if (slot < nunits) {
-    const int q = warp & 3;
-    if (32 * q < GB_K) {
-      mbar_wait(t_done, 0);
-      tc::fence_after_sync();
-      const int k = 32 * q + lane;
-      const int cls = k / GB_CLS, o = k - cls * GB_CLS;
-      const int py = cls >> 1, px = cls & 1;
-      for (int sh = 0; sh < 4; ++sh) {
-        const int dm = sh >> 1, dn = sh & 1;
-        const bool valid = k < GB_K && o < P.Cout && !(py == 0 && dm == 1) && !(px == 0 && dn == 1);
+      for (int i = 0; i < 4; ++i) {
+        const int k = 16 * mt + gq + 8 * (i >> 1);
+        const int cls = k / GB_CLS, o = k - cls * GB_CLS, py = cls >> 1, px = cls & 1;
+        if (o >= P.Cout || (py == 0 && dm == 1) || (px == 0 && dn == 1)) continue;
         const int ky = py == 0 ? 1 : (dm ? 0 : 2), kx = px == 0 ? 1 : (dn ? 0 : 2);
-        for (int c0 = 0; c0 < N; c0 += 16) {
-          float v[16];
-          tc::tmem_ld16(tmem_base + ((uint32_t)(32 * q) << 16) + sh * N + c0, v);
-          if (valid) {
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int c = grp * N + c0 + i;
-              if (c < P.Cin) atomicAdd(P.dW + ((size_t)c * P.Cout + o) * 9 + ky * 3 + kx, v[i]);
-              else if (P.dbias && c == P.ones_c && sh == 0) atomicAdd(P.dbias + o, v[i]);
-            }
-          }
+        for (int nt = 0; nt < NT; ++nt) {
+          const int c = grp * N + (half * NT + nt) * 8 + 2 * tq + (i & 1);
+          const float v = acc[mt][nt][i];
+          // (cls, shift) -> tap is one-to-one, so every element of the slot's partial has exactly one writer
+          if (c < P.Cin) part[((size_t)c * P.Cout + o) * 9 + ky * 3 + kx] = v;
+          else if (P.has_bias && c == P.ones_c && sh == 0) part[(size_t)P.Cin * P.Cout * 9 + cls * P.Cout + o] = v;
         }
       }
-    }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, ncols);
 }
 
-static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* dW, float* dbias, int B, int Hi, int Wi,
-                        int kcx, int kcx_total, int Cin, int Cout, int ones_c, int stack, int sms, cudaStream_t s) {
+static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* dW, float* dbias, float* part, int B, int Hi, int Wi,
+                        int kcx_total, int Cin, int Cout, int ones_c, int sms, cudaStream_t s) {
+  const int kcx = wgrad_kcx(kcx_total);
   // image rows per unit: the largest divisor of Hi (<= 8) whose two stages fit in shared memory
-  const int swap = (!stack && kcx == 16) ? g_tuning[LPB_TUNE_WGRAD_SWAP] : 0;
-  const int gcp = swap == 2 ? 2 : 1;
   int R = 0;
   for (int r = Hi < 8 ? Hi : 8; r >= 1; --r) {
     if (Hi % r) continue;
-    const int kr = (r * (Wi + 1) + 15) & ~15, xr = stack ? kr : ((kr + Wi + 2 + 7) & ~7);
-    if ((size_t)2 * gcp * GB_KC * kr * 16 + (size_t)2 * (stack ? 4 : 1) * kcx * xr * 16 + 64 <= 225 * 1024) {
+    const int kr = (r * (Wi + 1) + 15) & ~15, xr = (kr + Wi + 2 + 7) & ~7;
+    if ((size_t)2 * GB_KC * kr * 16 + (size_t)2 * kcx * xr * 16 + 64 <= 225 * 1024) {
       R = r;
       break;
     }
@@ -947,37 +823,37 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   p.X = X;
   p.G = G;
   p.L = make_row_layout(Hi, Wi);
-  p.dW = dW;
-  p.dbias = dbias;
+  p.part = part;
+  p.has_bias = dbias != nullptr;
   p.B = B;
   p.Hi = Hi;
   p.Wi = Wi;
   p.R = R;
   p.KR = (R * (Wi + 1) + 15) & ~15;
-  p.XR = stack ? p.KR : ((p.KR + Wi + 2 + 7) & ~7);
-  p.stack = stack;
-  p.swap = swap;
+  p.XR = (p.KR + Wi + 2 + 7) & ~7;
   p.kcx = kcx;
   p.kcx_total = kcx_total;
   p.Cin = Cin;
   p.Cout = Cout;
   p.ones_c = ones_c;
-  const size_t gb = (size_t)gcp * GB_KC * p.KR * 16, xb = (size_t)(stack ? 4 : 1) * kcx * p.XR * 16;
-  size_t body = 2 * gb + 2 * xb;
-  const size_t phantom = gb + (size_t)16 * p.KR * 16;  // address range the 16-chunk A descriptor of stage 1 spans
-  if (body < phantom) body = phantom;
-  body = (body + 15) & ~(size_t)15;
+  const size_t body = ((size_t)2 * GB_KC * p.KR * 16 + (size_t)2 * kcx * p.XR * 16 + 15) & ~(size_t)15;
   p.smem_bytes = (int)(body + 64);
   LPB_REQUIRE(p.smem_bytes <= 225 * 1024, "head_bwd_bf16: weight-gradient stages need %d B shared memory", p.smem_bytes);
-  LPB_CUDA(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p.smem_bytes));
   const int ngroups = kcx_total / kcx;
   const int nunits = B * (Hi / R);
   int slots = sms / ngroups;
+  if (slots > wgrad_max_slots(kcx_total)) slots = wgrad_max_slots(kcx_total);  // the partials' workspace
   if (slots < 1) slots = 1;
   if (slots > nunits) slots = nunits;
-  wgrad_kernel<<<slots * ngroups, WG_THREADS, p.smem_bytes, s>>>(p);
+  auto kern = kcx == 8 ? wgrad_kernel<4> : wgrad_kernel<2>;
+  LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, p.smem_bytes));
+  kern<<<slots * ngroups, WG_THREADS, p.smem_bytes, s>>>(p);
+  const size_t stride = wgrad_part_stride(Cin, Cout);
+  reduce_partials(part, slots, stride, 1, Cin * Cout * 9, dW, s);
+  if (dbias) reduce_partials(part + (size_t)Cin * Cout * 9, slots, stride, 4, Cout, dbias, s);
   return LPB_OK;
 }
+
 
 // bias gradient of a one-deconv head: column sums of the gradient rows, folded over the four classes
 __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* __restrict__ G, RowLayout L, int B, int cout,
@@ -999,7 +875,7 @@ __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* _
   }
 }
 
-// largest rows-per-band Hh (multiple of 4) whose accumulator fits the b3a TMEM tiling
+// largest rows-per-band Hh (multiple of 4) whose band fits the b3a shared-memory stages
 static int b3a_band_rows(int Hi1, int Wi1) {
   int hh = (256 / (Wi1 + 1)) & ~3;  // two accumulator buffers fit
   if (hh < 4) hh = (304 / (Wi1 + 1)) & ~3;  // wide maps: one buffer
@@ -1035,6 +911,15 @@ static bool make_dfeat_tensor_map(CUtensorMap* tm, void* dfeat, int B, int C4, i
 
 // workspace: [W1 dgrad pack][W2 dgrad pack][G2][G1][plane dots]   (G2 / G1: padded row layouts, row_layout.cuh);
 // a one-deconv head (c2 = 0) has no W2 pack and no G2: its output gradient is G1 directly
+// fixed-order reduction partials: [layer-1 wgrad][layer-2 wgrad][b2d bias]
+static size_t bwd_partials_bytes(int C, int c1, int c2) {
+  using namespace lpb;
+  const int nkc1 = C / 4 / 8;
+  size_t n = (size_t)wgrad_max_slots(nkc1) * wgrad_part_stride(C / 4, c1);
+  if (c2 > 0) n += (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) + (size_t)B2D_MAX_CTAS * 4 * GB_CLS;
+  return n * sizeof(float);
+}
+
 extern "C" int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {
   using namespace lpb;
   LPB_REQUIRE(bytes, "head_bwd_bf16_workspace_bytes: null pointer");
@@ -1043,7 +928,7 @@ extern "C" int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int
   const size_t w1 = (size_t)((C4 + 127) / 128) * 4 * GB_KC * 128 * 16, w2 = (size_t)4 * GB_KC * 32 * 16;
   const size_t g2 = c2 > 0 ? (size_t)B * GB_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0;
   const size_t g1 = (size_t)B * GB_KC * make_row_layout(2 * H, 2 * W).rows * 16;
-  *bytes = w1 + w2 + g2 + g1 + (((size_t)B * (c2 > 0 ? c2 : c1) * 4 + 255) & ~(size_t)255);
+  *bytes = w1 + w2 + g2 + g1 + (((size_t)B * (c2 > 0 ? c2 : c1) * 4 + 255) & ~(size_t)255) + bwd_partials_bytes(C, c1, c2);
   return LPB_OK;
 }
 
@@ -1077,7 +962,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   }
   const int Hh = b3a_band_rows(Hi1, Wi1);
   if (Hh < 4) {
-    set_error("head_bwd_bf16: feature map %dx%d outside this build's TMEM tiling", H, W);
+    set_error("head_bwd_bf16: feature map %dx%d outside this build's band tiling", H, W);
     return LPB_ERR_UNSUPPORTED;
   }
   int dev = 0, sms = 0;
@@ -1093,6 +978,9 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   __nv_bfloat16* G2 = reinterpret_cast<__nv_bfloat16*>(ws + w1b + w2b);
   __nv_bfloat16* G1 = reinterpret_cast<__nv_bfloat16*>(ws + w1b + w2b + g2b);
   float* ddot = reinterpret_cast<float*>(ws + w1b + w2b + g2b + g1b);
+  float* part1 = reinterpret_cast<float*>(ws + w1b + w2b + g2b + g1b + ((((size_t)B * kout * 4) + 255) & ~(size_t)255));
+  float* part2 = part1 + (size_t)wgrad_max_slots(C4 / 8) * wgrad_part_stride(C4, c1);
+  float* part_db1 = two ? part2 + (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) : nullptr;
   // the forward pass's mid activations (head_bf16.cu workspace layout: [packed w1][packed w2][mid])
   const size_t fwd_mid_off = (size_t)(C4 / 32 + 1) * (4 * 4 * 80 * 16);
   const __nv_bfloat16* mid = reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + fwd_mid_off);
@@ -1139,7 +1027,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   }
   if (two) {
     // layer 2: weight + bias gradient (bias from the all-ones channel c1 of mid), then data gradient -> G1 (+ db1)
-    const int rc = launch_wgrad(mid, G2, dw2, db2, B, Hi2, Wi2, 4, 4, c1, c2, c1, 1, sms, s);
+    const int rc = launch_wgrad(mid, G2, dw2, db2, part2, B, Hi2, Wi2, 4, c1, c2, c1, sms, s);
     if (rc != LPB_OK) return rc;
     B2dParams p;
     p.G2 = G2;
@@ -1147,7 +1035,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.G1 = G1;
     p.L2 = L2;
     p.L1 = L1;
-    p.db1 = db1;
+    p.db1_part = part_db1;
     p.B = B;
     p.Hi = Hi2;
     p.Wi = Wi2;
@@ -1158,16 +1046,17 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     const size_t smem = (size_t)GB_KC * rows_alloc * 16 + (size_t)4 * GB_KC * 32 * 16 + 64;
     LPB_REQUIRE(smem <= 113 * 1024 && p.R2 >= 1, "head_bwd_bf16: layer-2 width %d too large", Wi2);
     LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = B < 2 * sms ? B : 2 * sms;
+    int grid = B < 2 * sms ? B : 2 * sms;
+    if (grid > B2D_MAX_CTAS) grid = B2D_MAX_CTAS;  // the bias partials' workspace
     b2d_dgrad_kernel<<<grid, B2D_THREADS, smem, s>>>(p);
+    reduce_partials(part_db1, grid * 4, GB_CLS, 1, c1, db1, s);
   } else {
     rows_colsum_kernel<<<(unsigned)(B * GB_KC), 256, 0, s>>>(G1, L1, B, c1, db1);
   }
   // layer 1: weight gradient from the saved shuffled features, data gradient -> d features
   {
     const int nkc = C4 / 8;  // multiple of 4
-    const int kcx = nkc % 16 == 0 ? 16 : (nkc % 12 == 0 ? 12 : (nkc % 8 == 0 ? 8 : 4));
-    const int rc = launch_wgrad(static_cast<const __nv_bfloat16*>(saved_xs), G1, dw1, nullptr, B, Hi1, Wi1, kcx, nkc, C4, c1, -1, 0, sms, s);
+    const int rc = launch_wgrad(static_cast<const __nv_bfloat16*>(saved_xs), G1, dw1, nullptr, part1, B, Hi1, Wi1, nkc, C4, c1, -1, sms, s);
     if (rc != LPB_OK) return rc;
   }
   if (dfeat) {

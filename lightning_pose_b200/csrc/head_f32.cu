@@ -5,7 +5,7 @@
 // CUDA-core FMA with fp32 accumulation, gather-form transposed convolution (each thread owns one
 // input pixel and produces its 2x2 output quad for a group of output channels, so there is no
 // scatter / atomics), PixelShuffle folded into the shared-memory staging of the first layer.
-// The bf16 tensor-core (tcgen05) path lives in head_bf16.cu.
+// The bf16 tensor-core path lives in head_bf16.cu.
 #include <cstdint>
 
 #include "../../include/lpb200.h"

@@ -28,9 +28,11 @@ struct ConvtRowsParams {
 int launch_rows_shuffle(const __nv_bfloat16* feat, int B, int C, int H, int W, __nv_bfloat16* xs, cudaStream_t s);
 int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s);
 
-// bands the banded kernel cuts an (Hi x Wi) conv input into (R = 384 / (Wi + 1) image rows each)
+// raster rows per band of the banded kernel (its M-tiles x 128)
+constexpr int CR_BAND_ROWS = 256;
+// bands the banded kernel cuts an (Hi x Wi) conv input into (R = CR_BAND_ROWS / (Wi + 1) image rows each)
 inline int convt_rows_bands(int Hi, int Wi) {
-  int R = 384 / (Wi + 1);
+  int R = CR_BAND_ROWS / (Wi + 1);
   if (R > Hi) R = Hi;
   if (R < 1) R = 1;
   return (Hi + R - 1) / R;

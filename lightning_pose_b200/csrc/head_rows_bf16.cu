@@ -1,17 +1,17 @@
-// Shape-generic bf16 heatmap head on tcgen05: any feature map, one- or two-deconv heads (ViT / ResNet families).
+// Shape-generic bf16 heatmap head on the tensor cores: any feature map, one- or two-deconv heads (ViT / ResNet families).
 // Reference: lightning_pose/models/heads/heatmap.py:20-71 (layer stack; ViT stride 16 -> one deconv, :192-193),
 // :203-212 (forward).
 //
-// head_bf16.cu keeps a whole frame's accumulators in TMEM and therefore stops at 12x12 feature maps.  Here a
+// head_bf16.cu keeps a whole frame's operands in shared memory and therefore stops at 12x12 feature maps.  Here a
 // transposed convolution is a *banded* 4-shift GEMM on the padded row layout (row_layout.cuh):
 //   rows_shuffle_kernel   features (NCHW bf16) -> pixel-shuffled rows X[b][kchunk][row][8]      (one pass, HBM-bound)
 //   convt_rows_kernel     X rows --TMA bulk, one copy per K-chunk--> smem stages (K streamed 32 channels at a time)
-//                         --tcgen05.mma, 4 shifted views--> TMEM (<= 3 M-tiles = one band of image rows)
+//                         --mma.sync, 4 shifted views--> register accumulators (<= 2 M-tiles = one band of image rows)
 //                         --epilogue--> bf16 rows of the next layer | fp32 planes | two-pass plane softmax
-// The band height adapts to the image width (R = 384 / (Wi + 1) image rows), so TMEM (256 columns per CTA, two CTAs
-// per SM) and shared memory (two 49 KB stages) never depend on the frame size.  The softmax is computed by
-// recomputation as in head_bf16.cu: pass 0 streams every band once for the per-plane (max, sum), pass 1 re-issues the
-// GEMM and writes the normalised planes -- the logits never touch HBM.
+// The band height adapts to the image width (R = 256 / (Wi + 1) image rows), so the accumulators (48 registers per
+// tile and thread) and shared memory never depend on the frame size.  The softmax is computed by recomputation as in
+// head_bf16.cu: pass 0 streams every band once for the per-plane (max, sum), pass 1 re-issues the GEMM and writes the
+// normalised planes -- the logits never touch HBM.
 #include <cuda_bf16.h>
 
 #include <cstdint>
@@ -21,7 +21,7 @@
 #include "head_rows.cuh"
 #include "lpb_common.cuh"
 #include "row_layout.cuh"
-#include "tcgen05.cuh"
+#include "mma_sm90.cuh"
 
 namespace lpb {
 
@@ -72,9 +72,10 @@ int launch_rows_shuffle(const __nv_bfloat16* feat, int B, int C, int H, int W, _
 constexpr int CR_NCOLS = 80;   // 4 classes x 20
 constexpr int CR_CLS = 20;
 constexpr int CR_BSTAGE = 4 * 4 * CR_NCOLS * 16;  // packed weights of one 32-channel stage [shift][kchunk][80][16 B]
-constexpr int CR_THREADS = 320;  // warp 0 loader, warp 1 MMA issuer (+TMEM owner), warps 2-9 epilogue
+constexpr int CR_THREADS = 320;  // warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue
 constexpr int CR_EPI = 256;
-constexpr int CR_TILES = 3;      // M-tiles per band (3 * 80 = 240 of the CTA's 256 TMEM columns)
+constexpr int CR_TILES = 2;      // M-tiles per band: a warp's accumulators (CR_TILES x 32 rows x 48 columns) stay in registers
+static_assert(CR_TILES * 128 == CR_BAND_ROWS, "head_rows.cuh sizes the per-band softmax statistics with CR_BAND_ROWS");
 constexpr int CR_STAGES = 2;
 constexpr int CR_NMASK = 64;     // (band, tile) pairs of a frame the decode hints can cover
 constexpr int CR_HBOX = 16;      // decode hints: the box is rows / columns [arg - 16, arg + 15] = decode.cu's first window
@@ -83,7 +84,7 @@ constexpr int CR_HBOX = 16;      // decode hints: the box is rows / columns [arg
 // V2: softmax epilogue with one warp vote per tile (instead of one per plane), the running-max rescale out of the
 // common path, (shift, 1/sum) fetched as one 8-byte shared load and the output pointer advanced by addition.
 template <int MODE, int NPL, bool V2, bool HINT = false>
-__global__ void __launch_bounds__(CR_THREADS, 2) convt_rows_kernel(const __grid_constant__ ConvtRowsParams P) {
+__global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_constant__ ConvtRowsParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Pp = P.L.Pp, Wi = P.L.Wi, Hi = P.L.Hi;
   const int a_bytes = 4 * P.rows_alloc * 16, stage_bytes = a_bytes + CR_BSTAGE;
@@ -94,27 +95,18 @@ __global__ void __launch_bounds__(CR_THREADS, 2) convt_rows_kernel(const __grid_
   uint64_t* bars = reinterpret_cast<uint64_t*>(nmask + CR_NMASK);
   uint64_t* full = bars;       // [2]
   uint64_t* empty = bars + 2;  // [2]
-  uint64_t* t_full = bars + 4;
-  uint64_t* t_empty = bars + 5;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 6);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < CR_STAGES * stage_bytes / 16; i += CR_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     for (int s = 0; s < CR_STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], CR_EPI / 32);  // one arrival per MMA warp
     }
-    mbar_init(t_full, 1);
-    mbar_init(t_empty, CR_EPI);
     fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_ptr, 256);
   fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
 
   const int R = P.R, nbands = (Hi + R - 1) / R, nst = P.nst;
   const int npass = MODE == CONVT_ROWS_SOFTMAX ? 2 : 1;
@@ -159,52 +151,16 @@ __global__ void __launch_bounds__(CR_THREADS, 2) convt_rows_kernel(const __grid_
                        P.X + (((size_t)b * 4 * nst + 4 * st + lane) * P.L.rows + P.L.lead + (size_t)y0 * Pp) * 8, nbytes, &full[s]);
           }
         }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = tc::make_idesc_bf16_f32(128, CR_NCOLS);
-    const uint32_t lbo_a = P.rows_alloc * 16, lbo_b = CR_NCOLS * 16;
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    int it = 0, nb = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x)
-      for (int pass = 0; pass < npass; ++pass)
-        for (int bi = 0; bi < bands_per_item; ++bi, ++nb) {
-          const int band = PER_BAND ? item % nbands : bi;
-          const int rb = min(R, Hi - band * R), tiles = (rb * Pp + 127) / 128;
-          mbar_wait(t_empty, (nb & 1) ^ 1);
-          tc::fence_after_sync();
-          for (int st = 0; st < nst; ++st, ++it) {
-            const int s = it % CR_STAGES;
-            mbar_wait(&full[s], (it / CR_STAGES) & 1);
-            tc::fence_after_sync();
-            {  // whole warp, convergent; one elected lane issues (tcgen05.cuh)
-              const uint32_t a0 = smem_u32(smem + s * stage_bytes), b0 = a0 + a_bytes;
-              for (int t = 0; t < tiles; ++t) {
-#pragma unroll
-                for (int sh = 0; sh < 4; ++sh) {
-                  const int shift_rows = (sh >> 1) * Pp + (sh & 1);
-#pragma unroll
-                  for (int k16 = 0; k16 < 2; ++k16) {
-                    const uint32_t aa = a0 + (2 * k16) * lbo_a + (t * 128 + shift_rows) * 16;
-                    const uint32_t bb = b0 + (sh * 4 + 2 * k16) * lbo_b;
-                    tc::umma_bf16_e(tmem_u + t * CR_NCOLS, tc::make_smem_desc(aa, lbo_a, 128), tc::make_smem_desc(bb, lbo_b, 128),
-                                    idesc, (st | sh | k16) != 0 ? 1u : 0u);
-                  }
-                }
-              }
-              tc::umma_commit_e(&empty[s]);
-              if (st == nst - 1) tc::umma_commit_e(t_full);
-            }
-            __syncwarp();
-          }
-        }
-  } else {
-    // ================= epilogue: lane quarter q = warp % 4, output-row parity e = (warp - 2) / 4 ====================
-    // classes (py = e, px = 0 | 1) = TMEM columns [40e, 40e + 40); loads stay 16-column aligned: read [32e, 32e + 48)
+  } else if (warp >= 2) {
+    // ================= MMA + epilogue: row quarter q = warp % 4, output-row parity e = (warp - 2) / 4 ===============
+    // classes (py = e, px = 0 | 1) = accumulator columns [40e, 40e + 40); the warp accumulates [32e, 32e + 48) over the
+    // stages and reads them out in "lane = row" form
     const int q = warp & 3, e = (warp - 2) >> 2, ew = warp - 2;
     const float L2E = 1.4426950408889634f;
     const size_t plane_stride = (size_t)Ho * Wo;
     const bool use_bias = P.bias && (MODE == CONVT_ROWS_MID || MODE == CONVT_ROWS_PLANES);  // a per-plane constant does not change a softmax
-    int nb = 0;
+    const uint32_t lbo_a = P.rows_alloc * 16, lbo_b = CR_NCOLS * 16;
+    int it = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int b = PER_BAND ? item / nbands : item;
       float mx[CR_CLS], sm[CR_CLS];
@@ -230,17 +186,37 @@ __global__ void __launch_bounds__(CR_THREADS, 2) convt_rows_kernel(const __grid_
       }
       for (int pass = 0; pass < npass; ++pass) {
         const bool write = MODE == CONVT_ROWS_SOFTMAX_P0 ? false : (pass == npass - 1);
-        for (int bi = 0; bi < bands_per_item; ++bi, ++nb) {
+        for (int bi = 0; bi < bands_per_item; ++bi) {
           const int band = PER_BAND ? item - b * nbands : bi;
           const int y0 = band * R, rb = min(R, Hi - y0), tiles = (rb * Pp + 127) / 128;
-          mbar_wait_idle(t_full, nb & 1, P.backoff);
-          tc::fence_after_sync();
-          for (int t = 0; t < tiles; ++t) {
+          float acc[CR_TILES][2][6][4];
+#pragma unroll
+          for (int t = 0; t < CR_TILES; ++t) mma::zero(acc[t]);
+          for (int st = 0; st < nst; ++st, ++it) {
+            const int s = it % CR_STAGES;
+            mbar_wait_idle(&full[s], (it / CR_STAGES) & 1, P.backoff);
+            const uint32_t a0 = smem_u32(smem + s * stage_bytes), b0 = a0 + a_bytes;
+#pragma unroll
+            for (int t = 0; t < CR_TILES; ++t) {
+              if (t >= tiles) break;
+#pragma unroll
+              for (int sh = 0; sh < 4; ++sh) {
+                const int shift_rows = (sh >> 1) * Pp + (sh & 1);
+#pragma unroll
+                for (int k16 = 0; k16 < 2; ++k16)
+                  mma::kstep(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
+                             b0 + (sh * 4 + 2 * k16) * lbo_b + 32 * e * 16, lbo_b, lane);
+              }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
+          }
+#pragma unroll
+          for (int t = 0; t < CR_TILES; ++t) {
+            if (t >= tiles) break;
             float d[48];
 #pragma unroll
-            for (int cc = 0; cc < 3; ++cc)
-              tc::tmem_ld16_async(tmem_base + ((uint32_t)(32 * q) << 16) + t * CR_NCOLS + 32 * e + cc * 16, &d[cc * 16]);
-            tc::tmem_ld_wait();
+            for (int nt = 0; nt < 6; ++nt) mma::rows8(acc[t], nt, &d[8 * nt], lane);
             const int row = t * 128 + 32 * q + lane;
             const int ml = row / Pp, n = row - ml * Pp;
             const bool valid = (ml < rb) && (n < Wi);
@@ -368,8 +344,6 @@ __global__ void __launch_bounds__(CR_THREADS, 2) convt_rows_kernel(const __grid_
             if (e == 0) body(std::integral_constant<int, 0>{});
             else body(std::integral_constant<int, 1>{});
           }
-          tc::fence_before_sync();
-          tc::mbar_arrive(t_empty);
         }
         if ((npass == 2 && pass == 0) || MODE == CONVT_ROWS_SOFTMAX_P0) {
           // merge the online-softmax states: lanes -> warp (shuffles) -> 8 epilogue warps (smem)
@@ -445,9 +419,6 @@ __global__ void __launch_bounds__(CR_THREADS, 2) convt_rows_kernel(const __grid_
       }
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 256);
 }
 
 int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
@@ -465,7 +436,7 @@ int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
   p.backoff = g_tuning[LPB_TUNE_WAIT_BACKOFF];
   const int nbands = (p.L.Hi + p.R - 1) / p.R;
   auto run = [&](auto kern, long long nitems) -> int {
-    const int grid = (int)(nitems < 2 * sms ? nitems : 2 * sms);
+    const int grid = (int)(nitems < sms ? nitems : sms);  // one CTA per SM: the accumulators take the register file
     LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<grid, CR_THREADS, smem, s>>>(p);
     return LPB_OK;

@@ -99,7 +99,7 @@ extern "C" int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int 
   const bool resize = (out_h != H) || (out_w != W);
   const int64_t total = (int64_t)F * out_h * out_w;
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;  // 32 CTAs per SM of an H100 SXM
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int key = layout * 4 + (out_bf16 ? 2 : 0) + (resize ? 1 : 0);
   switch (key) {

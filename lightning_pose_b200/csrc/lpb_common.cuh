@@ -1,4 +1,4 @@
-// Shared helpers for the lpb200 CUDA library (sm_100a only).
+// Shared helpers for the lpb200 CUDA library (sm_90a).
 #pragma once
 #include <type_traits>
 #include <cuda_runtime.h>
@@ -57,36 +57,21 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// ---- packed fp32 pairs (sm_100: FFMA2 / FADD2 / FMUL2) ---------------------------------------------
-// Two IEEE fp32 operations per instruction: the same roundings as the scalar forms and the same FMA rate
-// (measured: 127 FMA/clk/SM either way, scripts/ubench/ffma.cu), but half the issue slots.  Operands that
-// are the same scalar in both halves (`dup2`) or a pair of kernel-parameter constants fold into the
-// instruction's broadcast / uniform-register operand forms, so they cost no extra moves.
+// ---- fp32 pairs -------------------------------------------------------------------------------------
+// Code written against pairs of fp32 values (two positions per thread).  sm_90 has no packed fp32 instructions, so each
+// pair operation is two scalar IEEE fp32 operations: the same roundings a packed form would give.
 struct f32x2 {
-  unsigned long long v;
+  float lo, hi;
 };
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-  return r;
-}
+__device__ __forceinline__ f32x2 pack2(float lo, float hi) { return f32x2{lo, hi}; }
 __device__ __forceinline__ f32x2 dup2(float x) { return pack2(x, x); }
-__device__ __forceinline__ void unpack2(f32x2 a, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(a.v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-  return r;
+__device__ __forceinline__ void unpack2(f32x2 a, float& lo, float& hi) {
+  lo = a.lo;
+  hi = a.hi;
 }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return f32x2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
 // compile-time loop: fn(std::integral_constant<int, I>{}) for I in [0, N)
 template <int I, int N, class Fn>
 __device__ __forceinline__ void static_for(Fn&& fn) {
@@ -112,6 +97,9 @@ __device__ __forceinline__ void fence_proxy_async() {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(

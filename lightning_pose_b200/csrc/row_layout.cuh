@@ -1,4 +1,4 @@
-// The padded "row layout" every tcgen05 kernel of the head exchanges through global memory:
+// The padded "row layout" every tensor-core kernel of the head exchanges through global memory:
 //   X[b][kchunk][row][8] bf16,  row = lead + y * (Wi + 1) + n
 // i.e. the image raster with one zero column per image row plus `lead` zero rows before and after.  It is
 // byte-for-byte the operand image the kernels keep in shared memory (zero column = horizontal halo, lead /

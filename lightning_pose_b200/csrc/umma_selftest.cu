@@ -1,19 +1,19 @@
-// Self-test of the hand-written UMMA plumbing (descriptor semantics), used by tests/test_gpu_parity.py.
+// Self-test of the tensor-core operand plumbing (mma_sm90.cuh), run by scripts/test_umma_selftest.py.
 // One CTA computes a small GEMM from operands stored in the library's "row layout"
 //   X[kchunk][row][8] bf16   (element (row, ch) at kchunk = ch/8, 16 bytes per row)
 // in two interpretations:
 //   mode 0  K-major : D[m][n] = sum_ch  A[row=m][ch] * B[row=n][ch]          (the forward shift-GEMMs)
 //   mode 1  MN-major: D[m][n] = sum_row A[row][ch=m] * B[row][ch=n]          (weight-gradient GEMMs:
-//           the SAME buffers read transposed: SBO = kchunk stride, LBO = 128 B, a_major = b_major = MN)
-// `row_shift` moves A's start address by whole rows (the shift trick), `col_off` accumulates into a TMEM
-// column offset and reads back from it (checks unaligned-column accumulators / loads).
+//           the SAME buffers read transposed, ldmatrix .trans)
+// `row_shift` moves A's start address by whole rows (the shift trick); `col_off` is kept by the C ABI and has no effect
+// (the accumulators live in registers).
 #include <cuda_bf16.h>
 
 #include <cstdint>
 
 #include "../../include/lpb200.h"
 #include "lpb_common.cuh"
-#include "tcgen05.cuh"
+#include "mma_sm90.cuh"
 
 namespace lpb {
 
@@ -22,7 +22,7 @@ struct SelfTestParams {
   const __nv_bfloat16* b;  // [kcb][rows_b][8]
   float* d;                // [128][n]
   int kca, rows_a, kcb, rows_b;
-  int mode, n, k, row_shift, col_off;
+  int mode, n, k, row_shift;
 };
 
 __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const __grid_constant__ SelfTestParams P) {
@@ -30,49 +30,26 @@ __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const __grid_cons
   const int a_bytes = P.kca * P.rows_a * 16, b_bytes = P.kcb * P.rows_b * 16;
   unsigned char* As = smem;
   unsigned char* Bs = smem + a_bytes;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(Bs + b_bytes);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < a_bytes / 16; i += 128) reinterpret_cast<uint4*>(As)[i] = reinterpret_cast<const uint4*>(P.a)[i];
   for (int i = tid; i < b_bytes / 16; i += 128) reinterpret_cast<uint4*>(Bs)[i] = reinterpret_cast<const uint4*>(P.b)[i];
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) tc::tmem_alloc(tmem_ptr, 256);
-  fence_proxy_async();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-  if (tid == 0) {
-    const uint32_t a0 = smem_u32(As) + P.row_shift * 16, b0 = smem_u32(Bs);
-    const uint32_t kst_a = P.rows_a * 16, kst_b = P.rows_b * 16;  // kchunk strides
-    uint32_t idesc = tc::make_idesc_bf16_f32(128, P.n);
-    if (P.mode == 1) idesc |= (1u << 15) | (1u << 16);  // a_major = b_major = MN
+  const uint32_t a0 = smem_u32(As) + P.row_shift * 16, b0 = smem_u32(Bs);
+  const uint32_t kst_a = P.rows_a * 16, kst_b = P.rows_b * 16;  // kchunk strides
+  for (int c0 = 0; c0 < P.n; c0 += 16) {  // warp = accumulator rows [32 warp, 32 warp + 32), 16 columns at a time
+    float acc[2][2][4];
+    mma::zero(acc);
     for (int k16 = 0; k16 < P.k / 16; ++k16) {
-      uint64_t ad, bd;
-      if (P.mode == 0) {  // K = channels: two kchunks per instruction
-        ad = tc::make_smem_desc(a0 + 2 * k16 * kst_a, kst_a, 128);
-        bd = tc::make_smem_desc(b0 + 2 * k16 * kst_b, kst_b, 128);
-      } else {            // K = rows: 16 rows per instruction; MN groups are the kchunks
-        ad = tc::make_smem_desc(a0 + k16 * 256, 128, kst_a);
-        bd = tc::make_smem_desc(b0 + k16 * 256, 128, kst_b);
-      }
-      tc::umma_bf16(tmem_base + P.col_off, ad, bd, idesc, k16 > 0 ? 1u : 0u);
+      if (P.mode == 0)  // K = channels: two kchunks per step
+        mma::kstep(acc, a0 + 2 * k16 * kst_a + 32 * warp * 16, kst_a, b0 + 2 * k16 * kst_b + c0 * 16, kst_b, lane);
+      else              // K = rows: 16 rows per step; M / N groups of 8 are the kchunks
+        mma::kstep_mn(acc, a0 + k16 * 256 + 4 * warp * kst_a, kst_a, b0 + k16 * 256 + (c0 / 8) * kst_b, kst_b, lane);
     }
-    tc::umma_commit(bar);
-  }
-  mbar_wait(bar, 0);
-  tc::fence_after_sync();
-  for (int c0 = 0; c0 < P.n; c0 += 16) {
     float v[16];
-    tc::tmem_ld16(tmem_base + ((uint32_t)(32 * warp) << 16) + P.col_off + c0, v);
+    mma::rows8(acc, 0, v, lane);
+    mma::rows8(acc, 1, v + 8, lane);
     for (int i = 0; i < 16 && c0 + i < P.n; ++i) P.d[(size_t)(32 * warp + lane) * P.n + c0 + i] = v[i];
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem_base, 256);
 }
 
 }  // namespace lpb
@@ -94,7 +71,7 @@ extern "C" int lpb_selftest_umma(const void* a, int kca, int rows_a, const void*
   P.n = n;
   P.k = k;
   P.row_shift = row_shift;
-  P.col_off = col_off;
+  (void)col_off;
   const size_t smem = (size_t)(kca * rows_a + kcb * rows_b) * 16 + 64;
   LPB_REQUIRE(smem <= 200 * 1024, "selftest_umma: operands too large");
   LPB_CUDA(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -5,7 +5,7 @@
 * ``LossFactory``        holds the instantiated losses, returns ``sum_l anneal_l * weight_l * loss_l``
   plus the logging dicts (:197-285); heatmap_{mse,kl,js} are exempt from annealing (:267).
 
-B200 specifics: the running total never touches the host (the reference starts it as a CPU
+H100 specifics: the running total never touches the host (the reference starts it as a CPU
 tensor and ``.to(device)``s it every iteration, :250,273), and when a factory holds more than one
 of {temporal, pca_singleview, pca_multiview} they are evaluated by ONE kernel launch whose result
 is handed to each loss object.

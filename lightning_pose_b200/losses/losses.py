@@ -1,4 +1,4 @@
-"""Loss classes on B200: drop-in for ``lightning_pose.losses.losses``.
+"""Loss classes on H100: drop-in for ``lightning_pose.losses.losses``.
 
 Every class keeps the reference's constructor keywords, attributes (``loss_name``, ``epsilon``,
 ``log_weight``, ``weight``), staged methods (``remove_nans`` / ``compute_loss`` /

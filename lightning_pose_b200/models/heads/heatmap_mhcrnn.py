@@ -1,4 +1,4 @@
-"""Multi-head convolutional-RNN head on B200: drop-in for ``lightning_pose.models.heads.heatmap_mhcrnn``.
+"""Multi-head convolutional-RNN head on H100: drop-in for ``lightning_pose.models.heads.heatmap_mhcrnn``.
 
 Same public surface as the reference module (``lightning_pose/models/heads/heatmap_mhcrnn.py``):
 ``HeatmapMHCRNNHead`` (:18-137) and ``UpsamplingCRNN`` (:139-316) with identical constructor arguments, attributes and
@@ -6,7 +6,7 @@ state-dict keys (``head_sf.upsampling_layers.<i>.*``, ``head_mf.{W_pre,W_f,H_f.0
 ``head_mf.layers.<i>`` aliases), so reference checkpoints load unchanged.
 
 What differs is what runs.  The modules are parameter containers; the arithmetic is
-  * ``W_pre`` / ``W_f`` / ``W_b``: the head's own transposed-convolution kernels (tcgen05 for bf16 features), applied to
+  * ``W_pre`` / ``W_f`` / ``W_b``: the head's own transposed-convolution kernels (tensor-core for bf16 features), applied to
     every frame ONCE - a frame that sits in five overlapping windows of a video sequence is never tiled five times
     (the reference does, ``models/base.py:380-390``);
   * the bidirectional recurrence: ``H_f`` / ``H_b`` (grouped Conv2d k2 s2 -> grouped ConvTranspose2d k2 s2, no

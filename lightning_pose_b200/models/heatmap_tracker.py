@@ -7,7 +7,7 @@
 (optimisers, logging, checkpointing) is out of scope.  The backbone is any module mapping images to
 ``(B, C, H/stride, W/stride)`` features - a dense-contraction provider outside this repository's kernels.
 
-B200 specifics: the head, decode, coordinate remap and losses all run in ``liblpb200.so``; the affine undo
+H100 specifics: the head, decode, coordinate remap and losses all run in ``liblpb200.so``; the affine undo
 and the model->frame map of the unlabeled branch are one launch; the keypoint tensor handed to the losses
 is a fresh tensor (the reference aliases ``keypoints_pred_augmented`` through an in-place view when there
 is no augmentation, ``heatmap_tracker.py:272-285`` - harmless there because no loss reads it).

@@ -4,7 +4,7 @@
 surface (``forward`` -> (heatmaps_sf, heatmaps_mf), ``get_loss_inputs_labeled`` with the sf/mf concatenation,
 ``predict_step`` picking the more confident of the two heads per keypoint, ``get_parameters``) as plain ``nn.Module``s.
 
-B200 specifics: an unlabeled video sequence ``(seq, 3, H, W)`` is pushed through the backbone once and handed to
+H100 specifics: an unlabeled video sequence ``(seq, 3, H, W)`` is pushed through the backbone once and handed to
 ``HeatmapMHCRNNHead.forward_sequence`` - the (seq, 5, C, h, w) window tensor of
 ``get_context_from_sequence`` (``models/base.py:159-196, :372-390``) is never built; labeled context batches
 ``(batch, 5, 3, H, W)`` follow the reference's reshape (their windows do not overlap).

@@ -8,7 +8,7 @@ supervised / multi-view PCA losses then run on that folded tensor.
 
 The transformer blocks themselves are the backbone (dense contractions supplied by a library module); this mirror owns
 what sits on this repository's path: the view-embedding / token bookkeeping of ``forward_vit``, the head on
-``views * batch`` feature maps (BASELINE config 4: (8 x 4, 384, 24, 24) -> (8, 68, 96, 96) through the banded tcgen05
+``views * batch`` feature maps (BASELINE config 4: (8 x 4, 384, 24, 24) -> (8, 68, 96, 96) through the banded tensor-core
 kernels), the fold, and the loss inputs.  3-D triangulation (``project_camera_pairs_to_3d``, needs camera calibration and
 aniposelib) is out of scope: the corresponding dict entries are ``None``, exactly what the reference returns for
 uncalibrated data (:299-307).

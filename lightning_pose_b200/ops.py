@@ -200,7 +200,7 @@ _BWD_WIDTHS = (4, 8, 12, 16, 24, 32)
 
 
 def head_bf16_supported(shape, channels, train: bool) -> bool:
-    """Whether the tcgen05 kernels cover this head: feature shape (B, C, H, W), deconv output channels (c1[, c2])."""
+    """Whether the tensor-core kernels cover this head: feature shape (B, C, H, W), deconv output channels (c1[, c2])."""
     _, c, h, w = shape
     n = len(channels)
     if n not in (1, 2) or c % 128 or (h * w) % 8:
@@ -216,7 +216,7 @@ def head_bf16_supported(shape, channels, train: bool) -> bool:
 
 
 def _head_forward_bf16(f, weights, biases, final_softmax, train=False, want_hints=False):
-    """tcgen05 path (one- or two-deconv heads); the caller checks ``head_bf16_supported`` first.
+    """tensor-core path (one- or two-deconv heads); the caller checks ``head_bf16_supported`` first.
 
     ``train=True`` returns ``(out, saved)`` where ``saved`` carries what ``head_backward_bf16`` needs
     (the row-layout copy of the shuffled features and the forward workspace with the inter-layer activations).
@@ -267,7 +267,7 @@ def decode_backward_windows(heatmaps, stats, grad_xy, ds, temperature):
 
 
 def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None):
-    """Gradients of the bf16 head (tcgen05): returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None).
+    """Gradients of the bf16 head: returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None).
 
     ``g_out``: dense gradient w.r.t. the head output or None; ``probs``: the head output when it ends in the
     spatial softmax (its backward is fused in), None for a logits head; ``windows``: result of
@@ -352,7 +352,7 @@ def head_forward_f32(features, weights, biases, final_softmax=True, keep_activat
 def head_forward(features, weights, biases, final_softmax=True):
     """PixelShuffle(2) + ConvTranspose2d stack + spatial softmax; forward only.
 
-    bf16 features take the tcgen05 tensor-core kernels (fp32 accumulate, fp32 heatmaps) when the head is a one- or
+    bf16 features take the tensor-core tensor-core kernels (fp32 accumulate, fp32 heatmaps) when the head is a one- or
     two-deconv head the tiling covers; everything else takes the full-precision CUDA-core kernels.  Training uses
     ``HeatmapHead`` which adds the backward.
     """

@@ -6,7 +6,7 @@ list of per-batch ``(keypoints, confidences)`` tuples (:472-521); ``PredictionHa
 ``(x, y, likelihood)`` columns with numpy (:180-206) and labels them with a DLC-style MultiIndex (:551-570).  It always
 runs with ``devices=1`` (:352, :474).
 
-Here one *chunk* of ``T`` frames is one CUDA-graph replay: head (tcgen05) -> soft-argmax decode -> model->frame remap ->
+Here one *chunk* of ``T`` frames is one CUDA-graph replay: head -> soft-argmax decode -> model->frame remap ->
 rows of a preallocated ``(N, 3K)`` device table at a device-resident cursor (``lpb_pack_predictions``).  Nothing
 returns to the host until the video is done; then ONE device->host copy of the table.  The table's column order is the
 reference's, so ``PredictionHandler.make_pred_arr_undo_resize`` / ``make_dlc_pandas_index`` below produce the same CSV.

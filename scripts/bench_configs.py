@@ -1,4 +1,4 @@
-"""Informal timings of the other BASELINE configs' hot paths (configs 3, 4, 5) on one B200: not bench lines (bench.py
+"""Informal timings of the other BASELINE configs' hot paths (configs 3, 4, 5) on one GPU: not bench lines (bench.py
 measures configs[1]), but the numbers DESIGN.md quotes for them.  Writes gpurun_out/r02_configs.json."""
 import json
 import os

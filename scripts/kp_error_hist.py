@@ -1,4 +1,4 @@
-"""Distribution of |d(x, y)| between the bf16 tcgen05 head (+ decode) and the fp32 CPU oracle on identical inputs
+"""Distribution of |d(x, y)| between the bf16 tensor-core head (+ decode) and the fp32 CPU oracle on identical inputs
 (BASELINE configs[1] shapes, bench.py's "trained-like" regime and a random-weights regime).  GPU box.
 Writes gpurun_out/r02_bf16_keypoint_error.json (copied to profiles/ afterwards)."""
 import json

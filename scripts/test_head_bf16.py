@@ -1,4 +1,4 @@
-"""Stand-alone check of the tcgen05 head (run under `timeout`): compares the intermediate activations
+"""Stand-alone check of the tensor-core head (run under `timeout`): compares the intermediate activations
 (k1a) and the final heatmaps (k1b) with the oracle on identically bf16-rounded tensors."""
 import ctypes as C
 import os

@@ -1,4 +1,4 @@
-"""Bring-up check of the tcgen05 head backward: every gradient vs torch autograd (fp32 math on bf16-rounded
+"""Bring-up check of the tensor-core head backward: every gradient vs torch autograd (fp32 math on bf16-rounded
 operands, same mid rounding as the forward kernel).  Run on the GPU box: python scripts/test_head_bwd_bf16.py"""
 import sys
 import time

@@ -1,4 +1,4 @@
-"""UMMA descriptor self-tests (K-major / MN-major views of the row layout, row shifts, TMEM column offsets)."""
+"""Tensor-core operand self-tests (K-major / MN-major views of the row layout, row shifts; col_off has no effect)."""
 import ctypes as C
 import os
 import sys

@@ -32,7 +32,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(_lib.lib, s), f"{s} declared in lpb200.h but not exported by liblpb200.so"
     assert sorted(_lib.SIGNATURES) == syms, "ctypes signature table out of sync with the header"
     assert _lib.lib.lpb_version() >= 100
-    assert _lib.lib.lpb_build_arch() == b"sm_100a"
+    assert _lib.lib.lpb_build_arch() == b"sm_90a"
 
 
 def test_argument_validation_without_gpu():
@@ -169,14 +169,14 @@ def test_round2_entry_points_validate_arguments_without_gpu():
 
     L = _lib.lib
     plan = C.c_int(-1)
-    assert L.lpb_head_bf16_plan(2048, 12, 12, 17, 17, C.byref(plan)) == 0 and plan.value == 1   # cfg 2: whole frame in TMEM
+    assert L.lpb_head_bf16_plan(2048, 12, 12, 17, 17, C.byref(plan)) == 0 and plan.value == 1   # cfg 2: whole-frame kernels
     assert L.lpb_head_bf16_plan(2048, 16, 16, 17, 17, C.byref(plan)) == 0 and plan.value == 0   # cfg 5: banded
     assert L.lpb_head_bf16_plan(384, 16, 16, 17, 0, C.byref(plan)) == 0 and plan.value == 0     # cfg 3: one deconv
     assert L.lpb_head_bf16_plan(384, 24, 24, 17, 0, C.byref(plan)) == 0 and plan.value == 0     # cfg 4
     assert L.lpb_head_bf16_plan(100, 12, 12, 17, 17, C.byref(plan)) == -1                          # C % 128
     assert L.lpb_head_bf16_plan(2048, 12, 12, 20, 17, C.byref(plan)) == -1                         # c1 must leave the ones channel
     n = C.c_size_t(0)
-    assert L.lpb_head_bf16_workspace_bytes(2, 384, 16, 16, 17, 0, C.byref(n)) == 0 and n.value == 3 * 20480 + 20480 + 1024  # no mid for one deconv; + split-softmax statistics (2 frames x 3 bands x 20 x 2 floats -> 1 KB)
+    assert L.lpb_head_bf16_workspace_bytes(2, 384, 16, 16, 17, 0, C.byref(n)) == 0 and n.value == 3 * 20480 + 20480 + 1792  # no mid for one deconv; + split-softmax statistics (2 frames x 5 bands x 20 x 2 floats, 256-byte aligned)
     assert L.lpb_head_bwd_bf16_workspace_bytes(2, 384, 16, 16, 17, 0, C.byref(n)) == 0 and n.value > 0
     for rc in (
         L.lpb_convt_fwd_f32(None, 1, 4, 4, 4, 1, None, None, 2, None, None),

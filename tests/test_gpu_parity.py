@@ -390,7 +390,7 @@ def test_tracker_semisupervised_step_vs_oracle(lpb, dev):
 
 
 # ------------------------------------------------------------------------------------------------
-# bf16 tensor-core head (tcgen05): north_star tolerance 1e-2 against the oracle on bf16-rounded tensors
+# bf16 tensor-core head: north_star tolerance 1e-2 against the oracle on bf16-rounded tensors
 # ------------------------------------------------------------------------------------------------
 def _bf16_head_oracle(feats_bf16, head):
     import torch.nn.functional as F
@@ -416,7 +416,7 @@ def test_head_bf16_tcgen05_vs_oracle(lpb, dev, shape):
     feats = (torch.randn(b, c, fh, fw) * 0.5).bfloat16()
     logits_ref, hm_ref = _bf16_head_oracle(feats, head)
     head = head.to(dev)
-    with torch.no_grad():  # forward-only: every listed shape is inside the tcgen05 forward tiling (training on the 4x6
+    with torch.no_grad():  # forward-only: every listed shape is inside the tensor-core forward tiling (training on the 4x6
         out = head(feats.to(dev))  # map, whose width has no dgrad epilogue, is routed to the fp32 kernels instead)
     assert out.dtype == torch.float32 and out.shape == hm_ref.shape
     # 1e-2 relative (north star, bf16).  A mid activation that sits on a bf16 rounding boundary may round the
@@ -435,9 +435,35 @@ def test_head_bf16_tcgen05_vs_oracle(lpb, dev, shape):
     assert float(((kp.cpu() - kp_ref).abs().reshape(b, 17, 2).amax(-1))[conf_ok].max()) < 0.5
 
 @pytest.mark.gpu
+def test_head_bf16_backward_is_bitwise_reproducible(lpb, dev):
+    """lpb_head_bwd_bf16 sums its gradients over CTAs in a fixed order: two identical backward calls (dense gradient of the
+    softmax output, enough frames for many weight-gradient and b2d CTAs) give bit-identical gradients."""
+    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
+
+    b, k = 64, 17
+    torch.manual_seed(31)
+    head = HeatmapHead("resnet50", 2048, k)
+    for layer in list(head.upsampling_layers)[1:]:
+        torch.nn.init.xavier_uniform_(layer.weight, gain=3.0)
+        torch.nn.init.uniform_(layer.bias, -0.3, 0.3)
+    head = head.to(dev)
+    feats = (torch.randn(b, 2048, 12, 12) * 0.5).bfloat16().to(dev)
+    gout = torch.randn(b, k, 96, 96, device=dev)
+    runs = []
+    for _ in range(2):
+        head.zero_grad(set_to_none=True)
+        f = feats.clone().requires_grad_(True)
+        (head(f) * gout).sum().backward()
+        runs.append([f.grad.clone()] + [p.grad.clone() for p in head.parameters() if p.grad is not None])
+    assert len(runs[0]) == 5  # d features, dw1, db1, dw2, db2
+    for x, y in zip(*runs):
+        assert torch.equal(x, y)
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("softmax", [True, False])
 def test_head_bf16_tcgen05_backward_vs_oracle_autograd(lpb, dev, softmax):
-    """lpb_head_bwd_bf16 (dgrad + wgrad on tcgen05) against fp32 autograd of the oracle head evaluated on the
+    """lpb_head_bwd_bf16 (dgrad + wgrad on tensor-core) against fp32 autograd of the oracle head evaluated on the
     same bf16-rounded operands; tolerance 1e-2 of each gradient's max (north star, bf16)."""
     import torch.nn.functional as F
     from lightning_pose_b200.models.heads.heatmap import HeatmapHead
@@ -993,7 +1019,7 @@ def test_mhcrnn_backward_vs_oracle_autograd(lpb, dev, golden, tag, arch, uf):
 
 
 def test_mhcrnn_bf16_real_shape_and_tracker(lpb, dev):
-    """config 3: ViT-S features (384, 16, 16) of a 256x256 clip, bf16, through the tcgen05 deconv maps + recurrence kernel."""
+    """config 3: ViT-S features (384, 16, 16) of a 256x256 clip, bf16, through the tensor-core deconv maps + recurrence kernel."""
     from lightning_pose_b200.models.heatmap_tracker_mhcrnn import SemiSupervisedHeatmapTrackerMHCRNN
     from lightning_pose_b200.losses.factory import LossFactory
 
