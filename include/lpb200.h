@@ -343,6 +343,52 @@ int lpb_unsup_losses_bwd(const float* keypoints, const float* confidences, int64
                          const lpb_pca_desc* pca_singleview, const lpb_pca_desc* pca_multiview,
                          const float* grad_out, float* grad_keypoints, void* stream);
 
+/* ---- calibrated multi-view geometry (lightning-pose 3-D mode) ------------------------------------
+ * Camera tensors per (batch, view), fp32, as the batch dict carries them: intrinsics [B, V, 3, 3], extrinsics
+ * [B, V, 3, 4], dist [B, V, P] with P in {4, 5, 8, 12} (OpenCV order k1 k2 p1 p2 k3 k4 k5 k6 s1 s2 s3 s4; tilt, P = 14,
+ * is rejected).  The distortion model reads fx, fy, cx, cy only.  Per-point geometry is evaluated in fp64.  Cameras
+ * get no gradient.  Backward calls sum every input gradient in one thread in a fixed order (bit-reproducible) and give
+ * NaN inputs a zero gradient.  2 <= V <= 64 for triangulation, 1 <= V <= 64 for projection.
+ *
+ * replaces project_camera_pairs_to_3d  lightning_pose/data/cameras.py:22-83
+ *   points [B, V, K, 2] frame pixels -> out [B, V(V-1)/2, K, 3], pairs in itertools.combinations order; undistortion
+ *   (kornia undistort_points, new_K = I, 5 iterations) then the DLT of each pair (smallest right singular vector,
+ *   kornia triangulate_points / convert_points_from_homogeneous).  A keypoint NaN in either view gives a NaN triple. */
+int lpb_triangulate_pairs_fwd(const float* points, const float* intrinsics, const float* extrinsics, const float* dist, int B,
+                              int V, int K, int P, float* out, void* stream);
+/* d loss / d points given d loss / d out (grad_out [B, V(V-1)/2, K, 3]); grad_points [B, V, K, 2] is overwritten. */
+int lpb_triangulate_pairs_bwd(const float* points, const float* intrinsics, const float* extrinsics, const float* dist,
+                              const float* grad_out, int B, int V, int K, int P, float* grad_points, void* stream);
+
+/* replaces project_3d_to_2d  lightning_pose/data/cameras.py:86-171  (+ torch.mean(dim=1) before it and
+ * frame_to_model_batch, lightning_pose/data/bboxes.py:194-219, after it, as the tracker chains them:
+ * lightning_pose/models/heatmap_tracker_multiview.py:281-291)
+ *   points3d [B, K, 3] (n_pairs = 0) or [B, n_pairs, K, 3] averaged over the pair axis first (NaN-propagating);
+ *   out [B, V, K, 2]: pinhole projection with K E, then distortion for the (b, v) whose dist row is not all zero, then
+ *   (bbox [B, 4V] of [x, y, h, w] per view, or NULL) frame -> model coordinates of a model_height x model_width input.
+ *   A NaN point is NaN in every view. */
+int lpb_project_points_fwd(const float* points3d, int n_pairs, const float* intrinsics, const float* extrinsics, const float* dist,
+                           const float* bbox, float model_height, float model_width, int B, int V, int K, int P, float* out,
+                           void* stream);
+/* d loss / d points3d given d loss / d out; grad_points3d (the shape of points3d) is overwritten. */
+int lpb_project_points_bwd(const float* points3d, int n_pairs, const float* intrinsics, const float* extrinsics, const float* dist,
+                           const float* bbox, float model_height, float model_width, const float* grad_out, int B, int V, int K,
+                           int P, float* grad_points3d, void* stream);
+
+/* replaces frame_to_model_batch  lightning_pose/data/bboxes.py:194-219
+ *   keypoints [B, V, K, 2] frame pixels -> out [B, V, K, 2]: ((x - bx) / bw * model_width, (y - by) / bh * model_height)
+ *   with bbox [B, 4V] = [x, y, h, w] per view; grad != 0 applies the linear part only (the backward). */
+int lpb_frame_to_model(const float* keypoints, int B, int V, int K, const float* bbox, float model_height, float model_width,
+                       int grad, float* out, void* stream);
+
+/* replaces PairwiseProjectionsLoss.__call__ (compute_loss + remove_nans + mean)  lightning_pose/losses/losses.py:1014-1126
+ * targets [B, K, 3], preds [B, n_pairs, K, 3]: mean L2 distance over the (b, pair, k) with neither side NaN, 0 when
+ * none is (no boolean gather, fixed-order reduction in one CTA).  out[0] = loss, out[1] = number of kept entries. */
+int lpb_pairwise_projections_loss_fwd(const float* targets, const float* preds, int B, int n_pairs, int K, float* out, void* stream);
+/* d loss / d preds (targets get no gradient); fwd_out = the forward's out, grad_out [1]; grad_preds is overwritten. */
+int lpb_pairwise_projections_loss_bwd(const float* targets, const float* preds, int B, int n_pairs, int K, const float* fwd_out,
+                                      const float* grad_out, float* grad_preds, void* stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * Tensor-core operand self-test (bring-up aid): one-CTA GEMM over operands in the library's row layout
  * [kchunk][row][8] bf16; mode 0 = K-major view, 1 = MN-major view; d [128][n] fp32.  col_off has no effect

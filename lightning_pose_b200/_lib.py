@@ -80,6 +80,13 @@ SIGNATURES = {
     "lpb_selftest_umma": (C.c_int, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "lpb_unsup_losses_fwd": (C.c_int, [_P, _P, _L, _I, _I, _P, _F, _I, C.POINTER(PcaDesc), C.POINTER(PcaDesc), _P, _P]),
     "lpb_unsup_losses_bwd": (C.c_int, [_P, _P, _L, _I, _I, _P, _F, _I, C.POINTER(PcaDesc), C.POINTER(PcaDesc), _P, _P, _P]),
+    "lpb_triangulate_pairs_fwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
+    "lpb_triangulate_pairs_bwd": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
+    "lpb_project_points_fwd": (C.c_int, [_P, _I, _P, _P, _P, _P, _F, _F, _I, _I, _I, _I, _P, _P]),
+    "lpb_project_points_bwd": (C.c_int, [_P, _I, _P, _P, _P, _P, _F, _F, _P, _I, _I, _I, _I, _P, _P]),
+    "lpb_frame_to_model": (C.c_int, [_P, _I, _I, _I, _P, _F, _F, _I, _P, _P]),
+    "lpb_pairwise_projections_loss_fwd": (C.c_int, [_P, _P, _I, _I, _I, _P, _P]),
+    "lpb_pairwise_projections_loss_bwd": (C.c_int, [_P, _P, _I, _I, _I, _P, _P, _P, _P]),
 }
 
 

@@ -1,6 +1,7 @@
 """Model -> frame coordinate transform: the hot-path part of ``lightning_pose.data.bboxes``.
 
-``model_to_frame_batch`` (reference ``data/bboxes.py:222-288``) and ``norm_to_frame`` (:74-105).
+``model_to_frame_batch`` (reference ``data/bboxes.py:222-288``), ``norm_to_frame`` (:74-105) and, for the calibrated
+multi-view losses, ``frame_to_model_batch`` (:194-219).
 Like the reference, ``in_place=True`` writes the result through the caller's tensor.
 """
 from __future__ import annotations
@@ -42,3 +43,12 @@ def model_to_frame_batch(batch_dict: dict, model_keypoints: torch.Tensor, in_pla
         in_place = False
     out = ops.remap_keypoints(kp, None, bbox, model_height, model_width, num_views=num_views, out=kp if in_place else None)
     return out.reshape(-1, model_keypoints.shape[1])
+
+
+def frame_to_model_batch(batch_dict: dict, frame_keypoints: torch.Tensor) -> torch.Tensor:
+    """(batch, num_views, num_keypoints, 2) frame pixels -> model-input pixels (reference ``data/bboxes.py:194-219``).
+
+    The v-th bbox quadruple [x, y, h, w] of ``batch_dict['bbox']`` maps view v; the model size is that of
+    ``batch_dict['images']``.  Returns a new tensor, differentiable in ``frame_keypoints``."""
+    img = batch_dict["images"]
+    return ops.frame_to_model(frame_keypoints, batch_dict["bbox"], img.shape[-2], img.shape[-1])

@@ -13,6 +13,7 @@ is one fused CUDA reduction (``csrc/losses.cu``) that produces the same scalar:
 * ``TemporalLoss`` / ``PCALoss``     -> ``ops.unsup_losses`` (one launch; the factory shares it)
 * ``TemporalHeatmapLoss``           -> ``ops.temporal_heatmap_loss``
 * ``ReprojectionHeatmapLoss``       -> ``ops.generate_heatmaps`` (differentiable) + ``ops.heatmap_loss``
+* ``PairwiseProjectionsLoss``       -> ``ops.pairwise_projections_loss`` (NaN entries dropped on device)
 
 The staged methods remain as small tensor utilities for callers/tests that use them directly; the
 coordinate-regression losses (not on the heatmap path) are plain tensor code.
@@ -378,7 +379,8 @@ class RegressionRMSELoss(RegressionMSELoss):
 
 
 class PairwiseProjectionsLoss(Loss):
-    """3D consistency across camera pairs (multiview + calibration only; surface kept)."""
+    """3D consistency across camera pairs (multiview + calibration only).  ``__call__`` is one CUDA reduction
+    (``ops.pairwise_projections_loss``); ``compute_loss`` / ``remove_nans`` stay as the staged tensor helpers."""
 
     loss_name = "supervised_pairwise_projections"
 
@@ -412,8 +414,7 @@ class PairwiseProjectionsLoss(Loss):
                 f"3D keypoints not available for {stage} stage. Camera params file is required but not found;"
                 "Turn off supervised_pairwise_projections loss to avoid this error."
             )
-        clean = self.remove_nans(loss=self.compute_loss(targets=keypoints_targ_3d, predictions=keypoints_pred_3d))
-        scalar_loss = self.reduce_loss(clean, method="mean")
+        scalar_loss = ops.pairwise_projections_loss(keypoints_targ_3d, keypoints_pred_3d)
         return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
 
 

@@ -9,9 +9,10 @@ supervised / multi-view PCA losses then run on that folded tensor.
 The transformer blocks themselves are the backbone (dense contractions supplied by a library module); this mirror owns
 what sits on this repository's path: the view-embedding / token bookkeeping of ``forward_vit``, the head on
 ``views * batch`` feature maps (BASELINE config 4: (8 x 4, 384, 24, 24) -> (8, 68, 96, 96) through the banded tensor-core
-kernels), the fold, and the loss inputs.  3-D triangulation (``project_camera_pairs_to_3d``, needs camera calibration and
-aniposelib) is out of scope: the corresponding dict entries are ``None``, exactly what the reference returns for
-uncalibrated data (:299-307).
+kernels), the fold, and the loss inputs.  Calibrated batches (``keypoints_3d`` plus per-view intrinsics, extrinsics and
+distortions) also get the 3-D entries the pairwise-projection and reprojection losses read (:263-303), computed by the
+camera kernels without a host sync; uncalibrated batches get ``None`` there, as in the reference (:300-303).  Unlike
+the reference, malformed camera inputs raise instead of being logged and turned into ``None``.
 """
 from __future__ import annotations
 
@@ -21,7 +22,9 @@ from typing import Any, Callable, Literal
 import torch
 from torch import nn
 
+from lightning_pose_b200 import ops
 from lightning_pose_b200.data.bboxes import model_to_frame_batch
+from lightning_pose_b200.data.cameras import project_camera_pairs_to_3d
 from lightning_pose_b200.losses.factory import LossFactory
 from lightning_pose_b200.losses.losses import RegressionRMSELoss
 from lightning_pose_b200.models.heads.heatmap import HeatmapHead
@@ -86,15 +89,30 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         pred_heatmaps, pred_keypoints, confidence = self.forward_with_keypoints(batch_dict["images"])
         target_keypoints = model_to_frame_batch(batch_dict, batch_dict["keypoints"])
         pred_keypoints = model_to_frame_batch(batch_dict, pred_keypoints)
+        keypoints_targ_3d = keypoints_pred_3d = keypoints_pred_2d_reprojected = None
+        # calibrated batches (reference :263-303): triangulate every camera pair; with the reprojection loss registered,
+        # also project the pair mean back into every view, in model coordinates (one launch: mean + project + frame->model)
+        if "keypoints_3d" in batch_dict and batch_dict["keypoints_3d"].shape[-1] == 3:
+            num_views = batch_dict["images"].shape[1]
+            num_keypoints = pred_keypoints.shape[1] // 2 // num_views
+            cameras = (batch_dict["intrinsic_matrix"], batch_dict["extrinsic_matrix"], batch_dict["distortions"])
+            keypoints_pred_3d = project_camera_pairs_to_3d(pred_keypoints.reshape(-1, num_views, num_keypoints, 2), *cameras)
+            keypoints_targ_3d = batch_dict["keypoints_3d"]
+            assert self.loss_factory is not None
+            if "supervised_reprojection_heatmap_mse" in self.loss_factory.loss_instance_dict:
+                images = batch_dict["images"]
+                keypoints_pred_2d_reprojected = ops.project_points(
+                    keypoints_pred_3d, *cameras, mean_over_pairs=True, bbox=batch_dict["bbox"], model_size=images.shape[-2:],
+                ).reshape(-1, num_views * num_keypoints, 2)
         return {
             "heatmaps_targ": batch_dict["heatmaps"],
             "heatmaps_pred": pred_heatmaps,
             "keypoints_targ": target_keypoints,
             "keypoints_pred": pred_keypoints,
             "confidences": confidence,
-            "keypoints_targ_3d": None,  # calibrated 3-D losses are out of scope (module docstring)
-            "keypoints_pred_3d": None,
-            "keypoints_pred_2d_reprojected": None,
+            "keypoints_targ_3d": keypoints_targ_3d,  # (batch, num_keypoints, 3)
+            "keypoints_pred_3d": keypoints_pred_3d,  # (batch, cam_pairs, num_keypoints, 3)
+            "keypoints_pred_2d_reprojected": keypoints_pred_2d_reprojected,  # (batch, num_views * num_keypoints, 2)
         }
 
     def predict_step(self, batch_dict: dict, batch_idx: int, return_heatmaps: bool = False):

@@ -31,6 +31,10 @@ __all__ = [
     "temporal_heatmap_loss",
     "unsup_losses",
     "PcaParams",
+    "triangulate_pairs",
+    "project_points",
+    "frame_to_model",
+    "pairwise_projections_loss",
 ]
 
 _KIND = {"mse": 0, "kl": 1, "js": 2}
@@ -731,3 +735,167 @@ def unsup_losses(keypoints, confidences=None, temporal_eps=None, prob_threshold=
             raise ValueError(f"temporal epsilon has {te.numel()} entries for {k} keypoints")
     out = _UnsupLosses.apply(kp, cf, te, prob_threshold, te is not None, pca_singleview, pca_multiview)
     return out[0] if squeeze else out
+
+
+# =====================================================================================
+# calibrated multi-view geometry (csrc/cameras.cu)
+# =====================================================================================
+_DIST_PARAMS = (4, 5, 8, 12)
+
+
+def _camera_tensors(intrinsics, extrinsics, dist, b, v):
+    """Batch-dict camera tensors -> contiguous fp32 CUDA tensors of the checked shapes (no gradient: batch data)."""
+    k = _cuda_f32(intrinsics, "intrinsics").detach()
+    e = _cuda_f32(extrinsics, "extrinsics").detach()
+    d = _cuda_f32(dist, "dist").detach()
+    if tuple(k.shape) != (b, v, 3, 3) or tuple(e.shape) != (b, v, 3, 4) or d.dim() != 3 or tuple(d.shape[:2]) != (b, v):
+        raise ValueError(f"cameras for {b} x {v} views: intrinsics {tuple(k.shape)} (want (B, V, 3, 3)), extrinsics "
+                         f"{tuple(e.shape)} (want (B, V, 3, 4)), dist {tuple(d.shape)} (want (B, V, P))")
+    if d.shape[-1] not in _DIST_PARAMS:
+        raise ValueError(f"dist has {d.shape[-1]} coefficients per view; supported: 4, 5, 8 or 12 (tilt distortion, 14, is not)")
+    return k, e, d
+
+
+class _TriangulatePairs(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pts, k, e, d):
+        b, v, n, _ = pts.shape
+        out = torch.empty((b, v * (v - 1) // 2, n, 3), device=pts.device, dtype=torch.float32)
+        with torch.cuda.device(pts.device):
+            check(lib.lpb_triangulate_pairs_fwd(_ptr(pts), _ptr(k), _ptr(e), _ptr(d), b, v, n, d.shape[-1], _ptr(out), _stream()))
+        ctx.save_for_backward(pts, k, e, d)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        pts, k, e, d = ctx.saved_tensors
+        b, v, n, _ = pts.shape
+        g = g.contiguous().float()
+        gp = torch.empty_like(pts)
+        with torch.cuda.device(pts.device):
+            check(lib.lpb_triangulate_pairs_bwd(_ptr(pts), _ptr(k), _ptr(e), _ptr(d), _ptr(g), b, v, n, d.shape[-1], _ptr(gp), _stream()))
+        return gp, None, None, None
+
+
+def triangulate_pairs(points, intrinsics, extrinsics, dist):
+    """(B, V, K, 2) frame pixels -> (B, V(V-1)/2, K, 3): undistort, then DLT per camera pair (combinations order).
+    Differentiable in ``points``."""
+    pts = _cuda_f32(points, "points")
+    if pts.dim() != 4 or pts.shape[-1] != 2 or pts.shape[1] < 2:
+        raise ValueError(f"points must be (batch, num_views >= 2, num_keypoints, 2); got {tuple(pts.shape)}")
+    k, e, d = _camera_tensors(intrinsics, extrinsics, dist, pts.shape[0], pts.shape[1])
+    return _TriangulatePairs.apply(pts, k, e, d)
+
+
+class _ProjectPoints(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, p3, n_pairs, k, e, d, bbox, model_height, model_width):
+        b, v = k.shape[:2]
+        n = p3.shape[-2]
+        out = torch.empty((b, v, n, 2), device=p3.device, dtype=torch.float32)
+        with torch.cuda.device(p3.device):
+            check(lib.lpb_project_points_fwd(_ptr(p3), n_pairs, _ptr(k), _ptr(e), _ptr(d), _ptr(bbox), model_height, model_width,
+                                             b, v, n, d.shape[-1], _ptr(out), _stream()))
+        ctx.save_for_backward(p3, k, e, d, bbox)
+        ctx.meta = (n_pairs, model_height, model_width)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        p3, k, e, d, bbox = ctx.saved_tensors
+        n_pairs, mh, mw = ctx.meta
+        b, v = k.shape[:2]
+        g = g.contiguous().float()
+        gp = torch.empty_like(p3)
+        with torch.cuda.device(p3.device):
+            check(lib.lpb_project_points_bwd(_ptr(p3), n_pairs, _ptr(k), _ptr(e), _ptr(d), _ptr(bbox), mh, mw, _ptr(g),
+                                             b, v, p3.shape[-2], d.shape[-1], _ptr(gp), _stream()))
+        return gp, None, None, None, None, None, None, None
+
+
+def project_points(points_3d, intrinsics, extrinsics, dist, mean_over_pairs=False, bbox=None, model_size=None):
+    """(B, K, 3) world points -> (B, V, K, 2) frame pixels (pinhole K E, then distortion where a view has any).
+
+    ``mean_over_pairs``: ``points_3d`` is (B, pairs, K, 3) and is averaged over the pair axis first (NaN-propagating, as
+    ``torch.mean(dim=1)``).  ``bbox`` (B, 4V) with ``model_size`` (height, width): the result is in model coordinates
+    (``frame_to_model``).  One launch each way; differentiable in ``points_3d``."""
+    p3 = _cuda_f32(points_3d, "points_3d")
+    if p3.shape[-1] != 3 or p3.dim() != (4 if mean_over_pairs else 3):
+        raise ValueError(f"points_3d must be {'(batch, pairs, num_keypoints, 3)' if mean_over_pairs else '(batch, num_keypoints, 3)'}; got {tuple(p3.shape)}")
+    b, v = p3.shape[0], intrinsics.shape[1]
+    k, e, d = _camera_tensors(intrinsics, extrinsics, dist, b, v)
+    bb, mh, mw = None, 0.0, 0.0
+    if bbox is not None:
+        bb = _cuda_f32(bbox, "bbox").detach()
+        if tuple(bb.shape) != (b, 4 * v) or model_size is None:
+            raise ValueError(f"bbox must be (batch, 4 * num_views) = ({b}, {4 * v}) with a model_size; got {tuple(bb.shape)}")
+        mh, mw = float(model_size[0]), float(model_size[1])
+    return _ProjectPoints.apply(p3, p3.shape[1] if mean_over_pairs else 0, k, e, d, bb, mh, mw)
+
+
+class _FrameToModel(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, kp, bbox, model_height, model_width):
+        b, v, n, _ = kp.shape
+        out = torch.empty_like(kp)
+        with torch.cuda.device(kp.device):
+            check(lib.lpb_frame_to_model(_ptr(kp), b, v, n, _ptr(bbox), model_height, model_width, 0, _ptr(out), _stream()))
+        ctx.save_for_backward(bbox)
+        ctx.meta = (model_height, model_width)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (bbox,) = ctx.saved_tensors
+        mh, mw = ctx.meta
+        g = g.contiguous().float()
+        b, v, n, _ = g.shape
+        gi = torch.empty_like(g)
+        with torch.cuda.device(g.device):
+            check(lib.lpb_frame_to_model(_ptr(g), b, v, n, _ptr(bbox), mh, mw, 1, _ptr(gi), _stream()))
+        return gi, None, None, None
+
+
+def frame_to_model(keypoints, bbox, model_height, model_width):
+    """(B, V, K, 2) frame pixels -> model pixels with per-view bbox [x, y, h, w] (B, 4V); differentiable in keypoints."""
+    kp = _cuda_f32(keypoints, "frame_keypoints")
+    if kp.dim() != 4 or kp.shape[-1] != 2:
+        raise ValueError(f"frame_keypoints must be (batch, num_views, num_keypoints, 2); got {tuple(kp.shape)}")
+    bb = _cuda_f32(bbox, "bbox").detach()
+    if tuple(bb.shape) != (kp.shape[0], 4 * kp.shape[1]):
+        raise ValueError(f"bbox must be (batch, 4 * num_views) = ({kp.shape[0]}, {4 * kp.shape[1]}); got {tuple(bb.shape)}")
+    return _FrameToModel.apply(kp, bb, float(model_height), float(model_width))
+
+
+class _PairwiseProjectionsLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, targ, pred):
+        b, p, n, _ = pred.shape
+        out = torch.empty((2,), device=pred.device, dtype=torch.float32)
+        with torch.cuda.device(pred.device):
+            check(lib.lpb_pairwise_projections_loss_fwd(_ptr(targ), _ptr(pred), b, p, n, _ptr(out), _stream()))
+        ctx.save_for_backward(targ, pred, out)
+        loss, count = out[0].clone(), out[1].clone()
+        ctx.mark_non_differentiable(count)
+        return loss, count
+
+    @staticmethod
+    def backward(ctx, g, _g_count):
+        targ, pred, out = ctx.saved_tensors
+        b, p, n, _ = pred.shape
+        gp = torch.empty_like(pred)
+        gg = g.reshape(1).contiguous().float()
+        with torch.cuda.device(pred.device):
+            check(lib.lpb_pairwise_projections_loss_bwd(_ptr(targ), _ptr(pred), b, p, n, _ptr(out), _ptr(gg), _ptr(gp), _stream()))
+        return None, gp
+
+
+def pairwise_projections_loss(targets, preds, return_count=False):
+    """Mean L2 distance between targets (B, K, 3) and per-pair predictions (B, pairs, K, 3) over entries with neither
+    side NaN; 0 (with a zero gradient) when there is none.  Differentiable in ``preds``."""
+    t = _cuda_f32(targets, "keypoints_targ_3d").detach()
+    p = _cuda_f32(preds, "keypoints_pred_3d")
+    if t.dim() != 3 or p.dim() != 4 or t.shape[-1] != 3 or p.shape[-1] != 3 or t.shape[0] != p.shape[0] or t.shape[1] != p.shape[2]:
+        raise ValueError(f"targets (batch, num_keypoints, 3) vs predictions (batch, pairs, num_keypoints, 3): {tuple(t.shape)} / {tuple(p.shape)}")
+    loss, count = _PairwiseProjectionsLoss.apply(t, p)
+    return (loss, count) if return_count else loss

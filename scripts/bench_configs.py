@@ -119,6 +119,83 @@ for use_graph, sub in ((True, None), (False, None), (True, 48)):
         "frames": chunk * nchunks, "ms": ms, "frames_per_s": chunk * nchunks / ms * 1e3, "algorithmic_bytes": nb, "frac_hbm": nb / ms / 1e6 / pk["hbm_gbs"],
         "mean_confidence": float(cf.mean()),
         "note": "trained-like planted response (unimodal heatmaps); features resident on the device (includes the D2D copy of each chunk into the graph's static input); K1+K2 algorithmic bytes = features + 204 B/frame"}
+
+# config 4 with a camera calibration (B = 8 per rank, 4 views, 17 keypoints, 384x384): the 3-D stage alone (pairwise
+# triangulation -> pair-mean reprojection into model coordinates -> pairwise-projection loss), forward and backward, and
+# the labeled multiview step (forward + backward, heatmap MSE) with the two 3-D losses on and off.  The transformer is a
+# stand-in (patch conv + one token-mixing linear layer), so the step time is the head + decode + loss path.
+import math  # noqa: E402
+import subprocess  # noqa: E402
+
+from lightning_pose_b200.losses.factory import LossFactory  # noqa: E402
+from lightning_pose_b200.models.heatmap_tracker_multiview import HeatmapTrackerMultiviewTransformer  # noqa: E402
+
+cb, cv, img = 8, 4, 384
+gen = torch.Generator().manual_seed(41)
+Kc, Ec = torch.zeros(cb, cv, 3, 3), torch.zeros(cb, cv, 3, 4)
+for j in range(cv):
+    a = j / cv * math.pi  # cameras on a half circle, none facing another
+    Kc[:, j] = torch.tensor([[800.0, 0.0, img / 2], [0.0, 800.0, img / 2], [0.0, 0.0, 1.0]])
+    Ec[:, j] = torch.tensor([[math.cos(a), 0.0, -math.sin(a), 0.0], [0.0, 1.0, 0.0, 0.0], [math.sin(a), 0.0, math.cos(a), 2.0]])
+Dc = torch.randn(cb, cv, 5, generator=gen) * 0.05
+cams = [t.to(dev) for t in (Kc, Ec, Dc)]
+kp_frame = (img / 2 - 2 + torch.rand(cb, cv, K, 2, generator=gen) * 4).to(dev).requires_grad_(True)
+kp3 = (torch.randn(cb, K, 3, generator=gen) * 0.3).to(dev)
+bbox_c = torch.tensor([[img / 2 - 2, img / 2 - 2, 4.0, 4.0] * cv], device=dev).repeat(cb, 1)  # rays near the optical axes
+
+
+def stage3d():
+    p3d = ops.triangulate_pairs(kp_frame, *cams)
+    rep = ops.project_points(p3d, *cams, mean_over_pairs=True, bbox=bbox_c, model_size=(img, img))
+    return ops.pairwise_projections_loss(kp3, p3d) + rep.sum() * 1e-6
+
+
+with torch.no_grad():
+    ms, _ = bench.time_stage(stage3d, flush)
+res["cfg4_calibrated_3d_stage_fwd"] = {"frames": cb * cv, "ms": ms, "launches": 3}
+ms, _ = bench.time_stage(lambda: torch.autograd.grad(stage3d(), kp_frame), flush)
+res["cfg4_calibrated_3d_stage_fwd+bwd"] = {"frames": cb * cv, "ms": ms, "launches": 6, "note": "includes torch autograd bookkeeping and the small elementwise ops it adds"}
+
+
+class Patch(torch.nn.Module):
+    def __init__(self):
+        super().__init__()
+        self.proj = torch.nn.Conv2d(3, 384, 16, stride=16)
+
+    def forward(self, x):
+        return self.proj(x).flatten(2).transpose(1, 2)
+
+
+class Mix(torch.nn.Module):
+    def __init__(self):
+        super().__init__()
+        self.lin = torch.nn.Linear(384, 384)
+
+    def forward(self, t):
+        return (self.lin(t) + t.mean(1, keepdim=True)).bfloat16()
+
+
+kp_model = (torch.rand(cb, cv * K * 2, generator=gen) * img).to(dev)
+batch = {"images": torch.randn(cb, cv, 3, img, img, generator=gen).to(dev), "keypoints": kp_model.clone(),
+         "heatmaps": ops.generate_heatmaps(kp_model.reshape(cb, cv * K, 2), img, img, (96, 96)), "bbox": bbox_c, "is_multiview": True,
+         "keypoints_3d": kp3, "intrinsic_matrix": cams[0], "extrinsic_matrix": cams[1], "distortions": cams[2]}
+losses_on = {"heatmap_mse": {"log_weight": 0.0}, "supervised_pairwise_projections": {"log_weight": 0.0},
+             "supervised_reprojection_heatmap_mse": {"log_weight": 0.0, "original_image_height": img, "original_image_width": img,
+                                                     "downsampled_image_height": 96, "downsampled_image_width": 96}}
+for tag, losses in (("3d_losses_off", {"heatmap_mse": {"log_weight": 0.0}}), ("3d_losses_on", losses_on)):
+    torch.manual_seed(3)
+    tr = HeatmapTrackerMultiviewTransformer(K, cv, Patch(), Mix(), 384, loss_factory=LossFactory(losses, None)).to(dev)
+    params = list(tr.head.parameters()) + [tr.view_embeddings]
+
+    def labeled_step():
+        batch["keypoints"].copy_(kp_model)
+        return torch.autograd.grad(tr.evaluate_labeled(batch, "train", 1.0), params)
+
+    ms, _ = bench.time_stage(labeled_step, flush)
+    res[f"cfg4_calibrated_labeled_step_{tag}"] = {"frames": cb * cv, "ms": ms, "note": "eager; stand-in transformer; includes the RMSE diagnostic"}
+card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+res["cfg4_calibrated_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
+
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 json.dump(res, open(os.path.join(ROOT, "gpurun_out", "r02_configs.json"), "w"), indent=1)
 print(json.dumps(res, indent=1))
