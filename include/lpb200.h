@@ -245,6 +245,46 @@ int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes, int ctx, 
 int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* mean3,
                          const float* std3, int layout, int out_bf16, void* out, void* stream);
 
+/* ---- crop-zoom inference (bbox mode of the video-ingest boundary) ------------------------------------------------
+ * replaces crop_and_resize_frames  lightning_pose/data/bboxes.py:291-343  and the bbox-row slicing in front of it
+ *   lightning_pose/data/video/dali.py:332-380, lightning_pose/data/video/pynvvc.py:266-283
+ * Frame f uses box row r = min(row0 + f, n_boxes - 1) of boxes [n_boxes, 4] (x, y, h, w fp32), row0 = *cursor (device
+ * int64, read, never advanced: lpb_pack_predictions advances it) or row0 when cursor is NULL; rows past the end repeat
+ * the final row (the reference pads the last chunk with it).  Clamp as the reference does: x1 = max(0, (int)x),
+ * x2 = max(x1 + 1, min(W, (int)x + (int)w)), likewise y with h, H ((int) truncates toward zero).  Where the reference
+ * raises, this does not: an origin at or past the far edge is clamped to W - 1 / H - 1 (a one-pixel crop), and a row
+ * holding a NaN or an infinity is the whole frame.  The crop is resized to out_h x out_w (bilinear, half-pixel centres,
+ * no antialiasing).
+ *   in_f32 = 0: frames uint8 [F, H, W, 3] decoded RGB, normalised with mean3 / std3 (HOST arrays, as for
+ *               lpb_frames_normalize) on the way out;
+ *   in_f32 = 1: frames fp32 [F, 3, H, W] already normalised (the reference function's own input); crop + resize only,
+ *               mean3 / std3 ignored (may be NULL).
+ * out: layout 0 [F, 3, out_h, out_w] or layout 1 [F, out_h, out_w, 3], fp32 or bf16 (out_bf16).
+ * boxes_out [F, 4]: the clamped boxes [x1, y1, y2 - y1, x2 - x1], the bbox that maps model coordinates back to the
+ * frame (lpb_remap_keypoints).  F <= 65535. */
+int lpb_frames_crop_normalize(const void* frames, int in_f32, int F, int H, int W, const float* boxes, int64_t n_boxes,
+                              const int64_t* cursor, int64_t row0, int out_h, int out_w, const float* mean3,
+                              const float* std3, int layout, int out_bf16, void* out, float* boxes_out, void* stream);
+
+/* replaces _calculate_bbox_size + _compute_bbox_df  lightning_pose/utils/cropzoom.py:31-143
+ * keypoints: frame n, keypoint k at keypoints[n * row_stride + k * point_stride] (x) and + 1 (y): point_stride 2 reads
+ * (N, K, 2) keypoints, 3 reads a (N, 3K) prediction table (lpb_pack_predictions) in place.  anchors: HOST array of
+ * n_anchors keypoint indices, summed in the order given (the reference's column order); n_anchors = 0: all K.
+ * Exactly one mode: crop_ratio > 0 (size = ceil(crop_ratio * max(x span, y span)), bumped to even, for h and w) or
+ * crop_height, crop_width > 0 (each bumped to even).  out [N, 4] fp32 x, y, h, w holding integers: top-left =
+ * int64(centroid - size // 2) evaluated in fp64, with h subtracted from x and w from y as the reference does
+ * (cropzoom.py:135).  A frame with a NaN or infinite anchor gets a NaN row. */
+#define LPB_BBOX_MAX_ANCHORS 256
+int lpb_bboxes_from_keypoints(const float* keypoints, int64_t n, int K, int64_t row_stride, int point_stride,
+                              const int32_t* anchors, int n_anchors, double crop_ratio, int crop_height, int crop_width,
+                              float* out, void* stream);
+
+/* replaces the smoothing of smooth_bbox  lightning_pose/utils/cropzoom.py:355-402
+ *   rolling(window, center=True, min_periods=1).median().round(0) of each column of bboxes [n, 4] -> out [n, 4]
+ * (not aliasing bboxes): pandas' centred and end-truncated windows, NaN skipped, the mean of the two middle values for
+ * an even count, round half to even; a window with no value gives NaN. */
+int lpb_bboxes_rolling_median(const float* bboxes, int64_t n, int window, float* out, void* stream);
+
 /* ---- batched inference (SURVEY 8f-1) ------------------------------------------------------------------
  * replaces PredictionHandler.unpack_preds + make_pred_arr_undo_resize  lightning_pose/utils/predictions.py:97-144,180-206
  * keypoints [n_frames, 2K], confidences [n_frames, K] of one chunk -> rows [r, r + n_frames) of the prediction table

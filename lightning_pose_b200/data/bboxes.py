@@ -1,11 +1,14 @@
 """Model -> frame coordinate transform: the hot-path part of ``lightning_pose.data.bboxes``.
 
-``model_to_frame_batch`` (reference ``data/bboxes.py:222-288``), ``norm_to_frame`` (:74-105) and, for the calibrated
-multi-view losses, ``frame_to_model_batch`` (:194-219).
+``model_to_frame_batch`` (reference ``data/bboxes.py:222-288``), ``norm_to_frame`` (:74-105), for the calibrated
+multi-view losses ``frame_to_model_batch`` (:194-219), and for crop-zoom pose models ``crop_and_resize_frames`` (:291-343).
 Like the reference, ``in_place=True`` writes the result through the caller's tensor.
 """
 from __future__ import annotations
 
+from typing import Sequence
+
+import numpy as np
 import torch
 
 from lightning_pose_b200 import ops
@@ -19,6 +22,26 @@ def norm_to_frame(keypoints: torch.Tensor, bbox: torch.Tensor) -> torch.Tensor:
     flat = keypoints.reshape(n, 2 * k)
     ops.remap_keypoints(flat, None, bbox, 1.0, 1.0, out=flat if flat.is_contiguous() else None)
     return keypoints
+
+
+def crop_and_resize_frames(frames: torch.Tensor, bbox_rows, resize_dims: Sequence[int]) -> tuple[torch.Tensor, torch.Tensor]:
+    """Crop each frame to its box and resize the crops to ``resize_dims`` (reference ``data/bboxes.py:291-343``), in one
+    launch (``lpb_frames_crop_normalize``).
+
+    ``frames``: (seq, 3, H, W) fp32 on the device, already normalised; ``bbox_rows``: DataFrame with columns
+    ``x, y, h, w``, or a (rows, 4) tensor, with at least ``seq`` rows (row i crops frame i).  Returns (frames
+    (seq, 3, h, w), the boxes actually used (seq, 4) [x1, y1, y2 - y1, x2 - x1], clamped to the frame).  Boxes the
+    reference rejects (origin past the far edge, NaN) give a one-pixel crop and the whole frame (DESIGN.md §2).
+    """
+    if not isinstance(frames, torch.Tensor) or not frames.is_cuda:
+        raise RuntimeError("lpb200: `frames` must be a CUDA tensor (this package has no CPU fallback)")
+    if isinstance(bbox_rows, torch.Tensor):
+        rows = bbox_rows.to(device=frames.device, dtype=torch.float32)
+    else:
+        rows = torch.as_tensor(bbox_rows[["x", "y", "h", "w"]].to_numpy(dtype=np.float64, copy=True), dtype=torch.float32, device=frames.device)
+    if rows.dim() != 2 or rows.shape[0] < frames.shape[0]:
+        raise ValueError(f"need one bbox row per frame: {frames.shape[0]} frames, bbox rows {tuple(rows.shape)}")
+    return ops.frames_crop_normalize(frames.float(), rows, resize_dims)
 
 
 def model_to_frame_batch(batch_dict: dict, model_keypoints: torch.Tensor, in_place: bool = True) -> torch.Tensor:

@@ -19,13 +19,26 @@ __all__ = ["frames_to_unlabeled_batch", "context_windows_step"]
 
 
 def frames_to_unlabeled_batch(frames_u8: torch.Tensor | Sequence[torch.Tensor], resize_dims: Sequence[int] | None = None,
-                              dtype: torch.dtype = torch.float32, channels_last: bool = False) -> dict:
+                              dtype: torch.dtype = torch.float32, channels_last: bool = False, bbox: torch.Tensor | None = None,
+                              bbox_row0: int = 0) -> dict:
     """uint8 (seq, H, W, 3) frames of one view - or a list of them, one per view - to the batch dict of the trackers.
 
     Single view -> ``UnlabeledBatchDict``; several views -> ``MultiviewUnlabeledBatchDict`` with frames
     (seq, views, 3, H, W), transforms (views, 1), bbox (seq, 4 * views) (reference :289-327).
+
+    Crop-zoom pose models (reference ``LitDaliWrapper._apply_bbox_crop``, :332-380): ``bbox`` is the video's (N, 4)
+    [x, y, h, w] device table and frame i is cropped to row ``min(bbox_row0 + i, N - 1)``, resized to ``resize_dims``
+    (required) and normalised, in one launch; the returned ``bbox`` holds the clamped boxes the remap needs.  Single
+    view only, as in the reference.
     """
     views = [frames_u8] if isinstance(frames_u8, torch.Tensor) else list(frames_u8)
+    if bbox is not None:
+        if len(views) > 1:
+            raise ValueError("bbox_file is not supported for multiview prediction")
+        if resize_dims is None:
+            raise ValueError("resize_dims is required when frames are cropped to bounding boxes")
+        frames, boxes = ops.frames_crop_normalize(views[0], bbox, resize_dims, row0=bbox_row0, channels_last=channels_last, dtype=dtype)
+        return {"frames": frames, "transforms": torch.tensor([-1.0], device=frames.device), "bbox": boxes, "is_multiview": False}
     outs, boxes = [], []
     for v in views:
         outs.append(ops.frames_normalize(v, size=resize_dims, channels_last=channels_last, dtype=dtype))

@@ -534,6 +534,80 @@ def frames_normalize(frames_u8, size=None, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     return out
 
 
+def _bbox_table(bboxes, name: str) -> torch.Tensor:
+    b = _cuda_f32(bboxes, name)
+    if b.dim() != 2 or b.shape[1] != 4 or b.shape[0] < 1:
+        raise ValueError(f"`{name}` must be (N >= 1, 4) [x, y, h, w]; got {tuple(b.shape)}")
+    return b
+
+
+def frames_crop_normalize(frames, bboxes, size, cursor=None, row0: int = 0, mean=IMAGENET_MEAN, std=IMAGENET_STD,
+                          channels_last=False, dtype=torch.float32):
+    """Per-frame crop to a box, bilinear resize to ``size`` and (for uint8 input) ImageNet normalisation, one launch.
+
+    ``frames``: uint8 (F, H, W, 3) decoded RGB, or fp32 (F, 3, H, W) already normalised (crop + resize only).
+    ``bboxes``: (N, 4) [x, y, h, w] device table; frame f uses row min(r0 + f, N - 1) with r0 = ``cursor`` (int64 device
+    tensor, read only) or ``row0``.  Returns (frames (F, 3, h, w) [or (F, h, w, 3)], clamped boxes (F, 4) fp32)."""
+    if not isinstance(frames, torch.Tensor) or not frames.is_cuda:
+        raise RuntimeError("lpb200: `frames` must be a CUDA tensor (this package has no CPU fallback)")
+    if frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3:
+        in_f32 = 0
+        f, h, w, _ = frames.shape
+    elif frames.dtype == torch.float32 and frames.dim() == 4 and frames.shape[1] == 3:
+        in_f32 = 1
+        f, _, h, w = frames.shape
+    else:
+        raise ValueError(f"frames must be uint8 (F, H, W, 3) or float32 (F, 3, H, W); got {tuple(frames.shape)} {frames.dtype}")
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError("dtype must be float32 or bfloat16")
+    if int(row0) < 0:
+        raise ValueError(f"row0 must be >= 0; got {row0}")
+    b = _bbox_table(bboxes, "bboxes")
+    if cursor is not None and (not cursor.is_cuda or cursor.dtype != torch.int64 or cursor.numel() != 1):
+        raise ValueError("cursor must be a one-element int64 CUDA tensor")
+    x = frames.contiguous()
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((f, oh, ow, 3) if channels_last else (f, 3, oh, ow), device=x.device, dtype=dtype)
+    boxes_out = torch.empty((f, 4), device=x.device, dtype=torch.float32)
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(x.device):
+        check(lib.lpb_frames_crop_normalize(_ptr(x), in_f32, f, h, w, _ptr(b), b.shape[0], _ptr(cursor), int(row0), oh, ow, m3, s3,
+                                            int(bool(channels_last)), int(dtype == torch.bfloat16), _ptr(out), _ptr(boxes_out), _stream()))
+    return out, boxes_out
+
+
+def bboxes_from_keypoints(keypoints, anchor_indices=(), crop_ratio=None, crop_height=None, crop_width=None):
+    """(N, K, 2) keypoints or an (N, 3K) prediction table (read in place) -> (N, 4) [x, y, h, w] boxes, one launch.
+    ``anchor_indices`` are summed in the order given; empty = all keypoints.  Exactly one of ``crop_ratio`` or
+    (``crop_height``, ``crop_width``)."""
+    kp = _cuda_f32(keypoints, "keypoints")
+    if kp.dim() == 3 and kp.shape[2] == 2:
+        n, k, point_stride = kp.shape[0], kp.shape[1], 2
+    elif kp.dim() == 2 and kp.shape[1] % 3 == 0:
+        n, k, point_stride = kp.shape[0], kp.shape[1] // 3, 3
+    else:
+        raise ValueError(f"keypoints must be (N, K, 2) or an (N, 3K) prediction table; got {tuple(kp.shape)}")
+    anchors = [int(i) for i in anchor_indices]
+    arr = (C.c_int32 * max(len(anchors), 1))(*anchors)
+    out = torch.empty((n, 4), device=kp.device, dtype=torch.float32)
+    with torch.cuda.device(kp.device):
+        check(lib.lpb_bboxes_from_keypoints(_ptr(kp), n, k, k * point_stride, point_stride, arr, len(anchors),
+                                            float(crop_ratio or 0.0), int(crop_height or 0), int(crop_width or 0), _ptr(out), _stream()))
+    return out
+
+
+def bboxes_rolling_median(bboxes, window: int = 5):
+    """Centred rolling median of each column of (N, 4) boxes, rounded half to even (pandas' ``rolling(window,
+    center=True, min_periods=1).median().round(0)``), one launch."""
+    b = _cuda_f32(bboxes, "bboxes")
+    if b.dim() != 2 or b.shape[1] != 4:
+        raise ValueError(f"bboxes must be (N, 4); got {tuple(b.shape)}")
+    out = torch.empty_like(b)
+    with torch.cuda.device(b.device):
+        check(lib.lpb_bboxes_rolling_median(_ptr(b), b.shape[0], int(window), _ptr(out), _stream()))
+    return out
+
+
 def pack_predictions(keypoints, confidences, table, cursor=None, row0: int = 0):
     """Write one chunk's (keypoints (T, 2K), confidences (T, K)) into rows of ``table`` (N, 3K) at the device cursor
     (int64 tensor, advanced by T) or at ``row0``.  Mutates ``table`` (and ``cursor``)."""

@@ -110,6 +110,27 @@ class PredictionHandler:
         return pd.DataFrame(arr, columns=make_dlc_pandas_index(self.model_type, self.keypoint_names))
 
 
+def _graph_kernel_count(graph: torch.cuda.CUDAGraph) -> int:
+    """Kernel nodes of a captured graph (driver API: cuGraphGetNodes / cuGraphNodeGetType)."""
+    import ctypes as C
+
+    cu = C.CDLL("libcuda.so.1")
+    g = C.c_void_p(graph.raw_cuda_graph())
+    n = C.c_size_t(0)
+    if cu.cuGraphGetNodes(g, None, C.byref(n)) != 0:
+        raise RuntimeError("cuGraphGetNodes failed")
+    nodes = (C.c_void_p * n.value)()
+    if cu.cuGraphGetNodes(g, nodes, C.byref(n)) != 0:
+        raise RuntimeError("cuGraphGetNodes failed")
+    kind = C.c_int(0)
+    count = 0
+    for node in nodes:
+        if cu.cuGraphNodeGetType(C.c_void_p(node), C.byref(kind)) != 0:
+            raise RuntimeError("cuGraphNodeGetType failed")
+        count += kind.value == 0  # CU_GRAPH_NODE_TYPE_KERNEL
+    return count
+
+
 class BatchedPredictor:
     """CUDA-graph chunk loop writing straight into a preallocated (N, 3K) device table.
 
@@ -118,11 +139,20 @@ class BatchedPredictor:
     module otherwise (library convolutions; its kernels are captured into the same graph).  Chunks are fixed-size ``T``
     (``dali.base.predict.sequence_length`` = 96 in the reference config); the last chunk is padded by the caller and its
     surplus rows are dropped by the table writer.
+
+    Crop mode (crop-zoom pose models, reference ``predict_video(..., bbox_file=...)``, ``utils/predictions.py:455-470``
+    and ``data/video/dali.py:332-380``): ``bboxes`` is the video's (N, 4) [x, y, h, w] device table (``compute_bboxes``
+    / ``smooth_bboxes``) and ``frame_hw`` the full frame size.  ``feed`` then takes uint8 (T, H, W, 3) decoded frames;
+    inside the chunk (and its graph) one launch crops each frame to its box row at the table's device cursor (rows past
+    the end repeat the last), resizes the crop to ``image_hw`` and normalises it into ``crop_dtype`` (channels-last if
+    ``crop_channels_last``) for ``features_of``, and the clamped boxes it writes map the keypoints back to the frame.
+    ``launches_per_chunk``: kernel launches in one captured chunk (set at capture).
     """
 
     def __init__(self, head, num_keypoints: int, n_frames: int, chunk: int, image_hw: tuple[int, int],
                  features_of: Callable[[torch.Tensor], torch.Tensor] | None = None, device=None, use_graph: bool = True,
-                 sub_chunk: int | None = None) -> None:
+                 sub_chunk: int | None = None, bboxes: torch.Tensor | None = None, frame_hw: tuple[int, int] | None = None,
+                 crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False) -> None:
         self.head, self.k, self.n_frames, self.chunk = head, int(num_keypoints), int(n_frames), int(chunk)
         # frames per head / decode call inside a chunk: small enough that the heatmaps written by the head are still in
         # the 126 MB L2 when the decode reads them (None: the whole chunk at once)
@@ -137,9 +167,21 @@ class BatchedPredictor:
         self._static_in = None
         self._static_bbox = None
         self.launches_per_chunk = None
+        self.bboxes = None
+        if bboxes is not None:
+            if frame_hw is None or features_of is None:
+                raise ValueError("crop mode needs frame_hw (the full frame size) and features_of (frames -> features)")
+            self.bboxes = ops._bbox_table(bboxes, "bboxes")
+            if self.bboxes.shape[0] != self.n_frames:
+                raise ValueError(f"bboxes has {self.bboxes.shape[0]} rows but the video has {self.n_frames} frames")
+            self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
+            self.crop_dtype, self.crop_channels_last = crop_dtype, bool(crop_channels_last)
 
     # one chunk, eager: everything below is enqueued on the current stream; no host sync
-    def _chunk(self, x: torch.Tensor, bbox: torch.Tensor) -> None:
+    def _chunk(self, x: torch.Tensor, bbox: torch.Tensor | None) -> None:
+        if self.bboxes is not None:  # crop to the rows at the cursor BEFORE pack_predictions advances it
+            x, bbox = ops.frames_crop_normalize(x, self.bboxes, self.image_hw, cursor=self.cursor, channels_last=self.crop_channels_last,
+                                                dtype=self.crop_dtype)
         feats = self.features_of(x) if self.features_of is not None else x
         with torch.no_grad():
             for i in range(0, self.chunk, self.sub_chunk):
@@ -150,9 +192,10 @@ class BatchedPredictor:
 
     def _capture(self, x: torch.Tensor, bbox: torch.Tensor) -> None:
         self._static_in = torch.empty_like(x)
-        self._static_bbox = torch.empty_like(bbox)
         self._static_in.copy_(x)
-        self._static_bbox.copy_(bbox)
+        if bbox is not None:
+            self._static_bbox = torch.empty_like(bbox)
+            self._static_bbox.copy_(bbox)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
@@ -162,16 +205,24 @@ class BatchedPredictor:
         torch.cuda.synchronize(self.device)
         self.cursor.zero_()
         self.table.zero_()
-        self._graph = torch.cuda.CUDAGraph()
+        self._graph = torch.cuda.CUDAGraph(keep_graph=True)  # kept so that its kernel nodes can be counted
         with torch.cuda.graph(self._graph):
             self._chunk(self._static_in, self._static_bbox)
+        self.launches_per_chunk = _graph_kernel_count(self._graph)
+        self._graph.instantiate()
         self.cursor.zero_()  # the capture itself does not execute, but keep the invariant explicit
 
     def feed(self, x: torch.Tensor, bbox: torch.Tensor | None = None) -> None:
-        """Process the next chunk (``x``: (T, ...) frames or features on the device)."""
+        """Process the next chunk (``x``: (T, ...) frames or features on the device; in crop mode uint8 (T, H, W, 3)
+        frames, and ``bbox`` must be None: the boxes come from the predictor's table)."""
         if x.shape[0] != self.chunk:
             raise ValueError(f"chunks are fixed-size ({self.chunk} frames); pad the last one (got {x.shape[0]})")
-        if bbox is None:
+        if self.bboxes is not None:
+            if bbox is not None:
+                raise ValueError("crop mode takes its boxes from the `bboxes` table given at construction")
+            if x.dtype != torch.uint8 or tuple(x.shape[1:]) != (*self.frame_hw, 3):
+                raise ValueError(f"crop mode expects uint8 ({self.chunk}, {self.frame_hw[0]}, {self.frame_hw[1]}, 3) frames; got {tuple(x.shape)} {x.dtype}")
+        elif bbox is None:
             bbox = torch.tensor([[0.0, 0.0, float(self.image_hw[0]), float(self.image_hw[1])]], device=self.device).repeat(self.chunk, 1)
         if not self.use_graph:
             self._chunk(x, bbox)
@@ -179,7 +230,8 @@ class BatchedPredictor:
         if self._graph is None:
             self._capture(x, bbox)
         self._static_in.copy_(x, non_blocking=True)
-        self._static_bbox.copy_(bbox, non_blocking=True)
+        if bbox is not None:
+            self._static_bbox.copy_(bbox, non_blocking=True)
         self._graph.replay()
 
     def run(self, chunks: Iterable[torch.Tensor | tuple[torch.Tensor, torch.Tensor]]) -> torch.Tensor:

@@ -196,6 +196,73 @@ for tag, losses in (("3d_losses_off", {"heatmap_mse": {"log_weight": 0.0}}), ("3
 card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 res["cfg4_calibrated_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
 
+# config 5 with a crop-zoom pose model: 96-frame chunks of 1024x1024 uint8 frames, each cropped to a random in-frame box
+# (sides 256-896 px) and resized to the 384x384 model input.  Bytes model of the crop kernel: output bytes plus the input
+# bytes its bilinear taps touch, at most min(crop side, 2 x output side) rows and columns of the crop per frame.  The
+# reference's path is its own crop_and_resize_frames (the staged oracle/_ref copy) on full-resolution normalised fp32
+# frames (what its DALI pipeline hands over), with that normalisation (torch, eager) timed as well.
+import pandas as pd  # noqa: E402
+
+from oracle import ref_loader  # noqa: E402
+
+cf_, cs_, cside_ = 96, 1024, 384
+gen = torch.Generator(device=dev).manual_seed(51)
+u8_pool = [torch.randint(0, 256, (cf_, cs_, cs_, 3), dtype=torch.uint8, device=dev, generator=gen) for _ in range(2)]
+n_crop = cf_ * 20
+side = torch.randint(256, 897, (n_crop, 2), device=dev, generator=gen).float()
+origin = torch.rand(n_crop, 2, device=dev, generator=gen) * (cs_ - side)
+boxes_c = torch.stack([origin[:, 0].floor(), origin[:, 1].floor(), side[:, 0], side[:, 1]], 1).contiguous()  # x, y, h, w
+bx = boxes_c[:cf_]
+touched = (torch.clamp(bx[:, 2], max=2 * cside_) * torch.clamp(bx[:, 3], max=2 * cside_)).sum().item() * 3
+for tag, dt, cl in (("fchw_f32", torch.float32, False), ("fchw_bf16", torch.bfloat16, False), ("fhwc_bf16", torch.bfloat16, True)):
+    out_bytes = cf_ * 3 * cside_ * cside_ * (4 if dt == torch.float32 else 2)
+    ms, med = bench.time_stage(lambda: ops.frames_crop_normalize(u8_pool[0], bx, (cside_, cside_), channels_last=cl, dtype=dt), flush)
+    res[f"cfg5_crop_kernel_{tag}"] = {"frames": cf_, "ms": ms, "ms_median": med, "bytes_model": out_bytes + touched,
+                                     "gbs": (out_bytes + touched) / ms / 1e6, "frac_hbm": (out_bytes + touched) / ms / 1e6 / pk["hbm_gbs"]}
+ref_bboxes = ref_loader.load("lightning_pose.data.bboxes")
+rows_df = pd.DataFrame(bx.cpu().numpy().astype(np.float64), columns=["x", "y", "h", "w"])
+mean_t, std_t = torch.tensor(ops.IMAGENET_MEAN, device=dev)[:, None, None], torch.tensor(ops.IMAGENET_STD, device=dev)[:, None, None]
+full_f32 = (u8_pool[0].permute(0, 3, 1, 2).float() / 255.0 - mean_t) / std_t
+with torch.no_grad():
+    ms_n, _ = bench.time_stage(lambda: (u8_pool[0].permute(0, 3, 1, 2).float() / 255.0 - mean_t) / std_t, flush, reps=5, warmup=1)
+    ms_c, _ = bench.time_stage(lambda: ref_bboxes.crop_and_resize_frames(full_f32, rows_df, [cside_, cside_]), flush, reps=5, warmup=1)
+    ref_out, ref_boxes = ref_bboxes.crop_and_resize_frames(full_f32, rows_df, [cside_, cside_])
+    mine, mine_boxes = ops.frames_crop_normalize(u8_pool[0], bx, (cside_, cside_))
+del full_f32
+res["cfg5_crop_reference"] = {"frames": cf_, "normalise_ms": ms_n, "crop_and_resize_frames_ms": ms_c, "total_ms": ms_n + ms_c,
+                              "max_abs_diff_vs_kernel": float((ref_out - mine).abs().max()), "boxes_equal": bool(torch.equal(ref_boxes, mine_boxes)),
+                              "note": "reference crop_and_resize_frames (staged oracle/_ref) on fp32 full-resolution frames; normalisation in eager torch"}
+del ref_out
+head_c = head_for("resnet50", 2048)
+head_c.eval()
+sel, scl = torch.arange(2048, device=dev) % 3, torch.randn(2048, device=dev)[None, :, None, None]
+
+
+def backbone(fr):  # stand-in backbone (elementwise): (T, 3, 384, 384) -> (T, 2048, 12, 12) bf16
+    return (torch.nn.functional.avg_pool2d(fr.float(), 32)[:, sel] * scl).bfloat16()
+
+
+for mode in ("on", "off"):
+    kw = {"bboxes": boxes_c, "frame_hw": (cs_, cs_)} if mode == "on" else {}
+    fo = backbone if mode == "on" else (lambda u8: backbone(ops.frames_normalize(u8, size=(cside_, cside_))))
+    bp = BatchedPredictor(head_c, K, n_crop, cf_, (cside_, cside_), features_of=fo, **kw)
+    bp.feed(u8_pool[0])  # capture / warm
+    bp.cursor.zero_()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(n_crop // cf_):
+        bp.feed(u8_pool[i % 2])
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / (n_crop // cf_)
+    res[f"cfg5_crop_predictor_chunk_crop_{mode}"] = {
+        "frames_per_chunk": cf_, "ms_per_chunk": ms, "launches_per_chunk": bp.launches_per_chunk,
+        "note": "graph replay per chunk incl. the D2D copy of the uint8 chunk into the graph's input; crop off = the same uint8 chunk "
+                "resized whole (lpb_frames_normalize); stand-in elementwise backbone, random head weights"}
+card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+res["cfg5_crop_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
+
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 json.dump(res, open(os.path.join(ROOT, "gpurun_out", "r02_configs.json"), "w"), indent=1)
 print(json.dumps(res, indent=1))
