@@ -294,6 +294,30 @@ int lpb_bboxes_rolling_median(const float* bboxes, int64_t n, int window, float*
 int lpb_pack_predictions(const float* keypoints, const float* confidences, int n_frames, int K, float* table,
                          int64_t n_rows, int64_t* cursor, int64_t row0, void* stream);
 
+/* ---- batched inference with context (MHCRNN) models --------------------------------------------------------------
+ * replaces the selection and model -> frame step of HeatmapTrackerMHCRNN.predict_step
+ *   lightning_pose/models/heatmap_tracker_mhcrnn.py:180-229 (torch.gt(confidence_mf, confidence_sf) per keypoint, then
+ *   model_to_frame_batch with the window's bbox rows [2:-2]), and the host stacking / shift of
+ *   PredictionHandler.unpack_preds + fix_context_preds_confs  lightning_pose/utils/predictions.py:97-177 for a reader of
+ *   windows of S = step + 4 frames with step S - 4  lightning_pose/data/video/dali.py:519-534, 600-619.
+ * Output frame i of the call is video frame f = c - 2 + i, c = *cursor (device int64: frames fed before this call,
+ * advanced by n_frames afterwards) or frame0 when cursor is NULL.  Its single-frame / multi-frame keypoints
+ * kp_* [n_frames, 2K] (model pixels) and confidences conf_* [n_frames, K]: mf where conf_mf > conf_sf (a NaN keeps sf),
+ * then x * (1 / model_width) * w + bbox_x, y * (1 / model_height) * h + bbox_y with bbox [n_frames, 4] (x, y, h, w)
+ * the frame's own box (lpb_remap_keypoints' operation order).  The result goes to every row r of table [n_rows, 3K]
+ * whose source is f.  With N = n_rows, T = step and R = T * (ceil((N - S) / T) + 1) the rows the reader produces
+ * (R = N for T = 1, where num_iters reads one window per frame, dali.py:509-510):
+ *   R >= N: row r <- frame clamp(r, 2, N - 3);
+ *   R <  N: row r <- frame r for 2 <= r <= R - 1, every other row (0, 1 and the last N - R <= 4) <- frame 2 (the
+ *           reference pads with preds_combined[0], predictions.py:163-170).
+ * Once frames 0 .. N have been fed (ceil(N / T) chunks of T frames, the last one padded) the table is final.  Only when R = N - 1 does a
+ * kept row (N - 2) depend on frame N, the padding of the last chunk.  N >= 5 (with fewer frames the reference has no
+ * window).  No atomics: every row is written by the one thread of its source frame. */
+int lpb_pack_context_predictions(const float* kp_sf, const float* conf_sf, const float* kp_mf, const float* conf_mf,
+                                 int n_frames, int K, const float* bbox, float model_height, float model_width,
+                                 float* table, int64_t n_rows, int64_t* cursor, int64_t frame0, int64_t step,
+                                 void* stream);
+
 /* ---- optimizer step (the tail of a training step) ---------------------------------------------------
  * replaces torch.optim.Adam / AdamW as configured by configure_optimizers  lightning_pose/models/base.py:458-477
  * (no amsgrad).  One launch over up to 16 fp32 tensors; params / grads / exp_avg / exp_avg_sq / numel are HOST arrays

@@ -72,6 +72,7 @@ SIGNATURES = {
     "lpb_bboxes_from_keypoints": (C.c_int, [_P, _L, _I, _L, _I, C.POINTER(C.c_int32), _I, C.c_double, _I, _I, _P, _P]),
     "lpb_bboxes_rolling_median": (C.c_int, [_P, _L, _I, _P, _P]),
     "lpb_pack_predictions": (C.c_int, [_P, _P, _I, _I, _P, _L, _P, _L, _P]),
+    "lpb_pack_context_predictions": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _F, _F, _P, _L, _P, _L, _L, _P]),
     "lpb_adam_step": (C.c_int, [_I, _P, _P, _P, _P, _P, _P, _P, _F, _P, C.c_double, C.c_double, _F, _F, _I, _P]),
     "lpb_plane_softmax_bwd": (C.c_int, [_P, _P, _L, _I, _P, _P]),
     "lpb_heatmap_loss_fwd": (C.c_int, [_P, _P, _L, _I, _I, _I, _P, _P, _P]),

@@ -621,6 +621,33 @@ def pack_predictions(keypoints, confidences, table, cursor=None, row0: int = 0):
     return table
 
 
+def pack_context_predictions(kp_sf, conf_sf, kp_mf, conf_mf, bbox, model_height, model_width, table, step, cursor=None,
+                             frame0: int = 0):
+    """Context-model rows of one call's output frames (frame ``c - 2 + i`` for i < T, c = ``cursor`` or ``frame0``, the
+    frames fed before the call): per keypoint the more confident of the single-frame (``*_sf``) and multi-frame
+    (``*_mf``) predictions (a NaN keeps sf), mapped model -> frame with ``bbox`` (T, 4), written to every row of
+    ``table`` (N, 3K) the reference's row rule assigns to that frame for ``sequence_length = step + 4`` (see
+    ``lpb_pack_context_predictions``).  Mutates ``table`` and advances ``cursor`` by T."""
+    kps, cfs = _cuda_f32(kp_sf, "kp_sf"), _cuda_f32(conf_sf, "conf_sf")
+    kpm, cfm = _cuda_f32(kp_mf, "kp_mf"), _cuda_f32(conf_mf, "conf_mf")
+    bb = _cuda_f32(bbox, "bbox")
+    t, k = cfs.shape
+    if kps.shape != (t, 2 * k) or kpm.shape != (t, 2 * k) or cfm.shape != (t, k) or bb.shape != (t, 4):
+        raise ValueError(f"shapes: kp_sf {tuple(kps.shape)}, kp_mf {tuple(kpm.shape)} (T, 2K); conf_sf {tuple(cfs.shape)}, "
+                         f"conf_mf {tuple(cfm.shape)} (T, K); bbox {tuple(bb.shape)} (T, 4)")
+    if not isinstance(table, torch.Tensor) or not table.is_cuda:
+        raise RuntimeError("lpb200: `table` must be a CUDA tensor (this package has no CPU fallback)")
+    if table.dtype != torch.float32 or not table.is_contiguous() or table.dim() != 2 or table.shape[1] != 3 * k:
+        raise ValueError(f"table must be contiguous fp32 (N, {3 * k}); got {tuple(table.shape)} {table.dtype}")
+    if cursor is not None and (not cursor.is_cuda or cursor.dtype != torch.int64 or cursor.numel() != 1):
+        raise ValueError("cursor must be a one-element int64 CUDA tensor")
+    with torch.cuda.device(kps.device):
+        check(lib.lpb_pack_context_predictions(_ptr(kps), _ptr(cfs), _ptr(kpm), _ptr(cfm), t, k, _ptr(bb), float(model_height),
+                                               float(model_width), _ptr(table), table.shape[0], _ptr(cursor), int(frame0),
+                                               int(step), _stream()))
+    return table
+
+
 def plane_softmax_backward(probs: torch.Tensor, grad_probs: torch.Tensor) -> torch.Tensor:
     p = _cuda_f32(probs, "probs")
     g = _cuda_f32(grad_probs, "grad_probs")

@@ -82,13 +82,15 @@ class PredictionHandler:
         out[:, 2::3] = confidence_np
         return out
 
-    def dataframe(self, table: torch.Tensor | np.ndarray):
-        """(N, 3K) prediction table (device or host) -> DataFrame with the reference's columns."""
+    def dataframe(self, table: torch.Tensor | np.ndarray, frame_aligned: bool = False):
+        """(N, 3K) prediction table (device or host) -> DataFrame with the reference's columns.  ``frame_aligned``: the
+        table is already final (row f is frame f, as a context-mode ``BatchedPredictor`` writes it), so the context
+        shift-and-fill is skipped."""
         import pandas as pd
 
         arr = table.detach().cpu().numpy() if isinstance(table, torch.Tensor) else np.asarray(table)
         arr = arr[: self.frame_count]
-        if self.do_context:
+        if self.do_context and not frame_aligned:
             k = len(self.keypoint_names)
             t = torch.from_numpy(arr)
             kp = self.fix_context_preds_confs(t.reshape(-1, k, 3)[:, :, :2].reshape(-1, 2 * k).clone())
@@ -147,13 +149,36 @@ class BatchedPredictor:
     the end repeat the last), resizes the crop to ``image_hw`` and normalises it into ``crop_dtype`` (channels-last if
     ``crop_channels_last``) for ``features_of``, and the clamped boxes it writes map the keypoints back to the frame.
     ``launches_per_chunk``: kernel launches in one captured chunk (set at capture).
+
+    Context mode (``head`` a ``HeatmapMHCRNNHead``, reference ``HeatmapTrackerMHCRNN.predict_step`` over a reader of
+    windows of ``S = chunk + 4`` frames with step ``chunk``, ``dali.context.predict.sequence_length``): ``chunk`` is the
+    number of NEW frames per call, the caller feeds ``ceil(N / chunk)`` non-overlapping chunks (the last one padded) and
+    chunk j yields the predictions of frames ``j * chunk - 2 .. j * chunk + chunk - 3``.  The two / four frames before a
+    chunk stay on the device between calls (their single-frame decode, their boxes and their W_f / W_b maps), so every
+    frame passes through ``features_of``, ``head_sf`` and the maps once.  ``lpb_pack_context_predictions`` writes each
+    frame's selected, remapped prediction to every row the reference's ``fix_context_preds_confs`` gives it, so after
+    the last chunk ``table`` is the reference's final table for ``sequence_length = chunk + 4`` with no host fix-up (use
+    ``PredictionHandler.dataframe(table, frame_aligned=True)``).  With R = chunk * (ceil((N - S) / chunk) + 1):
+    R >= N: row f is frame clamp(f, 2, N - 3); R < N: row f is frame f for 2 <= f <= R - 1 and frame 2 otherwise (the
+    reference pads the tail with its first row).  Only when R = N - 1 does a row (N - 2) depend on frame N, the first
+    padding frame of the last chunk; the reference reads the zero-filled frame its reader pads with there, so the
+    caller's padding matters in that case only.  N < 5 raises (the reference has no window to predict from).
     """
 
     def __init__(self, head, num_keypoints: int, n_frames: int, chunk: int, image_hw: tuple[int, int],
                  features_of: Callable[[torch.Tensor], torch.Tensor] | None = None, device=None, use_graph: bool = True,
                  sub_chunk: int | None = None, bboxes: torch.Tensor | None = None, frame_hw: tuple[int, int] | None = None,
-                 crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False) -> None:
+                 crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False, num_views: int = 1) -> None:
+        from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
+
         self.head, self.k, self.n_frames, self.chunk = head, int(num_keypoints), int(n_frames), int(chunk)
+        self.context = isinstance(head, HeatmapMHCRNNHead)
+        if self.context and int(num_views) > 1:
+            raise ValueError("context prediction is not supported for multiview models")
+        if self.context and self.n_frames < 5:
+            raise ValueError(f"a context model needs at least 5 frames to predict from; the video has {self.n_frames}")
+        if self.chunk < 1:
+            raise ValueError(f"chunk must be >= 1; got {self.chunk}")
         # frames per head / decode call inside a chunk: small enough that the heatmaps written by the head are still in
         # the 126 MB L2 when the decode reads them (None: the whole chunk at once)
         self.sub_chunk = int(sub_chunk) if sub_chunk else self.chunk
@@ -169,6 +194,8 @@ class BatchedPredictor:
         self.launches_per_chunk = None
         self.bboxes = None
         if bboxes is not None:
+            if int(num_views) > 1:
+                raise ValueError("bbox cropping is not supported for multiview models")
             if frame_hw is None or features_of is None:
                 raise ValueError("crop mode needs frame_hw (the full frame size) and features_of (frames -> features)")
             self.bboxes = ops._bbox_table(bboxes, "bboxes")
@@ -176,12 +203,60 @@ class BatchedPredictor:
                 raise ValueError(f"bboxes has {self.bboxes.shape[0]} rows but the video has {self.n_frames} frames")
             self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
             self.crop_dtype, self.crop_channels_last = crop_dtype, bool(crop_channels_last)
+        if self.context:
+            # halo + chunk buffers: index b of the maps holds frame cursor - 4 + b, of the others frame cursor - 2 + b; the
+            # maps' buffers are sized by the first chunk's maps
+            t, k, dev = self.chunk, self.k, self.device
+            self._wf = self._wb = None
+            self._kp_sf = torch.zeros((t + 2, 2 * k), dtype=torch.float32, device=dev)
+            self._cf_sf = torch.zeros((t + 2, k), dtype=torch.float32, device=dev)
+            self._box = torch.zeros((t + 2, 4), dtype=torch.float32, device=dev)
+            self._idx = (torch.arange(t, device=dev)[:, None] + torch.arange(5, device=dev)[None, :]).to(torch.int32)
+
+    def _reset(self) -> None:
+        self.cursor.zero_()
+        self.table.zero_()
+        if self.context:
+            for buf in (self._wf, self._wb, self._kp_sf, self._cf_sf, self._box):
+                if buf is not None:
+                    buf.zero_()
+
+    def _context_chunk(self, x: torch.Tensor, bbox: torch.Tensor) -> None:
+        """One context chunk, eager: T new frames -> the predictions of frames cursor - 2 .. cursor + T - 3."""
+        head, mf = self.head, self.head.head_mf
+        hf = (mf.H_f[0].weight, mf.H_f[0].bias, mf.H_f[1].weight, mf.H_f[1].bias)
+        hb = (mf.H_b[0].weight, mf.H_b[0].bias, mf.H_b[1].weight, mf.H_b[1].bias)
+        t = self.chunk
+        with torch.no_grad():
+            feats = self.features_of(x) if self.features_of is not None else x
+            self._box[2:].copy_(bbox)
+            for i in range(0, t, self.sub_chunk):
+                n = min(self.sub_chunk, t - i)
+                f = feats[i : i + n]
+                kp, cf = head.run_subpixelmaxima(head.head_sf(f))  # single-frame head, once per frame
+                self._kp_sf[2 + i : 2 + i + n].copy_(kp)
+                self._cf_sf[2 + i : 2 + i + n].copy_(cf)
+                wf, wb = mf._maps(f)  # W_f / W_b, once per frame
+                if self._wf is None:
+                    self._wf = torch.zeros((t + 4, *wf.shape[1:]), dtype=torch.float32, device=self.device)
+                    self._wb = torch.zeros_like(self._wf)
+                self._wf[4 + i : 4 + i + n].copy_(wf)
+                self._wb[4 + i : 4 + i + n].copy_(wb)
+                kp_mf, cf_mf = head.run_subpixelmaxima(ops.plane_softmax(ops.crnn_combine(self._wf, self._wb, self._idx[i : i + n], hf, hb)))
+                ops.pack_context_predictions(self._kp_sf[i : i + n], self._cf_sf[i : i + n], kp_mf, cf_mf, self._box[i : i + n],
+                                             self.image_hw[0], self.image_hw[1], self.table, t, cursor=self.cursor)
+            for buf, halo in ((self._wf, 4), (self._wb, 4), (self._kp_sf, 2), (self._cf_sf, 2), (self._box, 2)):
+                tail = buf[t : t + halo]
+                buf[:halo].copy_(tail.clone() if t < halo else tail)  # the last frames become the next chunk's halo
 
     # one chunk, eager: everything below is enqueued on the current stream; no host sync
     def _chunk(self, x: torch.Tensor, bbox: torch.Tensor | None) -> None:
-        if self.bboxes is not None:  # crop to the rows at the cursor BEFORE pack_predictions advances it
+        if self.bboxes is not None:  # crop to the rows at the cursor BEFORE the table writer advances it
             x, bbox = ops.frames_crop_normalize(x, self.bboxes, self.image_hw, cursor=self.cursor, channels_last=self.crop_channels_last,
                                                 dtype=self.crop_dtype)
+        if self.context:
+            self._context_chunk(x, bbox)
+            return
         feats = self.features_of(x) if self.features_of is not None else x
         with torch.no_grad():
             for i in range(0, self.chunk, self.sub_chunk):
@@ -203,8 +278,7 @@ class BatchedPredictor:
                 self._chunk(self._static_in, self._static_bbox)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
-        self.cursor.zero_()
-        self.table.zero_()
+        self._reset()
         self._graph = torch.cuda.CUDAGraph(keep_graph=True)  # kept so that its kernel nodes can be counted
         with torch.cuda.graph(self._graph):
             self._chunk(self._static_in, self._static_bbox)

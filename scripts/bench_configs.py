@@ -50,6 +50,76 @@ def fwd_bwd(name, arch, shape, hm):
                                      "frac_hbm": b * (2 * hb + 2 * fb) / ms / 1e6 / pk["hbm_gbs"]}
 
 
+def cfg3_context():
+    """Video prediction with the config-3 context model: 92 new frames per chunk (sequence_length 96) of (., 384, 16, 16)
+    bf16 features -> 64 x 64 heatmaps, K = 17, 40 chunks.  Three paths: the context predictor (graph replay / eager), the
+    reference's form (predict_step per overlapping window of 96 frames, i.e. forward_sequence + two decodes + selection +
+    remap, then host stacking and fix_context_preds_confs), and the same predictor in single-frame mode (sf head only)."""
+    import subprocess
+
+    from lightning_pose_b200 import ops
+    from lightning_pose_b200.utils.predictions import PredictionHandler
+
+    t, s, nch, k = 92, 96, 40, K
+    n = t * nch
+    torch.manual_seed(3)
+    mh = HeatmapMHCRNNHead("vits_dino", 384, k, upsampling_factor=1).to(dev).eval()
+    pool = [(torch.randn(t, 384, 16, 16, device=dev) * 0.5).bfloat16() for _ in range(2)]
+    box = torch.tensor([[0.0, 0.0, 256.0, 256.0]], device=dev).repeat(t, 1)
+
+    def timed(fn, reps):
+        fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for i in range(reps):
+            fn(i)
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    for mode in ("graph", "eager"):
+        bp = BatchedPredictor(mh, k, n, t, (256, 256), use_graph=mode == "graph")
+        ms = timed(lambda i=0: bp.feed(pool[i % 2], box), nch - 1)
+        res[f"cfg3_context_predictor_{mode}"] = {"new_frames_per_chunk": t, "ms_per_chunk": ms, "frames_per_s": 1e3 * t / ms,
+                                                 "launches_per_chunk": bp.launches_per_chunk}
+    sf_only = BatchedPredictor(mh.head_sf, k, n, t, (256, 256))
+    ms = timed(lambda i=0: sf_only.feed(pool[i % 2], box), nch - 1)
+    res["cfg3_context_single_frame_predictor_graph"] = {"frames_per_chunk": t, "ms_per_chunk": ms, "frames_per_s": 1e3 * t / ms,
+                                                        "launches_per_chunk": sf_only.launches_per_chunk}
+    # reference form: windows of 96 frames (4 of them re-run from the previous window), host stack + fix-up at the end
+    win = torch.cat([pool[0], pool[1][:4]])
+    wbox = box[:1].repeat(s, 1)
+    ph = PredictionHandler([f"bp{i}" for i in range(k)], n, model_type="heatmap_mhcrnn")
+
+    def reference_form(i=0):
+        preds = []
+        for _ in range(4):
+            with torch.no_grad():
+                sf, mf = mh.forward_sequence(win)
+                kp_sf, cf_sf = mh.run_subpixelmaxima(sf)
+                kp_mf, cf_mf = mh.run_subpixelmaxima(mf)
+            pick = torch.gt(cf_mf, cf_sf)
+            kp = torch.where(pick[..., None], kp_mf.reshape(-1, k, 2), kp_sf.reshape(-1, k, 2)).reshape(-1, 2 * k)
+            preds.append((ops.remap_keypoints(kp, None, wbox, 256, 256), torch.where(pick, cf_mf, cf_sf)))
+        kp_all = torch.vstack([p[0] for p in preds]).cpu()
+        ph.fix_context_preds_confs(kp_all)
+
+    ms = timed(reference_form, 5) / 4
+    res["cfg3_context_reference_form"] = {"new_frames_per_window": t, "ms_per_window": ms, "frames_per_s": 1e3 * t / ms,
+                                          "note": "eager; forward_sequence on 96 frames per window + host stack/fix-up, amortised over 4 windows"}
+    card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res["cfg3_context_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
+
+
+if sys.argv[1:2] == ["cfg3_context"]:  # only the context-prediction entries; an optional second argument names a JSON file
+    cfg3_context()
+    if len(sys.argv) > 2:
+        os.makedirs(os.path.dirname(os.path.abspath(sys.argv[2])), exist_ok=True)
+        json.dump(res, open(sys.argv[2], "w"), indent=1)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
 # config 3: ViT-S 256x256 (one deconv, 64x64 heatmaps); labeled context batch 16 x 5 frames + clip of 16
 fwd_bwd("cfg3_vits_256", "vits_dino", (96, 384, 16, 16), 64)
 # config 4: 4 views x 384x384 through the same head: (8 x 4, 384, 24, 24) -> 96x96
@@ -262,6 +332,7 @@ for mode in ("on", "off"):
                 "resized whole (lpb_frames_normalize); stand-in elementwise backbone, random head weights"}
 card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 res["cfg5_crop_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
+cfg3_context()
 
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 json.dump(res, open(os.path.join(ROOT, "gpurun_out", "r02_configs.json"), "w"), indent=1)
