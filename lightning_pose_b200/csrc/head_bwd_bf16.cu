@@ -855,9 +855,10 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
 }
 
 
-// bias gradient of a one-deconv head: column sums of the gradient rows, folded over the four classes
-__global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* __restrict__ G, RowLayout L, int B, int cout,
-                                                          float* __restrict__ db) {
+// bias gradient of a one-deconv head: column sums of the gradient rows, folded over the four classes.  Stage 1 writes
+// the eight column sums of every (frame, K-chunk); stage 2 adds them per output channel in a fixed order, so the bias
+// gradient is bit-reproducible like every other gradient of this file (no atomics).
+__global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* __restrict__ G, RowLayout L, float* __restrict__ part) {
   // one CTA per (frame, K-chunk): thread = (row stripe, e)
   const int b = blockIdx.x / GB_KC, kc = blockIdx.x - b * GB_KC;
   const __nv_bfloat16* slab = G + ((size_t)b * GB_KC + kc) * (size_t)L.rows * 8;
@@ -870,9 +871,24 @@ __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* _
   if (threadIdx.x < 8) {
     float t = 0.f;
     for (int i = threadIdx.x; i < 256; i += 8) t += red[i];
-    const int k = kc * 8 + threadIdx.x, o = k % GB_CLS;
-    if (o < cout && t != 0.f) atomicAdd(db + o, t);
+    part[(size_t)blockIdx.x * 8 + threadIdx.x] = t;
   }
+}
+
+// one CTA per output channel o: the partials of K entries k = kc * 8 + e with k % GB_CLS == o, in a fixed order
+__global__ void __launch_bounds__(256) rows_colsum_reduce_kernel(const float* __restrict__ part, long long n, float* __restrict__ db) {
+  const int o = blockIdx.x;
+  float acc = 0.f;
+  for (long long j = threadIdx.x; j < n; j += 256)
+    if ((int)(j % (GB_KC * 8)) % GB_CLS == o) acc += part[j];
+  __shared__ float red[256];
+  red[threadIdx.x] = acc;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (threadIdx.x < h) red[threadIdx.x] += red[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) db[o] = red[0];
 }
 
 // largest rows-per-band Hh (multiple of 4) whose band fits the b3a shared-memory stages
@@ -928,7 +944,9 @@ extern "C" int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int
   const size_t w1 = (size_t)((C4 + 127) / 128) * 4 * GB_KC * 128 * 16, w2 = (size_t)4 * GB_KC * 32 * 16;
   const size_t g2 = c2 > 0 ? (size_t)B * GB_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0;
   const size_t g1 = (size_t)B * GB_KC * make_row_layout(2 * H, 2 * W).rows * 16;
-  *bytes = w1 + w2 + g2 + g1 + (((size_t)B * (c2 > 0 ? c2 : c1) * 4 + 255) & ~(size_t)255) + bwd_partials_bytes(C, c1, c2);
+  // (+ a one-deconv head's bias-gradient partials: eight per (frame, K-chunk))
+  *bytes = w1 + w2 + g2 + g1 + (((size_t)B * (c2 > 0 ? c2 : c1) * 4 + 255) & ~(size_t)255) + bwd_partials_bytes(C, c1, c2) +
+           (c2 > 0 ? 0 : (size_t)B * GB_KC * 8 * sizeof(float));
   return LPB_OK;
 }
 
@@ -981,6 +999,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   float* part1 = reinterpret_cast<float*>(ws + w1b + w2b + g2b + g1b + ((((size_t)B * kout * 4) + 255) & ~(size_t)255));
   float* part2 = part1 + (size_t)wgrad_max_slots(C4 / 8) * wgrad_part_stride(C4, c1);
   float* part_db1 = two ? part2 + (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) : nullptr;
+  float* part_cs = two ? nullptr : part2;  // one-deconv head: the bias partials follow the layer-1 partials
   // the forward pass's mid activations (head_bf16.cu workspace layout: [packed w1][packed w2][mid])
   const size_t fwd_mid_off = (size_t)(C4 / 32 + 1) * (4 * 4 * 80 * 16);
   const __nv_bfloat16* mid = reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + fwd_mid_off);
@@ -1051,7 +1070,8 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     b2d_dgrad_kernel<<<grid, B2D_THREADS, smem, s>>>(p);
     reduce_partials(part_db1, grid * 4, GB_CLS, 1, c1, db1, s);
   } else {
-    rows_colsum_kernel<<<(unsigned)(B * GB_KC), 256, 0, s>>>(G1, L1, B, c1, db1);
+    rows_colsum_kernel<<<(unsigned)(B * GB_KC), 256, 0, s>>>(G1, L1, part_cs);
+    rows_colsum_reduce_kernel<<<(unsigned)c1, 256, 0, s>>>(part_cs, (long long)B * GB_KC * 8, db1);
   }
   // layer 1: weight gradient from the saved shuffled features, data gradient -> d features
   {
