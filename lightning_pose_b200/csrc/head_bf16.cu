@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
       const int cls = nrow / HB_CLS, o = nrow % HB_CLS;
       const int py = cls >> 1, px = cls & 1, dm = sh >> 1, dn = sh & 1;
       float v = 0.f;
-      if (c < Cin && o < Cout && !(py == 0 && dm == 1) && !(px == 0 && dn == 1)) {
+      if (c < Cin && o < Cout && tap_nonzero(cls, sh)) {
         const int ky = py == 0 ? 1 : (dm ? 0 : 2);
         const int kx = px == 0 ? 1 : (dn ? 0 : 2);
         v = w[((size_t)c * Cout + o) * 9 + ky * 3 + kx];
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
       const int cls = k / PREP_GB_CLS, o = k % PREP_GB_CLS;
       const int py = cls >> 1, px = cls & 1, dm = sh >> 1, dn = sh & 1;
       float v = 0.f;
-      if (c < Cin && o < Cout && !(py == 0 && dm == 1) && !(px == 0 && dn == 1)) {
+      if (c < Cin && o < Cout && tap_nonzero(cls, sh)) {
         const int ky = py == 0 ? 1 : (dm ? 0 : 2);
         const int kx = px == 0 ? 1 : (dn ? 0 : 2);
         v = w[((size_t)c * Cout + o) * 9 + ky * 3 + kx];
@@ -493,13 +493,13 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
         if (active) {
           const uint32_t a0 = smem_u32(stage_base + s * stage_bytes);
           const uint32_t b0 = a0 + a_stage_bytes;
-#pragma unroll
-          for (int sh = 0; sh < 4; ++sh) {
+          mma::for_shifts([&](auto shc) {  // only the n8 tiles with real taps of the shift (24 of 40)
+            constexpr int sh = decltype(shc)::value;
             const int shift_rows = (sh >> 1) * g.P + (sh & 1);
 #pragma unroll
             for (int k16 = 0; k16 < 2; ++k16)
-              mma::kstep(acc, a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
-          }
+              mma::kstep_nz<NZ_N8[sh]>(acc, a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
+          });
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);

@@ -674,11 +674,47 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
 //   dW[c, o, ky, kx] = sum_{frames, rows} X[row + shift][c] * G[row][(cls, o)]      ((cls, shift) -> tap)
 // a GEMM whose K dimension is the pixel raster.  Both operands are the row layout read TRANSPOSED (ldmatrix .trans,
 // mma_sm90.cuh kstep_mn / umma_selftest.cu mode 1): A = G (M = the 80 (cls, o) rows), B = X at a row offset (the
-// shift), N = this CTA's channel group.  MMA warp w owns shift w % 4 and half w / 4 of the channel group; its
-// accumulators D_sh[k][c] stay in registers across every (frame, row-chunk) unit of the CTA, and one epilogue at the
-// end adds them into dW with atomics.  An all-ones input channel (the bias lane of the mid activations) yields the bias
-// gradient from the same GEMM.
+// shift), N = this CTA's channel group.  Of the 4 shifts x 5 m16 tiles of A, 14 hold a real tap (NZ_M16, head_prep.cuh);
+// MMA warp w takes half w / 4 of the channel group and the (shift, m16 tile) units of role w % 4 (wg_unit) of it -- at most 4 each,
+// where one warp per shift would carry 5.  Its accumulators stay in registers across every (frame, row-chunk) unit of
+// the CTA, and one epilogue at the end writes them to the CTA's slot of the partials.  An all-ones input channel (the
+// bias lane of the mid activations) yields the bias gradient from the same GEMM.
 constexpr int WG_THREADS = 288;  // warp 0 loader, warps 1-8 MMA + epilogue
+constexpr int WG_UNITS = 4;
+struct WgUnit { int sh, mt; };  // sh = -1: unused
+// role r: shift r's non-zero tiles, except (shift 0, tile 3), which the shift-3 role takes: it shares that tile's A
+// fragment with its own (shift 3, tile 3)
+__host__ __device__ constexpr WgUnit wg_unit(int r, int v) {
+  constexpr WgUnit role[4][WG_UNITS] = {
+      {{0, 0}, {0, 1}, {0, 2}, {0, 4}},
+      {{1, 1}, {1, 2}, {1, 3}, {1, 4}},
+      {{2, 2}, {2, 3}, {2, 4}, {-1, 0}},
+      {{3, 3}, {0, 3}, {3, 4}, {-1, 0}},
+  };
+  return role[r][v];
+}
+// m16 tiles (sh_bits = false) or shifts (true) a role reads
+__host__ __device__ constexpr unsigned wg_role_set(int r, bool sh_bits) {
+  unsigned m = 0;
+  for (int v = 0; v < WG_UNITS; ++v)
+    if (wg_unit(r, v).sh >= 0) m |= 1u << (sh_bits ? wg_unit(r, v).sh : wg_unit(r, v).mt);
+  return m;
+}
+// the roles cover exactly the non-zero units, each once
+constexpr bool wg_roles_exact() {
+  unsigned seen[4] = {0, 0, 0, 0};
+  for (int r = 0; r < 4; ++r)
+    for (int v = 0; v < WG_UNITS; ++v) {
+      const WgUnit u = wg_unit(r, v);
+      if (u.sh < 0) continue;
+      if (seen[u.sh] & (1u << u.mt)) return false;
+      seen[u.sh] |= 1u << u.mt;
+    }
+  for (int sh = 0; sh < 4; ++sh)
+    if (seen[sh] != NZ_M16[sh]) return false;
+  return true;
+}
+static_assert(wg_roles_exact(), "weight-gradient warp roles must cover each non-zero (shift, m16 tile) unit exactly once");
 
 struct WgParams {
   const __nv_bfloat16* X;     // [B][kcx_total][L.rows][8] padded row layout
@@ -768,40 +804,79 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
                  P.X + (((size_t)b * P.kcx_total + (size_t)grp * P.kcx + lane) * P.L.rows + row0) * 8, xbytes, &full[s]);
     }
   } else if (slot < nunits) {
-    const int cw = warp - 1, sh = cw & 3, half = cw >> 2;
-    const int dm = sh >> 1, dn = sh & 1, shift_rows = dm * Pp + dn;
+    const int cw = warp - 1, half = cw >> 2;
     const uint32_t g0 = smem_u32(Gs), x0 = smem_u32(Xs) + (uint32_t)(half * NT) * XR * 16;  // n8 tile = one K-chunk of X
-    float acc[GB_K / 16][NT][4];
-    mma::zero(acc);
-    int j = 0;
-    for (int u = slot; u < nunits; u += nslot, ++j) {
-      const int s = j & 1;
-      mbar_wait(&full[s], (j >> 1) & 1);
-      for (int k16 = 0; k16 < KR / 16; ++k16)
-        mma::kstep_mn(acc, g0 + s * g_bytes + k16 * 256, KR * 16, x0 + s * x_bytes + (k16 * 16 + shift_rows) * 16, XR * 16, lane);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);
-    }
-    // accumulator (k = 16 mt + g (+8), c = 8 nt + 2 t (+1)) of shift sh -> this slot's partial of dW[c][o][ky][kx]
     float* part = P.part + (size_t)slot * wgrad_part_stride(P.Cin, P.Cout);
-    const int gq = lane >> 2, tq = lane & 3;
+    // warp role r = cw % 4 owns the (shift, m16 tile) units wg_unit(r, .) of channel half `half`
+    auto run = [&](auto rc) {
+      constexpr int ROLE = decltype(rc)::value;
+      constexpr unsigned mt_set = wg_role_set(ROLE, false), sh_set = wg_role_set(ROLE, true);
+      float acc[WG_UNITS][NT][4];
+      mma::zero(acc);
+      int j = 0;
+      for (int u = slot; u < nunits; u += nslot, ++j) {
+        const int s = j & 1;
+        mbar_wait(&full[s], (j >> 1) & 1);
+        const uint32_t a = g0 + s * g_bytes, b = x0 + s * x_bytes;
+        for (int k16 = 0; k16 < KR / 16; ++k16) {
+          // A (G) fragments of the role's m16 tiles, B (X) fragments of its shifts; each loaded once per K step
+          uint32_t af[GB_K / 16][4], bf[4][NT / 2][4];
 #pragma unroll
-    for (int mt = 0; mt < GB_K / 16; ++mt)
+          for (int mt = 0; mt < GB_K / 16; ++mt)
+            if ((mt_set >> mt) & 1u)
+              mma::ldsm_x4_t(af[mt], a + k16 * 256 + (uint32_t)(2 * mt + ((lane >> 3) & 1)) * KR * 16 + (uint32_t)((lane >> 4) * 8 + (lane & 7)) * 16);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int k = 16 * mt + gq + 8 * (i >> 1);
-        const int cls = k / GB_CLS, o = k - cls * GB_CLS, py = cls >> 1, px = cls & 1;
-        if (o >= P.Cout || (py == 0 && dm == 1) || (px == 0 && dn == 1)) continue;
-        const int ky = py == 0 ? 1 : (dm ? 0 : 2), kx = px == 0 ? 1 : (dn ? 0 : 2);
+          for (int sh = 0; sh < 4; ++sh)
+            if ((sh_set >> sh) & 1u)
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-          const int c = grp * N + (half * NT + nt) * 8 + 2 * tq + (i & 1);
-          const float v = acc[mt][nt][i];
-          // (cls, shift) -> tap is one-to-one, so every element of the slot's partial has exactly one writer
-          if (c < P.Cin) part[((size_t)c * P.Cout + o) * 9 + ky * 3 + kx] = v;
-          else if (P.has_bias && c == P.ones_c && sh == 0) part[(size_t)P.Cin * P.Cout * 9 + cls * P.Cout + o] = v;
+              for (int np = 0; np < NT / 2; ++np)
+                mma::ldsm_x4_t(bf[sh][np], b + (k16 * 16 + (sh >> 1) * Pp + (sh & 1)) * 16 + (uint32_t)(2 * np + (lane >> 4)) * XR * 16 +
+                                               (uint32_t)(((lane >> 3) & 1) * 8 + (lane & 7)) * 16);
+#pragma unroll
+          for (int v = 0; v < WG_UNITS; ++v) {
+            const int ush = wg_unit(ROLE, v).sh, umt = wg_unit(ROLE, v).mt;
+            if (ush < 0) continue;
+#pragma unroll
+            for (int np = 0; np < NT / 2; ++np) {
+              mma::mma_bf16(acc[v][2 * np], af[umt], bf[ush][np][0], bf[ush][np][1]);
+              mma::mma_bf16(acc[v][2 * np + 1], af[umt], bf[ush][np][2], bf[ush][np][3]);
+            }
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+      }
+      // accumulator (k = 16 mt + g (+8), c = 8 nt + 2 t (+1)) of unit (shift, mt) -> this slot's partial of dW[c][o][ky][kx]
+      const int gq = lane >> 2, tq = lane & 3;
+#pragma unroll
+      for (int v = 0; v < WG_UNITS; ++v) {
+        const int sh = wg_unit(ROLE, v).sh, mt = wg_unit(ROLE, v).mt;
+        if (sh < 0) continue;
+        const int dm = sh >> 1, dn = sh & 1;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int k = 16 * mt + gq + 8 * (i >> 1);
+          const int cls = k / GB_CLS, o = k - cls * GB_CLS, py = cls >> 1, px = cls & 1;
+          if (o >= P.Cout || !tap_nonzero(cls, sh)) continue;
+          const int ky = py == 0 ? 1 : (dm ? 0 : 2), kx = px == 0 ? 1 : (dn ? 0 : 2);
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) {
+            const int c = grp * N + (half * NT + nt) * 8 + 2 * tq + (i & 1);
+            const float val = acc[v][nt][i];
+            // (cls, shift) -> tap is one-to-one and every unit has one owner, so every element of the slot's partial has
+            // exactly one writer
+            if (c < P.Cin) part[((size_t)c * P.Cout + o) * 9 + ky * 3 + kx] = val;
+            else if (P.has_bias && c == P.ones_c && sh == 0) part[(size_t)P.Cin * P.Cout * 9 + cls * P.Cout + o] = val;
+          }
         }
       }
+    };
+    switch (cw & 3) {
+      case 0: run(std::integral_constant<int, 0>{}); break;
+      case 1: run(std::integral_constant<int, 1>{}); break;
+      case 2: run(std::integral_constant<int, 2>{}); break;
+      default: run(std::integral_constant<int, 3>{}); break;
+    }
   }
 }
 

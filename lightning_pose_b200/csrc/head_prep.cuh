@@ -9,6 +9,26 @@
 
 namespace lpb {
 
+// A stride-2 3x3 transposed convolution in the 4-shift form (head_bf16.cu): output class cls = 2 py + px reads input
+// shift sh = 2 dm + dn through a real tap unless (py == 0 && dm == 1) or (px == 0 && dn == 1) -- 9 of the 16 pairs.  The
+// packers write exact zeros for the other 7, and the GEMMs skip the tiles that hold nothing else.
+__host__ __device__ constexpr bool tap_nonzero(int cls, int sh) {
+  return !((cls >> 1) == 0 && (sh >> 1) == 1) && !((cls & 1) == 0 && (sh & 1) == 1);
+}
+// bit i: the `width` class-major columns [width i, width i + width) of the 80 (cls * 20 + o) hold a non-zero weight for shift sh
+constexpr unsigned nz_tiles(int sh, int width) {
+  unsigned m = 0;
+  for (int i = 0; i < 80 / width; ++i)
+    for (int k = width * i; k < width * (i + 1); ++k)
+      if (tap_nonzero(k / 20, sh)) m |= 1u << i;
+  return m;
+}
+// per shift: n8 column tiles of the forward GEMMs' B operand, m16 row tiles of the weight gradient's A operand
+constexpr unsigned NZ_N8[4] = {nz_tiles(0, 8), nz_tiles(1, 8), nz_tiles(2, 8), nz_tiles(3, 8)};
+constexpr unsigned NZ_M16[4] = {nz_tiles(0, 16), nz_tiles(1, 16), nz_tiles(2, 16), nz_tiles(3, 16)};
+static_assert(NZ_N8[0] == 0x3ffu && NZ_N8[1] == 0x39cu && NZ_N8[2] == 0x3e0u && NZ_N8[3] == 0x380u, "n8 tiles of the 4-shift form");
+static_assert(NZ_M16[0] == 0x1fu && NZ_M16[1] == 0x1eu && NZ_M16[2] == 0x1cu && NZ_M16[3] == 0x18u, "m16 tiles of the 4-shift form");
+
 struct PrepJobs {
   // forward operand packs: W[Cin][Cout][3][3] -> B[stage][shift][kchunk][80][8]   (head_bf16.cu)
   struct { const float* w; const float* bias; int Cin, Cout, nstages; __nv_bfloat16* out; } fpack[2];

@@ -18,6 +18,7 @@
 #include <type_traits>
 
 #include "../../include/lpb200.h"
+#include "head_prep.cuh"
 #include "head_rows.cuh"
 #include "lpb_common.cuh"
 #include "row_layout.cuh"
@@ -196,17 +197,42 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             const int s = it % CR_STAGES;
             mbar_wait_idle(&full[s], (it / CR_STAGES) & 1, P.backoff);
             const uint32_t a0 = smem_u32(smem + s * stage_bytes), b0 = a0 + a_bytes;
+            // only the n8 tiles (of the warp's six, from column 32e) that the epilogue reads -- [40e, 40e + 40) -- and that
+            // hold real taps of the shift: 8 tile-steps for e = 0 (shifts with dm = 1 carry nothing for py = 0), 16 for e = 1.
+            // The V2 softmax forms with a run-time plane count issue all six tiles with one body for both parities: there,
+            // two per-parity bodies raised ptxas's local-memory spills.
+            if constexpr (V2 && NPL == 0 && MODE != CONVT_ROWS_MID && MODE != CONVT_ROWS_PLANES) {
 #pragma unroll
-            for (int t = 0; t < CR_TILES; ++t) {
-              if (t >= tiles) break;
+              for (int t = 0; t < CR_TILES; ++t) {
+                if (t >= tiles) break;
 #pragma unroll
-              for (int sh = 0; sh < 4; ++sh) {
-                const int shift_rows = (sh >> 1) * Pp + (sh & 1);
+                for (int sh = 0; sh < 4; ++sh) {
+                  const int shift_rows = (sh >> 1) * Pp + (sh & 1);
 #pragma unroll
-                for (int k16 = 0; k16 < 2; ++k16)
-                  mma::kstep(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
-                             b0 + (sh * 4 + 2 * k16) * lbo_b + 32 * e * 16, lbo_b, lane);
+                  for (int k16 = 0; k16 < 2; ++k16)
+                    mma::kstep(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
+                               b0 + (sh * 4 + 2 * k16) * lbo_b + 32 * e * 16, lbo_b, lane);
+                }
               }
+            } else {
+              auto band_mma = [&](auto ec) {
+                constexpr int E = decltype(ec)::value;
+#pragma unroll
+                for (int t = 0; t < CR_TILES; ++t) {
+                  if (t >= tiles) break;
+                  mma::for_shifts([&](auto shc) {
+                    constexpr int sh = decltype(shc)::value;
+                    constexpr unsigned mask = (NZ_N8[sh] >> (4 * E)) & (E ? 0x3eu : 0x1fu);
+                    const int shift_rows = (sh >> 1) * Pp + (sh & 1);
+#pragma unroll
+                    for (int k16 = 0; k16 < 2; ++k16)
+                      mma::kstep_nz<mask>(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
+                                          b0 + (sh * 4 + 2 * k16) * lbo_b + 32 * E * 16, lbo_b, lane);
+                  });
+                }
+              };
+              if (e == 0) band_mma(std::integral_constant<int, 0>{});
+              else band_mma(std::integral_constant<int, 1>{});
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[s]);

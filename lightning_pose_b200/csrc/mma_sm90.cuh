@@ -7,6 +7,7 @@
 // rows8() turns one n8 tile into "lane = accumulator row" form, the layout every epilogue of the head reads.
 #pragma once
 #include <cstdint>
+#include <type_traits>
 
 #include "lpb_common.cuh"
 
@@ -15,6 +16,9 @@ namespace mma {
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x2(uint32_t (&r)[2], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];" : "=r"(r[0]), "=r"(r[1]) : "r"(addr));
 }
 __device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
@@ -53,6 +57,49 @@ __device__ __forceinline__ void kstep(float (&acc)[MT][NT][4], uint32_t a, uint3
       mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
     }
   }
+}
+
+// kstep over the n8 tiles set in MASK only (compile time): the others keep their accumulators and cost no B load, and
+// a pair with one tile left is loaded with ldmatrix .x2.  MASK == 0 issues nothing, not even the A loads.
+template <unsigned MASK, int MT, int NT>
+__device__ __forceinline__ void kstep_nz(float (&acc)[MT][NT][4], uint32_t a, uint32_t lbo_a, uint32_t b, uint32_t lbo_b, int lane) {
+  static_assert(NT % 2 == 0 && (MASK >> NT) == 0, "n8 tiles are loaded in pairs");
+  if constexpr (MASK != 0) {
+    uint32_t af[MT][4];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) ldsm_x4(af[mt], a + (uint32_t)(16 * mt + ((lane >> 3) & 1) * 8 + (lane & 7)) * 16 + (uint32_t)(lane >> 4) * lbo_a);
+    // one lane offset for both load widths (.x2 reads the addresses of lanes 0-15 only: tile 2 np, or 2 np + 1 one
+    // tile further on), so no second per-lane address stays live
+    const uint32_t bl = b + (uint32_t)((lane >> 4) * 8 + (lane & 7)) * 16 + (uint32_t)((lane >> 3) & 1) * lbo_b;
+#pragma unroll
+    for (int np = 0; np < NT / 2; ++np) {
+      const bool lo = (MASK >> (2 * np)) & 1u, hi = (MASK >> (2 * np + 1)) & 1u;
+      if (lo && hi) {
+        uint32_t bf[4];
+        ldsm_x4(bf, bl + (uint32_t)(16 * np) * 16);
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          mma_bf16(acc[mt][2 * np], af[mt], bf[0], bf[1]);
+          mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
+        }
+      } else if (lo || hi) {
+        const int nt = 2 * np + (hi ? 1 : 0);
+        uint32_t bf[2];
+        ldsm_x2(bf, bl + (uint32_t)(8 * nt) * 16);
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) mma_bf16(acc[mt][nt], af[mt], bf[0], bf[1]);
+      }
+    }
+  }
+}
+
+// f(integral_constant<int, sh>) for the four input shifts, so that per-shift tile masks are compile-time
+template <typename F>
+__device__ __forceinline__ void for_shifts(F&& f) {
+  f(std::integral_constant<int, 0>{});
+  f(std::integral_constant<int, 1>{});
+  f(std::integral_constant<int, 2>{});
+  f(std::integral_constant<int, 3>{});
 }
 
 // One K = 16 step, both operands MN-major (the row layout read transposed: K = rows, M / N = channels):
