@@ -8,6 +8,7 @@ prints two counts of mma.sync m16n8k16 FLOPs and the rate each implies over the 
   non-zero   -- only the tiles whose weights hold one of the 9 real (class, shift) taps of 16 (head_prep.cuh NZ_N8 /
                 NZ_M16; for the banded kernel, of the columns its epilogue reads).
 Kernels that skip the zero tiles issue the non-zero count; kernels that do not, the all-tiles count.  The card's name, power limit and SM clocks are read in the same run.
+It also prints the head backward's fixed-order gradient sums (every reduce_partials* launch) as one row: µs and launches per step.
 
     python scripts/profile_head_gemms.py [--clips 16] [--steps 10] [--warmup 3] [--json OUT]
 """
@@ -111,11 +112,15 @@ def main():
                 hp.step(feats)
             torch.cuda.synchronize()
     clocks = clk.summary()
-    per = {}
+    per, calls = {}, {}
     for e in prof.key_averages():
         if e.device_time_total > 0:
             per[e.key] = per.get(e.key, 0.0) + e.device_time_total / args.steps
+            calls[e.key] = calls.get(e.key, 0) + e.count / args.steps
     total = sum(per.values())
+    # the head backward's fixed-order gradient sums (dW2, db2, db1, dW1 of each chain), all launches of reduce_partials*
+    sums = [k for k in per if "reduce_partials" in k]
+    fixed_sums = {"us_per_step": round(sum(per[k] for k in sums), 1), "launches_per_step": round(sum(calls[k] for k in sums), 2)}
 
     nf = args.clips * (bench.B_LABELED + bench.T_UNLABELED)
     c4, h = bench.FEAT_C // 4, bench.FEAT_HW
@@ -131,13 +136,14 @@ def main():
                      "all_tiles_tflops": round(all_t / us / 1e6, 1) if us else None, "nonzero_tflops": round(nz / us / 1e6, 1) if us else None})
     top = sorted(per.items(), key=lambda kv: -kv[1])[:15]
     res = {"gpu": info, "clocks_during_profile": clocks, "frames_per_step": nf, "steps": args.steps,
-           "kernel_us_per_step_total": round(total, 1), "head_gemms": rows,
+           "kernel_us_per_step_total": round(total, 1), "head_gemms": rows, "fixed_order_sums": fixed_sums,
            "top_kernels": [{"kernel": k[:90], "us_per_step": round(v, 1)} for k, v in top]}
     print(f"{info.get('name')}  power limit {info.get('power.limit')}  SM clock {clocks.get('sm_mhz')} MHz (max {clocks.get('sm_max_mhz')})  "
           f"{nf} frames/step, {args.steps} steps")
     print(f"{'kernel':28s} {'us/step':>9s} {'all-tiles TFLOP':>16s} {'non-zero TFLOP':>15s} {'all-tiles TFLOP/s':>18s} {'non-zero TFLOP/s':>17s}")
     for r in rows:
         print(f"{r['kernel']:28s} {r['us_per_step']:9.1f} {r['all_tiles_tflop']:16.4f} {r['nonzero_tflop']:15.4f} {r['all_tiles_tflops'] or 0:18.1f} {r['nonzero_tflops'] or 0:17.1f}")
+    print(f"{'fixed-order sums':28s} {fixed_sums['us_per_step']:9.1f} us/step in {fixed_sums['launches_per_step']:g} launches/step (reduce_partials*)")
     print(f"all kernels: {total:.1f} us/step (summed over both streams)")
     for t in res["top_kernels"]:
         print(f"  {t['us_per_step']:9.1f}  {t['kernel']}")
