@@ -245,6 +245,28 @@ int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes, int ctx, 
 int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* mean3,
                          const float* std3, int layout, int out_bf16, void* out, void* stream);
 
+/* ---- augmented video ingest: the unlabeled branch's DALI augmentation ----------------------------------------
+ * replaces  lightning_pose/data/video/dali.py:154-192  (training.imgaug "dlc" / "dlc-top-down") in front of the
+ * normalisation of lpb_frames_normalize, one view, one draw per call.  Per frame of frames_u8 [F, H, W, 3]:
+ *   1. resize to out_h x out_w exactly as lpb_frames_normalize (bilinear, half-pixel centres, no antialiasing);
+ *   2. params (DEVICE, 6 floats, read at run time) = angle (degrees), sx, sy, brightness, contrast, factor;
+ *   3. M = S_c R_c (fn.transforms.rotation(angle, center=c), then fn.transforms.scale(scale, center=c)) in (x, y):
+ *      A = diag(sx, sy) [[cos, -sin], [sin, cos]], t = c - A c, c = (out_h / 2, out_w / 2) taken as (x, y), the
+ *      reference's own centre (off the image centre when out_h != out_w);
+ *   4. fn.warp_affine(matrix=M, inverse_map=False, fill_value=0): destination pixel (x, y) samples the resized image
+ *      bilinearly at M^-1 (x + 0.5, y + 0.5) - 0.5; taps outside it read 0;
+ *   5. fn.brightness_contrast: brightness * (0.5 + contrast * (v - 0.5)) on 0..255 values (float contrast centre);
+ *   6. fn.noise.shot: Poisson(max(0, v / factor)) * factor, v when factor == 0; Philox4x32-10 keyed by *seed (DEVICE
+ *      int64) and counted by (x, y, frame, channel): the noise does not depend on the launch shape;
+ *   7. / 255 and mean3 / std3 (HOST arrays) to out, layout 0 [F, 3, out_h, out_w] or 1 [F, out_h, out_w, 3], fp32 or
+ *      bf16 (out_bf16).
+ * transform_out (DEVICE, 6 floats): M row-major [[a00, a01, t0], [a10, a11, t1]], the transform lpb_remap_keypoints
+ * undoes.  Reading params and seed on the device lets draws made inside a captured graph take effect on replay.
+ * F = 0 is a no-op. */
+int lpb_frames_augment_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* params,
+                                 const int64_t* seed, const float* mean3, const float* std3, int layout, int out_bf16,
+                                 void* out, float* transform_out, void* stream);
+
 /* ---- crop-zoom inference (bbox mode of the video-ingest boundary) ------------------------------------------------
  * replaces crop_and_resize_frames  lightning_pose/data/bboxes.py:291-343  and the bbox-row slicing in front of it
  *   lightning_pose/data/video/dali.py:332-380, lightning_pose/data/video/pynvvc.py:266-283

@@ -68,6 +68,7 @@ SIGNATURES = {
     "lpb_crnn_combine_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_context_gather": (C.c_int, [_P, _L, _L, _I, _P, _P]),
     "lpb_frames_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
+    "lpb_frames_augment_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
     "lpb_frames_crop_normalize": (C.c_int, [_P, _I, _I, _I, _I, _P, _L, _P, _L, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
     "lpb_bboxes_from_keypoints": (C.c_int, [_P, _L, _I, _L, _I, C.POINTER(C.c_int32), _I, C.c_double, _I, _I, _P, _P]),
     "lpb_bboxes_rolling_median": (C.c_int, [_P, _L, _I, _P, _P]),

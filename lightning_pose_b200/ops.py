@@ -534,6 +534,62 @@ def frames_normalize(frames_u8, size=None, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     return out
 
 
+# training.imgaug "dlc" draw ranges (lightning_pose/data/video/dali.py:160-175) by column of the augment kernel's
+# params: angle (degrees), sx and sy, brightness and contrast, shot-noise factor
+DLC_PARAM_RANGES = ((slice(0, 1), -10.0, 10.0), (slice(1, 3), 0.8, 1.2), (slice(3, 5), 0.75, 1.25), (slice(5, 6), 0.0, 10.0))
+
+
+def draw_dlc_params(num_views: int, device, generator: torch.Generator | None = None):
+    """One draw of the DALI video augmentation per view, on the device: (params (V, 6) fp32, seeds (V,) int64).
+
+    Uniform in the reference's ranges (``DLC_PARAM_RANGES``); seeds key each view's shot noise.  ``generator`` is a
+    torch generator on ``device`` (default: the device's default generator, which a captured CUDA graph replays with
+    fresh draws)."""
+    params = torch.empty((int(num_views), 6), device=device, dtype=torch.float32)
+    for cols, lo, hi in DLC_PARAM_RANGES:
+        params[:, cols].uniform_(lo, hi, generator=generator)
+    seeds = torch.randint(-(2**63), 2**63 - 1, (int(num_views),), device=device, dtype=torch.int64, generator=generator)
+    return params, seeds
+
+
+def frames_augment_normalize(frames_u8, size, params, seed, mean=IMAGENET_MEAN, std=IMAGENET_STD, channels_last=False,
+                             dtype=torch.float32, transform_out=None):
+    """uint8 (F, H, W, 3) frames of one view -> resize, rotate-scale warp, brightness/contrast, shot noise and
+    normalisation in one pass (the DALI augmentation of training.imgaug "dlc", include/lpb200.h).
+
+    ``params``: (6,) fp32 CUDA tensor [angle (degrees), sx, sy, brightness, contrast, factor]; ``seed``: one-element
+    int64 CUDA tensor.  Both are read by the kernel, not the host.  Returns (frames (F, 3, h, w) [or (F, h, w, 3)],
+    transform (2, 3) fp32: the source -> destination matrix the warp applied, what ``remap_keypoints`` undoes); the
+    transform is written into ``transform_out`` when given (a CUDA fp32 tensor of 6 elements)."""
+    if not isinstance(frames_u8, torch.Tensor) or not frames_u8.is_cuda:
+        raise RuntimeError("lpb200: `frames` must be a CUDA tensor (this package has no CPU fallback)")
+    if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[-1] != 3:
+        raise ValueError(f"frames must be uint8 (F, H, W, 3); got {tuple(frames_u8.shape)} {frames_u8.dtype}")
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError("dtype must be float32 or bfloat16")
+    if size is None or len(size) != 2:
+        raise ValueError("size (h, w) is required: the augmentation runs on resized frames")
+    dev = frames_u8.device
+    if not isinstance(params, torch.Tensor) or params.device != dev or params.dtype != torch.float32 or params.numel() != 6:
+        raise ValueError("params must be a 6-element float32 tensor on the frames' device")
+    if not isinstance(seed, torch.Tensor) or seed.device != dev or seed.dtype != torch.int64 or seed.numel() != 1:
+        raise ValueError("seed must be a one-element int64 tensor on the frames' device")
+    if transform_out is None:
+        transform_out = torch.empty((2, 3), device=dev, dtype=torch.float32)
+    elif transform_out.device != dev or transform_out.dtype != torch.float32 or transform_out.numel() != 6 or not transform_out.is_contiguous():
+        raise ValueError("transform_out must be a contiguous 6-element float32 tensor on the frames' device")
+    x = frames_u8.contiguous()
+    p, sd = params.contiguous(), seed.contiguous()
+    f, h, w, _ = x.shape
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((f, oh, ow, 3) if channels_last else (f, 3, oh, ow), device=dev, dtype=dtype)
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(dev):
+        check(lib.lpb_frames_augment_normalize(_ptr(x), f, h, w, oh, ow, _ptr(p), _ptr(sd), m3, s3, int(bool(channels_last)),
+                                               int(dtype == torch.bfloat16), _ptr(out), _ptr(transform_out), _stream()))
+    return out, transform_out.view(2, 3)
+
+
 def _bbox_table(bboxes, name: str) -> torch.Tensor:
     b = _cuda_f32(bboxes, name)
     if b.dim() != 2 or b.shape[1] != 4 or b.shape[0] < 1:

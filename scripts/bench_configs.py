@@ -2,6 +2,7 @@
 measures configs[1]), but the numbers DESIGN.md quotes for them.  Writes gpurun_out/r02_configs.json."""
 import json
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -48,6 +49,72 @@ def fwd_bwd(name, arch, shape, hm):
     ms, med = bench.time_stage(lambda: torch.autograd.grad(out, [f] + params, g, retain_graph=True), flush)
     res[f"{name}_head_bwd_dense"] = {"frames": b, "ms": ms, "us_per_frame": 1e3 * ms / b, "algorithmic_bytes": b * (2 * hb + 2 * fb),
                                      "frac_hbm": b * (2 * hb + 2 * fb) / ms / 1e6 / pk["hbm_gbs"]}
+
+
+def cfg2_unlabeled_aug():
+    """One reference unlabeled training step's augmented ingest (training.imgaug "dlc"): T = 32 uint8 frames
+    (dali.base.train.sequence_length) of a 1024 x 1024 and a 406 x 396 source, resized to 384 x 384.  The augmented
+    kernel (FCHW fp32 and FHWC bf16, shot noise on and off) against its bytes model (each source byte read once, each
+    output written once), the plain lpb_frames_normalize on the same frames, and the eager torch composition
+    (interpolate -> affine_grid / grid_sample -> brightness / contrast -> torch.poisson -> normalise)."""
+    import torch.nn.functional as F
+
+    from lightning_pose_b200 import ops
+
+    t, side = 32, 384
+    mean_t = torch.tensor(ops.IMAGENET_MEAN, device=dev)[:, None, None]
+    std_t = torch.tensor(ops.IMAGENET_STD, device=dev)[:, None, None]
+    seed = torch.tensor([12345], dtype=torch.int64, device=dev)
+    for sh, sw in ((1024, 1024), (406, 396)):
+        tag = f"{sh}x{sw}"
+        u8 = torch.randint(0, 256, (t, sh, sw, 3), dtype=torch.uint8, device=dev)
+        src_bytes = t * sh * sw * 3
+        for noise in ("on", "off"):
+            params = torch.tensor([6.0, 1.1, 0.9, 1.05, 0.95, 5.0 if noise == "on" else 0.0], device=dev)
+            for dtype, cl, form in ((torch.float32, False, "fchw_f32"), (torch.bfloat16, True, "fhwc_bf16")):
+                fn = lambda: ops.frames_augment_normalize(u8, (side, side), params, seed, channels_last=cl, dtype=dtype)
+                ms, med = bench.time_stage(fn, flush)
+                nbytes = src_bytes + t * 3 * side * side * (4 if dtype == torch.float32 else 2)
+                res[f"cfg2_unlabeled_aug_{tag}_{form}_noise_{noise}"] = {
+                    "frames": t, "ms": ms, "ms_median": med, "bytes_model": nbytes, "gbs": nbytes / ms / 1e6,
+                    "frac_hbm": nbytes / ms / 1e6 / pk["hbm_gbs"]}
+        for dtype, cl, form in ((torch.float32, False, "fchw_f32"), (torch.bfloat16, True, "fhwc_bf16")):
+            ms, med = bench.time_stage(lambda: ops.frames_normalize(u8, size=(side, side), channels_last=cl, dtype=dtype), flush)
+            nbytes = src_bytes + t * 3 * side * side * (4 if dtype == torch.float32 else 2)
+            res[f"cfg2_unlabeled_aug_{tag}_{form}_plain_ingest"] = {"frames": t, "ms": ms, "ms_median": med, "bytes_model": nbytes,
+                                                                   "gbs": nbytes / ms / 1e6, "frac_hbm": nbytes / ms / 1e6 / pk["hbm_gbs"]}
+
+        def eager():
+            p, _ = ops.draw_dlc_params(1, dev)
+            ang, sx, sy, br, ct, fac = p[0].unbind()
+            x = F.interpolate(u8.permute(0, 3, 1, 2).float(), size=(side, side), mode="bilinear", align_corners=False)
+            th = torch.deg2rad(ang)
+            a = torch.stack([torch.stack([sx * torch.cos(th), -sx * torch.sin(th)]), torch.stack([sy * torch.sin(th), sy * torch.cos(th)])])
+            ai = torch.linalg.inv(a)  # destination -> source, about c in pixel units, then in grid_sample's [-1, 1] units
+            c = torch.tensor([side / 2.0, side / 2.0], device=dev)
+            theta = torch.cat([ai, (c - ai @ c)[:, None]], dim=1)
+            to_norm = torch.tensor([[2.0 / side, 0, -1], [0, 2.0 / side, -1], [0, 0, 1]], device=dev)
+            full = torch.cat([theta, torch.tensor([[0.0, 0.0, 1.0]], device=dev)])
+            theta_n = (to_norm @ full @ torch.linalg.inv(to_norm))[:2]
+            grid = F.affine_grid(theta_n[None].expand(t, 2, 3), [t, 3, side, side], align_corners=False)
+            x = F.grid_sample(x, grid, mode="bilinear", padding_mode="zeros", align_corners=False)
+            x = br * (0.5 + ct * (x - 0.5))
+            x = torch.poisson(torch.clamp(x / fac, min=0)) * fac
+            return (x / 255.0 - mean_t) / std_t
+
+        with torch.no_grad():
+            ms, med = bench.time_stage(eager, flush, reps=10, warmup=2)
+        res[f"cfg2_unlabeled_aug_{tag}_eager_torch"] = {"frames": t, "ms": ms, "ms_median": med,
+                                                        "note": "FCHW fp32, noise on; interpolate -> affine_grid/grid_sample -> elementwise -> torch.poisson -> normalise"}
+        del u8
+    card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res["cfg2_unlabeled_aug_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0), "hbm_gbs_used": pk["hbm_gbs"]}
+
+
+if sys.argv[1:] == ["cfg2_unlabeled_aug"]:  # these entries alone, as JSON on stdout: python scripts/bench_configs.py cfg2_unlabeled_aug
+    cfg2_unlabeled_aug()
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
 
 
 def cfg3_context():
@@ -333,6 +400,7 @@ for mode in ("on", "off"):
 card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 res["cfg5_crop_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
 cfg3_context()
+cfg2_unlabeled_aug()
 
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 json.dump(res, open(os.path.join(ROOT, "gpurun_out", "r02_configs.json"), "w"), indent=1)
