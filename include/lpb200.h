@@ -40,11 +40,11 @@ const char* lpb_build_arch(void);     /* "sm_90a" */
 
 /* kernel-variant switches: a bring-up / profiling aid (A/B two implementations of the same stage on the same inputs);
  * every variant computes the same results.  lpb_get_tuning returns -1 for an unknown key. */
-#define LPB_TUNE_K1A_ROW_TRANSPOSER 0   /* 1: row-per-lane operand transposer (coalesced saved-copy stores); 0 (default): 8x8 register blocks */
+#define LPB_TUNE_K1A_ROW_TRANSPOSER 0   /* no effect in this build (accepted for compatibility): k1a has one operand transposer */
 #define LPB_TUNE_SOFTMAX_EPILOGUE_V2 1  /* 1 (default): softmax epilogue with one vote per tile and hoisted addressing */
 #define LPB_TUNE_WAIT_BACKOFF 2         /* 1 (default): idle warps back off between mbarrier polls */
 #define LPB_TUNE_DECODE_RING 3          /* 1: soft-argmax planes staged once in shared memory by a bulk-copy ring; 0 (default): warp per plane from global */
-#define LPB_TUNE_K1A_BULK_XS 4          /* 1: the saved operand copy leaves k1a by TMA bulk stores from the operand stage; 0 (default): producer stores */
+#define LPB_TUNE_K1A_BULK_XS 4          /* no effect in this build (accepted for compatibility): k1a has one saved-copy form */
 #define LPB_TUNE_DECODE_L2_HINTS 5      /* 1 (default): L2 evict_last / evict_first hints on the decode's two sweeps of a plane */
 #define LPB_TUNE_B3A_PREFETCH 6         /* 1 (default): b3a epilogue issues the next item's accumulator blocks before storing the current one */
 #define LPB_TUNE_SOFTMAX_SPLIT 7         /* 1 (default): plane softmax as two launches parallel over (frame, band) when there are fewer frames than SMs, else one per-frame two-pass kernel; 0: never split; 2: always */
@@ -55,7 +55,7 @@ const char* lpb_build_arch(void);     /* "sm_90a" */
 #define LPB_TUNE_G2_PATCH 12            /* 1 (default): decode windows enter the gradient rows in a patch pass (one warp per plane) after a look-up-free streaming pass; 0: look-ups fused into the streaming pass */
 #define LPB_TUNE_MMA_TILE_INNER 13      /* no effect in this build (accepted for compatibility): k1a has one MMA order */
 #define LPB_TUNE_DECODE_HINTS 14        /* 1: the fused two-pass softmax emits per-plane decode hints (arg max + largest value outside its 32x32 box) and the decode skips its plane sweeps when they allow; 0 (default): hints never produced (measured: what the decode saves, the issue-bound softmax epilogue pays) */
-#define LPB_TUNE_K1A_XS_COPY 15         /* k1a's saved operand copy: 2 (default): a dedicated extra warp sends each finished operand stage out with TMA bulk stores (the transposers store nothing); 1: streamed out of the finished stage by the transposer threads (whole sectors); 0: each transposer thread stores the rows it produced */
+#define LPB_TUNE_K1A_XS_COPY 15         /* no effect in this build (accepted for compatibility): each k1a item's store warp sends its rows of the finished operand stage to the saved copy with TMA bulk stores */
 #define LPB_TUNE_COUNT 16
 int lpb_set_tuning(int key, int value);
 int lpb_get_tuning(int key);

@@ -13,11 +13,11 @@ extern "C" const char* lpb_build_arch(void) { return "sm_90a"; }
 // launch time only.
 namespace lpb {
 int g_tuning[LPB_TUNE_COUNT] = {
-    0,  // LPB_TUNE_K1A_ROW_TRANSPOSER (measured: 2x the instructions of the block form, slower)
+    0,  // LPB_TUNE_K1A_ROW_TRANSPOSER (no effect)
     1,  // LPB_TUNE_SOFTMAX_EPILOGUE_V2
     1,  // LPB_TUNE_WAIT_BACKOFF
     0,  // LPB_TUNE_DECODE_RING (measured: 1.0x DRAM traffic but too few resident warps: 2x slower at 96x96)
-    0,  // LPB_TUNE_K1A_BULK_XS (measured: 268 vs 223 us per 512 frames: the loader's wait on the filled stage costs more than the producers' stores)
+    0,  // LPB_TUNE_K1A_BULK_XS (no effect)
     1,  // LPB_TUNE_DECODE_L2_HINTS
     1,  // LPB_TUNE_B3A_PREFETCH
     1,  // LPB_TUNE_SOFTMAX_SPLIT
@@ -28,7 +28,7 @@ int g_tuning[LPB_TUNE_COUNT] = {
     1,  // LPB_TUNE_G2_PATCH
     1,  // LPB_TUNE_MMA_TILE_INNER (no effect)
     0,  // LPB_TUNE_DECODE_HINTS (measured: decode 118 -> 52 us per 512 frames, but the bound costs the softmax epilogue +80 us: net zero)
-    2,  // LPB_TUNE_K1A_XS_COPY (2: a dedicated warp sends the finished stage to the saved copy with TMA bulk stores)
+    2,  // LPB_TUNE_K1A_XS_COPY (no effect)
 };
 }
 extern "C" int lpb_set_tuning(int key, int value) {

@@ -28,6 +28,7 @@
 #include "lpb_common.cuh"
 #include "row_layout.cuh"
 #include "mma_sm90.cuh"
+#include "tensor_map.cuh"
 
 namespace lpb {
 
@@ -152,366 +153,135 @@ int launch_head_prep(const PrepJobs& jobs, cudaStream_t s) {
 // =====================================================================================================
 // k1a: PixelShuffle + first transposed convolution
 // =====================================================================================================
-// warps 0..TW-1 transposers, warps TW..TW+CW-1 MMA + epilogue, warp TW+CW TMA loader (+ warp TW+CW+1: saved-copy stores)
-// A CTA works on (frame, tile group) items: the group's K1A_TPG M-tiles of 128 raster rows keep their fp32 accumulators in
-// the MMA warps' registers across all channel stages (warp = one tile's 32-row quarter, 80 columns = 80 registers).
-constexpr int K1A_TW = 4;                      // transposer warps
-constexpr int K1A_TPG = 2;                     // M-tiles per item
-constexpr int K1A_CW = 4 * K1A_TPG;            // MMA warps
-constexpr int K1A_LOADER = K1A_TW + K1A_CW;
-constexpr int K1A_THREADS = 32 * (K1A_TW + K1A_CW + 1);
-constexpr int K1A_ASTAGES = 2;  // K-major operand stages (A + packed weights)
-constexpr int K1A_RSTAGES = 2;  // raw NCHW stages filled by the TMA engine
-constexpr int K1A_MAXPAD = 6;   // pad rows of the saved copy a transposer thread writes per stage (host falls back to head_prep beyond)
+// A CTA works on (frame, band) items.  A band is a run of feature rows (two shuffled image rows each); the G bands of a
+// frame are as equal as possible, and G is the smallest count whose largest band fits the MMA warps' registers: each of
+// the K1A_CW MMA warps keeps up to K1A_MT m16 row tiles x 80 columns of fp32 accumulators across all channel stages.
+// Per 128-channel stage an item stages only its band's feature rows plus the halo row below (the next band's first row;
+// the tensor map's zero fill past the frame's bottom edge), and the saved copy's rows are written by the item that holds
+// them.  16 warps = 4 warpgroups, 128 registers per thread at launch, rebalanced with setmaxnreg:
+//   warpgroup 0     transposers: raw NCHW rows -> K-major operand rows, PixelShuffle folded in
+//   warpgroups 1-2  MMA warps + epilogue
+//   warpgroup 3     warp 12 TMA loader, warp 13 saved-copy stores (training form), warps 14-15 exit
+constexpr int K1A_TW = 4;                                // transposer warps
+constexpr int K1A_CW = 8;                                // MMA warps
+constexpr int K1A_MT = 3;                                // m16 row tiles per MMA warp at most (120 accumulators)
+constexpr int K1A_BAND_ROWS = 16 * K1A_MT * K1A_CW;      // raster rows (incl. zero columns) of the largest band
+constexpr int K1A_LOADER = K1A_TW + K1A_CW;              // warp 12; warp 13 stores the saved copy
+constexpr int K1A_THREADS = 512;
+constexpr int K1A_STAGES = 2;                            // operand stages (A + packed weights), and as many raw stages
+constexpr int K1A_PROD_REGS = 80, K1A_MMA_REGS = 176;    // setmaxnreg: 128 x (2 x 80 + 2 x 176) = 64 K registers
+constexpr int K1A_ZROWS = 72;                            // zero rows: source of the saved copy's lead / trail rows (<= 71 for W <= 31)
+
+struct K1aGeom {
+  int H, W;            // feature map
+  int Wi, P;           // shuffled image width, operand row pitch Wi + 1 (zero column)
+  int G;               // bands per frame (0: no split fits, the shape takes the banded generic path)
+  int a, ubase, urem;  // band i = ubase + (i < urem) units of a feature rows (the last band clipped at H)
+  int nbmax;           // feature rows of the largest band
+  int nfs;             // feature rows staged per item: the largest band + the halo row (G > 1)
+  int box;             // raw elements per channel staged per item: nfs * W rounded up to 8 (a 16-byte TMA box row)
+  int rows_alloc;      // operand rows per K-chunk (multiple of 8)
+};
+
+__host__ inline K1aGeom make_k1a_geom(int H, int W) {
+  K1aGeom k;
+  k.H = H;
+  k.W = W;
+  k.Wi = 2 * W;
+  k.P = 2 * W + 1;
+  // A band starts at a feature row f0 whose first element f0 * W is a multiple of 8: the TMA box's start is then 16-byte
+  // aligned (a start at any other element raises an illegal-instruction error on the H100).  So bands are made of units
+  // of a = 8 / gcd(W, 8) feature rows, as equal as possible, and G is the smallest count whose largest band fits.
+  k.a = 8 / ((W & -W) < 8 ? (W & -W) : 8);
+  const int nu = (H + k.a - 1) / k.a;
+  k.G = 0;
+  for (int g = 1; g <= nu; ++g) {
+    const int units = (nu + g - 1) / g, nb = units * k.a < H ? units * k.a : H;
+    if (2 * nb * k.P <= K1A_BAND_ROWS) {
+      k.G = g;
+      break;
+    }
+  }
+  if (k.G == 0) return k;
+  k.ubase = nu / k.G;
+  k.urem = nu % k.G;
+  const int nbmax = (k.ubase + (k.urem > 0)) * k.a < H ? (k.ubase + (k.urem > 0)) * k.a : H;
+  k.nbmax = nbmax;
+  // one band: the frame's bottom edge is the halo, zero from the stages' one-time clear, so the box never reaches past
+  // the tensor (H * W is a multiple of 8: box <= H * W)
+  k.nfs = nbmax + (k.G > 1 ? 1 : 0);
+  k.box = (k.nfs * W + 7) & ~7;
+  // the MMAs read the band's m16 tiles shifted by up to P + 1 rows; the transposers write nfs feature rows
+  const int mma_rows = (2 * nbmax * k.P + 15) / 16 * 16 + k.P + 1, tr_rows = 2 * k.nfs * k.P;
+  k.rows_alloc = ((mma_rows > tr_rows ? mma_rows : tr_rows) + 7) & ~7;
+  return k;
+}
 
 struct K1aParams {
-  const __nv_bfloat16* feat;  // [B][C][H*W]
+  CUtensorMap feat;           // features [B * C][H * W] bf16, box {k.box, 128}: one stage's channels of an item's rows
   const __nv_bfloat16* wpk;   // packed weights [nstages][HB_BSTAGE_BYTES]
   const float* bias;          // [c1]
   __nv_bfloat16* mid;         // [B][4][Lmid.rows][8]  padded row layout of the next layer's input (row_layout.cuh)
-  __nv_bfloat16* xs;          // optional [B][C/32][Lxs.rows][8]: shuffled features in the padded row layout (weight gradient)
+  __nv_bfloat16* xs;          // [B][C/32][Lxs.rows][8] (training form): shuffled features in the padded row layout
   RowLayout Lmid, Lxs;
-  int B, C, HW, W;            // feature geometry (C = 4 * Cin)
+  int B, C;                   // feature batch and channels (C = 4 * Cin)
   int c1, nstages;
-  int row_transposer;         // 1: row-per-lane transposer (coalesced operand-copy stores); 0: 8x8 register-block transposer
-  int backoff;                // idle warps sleep between barrier polls
-  int xs_bulk;                // 1: the saved operand copy is written by TMA bulk stores straight from the operand stage
-  int xs_pads;                // 1: the block transposers also write the saved copy's pad rows (else head_prep cleared them)
-  int xs_copy;                // 1: the saved copy is streamed out of the finished operand stage by all transposer threads (coalesced)
-  int ntg;                    // tile groups per frame (items per frame); only group 0 writes the saved copy
-  HeadGeom g;
+  K1aGeom k;
 };
 
-// XS (compile time, block transposers): 0 = no saved copy (inference); 1 = the run-time forms (direct stores with / without
-// pad rows, bulk stores, the row-form transposer); 2 = copy-out of the finished operand stage.  Forms 0 and 2 carry none of
-// form 1's per-task address arithmetic (it cost the hot loop predicated-off instructions and local-memory spills).
-// 3 = a dedicated extra warp (block of K1A_THREADS + 32) sends each finished operand stage to the saved copy with TMA bulk
-// stores: the transposers store nothing, and unlike the loader-issued bulk form (xs_bulk) nothing else waits on the stores.
-template <int XS>
-__global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(const __grid_constant__ K1aParams P) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  const HeadGeom g = P.g;
-  const int a_stage_bytes = 4 * g.rows_alloc * 16;
-  const int stage_bytes = a_stage_bytes + HB_BSTAGE_BYTES;
-  const int raw_bytes = 4 * HB_KSTAGE * P.HW * 2;  // 128 source channels of one stage, contiguous in NCHW
-  unsigned char* stage_base = smem;
-  unsigned char* raw_base = smem + K1A_ASTAGES * stage_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(raw_base + K1A_RSTAGES * raw_bytes);
-  uint64_t* full = bars;                        // [2] operands ready (128 transposer arrivals + weight bytes)
-  uint64_t* empty = bars + 2;                   // [2] MMAs reading the stage have completed
-  uint64_t* raw_full = bars + 4;                // [2] TMA bytes landed
-  uint64_t* raw_empty = bars + 6;               // [2] transposers are done with the raw stage
-  unsigned char* zreg = reinterpret_cast<unsigned char*>(bars) + 128;  // 1 KB of zeros: source of the saved copy's lead rows
-  const bool xs_bulk = P.xs && P.xs_bulk;
+// item -> frame b, first feature row f0 and feature-row count nb of its band
+__device__ __forceinline__ void k1a_band(const K1aGeom& k, int item, int& b, int& f0, int& nb) {
+  b = item / k.G;
+  const int band = item - b * k.G;
+  f0 = k.a * (band * k.ubase + min(band, k.urem));
+  nb = min(k.a * (k.ubase + (band < k.urem ? 1 : 0)), k.H - f0);
+}
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-  // zero the operand stages once: halo rows/columns are never written again
-  for (int i = tid; i < K1A_ASTAGES * stage_bytes / 16; i += K1A_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (tid < 64) reinterpret_cast<uint4*>(zreg)[tid] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&full[s], 32 * K1A_TW + 1);
-      mbar_init(&empty[s], K1A_CW + ((xs_bulk || XS == 3) ? 1 : 0));  // the MMA warps have read the stage (+ the bulk stores of the saved copy have)
-      mbar_init(&raw_full[s], 1);
-      mbar_init(&raw_empty[s], 32 * K1A_TW);
+// One MMA warp's share of every item of its CTA: m16 tiles [m0, m0 + MT) of the band raster, all 80 columns, accumulated
+// over the item's stages; then + bias -> bf16 -> mid activations.  Per accumulator element
+// the MMA sequence is stages, then shifts, then k16, then the shift's non-zero n8 tiles.
+template <int MT>
+__device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* stage_base, int stage_bytes, int a_stage_bytes,
+                                             uint64_t* full, uint64_t* empty, int m0, int lane) {
+  const K1aGeom& k = P.k;
+  const uint32_t lbo_a = k.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
+  const int nitems = P.B * k.G;
+  int it0 = 0;
+  for (int item = blockIdx.x; item < nitems; item += gridDim.x, it0 += P.nstages) {
+    int b, f0, nb;
+    k1a_band(k, item, b, f0, nb);
+    float acc[MT > 0 ? MT : 1][HB_NCOLS / 8][4];
+    mma::zero(acc);
+    for (int st = 0; st < P.nstages; ++st) {
+      const int it = it0 + st, s = it % K1A_STAGES;
+      mbar_wait(&full[s], (it / K1A_STAGES) & 1);
+      if constexpr (MT > 0) {
+        const uint32_t a0 = smem_u32(stage_base + s * stage_bytes);
+        const uint32_t b0 = a0 + a_stage_bytes;
+        mma::for_shifts([&](auto shc) {  // only the n8 tiles with real taps of the shift (24 of 40)
+          constexpr int sh = decltype(shc)::value;
+          const int shift_rows = (sh >> 1) * k.P + (sh & 1);
+#pragma unroll
+          for (int k16 = 0; k16 < 2; ++k16)
+            mma::kstep_nz<NZ_N8[sh]>(acc, a0 + (2 * k16) * lbo_a + (16 * m0 + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
+        });
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-    fence_mbar_init();
-  }
-  fence_proxy_async();  // generic-proxy zero fill -> visible to the async proxy (bulk stores of the saved copy)
-  __syncthreads();
-
-  const int rows_mid = P.Lmid.rows;
-  const int nitems = P.B * P.ntg;
-  int nmine = 0;
-  for (int item = blockIdx.x; item < nitems; item += gridDim.x) ++nmine;
-  const int total_it = nmine * P.nstages;
-  // item of pipeline iteration it: frame b, tile group tg (group 0 also writes the saved copy)
-  auto item_of = [&](int it, int& b, int& tg) {
-    const int item = blockIdx.x + (it / P.nstages) * gridDim.x;
-    b = item / P.ntg;
-    tg = item - b * P.ntg;
-  };
-
-  if (warp == K1A_LOADER) {
-    // ================= TMA loader: raw feature slabs run ahead, weights follow the operand slots ====
-    if (lane == 0) {
-      auto issue_raw = [&](int it) {
-        const int r = it % K1A_RSTAGES;
-        mbar_wait(&raw_empty[r], ((it / K1A_RSTAGES) & 1) ^ 1);
-        int b, tg;
-        item_of(it, b, tg);
-        const int st = it % P.nstages;
-        mbar_expect_tx(&raw_full[r], (uint32_t)raw_bytes);
-        bulk_g2s(raw_base + r * raw_bytes, P.feat + ((size_t)b * P.C + (size_t)st * 4 * HB_KSTAGE) * P.HW, (uint32_t)raw_bytes,
-                 &raw_full[r]);
-      };
-      if (total_it > 0) issue_raw(0);
-      for (int it = 0; it < total_it; ++it) {
-        if (it + 1 < total_it) issue_raw(it + 1);
-        const int s = it % K1A_ASTAGES, st = it % P.nstages;
-        mbar_wait(&empty[s], ((it / K1A_ASTAGES) & 1) ^ 1);
-        mbar_expect_tx(&full[s], HB_BSTAGE_BYTES);
-        bulk_g2s(stage_base + s * stage_bytes + a_stage_bytes,
-                 reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * HB_BSTAGE_BYTES, HB_BSTAGE_BYTES, &full[s]);
-        if (xs_bulk) {
-          // The operand stage IS the saved copy's layout (row_layout.cuh): once the producers have filled it, each
-          // K-chunk goes to global memory as two bulk stores (the zero lead rows, then raster + halo rows) -- fully
-          // coalesced, asynchronous, and no store instruction on the producers' LSU path (their 16-byte stores at a
-          // 256-byte stride were k1a's critical path in training).  The stage is released once the MMAs AND these
-          // stores have read it.
-          mbar_wait(&full[s], (it / K1A_ASTAGES) & 1);
-          int b, tg;
-          item_of(it, b, tg);
-          if (tg == 0) {
-            unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
-            const unsigned char* As = stage_base + s * stage_bytes;
-            const uint32_t lead_b = (uint32_t)P.Lxs.lead * 16, body_b = (uint32_t)(g.rows + g.P + 1) * 16;
+    if constexpr (MT > 0) {
+      // epilogue, 32 rows (two m16 tiles) at a time: (+bias) -> bf16 -> mid activations (A layout); channel c1 of the mid
+      // activations is the constant 1 (lets the next layer fold its bias into the GEMM)
+      const int rows_mid = P.Lmid.rows;
+      static_for<0, (MT + 1) / 2>([&](auto pc) {
+        constexpr int M0 = 2 * decltype(pc)::value;
+        float d[HB_NCOLS];
 #pragma unroll
-            for (int kc = 0; kc < 4; ++kc) {
-              unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
-              bulk_s2g(dst, zreg, lead_b);
-              bulk_s2g(dst + lead_b, As + (size_t)kc * g.rows_alloc * 16, body_b);
-            }
-            bulk_commit_group();
-            bulk_wait_group_read0();
-          }
-          mbar_arrive(&empty[s]);
-        }
-      }
-      if (xs_bulk) bulk_wait_group0();  // the copies are in global memory before the kernel ends
-    }
-  } else if (warp < K1A_TW && P.row_transposer) {
-    // ================= transposers, row form: lane = shuffled pixel n of one image row ==================
-    // A warp takes (K-chunk kc, image row m) pairs; lane n gathers its 8 channels (source channels 4(8kc+e)+q, q =
-    // 2(m&1) + (n&1), position (m>>1, n>>1)) with 2-byte shared loads -- conflict-free: even / odd lanes read two
-    // channel rows 288 B apart -- and stores ONE 16-byte operand row.  Consecutive lanes write consecutive rows, so
-    // both the shared-memory store and the global store of the saved copy are fully coalesced (the 8x8 register-block
-    // form writes 16 bytes per lane at a 256-byte stride: 32 half-used sectors per store instruction, which made the
-    // transposers' LSU time -- not the tensor core -- the critical path of a training forward).
-    const int Hi = g.Hi, Wi = g.Wi, npair = 4 * Hi;
-    for (int it = 0; it < total_it; ++it) {
-      const int s = it % K1A_ASTAGES, r = it % K1A_RSTAGES;
-      mbar_wait(&raw_full[r], (it / K1A_RSTAGES) & 1);
-      mbar_wait(&empty[s], ((it / K1A_ASTAGES) & 1) ^ 1);
-      unsigned char* As = stage_base + s * stage_bytes;
-      unsigned char* xs_st = nullptr;
-      if (P.xs && !xs_bulk) {
-        int b, tg;
-        item_of(it, b, tg);
-        const int st = it % P.nstages;
-        if (tg == 0) xs_st = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
-      }
-      const unsigned short* raw = reinterpret_cast<const unsigned short*>(raw_base + r * raw_bytes);
-      for (int pr = warp; pr < npair; pr += K1A_TW) {
-        const int kc = pr / Hi, m = pr - kc * Hi;
-        const int chan0 = 32 * kc + 2 * (m & 1);  // source channel of e = 0, dj = 0
-        for (int n = lane; n < Wi; n += 32) {
-          const unsigned short* src = raw + (size_t)(chan0 + (n & 1)) * P.HW + (m >> 1) * P.W + (n >> 1);
-          uint32_t pk[4];
-#pragma unroll
-          for (int e2 = 0; e2 < 4; ++e2) pk[e2] = (uint32_t)src[(size_t)(8 * e2) * P.HW] | ((uint32_t)src[(size_t)(8 * e2 + 4) * P.HW] << 16);
-          const uint4 o = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          const int row = m * g.P + n;
-          *reinterpret_cast<uint4*>(As + ((size_t)kc * g.rows_alloc + row) * 16) = o;
-          if (xs_st) *reinterpret_cast<uint4*>(xs_st + ((size_t)kc * P.Lxs.rows + P.Lxs.lead + row) * 16) = o;
-        }
-      }
-      fence_proxy_async();
-      mbar_arrive(&full[s]);
-      mbar_arrive(&raw_empty[r]);
-    }
-  } else if (warp < K1A_TW) {
-    // ================= transposers: raw NCHW slab (smem) -> K-major rows, PixelShuffle folded in ======
-    // A task is one 8x8 bf16 transpose: 8 channels x 8 consecutive spatial positions (one 16-byte chunk per channel)
-    // of one sub-pixel class q -> 8 rows of 16 bytes.  Which tasks a thread owns, and where they read / write, is the
-    // same for every stage, so the index arithmetic (divisions by runtime sizes) is done once, up front.
-    const int nchunk = P.HW / 8;  // 16-byte chunks of 8 consecutive spatial positions per channel
-    const int ntasks = 4 * 4 * nchunk;
-    constexpr int MAXT = 3;
-    uint32_t t_raw[MAXT], t_a[MAXT], t_x[MAXT];
-    int t_wrap[MAXT];
-    int nt = 0;
-#pragma unroll
-    for (int k = 0; k < MAXT; ++k) {
-      const int task = tid + k * 32 * K1A_TW;
-      t_raw[k] = t_a[k] = t_x[k] = 0;
-      t_wrap[k] = 8;
-      if (task < ntasks) {
-        const int sc = task % nchunk, q = (task / nchunk) & 3, kc = task / (4 * nchunk);
-        const int sp0 = sc * 8, i0 = sp0 / P.W, jc0 = sp0 - i0 * P.W;
-        const int row0 = (2 * i0 + (q >> 1)) * g.P + 2 * jc0 + (q & 1);
-        t_raw[k] = (uint32_t)(((4 * kc * 8 + q) * P.HW + sc * 8) * 2);
-        t_a[k] = (uint32_t)((kc * g.rows_alloc + row0) * 16);
-        if (XS == 1) t_x[k] = (uint32_t)((kc * P.Lxs.rows + P.Lxs.lead + row0) * 16);
-        t_wrap[k] = P.W - jc0;  // position at which the image row wraps (W >= 8: at most once per task)
-        nt = k + 1;
-      }
-    }
-    const uint32_t chan_stride = (uint32_t)(4 * P.HW * 2);       // next shuffled channel e -> 4 source channels on
-    const uint32_t wrap_jump = (uint32_t)((2 * g.P - 2 * P.W) * 16);  // extra bytes once the position wraps to row i + 1
-    // The saved copy's pad rows (the zero column of every image row, the lead / trail rows) are written here as well, next
-    // to the real rows that share their 32-byte sectors: a separate clearing pass over those scattered 16-byte pieces
-    // cost 35 us per 512 frames in the preparation launch.  Per stage: 4 K-chunks x npad rows over the 128 transposer threads.
-    constexpr int MAXP = K1A_MAXPAD;
-    uint32_t t_pad[MAXP];
-    int npd = 0;
-    if (XS == 1) {
-      const RowLayout L = P.Lxs;
-      const int body1 = L.lead + L.Hi * L.Pp, ntail = L.rows - body1, npad = L.lead + ntail + L.Hi;
-#pragma unroll
-      for (int k = 0; k < MAXP; ++k) {
-        const int e = tid + k * 32 * K1A_TW;
-        t_pad[k] = 0;
-        if (e < 4 * npad) {
-          const int kc = e / npad, i = e - kc * npad;
-          const int row = i < L.lead ? i : (i < L.lead + ntail ? body1 + (i - L.lead) : L.lead + (i - L.lead - ntail) * L.Pp + L.Wi);
-          t_pad[k] = (uint32_t)((kc * L.rows + row) * 16);
-          npd = k + 1;
-        }
-      }
-    }
-    for (int it = 0; it < total_it; ++it) {
-      const int s = it % K1A_ASTAGES, r = it % K1A_RSTAGES;
-      mbar_wait(&raw_full[r], (it / K1A_RSTAGES) & 1);
-      mbar_wait(&empty[s], ((it / K1A_ASTAGES) & 1) ^ 1);
-      unsigned char* As = stage_base + s * stage_bytes;
-      unsigned char* xs_st = nullptr;  // this (frame, stage)'s 4 K-chunks of the saved copy
-      unsigned char* xs_cp = nullptr;  // copy-out form: the saved copy leaves through the operand stage (below)
-      int b_it, tg_it;
-      item_of(it, b_it, tg_it);
-      if (XS != 0 && XS != 3 && P.xs && !xs_bulk && tg_it == 0) {
-        const int st = it % P.nstages;
-        unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b_it * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
-        if (XS == 2) xs_cp = slab;
-        else xs_st = slab;
-      }
-      const unsigned char* raw = raw_base + r * raw_bytes;
-#pragma unroll
-      for (int k = 0; k < MAXT; ++k) {
-        if (k >= nt) break;
-        uint4 v[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = *reinterpret_cast<const uint4*>(raw + t_raw[k] + e * chan_stride);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint32_t wj[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) wj[e] = j == 0 ? v[e].x : (j == 1 ? v[e].y : (j == 2 ? v[e].z : v[e].w));
-#pragma unroll
-          for (int hl = 0; hl < 2; ++hl) {
-            const uint32_t sel = hl ? 0x7632u : 0x5410u;
-            uint4 o;
-            o.x = __byte_perm(wj[0], wj[1], sel);
-            o.y = __byte_perm(wj[2], wj[3], sel);
-            o.z = __byte_perm(wj[4], wj[5], sel);
-            o.w = __byte_perm(wj[6], wj[7], sel);
-            const int pos = 2 * j + hl;  // position within the task: spatial index sc*8 + pos
-            const uint32_t delta = (uint32_t)(pos * 32) + (pos >= t_wrap[k] ? wrap_jump : 0u);
-            *reinterpret_cast<uint4*>(As + t_a[k] + delta) = o;
-            if (XS == 1 && xs_st) *reinterpret_cast<uint4*>(xs_st + t_x[k] + delta) = o;
-          }
-        }
-      }
-      if (XS == 1 && xs_st && P.xs_pads) {
-#pragma unroll
-        for (int k = 0; k < MAXP; ++k)
-          if (k < npd) *reinterpret_cast<uint4*>(xs_st + t_pad[k]) = make_uint4(0, 0, 0, 0);
-      }
-      fence_proxy_async();
-      mbar_arrive(&full[s]);
-      mbar_arrive(&raw_empty[r]);
-      if (xs_cp) {
-        // Saved copy, copy-out form: the operand stage IS the copy's row layout (halo rows and zero columns included), so
-        // once all four transposer warps have written it, the 128 threads stream it out with consecutive 16-byte rows per
-        // lane -- every store instruction fills 16 whole sectors.  (The direct form stores each 16-byte row from the thread
-        // that transposed it: 32 half-used sectors per instruction, every sector written twice -- the transposers' LSU
-        // time was k1a's bound in training.)  The MMAs read the stage meanwhile; it is rewritten two stages later, after
-        // this loop's next barrier.
-        asm volatile("bar.sync 2, %0;" ::"n"(32 * K1A_TW) : "memory");
-        const int lead = P.Lxs.lead, nrows = P.Lxs.rows, nbody = nrows - lead;
-        constexpr int NT = 32 * K1A_TW, UB = 6;  // UB independent shared loads in flight per thread, then UB stores
-#pragma unroll 1
-        for (int kc = 0; kc < 4; ++kc) {
-          const unsigned char* srcp = As + (size_t)kc * g.rows_alloc * 16;
-          unsigned char* dstp = xs_cp + (size_t)kc * nrows * 16;
-          if (tid < lead) *reinterpret_cast<uint4*>(dstp + (size_t)tid * 16) = make_uint4(0, 0, 0, 0);  // lead <= 128 rows (host)
-          dstp += (size_t)lead * 16;
-#pragma unroll 1
-          for (int r0 = tid; r0 < nbody; r0 += UB * NT) {
-            uint4 v[UB];
-#pragma unroll
-            for (int u = 0; u < UB; ++u)
-              if (r0 + u * NT < nbody) v[u] = *reinterpret_cast<const uint4*>(srcp + (size_t)(r0 + u * NT) * 16);
-#pragma unroll
-            for (int u = 0; u < UB; ++u)
-              if (r0 + u * NT < nbody) *reinterpret_cast<uint4*>(dstp + (size_t)(r0 + u * NT) * 16) = v[u];
-          }
-        }
-      }
-    }
-  } else if (XS == 3 && warp == K1A_LOADER + 1) {
-    // ================= store warp: finished operand stage -> saved copy, by TMA bulk stores =========================
-    if (lane == 0) {
-      const uint32_t lead_b = (uint32_t)P.Lxs.lead * 16, body_b = (uint32_t)(g.rows + g.P + 1) * 16;
-      for (int it = 0; it < total_it; ++it) {
-        const int s = it % K1A_ASTAGES, st = it % P.nstages;
-        mbar_wait(&full[s], (it / K1A_ASTAGES) & 1);
-        int b, tg;
-        item_of(it, b, tg);
-        if (tg == 0) {
-          unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
-          const unsigned char* As = stage_base + s * stage_bytes;
-#pragma unroll
-          for (int kc = 0; kc < 4; ++kc) {
-            unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
-            bulk_s2g(dst, zreg, lead_b);
-            bulk_s2g(dst + lead_b, As + (size_t)kc * g.rows_alloc * 16, body_b);
-          }
-          bulk_commit_group();
-          bulk_wait_group_read0();
-        }
-        mbar_arrive(&empty[s]);
-      }
-      bulk_wait_group0();  // the copies are in global memory before the kernel ends
-    }
-  } else if (warp < K1A_LOADER) {
-    // ================= MMA warps: tile t = tg * K1A_TPG + tt, accumulator rows [32 q, 32 q + 32) of it, all 80 columns ====
-    // epilogue: (+bias) -> bf16 -> mid activations (A layout); channel c1 of the mid activations is the constant 1 (lets
-    // the next layer fold its bias into the GEMM)
-    const int cw = warp - K1A_TW, q = cw & 3, tt = cw >> 2;
-    const uint32_t lbo_a = g.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
-    int it = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int b = item / P.ntg, t = (item - b * P.ntg) * K1A_TPG + tt;
-      const bool active = t < g.tiles;
-      float acc[2][HB_NCOLS / 8][4];
-      mma::zero(acc);
-      for (int st = 0; st < P.nstages; ++st, ++it) {
-        const int s = it % K1A_ASTAGES;
-        mbar_wait(&full[s], (it / K1A_ASTAGES) & 1);
-        if (active) {
-          const uint32_t a0 = smem_u32(stage_base + s * stage_bytes);
-          const uint32_t b0 = a0 + a_stage_bytes;
-          mma::for_shifts([&](auto shc) {  // only the n8 tiles with real taps of the shift (24 of 40)
-            constexpr int sh = decltype(shc)::value;
-            const int shift_rows = (sh >> 1) * g.P + (sh & 1);
-#pragma unroll
-            for (int k16 = 0; k16 < 2; ++k16)
-              mma::kstep_nz<NZ_N8[sh]>(acc, a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
-          });
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);
-      }
-      if (!active) continue;
-      float d[HB_NCOLS];
-#pragma unroll
-      for (int nt = 0; nt < HB_NCOLS / 8; ++nt) mma::rows8(acc, nt, &d[nt * 8], lane);
-      {
-        const int row = t * 128 + 32 * q + lane;
-        const int m = row / g.P, n = row - m * g.P;
-        if (m < g.Hi && n < g.Wi) {
+        for (int nt = 0; nt < HB_NCOLS / 8; ++nt) mma::rows8_at<M0>(acc, nt, &d[nt * 8], lane);
+        const int row = 16 * (m0 + M0) + lane;  // band raster row
+        const int ml = row / k.P, n = row - ml * k.P;
+        if ((M0 + 1 < MT || lane < 16) && ml < 2 * nb && n < k.Wi) {
+          const int m = 2 * f0 + ml;
 #pragma unroll
           for (int cls = 0; cls < 4; ++cls) {
             const int y = 2 * m + (cls >> 1), x = 2 * n + (cls & 1);
@@ -537,12 +307,187 @@ __global__ void __launch_bounds__(K1A_THREADS + 32, 1) k1a_shuffle_convt_kernel(
                 __nv_bfloat162 h2 = __floats2bfloat162_rn(f[0], f[1]);
                 pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
               }
-              *reinterpret_cast<uint4*>(P.mid + ((((size_t)b * 4 + kc) * rows_mid + row2) * 8)) =
-                  make_uint4(pk[0], pk[1], pk[2], pk[3]);
+              *reinterpret_cast<uint4*>(P.mid + ((((size_t)b * 4 + kc) * rows_mid + row2) * 8)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
             }
           }
         }
+      });
+    }
+  }
+}
+
+// XS = 1: training form, warp 13 writes the saved operand copy; XS = 0: inference
+template <int XS>
+__global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const __grid_constant__ K1aParams P) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  const K1aGeom& k = P.k;
+  const int a_stage_bytes = 4 * k.rows_alloc * 16;
+  const int stage_bytes = a_stage_bytes + HB_BSTAGE_BYTES;
+  const int raw_bytes = 4 * HB_KSTAGE * k.box * 2;  // 128 source channels x the item's staged positions
+  unsigned char* stage_base = smem;
+  unsigned char* raw_base = smem + K1A_STAGES * stage_bytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(raw_base + K1A_STAGES * raw_bytes);
+  uint64_t* full = bars;                         // operands ready (128 transposer arrivals + weight bytes)
+  uint64_t* empty = bars + K1A_STAGES;           // the MMA warps (+ the saved-copy stores) have read the stage
+  uint64_t* raw_full = bars + 2 * K1A_STAGES;    // TMA bytes landed
+  uint64_t* raw_empty = bars + 3 * K1A_STAGES;   // the transposers are done with the raw stage
+  unsigned char* zrows = reinterpret_cast<unsigned char*>(bars) + 128;
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+
+  // zero the operand stages once: zero columns and rows past the staged ones are never written again
+  for (int i = tid; i < K1A_STAGES * stage_bytes / 16; i += K1A_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < K1A_ZROWS; i += K1A_THREADS) reinterpret_cast<uint4*>(zrows)[i] = make_uint4(0, 0, 0, 0);
+  if (tid == 0) {
+    for (int s = 0; s < K1A_STAGES; ++s) {
+      mbar_init(&full[s], 32 * K1A_TW + 1);
+      mbar_init(&empty[s], K1A_CW + XS);
+      mbar_init(&raw_full[s], 1);
+      mbar_init(&raw_empty[s], 32 * K1A_TW);
+    }
+    fence_mbar_init();
+  }
+  fence_proxy_async();  // generic-proxy zero fill -> visible to the async proxy (bulk stores of the saved copy)
+  __syncthreads();
+
+  const int nitems = P.B * k.G;
+  const int nmine = (nitems - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int total_it = nmine * P.nstages;
+  const int item_base = blockIdx.x;
+  auto item_of = [&](int it) { return item_base + (it / P.nstages) * (int)gridDim.x; };
+
+  const int wg = warp >> 2;
+  if (wg == 1 || wg == 2) {
+    setmaxnreg_inc<K1A_MMA_REGS>();
+    // ================= MMA warps: m16 tiles dealt contiguously and evenly (warps w and w + 4 share an SM sub-partition's
+    // tensor pipe, and warp w gets a tile more than warp w + 4 only when the others do).  The tiles of the LARGEST band are
+    // dealt for every item, so each warp has one tile count for the whole launch; a smaller band's extra rows are staged
+    // (feature rows past the band, or zeros) and their accumulator rows are not written.  =================
+    const int cw = warp - K1A_TW;
+    const int t16 = (2 * k.nbmax * k.P + 15) / 16, base = t16 / K1A_CW, extra = t16 - base * K1A_CW;
+    const int cnt = base + (cw < extra ? 1 : 0), m0 = cw * base + min(cw, extra);
+    if (cnt == 3) k1a_mma_warp<3>(P, stage_base, stage_bytes, a_stage_bytes, full, empty, m0, lane);
+    else if (cnt == 2) k1a_mma_warp<2>(P, stage_base, stage_bytes, a_stage_bytes, full, empty, m0, lane);
+    else if (cnt == 1) k1a_mma_warp<1>(P, stage_base, stage_bytes, a_stage_bytes, full, empty, m0, lane);
+    else k1a_mma_warp<0>(P, stage_base, stage_bytes, a_stage_bytes, full, empty, m0, lane);
+    return;
+  }
+  setmaxnreg_dec<K1A_PROD_REGS>();
+  if (wg == 0) {
+    // ================= transposers: raw NCHW rows (smem) -> K-major operand rows, PixelShuffle folded in ======
+    // A task is one 8x8 bf16 transpose: 8 channels x 8 consecutive staged positions (one 16-byte chunk per channel) of
+    // one sub-pixel class q -> 8 operand rows of 16 bytes.  Staged position p = (feature row - f0) * W + j is operand row
+    // (2 (p / W) + (q >> 1)) * P + 2 (p % W) + (q & 1).  Which tasks a thread owns, and where they read / write, is the
+    // same for every stage and item, so the index arithmetic is done once, up front.
+    const int nchunk = k.box / 8;
+    const int ntasks = 4 * 4 * nchunk;
+    const int npos = k.nfs * k.W;  // positions past it (the box's rounding) are not operand rows
+    constexpr int MAXT = 2;        // box <= 128 (make_k1a_geom: nfs * W <= 127), so <= 256 tasks over 128 threads
+    uint32_t t_raw[MAXT], t_a[MAXT];
+    int t_wrap[MAXT], t_lim[MAXT];
+    int nt = 0;
+#pragma unroll
+    for (int kk = 0; kk < MAXT; ++kk) {
+      const int task = tid + kk * 32 * K1A_TW;
+      t_raw[kk] = t_a[kk] = 0;
+      t_wrap[kk] = t_lim[kk] = 8;
+      if (task < ntasks) {
+        const int sc = task % nchunk, q = (task / nchunk) & 3, kc = task / (4 * nchunk);
+        const int sp0 = sc * 8, i0 = sp0 / k.W, jc0 = sp0 - i0 * k.W;
+        const int row0 = (2 * i0 + (q >> 1)) * k.P + 2 * jc0 + (q & 1);
+        t_raw[kk] = (uint32_t)(((4 * kc * 8 + q) * k.box + sp0) * 2);
+        t_a[kk] = (uint32_t)((kc * k.rows_alloc + row0) * 16);
+        t_wrap[kk] = k.W - jc0;  // position at which the image row wraps (W >= 4: at most once per task)
+        t_lim[kk] = npos - sp0;
+        nt = kk + 1;
       }
+    }
+    const uint32_t chan_stride = (uint32_t)(4 * k.box * 2);          // next shuffled channel e -> 4 source channels on
+    const uint32_t wrap_jump = (uint32_t)((2 * k.P - 2 * k.W) * 16);  // extra bytes once the position wraps to row i + 1
+    for (int it = 0; it < total_it; ++it) {
+      const int s = it % K1A_STAGES;
+      mbar_wait(&raw_full[s], (it / K1A_STAGES) & 1);
+      mbar_wait(&empty[s], ((it / K1A_STAGES) & 1) ^ 1);
+      unsigned char* As = stage_base + s * stage_bytes;
+      const unsigned char* raw = raw_base + s * raw_bytes;
+#pragma unroll
+      for (int kk = 0; kk < MAXT; ++kk) {
+        if (kk >= nt) break;
+        uint4 v[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = *reinterpret_cast<const uint4*>(raw + t_raw[kk] + e * chan_stride);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          uint32_t wj[8];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) wj[e] = j == 0 ? v[e].x : (j == 1 ? v[e].y : (j == 2 ? v[e].z : v[e].w));
+#pragma unroll
+          for (int hl = 0; hl < 2; ++hl) {
+            const uint32_t sel = hl ? 0x7632u : 0x5410u;
+            uint4 o;
+            o.x = __byte_perm(wj[0], wj[1], sel);
+            o.y = __byte_perm(wj[2], wj[3], sel);
+            o.z = __byte_perm(wj[4], wj[5], sel);
+            o.w = __byte_perm(wj[6], wj[7], sel);
+            const int pos = 2 * j + hl;  // position within the task: staged position sc*8 + pos
+            const uint32_t delta = (uint32_t)(pos * 32) + (pos >= t_wrap[kk] ? wrap_jump : 0u);
+            if (pos < t_lim[kk]) *reinterpret_cast<uint4*>(As + t_a[kk] + delta) = o;
+          }
+        }
+      }
+      fence_proxy_async();  // the saved-copy bulk stores read the stage through the async proxy
+      mbar_arrive(&full[s]);
+      mbar_arrive(&raw_empty[s]);
+    }
+  } else if (warp == K1A_LOADER) {
+    // ================= TMA loader: raw feature rows run one stage ahead, weights follow the operand slots ====
+    if (lane == 0) {
+      auto issue_raw = [&](int it) {
+        const int r = it % K1A_STAGES;
+        mbar_wait(&raw_empty[r], ((it / K1A_STAGES) & 1) ^ 1);
+        int b, f0, nb;
+        k1a_band(k, item_of(it), b, f0, nb);
+        const int st = it % P.nstages;
+        mbar_expect_tx(&raw_full[r], (uint32_t)raw_bytes);  // out-of-range elements (past the frame) land as zeros
+        tma_load_2d(raw_base + r * raw_bytes, &P.feat, f0 * k.W, b * P.C + st * 4 * HB_KSTAGE, &raw_full[r]);
+      };
+      if (total_it > 0) issue_raw(0);
+      for (int it = 0; it < total_it; ++it) {
+        if (it + 1 < total_it) issue_raw(it + 1);
+        const int s = it % K1A_STAGES, st = it % P.nstages;
+        mbar_wait(&empty[s], ((it / K1A_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&full[s], HB_BSTAGE_BYTES);
+        bulk_g2s(stage_base + s * stage_bytes + a_stage_bytes,
+                 reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * HB_BSTAGE_BYTES, HB_BSTAGE_BYTES, &full[s]);
+      }
+    }
+  } else if (XS && warp == K1A_LOADER + 1) {
+    // ================= store warp: the finished operand stage -> the saved copy, by TMA bulk stores =================
+    // The operand stage IS the saved copy's row layout (row_layout.cuh), zero columns included: per K-chunk, the band's
+    // image rows are one contiguous store.  The first band also writes the lead rows, the last band the trail rows, so
+    // every row of the copy is written exactly once.
+    if (lane == 0) {
+      const int lead = P.Lxs.lead, trail = P.Lxs.rows - lead - P.Lxs.Hi * P.Lxs.Pp;
+      for (int it = 0; it < total_it; ++it) {
+        const int s = it % K1A_STAGES, st = it % P.nstages;
+        mbar_wait(&full[s], (it / K1A_STAGES) & 1);
+        int b, f0, nb;
+        k1a_band(k, item_of(it), b, f0, nb);
+        unsigned char* slab = reinterpret_cast<unsigned char*>(P.xs + ((size_t)b * P.nstages + st) * 4 * (size_t)P.Lxs.rows * 8);
+        const unsigned char* As = stage_base + s * stage_bytes;
+        const uint32_t body_b = (uint32_t)(2 * nb * k.P) * 16;
+#pragma unroll
+        for (int kc = 0; kc < 4; ++kc) {
+          unsigned char* dst = slab + (size_t)kc * P.Lxs.rows * 16;
+          if (f0 == 0) bulk_s2g(dst, zrows, (uint32_t)lead * 16);
+          bulk_s2g(dst + (size_t)(lead + 2 * f0 * k.P) * 16, As + (size_t)kc * k.rows_alloc * 16, body_b);
+          if (f0 + nb == k.H) bulk_s2g(dst + (size_t)(P.Lxs.rows - trail) * 16, zrows, (uint32_t)trail * 16);
+        }
+        bulk_commit_group();
+        bulk_wait_group_read0();
+        mbar_arrive(&empty[s]);
+      }
+      bulk_wait_group0();  // the copies are in global memory before the kernel ends
     }
   }
 }
@@ -729,8 +674,20 @@ __global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const
   }
 }
 
-static size_t k1a_smem_bytes(const HeadGeom& g, int HW) {
-  return (size_t)K1A_ASTAGES * (4 * g.rows_alloc * 16 + HB_BSTAGE_BYTES) + (size_t)K1A_RSTAGES * 4 * HB_KSTAGE * HW * 2 + 128 + 1024;
+static size_t k1a_smem_bytes(const K1aGeom& k) {
+  return (size_t)K1A_STAGES * (4 * k.rows_alloc * 16 + HB_BSTAGE_BYTES) + (size_t)K1A_STAGES * 4 * HB_KSTAGE * k.box * 2 + 128 + K1A_ZROWS * 16;
+}
+
+// features [B][C][HW] bf16 viewed as [B * C][HW]; box = {box_px positions, 128 channels}, box_px <= HW (make_k1a_geom)
+static bool make_feat_tensor_map(CUtensorMap* tm, const void* feat, int B, int C, int HW, int box_px) {
+  const TensorMapEncodeFn encode = tensor_map_encoder();
+  if (!encode || (HW * 2) % 16 != 0 || (box_px * 2) % 16 != 0 || box_px > 256 || box_px > HW) return false;
+  const cuuint64_t gdim[2] = {(cuuint64_t)HW, (cuuint64_t)B * C};
+  const cuuint64_t gstride[1] = {(cuuint64_t)HW * 2};  // bytes, dim 1
+  const cuuint32_t box[2] = {(cuuint32_t)box_px, 4 * HB_KSTAGE};
+  const cuuint32_t estr[2] = {1, 1};
+  return encode(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(feat), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 static size_t k1b_smem_bytes(const HeadGeom& g) {
   return (size_t)4 * g.rows_alloc * 16 + HB_BSTAGE_BYTES + (2 * HB_CLS * 8 + 2 * HB_CLS + 8) * sizeof(float) + 64;
@@ -747,14 +704,16 @@ __host__ inline HeadGeom make_half_geom(int Hh, int Wi) {
 }  // namespace lpb
 
 // ---- which kernels serve a shape ---------------------------------------------------------------------------
-// fast path (k1a + k1b): two-deconv heads whose whole frame fits the shared-memory tiling above;
+// fast path (k1a + k1b): two-deconv heads whose bands fit the shared-memory tiling above;
 // generic path (head_rows_bf16.cu): everything else -- one-deconv heads, larger feature maps.
 static bool head_fast_path(int C, int H, int W, int c2, int max_smem) {
   using namespace lpb;
   if (c2 <= 0) return false;
-  if (!((W >= 7 || W == 4 || W == 6) && H * W <= 192 && W <= 31)) return false;  // W <= 31: the saved copy's lead rows fit the 1 KB zero source
-  const HeadGeom g1 = make_geom(2 * H, 2 * W), g2 = make_half_geom(2 * H, 4 * W);
-  return (int64_t)k1a_smem_bytes(g1, H * W) <= max_smem && (int64_t)k1b_smem_bytes(g2) <= max_smem;
+  // W <= 31: the saved copy's lead / trail rows fit the K1A_ZROWS zero source, and a band's staged rows one TMA box
+  if (!((W >= 7 || W == 4 || W == 6) && H * W <= 192 && W <= 31)) return false;
+  const HeadGeom g2 = make_half_geom(2 * H, 4 * W);
+  const K1aGeom k1 = make_k1a_geom(H, W);
+  return k1.G > 0 && (int64_t)k1a_smem_bytes(k1) <= max_smem && (int64_t)k1b_smem_bytes(g2) <= max_smem;
 }
 
 static int device_limits(int* max_smem, int* sms) {
@@ -824,6 +783,16 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
   int max_smem = 0, sms = 0;
   device_limits(&max_smem, &sms);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bool fast = head_fast_path(C, H, W, c2, max_smem);
+  const K1aGeom k1 = make_k1a_geom(H, W);
+  // k1a's feature tensor map, encoded before anything is queued, so a failure leaves the stream untouched.  The plan stays
+  // a function of the shape (CPU-only callers size buffers with it); every driver that runs sm_90a code has the encoder,
+  // so what can fail here is the caller's pointer (not 16-byte aligned).
+  CUtensorMap feat_map;
+  if (fast && !make_feat_tensor_map(&feat_map, features, B, C, H * W, k1.box)) {
+    set_error("head_fwd_bf16: cannot encode the feature tensor map (features must be 16-byte aligned)");
+    return LPB_ERR_INVALID;
+  }
   // decode hints are produced by the fused two-pass softmax of the banded kernel only (launch_convt_rows marks them invalid
   // on its other routes); the routes that never reach it do so here
   if (decode_hints && (!final_softmax || !g_tuning[LPB_TUNE_SOFTMAX_EPILOGUE_V2]))
@@ -835,12 +804,9 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
   __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + (size_t)nst * HB_BSTAGE_BYTES);
   __nv_bfloat16* mid = reinterpret_cast<__nv_bfloat16*>(ws + (size_t)(nst + 1) * HB_BSTAGE_BYTES);
   float* partials = reinterpret_cast<float*>(ws + (size_t)(nst + 1) * HB_BSTAGE_BYTES + (c2 > 0 ? (size_t)B * 4 * Lmid.rows * 16 : 0));
-  const bool fast = head_fast_path(C, H, W, c2, max_smem);
-  // k1a's block transposers write the saved copy's pad rows themselves when a thread's share fits its registers
-  const int xs_npad = Lxs.lead + (Lxs.rows - (Lxs.lead + Lxs.Hi * Lxs.Pp)) + Lxs.Hi;
-  const bool k1a_pads = fast && !g_tuning[LPB_TUNE_K1A_ROW_TRANSPOSER] && !g_tuning[LPB_TUNE_K1A_BULK_XS] && 4 * xs_npad <= K1A_MAXPAD * 32 * K1A_TW;
   {
-    // one launch: both operand packs + the pad rows of the fresh row-layout buffers
+    // one launch: both operand packs + the pad rows of the fresh row-layout buffers (k1a writes every row of the saved
+    // copy itself; the banded path's shuffle kernel writes its own pads)
     PrepJobs jobs{};
     jobs.fpack[0] = {w1, nullptr, C / 4, c1, nst, wp1};
     // layer 2: bias rides on the constant-one channel c1 of the mid activations (only needed without softmax:
@@ -849,8 +815,6 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
       jobs.fpack[1] = {w2, final_softmax ? nullptr : b2, c1, c2, 1, wp2};
       jobs.pads[0] = {mid, Lmid, (long long)B * 4};
     }
-    // (the block transposer of k1a writes the saved copy's pads itself; the row-form variant does not)
-    if (fast && saved_xs && !g_tuning[LPB_TUNE_K1A_BULK_XS] && !k1a_pads) jobs.pads[1] = {static_cast<__nv_bfloat16*>(saved_xs), Lxs, (long long)B * (C / 32)};  // (the banded path's shuffle kernel writes its own pads)
     launch_head_prep(jobs, s);
   }
   if (!fast) {
@@ -899,37 +863,30 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
     LPB_CUDA(cudaGetLastError());
     return LPB_OK;
   }
-  const HeadGeom g1 = make_geom(2 * H, 2 * W), g2 = make_half_geom(2 * H, 4 * W);  // layer 2: 4H rows in two halves
-  const size_t s1 = k1a_smem_bytes(g1, H * W), s2 = k1b_smem_bytes(g2);
-  K1aParams pa;
-  pa.feat = static_cast<const __nv_bfloat16*>(features);
-  pa.wpk = wp1;
-  pa.bias = b1;
-  pa.mid = mid;
-  pa.xs = static_cast<__nv_bfloat16*>(saved_xs);
-  pa.Lmid = Lmid;
-  pa.Lxs = Lxs;
-  pa.B = B;
-  pa.C = C;
-  pa.HW = H * W;
-  pa.W = W;
-  pa.c1 = c1;
-  pa.nstages = nst;
-  pa.row_transposer = g_tuning[LPB_TUNE_K1A_ROW_TRANSPOSER];
-  pa.backoff = g_tuning[LPB_TUNE_WAIT_BACKOFF];
-  pa.xs_bulk = g_tuning[LPB_TUNE_K1A_BULK_XS];
-  pa.xs_copy = (g_tuning[LPB_TUNE_K1A_XS_COPY] && !pa.row_transposer && !pa.xs_bulk) ? 1 : 0;
-  pa.xs_pads = k1a_pads ? 1 : 0;
-  pa.g = g1;
-  pa.ntg = (g1.tiles + K1A_TPG - 1) / K1A_TPG;
+  const HeadGeom g2 = make_half_geom(2 * H, 4 * W);  // layer 2: 4H rows in two halves
+  const size_t s1 = k1a_smem_bytes(k1), s2 = k1b_smem_bytes(g2);
   {
-    // compile-time form of the saved copy (see the kernel): none / run-time forms / copy-out
-    if (pa.xs_copy && Lxs.lead > 32 * K1A_TW) pa.xs_copy = 0;
-    const int form = (!pa.xs || pa.row_transposer || pa.xs_bulk) ? (pa.xs || pa.row_transposer ? 1 : 0) : (g_tuning[LPB_TUNE_K1A_XS_COPY] == 2 ? 3 : (pa.xs_copy ? 2 : 1));
-    auto kern = form == 0 ? k1a_shuffle_convt_kernel<0> : (form == 1 ? k1a_shuffle_convt_kernel<1> : (form == 2 ? k1a_shuffle_convt_kernel<2> : k1a_shuffle_convt_kernel<3>));
+    K1aParams pa{};
+    pa.feat = feat_map;
+    pa.wpk = wp1;
+    pa.bias = b1;
+    pa.mid = mid;
+    pa.xs = static_cast<__nv_bfloat16*>(saved_xs);
+    pa.Lmid = Lmid;
+    pa.Lxs = Lxs;
+    pa.B = B;
+    pa.C = C;
+    pa.c1 = c1;
+    pa.nstages = nst;
+    pa.k = k1;
+    auto kern = saved_xs ? k1a_shuffle_convt_kernel<1> : k1a_shuffle_convt_kernel<0>;
     LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s1));
-    const int items = B * pa.ntg;
-    kern<<<items < sms ? items : sms, K1A_THREADS + (form == 3 ? 32 : 0), s1, s>>>(pa);
+    // items are dealt round-robin (item = blockIdx.x + k gridDim.x), so with G = 2 and an even grid (132 SMs) a CTA always
+    // takes the same band, and likewise with G = 3 and a grid divisible by 3: bands of equal size keep the CTAs even.
+    // Unequal bands (H % G != 0, e.g. 16 x 12 features: 6 / 5 / 5 rows) leave the CTAs of the larger bands one row pair
+    // more per item.
+    const int items = B * k1.G;
+    kern<<<items < sms ? items : sms, K1A_THREADS, s1, s>>>(pa);
   }
   if (g_tuning[LPB_TUNE_SOFTMAX_EPILOGUE_V2]) {
     // layer 2 on the banded kernel (head_rows_bf16.cu): same GEMM, leaner softmax epilogue

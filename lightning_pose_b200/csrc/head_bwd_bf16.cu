@@ -15,9 +15,9 @@
 #include "../../include/lpb200.h"
 #include "head_prep.cuh"
 #include <cstring>
-#include <cuda.h>  // CUtensorMap (the encoder is fetched through cudaGetDriverEntryPoint: no libcuda link)
 
 #include "lpb_common.cuh"
+#include "tensor_map.cuh"
 #include "row_layout.cuh"
 #include "mma_sm90.cuh"
 
@@ -1028,20 +1028,8 @@ static int b3a_band_rows(int Hi1, int Wi1) {
 }
 
 // d features [B][4*C4][HW] bf16 viewed as [b][c'][pl][px]; box = {box_px pixels, one pl, 128 c', one frame}.
-// The encoder is a driver entry point; it is looked up once (no link-time dependency on libcuda).
 static bool make_dfeat_tensor_map(CUtensorMap* tm, void* dfeat, int B, int C4, int HW, int box_px) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                               const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = nullptr;
-  static bool looked_up = false;
-  if (!looked_up) {
-    looked_up = true;
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      encode = reinterpret_cast<EncodeFn>(fn);
-    (void)cudaGetLastError();
-  }
+  const TensorMapEncodeFn encode = tensor_map_encoder();
   if (!encode || (HW * 2) % 16 != 0 || (box_px * 2) % 16 != 0 || box_px > 256) return false;
   const cuuint64_t gdim[4] = {(cuuint64_t)HW, 4, (cuuint64_t)C4, (cuuint64_t)B};
   const cuuint64_t gstride[3] = {(cuuint64_t)HW * 2, (cuuint64_t)HW * 2 * 4, (cuuint64_t)HW * 2 * 4 * (cuuint64_t)C4};  // bytes, dims 1..3

@@ -145,6 +145,20 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
       : "memory");
 }
 
+// 2-D tiled TMA load of box {x0.., x1..} of tensor map `tm` (a __grid_constant__ CUtensorMap) into shared memory
+// (128-B aligned); elements outside the tensor land as zeros
+__device__ __forceinline__ void tma_load_2d(void* dst_smem, const void* tm, int x0, int x1, uint64_t* bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(smem_u32(dst_smem)),
+               "l"(tm), "r"(x0), "r"(x1), "r"(smem_u32(bar))
+               : "memory");
+}
+
+// warpgroup register budget (sm_90a): every warp of the warpgroup executes the same one
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // shared -> global bulk copy (TMA store, bulk-group completion); bytes % 16 == 0, both addresses 16-B aligned
 __device__ __forceinline__ void bulk_s2g(void* dst_gmem, const void* src_smem, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes) : "memory");

@@ -123,22 +123,29 @@ __device__ __forceinline__ void kstep_mn(float (&acc)[MT][NT][4], uint32_t a, ui
   }
 }
 
-// n8 tile `nt` of a 32-row block -> v[0..7] = D(lane, 8 nt + 0..7)
-template <int NT>
-__device__ __forceinline__ void rows8(const float (&acc)[2][NT][4], int nt, float* v, int lane) {
-  const int g = lane & 7, sel = lane >> 3;  // sel = 2 mt + (row >= 8 within the m16 tile)
+// n8 tile `nt` of the 32 rows of m16 tiles M0, M0 + 1 -> v[0..7] = D(16 M0 + lane, 8 nt + 0..7).  A lone last tile
+// (M0 + 1 == MT) fills lanes 16..31 with copies of its rows, which the caller ignores.
+template <int M0, int MT, int NT>
+__device__ __forceinline__ void rows8_at(const float (&acc)[MT][NT][4], int nt, float* v, int lane) {
+  constexpr int M1 = M0 + 1 < MT ? M0 + 1 : M0;
+  const int g = lane & 7, sel = lane >> 3;  // sel = 2 (tile - M0) + (row >= 8 within the m16 tile)
 #pragma unroll
   for (int t = 0; t < 4; ++t) {
     const int src = g * 4 + t;
 #pragma unroll
     for (int p = 0; p < 2; ++p) {
-      const float x0 = __shfl_sync(0xffffffffu, acc[0][nt][p], src);
-      const float x1 = __shfl_sync(0xffffffffu, acc[0][nt][2 + p], src);
-      const float x2 = __shfl_sync(0xffffffffu, acc[1][nt][p], src);
-      const float x3 = __shfl_sync(0xffffffffu, acc[1][nt][2 + p], src);
+      const float x0 = __shfl_sync(0xffffffffu, acc[M0][nt][p], src);
+      const float x1 = __shfl_sync(0xffffffffu, acc[M0][nt][2 + p], src);
+      const float x2 = __shfl_sync(0xffffffffu, acc[M1][nt][p], src);
+      const float x3 = __shfl_sync(0xffffffffu, acc[M1][nt][2 + p], src);
       v[2 * t + p] = sel == 0 ? x0 : (sel == 1 ? x1 : (sel == 2 ? x2 : x3));
     }
   }
+}
+// n8 tile `nt` of a 32-row block -> v[0..7] = D(lane, 8 nt + 0..7)
+template <int NT>
+__device__ __forceinline__ void rows8(const float (&acc)[2][NT][4], int nt, float* v, int lane) {
+  rows8_at<0>(acc, nt, v, lane);
 }
 
 }  // namespace mma

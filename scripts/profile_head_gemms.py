@@ -41,13 +41,15 @@ def nz_tiles(sh: int, width: int, lo: int = 0, hi: int = NCLS * CLS) -> int:
 
 
 def k1a_flops(frames: int, cin: int, h: int, w: int) -> tuple[float, float]:
-    """k1a: per active 128-row M-tile, 4 warps x 2 m16 x 10 n8 x 4 shifts x 2 k16 per 32-channel stage"""
-    hi, wi = 2 * h, 2 * w
-    tiles = (hi * (wi + 1) + 127) // 128
-    per_tile_stage = 4 * 2 * 2  # warps x m16 x k16
+    """k1a: per (frame, band) item, the band's m16 tiles x 10 n8 x 4 shifts x 2 k16 per 32-channel stage; the bands are as
+    head_bf16.cu's make_k1a_geom cuts them (the fewest whose largest band fits 8 warps x 3 m16 tiles = 384 raster rows)"""
+    p = 2 * w + 1
+    g = next(g for g in range(1, h + 1) if 2 * -(-h // g) * p <= 384)
+    m16 = sum(-(-2 * (h // g + (i < h % g)) * p // 16) for i in range(g))  # m16 tiles per frame
+    per_stage = m16 * 2  # x k16
     nst = cin // 32
-    all_t = frames * tiles * nst * per_tile_stage * 4 * 10
-    nonzero = frames * tiles * nst * per_tile_stage * sum(nz_tiles(sh, 8) for sh in range(4))
+    all_t = frames * nst * per_stage * 4 * 10
+    nonzero = frames * nst * per_stage * sum(nz_tiles(sh, 8) for sh in range(4))
     return all_t * MMA_FLOP, nonzero * MMA_FLOP
 
 
