@@ -38,25 +38,9 @@ int lpb_version(void);                /* e.g. 100 = 0.1.0 */
 const char* lpb_last_error(void);     /* message of the last failing call on this thread */
 const char* lpb_build_arch(void);     /* "sm_90a" */
 
-/* kernel-variant switches: a bring-up / profiling aid (A/B two implementations of the same stage on the same inputs);
- * every variant computes the same results.  lpb_get_tuning returns -1 for an unknown key. */
-#define LPB_TUNE_K1A_ROW_TRANSPOSER 0   /* no effect in this build (accepted for compatibility): k1a has one operand transposer */
-#define LPB_TUNE_SOFTMAX_EPILOGUE_V2 1  /* 1 (default): softmax epilogue with one vote per tile and hoisted addressing */
-#define LPB_TUNE_WAIT_BACKOFF 2         /* 1 (default): idle warps back off between mbarrier polls */
-#define LPB_TUNE_DECODE_RING 3          /* 1: soft-argmax planes staged once in shared memory by a bulk-copy ring; 0 (default): warp per plane from global */
-#define LPB_TUNE_K1A_BULK_XS 4          /* no effect in this build (accepted for compatibility): k1a has one saved-copy form */
-#define LPB_TUNE_DECODE_L2_HINTS 5      /* 1 (default): L2 evict_last / evict_first hints on the decode's two sweeps of a plane */
-#define LPB_TUNE_B3A_PREFETCH 6         /* 1 (default): b3a epilogue issues the next item's accumulator blocks before storing the current one */
-#define LPB_TUNE_SOFTMAX_SPLIT 7         /* 1 (default): plane softmax as two launches parallel over (frame, band) when there are fewer frames than SMs, else one per-frame two-pass kernel; 0: never split; 2: always */
-#define LPB_TUNE_DECODE_WARP_CTAS 8     /* > 0: resident CTAs per SM of the warp-per-plane decode are capped (fewer planes in flight than L2 holds); 0: no cap */
-#define LPB_TUNE_DECODE_REVERSE 9       /* 1: the decode walks the planes last-to-first (the producer's most recent writes are still in L2) */
-#define LPB_TUNE_B3A_TMA_STORE 10       /* 1 (default): b3a stages d features in shared memory and a TMA tensor store scatters them to NCHW; 0: direct 16-byte stores */
-#define LPB_TUNE_WGRAD_SWAP 11          /* no effect in this build (accepted for compatibility): the weight gradient has one form */
-#define LPB_TUNE_G2_PATCH 12            /* 1 (default): decode windows enter the gradient rows in a patch pass (one warp per plane) after a look-up-free streaming pass; 0: look-ups fused into the streaming pass */
-#define LPB_TUNE_MMA_TILE_INNER 13      /* no effect in this build (accepted for compatibility): k1a has one MMA order */
-#define LPB_TUNE_DECODE_HINTS 14        /* 1: the fused two-pass softmax emits per-plane decode hints (arg max + largest value outside its 32x32 box) and the decode skips its plane sweeps when they allow; 0 (default): hints never produced (measured: what the decode saves, the issue-bound softmax epilogue pays) */
-#define LPB_TUNE_K1A_XS_COPY 15         /* no effect in this build (accepted for compatibility): each k1a item's store warp sends its rows of the finished operand stage to the saved copy with TMA bulk stores */
-#define LPB_TUNE_COUNT 16
+/* tuning switch: which form of the head's final plane softmax runs (both compute the same results).  lpb_set_tuning
+ * returns LPB_ERR_INVALID and lpb_get_tuning -1 for any other key. */
+#define LPB_TUNE_SOFTMAX_SPLIT 7  /* 1 (default): plane softmax as two launches parallel over (frame, band) when there are fewer frames than SMs, else one per-frame two-pass kernel; 0: never split; 2: always */
 int lpb_set_tuning(int key, int value);
 int lpb_get_tuning(int key);
 
@@ -76,13 +60,6 @@ int lpb_get_tuning(int key);
 int lpb_decode_prepare(int h, int w, int ds);
 int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
                    float* xy, float* conf, float* stats, void* stream);
-/* lpb_decode_fwd with optional per-plane hints (16 bytes per plane: int32 arg-max row, int32 arg-max column, float32 bits of
- * the largest value outside the 32 x 32 box [row - 16, row + 15] x [col - 16, col + 15], int32 valid) as written by
- * lpb_head_fwd_bf16_hinted for the SAME heatmaps: planes whose outside bound is below the pruning threshold are decoded
- * from the window around the arg max alone (no sweep of the plane; identical candidate hull, identical results); planes
- * with valid = 0 and hints = NULL take the plain route.  No reference counterpart: the reference materialises the field. */
-int lpb_decode_fwd_hinted(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
-                          float* xy, float* conf, float* stats, const void* hints, void* stream);
 /* d loss / d heatmaps given d loss / d xy (confidence carries no gradient: it only feeds `<`
  * comparisons, lightning_pose/losses/losses.py:636). grad_heatmaps [n_planes,h,w] is overwritten. */
 int lpb_decode_bwd(const float* heatmaps, const float* stats, const float* grad_xy, int64_t n_planes,
@@ -168,11 +145,6 @@ int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, si
 int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
                       const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
                       void* workspace, void* stream);
-/* lpb_head_fwd_bf16 that also fills `decode_hints` ([B * K] x 16 bytes, see lpb_decode_fwd_hinted; NULL = none) when the
- * head ends in the plane softmax: the softmax pass knows each plane's maximum and what lies outside the box around it. */
-int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
-                             const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
-                             void* workspace, void* decode_hints, void* stream);
 /* saved_xs: on the fast path NULL for inference; for training (and always on the banded path) a device buffer of lpb_head_bf16_saved_bytes() bytes; it
  * receives the pixel-shuffled features in the padded row layout the weight-gradient GEMM reads, and must stay
  * alive (together with `workspace`, which holds the activations between the two deconvs) until

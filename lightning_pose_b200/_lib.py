@@ -40,7 +40,6 @@ SIGNATURES = {
     "lpb_get_tuning": (C.c_int, [_I]),
     "lpb_decode_prepare": (C.c_int, [_I, _I, _I]),
     "lpb_decode_fwd": (C.c_int, [_P, _L, _I, _I, _I, _F, _P, _P, _P, _P]),
-    "lpb_decode_fwd_hinted": (C.c_int, [_P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
     "lpb_decode_bwd": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _F, _P, _P]),
     "lpb_decode_bwd_windows": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
     "lpb_upsample2x": (C.c_int, [_P, _L, _I, _I, _P, _P]),
@@ -57,7 +56,6 @@ SIGNATURES = {
     "lpb_head_bf16_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bf16_saved_bytes": (C.c_int, [_I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_fwd_bf16": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
-    "lpb_head_fwd_bf16_hinted": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "lpb_head_bwd_bf16_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bwd_bf16": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_remap_keypoints": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
@@ -111,7 +109,7 @@ def _load() -> C.CDLL:
 
 lib = _load()
 
-# LPB_TUNE="key=value,..." selects kernel variants (include/lpb200.h LPB_TUNE_*): a profiling / bring-up aid
+# LPB_TUNE="key=value,..." sets tuning switches (include/lpb200.h LPB_TUNE_*): a profiling / bring-up aid
 for _kv in filter(None, os.environ.get("LPB_TUNE", "").split(",")):
     _k, _v = _kv.split("=")
     if lib.lpb_set_tuning(int(_k), int(_v)) != 0:

@@ -40,10 +40,6 @@ struct DecodeParams {
   int h, w, pitch, padl, bulk;
   int64_t n_planes;
   float T, lip, offset;
-  int l2_hints;       // warp kernel: L2 eviction-priority hints on its two sweeps (LPB_TUNE_DECODE_L2_HINTS)
-  int reverse;        // warp kernel: planes are taken last-to-first (LPB_TUNE_DECODE_REVERSE)
-  const int4* hints;  // optional per-plane hints from the head's softmax pass (head_rows.cuh): {arg-max row, col, bits(largest
-                      // value outside the 32 x 32 box around it), valid} -- the warp kernel then needs no sweep of peaked planes
   const int* queue;   // CTA kernel, queue mode: {count, plane ids ...} left over by the warp-per-plane kernel
   int* qcounter;      // [n_planes] arrival counters (zeroed) and
   float* qscratch;    // [n_planes][DEC_MAX_PARTS][4] partial softmax states of a plane split over several CTAs
@@ -620,10 +616,6 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
 // and run by the CTA kernel in queue mode, so every plane produces the same outputs either way.
 constexpr int DECW_WIN = 32, DECW_WP = 33;
 
-__device__ __forceinline__ void tc_free_slot(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 template <int DS>
 __device__ float eval_point_win(const float* tile, int r0w, int c0w, const float* __restrict__ tabH,
                                 const float* __restrict__ tabW, int i, int j) {
@@ -641,37 +633,30 @@ __device__ float eval_point_win(const float* tile, int r0w, int c0w, const float
   return acc;
 }
 
-template <int DS, bool STAGED>
 __device__ __forceinline__ void load_window(float* tile, const float* __restrict__ src, int h, int w, int r0w, int c0w, int lane) {
   const int x = c0w + lane;
   const bool xin = x >= 0 && x < w;
 #pragma unroll 8
   for (int r = 0; r < DECW_WIN; ++r) {
     const int y = r0w + r;
-    tile[r * DECW_WP + lane] = (xin && y >= 0 && y < h) ? (STAGED ? src[(size_t)y * w + x] : __ldg(src + (size_t)y * w + x)) : 0.f;
+    tile[r * DECW_WP + lane] = (xin && y >= 0 && y < h) ? __ldg(src + (size_t)y * w + x) : 0.f;
   }
 }
 
-// One plane, one warp.  STAGED = false: `src` is the plane in global memory (read-only path, three sweeps of it);
-// STAGED = true: `src` is the plane already staged in shared memory by the ring kernel below (one HBM read per plane).
-template <int DS, bool STAGED>
+// One plane, one warp; `src` is the plane in global memory (read-only path, three sweeps of it).
+template <int DS>
 __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, const float* __restrict__ src, float* tile,
                                   int* __restrict__ queue, int lane) {
   constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1;
   const int h = P.h, w = P.w, w4 = w >> 2, n4 = h * w4;
   const float4* __restrict__ src4 = reinterpret_cast<const float4*>(src);
-  // L2 residency hints (global form): the arg-max sweep asks L2 to KEEP the plane (evict_last), the hull sweep that
-  // follows re-reads it from L2 and releases it (evict_first) -- without them the second sweep misses L2 (measured
-  // DRAM traffic 2.05x the plane bytes: the kernel ran at ~80 % of HBM peak on twice the necessary bytes)
-  uint64_t pol_keep = 0, pol_drop = 0;
-  if (!STAGED && P.l2_hints) {
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_keep));
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_drop));
-  }
-  auto ld4 = [&](int idx) -> float4 { return STAGED ? src4[idx] : __ldg(src4 + idx); };
+  // L2 residency hints: the arg-max sweep asks L2 to KEEP the plane (evict_last), the hull sweep that follows re-reads it
+  // from L2 and releases it (evict_first) -- without them the second sweep misses L2 (measured DRAM traffic 2.05x the
+  // plane bytes: the kernel ran at ~80 % of HBM peak on twice the necessary bytes)
+  uint64_t pol_keep, pol_drop;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_keep));
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_drop));
   auto ld4h = [&](int idx, uint64_t pol) -> float4 {
-    if (STAGED) return src4[idx];
-    if (!P.l2_hints) return __ldg(src4 + idx);
     float4 v;
     asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(src4 + idx), "l"(pol));
     return v;
@@ -680,27 +665,11 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
     if (lane == 0) queue[1 + atomicAdd(queue, 1)] = (int)plane;
   };
 
-  // ---- hinted form: the producer of the plane (the head's softmax pass) already knows where its maximum is and how large
-  // the plane is OUTSIDE the 32 x 32 box around it; when that bound is below the candidate threshold, everything that can
-  // carry weight lies inside the first window and neither sweep of the plane is needed (same hull, same results)
-  bool hinted = false;
-  float hout = 0.f;
-  int besta = 0, bestb = 0;
-  if (!STAGED && P.hints) {
-    const int4 hv = __ldg(P.hints + plane);
-    if (hv.w == 1 && (unsigned)hv.x < (unsigned)h && (unsigned)hv.y < (unsigned)w) {
-      hinted = true;
-      besta = hv.x;
-      bestb = hv.y;
-      hout = __int_as_float(hv.z);
-    }
-  }
   // ---- pass 1: arg max of |h| ----------------------------------------------------------------------------
   float best = -1.f;
   int bidx = 0;
-  if (hinted) best = fabsf(__ldg(src + (size_t)besta * w + bestb));
 #pragma unroll 8
-  for (int idx = hinted ? n4 : lane; idx < n4; idx += 32) {
+  for (int idx = lane; idx < n4; idx += 32) {
     const float4 x = ld4h(idx, pol_keep);
     const float m4 = fmaxf(fmaxf(fabsf(x.x), fabsf(x.y)), fmaxf(fabsf(x.z), fabsf(x.w)));
     if (m4 > best) {
@@ -721,15 +690,15 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
     to_queue();
     return;
   }
-  if (!hinted) {
-    besta = bidx / w4;
-    bestb = (bidx - besta * w4) * 4;
-    const float4 x = ld4(bidx);
+  const int besta = bidx / w4;
+  int bestb = (bidx - besta * w4) * 4;
+  {
+    const float4 x = __ldg(src4 + bidx);
     bestb += (fabsf(x.x) == best) ? 0 : ((fabsf(x.y) == best) ? 1 : ((fabsf(x.z) == best) ? 2 : 3));
   }
   // ---- lower bound of the field maximum: exact values on the arg max's F x F block ---------------------
   int r0w = besta - DECW_WIN / 2, c0w = bestb - DECW_WIN / 2;
-  load_window<DS, STAGED>(tile, src, h, w, r0w, c0w, lane);
+  load_window(tile, src, h, w, r0w, c0w, lane);
   __syncwarp();
   float lb = -3.0e38f;
   if (lane < F * F) lb = eval_point_win<DS>(tile, r0w, c0w, P.tabH, P.tabW, besta * F + lane / F, bestb * F + lane % F);
@@ -739,22 +708,7 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
 
   // ---- pass 2: hull of the candidates (|h| >= theta), 4-column granularity like the CTA kernel -----------
   int amin = h, amax = -1, bmin = w, bmax = -1;
-  if (hinted && hout < theta) {
-    // candidates only inside the first window (still in `tile`): lane = window row, 4-column granularity as below
-    const int y = r0w + lane;
-    if (y >= 0 && y < h) {
-#pragma unroll 8
-      for (int cc = 0; cc < DECW_WIN; ++cc) {
-        const int x = c0w + cc;
-        if (x >= 0 && x < w && fabsf(tile[lane * DECW_WP + cc]) >= theta) {
-          amin = min(amin, y);
-          amax = max(amax, y);
-          bmin = min(bmin, x & ~3);
-          bmax = max(bmax, min((x & ~3) + 3, w - 1));
-        }
-      }
-    }
-  } else {
+  {
     int a = 0, g = lane;  // idx = a * w4 + g
     while (g >= w4) {
       g -= w4;
@@ -792,7 +746,7 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
   r0w = A0 - R - 1;
   c0w = B0 - R - 1;
   __syncwarp();
-  load_window<DS, STAGED>(tile, src, h, w, r0w, c0w, lane);
+  load_window(tile, src, h, w, r0w, c0w, lane);
   __syncwarp();
 
   // ---- rows that can carry weight (tap-decay bound, see decode_bwd_window_kernel); lane r owns window row r ----
@@ -901,66 +855,9 @@ template <int DS>
 __global__ void __launch_bounds__(128) decode_fwd_warp_kernel(const __grid_constant__ DecodeParams<DS> P, int* __restrict__ queue) {
   __shared__ float tile_s[4][DECW_WIN * DECW_WP];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  long long plane = (long long)blockIdx.x * 4 + warp;
+  const int plane = blockIdx.x * 4 + warp;  // n_planes < 2^31 (lpb_decode_fwd); the queue holds int plane ids as well
   if (plane >= P.n_planes) return;
-  if (P.reverse) plane = P.n_planes - 1 - plane;
-  decode_plane_warp<DS, false>(P, plane, P.heat + (size_t)plane * P.h * P.w, tile_s[warp], queue, lane);
-}
-
-// ---- ring form: every plane crosses HBM once -----------------------------------------------------------------
-// Persistent CTAs.  One producer thread streams whole planes (contiguous h*w*4 bytes = ONE bulk copy each) into a ring
-// of shared-memory slots; DECR_WARPS consumer warps each take the next filled slot and run the same per-plane code as
-// above on the staged copy -- the arg-max sweep, the candidate-hull sweep and both window loads read shared memory, so
-// DRAM traffic is the algorithmic 4*h*w bytes per plane (the warp kernel above reads each plane twice from
-// global memory: 2.05x measured).  Consumer warps never synchronise with each other, only with the producer through
-// the slot's full / empty mbarriers.
-constexpr int DECR_WARPS = 4;
-
-template <int DS>
-__global__ void __launch_bounds__(32 * (DECR_WARPS + 1), 1) decode_fwd_ring_kernel(const __grid_constant__ DecodeParams<DS> P, int* __restrict__ queue,
-                                                                                    int nslots) {
-  extern __shared__ __align__(128) unsigned char dsm[];
-  const int plane_bytes = P.h * P.w * 4;
-  float* tiles = reinterpret_cast<float*>(dsm);                                   // [DECR_WARPS][WIN * WP]
-  unsigned char* slots = dsm + ((DECR_WARPS * DECW_WIN * DECW_WP * 4 + 127) & ~127);  // [nslots][plane_bytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(slots + (size_t)nslots * plane_bytes);  // full[nslots], empty[nslots]
-  uint64_t* full = bars;
-  uint64_t* empty = bars + nslots;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < nslots; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  // planes of this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...
-  const long long first = blockIdx.x, stride = gridDim.x;
-  const long long mine = first < P.n_planes ? (P.n_planes - first + stride - 1) / stride : 0;
-  if (warp == DECR_WARPS) {
-    if (lane == 0) {
-      for (long long i = 0; i < mine; ++i) {
-        const int sl = (int)(i % nslots);
-        mbar_wait(&empty[sl], (uint32_t)(((i / nslots) & 1) ^ 1));
-        mbar_expect_tx(&full[sl], (uint32_t)plane_bytes);
-        bulk_g2s(slots + (size_t)sl * plane_bytes, P.heat + (size_t)(first + i * stride) * P.h * P.w, (uint32_t)plane_bytes, &full[sl]);
-      }
-    }
-    return;
-  }
-  // a consumer may wait for phase p of a slot only once phase p - 1 has completed (a parity wait cannot tell phases two
-  // apart): with static assignment that holds iff the number of consumers does not exceed the number of slots
-  const int ncons = nslots < DECR_WARPS ? nslots : DECR_WARPS;
-  if (warp >= ncons) return;
-  for (long long i = warp; i < mine; i += ncons) {
-    const int sl = (int)(i % nslots);
-    mbar_wait(&full[sl], (uint32_t)((i / nslots) & 1));
-    decode_plane_warp<DS, true>(P, first + i * stride, reinterpret_cast<const float*>(slots + (size_t)sl * plane_bytes),
-                                tiles + warp * DECW_WIN * DECW_WP, queue, lane);
-    __syncwarp();
-    if (lane == 0) tc_free_slot(&empty[sl]);
-  }
+  decode_plane_warp<DS>(P, plane, P.heat + (size_t)plane * P.h * P.w, tile_s[warp], queue, lane);
 }
 
 // d loss / d h = U_H^T G U_W with G[i,j] = T * p[i,j] * ((j - xhat) gx + (i - yhat) gy), p the
@@ -1363,7 +1260,7 @@ __global__ void __launch_bounds__(DEC_THREADS) upsample2x_kernel(const float* __
 // ------------------------------------------------------------------------------------------------
 template <int DS>
 static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, float T, float* xy, float* conf,
-                             float* stats, cudaStream_t stream, const void* hints = nullptr) {
+                             float* stats, cudaStream_t stream) {
   using G = UpsampleGeom<DS>;
   const DeviceTable* th = get_device_table(h, DS);
   const DeviceTable* tw = get_device_table(w, DS);
@@ -1404,9 +1301,6 @@ static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, 
   P.queue = nullptr;
   P.qcounter = nullptr;
   P.qscratch = nullptr;
-  P.hints = static_cast<const int4*>(hints);
-  P.l2_hints = g_tuning[LPB_TUNE_DECODE_L2_HINTS];
-  P.reverse = g_tuning[LPB_TUNE_DECODE_REVERSE];
   P.lipw = tw->host.lip;
   for (int t = 0; t < G::W; ++t) {
     float m = 0.f;
@@ -1435,26 +1329,7 @@ static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, 
     }
     LPB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&queue), sizeof(int) * qints, stream));
     LPB_CUDA(cudaMemsetAsync(queue, 0, sizeof(int) * (size_t)(2 * n_planes + 1), stream));
-    // ring form when at least two planes (+ the per-warp windows) fit in shared memory: one HBM read per plane
-    const size_t plane_bytes = (size_t)h * w * 4, tiles_b = (size_t)((DECR_WARPS * DECW_WIN * DECW_WP * 4 + 127) & ~127);
-    int nslots = (int)(((size_t)max_smem - tiles_b - 256) / plane_bytes);
-    if (nslots > 8) nslots = 8;
-    if (g_tuning[LPB_TUNE_DECODE_RING] && nslots >= 2 && plane_bytes % 16 == 0) {
-      const size_t rsm = tiles_b + (size_t)nslots * plane_bytes + (size_t)2 * nslots * 8 + 64;
-      LPB_CUDA(cudaFuncSetAttribute(decode_fwd_ring_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsm));
-      decode_fwd_ring_kernel<DS><<<(unsigned)(n_planes < sms ? n_planes : sms), 32 * (DECR_WARPS + 1), rsm, stream>>>(P, queue, nslots);
-    } else {
-      // optional occupancy cap: unused dynamic shared memory keeps the resident planes (4 per CTA) within L2's reach
-      size_t pad = 0;
-      const int cap = g_tuning[LPB_TUNE_DECODE_WARP_CTAS];
-      if (cap > 0) {
-        const size_t per_cta = ((size_t)max_smem + 1024) / (size_t)(cap + 1) + 1024, stat = sizeof(float) * 4 * DECW_WIN * DECW_WP + 1024;
-        pad = per_cta > stat ? per_cta - stat : 0;
-        if (pad + stat > (size_t)max_smem) pad = (size_t)max_smem - stat;
-        LPB_CUDA(cudaFuncSetAttribute(decode_fwd_warp_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pad));
-      }
-      decode_fwd_warp_kernel<DS><<<(unsigned)((n_planes + 3) / 4), 128, pad, stream>>>(P, queue);
-    }
+    decode_fwd_warp_kernel<DS><<<(unsigned)((n_planes + 3) / 4), 128, 0, stream>>>(P, queue);
     P.queue = queue;
     P.qcounter = queue + 1 + n_planes;
     P.qscratch = reinterpret_cast<float*>(queue + 1 + 2 * n_planes);
@@ -1535,11 +1410,6 @@ extern "C" int lpb_decode_prepare(int h, int w, int ds) {
 
 extern "C" int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
                               float* xy, float* conf, float* stats, void* stream) {
-  return lpb_decode_fwd_hinted(heatmaps, n_planes, h, w, ds, temperature, xy, conf, stats, nullptr, stream);
-}
-
-extern "C" int lpb_decode_fwd_hinted(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
-                                     float* xy, float* conf, float* stats, const void* hints, void* stream) {
   using namespace lpb;
   LPB_REQUIRE(heatmaps && xy && conf, "decode_fwd: null pointer");
   LPB_REQUIRE(h >= 1 && w >= 1 && ds >= 1 && ds <= 3, "decode_fwd: bad shape h=%d w=%d ds=%d", h, w, ds);
@@ -1551,9 +1421,9 @@ extern "C" int lpb_decode_fwd_hinted(const float* heatmaps, int64_t n_planes, in
   if (n_planes == 0) return LPB_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   switch (ds) {
-    case 1: return launch_decode_fwd<1>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s, hints);
-    case 2: return launch_decode_fwd<2>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s, hints);
-    default: return launch_decode_fwd<3>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s, hints);
+    case 1: return launch_decode_fwd<1>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s);
+    case 2: return launch_decode_fwd<2>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s);
+    default: return launch_decode_fwd<3>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s);
   }
 }
 

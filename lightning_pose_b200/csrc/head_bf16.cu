@@ -15,8 +15,7 @@
 //
 //   k1a: features (NCHW bf16) --[PixelShuffle folded into a transposing producer]--> smem A stages
 //        --mma.sync--> registers --epilogue(+bias, ->bf16)--> mid activations in the A layout (global)
-//   k1b: mid (A layout, TMA bulk rows) --mma.sync--> registers --epilogue--> two-pass plane softmax
-//        (pass 0: online max/sum, pass 1: recompute the cheap K=32 GEMM and write normalised fp32)
+//   layer 2: mid activations --banded kernel (head_rows_bf16.cu)--> planes or two-pass plane softmax
 #include <cuda_bf16.h>
 
 #include <cstdint>
@@ -36,25 +35,6 @@ constexpr int HB_NCOLS = 80;         // 4 classes x 20 (>= 17 keypoints), multip
 constexpr int HB_CLS = 20;
 constexpr int HB_KSTAGE = 32;        // channels per pipeline stage (4 K-chunks of 8)
 constexpr int HB_BSTAGE_BYTES = 4 * 4 * HB_NCOLS * 16;  // [shift][kchunk][80 rows][16 B]
-
-struct HeadGeom {
-  int Hi, Wi;       // conv input spatial size (after PixelShuffle for layer 1)
-  int P;            // row pitch = Wi + 1 (zero column)
-  int rows;         // Hi * P
-  int tiles;        // ceil(rows / 128)
-  int rows_alloc;   // smem rows per K-chunk (multiple of 8), covers tiles*128 + P + 1
-};
-
-__host__ inline HeadGeom make_geom(int Hi, int Wi) {
-  HeadGeom g;
-  g.Hi = Hi;
-  g.Wi = Wi;
-  g.P = Wi + 1;
-  g.rows = Hi * g.P;
-  g.tiles = (g.rows + 127) / 128;
-  g.rows_alloc = (g.tiles * 128 + g.P + 1 + 7) & ~7;
-  return g;
-}
 
 // ---- everything a head call prepares, in one launch (head_prep.cuh) -------------------------------------------
 // forward packs: W[Cin][Cout][3][3] (fp32) -> B[stage][shift][kchunk][80][8] bf16; a non-null bias rides on input
@@ -492,188 +472,6 @@ __global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const
   }
 }
 
-// =====================================================================================================
-// k1b: second transposed convolution + plane softmax (two CTAs per SM, half a frame resident at a time)
-// =====================================================================================================
-// warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue: row quarter q = warp % 4 of each 128-row M-tile,
-// output-row parity e = (warp - 2) / 4 (classes 2e, 2e+1 = accumulator columns [40e, 40e+40)).  The whole K (4 shifts x
-// 32 channels) of a half frame is resident, so a warp computes each 16-column block of its rows when its epilogue needs it.
-constexpr int K1B_THREADS = 320;
-constexpr int K1B_EPI = 256;    // epilogue threads
-
-struct K1bParams {
-  const __nv_bfloat16* mid;   // [B][4][L.rows][8] padded row layout
-  RowLayout L;
-  const __nv_bfloat16* wpk;   // packed weights, one stage (K = 32); bias folded into channel c1
-  float* out;                 // [B][c2][2Hi][2Wi]
-  int B, c2, final_softmax;
-  int Hh;                     // image rows per half (Hi / 2)
-  HeadGeom g;                 // geometry of one half: Hi = Hh, rows_alloc covers Hh + 1 rows
-};
-
-__global__ void __launch_bounds__(K1B_THREADS, 2) k1b_convt_softmax_kernel(const __grid_constant__ K1bParams P) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  const HeadGeom g = P.g;
-  const int a_bytes = 4 * g.rows_alloc * 16;
-  unsigned char* As = smem;
-  unsigned char* Bs = smem + a_bytes;
-  float* stat = reinterpret_cast<float*>(Bs + HB_BSTAGE_BYTES);  // [2][HB_CLS][8 warps]
-  float* fin = stat + 2 * HB_CLS * 8;                            // [2][HB_CLS]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(fin + 2 * HB_CLS + 8);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = bars + 1;
-  uint64_t* b_full = bars + 2;
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int i = tid; i < a_bytes / 16; i += K1B_THREADS) reinterpret_cast<uint4*>(As)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    mbar_init(a_full, 1);
-    mbar_init(a_empty, K1B_EPI / 32);
-    mbar_init(b_full, 1);
-    fence_mbar_init();
-  }
-  fence_proxy_async();
-  __syncthreads();
-
-  const int Hi = 2 * P.Hh, Wi = g.Wi;        // full conv-input image
-  const int Ho = 2 * Hi, Wo = 2 * Wi;
-  const int npix = Hi * Wi;
-  const int npass = P.final_softmax ? 2 : 1;
-  const int nphase = 2 * npass;  // (pass, half)
-
-  if (warp == 0) {
-    // ================= loader =================
-    if (lane == 0) {
-      mbar_expect_tx(b_full, HB_BSTAGE_BYTES);
-      bulk_g2s(Bs, P.wpk, HB_BSTAGE_BYTES, b_full);
-    }
-    int ph = 0;
-    for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
-      for (int phase = 0; phase < nphase; ++phase, ++ph) {
-        const int hf = phase & 1;
-        mbar_wait(a_empty, (ph & 1) ^ 1);
-        // one contiguous copy per K-chunk: Hh image rows + the halo row below, zero column included
-        const uint32_t nbytes = (uint32_t)((P.Hh + 1) * g.P * 16);
-        if (lane < 4) {
-          if (lane == 0) mbar_expect_tx(a_full, 4 * nbytes);
-          __syncwarp(0xf);
-          bulk_g2s(As + (size_t)lane * g.rows_alloc * 16,
-                   P.mid + (((size_t)b * 4 + lane) * P.L.rows + P.L.lead + (size_t)hf * P.Hh * g.P) * 8, nbytes, a_full);
-        }
-      }
-    }
-  } else if (warp >= 2) {
-    // ================= epilogue =================
-    const int q = warp & 3, e = (warp - 2) >> 2;
-    const int ew = warp - 2;  // 0..7
-    const float L2E = 1.4426950408889634f;
-    const size_t plane_stride = (size_t)Ho * Wo;
-    const uint32_t lbo_a = g.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
-    const uint32_t a0 = smem_u32(As), b0 = smem_u32(Bs);
-    mbar_wait(b_full, 0);
-    int ph = 0;
-    for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
-      float mx[HB_CLS], sm[HB_CLS];
-#pragma unroll
-      for (int o = 0; o < HB_CLS; ++o) {
-        mx[o] = -3.0e38f;
-        sm[o] = 0.f;
-      }
-      for (int phase = 0; phase < nphase; ++phase) {
-        const int hf = phase & 1;
-        const bool write = (phase >= nphase - 2);
-        mbar_wait(a_full, ph & 1);
-        {
-          for (int t = 0; t < g.tiles; ++t) {
-            // columns [40e, 40e+40) = classes (py = e, px = 0|1) of this tile; computed in 16-column blocks [32e, 32e+48)
-            // and picked with compile-time register indices
-            float d[48];
-#pragma unroll
-            for (int cc = 0; cc < 3; ++cc) {
-              float acc[2][2][4];
-              mma::zero(acc);
-#pragma unroll
-              for (int sh = 0; sh < 4; ++sh) {
-                const int shift_rows = (sh >> 1) * g.P + (sh & 1);
-#pragma unroll
-                for (int k16 = 0; k16 < 2; ++k16)
-                  mma::kstep(acc, a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
-                             b0 + (sh * 4 + 2 * k16) * lbo_b + (32 * e + 16 * cc) * 16, lbo_b, lane);
-              }
-              mma::rows8(acc, 0, &d[cc * 16], lane);
-              mma::rows8(acc, 1, &d[cc * 16 + 8], lane);
-            }
-            const int row = t * 128 + 32 * q + lane;
-            const int ml = row / g.P, n = row - ml * g.P;
-            const bool valid = (ml < P.Hh) && (n < Wi);
-            const int m = hf * P.Hh + ml;
-            float* dst = P.out + ((size_t)b * P.c2 * Ho + 2 * m + e) * Wo + 2 * n;  // plane o adds o * Ho * Wo
-            auto planes = [&](auto ec) {  // compile-time class offset: no per-value selects
-              constexpr int E = decltype(ec)::value;
-#pragma unroll
-              for (int o = 0; o < HB_CLS; ++o) {
-                if (o >= P.c2) break;
-                const float l0 = d[8 * E + o], l1 = d[8 * E + HB_CLS + o];
-                if (!write) {
-                  const float mm = valid ? fmaxf(l0, l1) : -3.0e38f;
-                  if (__any_sync(0xffffffffu, mm > mx[o])) {
-                    const float mn = fmaxf(mx[o], mm);
-                    sm[o] *= fast_exp2((mx[o] - mn) * L2E);
-                    mx[o] = mn;
-                  }
-                  if (valid) {
-                    const float mL = mx[o] * L2E;
-                    sm[o] += fast_exp2(fmaf(l0, L2E, -mL)) + fast_exp2(fmaf(l1, L2E, -mL));
-                  }
-                } else if (valid) {
-                  float p0 = l0, p1 = l1;
-                  if (P.final_softmax) {
-                    const float mL = fin[o], inv = fin[HB_CLS + o];
-                    p0 = fast_exp2(fmaf(l0, L2E, -mL)) * inv;
-                    p1 = fast_exp2(fmaf(l1, L2E, -mL)) * inv;
-                  }
-                  *reinterpret_cast<float2*>(dst + (size_t)o * plane_stride) = make_float2(p0, p1);
-                }
-              }
-            };
-            if (e == 0) planes(std::integral_constant<int, 0>{});
-            else planes(std::integral_constant<int, 1>{});
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(a_empty);  // this warp's reads of the half are done
-          ++ph;
-        }
-        if (P.final_softmax && phase == 1) {
-          // merge the online-softmax states: lanes -> warp (shuffles) -> 8 epilogue warps (smem)
-#pragma unroll
-          for (int o = 0; o < HB_CLS; ++o) {
-            if (o >= P.c2) break;
-            const float M = warp_max(mx[o]);
-            const float S = warp_sum(sm[o] * fast_exp2((mx[o] - M) * L2E));
-            if (lane == 0) {
-              stat[o * 8 + ew] = M;
-              stat[(HB_CLS + o) * 8 + ew] = S;
-            }
-          }
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (tid - 64 < P.c2) {
-            const int o = tid - 64;
-            float M = stat[o * 8];
-#pragma unroll
-            for (int i = 1; i < 8; ++i) M = fmaxf(M, stat[o * 8 + i]);
-            float S = 0.f;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) S += stat[(HB_CLS + o) * 8 + i] * fast_exp2((stat[o * 8 + i] - M) * L2E);
-            fin[o] = M * L2E;
-            fin[HB_CLS + o] = 1.0f / S;
-          }
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-        }
-      }
-    }
-  }
-}
-
 static size_t k1a_smem_bytes(const K1aGeom& k) {
   return (size_t)K1A_STAGES * (4 * k.rows_alloc * 16 + HB_BSTAGE_BYTES) + (size_t)K1A_STAGES * 4 * HB_KSTAGE * k.box * 2 + 128 + K1A_ZROWS * 16;
 }
@@ -689,31 +487,18 @@ static bool make_feat_tensor_map(CUtensorMap* tm, const void* feat, int B, int C
   return encode(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(feat), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-static size_t k1b_smem_bytes(const HeadGeom& g) {
-  return (size_t)4 * g.rows_alloc * 16 + HB_BSTAGE_BYTES + (2 * HB_CLS * 8 + 2 * HB_CLS + 8) * sizeof(float) + 64;
-}
-
-// geometry of one half image (Hh rows + 1 halo row) of the second layer
-__host__ inline HeadGeom make_half_geom(int Hh, int Wi) {
-  HeadGeom g = make_geom(Hh, Wi);
-  g.rows_alloc = (g.tiles * 128 + g.P + 1 + 7) & ~7;
-  if (g.rows_alloc < (Hh + 1) * g.P + 8) g.rows_alloc = ((Hh + 1) * g.P + 8 + 7) & ~7;
-  return g;
-}
-
 }  // namespace lpb
 
 // ---- which kernels serve a shape ---------------------------------------------------------------------------
-// fast path (k1a + k1b): two-deconv heads whose bands fit the shared-memory tiling above;
+// fast path (k1a, then layer 2 on the banded kernel): two-deconv heads whose bands fit the shared-memory tiling above;
 // generic path (head_rows_bf16.cu): everything else -- one-deconv heads, larger feature maps.
 static bool head_fast_path(int C, int H, int W, int c2, int max_smem) {
   using namespace lpb;
   if (c2 <= 0) return false;
   // W <= 31: the saved copy's lead / trail rows fit the K1A_ZROWS zero source, and a band's staged rows one TMA box
   if (!((W >= 7 || W == 4 || W == 6) && H * W <= 192 && W <= 31)) return false;
-  const HeadGeom g2 = make_half_geom(2 * H, 4 * W);
   const K1aGeom k1 = make_k1a_geom(H, W);
-  return k1.G > 0 && (int64_t)k1a_smem_bytes(k1) <= max_smem && (int64_t)k1b_smem_bytes(g2) <= max_smem;
+  return k1.G > 0 && (int64_t)k1a_smem_bytes(k1) <= max_smem;
 }
 
 static int device_limits(int* max_smem, int* sms) {
@@ -766,12 +551,6 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
 extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
                                  const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
                                  void* workspace, void* stream) {
-  return lpb_head_fwd_bf16_hinted(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, out, saved_xs, workspace, nullptr, stream);
-}
-
-extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
-                                        const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
-                                        void* workspace, void* decode_hints, void* stream) {
   using namespace lpb;
   LPB_REQUIRE(features && w1 && b1 && out && workspace, "head_fwd_bf16: null pointer");
   LPB_REQUIRE(c2 == 0 || (w2 && b2), "head_fwd_bf16: a two-deconv head needs w2 and b2");
@@ -793,10 +572,6 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
     set_error("head_fwd_bf16: cannot encode the feature tensor map (features must be 16-byte aligned)");
     return LPB_ERR_INVALID;
   }
-  // decode hints are produced by the fused two-pass softmax of the banded kernel only (launch_convt_rows marks them invalid
-  // on its other routes); the routes that never reach it do so here
-  if (decode_hints && (!final_softmax || !g_tuning[LPB_TUNE_SOFTMAX_EPILOGUE_V2]))
-    LPB_CUDA(cudaMemsetAsync(decode_hints, 0, (size_t)16 * B * (c2 > 0 ? c2 : c1), s));
   const int nst = C / 4 / HB_KSTAGE;
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const RowLayout Lxs = make_row_layout(2 * H, 2 * W), Lmid = make_row_layout(4 * H, 4 * W);
@@ -835,37 +610,19 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
     p.out = out;
     p.partials = partials;
     if (c2 == 0) {
-      p.hints = final_softmax ? static_cast<int4*>(decode_hints) : nullptr;
       p.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
       rc = launch_convt_rows(p, sms, s);
       if (rc != LPB_OK) return rc;
-    } else {
-      p.mode = CONVT_ROWS_MID;
-      p.mid = mid;
-      p.Lout = Lmid;
-      rc = launch_convt_rows(p, sms, s);
-      if (rc != LPB_OK) return rc;
-      ConvtRowsParams p2{};
-      p2.X = mid;
-      p2.L = Lmid;
-      p2.wpk = wp2;
-      p2.bias = nullptr;  // folded into the GEMM through the ones channel (see the pack above)
-      p2.nst = 1;
-      p2.B = B;
-      p2.cout = c2;
-      p2.out = out;
-      p2.partials = partials;
-      p2.hints = final_softmax ? static_cast<int4*>(decode_hints) : nullptr;
-      p2.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
-      rc = launch_convt_rows(p2, sms, s);
-      if (rc != LPB_OK) return rc;
+      LPB_CUDA(cudaGetLastError());
+      return LPB_OK;
     }
-    LPB_CUDA(cudaGetLastError());
-    return LPB_OK;
-  }
-  const HeadGeom g2 = make_half_geom(2 * H, 4 * W);  // layer 2: 4H rows in two halves
-  const size_t s1 = k1a_smem_bytes(k1), s2 = k1b_smem_bytes(g2);
-  {
+    p.mode = CONVT_ROWS_MID;
+    p.mid = mid;
+    p.Lout = Lmid;
+    rc = launch_convt_rows(p, sms, s);
+    if (rc != LPB_OK) return rc;
+  } else {
+    const size_t s1 = k1a_smem_bytes(k1);
     K1aParams pa{};
     pa.feat = feat_map;
     pa.wpk = wp1;
@@ -888,38 +645,20 @@ extern "C" int lpb_head_fwd_bf16_hinted(const void* features, int B, int C, int 
     const int items = B * k1.G;
     kern<<<items < sms ? items : sms, K1A_THREADS, s1, s>>>(pa);
   }
-  if (g_tuning[LPB_TUNE_SOFTMAX_EPILOGUE_V2]) {
-    // layer 2 on the banded kernel (head_rows_bf16.cu): same GEMM, leaner softmax epilogue
-    ConvtRowsParams p2{};
-    p2.X = mid;
-    p2.L = Lmid;
-    p2.wpk = wp2;
-    p2.bias = nullptr;  // folded into the GEMM through the ones channel
-    p2.nst = 1;
-    p2.B = B;
-    p2.cout = c2;
-    p2.out = out;
-    p2.partials = partials;
-    p2.hints = final_softmax ? static_cast<int4*>(decode_hints) : nullptr;
-    p2.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
-    const int rc = launch_convt_rows(p2, sms, s);
-    if (rc != LPB_OK) return rc;
-    LPB_CUDA(cudaGetLastError());
-    return LPB_OK;
-  }
-  K1bParams pb;
-  pb.mid = mid;
-  pb.L = Lmid;
-  pb.wpk = wp2;
-  pb.out = out;
-  pb.B = B;
-  pb.c2 = c2;
-  pb.final_softmax = final_softmax;
-  pb.Hh = 2 * H;
-  pb.g = g2;
-  LPB_CUDA(cudaFuncSetAttribute(k1b_convt_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s2));
-  const int grid2 = B < 2 * sms ? B : 2 * sms;
-  k1b_convt_softmax_kernel<<<grid2, K1B_THREADS, s2, s>>>(pb);
+  // ---- layer 2 of a two-deconv head, on both paths: the banded kernel over the mid activations ----
+  ConvtRowsParams p2{};
+  p2.X = mid;
+  p2.L = Lmid;
+  p2.wpk = wp2;
+  p2.bias = nullptr;  // folded into the GEMM through the ones channel (see the pack above)
+  p2.nst = 1;
+  p2.B = B;
+  p2.cout = c2;
+  p2.out = out;
+  p2.partials = partials;
+  p2.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
+  const int rc = launch_convt_rows(p2, sms, s);
+  if (rc != LPB_OK) return rc;
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

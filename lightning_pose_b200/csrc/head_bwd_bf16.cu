@@ -104,27 +104,19 @@ __global__ void __launch_bounds__(256) plane_dot_sparse_kernel(G2Src S, long lon
 }
 
 // Thread t of a frame handles input-grid pixel (m, n) = divmod(t, Wi): the 2x2 output block x all channels.
-// Loads are issued as independent batches (probs, dense gradient) before any dependent work; the window
-// look-ups are rare (a 32x32 patch of a 96x96 plane) and come last.
+// Loads are issued as independent batches (probs, dense gradient) before any dependent work; the decode windows are
+// added afterwards by g2_patch_kernel.
 constexpr int G2B_THREADS = 128;
 
-// HAS_WIN: the decode windows are staged per CTA into shared memory first (the CTA's 128 input-grid pixels span at
-// most G2B_MROWS rows m, i.e. 2 * G2B_MROWS output rows; a window contributes 32 columns of each), so the main loop
-// adds them with branch-free shared-memory reads instead of divergent global gathers.
-constexpr int G2B_MROWS = 4;  // input-grid rows a CTA can touch: ceil(128 / Wi) + 1 for Wi >= 43 (host checks)
-
-// HAS_OV (window-less pass ahead of the patch kernel): planes whose decode gradient is dense (flag 2, the decode's overflow
-// buffer) are added here, in the streaming pass -- in the fresh-init regime that is every plane.
-template <bool HAS_G, bool HAS_P, bool HAS_WIN, bool HAS_OV = false>
+// HAS_OV (pass ahead of the patch kernel): planes whose decode gradient is dense (flag 2, the decode's overflow buffer) are
+// added here, in the streaming pass -- in the fresh-init regime that is every plane.
+template <bool HAS_G, bool HAS_P, bool HAS_OV>
 __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B, int C, int Hi, int Wi, int ctas_per_frame,
                                                                __nv_bfloat16* __restrict__ G, RowLayout L) {
   const int b = blockIdx.x / ctas_per_frame, t0 = (blockIdx.x - b * ctas_per_frame) * G2B_THREADS, t = t0 + threadIdx.x;
   const int Wo = 2 * Wi, Ho = 2 * Hi;
   __shared__ float sdot[GB_CLS];
-  __shared__ int4 smeta[GB_CLS];
-  __shared__ float wtile[HAS_WIN ? GB_CLS * 2 * G2B_MROWS * 32 : 1];
-  __shared__ unsigned shit, sov;
-  const int m0 = t0 / Wi;
+  __shared__ unsigned sov;
   if (threadIdx.x < GB_CLS) {
     float d = 0.f;
     int4 mt = make_int4(0, 0, 0, 0);
@@ -137,42 +129,9 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
       }
     }
     sdot[threadIdx.x] = d;
-    smeta[threadIdx.x] = mt;
     if (HAS_OV) {
       const unsigned bov = __ballot_sync((1u << GB_CLS) - 1, mt.z == 2);
       if (threadIdx.x == 0) sov = bov;
-    }
-    if (HAS_WIN) {
-      // does this plane's window (or its dense fallback) touch the CTA's output rows [2 m0, 2 m0 + 2 MROWS)?  A 32x32
-      // window covers a ninth of a 96x96 plane: most (CTA, plane) pairs skip the look-ups altogether (uniform branch)
-      const bool hit = mt.z == 2 || (mt.z == 1 && mt.x < 2 * m0 + 2 * G2B_MROWS && mt.x + 32 > 2 * m0);
-      const unsigned bal = __ballot_sync((1u << GB_CLS) - 1, hit);
-      if (threadIdx.x == 0) shit = bal;
-    }
-  }
-  if (HAS_WIN) {
-    __syncthreads();
-    // wtile[o][yl][lx] = win[o][2*m0 + yl - row0][lx] (0 outside the window / for planes without one)
-    // one window row (32 floats) per warp and step, all steps unrolled: the predicated loads are independent
-    const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
-    constexpr int NROW = GB_CLS * 2 * G2B_MROWS, NSTEP = NROW / (G2B_THREADS / 32), NB = 10;  // NB loads in flight per thread
-    static_assert(NSTEP % NB == 0, "window staging batches");
-#pragma unroll 1
-    for (int k0 = 0; k0 < NSTEP; k0 += NB) {
-      float stage[NB];
-#pragma unroll
-      for (int k = 0; k < NB; ++k) {
-        const int r = wq + (k0 + k) * (G2B_THREADS / 32), o = r / (2 * G2B_MROWS), yl = r - o * (2 * G2B_MROWS);
-        float v = 0.f;
-        if (o < C && ((shit >> o) & 1u)) {
-          const int4 mt = smeta[o];
-          const int ly = 2 * m0 + yl - mt.x;
-          if (mt.z == 1 && (unsigned)ly < 32u) v = __ldg(S.win + ((size_t)b * C + o) * 1024 + ly * 32 + lane);
-        }
-        stage[k] = v;
-      }
-#pragma unroll
-      for (int k = 0; k < NB; ++k) wtile[(wq + (k0 + k) * (G2B_THREADS / 32)) * 32 + lane] = stage[k];
     }
   }
   __syncthreads();
@@ -191,25 +150,6 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
       if (o < C) {
         if (HAS_P) pv[o] = __ldg(reinterpret_cast<const float2*>(S.probs + off0 + o * pstride));
         if (HAS_G) gv[o] = __ldg(reinterpret_cast<const float2*>(S.g_out + off0 + o * pstride));
-      }
-    }
-    if (HAS_WIN) {
-      const float* wrow = wtile + (2 * (m - m0) + py) * 32;
-      const unsigned hits = shit;
-#pragma unroll
-      for (int o = 0; o < GB_CLS; ++o) {
-        if (o < C && ((hits >> o) & 1u)) {
-          const int4 mt = smeta[o];
-          const int lx = x - mt.y;  // window column of output pixel x; x + 1 -> lx + 1
-          const float w0 = wrow[o * (64 * G2B_MROWS) + min(max(lx, 0), 31)];
-          const float w1 = wrow[o * (64 * G2B_MROWS) + min(max(lx + 1, 0), 31)];
-          gv[o].x += (unsigned)lx < 32u ? w0 : 0.f;
-          gv[o].y += (unsigned)(lx + 1) < 32u ? w1 : 0.f;
-          if (mt.z == 2) {  // dense fallback plane (rare; uniform per CTA)
-            const float2 u = __ldg(reinterpret_cast<const float2*>(S.gov + off0 + o * pstride));
-            gv[o].x += u.x, gv[o].y += u.y;
-          }
-        }
       }
     }
     if (HAS_OV && sov) {  // uniform per frame
@@ -302,20 +242,13 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
 template <bool HAS_G, bool HAS_P>
 static void launch_g2_build(const G2Src& S, int B, int C, int Hi, int Wi, __nv_bfloat16* G, RowLayout L, cudaStream_t s) {
   const int cpf = (Hi * Wi + G2B_THREADS - 1) / G2B_THREADS;
-  const bool fits = (G2B_THREADS + Wi - 1) / Wi + 1 <= G2B_MROWS;  // rows m a CTA's pixels can span
-  if (S.win && fits && !g_tuning[LPB_TUNE_G2_PATCH]) {
-    g2_build_kernel<HAS_G, HAS_P, true><<<(unsigned)(B * cpf), G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
-    return;
-  }
   if (!S.win) {
     g2_build_kernel<HAS_G, HAS_P, false><<<(unsigned)(B * cpf), G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
     return;
   }
-  g2_build_kernel<HAS_G, HAS_P, false, true><<<(unsigned)(B * cpf), G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
-  {
-    const long long np = (long long)B * C;
-    g2_patch_kernel<HAS_G, HAS_P><<<(unsigned)((np + 3) / 4), 128, 0, s>>>(S, np, C, Hi, Wi, G, L);
-  }
+  g2_build_kernel<HAS_G, HAS_P, true><<<(unsigned)(B * cpf), G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
+  const long long np = (long long)B * C;
+  g2_patch_kernel<HAS_G, HAS_P><<<(unsigned)((np + 3) / 4), 128, 0, s>>>(S, np, C, Hi, Wi, G, L);
 }
 
 // (the data-gradient operand packs  out[tile][shift][kchunk][r][8]: element (r, k) = W[tile*rows_per_tile + r][o][ky][kx]
@@ -466,7 +399,6 @@ struct B3aParams {
   int B, C4, Hi, Wi;         // shuffled-image geometry (Hi = 2H, Wi = 2W)
   int Hh;                    // image rows per band (multiple of 4)
   int ncols;                 // accumulator columns per band = Hh * (Wi + 1) rounded up to 16 (<= 304)
-  int backoff, prefetch;
   int tma_store;             // 1: the epilogue stages bf16 rows in shared memory and a TMA tensor store writes them (below)
 };
 
@@ -554,7 +486,7 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
       for (int band = 0; band < nbands; ++band, ++it) {
         const int st = it & 1, y0 = band * Hh, hb = min(Hh, Hi - y0);
         const int npairs = hb / 4;  // feature-row pairs in this band
-        mbar_wait_idle(&g_full[st], (it >> 1) & 1, P.backoff);
+        mbar_wait_idle(&g_full[st], (it >> 1) & 1);
         const uint32_t g0 = smem_u32(Gs + (size_t)st * g_bytes);
         auto issue = [&](int item, float (&buf)[2][NCH * 16]) {
           const int ml = 4 * (item >> 1) + (item & 1);  // first accumulator row of the item within this band
@@ -641,7 +573,7 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
               bulk_commit_group();
             }
           }
-        } else if (NCH <= 2 && P.prefetch) {
+        } else if (NCH <= 2) {
           // the next item's blocks are computed before the current item is converted and stored
           float va[2][NCH * 16], vb[2][NCH * 16];
           if (e < nitems) issue(e, va);
@@ -1207,18 +1139,17 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.Wi = Wi1;
     p.Hh = Hh;
     p.ncols = (Hh * (Wi1 + 1) + 15) & ~15;
-    p.backoff = g_tuning[LPB_TUNE_WAIT_BACKOFF];
-    p.prefetch = g_tuning[LPB_TUNE_B3A_PREFETCH];
     const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
     size_t smem = (size_t)2 * GB_KC * rows_alloc * 16 + (size_t)4 * GB_KC * 128 * 16 + 160;
     LPB_REQUIRE(smem <= 225 * 1024, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
-    // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit
+    // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit, dfeat is 16-byte
+    // aligned and the tensor map encodes; otherwise direct 16-byte stores
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     p.tma_store = 0;
     {
       const size_t stage = (size_t)2 * 4 * 128 * 4 * W + 128;
-      if (g_tuning[LPB_TUNE_B3A_TMA_STORE] && smem + stage <= 225 * 1024 && (reinterpret_cast<uintptr_t>(dfeat) % 16) == 0 &&
+      if (smem + stage <= 225 * 1024 && (reinterpret_cast<uintptr_t>(dfeat) % 16) == 0 &&
           make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
         p.tma_store = 1;
         smem += stage;

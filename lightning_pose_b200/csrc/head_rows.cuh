@@ -20,9 +20,7 @@ struct ConvtRowsParams {
   RowLayout Lout;
   float* out;                // planes [B][cout][2Hi][2Wi] (raw or softmaxed)
   float* partials;           // split softmax: [B][nbands][20][2] (max, sum) per (frame, band, plane), or null (fused two-pass form)
-  int4* hints;               // optional [B][cout] decode hints {arg-max row, col, bits(max outside the 32x32 box around it), valid}:
-                             // written by the fused two-pass softmax (planes up to 128 x 128), zeroed (invalid) by every other form
-  int R, rows_alloc, backoff;  // filled by launch_convt_rows
+  int R, rows_alloc;         // filled by launch_convt_rows
 };
 
 int launch_rows_shuffle(const __nv_bfloat16* feat, int B, int C, int H, int W, __nv_bfloat16* xs, cudaStream_t s);

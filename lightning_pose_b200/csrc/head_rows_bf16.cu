@@ -78,22 +78,18 @@ constexpr int CR_EPI = 256;
 constexpr int CR_TILES = 2;      // M-tiles per band: a warp's accumulators (CR_TILES x 32 rows x 48 columns) stay in registers
 static_assert(CR_TILES * 128 == CR_BAND_ROWS, "head_rows.cuh sizes the per-band softmax statistics with CR_BAND_ROWS");
 constexpr int CR_STAGES = 2;
-constexpr int CR_NMASK = 64;     // (band, tile) pairs of a frame the decode hints can cover
-constexpr int CR_HBOX = 16;      // decode hints: the box is rows / columns [arg - 16, arg + 15] = decode.cu's first window
 
 // NPL: compile-time plane count (17 = the usual keypoint count) or 0 for a run-time count <= 20.
-// V2: softmax epilogue with one warp vote per tile (instead of one per plane), the running-max rescale out of the
-// common path, (shift, 1/sum) fetched as one 8-byte shared load and the output pointer advanced by addition.
-template <int MODE, int NPL, bool V2, bool HINT = false>
+// The softmax modes' epilogue takes one warp vote per tile (instead of one per plane), keeps the running-max rescale out
+// of the common path, fetches (shift, 1/sum) as one 8-byte shared load and advances the output pointer by addition.
+template <int MODE, int NPL>
 __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_constant__ ConvtRowsParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Pp = P.L.Pp, Wi = P.L.Wi, Hi = P.L.Hi;
   const int a_bytes = 4 * P.rows_alloc * 16, stage_bytes = a_bytes + CR_BSTAGE;
   float* stat = reinterpret_cast<float*>(smem + CR_STAGES * stage_bytes);  // [2][CR_CLS][8 warps]
   float* fin = stat + 2 * CR_CLS * 8;                                       // [CR_CLS][2] = (max * log2 e, 1 / sum)
-  int* finA = reinterpret_cast<int*>(fin + 2 * CR_CLS + 8);                 // [CR_CLS] decode hints: arg max (row << 16 | col)
-  unsigned* nmask = reinterpret_cast<unsigned*>(finA + CR_CLS);             // [CR_NMASK] per (band, tile): planes whose box the tile's rows meet
-  uint64_t* bars = reinterpret_cast<uint64_t*>(nmask + CR_NMASK);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(fin + 2 * CR_CLS);
   uint64_t* full = bars;       // [2]
   uint64_t* empty = bars + 2;  // [2]
 
@@ -120,12 +116,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
   const int nitems = PER_BAND ? P.B * nbands : P.B;
   const int bands_per_item = PER_BAND ? 1 : nbands;
   const int ncls = NPL ? NPL : P.cout;  // planes handled by the unrolled loops
-  // Decode hints (fused two-pass softmax only): the running max of pass 0 carries the pixel index in its 14 low mantissa
-  // bits (any value within 2^-9 of the max is as good a softmax shift, and every use of the shift is relative to the stored
-  // value), so the plane's arg max falls out of the existing max-merge; pass 1 tracks the largest probability OUTSIDE the
-  // 32 x 32 box around it.  decode.cu then needs no sweep of the plane when that bound is below its pruning threshold.
-  // (HINT instantiation: the launch has checked planes <= 128 x 128 and nbands * CR_TILES <= CR_NMASK)
-  constexpr bool hint_on = HINT && V2 && MODE == CONVT_ROWS_SOFTMAX;
+  constexpr bool SOFTMAX = MODE == CONVT_ROWS_SOFTMAX || MODE == CONVT_ROWS_SOFTMAX_P0 || MODE == CONVT_ROWS_SOFTMAX_P1;
 
   if (warp == 0) {
     // ================= loader: one bulk copy per K-chunk (band rows + the halo row below) + the stage's weights ====
@@ -139,7 +130,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
           const uint32_t nbytes = (uint32_t)((rb + 1) * Pp * 16);
           for (int st = 0; st < nst; ++st, ++it) {
             const int s = it % CR_STAGES;
-            mbar_wait_idle(&empty[s], ((it / CR_STAGES) & 1) ^ 1, P.backoff);
+            mbar_wait_idle(&empty[s], ((it / CR_STAGES) & 1) ^ 1);
             unsigned char* As = smem + s * stage_bytes;
             const bool load_b = nst > 1 || it < CR_STAGES;
             if (lane == 0) {
@@ -195,13 +186,13 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
           for (int t = 0; t < CR_TILES; ++t) mma::zero(acc[t]);
           for (int st = 0; st < nst; ++st, ++it) {
             const int s = it % CR_STAGES;
-            mbar_wait_idle(&full[s], (it / CR_STAGES) & 1, P.backoff);
+            mbar_wait_idle(&full[s], (it / CR_STAGES) & 1);
             const uint32_t a0 = smem_u32(smem + s * stage_bytes), b0 = a0 + a_bytes;
             // only the n8 tiles (of the warp's six, from column 32e) that the epilogue reads -- [40e, 40e + 40) -- and that
             // hold real taps of the shift: 8 tile-steps for e = 0 (shifts with dm = 1 carry nothing for py = 0), 16 for e = 1.
-            // The V2 softmax forms with a run-time plane count issue all six tiles with one body for both parities: there,
+            // The softmax forms with a run-time plane count issue all six tiles with one body for both parities: there,
             // two per-parity bodies raised ptxas's local-memory spills.
-            if constexpr (V2 && NPL == 0 && MODE != CONVT_ROWS_MID && MODE != CONVT_ROWS_PLANES) {
+            if constexpr (SOFTMAX && NPL == 0) {
 #pragma unroll
               for (int t = 0; t < CR_TILES; ++t) {
                 if (t >= tiles) break;
@@ -247,7 +238,6 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             const int ml = row / Pp, n = row - ml * Pp;
             const bool valid = (ml < rb) && (n < Wi);
             const int y = 2 * (y0 + ml) + e, x = 2 * n;
-            const unsigned near = (hint_on && write) ? nmask[bi * CR_TILES + t] : 0u;
             auto body = [&](auto ec) {
               constexpr int E = decltype(ec)::value;
               if constexpr (MODE == CONVT_ROWS_MID) {
@@ -284,7 +274,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                 return;
               }
               float* dst = P.out + ((size_t)b * P.cout * Ho + y) * Wo + x;  // plane o adds o * Ho * Wo
-              if constexpr (V2 && (MODE == CONVT_ROWS_SOFTMAX || MODE == CONVT_ROWS_SOFTMAX_P0 || MODE == CONVT_ROWS_SOFTMAX_P1)) {
+              if constexpr (SOFTMAX) {
                 if (!write) {
                   // ---- pass 0: per-thread online (max, sum) per plane; the rescale is rare after the first tiles ----
                   bool need = false;
@@ -298,10 +288,8 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 #pragma unroll
                       for (int o = 0; o < CR_CLS; ++o) {
                         if (o >= ncls) break;
-                        float tm = fmaxf(d[8 * E + o], d[8 * E + CR_CLS + o]);
+                        const float tm = fmaxf(d[8 * E + o], d[8 * E + CR_CLS + o]);
                         if (tm > mx[o]) {
-                          if (hint_on)
-                            tm = __int_as_float((__float_as_int(tm) & ~0x3FFF) | (y * Wo + x + (d[8 * E + CR_CLS + o] > d[8 * E + o] ? 1 : 0)));
                           sm[o] *= fast_exp2((mx[o] - tm) * L2E);
                           mx[o] = tm;
                         }
@@ -326,44 +314,16 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                     const float p1 = fast_exp2(fmaf(d[8 * E + CR_CLS + o], L2E, -f.x)) * f.y;
                     *reinterpret_cast<float2*>(dst) = make_float2(p0, p1);
                     dst += plane_stride;
-                    if (hint_on) {
-                      if ((near >> o) & 1u) {  // this tile's rows meet plane o's box: per-pixel test (uniform branch)
-                        const int a = finA[o];
-                        const bool iny = (unsigned)(y - (a >> 16) + CR_HBOX) < 2u * CR_HBOX;
-                        const int dx = x - (a & 0xffff) + CR_HBOX;
-                        mx[o] = fmaxf(mx[o], fmaxf((iny && (unsigned)dx < 2u * CR_HBOX) ? 0.f : p0, (iny && (unsigned)(dx + 1) < 2u * CR_HBOX) ? 0.f : p1));
-                      } else {
-                        mx[o] = fmaxf(mx[o], fmaxf(p0, p1));
-                      }
-                    }
                   }
                 }
-                return;
-              }
+              } else {
+                // CONVT_ROWS_PLANES: raw planes (+ bias)
 #pragma unroll
-              for (int o = 0; o < CR_CLS; ++o) {
-                if (o >= ncls) break;
-                const float bo = use_bias ? __ldg(P.bias + o) : 0.f;
-                const float l0 = d[8 * E + o] + bo, l1 = d[8 * E + CR_CLS + o] + bo;
-                if (!write) {
-                  const float mm = valid ? fmaxf(l0, l1) : -1.0e30f;
-                  if (__any_sync(0xffffffffu, mm > mx[o])) {
-                    const float mn = fmaxf(mx[o], mm);
-                    sm[o] *= fast_exp2((mx[o] - mn) * L2E);
-                    mx[o] = mn;
-                  }
-                  if (valid) {
-                    const float mL = mx[o] * L2E;
-                    sm[o] += fast_exp2(fmaf(l0, L2E, -mL)) + fast_exp2(fmaf(l1, L2E, -mL));
-                  }
-                } else if (valid) {
-                  float p0 = l0, p1 = l1;
-                  if (MODE == CONVT_ROWS_SOFTMAX || MODE == CONVT_ROWS_SOFTMAX_P1) {
-                    const float mL = fin[2 * o], inv = fin[2 * o + 1];
-                    p0 = fast_exp2(fmaf(l0, L2E, -mL)) * inv;
-                    p1 = fast_exp2(fmaf(l1, L2E, -mL)) * inv;
-                  }
-                  *reinterpret_cast<float2*>(dst + (size_t)o * plane_stride) = make_float2(p0, p1);
+                for (int o = 0; o < CR_CLS; ++o) {
+                  if (o >= ncls) break;
+                  const float bo = use_bias ? __ldg(P.bias + o) : 0.f;
+                  const float l0 = d[8 * E + o] + bo, l1 = d[8 * E + CR_CLS + o] + bo;
+                  if (valid) *reinterpret_cast<float2*>(dst + (size_t)o * plane_stride) = make_float2(l0, l1);
                 }
               }
             };
@@ -399,49 +359,10 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             } else {
               fin[2 * o] = M * L2E;
               fin[2 * o + 1] = 1.0f / S;
-              if (hint_on) {
-                const int loc = __float_as_int(M) & 0x3FFF, ay = loc / Wo;
-                finA[o] = (ay << 16) | (loc - ay * Wo);
-              }
             }
           }
           asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (hint_on) {
-            // per (band, tile): the planes whose box rows [ay - 16, ay + 15] the tile's output rows can meet
-            if (tid - 64 < nbands * CR_TILES) {
-              const int bj = (tid - 64) / CR_TILES, tj = (tid - 64) - bj * CR_TILES;
-              const int ylo = 2 * (bj * R + (tj * 128) / Pp), yhi = 2 * (bj * R + (tj * 128 + 127) / Pp) + 1;
-              unsigned m = 0;
-              for (int o = 0; o < ncls; ++o) {
-                const int ay = finA[o] >> 16;
-                if (yhi >= ay - CR_HBOX && ylo <= ay + CR_HBOX - 1) m |= 1u << o;
-              }
-              nmask[tid - 64] = m;
-            }
-#pragma unroll
-            for (int o = 0; o < CR_CLS; ++o) mx[o] = 0.f;  // pass 1 reuses mx[] for the largest probability outside the box
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-          }
         }
-      }
-      if (hint_on) {
-        // merge the outside-the-box maxima: lanes -> warp -> 8 epilogue warps, then one 16-byte hint per plane
-#pragma unroll
-        for (int o = 0; o < CR_CLS; ++o) {
-          if (o >= ncls) break;
-          const float M = warp_max(mx[o]);
-          if (lane == 0) stat[o * 8 + ew] = M;
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (tid - 64 < ncls) {
-          const int o = tid - 64;
-          float M = stat[o * 8];
-#pragma unroll
-          for (int i = 1; i < 8; ++i) M = fmaxf(M, stat[o * 8 + i]);
-          const int a = finA[o];
-          P.hints[(size_t)b * ncls + o] = make_int4(a >> 16, a & 0xffff, __float_as_int(M), 1);
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // stat / finA are free for the next frame
       }
     }
   }
@@ -457,9 +378,8 @@ int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
   const int tiles = (p.R * Pp + 127) / 128;
   p.rows_alloc = (tiles * 128 + Pp + 1 + 7) & ~7;
   if (p.rows_alloc < (p.R + 1) * Pp + 8) p.rows_alloc = ((p.R + 1) * Pp + 8 + 7) & ~7;
-  const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + CR_BSTAGE) + (2 * CR_CLS * 8 + 2 * CR_CLS + 8 + CR_CLS + CR_NMASK) * sizeof(float) + 64;
+  const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + CR_BSTAGE) + (2 * CR_CLS * 8 + 2 * CR_CLS) * sizeof(float) + 64;
   LPB_REQUIRE(smem <= 113 * 1024, "head_fwd_bf16: band stages need %zu B shared memory", smem);
-  p.backoff = g_tuning[LPB_TUNE_WAIT_BACKOFF];
   const int nbands = (p.L.Hi + p.R - 1) / p.R;
   auto run = [&](auto kern, long long nitems) -> int {
     const int grid = (int)(nitems < sms ? nitems : sms);  // one CTA per SM: the accumulators take the register file
@@ -467,33 +387,21 @@ int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
     kern<<<grid, CR_THREADS, smem, s>>>(p);
     return LPB_OK;
   };
-  const bool v2 = g_tuning[LPB_TUNE_SOFTMAX_EPILOGUE_V2] != 0, k17 = p.cout == 17;
+  const bool k17 = p.cout == 17;
   const long long per_band = (long long)p.B * nbands;
-  if (p.hints) {
-    // decode hints come from the fused two-pass softmax only (same condition as the kernel's hint_on); every other route
-    // marks them invalid
-    const bool fused = p.mode == CONVT_ROWS_SOFTMAX && v2 &&
-                       !(p.partials && (g_tuning[LPB_TUNE_SOFTMAX_SPLIT] == 2 || (g_tuning[LPB_TUNE_SOFTMAX_SPLIT] == 1 && p.B < sms)));
-    if (!fused || 4 * p.L.Hi * p.L.Wi > 16384 || nbands * CR_TILES > CR_NMASK || !g_tuning[LPB_TUNE_DECODE_HINTS]) {
-      LPB_CUDA(cudaMemsetAsync(p.hints, 0, sizeof(int4) * (size_t)p.B * p.cout, s));
-      p.hints = nullptr;
-    }
-  }
-  if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<CONVT_ROWS_MID, 0, false>, per_band);
-  if (p.mode == CONVT_ROWS_PLANES) return k17 ? run(convt_rows_kernel<CONVT_ROWS_PLANES, 17, false>, per_band) : run(convt_rows_kernel<CONVT_ROWS_PLANES, 0, false>, per_band);
+  if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<CONVT_ROWS_MID, 0>, per_band);
+  if (p.mode == CONVT_ROWS_PLANES) return k17 ? run(convt_rows_kernel<CONVT_ROWS_PLANES, 17>, per_band) : run(convt_rows_kernel<CONVT_ROWS_PLANES, 0>, per_band);
   // split softmax (statistics launch + normalising launch, both parallel over (frame, band)) when one CTA per frame would
   // leave SMs idle (fewer frames than SMs); otherwise the single two-pass kernel is faster, because a frame's second pass
   // re-reads operands its first pass left in L2 (768-frame step 1.768 vs 1.802 ms; with the 256-frame labeled call fused
   // as well: step 1.565 vs 1.583 ms, forward-only 0.611 vs 0.635 ms).  Key value 2 forces the split.
-  const int split_key = g_tuning[LPB_TUNE_SOFTMAX_SPLIT];
-  if (v2 && p.partials && (split_key == 2 || (split_key == 1 && p.B < sms))) {
-    int rc = k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 17, true>, per_band) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 0, true>, per_band);
+  const int split_key = g_softmax_split;
+  if (p.partials && (split_key == 2 || (split_key == 1 && p.B < sms))) {
+    int rc = k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 17>, per_band) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 0>, per_band);
     if (rc != LPB_OK) return rc;
-    return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 17, true>, per_band) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 0, true>, per_band);
+    return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 17>, per_band) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 0>, per_band);
   }
-  if (v2 && p.hints) return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 17, true, true>, p.B) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0, true, true>, p.B);
-  if (v2) return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 17, true>, p.B) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0, true>, p.B);
-  return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 17, false>, p.B) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0, false>, p.B);
+  return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 17>, p.B) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0>, p.B);
 }
 
 }  // namespace lpb

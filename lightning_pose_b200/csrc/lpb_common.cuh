@@ -28,7 +28,7 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
     if (e__ != cudaSuccess) return ::lpb::cuda_fail(e__, #call, __FILE__, __LINE__); \
   } while (0)
 
-extern int g_tuning[];  // abi.cu: kernel-variant switches (LPB_TUNE_*)
+extern int g_softmax_split;  // abi.cu: LPB_TUNE_SOFTMAX_SPLIT
 
 // ---- device helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float warp_max(float v) {
@@ -116,11 +116,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 // the same wait for warps that expect to idle for a long time (epilogue warps during a frame's MMAs, loaders ahead of
 // their consumers): poll, then sleep between polls so the spinning does not take issue slots from the working warps
-__device__ __forceinline__ void mbar_wait_idle(uint64_t* bar, uint32_t parity, int backoff) {
-  if (!backoff) {
-    mbar_wait(bar, parity);
-    return;
-  }
+__device__ __forceinline__ void mbar_wait_idle(uint64_t* bar, uint32_t parity) {
   uint32_t done = 0;
   while (true) {
     asm volatile(

@@ -82,14 +82,11 @@ class _HeadFunction(torch.autograd.Function):
     def forward(ctx, features, final_softmax, decode, train, *params):
         n = len(params) // 2
         weights, biases = list(params[:n]), list(params[n:])
-        saved = acts = hints = None
+        saved = acts = None
         if features.dtype == torch.bfloat16 and features.is_cuda and ops.head_bf16_supported(
                 tuple(features.shape), [w.shape[1] for w in weights], train=train):
-            res = ops._head_forward_bf16(features.contiguous(), weights, biases, final_softmax, train=train, want_hints=decode is not None)
-            if decode is not None:
-                out, saved, hints = res if train else (res[0], None, res[1])
-            else:
-                out, saved = res if train else (res, None)
+            res = ops._head_forward_bf16(features.contiguous(), weights, biases, final_softmax, train=train)
+            out, saved = res if train else (res, None)
         elif train:
             out, acts = ops.head_forward_f32(features, weights, biases, final_softmax, keep_activations=True)
         else:
@@ -102,8 +99,7 @@ class _HeadFunction(torch.autograd.Function):
             ctx.save_for_backward(features, out, *params, *extra)
             return out
         ds, temperature = decode
-        # (hints: what the bf16 head's softmax pass knows about each plane -- peaked planes are decoded without a sweep)
-        xy, conf, stats = ops.decode_forward_hinted(out, int(ds), float(temperature), hints)
+        xy, conf, stats = ops.decode_forward(out, int(ds), float(temperature))
         ctx.save_for_backward(features, out, *params, *extra, stats)
         ctx.mark_non_differentiable(conf)
         return out, xy.reshape(-1, out.shape[1] * 2), conf

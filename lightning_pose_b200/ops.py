@@ -59,8 +59,9 @@ def _cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
 # =====================================================================================
 # soft-argmax decode
 # =====================================================================================
-@torch.library.custom_op("lpb200::decode_fwd", mutates_args=())
-def _decode_fwd(heatmaps: torch.Tensor, ds: int, temperature: float) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+def decode_forward(heatmaps: torch.Tensor, ds: int, temperature: float):
+    """soft-argmax decode -> (xy, conf, stats).  No autograd node of its own (``_decode_fwd`` and ``_HeadFunction`` own
+    the backward)."""
     b, k, h, w = heatmaps.shape
     xy = torch.empty((b, k, 2), device=heatmaps.device, dtype=torch.float32)
     conf = torch.empty((b, k), device=heatmaps.device, dtype=torch.float32)
@@ -70,17 +71,16 @@ def _decode_fwd(heatmaps: torch.Tensor, ds: int, temperature: float) -> tuple[to
     return xy, conf, stats
 
 
+@torch.library.custom_op("lpb200::decode_fwd", mutates_args=())
+def _decode_fwd(heatmaps: torch.Tensor, ds: int, temperature: float) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    return decode_forward(heatmaps, ds, temperature)
+
+
 def decode_forward_hinted(heatmaps: torch.Tensor, ds: int, temperature: float, hints):
-    """``_decode_fwd`` with the per-plane hints the bf16 head's softmax pass wrote for these very heatmaps (or None):
-    peaked planes are decoded from the window around their maximum without a sweep of the plane; same results.
-    No autograd node of its own (``_HeadFunction`` owns the backward)."""
-    b, k, h, w = heatmaps.shape
-    xy = torch.empty((b, k, 2), device=heatmaps.device, dtype=torch.float32)
-    conf = torch.empty((b, k), device=heatmaps.device, dtype=torch.float32)
-    stats = torch.empty((b, k, 8), device=heatmaps.device, dtype=torch.float32)
-    with torch.cuda.device(heatmaps.device):
-        check(lib.lpb_decode_fwd_hinted(_ptr(heatmaps), b * k, h, w, ds, temperature, _ptr(xy), _ptr(conf), _ptr(stats), _ptr(hints), _stream()))
-    return xy, conf, stats
+    # kept for bench.py's call, which passes what _head_forward_bf16(..., want_hints=True) returned: always None
+    if hints is not None:
+        raise ValueError("decode_forward_hinted: the head produces no decode hints; pass hints=None")
+    return decode_forward(heatmaps, ds, temperature)
 
 
 @_decode_fwd.register_fake
@@ -243,14 +243,10 @@ def _head_forward_bf16(f, weights, biases, final_softmax, train=False, want_hint
     if train or plan.value == 0:  # row-layout copy of the shuffled features: the banded path's operand / the wgrad's input
         check(lib.lpb_head_bf16_saved_bytes(b, c, h, w, C.byref(nbytes)))
         xs = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
-    # decode hints (want_hints: a soft-argmax decode of `out` follows): 16 bytes per plane, see lpb_decode_fwd_hinted
-    hints = None
-    if want_hints and final_softmax and lib.lpb_get_tuning(14) == 1:  # LPB_TUNE_DECODE_HINTS
-        hints = torch.empty((b * out.shape[1], 4), device=f.device, dtype=torch.int32)
     with torch.cuda.device(f.device):
-        check(lib.lpb_head_fwd_bf16_hinted(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), _ptr(out), _ptr(xs), _ptr(ws), _ptr(hints), _stream()))
-    if want_hints:
-        return (out, (xs, ws), hints) if train else (out, hints)
+        check(lib.lpb_head_fwd_bf16(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), _ptr(out), _ptr(xs), _ptr(ws), _stream()))
+    if want_hints:  # kept for bench.py's call, which unpacks a decode-hints slot (always None)
+        return (out, (xs, ws), None) if train else (out, None)
     if train:
         return out, (xs, ws)
     return out

@@ -1,5 +1,5 @@
 """Stand-alone check of the tensor-core head (run under `timeout`): compares the intermediate activations
-(k1a) and the final heatmaps (k1b) with the oracle on identically bf16-rounded tensors."""
+(k1a) and the final heatmaps (layer 2) with the oracle on identically bf16-rounded tensors."""
 import ctypes as C
 import os
 import sys

@@ -35,15 +35,10 @@ def test_library_exports_every_declared_symbol():
     assert _lib.lib.lpb_build_arch() == b"sm_90a"
 
 
-def test_argument_validation_without_gpu():
+def test_entry_points_validate_arguments_without_gpu():
     from lightning_pose_b200 import _lib
 
     rc = _lib.lib.lpb_decode_fwd(None, 1, 8, 8, 2, 1000.0, None, None, None, None)
-    assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
-    # the hinted forms validate like the plain ones (hints themselves are optional: NULL = plain route)
-    rc = _lib.lib.lpb_decode_fwd_hinted(None, 1, 8, 8, 2, 1000.0, None, None, None, None, None)
-    assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
-    rc = _lib.lib.lpb_head_fwd_bf16_hinted(None, 1, 384, 16, 16, None, None, 17, None, None, 0, 1, None, None, None, None, None)
     assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
     rc = _lib.lib.lpb_decode_prepare(8, 8, 7)
     assert rc == -1 and b"bad shape" in _lib.lib.lpb_last_error()
@@ -197,9 +192,18 @@ def test_round2_entry_points_validate_arguments_without_gpu():
     ):
         assert rc == -1, (rc, L.lpb_last_error())
     assert L.lpb_context_gather(C.c_void_p(16), 4, 24, 5, C.c_void_p(16), None) == -1  # items must be 16-byte multiples
+
+
+def test_tuning_switch_takes_only_softmax_split():
+    """LPB_TUNE_SOFTMAX_SPLIT (key 7) is the one tuning switch: its default splits below one wave, and every other key
+    is rejected by lpb_set_tuning and reads -1."""
+    from lightning_pose_b200 import _lib
+
+    L = _lib.lib
     assert L.lpb_set_tuning(99, 1) == -1 and L.lpb_get_tuning(99) == -1
-    for k in range(16):
-        assert 0 <= L.lpb_get_tuning(k) <= 8
+    assert L.lpb_get_tuning(7) == 1
+    for k in [*range(7), *range(8, 16)]:
+        assert L.lpb_set_tuning(k, 1) == -1 and L.lpb_get_tuning(k) == -1
 
 
 def test_head_shape_planner_python_side():

@@ -1113,9 +1113,9 @@ def test_multiview_transformer_tracker_config4(lpb, dev):
 
 
 def test_kernel_variants_agree(lpb, dev):
-    """Every LPB_TUNE_* switch selects a different implementation of the SAME stage: results must agree to rounding
-    (row-form vs block-form operand producer: bit-identical operands; softmax epilogues and decode drivers: same math
-    in a different order)."""
+    """LPB_TUNE_SOFTMAX_SPLIT (key 7) selects a different implementation of the SAME stage: the plane softmax as two
+    launches parallel over (frame, band) (2: always) or one per-frame two-pass kernel (0: never split); results must agree
+    to rounding (same math in a different order), and the default (which splits below one wave: 6 frames) with both."""
     from lightning_pose_b200._lib import lib
 
     head = _rand_head("resnet50", 2048, 17, gain=4.0, seed=41).to(dev)
@@ -1129,19 +1129,15 @@ def test_kernel_variants_agree(lpb, dev):
         ((kp * gk).sum() * 1e-3 + (hm * hm).sum()).backward()
         return hm.detach().clone(), kp.detach().clone(), cf.detach().clone(), f.grad.float().clone(), list(head.upsampling_layers)[1].weight.grad.clone()
 
-    nkeys = 16
-    saved = [lib.lpb_get_tuning(k) for k in range(nkeys)]
-    cur = run()  # the defaults (some keys have more than two settings, e.g. 11 = 2)
+    saved = lib.lpb_get_tuning(7)
+    cur = run()  # the default
     try:
-        for k in range(nkeys):
-            lib.lpb_set_tuning(k, 3 if k == 8 else 1)  # key 8 is a count (resident decode CTAs per SM), the others are switches
+        assert lib.lpb_set_tuning(7, 2) == 0
         new = run()
-        for k in range(nkeys):
-            lib.lpb_set_tuning(k, 0)
+        assert lib.lpb_set_tuning(7, 0) == 0
         old = run()
     finally:
-        for k, v in enumerate(saved):
-            lib.lpb_set_tuning(k, v)
+        lib.lpb_set_tuning(7, saved)
     close(new[0], old[0], atol=1e-9, rtol=2e-5)   # heatmaps
     close(new[1], old[1], atol=2e-3, rtol=1e-5)   # keypoints (T = 1000 amplifies the last ulp of a heatmap)
     close(new[2], old[2], atol=1e-5, rtol=1e-4)   # confidences
@@ -1204,84 +1200,3 @@ def test_fused_adam_graph_replay(lpb, dev):
     torch.cuda.synchronize(dev)
     assert float(opt.state[p]["step"]) == 4.0
     close(p, q, atol=1e-6, rtol=2e-5)
-
-
-def _torch_hints(hm, rows, cols):
-    """largest value outside the box [row - 16, row + 15] x [col - 16, col + 15] of every plane (the hint definition)."""
-    b, k, h, w = hm.shape
-    yy = torch.arange(h, device=hm.device).view(1, 1, h, 1)
-    xx = torch.arange(w, device=hm.device).view(1, 1, 1, w)
-    r, c = rows.view(b, k, 1, 1), cols.view(b, k, 1, 1)
-    inside = (yy >= r - 16) & (yy <= r + 15) & (xx >= c - 16) & (xx <= c + 15)
-    return hm.masked_fill(inside, 0.0).amax(dim=(2, 3))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("shape,ds", [((6, 17, 96, 96), 2), ((3, 17, 64, 64), 2), ((2, 5, 128, 128), 2)])
-def test_decode_hinted_equals_plain(lpb, dev, shape, ds):
-    """lpb_decode_fwd_hinted: peaked planes decoded from the window around the hinted maximum (no sweep) give the plain
-    route's outputs; hints that do not allow it (large value outside the box), invalid hints and slightly misplaced
-    maxima (any point is a valid lower bound) fall back or still agree."""
-    from lightning_pose_b200 import ops
-
-    b, k, h, w = shape
-    g = torch.Generator().manual_seed(5)
-    cy = torch.rand(b, k, generator=g) * (h - 1)
-    cx = torch.rand(b, k, generator=g) * (w - 1)
-    yy = torch.arange(h).view(1, 1, h, 1).float()
-    xx = torch.arange(w).view(1, 1, 1, w).float()
-    logits = -((yy - cy.view(b, k, 1, 1)) ** 2 + (xx - cx.view(b, k, 1, 1)) ** 2) / (2 * 1.5**2) * 0.9 + 0.05 * torch.randn(b, k, h, w, generator=g)
-    logits[0, 0] += 6.0 * torch.exp(-((yy[0, 0] - (h - 5)) ** 2 + (xx[0, 0] - 4.0) ** 2) / 4.0)  # a second, far peak: must fall back
-    logits[0, 1] = 0.01 * torch.randn(h, w, generator=g)                                             # flat plane: queued either way
-    hm = torch.softmax(logits.reshape(b, k, -1), -1).reshape(b, k, h, w).to(dev).contiguous()
-    flat = hm.reshape(b, k, -1).argmax(-1)
-    rows, cols = flat // w, flat % w
-    plain = ops._decode_fwd(hm, ds, 1000.0)
-
-    def run(r, c, valid=1):
-        hint = torch.stack([r.int(), c.int(), _torch_hints(hm, r, c).view(torch.int32), torch.full_like(r, valid).int()], -1).reshape(-1, 4).contiguous()
-        return ops.decode_forward_hinted(hm, ds, 1000.0, hint)
-
-    for got in (run(rows, cols), run(rows, cols, valid=0)):
-        for a, bb in zip(got, plain):
-            assert torch.equal(a, bb)
-    # maxima misplaced by a few pixels (still valid hints: the bound is taken for the box actually named)
-    r2 = (rows + 2).clamp(max=h - 1)
-    c2 = (cols - 1).clamp(min=0)
-    got = run(r2, c2)
-    close(got[0], plain[0], atol=2e-4, rtol=1e-5)
-    close(got[1], plain[1], atol=1e-5, rtol=1e-4)
-    torch.cuda.synchronize()
-
-
-@pytest.mark.gpu
-def test_head_softmax_emits_decode_hints(lpb, dev):
-    """The fused two-pass softmax of the bf16 head writes per-plane decode hints: a (near-)maximal pixel and EXACTLY the
-    largest stored probability outside the box around it; forward_with_keypoints with hints equals the unhinted decode."""
-    from lightning_pose_b200 import ops
-    from lightning_pose_b200._lib import lib
-
-    head = _rand_head("resnet50", 2048, 17, gain=6.0, seed=3).to(dev)
-    feats = (torch.randn(5, 2048, 12, 12) * 0.5).bfloat16().to(dev)
-    d1, d2 = list(head.upsampling_layers)[1:]
-    saved, saved14 = lib.lpb_get_tuning(7), lib.lpb_get_tuning(14)
-    try:
-        lib.lpb_set_tuning(7, 0)  # never split: the fused two-pass form also for this small batch
-        lib.lpb_set_tuning(14, 1)  # hints on (off by default: see include/lpb200.h)
-        with torch.no_grad():
-            hm, hints = ops._head_forward_bf16(feats, [d1.weight, d2.weight], [d1.bias, d2.bias], True, want_hints=True)
-            _, kp, cf = head.forward_with_keypoints(feats)
-    finally:
-        lib.lpb_set_tuning(7, saved)
-        lib.lpb_set_tuning(14, saved14)
-    hints = hints.view(5, 17, 4)
-    assert bool((hints[..., 3] == 1).all())
-    rows, cols = hints[..., 0].long(), hints[..., 1].long()
-    at = hm[torch.arange(5, device=dev).view(5, 1), torch.arange(17, device=dev).view(1, 17), rows, cols]
-    mx = hm.amax(dim=(2, 3))
-    assert bool((at >= 0.7 * mx).all()), (at / mx).min()  # the arg max is exact up to 2^-9 of the LOGIT (it rides in the low mantissa bits of the softmax shift)
-    hout = hints[..., 2].contiguous().view(torch.float32)
-    assert torch.equal(hout, _torch_hints(hm, rows, cols))
-    xy, conf, _ = ops._decode_fwd(hm, 2, 1000.0)
-    close(kp, xy.reshape(5, -1), atol=2e-4, rtol=1e-5)
-    close(cf, conf, atol=1e-5, rtol=1e-4)
