@@ -161,7 +161,9 @@ int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes);
  *   NULL when the head returns logits.
  * dfeat [B, C, H, W] bf16 or NULL (frozen backbone); dw1 [C/4, c1, 3, 3], db1 [c1], dw2 [c1, c2, 3, 3],
  * db2 [c2] fp32 (overwritten).  One-deconv heads: w2 = dw2 = db2 = NULL, c2 = 0 (output [B, c1, 4H, 4W]).
- * Feature maps: H even, W in {4, 8, 12, 16, 24, 32}.  workspace: lpb_head_bwd_bf16_workspace_bytes(). */
+ * Shapes: the forward's channel limits, and feature maps with H even, W in {4, 8, 12, 16, 24, 32}; both entries return
+ * LPB_ERR_UNSUPPORTED for any other shape, so lpb_head_bwd_bf16_workspace_bytes (which needs no GPU) tells whether a
+ * head can train on this path.  workspace: lpb_head_bwd_bf16_workspace_bytes() bytes. */
 int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes);
 int lpb_head_bwd_bf16(const float* g_out, const float* probs, const float* win, const int32_t* win_meta,
                       const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H,

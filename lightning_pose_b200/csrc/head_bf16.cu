@@ -31,16 +31,9 @@
 
 namespace lpb {
 
-constexpr int HB_NCOLS = 80;         // 4 classes x 20 (>= 17 keypoints), multiple of 16
-constexpr int HB_CLS = 20;
-constexpr int HB_KSTAGE = 32;        // channels per pipeline stage (4 K-chunks of 8)
-constexpr int HB_BSTAGE_BYTES = 4 * 4 * HB_NCOLS * 16;  // [shift][kchunk][80 rows][16 B]
-
 // ---- everything a head call prepares, in one launch (head_prep.cuh) -------------------------------------------
 // forward packs: W[Cin][Cout][3][3] (fp32) -> B[stage][shift][kchunk][80][8] bf16; a non-null bias rides on input
 // channel `Cin` (the constant-one channel of the mid activations; shift (0,0) only, which every output class uses once)
-constexpr int PREP_GB_K = 80, PREP_GB_KC = 10, PREP_GB_CLS = 20;  // class-major K of the gradient operands (head_bwd_bf16.cu)
-
 __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ PrepJobs J) {
   const long long tid0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
 #pragma unroll
@@ -49,18 +42,18 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
     const float* w = J.fpack[j].w;
     const float* bias = J.fpack[j].bias;
     const int Cin = J.fpack[j].Cin, Cout = J.fpack[j].Cout;
-    const long long total = (long long)J.fpack[j].nstages * 4 * 4 * HB_NCOLS * 8;
+    const long long total = (long long)J.fpack[j].nstages * 4 * 4 * HEAD_NCOLS * 8;
     for (long long i = tid0; i < total; i += nthr) {
       const int e = (int)(i & 7);
       long long r = i >> 3;
-      const int nrow = (int)(r % HB_NCOLS);
-      r /= HB_NCOLS;
+      const int nrow = (int)(r % HEAD_NCOLS);
+      r /= HEAD_NCOLS;
       const int kc = (int)(r & 3);
       r >>= 2;
       const int sh = (int)(r & 3);
       const int st = (int)(r >> 2);
-      const int c = st * HB_KSTAGE + kc * 8 + e;
-      const int cls = nrow / HB_CLS, o = nrow % HB_CLS;
+      const int c = st * HEAD_KSTAGE + kc * 8 + e;
+      const int cls = nrow / HEAD_CLS, o = nrow % HEAD_CLS;
       const int py = cls >> 1, px = cls & 1, dm = sh >> 1, dn = sh & 1;
       float v = 0.f;
       if (c < Cin && o < Cout && tap_nonzero(cls, sh)) {
@@ -78,19 +71,19 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
     if (!J.dpack[j].out) continue;
     const float* w = J.dpack[j].w;
     const int Cin = J.dpack[j].Cin, Cout = J.dpack[j].Cout, rpt = J.dpack[j].rows_per_tile;
-    const long long total = (long long)J.dpack[j].ntiles * 4 * PREP_GB_KC * rpt * 8;
+    const long long total = (long long)J.dpack[j].ntiles * 4 * HEAD_KC * rpt * 8;
     for (long long i = tid0; i < total; i += nthr) {
       const int e = (int)(i & 7);
       long long r = i >> 3;
       const int row = (int)(r % rpt);
       r /= rpt;
-      const int kc = (int)(r % PREP_GB_KC);
-      r /= PREP_GB_KC;
+      const int kc = (int)(r % HEAD_KC);
+      r /= HEAD_KC;
       const int sh = (int)(r & 3);
       const int tile = (int)(r >> 2);
       const int c = tile * rpt + row;
       const int k = kc * 8 + e;
-      const int cls = k / PREP_GB_CLS, o = k % PREP_GB_CLS;
+      const int cls = k / HEAD_CLS, o = k % HEAD_CLS;
       const int py = cls >> 1, px = cls & 1, dm = sh >> 1, dn = sh & 1;
       float v = 0.f;
       if (c < Cin && o < Cout && tap_nonzero(cls, sh)) {
@@ -199,7 +192,7 @@ __host__ inline K1aGeom make_k1a_geom(int H, int W) {
 
 struct K1aParams {
   CUtensorMap feat;           // features [B * C][H * W] bf16, box {k.box, 128}: one stage's channels of an item's rows
-  const __nv_bfloat16* wpk;   // packed weights [nstages][HB_BSTAGE_BYTES]
+  const __nv_bfloat16* wpk;   // packed weights [nstages][HEAD_BSTAGE_BYTES]
   const float* bias;          // [c1]
   __nv_bfloat16* mid;         // [B][4][Lmid.rows][8]  padded row layout of the next layer's input (row_layout.cuh)
   __nv_bfloat16* xs;          // [B][C/32][Lxs.rows][8] (training form): shuffled features in the padded row layout
@@ -224,13 +217,13 @@ template <int MT>
 __device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* stage_base, int stage_bytes, int a_stage_bytes,
                                              uint64_t* full, uint64_t* empty, int m0, int lane) {
   const K1aGeom& k = P.k;
-  const uint32_t lbo_a = k.rows_alloc * 16, lbo_b = HB_NCOLS * 16;
+  const uint32_t lbo_a = k.rows_alloc * 16, lbo_b = HEAD_NCOLS * 16;
   const int nitems = P.B * k.G;
   int it0 = 0;
   for (int item = blockIdx.x; item < nitems; item += gridDim.x, it0 += P.nstages) {
     int b, f0, nb;
     k1a_band(k, item, b, f0, nb);
-    float acc[MT > 0 ? MT : 1][HB_NCOLS / 8][4];
+    float acc[MT > 0 ? MT : 1][HEAD_NCOLS / 8][4];
     mma::zero(acc);
     for (int st = 0; st < P.nstages; ++st) {
       const int it = it0 + st, s = it % K1A_STAGES;
@@ -255,9 +248,9 @@ __device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* 
       const int rows_mid = P.Lmid.rows;
       static_for<0, (MT + 1) / 2>([&](auto pc) {
         constexpr int M0 = 2 * decltype(pc)::value;
-        float d[HB_NCOLS];
+        float d[HEAD_NCOLS];
 #pragma unroll
-        for (int nt = 0; nt < HB_NCOLS / 8; ++nt) mma::rows8_at<M0>(acc, nt, &d[nt * 8], lane);
+        for (int nt = 0; nt < HEAD_NCOLS / 8; ++nt) mma::rows8_at<M0>(acc, nt, &d[nt * 8], lane);
         const int row = 16 * (m0 + M0) + lane;  // band raster row
         const int ml = row / k.P, n = row - ml * k.P;
         if ((M0 + 1 < MT || lane < 16) && ml < 2 * nb && n < k.Wi) {
@@ -276,8 +269,8 @@ __device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* 
                 for (int hh = 0; hh < 2; ++hh) {
                   const int ch = kc * 8 + 2 * e2 + hh;  // compile-time
                   float val = 0.f;
-                  if (ch < HB_CLS) {
-                    if (ch < P.c1) val = d[cls * HB_CLS + ch] + __ldg(P.bias + ch);
+                  if (ch < HEAD_CLS) {
+                    if (ch < P.c1) val = d[cls * HEAD_CLS + ch] + __ldg(P.bias + ch);
                     else if (ch == P.c1) val = 1.0f;
                   } else if (ch == P.c1) {
                     val = 1.0f;
@@ -302,8 +295,8 @@ __global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const
   extern __shared__ __align__(1024) unsigned char smem[];
   const K1aGeom& k = P.k;
   const int a_stage_bytes = 4 * k.rows_alloc * 16;
-  const int stage_bytes = a_stage_bytes + HB_BSTAGE_BYTES;
-  const int raw_bytes = 4 * HB_KSTAGE * k.box * 2;  // 128 source channels x the item's staged positions
+  const int stage_bytes = a_stage_bytes + HEAD_BSTAGE_BYTES;
+  const int raw_bytes = 4 * HEAD_KSTAGE * k.box * 2;  // 128 source channels x the item's staged positions
   unsigned char* stage_base = smem;
   unsigned char* raw_base = smem + K1A_STAGES * stage_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(raw_base + K1A_STAGES * raw_bytes);
@@ -429,16 +422,16 @@ __global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const
         k1a_band(k, item_of(it), b, f0, nb);
         const int st = it % P.nstages;
         mbar_expect_tx(&raw_full[r], (uint32_t)raw_bytes);  // out-of-range elements (past the frame) land as zeros
-        tma_load_2d(raw_base + r * raw_bytes, &P.feat, f0 * k.W, b * P.C + st * 4 * HB_KSTAGE, &raw_full[r]);
+        tma_load_2d(raw_base + r * raw_bytes, &P.feat, f0 * k.W, b * P.C + st * 4 * HEAD_KSTAGE, &raw_full[r]);
       };
       if (total_it > 0) issue_raw(0);
       for (int it = 0; it < total_it; ++it) {
         if (it + 1 < total_it) issue_raw(it + 1);
         const int s = it % K1A_STAGES, st = it % P.nstages;
         mbar_wait(&empty[s], ((it / K1A_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&full[s], HB_BSTAGE_BYTES);
+        mbar_expect_tx(&full[s], HEAD_BSTAGE_BYTES);
         bulk_g2s(stage_base + s * stage_bytes + a_stage_bytes,
-                 reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * HB_BSTAGE_BYTES, HB_BSTAGE_BYTES, &full[s]);
+                 reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * HEAD_BSTAGE_BYTES, HEAD_BSTAGE_BYTES, &full[s]);
       }
     }
   } else if (XS && warp == K1A_LOADER + 1) {
@@ -473,7 +466,7 @@ __global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const
 }
 
 static size_t k1a_smem_bytes(const K1aGeom& k) {
-  return (size_t)K1A_STAGES * (4 * k.rows_alloc * 16 + HB_BSTAGE_BYTES) + (size_t)K1A_STAGES * 4 * HB_KSTAGE * k.box * 2 + 128 + K1A_ZROWS * 16;
+  return (size_t)K1A_STAGES * (4 * k.rows_alloc * 16 + HEAD_BSTAGE_BYTES) + (size_t)K1A_STAGES * 4 * HEAD_KSTAGE * k.box * 2 + 128 + K1A_ZROWS * 16;
 }
 
 // features [B][C][HW] bf16 viewed as [B * C][HW]; box = {box_px positions, 128 channels}, box_px <= HW (make_k1a_geom)
@@ -482,7 +475,7 @@ static bool make_feat_tensor_map(CUtensorMap* tm, const void* feat, int B, int C
   if (!encode || (HW * 2) % 16 != 0 || (box_px * 2) % 16 != 0 || box_px > 256 || box_px > HW) return false;
   const cuuint64_t gdim[2] = {(cuuint64_t)HW, (cuuint64_t)B * C};
   const cuuint64_t gstride[1] = {(cuuint64_t)HW * 2};  // bytes, dim 1
-  const cuuint32_t box[2] = {(cuuint32_t)box_px, 4 * HB_KSTAGE};
+  const cuuint32_t box[2] = {(cuuint32_t)box_px, 4 * HEAD_KSTAGE};
   const cuuint32_t estr[2] = {1, 1};
   return encode(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(feat), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
@@ -517,7 +510,7 @@ extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan
   using namespace lpb;
   LPB_REQUIRE(plan, "head_bf16_plan: null pointer");
   LPB_REQUIRE(C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && (H * W) % 8 == 0 && c1 >= 1 && c2 >= 0, "head_bf16_plan: bad shape");
-  LPB_REQUIRE(c2 == 0 ? c1 <= HB_CLS : (c1 < HB_CLS && c2 <= HB_CLS), "head_bf16_plan: channel counts %d/%d exceed %d", c1, c2, HB_CLS);
+  LPB_REQUIRE(c2 == 0 ? c1 <= HEAD_CLS : (c1 < HEAD_CLS && c2 <= HEAD_CLS), "head_bf16_plan: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
   int max_smem, sms;
   device_limits(&max_smem, &sms);
   plan[0] = head_fast_path(C, H, W, c2, max_smem) ? 1 : 0;
@@ -528,7 +521,6 @@ extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan
   return LPB_OK;
 }
 
-// workspace layout: [packed w1][packed w2][mid activations (padded row layout; two-deconv heads only)]
 extern "C" int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes) {
   using namespace lpb;
   LPB_REQUIRE(bytes && B >= 0 && C >= 32 && C % 32 == 0 && H >= 1 && W >= 1, "head_bf16_saved_bytes: bad arguments");
@@ -540,11 +532,7 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
   using namespace lpb;
   LPB_REQUIRE(bytes, "head_bf16_workspace_bytes: null pointer");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_bf16_workspace_bytes: bad shape");
-  const size_t w1 = (size_t)(C / 4 / HB_KSTAGE) * HB_BSTAGE_BYTES, w2 = HB_BSTAGE_BYTES;
-  const size_t mid = c2 > 0 ? (size_t)B * 4 * make_row_layout(4 * H, 4 * W).rows * 16 : 0;
-  // + the split softmax's per-band statistics of the LAST layer
-  const size_t part = c2 > 0 ? convt_rows_partials_bytes(B, 4 * H, 4 * W) : convt_rows_partials_bytes(B, 2 * H, 2 * W);
-  *bytes = w1 + w2 + mid + ((part + 255) & ~(size_t)255);
+  *bytes = head_fwd_layout(B, C, H, W, c2).total;
   return LPB_OK;
 }
 
@@ -556,8 +544,8 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   LPB_REQUIRE(c2 == 0 || (w2 && b2), "head_fwd_bf16: a two-deconv head needs w2 and b2");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "head_fwd_bf16: bad feature shape C=%d H=%d W=%d", C, H, W);
   LPB_REQUIRE((H * W) % 8 == 0, "head_fwd_bf16: H*W must be a multiple of 8 (got %d)", H * W);
-  LPB_REQUIRE(c2 == 0 ? (c1 >= 1 && c1 <= HB_CLS) : (c1 >= 1 && c1 < HB_CLS && c2 >= 1 && c2 <= HB_CLS),
-              "head_fwd_bf16: channel counts %d/%d exceed %d", c1, c2, HB_CLS);
+  LPB_REQUIRE(c2 == 0 ? (c1 >= 1 && c1 <= HEAD_CLS) : (c1 >= 1 && c1 < HEAD_CLS && c2 >= 1 && c2 <= HEAD_CLS),
+              "head_fwd_bf16: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
   if (B == 0) return LPB_OK;
   int max_smem = 0, sms = 0;
   device_limits(&max_smem, &sms);
@@ -572,13 +560,14 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     set_error("head_fwd_bf16: cannot encode the feature tensor map (features must be 16-byte aligned)");
     return LPB_ERR_INVALID;
   }
-  const int nst = C / 4 / HB_KSTAGE;
+  const int nst = C / 4 / HEAD_KSTAGE;
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const RowLayout Lxs = make_row_layout(2 * H, 2 * W), Lmid = make_row_layout(4 * H, 4 * W);
-  __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws);
-  __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + (size_t)nst * HB_BSTAGE_BYTES);
-  __nv_bfloat16* mid = reinterpret_cast<__nv_bfloat16*>(ws + (size_t)(nst + 1) * HB_BSTAGE_BYTES);
-  float* partials = reinterpret_cast<float*>(ws + (size_t)(nst + 1) * HB_BSTAGE_BYTES + (c2 > 0 ? (size_t)B * 4 * Lmid.rows * 16 : 0));
+  const HeadFwdLayout wl = head_fwd_layout(B, C, H, W, c2);
+  __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.w1);
+  __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.w2);
+  __nv_bfloat16* mid = reinterpret_cast<__nv_bfloat16*>(ws + wl.mid);
+  float* partials = reinterpret_cast<float*>(ws + wl.partials);
   {
     // one launch: both operand packs + the pad rows of the fresh row-layout buffers (k1a writes every row of the saved
     // copy itself; the banded path's shuffle kernel writes its own pads)

@@ -14,6 +14,7 @@
 
 #include "../../include/lpb200.h"
 #include "head_prep.cuh"
+#include "head_rows.cuh"
 #include <cstring>
 
 #include "lpb_common.cuh"
@@ -22,10 +23,6 @@
 #include "mma_sm90.cuh"
 
 namespace lpb {
-
-constexpr int GB_CLS = 20;            // class stride in K
-constexpr int GB_K = 4 * GB_CLS;      // 80
-constexpr int GB_KC = GB_K / 8;       // 10 K-chunks
 
 // ---- gradient front end: everything upstream of the second deconv's output, fused into the G2 writer --------
 // The gradient w.r.t. the head output arrives as a sum of
@@ -115,9 +112,9 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
                                                                __nv_bfloat16* __restrict__ G, RowLayout L) {
   const int b = blockIdx.x / ctas_per_frame, t0 = (blockIdx.x - b * ctas_per_frame) * G2B_THREADS, t = t0 + threadIdx.x;
   const int Wo = 2 * Wi, Ho = 2 * Hi;
-  __shared__ float sdot[GB_CLS];
+  __shared__ float sdot[HEAD_CLS];
   __shared__ unsigned sov;
-  if (threadIdx.x < GB_CLS) {
+  if (threadIdx.x < HEAD_CLS) {
     float d = 0.f;
     int4 mt = make_int4(0, 0, 0, 0);
     if (threadIdx.x < C) {
@@ -130,7 +127,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
     }
     sdot[threadIdx.x] = d;
     if (HAS_OV) {
-      const unsigned bov = __ballot_sync((1u << GB_CLS) - 1, mt.z == 2);
+      const unsigned bov = __ballot_sync((1u << HEAD_CLS) - 1, mt.z == 2);
       if (threadIdx.x == 0) sov = bov;
     }
   }
@@ -142,9 +139,9 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
     const int y = 2 * m + py, x = 2 * n;
     const size_t off0 = (((size_t)b * C) * Ho + y) * Wo + x;
     const size_t pstride = (size_t)Ho * Wo;
-    float2 pv[GB_CLS], gv[GB_CLS];
+    float2 pv[HEAD_CLS], gv[HEAD_CLS];
 #pragma unroll
-    for (int o = 0; o < GB_CLS; ++o) {
+    for (int o = 0; o < HEAD_CLS; ++o) {
       pv[o] = make_float2(0.f, 0.f);
       gv[o] = make_float2(0.f, 0.f);
       if (o < C) {
@@ -155,7 +152,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
     if (HAS_OV && sov) {  // uniform per frame
       const unsigned ovm = sov;
 #pragma unroll
-      for (int o = 0; o < GB_CLS; ++o) {
+      for (int o = 0; o < HEAD_CLS; ++o) {
         if (o < C && ((ovm >> o) & 1u)) {
           const float2 u = __ldg(reinterpret_cast<const float2*>(S.gov + off0 + o * pstride));
           gv[o].x += u.x, gv[o].y += u.y;
@@ -164,7 +161,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
     }
     if (HAS_P) {
 #pragma unroll
-      for (int o = 0; o < GB_CLS; ++o) {
+      for (int o = 0; o < HEAD_CLS; ++o) {
         const float d = sdot[o];
         gv[o].x = pv[o].x * (gv[o].x - d);
         gv[o].y = pv[o].y * (gv[o].y - d);
@@ -177,12 +174,12 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
 #pragma unroll
       for (int e2 = 0; e2 < 4; ++e2) {
         const int k0 = ch * 8 + 2 * e2, k1 = k0 + 1;  // 0..39 within this py
-        const float f0 = k0 < GB_CLS ? gv[k0].x : gv[k0 - GB_CLS].y;
-        const float f1 = k1 < GB_CLS ? gv[k1].x : gv[k1 - GB_CLS].y;
+        const float f0 = k0 < HEAD_CLS ? gv[k0].x : gv[k0 - HEAD_CLS].y;
+        const float f1 = k1 < HEAD_CLS ? gv[k1].x : gv[k1 - HEAD_CLS].y;
         __nv_bfloat162 h2 = __floats2bfloat162_rn(f0, f1);
         pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
       }
-      *reinterpret_cast<uint4*>(G + ((((size_t)b * GB_KC + 5 * py + ch) * L.rows) + L.lead + (size_t)m * L.Pp + n) * 8) =
+      *reinterpret_cast<uint4*>(G + ((((size_t)b * HEAD_KC + 5 * py + ch) * L.rows) + L.lead + (size_t)m * L.Pp + n) * 8) =
           make_uint4(pk[0], pk[1], pk[2], pk[3]);
     }
   }
@@ -211,8 +208,8 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
       const int x = mt.y + lane;
       const bool xin = (unsigned)x < (unsigned)Wo;
       // k = cls * 20 + o with cls = 2 (y & 1) + (x & 1): the K-chunk / element of this lane for even and odd rows
-      const int kx = (x & 1) * GB_CLS + o;
-      __nv_bfloat16* gcol = G + ((size_t)b * GB_KC * L.rows + L.lead + (x >> 1)) * 8;
+      const int kx = (x & 1) * HEAD_CLS + o;
+      __nv_bfloat16* gcol = G + ((size_t)b * HEAD_KC * L.rows + L.lead + (x >> 1)) * 8;
 #pragma unroll 1
       for (int r0 = 0; r0 < 32; r0 += 8) {
         float gw[8], pv[8], go[8];
@@ -231,7 +228,7 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
           if (!(xin && gw[k] != 0.f && (unsigned)y < (unsigned)Ho)) continue;
           float g = gw[k] + go[k];
           if (HAS_P) g = pv[k] * (g - dot);
-          const int kk = kx + 2 * GB_CLS * (y & 1);
+          const int kk = kx + 2 * HEAD_CLS * (y & 1);
           gcol[((size_t)(kk >> 3) * L.rows + (size_t)(y >> 1) * L.Pp) * 8 + (kk & 7)] = __float2bfloat16_rn(g);
         }
       }
@@ -265,7 +262,7 @@ struct B2dParams {
   const __nv_bfloat16* wpk;   // [4][10][32][8]
   __nv_bfloat16* G1;          // [B][10][L1.rows][8] padded row layout of the (Hi/2 x Wi/2) grid
   RowLayout L2, L1;
-  float* db1_part;            // [gridDim.x * 4 MMA warps][GB_CLS]: each warp's bias-gradient sum (reduced in a fixed order)
+  float* db1_part;            // [gridDim.x * 4 MMA warps][HEAD_CLS]: each warp's bias-gradient sum (reduced in a fixed order)
   int B, Hi, Wi, c1;
   int R2;                     // image rows per chunk
 };
@@ -275,8 +272,8 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1;
   const int LEAD = Pp + 1;  // one zero row + the previous image row
   const int rows_alloc = (LEAD + B2D_TILES * 128 + 7) & ~7;
-  const int a_bytes = GB_KC * rows_alloc * 16;
-  const int w_bytes = 4 * GB_KC * 32 * 16;
+  const int a_bytes = HEAD_KC * rows_alloc * 16;
+  const int w_bytes = 4 * HEAD_KC * 32 * 16;
   unsigned char* As = smem;
   unsigned char* Ws = smem + a_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(Ws + w_bytes);
@@ -311,11 +308,11 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
         // included); the row above the image comes from the layout's zero lead rows.  A short last chunk copies only its
         // own rows (stale rows further down feed accumulator rows the epilogue skips).
         const uint32_t nbytes = (uint32_t)((1 + (min(B2D_ROWS, Hi - y0) + 1) * Pp) * 16);
-        if (lane < GB_KC) {
-          if (lane == 0) mbar_expect_tx(a_full, GB_KC * nbytes);
-          __syncwarp((1u << GB_KC) - 1);
+        if (lane < HEAD_KC) {
+          if (lane == 0) mbar_expect_tx(a_full, HEAD_KC * nbytes);
+          __syncwarp((1u << HEAD_KC) - 1);
           bulk_g2s(As + (size_t)lane * rows_alloc * 16,
-                   P.G2 + (((size_t)b * GB_KC + lane) * P.L2.rows + P.L2.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, a_full);
+                   P.G2 + (((size_t)b * HEAD_KC + lane) * P.L2.rows + P.L2.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, a_full);
         }
       }
     }
@@ -324,9 +321,9 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
     const uint32_t lbo_a = rows_alloc * 16, lbo_b = 32 * 16;
     const uint32_t a0 = smem_u32(As), b0 = smem_u32(Ws);
     mbar_wait(w_full, 0);
-    float dbs[GB_CLS];
+    float dbs[HEAD_CLS];
 #pragma unroll
-    for (int o = 0; o < GB_CLS; ++o) dbs[o] = 0.f;
+    for (int o = 0; o < HEAD_CLS; ++o) dbs[o] = 0.f;
     int it = 0;
     for (int b = blockIdx.x; b < P.B; b += gridDim.x) {
       for (int ck = 0; ck < nchunk; ++ck, ++it) {
@@ -341,9 +338,9 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
             for (int sh = 0; sh < 4; ++sh) {
               const int shift_rows = (sh >> 1) * Pp + (sh & 1);
 #pragma unroll
-              for (int k16 = 0; k16 < GB_K / 16; ++k16) {
+              for (int k16 = 0; k16 < HEAD_NCOLS / 16; ++k16) {
                 if (k16 < sh) continue;  // all-zero weight chunks of this shift (see b3a)
-                mma::kstep(acc, a0 + (2 * k16) * lbo_a + (LEAD + t * 128 + 32 * q - shift_rows) * 16, lbo_a, b0 + (sh * GB_KC + 2 * k16) * lbo_b,
+                mma::kstep(acc, a0 + (2 * k16) * lbo_a + (LEAD + t * 128 + 32 * q - shift_rows) * 16, lbo_a, b0 + (sh * HEAD_KC + 2 * k16) * lbo_b,
                            lbo_b, lane);
               }
             }
@@ -355,12 +352,12 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
           if (ml < nrow && n < Wi) {
             const int y = y0 + ml;
             const int row1 = P.L1.lead + (y >> 1) * P.L1.Pp + (n >> 1);
-            const int k0 = GB_CLS * (((y & 1) << 1) | (n & 1));
+            const int k0 = HEAD_CLS * (((y & 1) << 1) | (n & 1));
 #pragma unroll
-            for (int o = 0; o < GB_CLS; ++o)
+            for (int o = 0; o < HEAD_CLS; ++o)
               if (o < P.c1) dbs[o] += d[o];
 #pragma unroll
-            for (int i = 0; i < GB_CLS / 4; ++i) {
+            for (int i = 0; i < HEAD_CLS / 4; ++i) {
               uint32_t pk[2];
 #pragma unroll
               for (int e2 = 0; e2 < 2; ++e2) {
@@ -369,7 +366,7 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
                 pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
               }
               const int k = k0 + 4 * i;
-              *reinterpret_cast<uint2*>(P.G1 + (((size_t)b * GB_KC + (k >> 3)) * P.L1.rows + row1) * 8 + (k & 7)) = make_uint2(pk[0], pk[1]);
+              *reinterpret_cast<uint2*>(P.G1 + (((size_t)b * HEAD_KC + (k >> 3)) * P.L1.rows + row1) * 8 + (k & 7)) = make_uint2(pk[0], pk[1]);
             }
           }
         }
@@ -377,9 +374,9 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
         if (lane == 0) mbar_arrive(a_empty);
       }
     }
-    float* part = P.db1_part + ((size_t)blockIdx.x * 4 + q) * GB_CLS;
+    float* part = P.db1_part + ((size_t)blockIdx.x * 4 + q) * HEAD_CLS;
 #pragma unroll
-    for (int o = 0; o < GB_CLS; ++o) {
+    for (int o = 0; o < HEAD_CLS; ++o) {
       const float s = warp_sum(dbs[o]);
       if (lane == 0) part[o] = s;
     }
@@ -422,8 +419,8 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1, LEAD = Pp + 1;
   const int Hh = P.Hh, nbands = (Hi + Hh - 1) / Hh;
   const int rows_alloc = (LEAD + P.ncols + 7) & ~7;
-  const int g_bytes = GB_KC * rows_alloc * 16;
-  const int w_bytes = 4 * GB_KC * 128 * 16;
+  const int g_bytes = HEAD_KC * rows_alloc * 16;
+  const int w_bytes = 4 * HEAD_KC * 128 * 16;
   unsigned char* Gs = smem;                 // [2 stages][10][rows_alloc][16 B]
   unsigned char* Ws = smem + 2 * g_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(Ws + w_bytes);
@@ -461,11 +458,11 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
         // one copy per K-chunk: the zero entry before image row y0 - 1, that row (zero lead rows of the layout when
         // y0 = 0), and the band's rows, zero columns included
         const uint32_t nbytes = (uint32_t)((1 + (hb + 1) * Pp) * 16);
-        if (lane < GB_KC) {
-          if (lane == 0) mbar_expect_tx(&g_full[st], GB_KC * nbytes);
-          __syncwarp((1u << GB_KC) - 1);
+        if (lane < HEAD_KC) {
+          if (lane == 0) mbar_expect_tx(&g_full[st], HEAD_KC * nbytes);
+          __syncwarp((1u << HEAD_KC) - 1);
           bulk_g2s(Gs + (size_t)st * g_bytes + (size_t)lane * rows_alloc * 16,
-                   P.G1 + (((size_t)b * GB_KC + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, &g_full[st]);
+                   P.G1 + (((size_t)b * HEAD_KC + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, &g_full[st]);
         }
       }
   } else if (warp >= 2) {
@@ -501,12 +498,12 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
               for (int sh = 0; sh < 4; ++sh) {
                 const int shift_rows = (sh >> 1) * Pp + (sh & 1);
 #pragma unroll
-                for (int k16 = 0; k16 < GB_K / 16; ++k16) {
+                for (int k16 = 0; k16 < HEAD_NCOLS / 16; ++k16) {
                   // K = (cls, o), cls = 2 py + px at stride 20: shift (dm, dn) has no tap for classes with py < dm or px < dn,
                   // so its packed weights are zero for k < 20 (dn), k < 40 (dm), k < 60 (both): the 16-wide chunks k16 < sh
                   // are all-zero and skipped (14 of 20 remain)
                   if (k16 < sh) continue;
-                  mma::kstep(acc, w0 + ((sh * GB_KC + 2 * k16) * 128 + 32 * q) * 16, lbo_w,
+                  mma::kstep(acc, w0 + ((sh * HEAD_KC + 2 * k16) * 128 + 32 * q) * 16, lbo_w,
                              g0 + (2 * k16) * lbo_g + (LEAD - shift_rows + col0) * 16, lbo_g, lane);
                 }
               }
@@ -749,7 +746,7 @@ template <int NT>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_constant__ WgParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1, R = P.R, KR = P.KR, XR = P.XR;
-  const int g_bytes = GB_KC * KR * 16, x_bytes = P.kcx * XR * 16;
+  const int g_bytes = HEAD_KC * KR * 16, x_bytes = P.kcx * XR * 16;
   unsigned char* Gs = smem;
   unsigned char* Xs = smem + 2 * g_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + P.smem_bytes - 64);
@@ -779,11 +776,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
       mbar_wait(&empty[s], ((j >> 1) & 1) ^ 1);
       // one copy per K-chunk: R image rows of G; R + 1 rows of X (the row below is the shifts' halo)
       const uint32_t gbytes = (uint32_t)(R * Pp * 16), xbytes = (uint32_t)((R + 1) * Pp * 16);
-      if (lane == 0) mbar_expect_tx(&full[s], GB_KC * gbytes + P.kcx * xbytes);
+      if (lane == 0) mbar_expect_tx(&full[s], HEAD_KC * gbytes + P.kcx * xbytes);
       __syncwarp();
       const size_t row0 = (size_t)P.L.lead + (size_t)y0 * Pp;
-      if (lane < GB_KC)
-        bulk_g2s(Gs + (size_t)s * g_bytes + (size_t)lane * KR * 16, P.G + (((size_t)b * GB_KC + lane) * P.L.rows + row0) * 8, gbytes, &full[s]);
+      if (lane < HEAD_KC)
+        bulk_g2s(Gs + (size_t)s * g_bytes + (size_t)lane * KR * 16, P.G + (((size_t)b * HEAD_KC + lane) * P.L.rows + row0) * 8, gbytes, &full[s]);
       if (lane < P.kcx)
         bulk_g2s(Xs + (size_t)s * x_bytes + (size_t)lane * XR * 16,
                  P.X + (((size_t)b * P.kcx_total + (size_t)grp * P.kcx + lane) * P.L.rows + row0) * 8, xbytes, &full[s]);
@@ -805,9 +802,9 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
         const uint32_t a = g0 + s * g_bytes, b = x0 + s * x_bytes;
         for (int k16 = 0; k16 < KR / 16; ++k16) {
           // A (G) fragments of the role's m16 tiles, B (X) fragments of its shifts; each loaded once per K step
-          uint32_t af[GB_K / 16][4], bf[4][NT / 2][4];
+          uint32_t af[HEAD_NCOLS / 16][4], bf[4][NT / 2][4];
 #pragma unroll
-          for (int mt = 0; mt < GB_K / 16; ++mt)
+          for (int mt = 0; mt < HEAD_NCOLS / 16; ++mt)
             if ((mt_set >> mt) & 1u)
               mma::ldsm_x4_t(af[mt], a + k16 * 256 + (uint32_t)(2 * mt + ((lane >> 3) & 1)) * KR * 16 + (uint32_t)((lane >> 4) * 8 + (lane & 7)) * 16);
 #pragma unroll
@@ -841,7 +838,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int k = 16 * mt + gq + 8 * (i >> 1);
-          const int cls = k / GB_CLS, o = k - cls * GB_CLS, py = cls >> 1, px = cls & 1;
+          const int cls = k / HEAD_CLS, o = k - cls * HEAD_CLS, py = cls >> 1, px = cls & 1;
           if (o >= P.Cout || !tap_nonzero(cls, sh)) continue;
           const int ky = py == 0 ? 1 : (dm ? 0 : 2), kx = px == 0 ? 1 : (dn ? 0 : 2);
 #pragma unroll
@@ -873,7 +870,7 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   for (int r = Hi < 8 ? Hi : 8; r >= 1; --r) {
     if (Hi % r) continue;
     const int kr = (r * (Wi + 1) + 15) & ~15, xr = (kr + Wi + 2 + 7) & ~7;
-    if ((size_t)2 * GB_KC * kr * 16 + (size_t)2 * kcx * xr * 16 + 64 <= 225 * 1024) {
+    if ((size_t)2 * HEAD_KC * kr * 16 + (size_t)2 * kcx * xr * 16 + 64 <= 225 * 1024) {
       R = r;
       break;
     }
@@ -896,7 +893,7 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   p.Cin = Cin;
   p.Cout = Cout;
   p.ones_c = ones_c;
-  const size_t body = ((size_t)2 * GB_KC * p.KR * 16 + (size_t)2 * kcx * p.XR * 16 + 15) & ~(size_t)15;
+  const size_t body = ((size_t)2 * HEAD_KC * p.KR * 16 + (size_t)2 * kcx * p.XR * 16 + 15) & ~(size_t)15;
   p.smem_bytes = (int)(body + 64);
   LPB_REQUIRE(p.smem_bytes <= 225 * 1024, "head_bwd_bf16: weight-gradient stages need %d B shared memory", p.smem_bytes);
   const int ngroups = kcx_total / kcx;
@@ -920,8 +917,8 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
 // gradient is bit-reproducible like every other gradient of this file (no atomics).
 __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* __restrict__ G, RowLayout L, float* __restrict__ part) {
   // one CTA per (frame, K-chunk): thread = (row stripe, e)
-  const int b = blockIdx.x / GB_KC, kc = blockIdx.x - b * GB_KC;
-  const __nv_bfloat16* slab = G + ((size_t)b * GB_KC + kc) * (size_t)L.rows * 8;
+  const int b = blockIdx.x / HEAD_KC, kc = blockIdx.x - b * HEAD_KC;
+  const __nv_bfloat16* slab = G + ((size_t)b * HEAD_KC + kc) * (size_t)L.rows * 8;
   const int e = threadIdx.x & 7;
   float acc = 0.f;
   for (int r = L.lead + (threadIdx.x >> 3); r < L.lead + L.Hi * L.Pp; r += 32) acc += __bfloat162float(slab[(size_t)r * 8 + e]);
@@ -935,12 +932,12 @@ __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* _
   }
 }
 
-// one CTA per output channel o: the partials of K entries k = kc * 8 + e with k % GB_CLS == o, in a fixed order
+// one CTA per output channel o: the partials of K entries k = kc * 8 + e with k % HEAD_CLS == o, in a fixed order
 __global__ void __launch_bounds__(256) rows_colsum_reduce_kernel(const float* __restrict__ part, long long n, float* __restrict__ db) {
   const int o = blockIdx.x;
   float acc = 0.f;
   for (long long j = threadIdx.x; j < n; j += 256)
-    if ((int)(j % (GB_KC * 8)) % GB_CLS == o) acc += part[j];
+    if ((int)(j % (HEAD_KC * 8)) % HEAD_CLS == o) acc += part[j];
   __shared__ float red[256];
   red[threadIdx.x] = acc;
   __syncthreads();
@@ -971,30 +968,54 @@ static bool make_dfeat_tensor_map(CUtensorMap* tm, void* dfeat, int B, int C4, i
                 CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-}  // namespace lpb
-
-// workspace: [W1 dgrad pack][W2 dgrad pack][G2][G1][plane dots]   (G2 / G1: padded row layouts, row_layout.cuh);
-// a one-deconv head (c2 = 0) has no W2 pack and no G2: its output gradient is G1 directly
-// fixed-order reduction partials: [layer-1 wgrad][layer-2 wgrad][b2d bias]
-static size_t bwd_partials_bytes(int C, int c1, int c2) {
-  using namespace lpb;
-  const int nkc1 = C / 4 / 8;
-  size_t n = (size_t)wgrad_max_slots(nkc1) * wgrad_part_stride(C / 4, c1);
-  if (c2 > 0) n += (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) + (size_t)B2D_MAX_CTAS * 4 * GB_CLS;
-  return n * sizeof(float);
+// The shapes the backward serves (lpb200.h): H even, W one of the widths b3a_dgrad_kernel is instantiated for, and the
+// forward's channel limits.  LPB_OK, or LPB_ERR_UNSUPPORTED with the message set.
+static int head_bwd_covers(const char* who, int H, int W, int c1, int c2) {
+  const bool width = W == 4 || W == 8 || W == 12 || W == 16 || W == 24 || W == 32;
+  if (H % 2 == 0 && width && (c2 > 0 ? c1 < HEAD_CLS && c2 <= HEAD_CLS : c1 <= HEAD_CLS)) return LPB_OK;
+  set_error("%s: head %dx%d with %d/%d channels outside this build's set (H even, W in {4, 8, 12, 16, 24, 32}, at most %d "
+            "channels per layer, fewer in the first of two)", who, H, W, c1, c2, HEAD_CLS);
+  return LPB_ERR_UNSUPPORTED;
 }
+
+// Byte offsets into the backward's workspace: [W1 dgrad pack][W2 dgrad pack][G2][G1][plane dots, 256-byte rounded] and
+// the fixed-order reduction partials [layer-1 wgrad][layer-2 wgrad][b2d bias].  G2 / G1 are padded row layouts
+// (row_layout.cuh).  A one-deconv head (c2 = 0) has no G2 (its output gradient is G1 directly) but keeps the W2 pack's
+// space, and its partials are [layer-1 wgrad][bias column sums: eight per (frame, K-chunk)].  Members a head does not
+// have are 0.
+struct HeadBwdLayout {
+  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, total;
+};
+static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2) {
+  const int C4 = C / 4;
+  const bool two = c2 > 0;
+  HeadBwdLayout l{};
+  l.wp1 = 0;
+  l.wp2 = l.wp1 + (size_t)((C4 + 127) / 128) * 4 * HEAD_KC * 128 * 16;
+  l.G2 = l.wp2 + (size_t)4 * HEAD_KC * 32 * 16;
+  l.G1 = l.G2 + (two ? (size_t)B * HEAD_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
+  l.ddot = l.G1 + (size_t)B * HEAD_KC * make_row_layout(2 * H, 2 * W).rows * 16;
+  l.part1 = l.ddot + (((size_t)B * (two ? c2 : c1) * 4 + 255) & ~(size_t)255);
+  const size_t part1_end = l.part1 + (size_t)wgrad_max_slots(C4 / 8) * wgrad_part_stride(C4, c1) * sizeof(float);
+  if (two) {
+    l.part2 = part1_end;
+    l.part_db1 = l.part2 + (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) * sizeof(float);
+    l.total = l.part_db1 + (size_t)B2D_MAX_CTAS * 4 * HEAD_CLS * sizeof(float);
+  } else {
+    l.part_cs = part1_end;
+    l.total = l.part_cs + (size_t)B * HEAD_KC * 8 * sizeof(float);
+  }
+  return l;
+}
+
+}  // namespace lpb
 
 extern "C" int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {
   using namespace lpb;
   LPB_REQUIRE(bytes, "head_bwd_bf16_workspace_bytes: null pointer");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_bwd_bf16_workspace_bytes: bad shape");
-  const int C4 = C / 4;
-  const size_t w1 = (size_t)((C4 + 127) / 128) * 4 * GB_KC * 128 * 16, w2 = (size_t)4 * GB_KC * 32 * 16;
-  const size_t g2 = c2 > 0 ? (size_t)B * GB_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0;
-  const size_t g1 = (size_t)B * GB_KC * make_row_layout(2 * H, 2 * W).rows * 16;
-  // (+ a one-deconv head's bias-gradient partials: eight per (frame, K-chunk))
-  *bytes = w1 + w2 + g2 + g1 + (((size_t)B * (c2 > 0 ? c2 : c1) * 4 + 255) & ~(size_t)255) + bwd_partials_bytes(C, c1, c2) +
-           (c2 > 0 ? 0 : (size_t)B * GB_KC * 8 * sizeof(float));
+  if (const int rc = head_bwd_covers("head_bwd_bf16_workspace_bytes", H, W, c1, c2); rc != LPB_OK) return rc;
+  *bytes = head_bwd_layout(B, C, H, W, c1, c2).total;
   return LPB_OK;
 }
 
@@ -1008,12 +1029,8 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   LPB_REQUIRE(!two || (w2 && dw2 && db2), "head_bwd_bf16: a two-deconv head needs w2, dw2, db2");
   LPB_REQUIRE(g_out || win, "head_bwd_bf16: neither a dense gradient nor decode windows given");
   LPB_REQUIRE(!win || (win_meta && g_overflow), "head_bwd_bf16: windows need their meta and overflow buffers");
-  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "head_bwd_bf16: bad feature shape C=%d H=%d W=%d", C, H, W);
-  LPB_REQUIRE(two ? (c1 >= 1 && c1 < GB_CLS && c2 <= GB_CLS) : (c1 >= 1 && c1 <= GB_CLS), "head_bwd_bf16: channel counts %d/%d exceed %d", c1, c2, GB_CLS);
-  if ((W % 4) != 0 || (H % 2) != 0 || !(W == 4 || W == 8 || W == 12 || W == 16 || W == 24 || W == 32)) {
-    set_error("head_bwd_bf16: feature map %dx%d outside this build's epilogue set (H even, W in {4, 8, 12, 16, 24, 32})", H, W);
-    return LPB_ERR_UNSUPPORTED;
-  }
+  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1, "head_bwd_bf16: bad shape C=%d H=%d W=%d c1=%d", C, H, W, c1);
+  if (const int rc = head_bwd_covers("head_bwd_bf16", H, W, c1, c2); rc != LPB_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int C4 = C / 4, Hi1 = 2 * H, Wi1 = 2 * W, Hi2 = 4 * H, Wi2 = 4 * W;
   const int kout = two ? c2 : c1;
@@ -1037,31 +1054,30 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   const RowLayout L2 = make_row_layout(Hi2, Wi2), L1 = make_row_layout(Hi1, Wi1);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const int ntile1 = (C4 + 127) / 128;
-  const size_t w1b = (size_t)ntile1 * 4 * GB_KC * 128 * 16, w2b = (size_t)4 * GB_KC * 32 * 16;
-  const size_t g2b = two ? (size_t)B * GB_KC * L2.rows * 16 : 0, g1b = (size_t)B * GB_KC * L1.rows * 16;
-  __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws);
-  __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + w1b);
-  __nv_bfloat16* G2 = reinterpret_cast<__nv_bfloat16*>(ws + w1b + w2b);
-  __nv_bfloat16* G1 = reinterpret_cast<__nv_bfloat16*>(ws + w1b + w2b + g2b);
-  float* ddot = reinterpret_cast<float*>(ws + w1b + w2b + g2b + g1b);
-  float* part1 = reinterpret_cast<float*>(ws + w1b + w2b + g2b + g1b + ((((size_t)B * kout * 4) + 255) & ~(size_t)255));
-  float* part2 = part1 + (size_t)wgrad_max_slots(C4 / 8) * wgrad_part_stride(C4, c1);
-  float* part_db1 = two ? part2 + (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) : nullptr;
-  float* part_cs = two ? nullptr : part2;  // one-deconv head: the bias partials follow the layer-1 partials
-  // the forward pass's mid activations (head_bf16.cu workspace layout: [packed w1][packed w2][mid])
-  const size_t fwd_mid_off = (size_t)(C4 / 32 + 1) * (4 * 4 * 80 * 16);
-  const __nv_bfloat16* mid = reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + fwd_mid_off);
+  const HeadBwdLayout wl = head_bwd_layout(B, C, H, W, c1, c2);
+  __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.wp1);
+  __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.wp2);
+  __nv_bfloat16* G2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.G2);
+  __nv_bfloat16* G1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.G1);
+  float* ddot = reinterpret_cast<float*>(ws + wl.ddot);
+  float* part1 = reinterpret_cast<float*>(ws + wl.part1);
+  float* part2 = two ? reinterpret_cast<float*>(ws + wl.part2) : nullptr;
+  float* part_db1 = two ? reinterpret_cast<float*>(ws + wl.part_db1) : nullptr;
+  float* part_cs = two ? nullptr : reinterpret_cast<float*>(ws + wl.part_cs);
+  // the forward pass's mid activations
+  const __nv_bfloat16* mid =
+      reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + head_fwd_layout(B, C, H, W, c2).mid);
 
   {
     // one launch: gradient accumulators zeroed, both data-gradient operand packs, pad rows of G2 / G1
     PrepJobs jobs{};
     jobs.dpack[0] = {w1, C4, c1, ntile1, 128, wp1};
-    jobs.pads[0] = {G1, L1, (long long)B * GB_KC};
+    jobs.pads[0] = {G1, L1, (long long)B * HEAD_KC};
     jobs.zero[0] = {dw1, (long long)C4 * c1 * 9};
     jobs.zero[1] = {db1, (long long)c1};
     if (two) {
       jobs.dpack[1] = {w2, c1, c2, 1, 32, wp2};
-      jobs.pads[1] = {G2, L2, (long long)B * GB_KC};
+      jobs.pads[1] = {G2, L2, (long long)B * HEAD_KC};
       jobs.zero[2] = {dw2, (long long)c1 * c2 * 9};
       jobs.zero[3] = {db2, (long long)c2};
     }
@@ -1110,16 +1126,16 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.R2 = (B2D_TILES * 128) / (Wi2 + 1);
     if (p.R2 > Hi2) p.R2 = Hi2;
     const int rows_alloc = (Wi2 + 2 + B2D_TILES * 128 + 7) & ~7;
-    const size_t smem = (size_t)GB_KC * rows_alloc * 16 + (size_t)4 * GB_KC * 32 * 16 + 64;
+    const size_t smem = (size_t)HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 32 * 16 + 64;
     LPB_REQUIRE(smem <= 113 * 1024 && p.R2 >= 1, "head_bwd_bf16: layer-2 width %d too large", Wi2);
     LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int grid = B < 2 * sms ? B : 2 * sms;
     if (grid > B2D_MAX_CTAS) grid = B2D_MAX_CTAS;  // the bias partials' workspace
     b2d_dgrad_kernel<<<grid, B2D_THREADS, smem, s>>>(p);
-    reduce_partials<1>(part_db1, grid * 4, GB_CLS, c1, db1, sms, s);
+    reduce_partials<1>(part_db1, grid * 4, HEAD_CLS, c1, db1, sms, s);
   } else {
-    rows_colsum_kernel<<<(unsigned)(B * GB_KC), 256, 0, s>>>(G1, L1, part_cs);
-    rows_colsum_reduce_kernel<<<(unsigned)c1, 256, 0, s>>>(part_cs, (long long)B * GB_KC * 8, db1);
+    rows_colsum_kernel<<<(unsigned)(B * HEAD_KC), 256, 0, s>>>(G1, L1, part_cs);
+    rows_colsum_reduce_kernel<<<(unsigned)c1, 256, 0, s>>>(part_cs, (long long)B * HEAD_KC * 8, db1);
   }
   // layer 1: weight gradient from the saved shuffled features, data gradient -> d features
   {
@@ -1140,7 +1156,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.Hh = Hh;
     p.ncols = (Hh * (Wi1 + 1) + 15) & ~15;
     const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
-    size_t smem = (size_t)2 * GB_KC * rows_alloc * 16 + (size_t)4 * GB_KC * 128 * 16 + 160;
+    size_t smem = (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
     LPB_REQUIRE(smem <= 225 * 1024, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
     // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit, dfeat is 16-byte
     // aligned and the tensor map encodes; otherwise direct 16-byte stores

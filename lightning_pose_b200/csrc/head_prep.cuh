@@ -15,12 +15,21 @@ namespace lpb {
 __host__ __device__ constexpr bool tap_nonzero(int cls, int sh) {
   return !((cls >> 1) == 0 && (sh >> 1) == 1) && !((cls & 1) == 0 && (sh & 1) == 1);
 }
+
+// The operand format of the 4-shift form, shared by the forward, the backward and the packs below.  The forward GEMMs'
+// columns and the gradient GEMMs' K are class-major: k = cls * HEAD_CLS + o for output channel o.
+constexpr int HEAD_CLS = 20;                                // class stride: output channels per head layer at most (>= 17 keypoints)
+constexpr int HEAD_NCOLS = 4 * HEAD_CLS;                    // 80 class-major columns, a multiple of 16
+constexpr int HEAD_KC = HEAD_NCOLS / 8;                     // 10 K-chunks of 8 in the gradients' class-major K
+constexpr int HEAD_KSTAGE = 32;                             // input channels per forward K stage (4 K-chunks of 8)
+constexpr int HEAD_BSTAGE_BYTES = 4 * 4 * HEAD_NCOLS * 16;  // one stage's packed forward weights [shift][kchunk][80][16 B]
+
 // bit i: the `width` class-major columns [width i, width i + width) of the 80 (cls * 20 + o) hold a non-zero weight for shift sh
 constexpr unsigned nz_tiles(int sh, int width) {
   unsigned m = 0;
-  for (int i = 0; i < 80 / width; ++i)
+  for (int i = 0; i < HEAD_NCOLS / width; ++i)
     for (int k = width * i; k < width * (i + 1); ++k)
-      if (tap_nonzero(k / 20, sh)) m |= 1u << i;
+      if (tap_nonzero(k / HEAD_CLS, sh)) m |= 1u << i;
   return m;
 }
 // per shift: n8 column tiles of the forward GEMMs' B operand, m16 row tiles of the weight gradient's A operand

@@ -1,8 +1,10 @@
-// Shape-generic building blocks of the bf16 head (head_rows_bf16.cu), shared with the C-ABI entry in head_bf16.cu.
+// Shape-generic building blocks of the bf16 head (head_rows_bf16.cu), shared with the C-ABI entry in head_bf16.cu, and
+// the forward's workspace layout, which the backward reads too.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include "head_prep.cuh"
 #include "row_layout.cuh"
 
 namespace lpb {
@@ -35,6 +37,23 @@ inline int convt_rows_bands(int Hi, int Wi) {
   if (R < 1) R = 1;
   return (Hi + R - 1) / R;
 }
-inline size_t convt_rows_partials_bytes(int B, int Hi, int Wi) { return (size_t)B * convt_rows_bands(Hi, Wi) * 20 * 2 * sizeof(float); }
+inline size_t convt_rows_partials_bytes(int B, int Hi, int Wi) { return (size_t)B * convt_rows_bands(Hi, Wi) * HEAD_CLS * 2 * sizeof(float); }
+
+// Byte offsets into the forward's workspace (lpb_head_fwd_bf16): [packed w1][packed w2][mid activations][split-softmax
+// statistics of the last layer].  mid (padded row layout, channel c1 the constant one) exists for two-deconv heads only;
+// the w2 stage is reserved for one-deconv heads as well.  The backward reads mid from here.
+struct HeadFwdLayout {
+  size_t w1, w2, mid, partials, total;
+};
+inline HeadFwdLayout head_fwd_layout(int B, int C, int H, int W, int c2) {
+  HeadFwdLayout l;
+  l.w1 = 0;
+  l.w2 = (size_t)(C / 4 / HEAD_KSTAGE) * HEAD_BSTAGE_BYTES;
+  l.mid = l.w2 + HEAD_BSTAGE_BYTES;
+  l.partials = l.mid + (c2 > 0 ? (size_t)B * 4 * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
+  const size_t part = c2 > 0 ? convt_rows_partials_bytes(B, 4 * H, 4 * W) : convt_rows_partials_bytes(B, 2 * H, 2 * W);
+  l.total = l.partials + ((part + 255) & ~(size_t)255);
+  return l;
+}
 
 }  // namespace lpb

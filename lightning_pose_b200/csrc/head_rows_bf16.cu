@@ -70,9 +70,6 @@ int launch_rows_shuffle(const __nv_bfloat16* feat, int B, int C, int H, int W, _
 }
 
 // ---- banded transposed-convolution GEMM ---------------------------------------------------------------------------
-constexpr int CR_NCOLS = 80;   // 4 classes x 20
-constexpr int CR_CLS = 20;
-constexpr int CR_BSTAGE = 4 * 4 * CR_NCOLS * 16;  // packed weights of one 32-channel stage [shift][kchunk][80][16 B]
 constexpr int CR_THREADS = 320;  // warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue
 constexpr int CR_EPI = 256;
 constexpr int CR_TILES = 2;      // M-tiles per band: a warp's accumulators (CR_TILES x 32 rows x 48 columns) stay in registers
@@ -86,10 +83,10 @@ template <int MODE, int NPL>
 __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_constant__ ConvtRowsParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Pp = P.L.Pp, Wi = P.L.Wi, Hi = P.L.Hi;
-  const int a_bytes = 4 * P.rows_alloc * 16, stage_bytes = a_bytes + CR_BSTAGE;
-  float* stat = reinterpret_cast<float*>(smem + CR_STAGES * stage_bytes);  // [2][CR_CLS][8 warps]
-  float* fin = stat + 2 * CR_CLS * 8;                                       // [CR_CLS][2] = (max * log2 e, 1 / sum)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(fin + 2 * CR_CLS);
+  const int a_bytes = 4 * P.rows_alloc * 16, stage_bytes = a_bytes + HEAD_BSTAGE_BYTES;
+  float* stat = reinterpret_cast<float*>(smem + CR_STAGES * stage_bytes);  // [2][HEAD_CLS][8 warps]
+  float* fin = stat + 2 * HEAD_CLS * 8;                                       // [HEAD_CLS][2] = (max * log2 e, 1 / sum)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(fin + 2 * HEAD_CLS);
   uint64_t* full = bars;       // [2]
   uint64_t* empty = bars + 2;  // [2]
 
@@ -134,8 +131,8 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             unsigned char* As = smem + s * stage_bytes;
             const bool load_b = nst > 1 || it < CR_STAGES;
             if (lane == 0) {
-              mbar_expect_tx(&full[s], 4 * nbytes + (load_b ? CR_BSTAGE : 0));
-              if (load_b) bulk_g2s(As + a_bytes, reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * CR_BSTAGE, CR_BSTAGE, &full[s]);
+              mbar_expect_tx(&full[s], 4 * nbytes + (load_b ? HEAD_BSTAGE_BYTES : 0));
+              if (load_b) bulk_g2s(As + a_bytes, reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * HEAD_BSTAGE_BYTES, HEAD_BSTAGE_BYTES, &full[s]);
             }
             __syncwarp();
             if (lane < 4)
@@ -151,13 +148,13 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
     const float L2E = 1.4426950408889634f;
     const size_t plane_stride = (size_t)Ho * Wo;
     const bool use_bias = P.bias && (MODE == CONVT_ROWS_MID || MODE == CONVT_ROWS_PLANES);  // a per-plane constant does not change a softmax
-    const uint32_t lbo_a = P.rows_alloc * 16, lbo_b = CR_NCOLS * 16;
+    const uint32_t lbo_a = P.rows_alloc * 16, lbo_b = HEAD_NCOLS * 16;
     int it = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int b = PER_BAND ? item / nbands : item;
-      float mx[CR_CLS], sm[CR_CLS];
+      float mx[HEAD_CLS], sm[HEAD_CLS];
 #pragma unroll
-      for (int o = 0; o < CR_CLS; ++o) {
+      for (int o = 0; o < HEAD_CLS; ++o) {
         mx[o] = -1.0e30f;
         sm[o] = 0.f;
       }
@@ -166,11 +163,11 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
         asm volatile("bar.sync 1, 256;" ::: "memory");  // previous item's readers of fin are done
         if (tid - 64 < ncls) {
           const int o = tid - 64;
-          const float* pp = P.partials + ((size_t)b * nbands * CR_CLS + o) * 2;
+          const float* pp = P.partials + ((size_t)b * nbands * HEAD_CLS + o) * 2;
           float M = -1.0e30f;
-          for (int j = 0; j < nbands; ++j) M = fmaxf(M, pp[(size_t)j * CR_CLS * 2]);
+          for (int j = 0; j < nbands; ++j) M = fmaxf(M, pp[(size_t)j * HEAD_CLS * 2]);
           float S = 0.f;
-          for (int j = 0; j < nbands; ++j) S += pp[(size_t)j * CR_CLS * 2 + 1] * fast_exp2((pp[(size_t)j * CR_CLS * 2] - M) * L2E);
+          for (int j = 0; j < nbands; ++j) S += pp[(size_t)j * HEAD_CLS * 2 + 1] * fast_exp2((pp[(size_t)j * HEAD_CLS * 2] - M) * L2E);
           fin[2 * o] = M * L2E;
           fin[2 * o + 1] = 1.0f / S;
         }
@@ -256,8 +253,8 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                         for (int hh = 0; hh < 2; ++hh) {
                           const int ch = kc * 8 + 2 * e2 + hh;  // compile-time
                           float val = 0.f;
-                          if (ch < CR_CLS) {
-                            if (ch < P.cout) val = d[8 * E + px * CR_CLS + ch] + (use_bias ? __ldg(P.bias + ch) : 0.f);
+                          if (ch < HEAD_CLS) {
+                            if (ch < P.cout) val = d[8 * E + px * HEAD_CLS + ch] + (use_bias ? __ldg(P.bias + ch) : 0.f);
                             else if (ch == P.cout) val = 1.0f;
                           } else if (ch == P.cout) {
                             val = 1.0f;
@@ -279,16 +276,16 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                   // ---- pass 0: per-thread online (max, sum) per plane; the rescale is rare after the first tiles ----
                   bool need = false;
 #pragma unroll
-                  for (int o = 0; o < CR_CLS; ++o) {
+                  for (int o = 0; o < HEAD_CLS; ++o) {
                     if (o >= ncls) break;
-                    need |= fmaxf(d[8 * E + o], d[8 * E + CR_CLS + o]) > mx[o];
+                    need |= fmaxf(d[8 * E + o], d[8 * E + HEAD_CLS + o]) > mx[o];
                   }
                   if (__any_sync(0xffffffffu, need && valid)) {
                     if (valid) {
 #pragma unroll
-                      for (int o = 0; o < CR_CLS; ++o) {
+                      for (int o = 0; o < HEAD_CLS; ++o) {
                         if (o >= ncls) break;
-                        const float tm = fmaxf(d[8 * E + o], d[8 * E + CR_CLS + o]);
+                        const float tm = fmaxf(d[8 * E + o], d[8 * E + HEAD_CLS + o]);
                         if (tm > mx[o]) {
                           sm[o] *= fast_exp2((mx[o] - tm) * L2E);
                           mx[o] = tm;
@@ -298,20 +295,20 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                   }
                   if (valid) {
 #pragma unroll
-                    for (int o = 0; o < CR_CLS; ++o) {
+                    for (int o = 0; o < HEAD_CLS; ++o) {
                       if (o >= ncls) break;
                       const float mL = mx[o] * L2E;
-                      sm[o] += fast_exp2(fmaf(d[8 * E + o], L2E, -mL)) + fast_exp2(fmaf(d[8 * E + CR_CLS + o], L2E, -mL));
+                      sm[o] += fast_exp2(fmaf(d[8 * E + o], L2E, -mL)) + fast_exp2(fmaf(d[8 * E + HEAD_CLS + o], L2E, -mL));
                     }
                   }
                 } else if (valid) {
                   // ---- pass 1: normalise and store; (shift, 1 / sum) is one 8-byte shared load per plane ----
 #pragma unroll
-                  for (int o = 0; o < CR_CLS; ++o) {
+                  for (int o = 0; o < HEAD_CLS; ++o) {
                     if (o >= ncls) break;
                     const float2 f = reinterpret_cast<const float2*>(fin)[o];
                     const float p0 = fast_exp2(fmaf(d[8 * E + o], L2E, -f.x)) * f.y;
-                    const float p1 = fast_exp2(fmaf(d[8 * E + CR_CLS + o], L2E, -f.x)) * f.y;
+                    const float p1 = fast_exp2(fmaf(d[8 * E + HEAD_CLS + o], L2E, -f.x)) * f.y;
                     *reinterpret_cast<float2*>(dst) = make_float2(p0, p1);
                     dst += plane_stride;
                   }
@@ -319,10 +316,10 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
               } else {
                 // CONVT_ROWS_PLANES: raw planes (+ bias)
 #pragma unroll
-                for (int o = 0; o < CR_CLS; ++o) {
+                for (int o = 0; o < HEAD_CLS; ++o) {
                   if (o >= ncls) break;
                   const float bo = use_bias ? __ldg(P.bias + o) : 0.f;
-                  const float l0 = d[8 * E + o] + bo, l1 = d[8 * E + CR_CLS + o] + bo;
+                  const float l0 = d[8 * E + o] + bo, l1 = d[8 * E + HEAD_CLS + o] + bo;
                   if (valid) *reinterpret_cast<float2*>(dst + (size_t)o * plane_stride) = make_float2(l0, l1);
                 }
               }
@@ -334,13 +331,13 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
         if ((npass == 2 && pass == 0) || MODE == CONVT_ROWS_SOFTMAX_P0) {
           // merge the online-softmax states: lanes -> warp (shuffles) -> 8 epilogue warps (smem)
 #pragma unroll
-          for (int o = 0; o < CR_CLS; ++o) {
+          for (int o = 0; o < HEAD_CLS; ++o) {
             if (o >= ncls) break;
             const float M = warp_max(mx[o]);
             const float S = warp_sum(sm[o] * fast_exp2((mx[o] - M) * L2E));
             if (lane == 0) {
               stat[o * 8 + ew] = M;
-              stat[(CR_CLS + o) * 8 + ew] = S;
+              stat[(HEAD_CLS + o) * 8 + ew] = S;
             }
           }
           asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -351,9 +348,9 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             for (int i = 1; i < 8; ++i) M = fmaxf(M, stat[o * 8 + i]);
             float S = 0.f;
 #pragma unroll
-            for (int i = 0; i < 8; ++i) S += stat[(CR_CLS + o) * 8 + i] * fast_exp2((stat[o * 8 + i] - M) * L2E);
+            for (int i = 0; i < 8; ++i) S += stat[(HEAD_CLS + o) * 8 + i] * fast_exp2((stat[o * 8 + i] - M) * L2E);
             if constexpr (MODE == CONVT_ROWS_SOFTMAX_P0) {
-              float* pp = P.partials + (((size_t)b * nbands + (item - b * nbands)) * CR_CLS + o) * 2;
+              float* pp = P.partials + (((size_t)b * nbands + (item - b * nbands)) * HEAD_CLS + o) * 2;
               pp[0] = M;
               pp[1] = S;
             } else {
@@ -371,14 +368,14 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
   const int Pp = p.L.Pp;
   LPB_REQUIRE(Pp <= CR_TILES * 128, "head_fwd_bf16: image width %d too large for one band", p.L.Wi);
-  LPB_REQUIRE(p.cout >= 1 && p.cout <= CR_CLS && (p.mode != CONVT_ROWS_MID || p.cout < CR_CLS), "head_fwd_bf16: %d output channels exceed %d",
-              p.cout, CR_CLS);
+  LPB_REQUIRE(p.cout >= 1 && p.cout <= HEAD_CLS && (p.mode != CONVT_ROWS_MID || p.cout < HEAD_CLS), "head_fwd_bf16: %d output channels exceed %d",
+              p.cout, HEAD_CLS);
   p.R = (CR_TILES * 128) / Pp;
   if (p.R > p.L.Hi) p.R = p.L.Hi;
   const int tiles = (p.R * Pp + 127) / 128;
   p.rows_alloc = (tiles * 128 + Pp + 1 + 7) & ~7;
   if (p.rows_alloc < (p.R + 1) * Pp + 8) p.rows_alloc = ((p.R + 1) * Pp + 8 + 7) & ~7;
-  const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + CR_BSTAGE) + (2 * CR_CLS * 8 + 2 * CR_CLS) * sizeof(float) + 64;
+  const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + HEAD_BSTAGE_BYTES) + (2 * HEAD_CLS * 8 + 2 * HEAD_CLS) * sizeof(float) + 64;
   LPB_REQUIRE(smem <= 113 * 1024, "head_fwd_bf16: band stages need %zu B shared memory", smem);
   const int nbands = (p.L.Hi + p.R - 1) / p.R;
   auto run = [&](auto kern, long long nitems) -> int {

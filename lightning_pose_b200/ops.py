@@ -200,23 +200,20 @@ def evaluate_heatmaps_at_location(heatmaps, locs, radius: int = 2):
 # =====================================================================================
 # heatmap head
 # =====================================================================================
-_BWD_WIDTHS = (4, 8, 12, 16, 24, 32)
-
-
 def head_bf16_supported(shape, channels, train: bool) -> bool:
-    """Whether the tensor-core kernels cover this head: feature shape (B, C, H, W), deconv output channels (c1[, c2])."""
-    _, c, h, w = shape
-    n = len(channels)
-    if n not in (1, 2) or c % 128 or (h * w) % 8:
+    """Whether the tensor-core kernels cover this head: feature shape (B, C, H, W), deconv output channels (c1[, c2]).
+
+    The library owns the shape rules: the forward's in ``lpb_head_bf16_plan``, the backward's (``train``) in
+    ``lpb_head_bwd_bf16_workspace_bytes``.  Neither needs a GPU."""
+    b, c, h, w = shape
+    if len(channels) not in (1, 2):
         return False
-    if (n == 1 and channels[0] > 20) or (n == 2 and (channels[0] >= 20 or channels[1] > 20)):
-        return False
+    c1, c2 = channels[0], (channels[1] if len(channels) == 2 else 0)
     plan = C.c_int(0)
-    if lib.lpb_head_bf16_plan(c, h, w, channels[0], channels[1] if n == 2 else 0, C.byref(plan)) != 0:
+    if lib.lpb_head_bf16_plan(c, h, w, c1, c2, C.byref(plan)) != 0:
         return False
-    if train and (h % 2 or w not in _BWD_WIDTHS or (304 // (2 * w + 1)) < 4):
-        return False
-    return True
+    nbytes = C.c_size_t(0)
+    return not train or lib.lpb_head_bwd_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)) == 0
 
 
 def _head_forward_bf16(f, weights, biases, final_softmax, train=False, want_hints=False):

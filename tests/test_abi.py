@@ -217,3 +217,13 @@ def test_head_shape_planner_python_side():
     assert not ok((8, 2048, 12, 12), [20, 17], train=False)      # no room for the ones channel
     assert ok((8, 512, 6, 4), [17, 17], train=False) and not ok((8, 512, 6, 20), [17, 17], train=True)  # width outside the dgrad epilogue set
     assert not ok((8, 384, 15, 16), [17], train=True) and ok((8, 384, 15, 16), [17], train=False)      # odd height: forward only
+
+    # the backward's shape rule lives in the library: its workspace query refuses what lpb_head_bwd_bf16 would refuse
+    from lightning_pose_b200 import _lib
+
+    n = ctypes.c_size_t(0)
+    unsupported = -3  # LPB_ERR_UNSUPPORTED
+    assert _lib.lib.lpb_head_bwd_bf16_workspace_bytes(8, 384, 15, 16, 17, 0, ctypes.byref(n)) == unsupported
+    assert _lib.lib.lpb_head_bwd_bf16_workspace_bytes(8, 512, 6, 20, 17, 17, ctypes.byref(n)) == unsupported
+    for c, h, w, c2 in ((2048, 12, 12, 17), (2048, 16, 16, 17), (384, 16, 16, 0), (384, 24, 24, 0)):  # cfg 2, 5, 3, 4
+        assert _lib.lib.lpb_head_bwd_bf16_workspace_bytes(8, c, h, w, 17, c2, ctypes.byref(n)) == 0 and n.value > 0

@@ -4,7 +4,8 @@ the fast path at config 2 and at shapes on its edges (one, two and three bands, 
 28) with a batch of 2S + 7 frames, so every CTA loops over several items, and checks:
   * the saved copy (filled with 0xFF bytes before the call) byte for byte against a torch construction of the padded row
     layout: every pad row is written by the kernel;
-  * the mid activations in the workspace against the float64 reference at the bf16 tolerance;
+  * the mid activations in the workspace (also filled with 0xFF bytes) against the float64 reference at the bf16
+    tolerance, and their pad rows and zero column as all-zero bits;
   * that a frame alone and the same frame inside the batch give identical bits."""
 import ctypes
 
@@ -17,7 +18,7 @@ import scale_oracle as S
 pytestmark = pytest.mark.gpu
 
 K = 17
-HB_BSTAGE_BYTES = 4 * 4 * 80 * 16  # packed weights of one 32-channel stage (head_bf16.cu)
+HB_BSTAGE_BYTES = 4 * 4 * 80 * 16  # packed weights of one 32-channel stage (head_prep.cuh)
 
 # (C, H, W) -> bands as (first feature row, rows): config 2 (0,6 6,6); W = 4 (0,16 16,16 32,16); W = 6, last band shorter
 # (0,12 12,12 24,8); one band in the training form with W = 6 and W = 7 (the frame's bottom edge is the only halo); H * W =
@@ -55,7 +56,7 @@ def head_call(lib, feats, w1, b1, w2, b2):
     b, c, h, w = feats.shape
     size = ctypes.c_size_t(0)
     assert lib.lpb_head_bf16_workspace_bytes(b, c, h, w, K, K, ctypes.byref(size)) == 0
-    ws = torch.zeros(size.value, dtype=torch.uint8, device=feats.device)
+    ws = torch.full((size.value,), 0xFF, dtype=torch.uint8, device=feats.device)
     assert lib.lpb_head_bf16_saved_bytes(b, c, h, w, ctypes.byref(size)) == 0
     xs = torch.full((size.value,), 0xFF, dtype=torch.uint8, device=feats.device)
     out = torch.empty(b, K, 8 * h, 8 * w, device=feats.device)
@@ -91,6 +92,15 @@ def mid_planes(mid, b, h, w):
     return m.permute(0, 1, 4, 2, 3).reshape(b, 32, hi, wi).to(torch.float64)
 
 
+def mid_pads_zero(mid, b, h, w):
+    """whether the mid activations' lead / trail rows and zero column (layer 2's halo) hold all-zero bits"""
+    hi, wi = 4 * h, 4 * w
+    pp, lead, rows = row_layout(hi, wi)
+    m = mid.reshape(b, 4, rows, 8)
+    zero_col = m[:, :, lead:lead + hi * pp].reshape(b, 4, hi, pp, 8)[:, :, :, wi:]
+    return not (m[:, :, :lead].any() or m[:, :, lead + hi * pp:].any() or zero_col.any())
+
+
 @pytest.mark.parametrize("shape", list(SHAPES))
 def test_k1a_bands(lib, dev, shape):
     c, h, w = SHAPES[shape]
@@ -110,6 +120,7 @@ def test_k1a_bands(lib, dev, shape):
         xs, mid = head_call(lib, feats, w1, b1, w2, b2)
         assert torch.equal(xs, saved_copy_ref(feats))
 
+        assert mid_pads_zero(mid, b, h, w)
         got = mid_planes(mid, b, h, w)
         assert bool((got[:, K] == 1).all()) and bool((got[:, K + 1:] == 0).all())  # the constant-one channel, zero padding
         for i in range(0, b, 64):
