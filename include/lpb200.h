@@ -148,7 +148,8 @@ int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const fl
 /* saved_xs: on the fast path NULL for inference; for training (and always on the banded path) a device buffer of lpb_head_bf16_saved_bytes() bytes; it
  * receives the pixel-shuffled features in the padded row layout the weight-gradient GEMM reads, and must stay
  * alive (together with `workspace`, which holds the activations between the two deconvs) until
- * lpb_head_bwd_bf16. */
+ * lpb_head_bwd_bf16.  features, saved_xs and workspace must be 16-byte aligned, out 8-byte aligned (LPB_ERR_INVALID
+ * otherwise, before anything is queued). */
 int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes);
 
 /* backward of lpb_head_fwd_bf16 (replaces autograd through heatmap.py:203-212 and, fused into its front end,
@@ -163,7 +164,9 @@ int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes);
  * db2 [c2] fp32 (overwritten).  One-deconv heads: w2 = dw2 = db2 = NULL, c2 = 0 (output [B, c1, 4H, 4W]).
  * Shapes: the forward's channel limits, and feature maps with H even, W in {4, 8, 12, 16, 24, 32}; both entries return
  * LPB_ERR_UNSUPPORTED for any other shape, so lpb_head_bwd_bf16_workspace_bytes (which needs no GPU) tells whether a
- * head can train on this path.  workspace: lpb_head_bwd_bf16_workspace_bytes() bytes. */
+ * head can train on this path.  workspace: lpb_head_bwd_bf16_workspace_bytes() bytes.  g_out, probs, win_meta,
+ * g_overflow, saved_xs, fwd_workspace, dfeat and workspace must be 16-byte aligned (LPB_ERR_INVALID otherwise, before
+ * anything is queued). */
 int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes);
 int lpb_head_bwd_bf16(const float* g_out, const float* probs, const float* win, const int32_t* win_meta,
                       const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H,

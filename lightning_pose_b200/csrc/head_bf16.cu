@@ -546,6 +546,11 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   LPB_REQUIRE((H * W) % 8 == 0, "head_fwd_bf16: H*W must be a multiple of 8 (got %d)", H * W);
   LPB_REQUIRE(c2 == 0 ? (c1 >= 1 && c1 <= HEAD_CLS) : (c1 >= 1 && c1 < HEAD_CLS && c2 >= 1 && c2 <= HEAD_CLS),
               "head_fwd_bf16: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
+  // features: TMA or uint4 loads; saved_xs, workspace: bulk copies and uint4 stores; out: float2 stores
+  LPB_REQUIRE(aligned_to(features, 16), "head_fwd_bf16: features must be 16-byte aligned");
+  LPB_REQUIRE(aligned_to(saved_xs, 16), "head_fwd_bf16: saved_xs must be 16-byte aligned");
+  LPB_REQUIRE(aligned_to(workspace, 16), "head_fwd_bf16: workspace must be 16-byte aligned");
+  LPB_REQUIRE(aligned_to(out, 8), "head_fwd_bf16: out must be 8-byte aligned");
   if (B == 0) return LPB_OK;
   int max_smem = 0, sms = 0;
   device_limits(&max_smem, &sms);
@@ -554,10 +559,10 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   const K1aGeom k1 = make_k1a_geom(H, W);
   // k1a's feature tensor map, encoded before anything is queued, so a failure leaves the stream untouched.  The plan stays
   // a function of the shape (CPU-only callers size buffers with it); every driver that runs sm_90a code has the encoder,
-  // so what can fail here is the caller's pointer (not 16-byte aligned).
+  // and the features' alignment was checked with the arguments.
   CUtensorMap feat_map;
   if (fast && !make_feat_tensor_map(&feat_map, features, B, C, H * W, k1.box)) {
-    set_error("head_fwd_bf16: cannot encode the feature tensor map (features must be 16-byte aligned)");
+    set_error("head_fwd_bf16: cannot encode the feature tensor map");
     return LPB_ERR_INVALID;
   }
   const int nst = C / 4 / HEAD_KSTAGE;

@@ -1031,6 +1031,13 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   LPB_REQUIRE(!win || (win_meta && g_overflow), "head_bwd_bf16: windows need their meta and overflow buffers");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1, "head_bwd_bf16: bad shape C=%d H=%d W=%d c1=%d", C, H, W, c1);
   if (const int rc = head_bwd_covers("head_bwd_bf16", H, W, c1, c2); rc != LPB_OK) return rc;
+  {
+    // read or written with 16-byte vectors (g_out, probs, g_overflow: float4 plane dots; win_meta: int4; dfeat: uint4 or
+    // TMA stores) or bulk copies (saved_xs, fwd_workspace, workspace)
+    const struct { const void* p; const char* name; } bufs[] = {{g_out, "g_out"}, {probs, "probs"}, {win_meta, "win_meta"},
+        {g_overflow, "g_overflow"}, {saved_xs, "saved_xs"}, {fwd_workspace, "fwd_workspace"}, {dfeat, "dfeat"}, {workspace, "workspace"}};
+    for (const auto& b : bufs) LPB_REQUIRE(aligned_to(b.p, 16), "head_bwd_bf16: %s must be 16-byte aligned", b.name);
+  }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int C4 = C / 4, Hi1 = 2 * H, Wi1 = 2 * W, Hi2 = 4 * H, Wi2 = 4 * W;
   const int kout = two ? c2 : c1;
@@ -1158,15 +1165,14 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
     size_t smem = (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
     LPB_REQUIRE(smem <= 225 * 1024, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
-    // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit, dfeat is 16-byte
-    // aligned and the tensor map encodes; otherwise direct 16-byte stores
+    // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit and the tensor map
+    // encodes; otherwise direct 16-byte stores (dfeat's alignment was checked with the arguments)
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     p.tma_store = 0;
     {
       const size_t stage = (size_t)2 * 4 * 128 * 4 * W + 128;
-      if (smem + stage <= 225 * 1024 && (reinterpret_cast<uintptr_t>(dfeat) % 16) == 0 &&
-          make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
+      if (smem + stage <= 225 * 1024 && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
         p.tma_store = 1;
         smem += stage;
       }

@@ -28,6 +28,10 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
     if (e__ != cudaSuccess) return ::lpb::cuda_fail(e__, #call, __FILE__, __LINE__); \
   } while (0)
 
+// A caller's device pointer that is null or a multiple of `bytes`.  Entry points check the buffers their kernels move with
+// vector accesses, bulk copies or TMA up front: a misaligned one would otherwise fault on the device.
+inline bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
+
 extern int g_softmax_split;  // abi.cu: LPB_TUNE_SOFTMAX_SPLIT
 
 // ---- device helpers ---------------------------------------------------------------------------

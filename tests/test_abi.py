@@ -116,6 +116,41 @@ def test_head_training_entry_points_validate_without_gpu():
     assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
 
 
+_BWD_VECTOR_BUFFERS = ["dfeat", "g_out", "probs", "win_meta", "g_overflow", "saved_xs", "fwd_workspace", "workspace"]
+
+
+@pytest.mark.parametrize("misaligned", _BWD_VECTOR_BUFFERS)
+def test_head_bwd_refuses_misaligned_buffers_without_gpu(misaligned):
+    """lpb_head_bwd_bf16 moves these buffers with 16-byte vectors, bulk copies or TMA.  A pointer that is 2-byte but not
+    16-byte aligned (0x1002) is refused with LPB_ERR_INVALID while the arguments are checked: the other pointers are fake,
+    so a queued kernel or a CUDA call (LPB_ERR_CUDA without a GPU) would show here."""
+    from lightning_pose_b200 import _lib
+
+    p = {name: 0x1000 for name in _BWD_VECTOR_BUFFERS + ["win", "w1", "w2", "dw1", "db1", "dw2", "db2"]}
+    p[misaligned] = 0x1002
+    rc = _lib.lib.lpb_head_bwd_bf16(p["g_out"], p["probs"], p["win"], p["win_meta"], p["g_overflow"], p["saved_xs"], p["fwd_workspace"],
+                                    3, 512, 8, 8, p["w1"], 9, p["w2"], 9, p["dfeat"], p["dw1"], p["db1"], p["dw2"], p["db2"], p["workspace"], None)
+    assert rc == -1, (rc, _lib.lib.lpb_last_error())
+    assert _lib.lib.lpb_last_error() == f"head_bwd_bf16: {misaligned} must be 16-byte aligned".encode()
+
+
+@pytest.mark.parametrize("misaligned,addr,need", [("features", 0x1002, 16), ("saved_xs", 0x1008, 16), ("workspace", 0x1004, 16),
+                                                   ("out", 0x1004, 8)])
+@pytest.mark.parametrize("c,h,w,c2", [(2048, 12, 12, 17), (384, 16, 16, 0)])  # fast path, banded path
+def test_head_fwd_refuses_misaligned_buffers_without_gpu(misaligned, addr, need, c, h, w, c2):
+    """lpb_head_fwd_bf16 reads the features with TMA or 16-byte loads, moves saved_xs / workspace with bulk copies and
+    writes out with 8-byte stores: a pointer short of that alignment is refused before anything is queued, on either
+    kernel family."""
+    from lightning_pose_b200 import _lib
+
+    p = {name: 0x1000 for name in ("features", "w1", "b1", "w2", "b2", "out", "saved_xs", "workspace")}
+    p[misaligned] = addr
+    rc = _lib.lib.lpb_head_fwd_bf16(p["features"], 2, c, h, w, p["w1"], p["b1"], 17, p["w2"] if c2 else None, p["b2"] if c2 else None, c2, 1,
+                                    p["out"], p["saved_xs"], p["workspace"], None)
+    assert rc == -1, (rc, _lib.lib.lpb_last_error())
+    assert _lib.lib.lpb_last_error() == f"head_fwd_bf16: {misaligned} must be {need}-byte aligned".encode()
+
+
 def test_fused_head_node_refuses_cpu_tensors():
     from lightning_pose_b200.models.heads.heatmap import HeatmapHead
 
