@@ -55,11 +55,14 @@ int lpb_get_tuning(int key);
  * conf      [n_planes]
  * stats     [n_planes, 8] or NULL: {shift M, sum S, xhat, yhat (field coords), A0, A1, B0, B1
  *           (evaluated coarse region)} - the residual lpb_decode_bwd needs.
+ * workspace lpb_decode_fwd_workspace_bytes(n_planes) bytes of device scratch, 4-byte aligned; NULL only when
+ *           n_planes == 0.  Only the call's own kernels use it, so one buffer can serve every call on a stream.
  * ds in {1,2,3}.  Evaluation is exact up to a dropped softmax mass < 1e-12 (see DESIGN.md).
  */
 int lpb_decode_prepare(int h, int w, int ds);
+int lpb_decode_fwd_workspace_bytes(int64_t n_planes, size_t* bytes);
 int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
-                   float* xy, float* conf, float* stats, void* stream);
+                   float* xy, float* conf, float* stats, void* workspace, void* stream);
 /* d loss / d heatmaps given d loss / d xy (confidence carries no gradient: it only feeds `<`
  * comparisons, lightning_pose/losses/losses.py:636). grad_heatmaps [n_planes,h,w] is overwritten. */
 int lpb_decode_bwd(const float* heatmaps, const float* stats, const float* grad_xy, int64_t n_planes,

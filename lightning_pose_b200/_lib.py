@@ -39,7 +39,8 @@ SIGNATURES = {
     "lpb_set_tuning": (C.c_int, [_I, _I]),
     "lpb_get_tuning": (C.c_int, [_I]),
     "lpb_decode_prepare": (C.c_int, [_I, _I, _I]),
-    "lpb_decode_fwd": (C.c_int, [_P, _L, _I, _I, _I, _F, _P, _P, _P, _P]),
+    "lpb_decode_fwd_workspace_bytes": (C.c_int, [_L, C.POINTER(_Z)]),
+    "lpb_decode_fwd": (C.c_int, [_P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
     "lpb_decode_bwd": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _F, _P, _P]),
     "lpb_decode_bwd_windows": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
     "lpb_upsample2x": (C.c_int, [_P, _L, _I, _I, _P, _P]),

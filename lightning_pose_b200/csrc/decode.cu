@@ -6,15 +6,17 @@
 //   (x, y) = sum p * (col, row);  conf = sum of the 5x5 window of p around (trunc y, trunc x)
 //   (x, y) -= {0.5, 1.5, 2.5}
 //
-// Design (DESIGN.md "K2"): one CTA per plane; the plane is staged ONCE into shared memory by
-// the TMA engine (cp.async.bulk, one copy per row into a zero-padded tile); the 4x-upsampled field
-// is never materialised: field = U_H h U_W^T is evaluated separably in registers (horizontal pass
-// from smem, vertical pass on a sliding register window with the phase-periodic interior weights
-// in the constant bank) and only inside the coarse bounding box that can hold softmax mass
-// > exp(-40) relative to the peak (rigorous bound |field| <= lip * max|h| over the tap footprint).
-// Flat (fresh-init) planes fall through to the same code with the box = whole plane.
+// Design (DESIGN.md "K2"): the 4x-upsampled field is never materialised: field = U_H h U_W^T is evaluated separably in
+// registers (horizontal pass from shared memory, vertical pass on a sliding register window with the phase-periodic
+// interior weights in the constant bank).
+// Forward: one warp per plane (decode_fwd_warp_kernel) bounds the coarse box that can hold softmax mass > exp(-40)
+// relative to the peak (rigorous bound |field| <= lip * max|h| over the tap footprint) with two sweeps of the plane, and
+// evaluates only that box, from a 32 x 32 window in shared memory.  The planes whose box does not fit the window
+// (diffuse / multi-modal: freshly initialised networks), NaN planes and T <= 0 are queued for decode_fwd_kernel, which
+// stages each queued plane into shared memory once (TMA row copies into a zero-padded tile, or plain loads), splits it
+// over several CTAs and evaluates all of it.
+// Backward: the same split, a 32 x 32 window per plane (decode_bwd_window_kernel) or the whole plane (decode_bwd_kernel).
 #include <cstdint>
-#include <cstdlib>
 
 #include "../../include/lpb200.h"
 #include "lpb_common.cuh"
@@ -28,25 +30,31 @@ constexpr float DEC_CUT = 40.0f;  // dropped pixels have weight < exp(-40) = 4e-
 constexpr int DEC_MAX_PARTS = 16;  // CTAs a queued (dense) plane can be split over
 constexpr int DEC_CONF_R = 2;     // floor(1.25 * 2), lightning_pose/data/heatmaps.py:111
 
+// What the forward and backward kernels share: the planes, their upsampling tables and the tap constants (decode_geom).
 template <int DS>
-struct DecodeParams {
+struct DecodeGeom {
   static constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1;
   const float* heat;
   const float* tabH;  // [h*F][W] vertical-axis window weights
   const float* tabW;  // [w*F][W] horizontal-axis window weights
+  int h, w, pitch, padl;  // a plane's zero-padded shared-memory tile: row pitch, first plane column (floats)
+  int bulk;           // w % 4 == 0 and heat 16-byte aligned: TMA row copies, 16-byte loads
+  int64_t n_planes;
+  float T;
+  float lipw;         // max row sum of |horizontal taps|
+  float wabs[W];      // max over rows / phases of |vertical tap| per offset (row pruning of the window kernels)
+  float2 phase2[F / 2][W];  // vertical taps of the interior rows' phases 2q, 2q+1: packed-pair constant-bank operands
+};
+
+template <int DS>
+struct DecodeParams : DecodeGeom<DS> {
   float* xy;
   float* conf;
   float* stats;
-  int h, w, pitch, padl, bulk;
-  int64_t n_planes;
-  float T, lip, offset;
-  const int* queue;   // CTA kernel, queue mode: {count, plane ids ...} left over by the warp-per-plane kernel
+  float lip, offset;
+  int* queue;         // {count, plane ids ...}: the planes the warp kernel leaves for the CTA kernel
   int* qcounter;      // [n_planes] arrival counters (zeroed) and
   float* qscratch;    // [n_planes][DEC_MAX_PARTS][4] partial softmax states of a plane split over several CTAs
-  float lipw;         // max row sum of |horizontal taps|
-  float wabs[W];      // max over rows / phases of |vertical tap| per offset (row pruning in the warp kernel)
-  float phase[F][W];  // interior rows (constant bank operands)
-  float2 phase2[F / 2][W];  // {phase[2q][t], phase[2q+1][t]}: packed-pair operands of the strip evaluation
 };
 
 __host__ __device__ inline int dec_padl(int R) { return (R + 3) & ~3; }
@@ -60,7 +68,7 @@ __device__ __forceinline__ float dot_w(const float* __restrict__ p, const float 
   return r;
 }
 
-// exact field value at fine pixel (i, j) (W*W taps); used for the lower bound and the confidence
+// exact field value at fine pixel (i, j) (W*W taps)
 template <int DS>
 __device__ float eval_point(const float* tile, int pitch, int padl, const float* __restrict__ tabH,
                             const float* __restrict__ tabW, int i, int j) {
@@ -78,9 +86,9 @@ __device__ float eval_point(const float* tile, int pitch, int padl, const float*
   return acc;
 }
 
-// exact field values at up to F*F fine pixels (scratch: npts * W floats), spread over the CTA: thread (pt, t) evaluates one horizontal tap row, the W rows
-// of a point meet in shared memory.  (One thread per point walked W x W dependent table loads: ~3 us per call, twice per
-// plane -- a fifth of a queued plane's latency.)  Returns the value of point `tid` for tid < npts; contains a __syncthreads().
+// exact field values at npts fine pixels (scratch: npts * W floats), spread over the CTA: thread (pt, t) evaluates one horizontal tap row, the W rows
+// of a point meet in shared memory.  (One thread per point walked W x W dependent table loads: ~3 us per call.)
+// Returns the value of point `tid` for tid < npts; contains a __syncthreads().
 template <int DS, class CoordFn>
 __device__ __forceinline__ float eval_points_cta(const float* tile, int pitch, int padl, const float* __restrict__ tabH,
                                                  const float* __restrict__ tabW, int npts, CoordFn coord, float* scratch, int tid) {
@@ -110,7 +118,7 @@ __device__ __forceinline__ float eval_points_cta(const float* tile, int pitch, i
 // one coarse row of the vertical pass: F fine values from the W-row window `t`, as F/2 packed pairs of phases
 // (fma.rn.f32x2: the same fp32 roundings as the scalar chain, half the issue slots)
 template <int DS>
-__device__ __forceinline__ void column_pass(const DecodeParams<DS>& P, int a, int h, const float* t, f32x2* v2) {
+__device__ __forceinline__ void column_pass(const DecodeGeom<DS>& P, int a, int h, const float* t, f32x2* v2) {
   constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1, HP = F / 2;
   if (a >= R && a <= h - 1 - R) {  // interior: phase-periodic weights are kernel-parameter constants (uniform registers)
 #pragma unroll
@@ -179,7 +187,7 @@ __device__ __forceinline__ void softmax_row(const f32x2* v2, float yrow, float c
 // (fma.rn.f32x2 over two tile rows).  In the round-2 capture of the dense kernel the shifting moves and their integer
 // bookkeeping were 40 % of the loop's instructions.
 template <int DS>
-__device__ __forceinline__ void fwd_strip(const DecodeParams<DS>& P, const float* base, int pitch, const float (&wc)[2 * (DS + 2) + 1],
+__device__ __forceinline__ void fwd_strip(const DecodeGeom<DS>& P, const float* base, int pitch, const float (&wc)[2 * (DS + 2) + 1],
                                           int r0, int r1, float c, float kill, float& m, float& mc, float& s_it, float& sy_it) {
   constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1, NS = W + 1, NP2 = NS / 2, HP = F / 2;
   const int h = P.h, nrows = r1 - r0, kmax = nrows - 1 + 2 * R;  // last window row a valid coarse row uses
@@ -222,18 +230,26 @@ __device__ __forceinline__ void fwd_strip(const DecodeParams<DS>& P, const float
   }
 }
 
+// Shared memory the CTA kernel requests beyond its tile, in floats.  The kernel uses less; the request keeps the size it
+// had when the kernel also pruned planes itself, because the request sets how many CTAs are resident, and with that over
+// how many CTAs each queued plane is split and in which order its partial sums are added.
+constexpr int DEC_FWD_SCRATCH = 880;
+
+// The planes the warp kernel queued, evaluated whole.  A queued plane is split over NP CTAs (a call queues few planes,
+// which alone would leave most SMs idle): its work items -- (32-fine-column strip, row segment) pairs -- are dealt
+// round-robin over the parts, the parts' online-softmax states meet in global scratch, and the last CTA to arrive merges
+// them and finishes the plane.  The CTAs are persistent over the (plane, part) pairs.
 template <int DS>
 __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kernel(const __grid_constant__ DecodeParams<DS> P) {
-  constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1;
-  constexpr int CPS = 32 / F;  // coarse columns per 32-fine-column strip
+  constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1, CW = 2 * DEC_CONF_R + 1;
+  static_assert(4 * DEC_WARPS + 3 + CW * CW * W <= DEC_FWD_SCRATCH, "decode_fwd_kernel: scratch exceeds the request");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int h = P.h, w = P.w, pitch = P.pitch, padl = P.padl;
   float* tile = reinterpret_cast<float*>(smem_raw);  // (h + 2R) x pitch; logical (a,b) at [(a+R)*pitch + padl + b]
-  float* red = tile + (h + 2 * R) * pitch;           // 64 floats of reduction scratch
-  int* redi = reinterpret_cast<int*>(red + 64);      // 112 ints
-  float* evs = reinterpret_cast<float*>(redi + 112);  // 704 floats (F*F*W at ds = 3): tap rows of eval_points_cta
-  uint64_t* bar = reinterpret_cast<uint64_t*>(evs + 704);
-  unsigned* smask = reinterpret_cast<unsigned*>(redi + 48);  // [32] per-strip bitmask of active row chunks
+  float* red = tile + (h + 2 * R) * pitch;           // [DEC_WARPS][4] per-warp softmax states
+  uint64_t* bar = reinterpret_cast<uint64_t*>(red + 4 * DEC_WARPS);
+  int* arrival = reinterpret_cast<int*>(bar + 1);       // this CTA's place among the parts of its plane
+  float* evs = reinterpret_cast<float*>(arrival + 1);  // CW * CW * W floats: tap rows of eval_points_cta
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   // ---- once per CTA: barrier + zero halo (the CTA is persistent; only the interior is rewritten) ----
@@ -253,25 +269,25 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
   __syncthreads();
 
   uint32_t tma_phase = 0;
-  // queue mode: the few planes the warp kernel left over are each split over NP CTAs (their work items are dealt
-  // round-robin; partial softmax states meet in global scratch, the last CTA to arrive merges and finishes)
-  const int qcount = P.queue ? P.queue[0] : 0;
-  const int NP = (P.queue && qcount > 0) ? min(DEC_MAX_PARTS, max(1, (int)gridDim.x / qcount)) : 1;
-  const size_t nwork = P.queue ? (size_t)qcount * NP : (size_t)P.n_planes;
+  const int qcount = P.queue[0];
+  const int NP = qcount > 0 ? min(DEC_MAX_PARTS, max(1, (int)gridDim.x / qcount)) : 1;
+  const size_t nwork = (size_t)qcount * NP;
   for (size_t work = blockIdx.x; work < nwork; work += gridDim.x) {
   const size_t slot = work / NP;
   const int part = (int)(work - slot * NP);
-  const size_t plane = P.queue ? (size_t)P.queue[1 + slot] : work;
+  const size_t plane = (size_t)P.queue[1 + slot];
   const float* __restrict__ src = P.heat + plane * (size_t)h * w;
 
-  // ---- stage the plane: TMA bulk row copies into the zero-padded tile -------------------------
+  // ---- stage the plane: TMA bulk row copies into the zero-padded tile, or plain loads ------------
   if (P.bulk) {
     if (warp == 0) {
       if (lane == 0) mbar_expect_tx(bar, (uint32_t)(h * w * 4));
       __syncwarp();
       for (int a = lane; a < h; a += 32)
         bulk_g2s(tile + (a + R) * pitch + padl, src + (size_t)a * w, (uint32_t)(w * 4), bar);
+      mbar_wait(bar, tma_phase);  // one warp polls; the bytes are in shared memory once the phase flips
     }
+    tma_phase ^= 1;
   } else {
     for (int r = warp; r < h; r += DEC_WARPS) {
       const float* g = src + (size_t)r * w;
@@ -279,214 +295,24 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
       for (int b = lane; b < w; b += 32) row[b] = __ldg(g + b);
     }
   }
-  if (tid < 32) smask[tid] = 0u;
-  if (P.bulk) {
-    if (warp == 0) mbar_wait(bar, tma_phase);  // one warp polls; the bytes are in shared memory once the phase flips
-    tma_phase ^= 1;
-  }
   __syncthreads();
 
-  // ---- scan 1: arg max of |h|; each warp owns a band of rows, lanes read 4-column groups ------------
-  // (rows of the padded tile are 16-byte aligned and followed by >= R zero columns, so the last,
-  //  possibly partial, group is safe to read)
-  const int w4 = (w + 3) >> 2;
-  const int band = (h + DEC_WARPS - 1) / DEC_WARPS;
-  // Queue mode skips both scans: the planes that arrive here are the ones pruning cannot help (diffuse / multi-modal /
-  // NaN), and every CTA a plane is split over would repeat them -- they were half of the queued kernel's instructions.
-  // The online softmax starts from a low finite maximum instead of the arg-max bound and the whole plane is evaluated.
-  const int ab0 = warp * band, ab1 = P.queue ? ab0 : min(h, ab0 + band);
-  float best = -1.f;
-  int bpos = 0;
-  if (w4 <= 32) {  // common case: one 16-byte group per lane and row, no inner loop
-    const float4* row4 = reinterpret_cast<const float4*>(tile + (ab0 + R) * pitch + padl) + (lane < w4 ? lane : 0);
-    const int pitch4 = pitch >> 2;
-    for (int a = ab0; a < ab1; ++a, row4 += pitch4) {
-      const float4 x = *row4;
-      const float m4 = fmaxf(fmaxf(fabsf(x.x), fabsf(x.y)), fmaxf(fabsf(x.z), fabsf(x.w)));
-      if (m4 > best) {
-        best = m4;
-        bpos = a;
-      }
-    }
-    bpos = (bpos << 16) | (lane < w4 ? lane : 0);
-  } else {
-    for (int a = ab0; a < ab1; ++a) {
-      const float4* row4 = reinterpret_cast<const float4*>(tile + (a + R) * pitch + padl);
-      for (int b4 = lane; b4 < w4; b4 += 32) {
-        const float4 x = row4[b4];
-        const float m4 = fmaxf(fmaxf(fabsf(x.x), fabsf(x.y)), fmaxf(fabsf(x.z), fabsf(x.w)));
-        if (m4 > best) {
-          best = m4;
-          bpos = (a << 16) | b4;
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int op = __shfl_xor_sync(0xffffffffu, bpos, o);
-    if (ob > best) {
-      best = ob;
-      bpos = op;
-    }
-  }
-  const float bandmax = best;  // warp-uniform: max |h| over this warp's band
-  if (lane == 0) {
-    red[warp] = best;
-    redi[warp] = bpos;
-  }
-  __syncthreads();
-  best = red[0];
-  bpos = redi[0];
-#pragma unroll
-  for (int k = 1; k < DEC_WARPS; ++k)
-    if (red[k] > best) {
-      best = red[k];
-      bpos = redi[k];
-    }
-  const int besta = bpos >> 16;
-  int bestb = (bpos & 0xffff) * 4;
-  {
-    const float* g4 = tile + (besta + R) * pitch + padl + bestb;
-    bestb += (fabsf(g4[0]) == best) ? 0 : ((fabsf(g4[1]) == best) ? 1 : ((fabsf(g4[2]) == best) ? 2 : 3));
-    bestb = min(bestb, w - 1);
-  }
-
-  // ---- lower bound on the field maximum: exact values in the F x F block of the coarse arg max --
-  float lb = eval_points_cta<DS>(tile, pitch, padl, P.tabH, P.tabW, P.queue ? 0 : F * F, [&](int pt, int& i, int& j) {
-    i = besta * F + pt / F;
-    j = bestb * F + pt % F;
-    return true;
-  }, evs, tid);
-  if (tid >= F * F) lb = -3.0e38f;
-  lb = warp_max(lb);
-  if (lane == 0) red[8 + warp] = lb;
-  __syncthreads();
-  float mlb = red[8];
-#pragma unroll
-  for (int k = 1; k < DEC_WARPS; ++k) mlb = fmaxf(mlb, red[8 + k]);
-  if (P.queue) mlb = -1.0e30f;
-
-  // ---- scan 2: candidates (|h| >= theta) -> per-strip candidate row range + hull ---------------------
-  // a fine pixel can carry weight > exp(-CUT) only if a candidate lies within R coarse samples of it
-  const float theta = (P.T > 0.f) ? (mlb - DEC_CUT / P.T) / P.lip : -1.f;
+  // ---- the items of this part: a per-lane online softmax over the whole plane, from a low finite maximum ----------
+  // a strip's rows [0, h) are cut into nseg segments of seglen rows: at most 48 rows, and short enough that all the warps
+  // of all NP CTAs have an item (a queued plane's latency matters, not throughput).  These are the same for every plane,
+  // but computed outside the plane loop they took uniform registers that the interior tap constants of column_pass need:
+  // at ds = 2 the constants were then reloaded inside the strip loop, and flat planes decoded about 4 % slower.
   const int nstrips = (w * F + 31) >> 5;  // <= 32 (checked on the host)
-  int amin = h, amax = -1, bmin = w, bmax = -1;
-  const int CH = max(4, (h + 31) >> 5);  // coarse rows per chunk (<= 32 chunks per plane)
-  if (!P.queue && bandmax >= theta) {
-    unsigned cmask = 0u;  // lane s owns strip s: chunks whose rows lie within R of a candidate
-    const int nit = (w4 + 31) >> 5;
-    unsigned long long gmask = 0;  // 4-column groups that can reach strip `lane`
-    if (lane < nstrips) {
-      const int cs0 = lane * CPS;
-      const int glo = max(cs0 - R, 0) >> 2, ghi = min(cs0 + CPS - 1 + R, w - 1) >> 2;
-      gmask = ((2ull << (ghi - glo)) - 1ull) << glo;
-    }
-    for (int a = ab0; a < ab1; ++a) {
-      const float4* row4 = reinterpret_cast<const float4*>(tile + (a + R) * pitch + padl);
-      unsigned long long cm = 0;
-      for (int it = 0; it < nit; ++it) {  // w4 <= 64: at most two ballots per row
-        const int b4 = lane + 32 * it;
-        bool c = false;
-        if (b4 < w4) {
-          const float4 x = row4[b4];
-          c = (fabsf(x.x) >= theta) || (fabsf(x.y) >= theta) || (fabsf(x.z) >= theta) || (fabsf(x.w) >= theta);
-        }
-        cm |= (unsigned long long)__ballot_sync(0xffffffffu, c) << (32 * it);
-      }
-      if (cm) {
-        amin = min(amin, a);
-        amax = max(amax, a);
-        bmin = min(bmin, 4 * (__ffsll((long long)cm) - 1));
-        bmax = max(bmax, min(4 * (63 - __clzll((long long)cm)) + 3, w - 1));
-        if (cm & gmask) {
-          const int c0 = max(a - R, 0) / CH, c1 = min(a + R, h - 1) / CH;
-          cmask |= ((2u << (c1 - c0)) - 1u) << c0;
-        }
-      }
-    }
-    if (cmask) atomicOr(&smask[lane], cmask);
-  }
-  if (lane == 0) {  // amin..bmax are warp-uniform (derived from ballots)
-    redi[16 + 4 * warp + 0] = amin;
-    redi[16 + 4 * warp + 1] = amax;
-    redi[16 + 4 * warp + 2] = bmin;
-    redi[16 + 4 * warp + 3] = bmax;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < DEC_WARPS; ++k) {
-    amin = min(amin, redi[16 + 4 * k + 0]);
-    amax = max(amax, redi[16 + 4 * k + 1]);
-    bmin = min(bmin, redi[16 + 4 * k + 2]);
-    bmax = max(bmax, redi[16 + 4 * k + 3]);
-  }
-  unsigned my_mask = (lane < nstrips) ? smask[lane] : 0u;
-  if (amax < 0) {  // only reachable with NaN input: evaluate everything
-    amin = 0;
-    amax = h - 1;
-    bmin = 0;
-    bmax = w - 1;
-    if (lane < nstrips) my_mask = 0xffffffffu >> (32 - (h + CH - 1) / CH);
-  }
-  const int A0 = max(amin - R, 0), A1 = min(amax + R, h - 1);
-  const int B0 = max(bmin - R, 0), B1 = min(bmax + R, w - 1);
-
-  // ---- work items: lane s describes strip s; one item per run of active chunks (long runs split in two)
-  auto next_run = [&](unsigned& m, int& q0, int& q1) {  // pops the lowest run of set bits -> rows [q0, q1)
-    const int st = __ffs(m) - 1;
-    const unsigned sh = m >> st;
-    const int len = __ffs(~sh) - 1;  // sh has a zero bit unless all 32 chunks are active
-    q0 = st * CH;
-    q1 = min((st + (len < 0 ? 32 - st : len)) * CH, h);
-    m = (len < 0 || st + len >= 32) ? 0u : (m & ~(((1u << len) - 1u) << st));
-  };
-  // rows per work item: at most 48 (a full-height strip is split in two) when planes fill the grid; the few planes of
-  // queue mode are cut finer, so that all warps of all the CTAs a plane is split over have an item (latency, not throughput)
-  const int per_strip = max(1, (NP * DEC_WARPS) / nstrips);  // row segments a strip can have with one item per warp
-  const int seg_cap = P.queue ? min(48, max(8, (h + per_strip - 1) / per_strip)) : 48;
-  int nmine = 0;
-  {
-    unsigned m = my_mask;
-    while (m) {
-      int q0, q1;
-      next_run(m, q0, q1);
-      nmine += (q1 - q0 + seg_cap - 1) / seg_cap;
-    }
-  }
-  int istart = nmine;  // exclusive prefix sum over lanes
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, istart, o);
-    if (lane >= o) istart += t;
-  }
-  const int nitems = __shfl_sync(0xffffffffu, istart, 31);
-  istart -= nmine;
-
+  const int per_strip = max(1, (NP * DEC_WARPS) / nstrips);
+  const int seg_cap = min(48, max(8, (h + per_strip - 1) / per_strip));
+  const int nseg = (h + seg_cap - 1) / seg_cap, seglen = (h + nseg - 1) / nseg, nitems = nstrips * nseg;
   const float c = P.T * 1.4426950408889634f;
-  float M = mlb, S = 0.f, SX = 0.f, SY = 0.f;
-
+  float M = -1.0e30f, S = 0.f, SX = 0.f, SY = 0.f;
   for (int itw = warp;; itw += DEC_WARPS) {
     const int item = itw * NP + part;
     if (item >= nitems) break;
-    const unsigned own = __ballot_sync(0xffffffffu, item >= istart && item < istart + nmine);
-    const int sl = __ffs(own) - 1;  // strip index
-    unsigned rm = __shfl_sync(0xffffffffu, my_mask, sl);
-    int k = item - __shfl_sync(0xffffffffu, istart, sl);
-    int r0 = 0, r1 = 0;
-    while (rm) {
-      int q0, q1;
-      next_run(rm, q0, q1);
-      const int ns = (q1 - q0 + seg_cap - 1) / seg_cap;
-      if (k < ns) {
-        const int seglen = (q1 - q0 + ns - 1) / ns;
-        r0 = q0 + k * seglen;
-        r1 = min(r0 + seglen, q1);
-        break;
-      }
-      k -= ns;
-    }
+    const int sl = item / nseg;  // strip index
+    const int r0 = (item - sl * nseg) * seglen, r1 = min(r0 + seglen, h);
     if (r0 >= r1) continue;
     const int jf = sl * 32 + lane;
     const bool ok = jf < w * F;
@@ -516,25 +342,25 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
     SX = warp_sum(SX * sc);
     SY = warp_sum(SY * sc);
     if (lane == 0) {
-      red[16 + 4 * warp + 0] = Mw;
-      red[16 + 4 * warp + 1] = S;
-      red[16 + 4 * warp + 2] = SX;
-      red[16 + 4 * warp + 3] = SY;
+      red[4 * warp + 0] = Mw;
+      red[4 * warp + 1] = S;
+      red[4 * warp + 2] = SX;
+      red[4 * warp + 3] = SY;
     }
   }
   __syncthreads();
-  M = red[16];
+  M = red[0];
 #pragma unroll
-  for (int k = 1; k < DEC_WARPS; ++k) M = fmaxf(M, red[16 + 4 * k]);
+  for (int k = 1; k < DEC_WARPS; ++k) M = fmaxf(M, red[4 * k]);
   S = 0.f;
   SX = 0.f;
   SY = 0.f;
 #pragma unroll
   for (int k = 0; k < DEC_WARPS; ++k) {
-    const float sc = fast_exp2((red[16 + 4 * k] - M) * c);
-    S = fmaf(red[16 + 4 * k + 1], sc, S);
-    SX = fmaf(red[16 + 4 * k + 2], sc, SX);
-    SY = fmaf(red[16 + 4 * k + 3], sc, SY);
+    const float sc = fast_exp2((red[4 * k] - M) * c);
+    S = fmaf(red[4 * k + 1], sc, S);
+    SX = fmaf(red[4 * k + 2], sc, SX);
+    SY = fmaf(red[4 * k + 3], sc, SY);
   }
   bool finisher = true;
   if (NP > 1) {  // cross-CTA merge of the parts of this plane
@@ -545,10 +371,10 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
       part_state[2] = SX;
       part_state[3] = SY;
       __threadfence();
-      redi[0] = atomicAdd(P.qcounter + slot, 1);
+      *arrival = atomicAdd(P.qcounter + slot, 1);
     }
     __syncthreads();
-    finisher = redi[0] == NP - 1;
+    finisher = *arrival == NP - 1;
     if (finisher) {
       __threadfence();
       const volatile float* ps = P.qscratch + slot * DEC_MAX_PARTS * 4;
@@ -569,7 +395,6 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
   const float xhat = SX / S, yhat = SY / S;
 
   // ---- confidence: softmax mass of the (2r+1)^2 window around (trunc y, trunc x) -----------------
-  constexpr int CW = 2 * DEC_CONF_R + 1;
   float cw = 0.f;
   {
     auto wcoord = [&](int pt, int& i, int& j) {
@@ -586,16 +411,16 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
     P.xy[2 * plane + 0] = xhat - P.offset;
     P.xy[2 * plane + 1] = yhat - P.offset;
     P.conf[plane] = cw;
-    if (P.stats) {
+    if (P.stats) {  // the evaluated box is the whole plane
       float* st = P.stats + 8 * plane;
       st[0] = M;
       st[1] = S;
       st[2] = xhat;
       st[3] = yhat;
-      st[4] = (float)A0;
-      st[5] = (float)A1;
-      st[6] = (float)B0;
-      st[7] = (float)B1;
+      st[4] = 0.f;
+      st[5] = (float)(h - 1);
+      st[6] = 0.f;
+      st[7] = (float)(w - 1);
     }
   }
   }  // finisher
@@ -604,16 +429,19 @@ __global__ void __launch_bounds__(DEC_THREADS, DS == 3 ? 2 : 4) decode_fwd_kerne
 }
 
 // ------------------------------------------------------------------------------------------------
-// Warp-per-plane forward for planes whose mass sits in one small box (trained networks: all of them).
-// The CTA kernel above synchronises eight warps five times per plane and more than half of its stall samples
-// are at those barriers; here one warp owns a plane end to end and only warp-level primitives are used:
-//   pass 1  stream the plane (16-byte loads), arg max |h|
+// Warp-per-plane forward, run on every plane.  One warp owns a plane end to end and only warp-level primitives are used
+// (a CTA per plane synchronised eight warps five times per plane, and more than half of its stall samples were at
+// those barriers):
+//   pass 1  stream the plane in 4-column groups, arg max |h|
 //   window  32x32 coarse pixels around the arg max -> shared memory; m_lb = exact field on the arg max's F x F block
 //   pass 2  stream the plane again (L2), hull of the candidates |h| >= theta
 //   window  re-centred on the hull +- R; rows pruned with the tap-decay bound; separable evaluation of the strips
 //           with a per-lane online softmax; exact 5x5 confidence window
-// Planes whose hull does not fit a window (diffuse / multi-modal), NaN planes and T <= 0 are appended to a queue
-// and run by the CTA kernel in queue mode, so every plane produces the same outputs either way.
+// Planes whose hull does not fit a window (diffuse / multi-modal), NaN planes and T <= 0 are appended to the queue of
+// decode_fwd_kernel.
+// BULK (w % 4 == 0, plane 16-byte aligned): a group is one 16-byte load.  Otherwise it is four scalar loads, columns >= w
+// read as 0: the same groups in the same order with the same tie-breaks, so an aligned and a misaligned copy of the same
+// planes decode to the same bits.
 constexpr int DECW_WIN = 32, DECW_WP = 33;
 
 template <int DS>
@@ -644,11 +472,11 @@ __device__ __forceinline__ void load_window(float* tile, const float* __restrict
 }
 
 // One plane, one warp; `src` is the plane in global memory (read-only path, three sweeps of it).
-template <int DS>
+template <int DS, bool BULK>
 __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, const float* __restrict__ src, float* tile,
                                   int* __restrict__ queue, int lane) {
   constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1;
-  const int h = P.h, w = P.w, w4 = w >> 2, n4 = h * w4;
+  const int h = P.h, w = P.w, w4 = BULK ? w >> 2 : (w + 3) >> 2, n4 = h * w4;
   const float4* __restrict__ src4 = reinterpret_cast<const float4*>(src);
   // L2 residency hints: the arg-max sweep asks L2 to KEEP the plane (evict_last), the hull sweep that follows re-reads it
   // from L2 and releases it (evict_first) -- without them the second sweep misses L2 (measured DRAM traffic 2.05x the
@@ -656,10 +484,23 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
   uint64_t pol_keep, pol_drop;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_keep));
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_drop));
-  auto ld4h = [&](int idx, uint64_t pol) -> float4 {
-    float4 v;
-    asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(src4 + idx), "l"(pol));
-    return v;
+  auto ld4 = [&](int idx) -> float4 {  // 4-column group idx = a * w4 + g
+    if constexpr (BULK) {
+      return __ldg(src4 + idx);
+    } else {
+      const int a = idx / w4, b = 4 * (idx - a * w4);
+      const float* p = src + (size_t)a * w + b;
+      return make_float4(__ldg(p), b + 1 < w ? __ldg(p + 1) : 0.f, b + 2 < w ? __ldg(p + 2) : 0.f, b + 3 < w ? __ldg(p + 3) : 0.f);
+    }
+  };
+  auto ld4h = [&](int idx, uint64_t pol) -> float4 {  // the same, with the L2 hint where the load is one instruction
+    if constexpr (BULK) {
+      float4 v;
+      asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(src4 + idx), "l"(pol));
+      return v;
+    } else {
+      return ld4(idx);
+    }
   };
   auto to_queue = [&]() {
     if (lane == 0) queue[1 + atomicAdd(queue, 1)] = (int)plane;
@@ -686,15 +527,16 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
       bidx = oi;
     }
   }
-  if (!(best >= 0.f) || !(P.T > 0.f)) {  // NaN plane or no temperature: the CTA kernel's full evaluation
+  if (!(best >= 0.f) || !(P.T > 0.f)) {  // NaN plane or no temperature: the CTA kernel's whole-plane evaluation
     to_queue();
     return;
   }
   const int besta = bidx / w4;
   int bestb = (bidx - besta * w4) * 4;
   {
-    const float4 x = __ldg(src4 + bidx);
+    const float4 x = ld4(bidx);
     bestb += (fabsf(x.x) == best) ? 0 : ((fabsf(x.y) == best) ? 1 : ((fabsf(x.z) == best) ? 2 : 3));
+    if constexpr (!BULK) bestb = min(bestb, w - 1);
   }
   // ---- lower bound of the field maximum: exact values on the arg max's F x F block ---------------------
   int r0w = besta - DECW_WIN / 2, c0w = bestb - DECW_WIN / 2;
@@ -706,7 +548,7 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
   const float thr = mlb - DEC_CUT / P.T;
   const float theta = thr / P.lip;
 
-  // ---- pass 2: hull of the candidates (|h| >= theta), 4-column granularity like the CTA kernel -----------
+  // ---- pass 2: hull of the candidates (|h| >= theta), 4-column granularity ---------------------------------
   int amin = h, amax = -1, bmin = w, bmax = -1;
   {
     int a = 0, g = lane;  // idx = a * w4 + g
@@ -851,13 +693,13 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
   }
 }
 
-template <int DS>
-__global__ void __launch_bounds__(128) decode_fwd_warp_kernel(const __grid_constant__ DecodeParams<DS> P, int* __restrict__ queue) {
+template <int DS, bool BULK>
+__global__ void __launch_bounds__(128) decode_fwd_warp_kernel(const __grid_constant__ DecodeParams<DS> P) {
   __shared__ float tile_s[4][DECW_WIN * DECW_WP];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int plane = blockIdx.x * 4 + warp;  // n_planes < 2^31 (lpb_decode_fwd); the queue holds int plane ids as well
   if (plane >= P.n_planes) return;
-  decode_plane_warp<DS>(P, plane, P.heat + (size_t)plane * P.h * P.w, tile_s[warp], queue, lane);
+  decode_plane_warp<DS, BULK>(P, plane, P.heat + (size_t)plane * P.h * P.w, tile_s[warp], P.queue, lane);
 }
 
 // d loss / d h = U_H^T G U_W with G[i,j] = T * p[i,j] * ((j - xhat) gx + (i - yhat) gy), p the
@@ -865,22 +707,11 @@ __global__ void __launch_bounds__(128) decode_fwd_warp_kernel(const __grid_const
 // recomputes the field on its strip exactly as the forward does and scatters G through the same taps
 // into a zero-initialised smem gradient plane, which is then written out with coalesced stores.
 template <int DS>
-struct DecodeBwdParams {
-  static constexpr int F = 1 << DS, R = DS + 2, W = 2 * R + 1;
-  const float* heat;
+struct DecodeBwdParams : DecodeGeom<DS> {
   const float* stats;
   const float* gxy;
-  const float* tabH;
-  const float* tabW;
   float* gheat;
   const int* queue;      // optional {count, plane ids...}: dense fallback units of the window path
-  float lipw;            // max row sum of |horizontal taps|
-  float wabs[W];         // max over rows / phases of |vertical tap| per offset (window kernel's row pruning)
-  long long n_planes;
-  int h, w, pitch, padl, bulk;
-  float T;
-  float phase[F][W];
-  float2 phase2[F / 2][W];  // {phase[2q][t], phase[2q+1][t]}: packed-pair operands of the strip evaluation
 };
 
 // Transposed horizontal pass for one coarse row of one 32-fine-column strip: out[oc] = sum_jj gv[jj] * tabW[jj][oc - jj/F]
@@ -896,7 +727,7 @@ struct ScatterPlan {
   float wt[16];  // weight of fine column jstart + i for this lane's output column (0 outside the band / the strip)
   int oc, jstart;
   bool writer;
-  __device__ __forceinline__ void init(const float* __restrict__ tabW, int jf0, int J1, int lane) {
+  __device__ __forceinline__ void init(const DecodeGeom<DS>& g, int jf0, int J1, int lane) {
     const int part = SPLIT == 2 ? (lane & 1) : 0;
     oc = SPLIT == 2 ? (lane >> 1) : lane;
     if (SPLIT == 2) {
@@ -909,7 +740,7 @@ struct ScatterPlan {
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int jj = jstart + i, u = oc - jj / F;
-      wt[i] = (oc < NOUT && u >= 0 && u < W && jf0 + jj < J1) ? __ldg(tabW + (size_t)(jf0 + jj) * W + u) : 0.f;
+      wt[i] = (oc < NOUT && u >= 0 && u < W && jf0 + jj < J1) ? __ldg(g.tabW + (size_t)(jf0 + jj) * W + u) : 0.f;
     }
   }
 };
@@ -940,7 +771,7 @@ __device__ __forceinline__ void scatter_row(float* grow0, float gv, const Scatte
 // softmax weights of the fine field and accumulates U_H^T G U_W into gt.  `tile` / `gt` are addressed as
 // row * pitch + column with (trow0, tcol0) the tile coordinates of coarse row r0 - R and of coarse column jf0/F - R.
 template <int DS, bool ATOMIC>
-__device__ __forceinline__ void decode_bwd_strip(const DecodeBwdParams<DS>& P, const float* tile, float* gt, int pitch,
+__device__ __forceinline__ void decode_bwd_strip(const DecodeGeom<DS>& P, const float* tile, float* gt, int pitch,
                                                  int trow0, int tcol0, int maxcols, int jf0, int J1, int r0, int r1, float M,
                                                  float c, float kscale, float xhat, float yhat, float gx, float gy, int lane,
                                                  float* srow) {
@@ -954,7 +785,7 @@ __device__ __forceinline__ void decode_bwd_strip(const DecodeBwdParams<DS>& P, c
   for (int t = 0; t < W; ++t) wc[t] = __ldg(P.tabW + jc * W + t);
   const float* colbase = tile + tcol0 + (jc / F - jf0 / F);
   ScatterPlan<DS> sp;
-  sp.init(P.tabW, jf0, J1, lane);
+  sp.init(P, jf0, J1, lane);
   // Register windows over the W coarse rows a-R .. a+R that the fine rows of coarse row a touch.  They are ROTATED, not
   // shifted: the row loop is unrolled W times and in its `rot`-th copy tap t lives in slot (t + rot) % W, so advancing a
   // row costs no register moves.  The F phases are processed as pairs (packed fp32, lpb_common.cuh): `gacc[slot]` holds
@@ -1258,86 +1089,81 @@ __global__ void __launch_bounds__(DEC_THREADS) upsample2x_kernel(const float* __
 }
 
 // ------------------------------------------------------------------------------------------------
+struct DecodeDevice {
+  int max_smem;  // opt-in shared memory per block
+  int sms;
+};
+
+// Fills what both directions share and queries the device.  lip (forward): Lipschitz bound of the 2-D upsampling.
 template <int DS>
-static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, float T, float* xy, float* conf,
-                             float* stats, cudaStream_t stream) {
+static int decode_geom(DecodeGeom<DS>& g, DecodeDevice& d, const float* heat, int64_t n_planes, int h, int w, float T,
+                       float* lip = nullptr) {
   using G = UpsampleGeom<DS>;
   const DeviceTable* th = get_device_table(h, DS);
   const DeviceTable* tw = get_device_table(w, DS);
   if (!th || !tw) return LPB_ERR_INVALID;
-  DecodeParams<DS> P;
-  P.heat = heat;
-  P.tabH = th->win;
-  P.tabW = tw->win;
-  P.xy = xy;
-  P.conf = conf;
-  P.stats = stats;
-  P.h = h;
-  P.w = w;
-  P.padl = dec_padl(G::R);
-  P.pitch = dec_pitch(w, G::R);
-  P.bulk = ((w % 4) == 0 && (reinterpret_cast<uintptr_t>(heat) % 16) == 0) ? 1 : 0;
-  P.n_planes = n_planes;
-  P.T = T;
-  P.lip = th->host.lip * tw->host.lip;
-  P.offset = (DS == 1) ? 0.5f : (DS == 2 ? 1.5f : 2.5f);  // lightning_pose/models/heads/heatmap.py:131-136
-  for (int p = 0; p < G::F; ++p)
-    for (int t = 0; t < G::W; ++t) P.phase[p][t] = th->host.phase[(size_t)p * G::W + t];
-  for (int q = 0; q < G::F / 2; ++q)
-    for (int t = 0; t < G::W; ++t) P.phase2[q][t] = make_float2(P.phase[2 * q][t], P.phase[2 * q + 1][t]);
-  const size_t smem = ((size_t)(h + 2 * G::R) * P.pitch + 64 + 112 + 704) * sizeof(float) + 16;
-  int dev = 0, max_smem = 0;
-  LPB_CUDA(cudaGetDevice(&dev));
-  LPB_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if ((int64_t)smem > max_smem) {
-    set_error("decode: plane %dx%d needs %zu B shared memory (> %d)", h, w, smem, max_smem);
-    return LPB_ERR_UNSUPPORTED;
-  }
-  LPB_CUDA(cudaFuncSetAttribute(decode_fwd_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0, per_sm = 0;
-  LPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  LPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_fwd_kernel<DS>, DEC_THREADS, smem));
-  const int64_t resident = (int64_t)sms * (per_sm > 0 ? per_sm : 1);  // persistent CTAs: one wave
-  P.queue = nullptr;
-  P.qcounter = nullptr;
-  P.qscratch = nullptr;
-  P.lipw = tw->host.lip;
+  g.heat = heat;
+  g.tabH = th->win;
+  g.tabW = tw->win;
+  g.h = h;
+  g.w = w;
+  g.padl = dec_padl(G::R);
+  g.pitch = dec_pitch(w, G::R);
+  g.bulk = ((w % 4) == 0 && aligned_to(heat, 16)) ? 1 : 0;
+  g.n_planes = n_planes;
+  g.T = T;
+  g.lipw = tw->host.lip;
   for (int t = 0; t < G::W; ++t) {
     float m = 0.f;
     for (size_t i = 0; i < (size_t)h * G::F; ++i) m = std::fmax(m, std::fabs(th->host.win[i * G::W + t]));
-    P.wabs[t] = m * (1.0f + 1e-6f);
+    g.wabs[t] = m * (1.0f + 1e-6f);
   }
-  if (P.bulk && getenv("LPB_DECODE_CTA_ONLY") == nullptr) {
-    // warp-per-plane first; what it cannot take (diffuse / multi-modal / NaN planes) is queued for the CTA kernel
-    int* queue = nullptr;  // [1 + n queue][n counters][n * 8 * 4 floats of partial states]
-    const size_t qints = (size_t)(2 * n_planes + 1) + (size_t)n_planes * DEC_MAX_PARTS * 4;
-    {
-      // The scratch comes from the device's stream-ordered pool.  With the pool's default release threshold (0) the
-      // driver hands freed memory back to the OS at every synchronisation point, so each eager call pays a fresh
-      // allocation (measured: the same decode taking 0.05 or 0.26 ms, and a 20x slower eager prediction loop); keep
-      // freed blocks in the pool instead.  Once per device.
-      static bool pool_ready[64] = {};
-      if (dev >= 0 && dev < 64 && !pool_ready[dev]) {
-        cudaMemPool_t pool;
-        if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-          uint64_t thr = UINT64_MAX;
-          (void)cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
-        }
-        (void)cudaGetLastError();
-        pool_ready[dev] = true;
-      }
-    }
-    LPB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&queue), sizeof(int) * qints, stream));
-    LPB_CUDA(cudaMemsetAsync(queue, 0, sizeof(int) * (size_t)(2 * n_planes + 1), stream));
-    decode_fwd_warp_kernel<DS><<<(unsigned)((n_planes + 3) / 4), 128, 0, stream>>>(P, queue);
-    P.queue = queue;
-    P.qcounter = queue + 1 + n_planes;
-    P.qscratch = reinterpret_cast<float*>(queue + 1 + 2 * n_planes);
-    decode_fwd_kernel<DS><<<(unsigned)(n_planes < resident ? n_planes : resident), DEC_THREADS, smem, stream>>>(P);
-    LPB_CUDA(cudaFreeAsync(queue, stream));
-  } else {
-    decode_fwd_kernel<DS><<<(unsigned)(n_planes < resident ? n_planes : resident), DEC_THREADS, smem, stream>>>(P);
+  for (int q = 0; q < G::F / 2; ++q)
+    for (int t = 0; t < G::W; ++t)
+      g.phase2[q][t] = make_float2(th->host.phase[(size_t)(2 * q) * G::W + t], th->host.phase[(size_t)(2 * q + 1) * G::W + t]);
+  if (lip) *lip = th->host.lip * tw->host.lip;
+  int dev = 0;
+  LPB_CUDA(cudaGetDevice(&dev));
+  LPB_CUDA(cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  LPB_CUDA(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
+  return LPB_OK;
+}
+
+// forward workspace: {queue count, queued plane ids}[1 + n] and arrival counters[n] (ints, zeroed by every call), then the
+// partial softmax states of split planes, float[n][DEC_MAX_PARTS][4]
+static size_t decode_fwd_workspace_bytes(int64_t n_planes) {
+  return sizeof(int) * (size_t)(2 * n_planes + 1) + sizeof(float) * (size_t)n_planes * DEC_MAX_PARTS * 4;
+}
+
+template <int DS>
+static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, float T, float* xy, float* conf,
+                             float* stats, void* workspace, cudaStream_t stream) {
+  using G = UpsampleGeom<DS>;
+  DecodeParams<DS> P;
+  DecodeDevice dev;
+  if (const int rc = decode_geom<DS>(P, dev, heat, n_planes, h, w, T, &P.lip); rc != LPB_OK) return rc;
+  P.xy = xy;
+  P.conf = conf;
+  P.stats = stats;
+  P.offset = (DS == 1) ? 0.5f : (DS == 2 ? 1.5f : 2.5f);  // lightning_pose/models/heads/heatmap.py:131-136
+  P.queue = static_cast<int*>(workspace);
+  P.qcounter = P.queue + 1 + n_planes;
+  P.qscratch = reinterpret_cast<float*>(P.queue + 1 + 2 * n_planes);
+  const size_t smem = ((size_t)(h + 2 * G::R) * P.pitch + DEC_FWD_SCRATCH) * sizeof(float) + 16;
+  if ((int64_t)smem > dev.max_smem) {
+    set_error("decode: plane %dx%d needs %zu B shared memory (> %d)", h, w, smem, dev.max_smem);
+    return LPB_ERR_UNSUPPORTED;
   }
+  LPB_CUDA(cudaFuncSetAttribute(decode_fwd_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 0;
+  LPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_fwd_kernel<DS>, DEC_THREADS, smem));
+  const int64_t resident = (int64_t)dev.sms * (per_sm > 0 ? per_sm : 1);  // persistent CTAs: one wave
+  // warp per plane first; what it cannot take (diffuse / multi-modal / NaN planes) is queued for the CTA kernel
+  LPB_CUDA(cudaMemsetAsync(P.queue, 0, sizeof(int) * (size_t)(2 * n_planes + 1), stream));
+  const unsigned wgrid = (unsigned)((n_planes + 3) / 4);
+  if (P.bulk) decode_fwd_warp_kernel<DS, true><<<wgrid, 128, 0, stream>>>(P);
+  else decode_fwd_warp_kernel<DS, false><<<wgrid, 128, 0, stream>>>(P);
+  decode_fwd_kernel<DS><<<(unsigned)(n_planes < resident ? n_planes : resident), DEC_THREADS, smem, stream>>>(P);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
@@ -1347,53 +1173,25 @@ static int launch_decode_bwd(const float* heat, const float* stats, const float*
                              float T, float* gheat, cudaStream_t stream, float* win = nullptr, int* meta = nullptr,
                              int* queue = nullptr) {
   using G = UpsampleGeom<DS>;
-  const DeviceTable* th = get_device_table(h, DS);
-  const DeviceTable* tw = get_device_table(w, DS);
-  if (!th || !tw) return LPB_ERR_INVALID;
   DecodeBwdParams<DS> P;
-  P.heat = heat;
+  DecodeDevice dev;
+  if (const int rc = decode_geom<DS>(P, dev, heat, n_planes, h, w, T); rc != LPB_OK) return rc;
   P.stats = stats;
   P.gxy = gxy;
-  P.tabH = th->win;
-  P.tabW = tw->win;
   P.gheat = gheat;
   P.queue = queue;
-  P.lipw = tw->host.lip;
-  for (int t = 0; t < G::W; ++t) {
-    float m = 0.f;
-    for (size_t i = 0; i < (size_t)h * G::F; ++i) m = std::fmax(m, std::fabs(th->host.win[i * G::W + t]));
-    P.wabs[t] = m * (1.0f + 1e-6f);
-  }
-  P.n_planes = n_planes;
-  P.h = h;
-  P.w = w;
-  P.padl = dec_padl(G::R);
-  P.pitch = dec_pitch(w, G::R);
-  P.bulk = ((w % 4) == 0 && (reinterpret_cast<uintptr_t>(heat) % 16) == 0) ? 1 : 0;
-  P.T = T;
-  for (int p = 0; p < G::F; ++p)
-    for (int t = 0; t < G::W; ++t) P.phase[p][t] = th->host.phase[(size_t)p * G::W + t];
-  for (int q = 0; q < G::F / 2; ++q)
-    for (int t = 0; t < G::W; ++t) P.phase2[q][t] = make_float2(P.phase[2 * q][t], P.phase[2 * q + 1][t]);
   if (win) {  // sparse windows first; the dense kernel below then only runs the planes they queued
     LPB_CUDA(cudaMemsetAsync(queue, 0, sizeof(int), stream));
     decode_bwd_window_kernel<DS><<<(unsigned)((n_planes + 3) / 4), 128, 0, stream>>>(P, win, meta, queue);
   }
   const size_t smem = ((size_t)2 * (h + 2 * G::R) * P.pitch + DEC_WARPS * 64) * sizeof(float) + 16;
-  int dev = 0, max_smem = 0;
-  LPB_CUDA(cudaGetDevice(&dev));
-  LPB_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if ((int64_t)smem > max_smem) {
-    set_error("decode_bwd: plane %dx%d needs %zu B shared memory (> %d)", h, w, smem, max_smem);
+  if ((int64_t)smem > dev.max_smem) {
+    set_error("decode_bwd: plane %dx%d needs %zu B shared memory (> %d)", h, w, smem, dev.max_smem);
     return LPB_ERR_UNSUPPORTED;
   }
   LPB_CUDA(cudaFuncSetAttribute(decode_bwd_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   unsigned grid = (unsigned)n_planes;
-  if (queue) {  // queue mode: one wave of resident CTAs
-    int sms = 0;
-    LPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    if (grid > (unsigned)(2 * sms)) grid = (unsigned)(2 * sms);
-  }
+  if (queue && grid > (unsigned)(2 * dev.sms)) grid = (unsigned)(2 * dev.sms);  // queue mode: one wave of resident CTAs
   decode_bwd_kernel<DS><<<grid, DEC_THREADS, smem, stream>>>(P);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
@@ -1408,12 +1206,22 @@ extern "C" int lpb_decode_prepare(int h, int w, int ds) {
   return LPB_OK;
 }
 
+extern "C" int lpb_decode_fwd_workspace_bytes(int64_t n_planes, size_t* bytes) {
+  using namespace lpb;
+  LPB_REQUIRE(bytes, "decode_fwd_workspace_bytes: null pointer");
+  LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "decode_fwd_workspace_bytes: bad n_planes");
+  *bytes = decode_fwd_workspace_bytes(n_planes);
+  return LPB_OK;
+}
+
 extern "C" int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
-                              float* xy, float* conf, float* stats, void* stream) {
+                              float* xy, float* conf, float* stats, void* workspace, void* stream) {
   using namespace lpb;
   LPB_REQUIRE(heatmaps && xy && conf, "decode_fwd: null pointer");
   LPB_REQUIRE(h >= 1 && w >= 1 && ds >= 1 && ds <= 3, "decode_fwd: bad shape h=%d w=%d ds=%d", h, w, ds);
   LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "decode_fwd: bad n_planes");
+  LPB_REQUIRE(workspace || n_planes == 0, "decode_fwd: null workspace");
+  LPB_REQUIRE(aligned_to(workspace, 4), "decode_fwd: workspace must be 4-byte aligned");
   if (((int64_t)w << ds) > 1024 || w > 256) {
     lpb::set_error("decode_fwd: heatmap width %d (x%d) exceeds this build's 1024-column field limit", w, 1 << ds);
     return LPB_ERR_UNSUPPORTED;
@@ -1421,9 +1229,9 @@ extern "C" int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, in
   if (n_planes == 0) return LPB_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   switch (ds) {
-    case 1: return launch_decode_fwd<1>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s);
-    case 2: return launch_decode_fwd<2>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s);
-    default: return launch_decode_fwd<3>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, s);
+    case 1: return launch_decode_fwd<1>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s);
+    case 2: return launch_decode_fwd<2>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s);
+    default: return launch_decode_fwd<3>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s);
   }
 }
 

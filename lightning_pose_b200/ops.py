@@ -66,8 +66,11 @@ def decode_forward(heatmaps: torch.Tensor, ds: int, temperature: float):
     xy = torch.empty((b, k, 2), device=heatmaps.device, dtype=torch.float32)
     conf = torch.empty((b, k), device=heatmaps.device, dtype=torch.float32)
     stats = torch.empty((b, k, 8), device=heatmaps.device, dtype=torch.float32)
+    nbytes = C.c_size_t(0)
+    check(lib.lpb_decode_fwd_workspace_bytes(b * k, C.byref(nbytes)))
+    workspace = torch.empty((nbytes.value,), device=heatmaps.device, dtype=torch.uint8)
     with torch.cuda.device(heatmaps.device):
-        check(lib.lpb_decode_fwd(_ptr(heatmaps), b * k, h, w, ds, temperature, _ptr(xy), _ptr(conf), _ptr(stats), _stream()))
+        check(lib.lpb_decode_fwd(_ptr(heatmaps), b * k, h, w, ds, temperature, _ptr(xy), _ptr(conf), _ptr(stats), _ptr(workspace), _stream()))
     return xy, conf, stats
 
 

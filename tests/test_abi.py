@@ -38,7 +38,7 @@ def test_library_exports_every_declared_symbol():
 def test_entry_points_validate_arguments_without_gpu():
     from lightning_pose_b200 import _lib
 
-    rc = _lib.lib.lpb_decode_fwd(None, 1, 8, 8, 2, 1000.0, None, None, None, None)
+    rc = _lib.lib.lpb_decode_fwd(None, 1, 8, 8, 2, 1000.0, None, None, None, None, None)
     assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
     rc = _lib.lib.lpb_decode_prepare(8, 8, 7)
     assert rc == -1 and b"bad shape" in _lib.lib.lpb_last_error()
@@ -114,6 +114,26 @@ def test_head_training_entry_points_validate_without_gpu():
     assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
     rc = _lib.lib.lpb_decode_bwd_windows(None, None, None, 1, 8, 8, 2, 1000.0, None, None, None, None, None)
     assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
+
+
+def test_decode_fwd_workspace_without_gpu():
+    """The forward decode's scratch is the caller's: (2n + 1) ints of queue and arrival counters, then n x 16 x 4 floats of
+    partial softmax states.  The size query needs no GPU, and lpb_decode_fwd refuses a missing or misaligned workspace
+    before it queues anything (the other pointers are fake)."""
+    from lightning_pose_b200 import _lib
+
+    L = _lib.lib
+    n = ctypes.c_size_t(0)
+    for planes in (0, 1, 17, 768 * 17):
+        assert L.lpb_decode_fwd_workspace_bytes(planes, ctypes.byref(n)) == 0
+        assert n.value == 4 * (2 * planes + 1) + 4 * planes * 16 * 4
+    assert L.lpb_decode_fwd_workspace_bytes(-1, ctypes.byref(n)) == -1
+    assert L.lpb_decode_fwd_workspace_bytes(1, None) == -1
+    fake = ctypes.c_void_p(0x1000)
+    rc = L.lpb_decode_fwd(fake, 17, 96, 96, 2, 1000.0, fake, fake, fake, None, None)
+    assert rc == -1 and L.lpb_last_error() == b"decode_fwd: null workspace"
+    rc = L.lpb_decode_fwd(fake, 17, 96, 96, 2, 1000.0, fake, fake, fake, ctypes.c_void_p(0x1002), None)
+    assert rc == -1 and L.lpb_last_error() == b"decode_fwd: workspace must be 4-byte aligned"
 
 
 _BWD_VECTOR_BUFFERS = ["dfeat", "g_out", "probs", "win_meta", "g_overflow", "saved_xs", "fwd_workspace", "workspace"]
