@@ -138,11 +138,19 @@ int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, in
 
 /* bf16 tensor-core path (tensor-core mma): features bf16 NCHW, fp32 master weights (rounded to bf16 on device, as
  * autocast does), fp32 accumulate, fp32 heatmaps.  One-deconv heads (ViT family, heads/heatmap.py:192-193: pass
- * w2 = b2 = NULL, c2 = 0) and two-deconv heads (ResNet family); C % 128 == 0, H*W % 8 == 0, c1, c2 <= 20 (c1 < 20 for
- * two deconvs).  Two kernel families serve it: whole-frame kernels for two-deconv heads on feature maps up to
- * 12x12 ("fast path"), and banded kernels for everything else (one-deconv heads, 16x16 / 24x24 ... maps).
+ * w2 = b2 = NULL, c2 = 0) and two-deconv heads (ResNet family); C % 128 == 0, H*W % 8 == 0, and channel counts of
+ *   narrow heads: c1, c2 <= 20 (c1 < 20 for two deconvs), or
+ *   wide heads:   a last layer of 21 .. LPB_HEAD_MAX_CHANNELS channels (c1 > 20 for one deconv, c2 > 20 for two) and
+ *                 1 <= c1 <= LPB_HEAD_MAX_CHANNELS in front of it.
+ * The output channels of a wide layer are keypoint groups of 20, each one GEMM of a banded-kernel work item.
+ * Two kernel families serve it: whole-frame kernels for narrow two-deconv heads on feature maps up to
+ * 12x12 ("fast path"), and banded kernels for everything else (one-deconv heads, 16x16 / 24x24 ... maps, wide heads).
  * lpb_head_bf16_plan reports which one a shape takes: plan[0] = 1 fast path, 0 banded (then saved_xs is REQUIRED by
- * lpb_head_fwd_bf16: it is the pixel-shuffled operand itself); LPB_ERR_UNSUPPORTED if neither fits. */
+ * lpb_head_fwd_bf16: it is the pixel-shuffled operand itself); LPB_ERR_UNSUPPORTED if neither fits or the last layer
+ * has more than LPB_HEAD_MAX_CHANNELS channels (the head then runs the fp32 kernels).  The cap is four keypoint groups:
+ * the forward's registers and shared memory do not grow with the group count (a group is a work item), so it bounds the
+ * workspace and the range the tests cover. */
+#define LPB_HEAD_MAX_CHANNELS 80
 int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan);
 int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes);
 int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
@@ -165,7 +173,7 @@ int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes);
  *   NULL when the head returns logits.
  * dfeat [B, C, H, W] bf16 or NULL (frozen backbone); dw1 [C/4, c1, 3, 3], db1 [c1], dw2 [c1, c2, 3, 3],
  * db2 [c2] fp32 (overwritten).  One-deconv heads: w2 = dw2 = db2 = NULL, c2 = 0 (output [B, c1, 4H, 4W]).
- * Shapes: the forward's channel limits, and feature maps with H even, W in {4, 8, 12, 16, 24, 32}; both entries return
+ * Shapes: the forward's channel limits (narrow and wide heads), and feature maps with H even, W in {4, 8, 12, 16, 24, 32}; both entries return
  * LPB_ERR_UNSUPPORTED for any other shape, so lpb_head_bwd_bf16_workspace_bytes (which needs no GPU) tells whether a
  * head can train on this path.  workspace: lpb_head_bwd_bf16_workspace_bytes() bytes.  g_out, probs, win_meta,
  * g_overflow, saved_xs, fwd_workspace, dfeat and workspace must be 16-byte aligned (LPB_ERR_INVALID otherwise, before

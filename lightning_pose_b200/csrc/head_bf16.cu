@@ -32,8 +32,9 @@
 namespace lpb {
 
 // ---- everything a head call prepares, in one launch (head_prep.cuh) -------------------------------------------
-// forward packs: W[Cin][Cout][3][3] (fp32) -> B[stage][shift][kchunk][80][8] bf16; a non-null bias rides on input
-// channel `Cin` (the constant-one channel of the mid activations; shift (0,0) only, which every output class uses once)
+// forward packs: W[Cin][Cout][3][3] (fp32) -> B[group][stage][shift][kchunk][80][8] bf16 (output channel
+// o = HEAD_CLS * group + column % HEAD_CLS); a non-null bias rides on input channel `Cin` (the constant-one channel of the
+// mid activations; shift (0,0) only, which every output class uses once)
 __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ PrepJobs J) {
   const long long tid0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
 #pragma unroll
@@ -41,8 +42,8 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
     if (!J.fpack[j].out) continue;
     const float* w = J.fpack[j].w;
     const float* bias = J.fpack[j].bias;
-    const int Cin = J.fpack[j].Cin, Cout = J.fpack[j].Cout;
-    const long long total = (long long)J.fpack[j].nstages * 4 * 4 * HEAD_NCOLS * 8;
+    const int Cin = J.fpack[j].Cin, Cout = J.fpack[j].Cout, nst = J.fpack[j].nstages;
+    const long long total = (long long)J.fpack[j].ngroups * nst * 4 * 4 * HEAD_NCOLS * 8;
     for (long long i = tid0; i < total; i += nthr) {
       const int e = (int)(i & 7);
       long long r = i >> 3;
@@ -51,9 +52,10 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
       const int kc = (int)(r & 3);
       r >>= 2;
       const int sh = (int)(r & 3);
-      const int st = (int)(r >> 2);
+      r >>= 2;
+      const int st = (int)(r % nst), grp = (int)(r / nst);
       const int c = st * HEAD_KSTAGE + kc * 8 + e;
-      const int cls = nrow / HEAD_CLS, o = nrow % HEAD_CLS;
+      const int cls = nrow / HEAD_CLS, o = grp * HEAD_CLS + nrow % HEAD_CLS;
       const int py = cls >> 1, px = cls & 1, dm = sh >> 1, dn = sh & 1;
       float v = 0.f;
       if (c < Cin && o < Cout && tap_nonzero(cls, sh)) {
@@ -70,8 +72,9 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
   for (int j = 0; j < 2; ++j) {
     if (!J.dpack[j].out) continue;
     const float* w = J.dpack[j].w;
-    const int Cin = J.dpack[j].Cin, Cout = J.dpack[j].Cout, rpt = J.dpack[j].rows_per_tile;
-    const long long total = (long long)J.dpack[j].ntiles * 4 * HEAD_KC * rpt * 8;
+    const int Cin = J.dpack[j].Cin, Cout = J.dpack[j].Cout, rpt = J.dpack[j].rows_per_tile, tch = J.dpack[j].tile_ch;
+    const int ntiles = J.dpack[j].ntiles;
+    const long long total = (long long)J.dpack[j].kgroups * ntiles * 4 * HEAD_KC * rpt * 8;
     for (long long i = tid0; i < total; i += nthr) {
       const int e = (int)(i & 7);
       long long r = i >> 3;
@@ -80,13 +83,14 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
       const int kc = (int)(r % HEAD_KC);
       r /= HEAD_KC;
       const int sh = (int)(r & 3);
-      const int tile = (int)(r >> 2);
-      const int c = tile * rpt + row;
+      r >>= 2;
+      const int tile = (int)(r % ntiles), kg = (int)(r / ntiles);
+      const int c = tile * tch + row;
       const int k = kc * 8 + e;
-      const int cls = k / HEAD_CLS, o = k % HEAD_CLS;
+      const int cls = k / HEAD_CLS, o = kg * HEAD_CLS + k % HEAD_CLS;
       const int py = cls >> 1, px = cls & 1, dm = sh >> 1, dn = sh & 1;
       float v = 0.f;
-      if (c < Cin && o < Cout && tap_nonzero(cls, sh)) {
+      if (row < tch && c < Cin && o < Cout && tap_nonzero(cls, sh)) {
         const int ky = py == 0 ? 1 : (dm ? 0 : 2);
         const int kx = px == 0 ? 1 : (dn ? 0 : 2);
         v = w[((size_t)c * Cout + o) * 9 + ky * 3 + kx];
@@ -505,15 +509,22 @@ static int device_limits(int* max_smem, int* sms) {
   return 0;
 }
 
-// plan[0] = 1: fast path (saved_xs optional: training only); 0: generic path (saved_xs REQUIRED: it is the operand)
+static_assert(lpb::HEAD_MAX_CH == LPB_HEAD_MAX_CHANNELS, "the cap lpb200.h states is the keypoint groups' (head_prep.cuh)");
+
+// plan[0] = 1: fast path (saved_xs optional: training only); 0: generic path (saved_xs REQUIRED: it is the operand).
+// Wide heads (more than HEAD_CLS keypoints, head_prep.cuh) always take the generic path.
 extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan) {
   using namespace lpb;
   LPB_REQUIRE(plan, "head_bf16_plan: null pointer");
   LPB_REQUIRE(C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && (H * W) % 8 == 0 && c1 >= 1 && c2 >= 0, "head_bf16_plan: bad shape");
-  LPB_REQUIRE(c2 == 0 ? c1 <= HEAD_CLS : (c1 < HEAD_CLS && c2 <= HEAD_CLS), "head_bf16_plan: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
+  if ((c2 > 0 ? c2 : c1) > HEAD_CLS && !head_wide(c1, c2)) {
+    set_error("head_bf16_plan: channel counts %d/%d exceed the keypoint groups of this build (%d channels per layer)", c1, c2, HEAD_MAX_CH);
+    return LPB_ERR_UNSUPPORTED;
+  }
+  LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "head_bf16_plan: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
   int max_smem, sms;
   device_limits(&max_smem, &sms);
-  plan[0] = head_fast_path(C, H, W, c2, max_smem) ? 1 : 0;
+  plan[0] = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, max_smem) ? 1 : 0;
   if (!plan[0] && ((size_t)32 * H * W * 2 > 200 * 1024 || (c2 > 0 ? 4 : 2) * W + 1 > CR_BAND_ROWS)) {
     set_error("head_bf16_plan: feature map %dx%d too large for this build", H, W);
     return LPB_ERR_UNSUPPORTED;
@@ -532,7 +543,7 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
   using namespace lpb;
   LPB_REQUIRE(bytes, "head_bf16_workspace_bytes: null pointer");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_bf16_workspace_bytes: bad shape");
-  *bytes = head_fwd_layout(B, C, H, W, c2).total;
+  *bytes = head_fwd_layout(B, C, H, W, c1, c2).total;
   return LPB_OK;
 }
 
@@ -544,8 +555,7 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   LPB_REQUIRE(c2 == 0 || (w2 && b2), "head_fwd_bf16: a two-deconv head needs w2 and b2");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "head_fwd_bf16: bad feature shape C=%d H=%d W=%d", C, H, W);
   LPB_REQUIRE((H * W) % 8 == 0, "head_fwd_bf16: H*W must be a multiple of 8 (got %d)", H * W);
-  LPB_REQUIRE(c2 == 0 ? (c1 >= 1 && c1 <= HEAD_CLS) : (c1 >= 1 && c1 < HEAD_CLS && c2 >= 1 && c2 <= HEAD_CLS),
-              "head_fwd_bf16: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
+  LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "head_fwd_bf16: channel counts %d/%d outside this build's set (lpb200.h)", c1, c2);
   // features: TMA or uint4 loads; saved_xs, workspace: bulk copies and uint4 stores; out: float2 stores
   LPB_REQUIRE(aligned_to(features, 16), "head_fwd_bf16: features must be 16-byte aligned");
   LPB_REQUIRE(aligned_to(saved_xs, 16), "head_fwd_bf16: saved_xs must be 16-byte aligned");
@@ -555,7 +565,7 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   int max_smem = 0, sms = 0;
   device_limits(&max_smem, &sms);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bool fast = head_fast_path(C, H, W, c2, max_smem);
+  const bool fast = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, max_smem);
   const K1aGeom k1 = make_k1a_geom(H, W);
   // k1a's feature tensor map, encoded before anything is queued, so a failure leaves the stream untouched.  The plan stays
   // a function of the shape (CPU-only callers size buffers with it); every driver that runs sm_90a code has the encoder,
@@ -565,10 +575,10 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     set_error("head_fwd_bf16: cannot encode the feature tensor map");
     return LPB_ERR_INVALID;
   }
-  const int nst = C / 4 / HEAD_KSTAGE;
+  const int nst = C / 4 / HEAD_KSTAGE, nst2 = head_mid_stages(c1);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const RowLayout Lxs = make_row_layout(2 * H, 2 * W), Lmid = make_row_layout(4 * H, 4 * W);
-  const HeadFwdLayout wl = head_fwd_layout(B, C, H, W, c2);
+  const HeadFwdLayout wl = head_fwd_layout(B, C, H, W, c1, c2);
   __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.w1);
   __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.w2);
   __nv_bfloat16* mid = reinterpret_cast<__nv_bfloat16*>(ws + wl.mid);
@@ -577,12 +587,12 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     // one launch: both operand packs + the pad rows of the fresh row-layout buffers (k1a writes every row of the saved
     // copy itself; the banded path's shuffle kernel writes its own pads)
     PrepJobs jobs{};
-    jobs.fpack[0] = {w1, nullptr, C / 4, c1, nst, wp1};
+    jobs.fpack[0] = {w1, nullptr, C / 4, c1, nst, head_groups(c1), wp1};
     // layer 2: bias rides on the constant-one channel c1 of the mid activations (only needed without softmax:
     // a per-plane constant does not change a softmax)
     if (c2 > 0) {
-      jobs.fpack[1] = {w2, final_softmax ? nullptr : b2, c1, c2, 1, wp2};
-      jobs.pads[0] = {mid, Lmid, (long long)B * 4};
+      jobs.fpack[1] = {w2, final_softmax ? nullptr : b2, c1, c2, nst2, head_groups(c2), wp2};
+      jobs.pads[0] = {mid, Lmid, (long long)B * 4 * nst2};
     }
     launch_head_prep(jobs, s);
   }
@@ -613,6 +623,7 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     p.mode = CONVT_ROWS_MID;
     p.mid = mid;
     p.Lout = Lmid;
+    p.mid_kc = 4 * nst2;
     rc = launch_convt_rows(p, sms, s);
     if (rc != LPB_OK) return rc;
   } else {
@@ -645,7 +656,7 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   p2.L = Lmid;
   p2.wpk = wp2;
   p2.bias = nullptr;  // folded into the GEMM through the ones channel (see the pack above)
-  p2.nst = 1;
+  p2.nst = nst2;
   p2.B = B;
   p2.cout = c2;
   p2.out = out;

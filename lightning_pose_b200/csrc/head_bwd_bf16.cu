@@ -106,19 +106,21 @@ __global__ void __launch_bounds__(256) plane_dot_sparse_kernel(G2Src S, long lon
 constexpr int G2B_THREADS = 128;
 
 // HAS_OV (pass ahead of the patch kernel): planes whose decode gradient is dense (flag 2, the decode's overflow buffer) are
-// added here, in the streaming pass -- in the fresh-init regime that is every plane.
+// added here, in the streaming pass -- in the fresh-init regime that is every plane.  blockIdx.y is the keypoint group
+// (head_prep.cuh): planes [20 g, 20 g + 20) of the C, written to the group's 10 K-chunks of the frame's gridDim.y * 10.
 template <bool HAS_G, bool HAS_P, bool HAS_OV>
 __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B, int C, int Hi, int Wi, int ctas_per_frame,
                                                                __nv_bfloat16* __restrict__ G, RowLayout L) {
   const int b = blockIdx.x / ctas_per_frame, t0 = (blockIdx.x - b * ctas_per_frame) * G2B_THREADS, t = t0 + threadIdx.x;
   const int Wo = 2 * Wi, Ho = 2 * Hi;
+  const int g = blockIdx.y, o0 = HEAD_CLS * g, cg = min(HEAD_CLS, C - o0);
   __shared__ float sdot[HEAD_CLS];
   __shared__ unsigned sov;
   if (threadIdx.x < HEAD_CLS) {
     float d = 0.f;
     int4 mt = make_int4(0, 0, 0, 0);
-    if (threadIdx.x < C) {
-      const size_t plane = (size_t)b * C + threadIdx.x;
+    if (threadIdx.x < cg) {
+      const size_t plane = (size_t)b * C + o0 + threadIdx.x;
       if (S.meta) mt = reinterpret_cast<const int4*>(S.meta)[plane];
       if (HAS_P) {
         if (mt.z == 1) d = __int_as_float(mt.w);
@@ -137,14 +139,14 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
 #pragma unroll
   for (int py = 0; py < 2; ++py) {
     const int y = 2 * m + py, x = 2 * n;
-    const size_t off0 = (((size_t)b * C) * Ho + y) * Wo + x;
+    const size_t off0 = (((size_t)b * C + o0) * Ho + y) * Wo + x;
     const size_t pstride = (size_t)Ho * Wo;
     float2 pv[HEAD_CLS], gv[HEAD_CLS];
 #pragma unroll
     for (int o = 0; o < HEAD_CLS; ++o) {
       pv[o] = make_float2(0.f, 0.f);
       gv[o] = make_float2(0.f, 0.f);
-      if (o < C) {
+      if (o < cg) {
         if (HAS_P) pv[o] = __ldg(reinterpret_cast<const float2*>(S.probs + off0 + o * pstride));
         if (HAS_G) gv[o] = __ldg(reinterpret_cast<const float2*>(S.g_out + off0 + o * pstride));
       }
@@ -153,7 +155,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
       const unsigned ovm = sov;
 #pragma unroll
       for (int o = 0; o < HEAD_CLS; ++o) {
-        if (o < C && ((ovm >> o) & 1u)) {
+        if (o < cg && ((ovm >> o) & 1u)) {
           const float2 u = __ldg(reinterpret_cast<const float2*>(S.gov + off0 + o * pstride));
           gv[o].x += u.x, gv[o].y += u.y;
         }
@@ -179,7 +181,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
         __nv_bfloat162 h2 = __floats2bfloat162_rn(f0, f1);
         pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
       }
-      *reinterpret_cast<uint4*>(G + ((((size_t)b * HEAD_KC + 5 * py + ch) * L.rows) + L.lead + (size_t)m * L.Pp + n) * 8) =
+      *reinterpret_cast<uint4*>(G + ((((size_t)(b * gridDim.y + g) * HEAD_KC + 5 * py + ch) * L.rows) + L.lead + (size_t)m * L.Pp + n) * 8) =
           make_uint4(pk[0], pk[1], pk[2], pk[3]);
     }
   }
@@ -200,7 +202,7 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
     int4 mt = make_int4(0, 0, 0, 0);
     if (plane < n_planes) mt = reinterpret_cast<const int4*>(S.meta)[plane];
     if (mt.z == 1) {
-      const int b = (int)(plane / C), o = (int)(plane - (long long)b * C);
+      const int b = (int)(plane / C), oc = (int)(plane - (long long)b * C), g = oc / HEAD_CLS, o = oc - g * HEAD_CLS;
       float dot = 0.f;
       if (HAS_P) dot = __int_as_float(mt.w) + (S.ddot ? S.ddot[plane] : 0.f);
       const size_t poff = (size_t)plane * Ho * Wo;
@@ -209,7 +211,7 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
       const bool xin = (unsigned)x < (unsigned)Wo;
       // k = cls * 20 + o with cls = 2 (y & 1) + (x & 1): the K-chunk / element of this lane for even and odd rows
       const int kx = (x & 1) * HEAD_CLS + o;
-      __nv_bfloat16* gcol = G + ((size_t)b * HEAD_KC * L.rows + L.lead + (x >> 1)) * 8;
+      __nv_bfloat16* gcol = G + ((size_t)(b * head_groups(C) + g) * HEAD_KC * L.rows + L.lead + (x >> 1)) * 8;
 #pragma unroll 1
       for (int r0 = 0; r0 < 32; r0 += 8) {
         float gw[8], pv[8], go[8];
@@ -239,11 +241,12 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
 template <bool HAS_G, bool HAS_P>
 static void launch_g2_build(const G2Src& S, int B, int C, int Hi, int Wi, __nv_bfloat16* G, RowLayout L, cudaStream_t s) {
   const int cpf = (Hi * Wi + G2B_THREADS - 1) / G2B_THREADS;
+  const dim3 grid((unsigned)(B * cpf), (unsigned)head_groups(C));
   if (!S.win) {
-    g2_build_kernel<HAS_G, HAS_P, false><<<(unsigned)(B * cpf), G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
+    g2_build_kernel<HAS_G, HAS_P, false><<<grid, G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
     return;
   }
-  g2_build_kernel<HAS_G, HAS_P, true><<<(unsigned)(B * cpf), G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
+  g2_build_kernel<HAS_G, HAS_P, true><<<grid, G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
   const long long np = (long long)B * C;
   g2_patch_kernel<HAS_G, HAS_P><<<(unsigned)((np + 3) / 4), 128, 0, s>>>(S, np, C, Hi, Wi, G, L);
 }
@@ -265,8 +268,14 @@ struct B2dParams {
   float* db1_part;            // [gridDim.x * 4 MMA warps][HEAD_CLS]: each warp's bias-gradient sum (reduced in a fixed order)
   int B, Hi, Wi, c1;
   int R2;                     // image rows per chunk
+  // WIDE (keypoint groups): one launch per (c1 group, c2 group), c2 groups in order.  K is c2 group kc0 / 10 of the
+  // frame's kc_frame K-chunks of G2; the columns are mid channels [o0, o0 + cg); the result goes to (accumulate = 0) or is
+  // added to (1) the fp32 planes dmid, which the G1 writer reads afterwards.
+  float* dmid;                // [B][c1][Hi * Wi]
+  int kc_frame, kc0, o0, cg, accumulate;
 };
 
+template <bool WIDE>
 __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_constant__ B2dParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1;
@@ -312,7 +321,8 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
           if (lane == 0) mbar_expect_tx(a_full, HEAD_KC * nbytes);
           __syncwarp((1u << HEAD_KC) - 1);
           bulk_g2s(As + (size_t)lane * rows_alloc * 16,
-                   P.G2 + (((size_t)b * HEAD_KC + lane) * P.L2.rows + P.L2.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, a_full);
+                   P.G2 + (((size_t)b * (WIDE ? P.kc_frame : HEAD_KC) + (WIDE ? P.kc0 : 0) + lane) * P.L2.rows + P.L2.lead + (size_t)(y0 - 1) * Pp - 1) * 8,
+                   nbytes, a_full);
         }
       }
     }
@@ -349,7 +359,14 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
           }
           const int row = t * 128 + 32 * q + lane;
           const int ml = row / Pp, n = row - ml * Pp;
-          if (ml < nrow && n < Wi) {
+          if (WIDE && ml < nrow && n < Wi) {
+            // same sum order per element as the narrow form within a group; the groups are added in launch order
+            const size_t hw = (size_t)Hi * Wi;
+            float* dst = P.dmid + ((size_t)b * P.c1 + P.o0) * hw + (size_t)(y0 + ml) * Wi + n;
+#pragma unroll
+            for (int o = 0; o < HEAD_CLS; ++o)
+              if (o < P.cg) dst[o * hw] = P.accumulate ? dst[o * hw] + d[o] : d[o];
+          } else if (ml < nrow && n < Wi) {
             const int y = y0 + ml;
             const int row1 = P.L1.lead + (y >> 1) * P.L1.Pp + (n >> 1);
             const int k0 = HEAD_CLS * (((y & 1) << 1) | (n & 1));
@@ -374,11 +391,13 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
         if (lane == 0) mbar_arrive(a_empty);
       }
     }
-    float* part = P.db1_part + ((size_t)blockIdx.x * 4 + q) * HEAD_CLS;
+    if (!WIDE) {
+      float* part = P.db1_part + ((size_t)blockIdx.x * 4 + q) * HEAD_CLS;
 #pragma unroll
-    for (int o = 0; o < HEAD_CLS; ++o) {
-      const float s = warp_sum(dbs[o]);
-      if (lane == 0) part[o] = s;
+      for (int o = 0; o < HEAD_CLS; ++o) {
+        const float s = warp_sum(dbs[o]);
+        if (lane == 0) part[o] = s;
+      }
     }
   }
 }
@@ -397,6 +416,11 @@ struct B3aParams {
   int Hh;                    // image rows per band (multiple of 4)
   int ncols;                 // accumulator columns per band = Hh * (Wi + 1) rounded up to 16 (<= 304)
   int tma_store;             // 1: the epilogue stages bf16 rows in shared memory and a TMA tensor store writes them (below)
+  // ACC (keypoint groups): one launch per c1 group, in order.  K is group kc0 / 10 of the frame's kc_frame K-chunks of G1;
+  // the group's d features are added to the fp32 partial sums acc32 [B][4 C4][HW] of the groups before it (acc_in) and
+  // stored there (acc_out) or, for the last group, rounded to bf16 into dfeat.
+  float* acc32;
+  int acc_in, acc_out, kc_frame, kc0;
 };
 
 // TMA tensor store of d features.  The tensor map views the NCHW gradient as [b][c'][pl][px] (source plane 4c' + pl,
@@ -413,7 +437,7 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volat
 
 // A frame is processed in bands of Hh image rows (N = Hh * (Wi + 1) accumulator columns per band; the band's gradient
 // rows plus the halo row above are double-buffered in shared memory).
-template <int WS2>
+template <int WS2, bool ACC = false>
 __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_constant__ B3aParams P, const __grid_constant__ CUtensorMap TM) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1, LEAD = Pp + 1;
@@ -462,7 +486,8 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
           if (lane == 0) mbar_expect_tx(&g_full[st], HEAD_KC * nbytes);
           __syncwarp((1u << HEAD_KC) - 1);
           bulk_g2s(Gs + (size_t)st * g_bytes + (size_t)lane * rows_alloc * 16,
-                   P.G1 + (((size_t)b * HEAD_KC + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8, nbytes, &g_full[st]);
+                   P.G1 + (((size_t)b * (ACC ? P.kc_frame : HEAD_KC) + (ACC ? P.kc0 : 0) + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8,
+                   nbytes, &g_full[st]);
         }
       }
   } else if (warp >= 2) {
@@ -517,7 +542,35 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
           const int i0 = y0 / 2 + 2 * ip;  // first feature row of the pair
 #pragma unroll
           for (int dj = 0; dj < 2; ++dj) {
-            __nv_bfloat16* dst = P.dfeat + ((size_t)b * 4 * P.C4 + 4 * c + 2 * di + dj) * HW + (size_t)i0 * WS2;
+            const size_t off = ((size_t)b * 4 * P.C4 + 4 * c + 2 * di + dj) * HW + (size_t)i0 * WS2;
+            __nv_bfloat16* dst = P.dfeat + off;
+            if constexpr (ACC) {
+              float* a32 = P.acc32 + off;
+#pragma unroll
+              for (int s4 = 0; s4 < (2 * WS2) / 8; ++s4) {
+                float f[8];
+#pragma unroll
+                for (int x = 0; x < 8; ++x) f[x] = v[(8 * s4 + x) / WS2][2 * ((8 * s4 + x) % WS2) + dj];
+                if (P.acc_in) {
+                  const float4 p0 = *reinterpret_cast<const float4*>(a32 + 8 * s4), p1 = *reinterpret_cast<const float4*>(a32 + 8 * s4 + 4);
+                  f[0] = p0.x + f[0], f[1] = p0.y + f[1], f[2] = p0.z + f[2], f[3] = p0.w + f[3];
+                  f[4] = p1.x + f[4], f[5] = p1.y + f[5], f[6] = p1.z + f[6], f[7] = p1.w + f[7];
+                }
+                if (P.acc_out) {
+                  *reinterpret_cast<float4*>(a32 + 8 * s4) = make_float4(f[0], f[1], f[2], f[3]);
+                  *reinterpret_cast<float4*>(a32 + 8 * s4 + 4) = make_float4(f[4], f[5], f[6], f[7]);
+                } else {
+                  uint32_t pk[4];
+#pragma unroll
+                  for (int e2 = 0; e2 < 4; ++e2) {
+                    __nv_bfloat162 h2 = __floats2bfloat162_rn(f[2 * e2], f[2 * e2 + 1]);
+                    pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
+                  }
+                  *reinterpret_cast<uint4*>(dst + 8 * s4) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                }
+              }
+              continue;
+            }
 #pragma unroll
             for (int s4 = 0; s4 < (2 * WS2) / 8; ++s4) {  // 8 consecutive elements of [row r][j]
               uint32_t pk[4];
@@ -657,6 +710,7 @@ struct WgParams {
   int XR;                     // X rows per K-chunk in smem (KR + Wi + 2, multiple of 8)
   int kcx, kcx_total;         // K-chunks (8 channels) per CTA group / per frame
   int Cin, Cout, ones_c;
+  int ngo;                    // keypoint groups of Cout: G holds ngo * 10 K-chunks per frame, and a CTA takes one group
   int smem_bytes;
 };
 
@@ -755,7 +809,9 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int N = P.kcx * 8;
   const int ngroups = P.kcx_total / P.kcx;  // kcx_total may include K-chunks beyond the last group (ignored)
-  const int grp = blockIdx.x % ngroups, slot = blockIdx.x / ngroups, nslot = gridDim.x / ngroups;
+  // CTA tile = (channel group grp, output keypoint group go), slot = its share of the (frame, row-chunk) units
+  const int ntile = ngroups * P.ngo, tile = blockIdx.x % ntile, grp = tile % ngroups, go = tile / ngroups;
+  const int slot = blockIdx.x / ntile, nslot = gridDim.x / ntile;
   const int nchunk = Hi / R, nunits = P.B * nchunk;  // R divides Hi (host)
 
   for (int i = tid; i < (P.smem_bytes - 64) / 16; i += WG_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
@@ -780,7 +836,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
       __syncwarp();
       const size_t row0 = (size_t)P.L.lead + (size_t)y0 * Pp;
       if (lane < HEAD_KC)
-        bulk_g2s(Gs + (size_t)s * g_bytes + (size_t)lane * KR * 16, P.G + (((size_t)b * HEAD_KC + lane) * P.L.rows + row0) * 8, gbytes, &full[s]);
+        bulk_g2s(Gs + (size_t)s * g_bytes + (size_t)lane * KR * 16, P.G + (((size_t)(b * P.ngo + go) * HEAD_KC + lane) * P.L.rows + row0) * 8, gbytes,
+                 &full[s]);
       if (lane < P.kcx)
         bulk_g2s(Xs + (size_t)s * x_bytes + (size_t)lane * XR * 16,
                  P.X + (((size_t)b * P.kcx_total + (size_t)grp * P.kcx + lane) * P.L.rows + row0) * 8, xbytes, &full[s]);
@@ -838,7 +895,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int k = 16 * mt + gq + 8 * (i >> 1);
-          const int cls = k / HEAD_CLS, o = k - cls * HEAD_CLS, py = cls >> 1, px = cls & 1;
+          const int cls = k / HEAD_CLS, o = go * HEAD_CLS + k - cls * HEAD_CLS, py = cls >> 1, px = cls & 1;
           if (o >= P.Cout || !tap_nonzero(cls, sh)) continue;
           const int ky = py == 0 ? 1 : (dm ? 0 : 2), kx = px == 0 ? 1 : (dn ? 0 : 2);
 #pragma unroll
@@ -864,6 +921,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
 
 static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* dW, float* dbias, float* part, int B, int Hi, int Wi,
                         int kcx_total, int Cin, int Cout, int ones_c, int sms, cudaStream_t s) {
+  const int ngo = head_groups(Cout);
   const int kcx = wgrad_kcx(kcx_total);
   // image rows per unit: the largest divisor of Hi (<= 8) whose two stages fit in shared memory
   int R = 0;
@@ -893,10 +951,11 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   p.Cin = Cin;
   p.Cout = Cout;
   p.ones_c = ones_c;
+  p.ngo = ngo;
   const size_t body = ((size_t)2 * HEAD_KC * p.KR * 16 + (size_t)2 * kcx * p.XR * 16 + 15) & ~(size_t)15;
   p.smem_bytes = (int)(body + 64);
   LPB_REQUIRE(p.smem_bytes <= 225 * 1024, "head_bwd_bf16: weight-gradient stages need %d B shared memory", p.smem_bytes);
-  const int ngroups = kcx_total / kcx;
+  const int ngroups = kcx_total / kcx * ngo;  // CTA tiles
   const int nunits = B * (Hi / R);
   int slots = sms / ngroups;
   if (slots > wgrad_max_slots(kcx_total)) slots = wgrad_max_slots(kcx_total);  // the partials' workspace
@@ -916,9 +975,8 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
 // the eight column sums of every (frame, K-chunk); stage 2 adds them per output channel in a fixed order, so the bias
 // gradient is bit-reproducible like every other gradient of this file (no atomics).
 __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* __restrict__ G, RowLayout L, float* __restrict__ part) {
-  // one CTA per (frame, K-chunk): thread = (row stripe, e)
-  const int b = blockIdx.x / HEAD_KC, kc = blockIdx.x - b * HEAD_KC;
-  const __nv_bfloat16* slab = G + ((size_t)b * HEAD_KC + kc) * (size_t)L.rows * 8;
+  // one CTA per (frame, K-chunk): thread = (row stripe, e); the frame's chunks are consecutive, so block = b * nkc + kc
+  const __nv_bfloat16* slab = G + (size_t)blockIdx.x * (size_t)L.rows * 8;
   const int e = threadIdx.x & 7;
   float acc = 0.f;
   for (int r = L.lead + (threadIdx.x >> 3); r < L.lead + L.Hi * L.Pp; r += 32) acc += __bfloat162float(slab[(size_t)r * 8 + e]);
@@ -932,12 +990,15 @@ __global__ void __launch_bounds__(256) rows_colsum_kernel(const __nv_bfloat16* _
   }
 }
 
-// one CTA per output channel o: the partials of K entries k = kc * 8 + e with k % HEAD_CLS == o, in a fixed order
-__global__ void __launch_bounds__(256) rows_colsum_reduce_kernel(const float* __restrict__ part, long long n, float* __restrict__ db) {
+// one CTA per output channel o = 20 g + o': the partials of K entries k = kc * 8 + e of group g (k / 80 == g of the
+// frame's nkc * 8) with k % HEAD_CLS == o', in a fixed order
+__global__ void __launch_bounds__(256) rows_colsum_reduce_kernel(const float* __restrict__ part, long long n, int nkc, float* __restrict__ db) {
   const int o = blockIdx.x;
   float acc = 0.f;
-  for (long long j = threadIdx.x; j < n; j += 256)
-    if ((int)(j % (HEAD_KC * 8)) % HEAD_CLS == o) acc += part[j];
+  for (long long j = threadIdx.x; j < n; j += 256) {
+    const int k = (int)(j % (nkc * 8));
+    if ((k / HEAD_NCOLS) * HEAD_CLS + (k % HEAD_NCOLS) % HEAD_CLS == o) acc += part[j];
+  }
   __shared__ float red[256];
   red[threadIdx.x] = acc;
   __syncthreads();
@@ -972,9 +1033,9 @@ static bool make_dfeat_tensor_map(CUtensorMap* tm, void* dfeat, int B, int C4, i
 // forward's channel limits.  LPB_OK, or LPB_ERR_UNSUPPORTED with the message set.
 static int head_bwd_covers(const char* who, int H, int W, int c1, int c2) {
   const bool width = W == 4 || W == 8 || W == 12 || W == 16 || W == 24 || W == 32;
-  if (H % 2 == 0 && width && (c2 > 0 ? c1 < HEAD_CLS && c2 <= HEAD_CLS : c1 <= HEAD_CLS)) return LPB_OK;
-  set_error("%s: head %dx%d with %d/%d channels outside this build's set (H even, W in {4, 8, 12, 16, 24, 32}, at most %d "
-            "channels per layer, fewer in the first of two)", who, H, W, c1, c2, HEAD_CLS);
+  if (H % 2 == 0 && width && (head_narrow(c1, c2) || head_wide(c1, c2))) return LPB_OK;
+  set_error("%s: head %dx%d with %d/%d channels outside this build's set (H even, W in {4, 8, 12, 16, 24, 32}, the "
+            "forward's channel counts)", who, H, W, c1, c2);
   return LPB_ERR_UNSUPPORTED;
 }
 
@@ -983,27 +1044,38 @@ static int head_bwd_covers(const char* who, int H, int W, int c1, int c2) {
 // (row_layout.cuh).  A one-deconv head (c2 = 0) has no G2 (its output gradient is G1 directly) but keeps the W2 pack's
 // space, and its partials are [layer-1 wgrad][bias column sums: eight per (frame, K-chunk)].  Members a head does not
 // have are 0.
+// Keypoint groups (wide heads, head_prep.cuh): the packs hold one block per (K group, tile), G2 / G1 hold 10 K-chunks per
+// group of c2 / c1, and two fp32 buffers follow the narrow layout: dmid [B][c1][4H * 4W] (the mid activations' gradient,
+// summed over the c2 groups, two-deconv heads) and acc32 [B][C][H * W] (the d features of the c1 groups before the last,
+// when c1 has more than one group).  Narrow heads have one group everywhere and neither buffer.
 struct HeadBwdLayout {
-  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, total;
+  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, dmid, acc32, total;
 };
 static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2) {
   const int C4 = C / 4;
-  const bool two = c2 > 0;
+  const bool two = c2 > 0, wide = head_wide(c1, c2);
+  const int g1 = head_groups(c1), g2 = two ? head_groups(c2) : 1, nst2 = two ? head_mid_stages(c1) : 1;
   HeadBwdLayout l{};
   l.wp1 = 0;
-  l.wp2 = l.wp1 + (size_t)((C4 + 127) / 128) * 4 * HEAD_KC * 128 * 16;
-  l.G2 = l.wp2 + (size_t)4 * HEAD_KC * 32 * 16;
-  l.G1 = l.G2 + (two ? (size_t)B * HEAD_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
-  l.ddot = l.G1 + (size_t)B * HEAD_KC * make_row_layout(2 * H, 2 * W).rows * 16;
+  l.wp2 = l.wp1 + (size_t)g1 * ((C4 + 127) / 128) * 4 * HEAD_KC * 128 * 16;
+  l.G2 = l.wp2 + (size_t)(two ? g1 * g2 : 1) * 4 * HEAD_KC * 32 * 16;
+  l.G1 = l.G2 + (two ? (size_t)B * g2 * HEAD_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
+  l.ddot = l.G1 + (size_t)B * g1 * HEAD_KC * make_row_layout(2 * H, 2 * W).rows * 16;
   l.part1 = l.ddot + (((size_t)B * (two ? c2 : c1) * 4 + 255) & ~(size_t)255);
   const size_t part1_end = l.part1 + (size_t)wgrad_max_slots(C4 / 8) * wgrad_part_stride(C4, c1) * sizeof(float);
   if (two) {
     l.part2 = part1_end;
-    l.part_db1 = l.part2 + (size_t)wgrad_max_slots(4) * wgrad_part_stride(c1, c2) * sizeof(float);
+    l.part_db1 = l.part2 + (size_t)wgrad_max_slots(4 * nst2) * wgrad_part_stride(c1, c2) * sizeof(float);
     l.total = l.part_db1 + (size_t)B2D_MAX_CTAS * 4 * HEAD_CLS * sizeof(float);
   } else {
     l.part_cs = part1_end;
     l.total = l.part_cs + (size_t)B * HEAD_KC * 8 * sizeof(float);
+  }
+  if (wide) {
+    l.part_cs = l.total;  // the bias column sums of G1 (db1 of every wide head)
+    l.dmid = l.part_cs + (((size_t)B * g1 * HEAD_KC * 8 * sizeof(float) + 255) & ~(size_t)255);
+    l.acc32 = l.dmid + (two ? (size_t)B * c1 * 16 * H * W * sizeof(float) : 0);
+    l.total = l.acc32 + (g1 > 1 ? (size_t)B * C * H * W * sizeof(float) : 0);
   }
   return l;
 }
@@ -1070,21 +1142,27 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   float* part1 = reinterpret_cast<float*>(ws + wl.part1);
   float* part2 = two ? reinterpret_cast<float*>(ws + wl.part2) : nullptr;
   float* part_db1 = two ? reinterpret_cast<float*>(ws + wl.part_db1) : nullptr;
-  float* part_cs = two ? nullptr : reinterpret_cast<float*>(ws + wl.part_cs);
+  const bool wide = head_wide(c1, c2);
+  const int g1 = head_groups(c1), g2 = two ? head_groups(c2) : 1, nst2 = two ? head_mid_stages(c1) : 1;
+  float* part_cs = two && !wide ? nullptr : reinterpret_cast<float*>(ws + wl.part_cs);
+  float* dmid = wide && two ? reinterpret_cast<float*>(ws + wl.dmid) : nullptr;
+  float* acc32 = wide && g1 > 1 ? reinterpret_cast<float*>(ws + wl.acc32) : nullptr;
   // the forward pass's mid activations
   const __nv_bfloat16* mid =
-      reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + head_fwd_layout(B, C, H, W, c2).mid);
+      reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + head_fwd_layout(B, C, H, W, c1, c2).mid);
 
   {
     // one launch: gradient accumulators zeroed, both data-gradient operand packs, pad rows of G2 / G1
     PrepJobs jobs{};
-    jobs.dpack[0] = {w1, C4, c1, ntile1, 128, wp1};
-    jobs.pads[0] = {G1, L1, (long long)B * HEAD_KC};
+    jobs.dpack[0] = {w1, C4, c1, ntile1, 128, 128, g1, wp1};
+    jobs.pads[0] = {G1, L1, (long long)B * g1 * HEAD_KC};
     jobs.zero[0] = {dw1, (long long)C4 * c1 * 9};
     jobs.zero[1] = {db1, (long long)c1};
     if (two) {
-      jobs.dpack[1] = {w2, c1, c2, 1, 32, wp2};
-      jobs.pads[1] = {G2, L2, (long long)B * HEAD_KC};
+      // wide: tile t = the mid channels of c1 group t (20 of the 32 rows), K = one c2 group
+      if (wide) jobs.dpack[1] = {w2, c1, c2, g1, 32, HEAD_CLS, g2, wp2};
+      else jobs.dpack[1] = {w2, c1, c2, 1, 32, 32, 1, wp2};
+      jobs.pads[1] = {G2, L2, (long long)B * g2 * HEAD_KC};
       jobs.zero[2] = {dw2, (long long)c1 * c2 * 9};
       jobs.zero[3] = {db2, (long long)c2};
     }
@@ -1117,9 +1195,9 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
   }
   if (two) {
     // layer 2: weight + bias gradient (bias from the all-ones channel c1 of mid), then data gradient -> G1 (+ db1)
-    const int rc = launch_wgrad(mid, G2, dw2, db2, part2, B, Hi2, Wi2, 4, c1, c2, c1, sms, s);
+    const int rc = launch_wgrad(mid, G2, dw2, db2, part2, B, Hi2, Wi2, 4 * nst2, c1, c2, c1, sms, s);
     if (rc != LPB_OK) return rc;
-    B2dParams p;
+    B2dParams p{};
     p.G2 = G2;
     p.wpk = wp2;
     p.G1 = G1;
@@ -1135,14 +1213,35 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     const int rows_alloc = (Wi2 + 2 + B2D_TILES * 128 + 7) & ~7;
     const size_t smem = (size_t)HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 32 * 16 + 64;
     LPB_REQUIRE(smem <= 113 * 1024 && p.R2 >= 1, "head_bwd_bf16: layer-2 width %d too large", Wi2);
-    LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int grid = B < 2 * sms ? B : 2 * sms;
     if (grid > B2D_MAX_CTAS) grid = B2D_MAX_CTAS;  // the bias partials' workspace
-    b2d_dgrad_kernel<<<grid, B2D_THREADS, smem, s>>>(p);
-    reduce_partials<1>(part_db1, grid * 4, HEAD_CLS, c1, db1, sms, s);
-  } else {
-    rows_colsum_kernel<<<(unsigned)(B * HEAD_KC), 256, 0, s>>>(G1, L1, part_cs);
-    rows_colsum_reduce_kernel<<<(unsigned)c1, 256, 0, s>>>(part_cs, (long long)B * HEAD_KC * 8, db1);
+    if (!wide) {
+      LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      b2d_dgrad_kernel<false><<<grid, B2D_THREADS, smem, s>>>(p);
+      reduce_partials<1>(part_db1, grid * 4, HEAD_CLS, c1, db1, sms, s);
+    } else {
+      // keypoint groups: the mid activations' gradient in fp32 planes, the c2 groups added in order per c1 group, then
+      // written as G1 by the front end's writer (a dense gradient, no softmax) and the bias gradient from G1's columns
+      LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      p.dmid = dmid;
+      p.kc_frame = g2 * HEAD_KC;
+      for (int t = 0; t < g1; ++t)
+        for (int k = 0; k < g2; ++k) {
+          p.wpk = wp2 + (size_t)(k * g1 + t) * 4 * HEAD_KC * 32 * 8;
+          p.kc0 = k * HEAD_KC;
+          p.o0 = t * HEAD_CLS;
+          p.cg = c1 - p.o0 < HEAD_CLS ? c1 - p.o0 : HEAD_CLS;
+          p.accumulate = k > 0;
+          b2d_dgrad_kernel<true><<<grid, B2D_THREADS, smem, s>>>(p);
+        }
+      G2Src src{};
+      src.g_out = dmid;
+      launch_g2_build<true, false>(src, B, c1, Hi1, Wi1, G1, L1, s);
+    }
+  }
+  if (!two || wide) {
+    rows_colsum_kernel<<<(unsigned)(B * g1 * HEAD_KC), 256, 0, s>>>(G1, L1, part_cs);
+    rows_colsum_reduce_kernel<<<(unsigned)c1, 256, 0, s>>>(part_cs, (long long)B * g1 * HEAD_KC * 8, g1 * HEAD_KC, db1);
   }
   // layer 1: weight gradient from the saved shuffled features, data gradient -> d features
   {
@@ -1162,6 +1261,9 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.Wi = Wi1;
     p.Hh = Hh;
     p.ncols = (Hh * (Wi1 + 1) + 15) & ~15;
+    p.acc32 = acc32;
+    p.kc_frame = g1 * HEAD_KC;
+    p.acc_in = p.acc_out = p.kc0 = 0;
     const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
     size_t smem = (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
     LPB_REQUIRE(smem <= 225 * 1024, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
@@ -1170,7 +1272,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     p.tma_store = 0;
-    {
+    if (!acc32) {  // (the groups' fp32 sums take the direct stores)
       const size_t stage = (size_t)2 * 4 * 128 * 4 * W + 128;
       if (smem + stage <= 225 * 1024 && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
         p.tma_store = 1;
@@ -1180,19 +1282,31 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     int slots = sms / ntile1;
     if (slots < 1) slots = 1;
     if (slots > B) slots = B;
-    auto run = [&](auto kern) -> int {
-      LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      kern<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap);
+    auto run = [&](auto kern, auto kern_acc) -> int {
+      if (!acc32) {
+        LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap);
+        return LPB_OK;
+      }
+      // keypoint groups of c1: one launch per group, in order, each adding its d features to the groups' fp32 sums
+      LPB_CUDA(cudaFuncSetAttribute(kern_acc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      for (int g = 0; g < g1; ++g) {
+        p.wpk = wp1 + (size_t)g * ntile1 * 4 * HEAD_KC * 128 * 8;
+        p.kc0 = g * HEAD_KC;
+        p.acc_in = g > 0;
+        p.acc_out = g < g1 - 1;
+        kern_acc<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap);
+      }
       return LPB_OK;
     };
     int rc = LPB_ERR_UNSUPPORTED;
     switch (W) {
-      case 4: rc = run(b3a_dgrad_kernel<4>); break;
-      case 8: rc = run(b3a_dgrad_kernel<8>); break;
-      case 12: rc = run(b3a_dgrad_kernel<12>); break;
-      case 16: rc = run(b3a_dgrad_kernel<16>); break;
-      case 24: rc = run(b3a_dgrad_kernel<24>); break;
-      case 32: rc = run(b3a_dgrad_kernel<32>); break;
+      case 4: rc = run(b3a_dgrad_kernel<4>, b3a_dgrad_kernel<4, true>); break;
+      case 8: rc = run(b3a_dgrad_kernel<8>, b3a_dgrad_kernel<8, true>); break;
+      case 12: rc = run(b3a_dgrad_kernel<12>, b3a_dgrad_kernel<12, true>); break;
+      case 16: rc = run(b3a_dgrad_kernel<16>, b3a_dgrad_kernel<16, true>); break;
+      case 24: rc = run(b3a_dgrad_kernel<24>, b3a_dgrad_kernel<24, true>); break;
+      case 32: rc = run(b3a_dgrad_kernel<32>, b3a_dgrad_kernel<32, true>); break;
       default: set_error("head_bwd_bf16: feature width %d not in this build's epilogue set", W);
     }
     if (rc != LPB_OK) return rc;

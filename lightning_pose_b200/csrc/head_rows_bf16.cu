@@ -79,7 +79,11 @@ constexpr int CR_STAGES = 2;
 // NPL: compile-time plane count (17 = the usual keypoint count) or 0 for a run-time count <= 20.
 // The softmax modes' epilogue takes one warp vote per tile (instead of one per plane), keeps the running-max rescale out
 // of the common path, fetches (shift, 1/sum) as one 8-byte shared load and advances the output pointer by addition.
-template <int MODE, int NPL>
+// WIDE: the output channels are P.ngroups keypoint groups (head_prep.cuh) and a work item is (frame [, band], group): it
+// stages its rows, runs the group's 80-column GEMM and finishes the group's planes (or its mid channels [20g, 20g + 20),
+// written as 8-byte halves of the K-chunks, since two groups can share a chunk).  The per-warp accumulators are those of
+// a single group; a band is staged once per group and re-read from L2.
+template <int MODE, int NPL, bool WIDE = false>
 __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_constant__ ConvtRowsParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Pp = P.L.Pp, Wi = P.L.Wi, Hi = P.L.Hi;
@@ -110,29 +114,32 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
   // scratch; P1: normalise with the frame's merged statistics) -- is independent per (frame, band), so small batches
   // (inference chunks, ViT training batches) still fill the GPU and large ones balance to within one band.
   constexpr bool PER_BAND = MODE != CONVT_ROWS_SOFTMAX;
-  const int nitems = PER_BAND ? P.B * nbands : P.B;
+  const int ng = WIDE ? P.ngroups : 1;
+  const int nitems = (PER_BAND ? P.B * nbands : P.B) * ng;  // wide: the groups of a (frame, band) are consecutive items
   const int bands_per_item = PER_BAND ? 1 : nbands;
-  const int ncls = NPL ? NPL : P.cout;  // planes handled by the unrolled loops
   constexpr bool SOFTMAX = MODE == CONVT_ROWS_SOFTMAX || MODE == CONVT_ROWS_SOFTMAX_P0 || MODE == CONVT_ROWS_SOFTMAX_P1;
 
   if (warp == 0) {
     // ================= loader: one bulk copy per K-chunk (band rows + the halo row below) + the stage's weights ====
-    // single-stage GEMMs (K = 32) keep their weights resident: each ring slot receives them once
+    // single-stage GEMMs (K = 32) of one group keep their weights resident: each ring slot receives them once
     int it = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x)
       for (int pass = 0; pass < npass; ++pass)
         for (int bi = 0; bi < bands_per_item; ++bi) {
-          const int b = PER_BAND ? item / nbands : item, band = PER_BAND ? item - b * nbands : bi;
+          const int g = WIDE ? item % ng : 0, fi = WIDE ? item / ng : item;
+          const int b = PER_BAND ? fi / nbands : fi, band = PER_BAND ? fi - b * nbands : bi;
           const int y0 = band * R, rb = min(R, Hi - y0);
           const uint32_t nbytes = (uint32_t)((rb + 1) * Pp * 16);
           for (int st = 0; st < nst; ++st, ++it) {
             const int s = it % CR_STAGES;
             mbar_wait_idle(&empty[s], ((it / CR_STAGES) & 1) ^ 1);
             unsigned char* As = smem + s * stage_bytes;
-            const bool load_b = nst > 1 || it < CR_STAGES;
+            const bool load_b = nst > 1 || it < CR_STAGES || ng > 1;
             if (lane == 0) {
               mbar_expect_tx(&full[s], 4 * nbytes + (load_b ? HEAD_BSTAGE_BYTES : 0));
-              if (load_b) bulk_g2s(As + a_bytes, reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)st * HEAD_BSTAGE_BYTES, HEAD_BSTAGE_BYTES, &full[s]);
+              if (load_b)
+                bulk_g2s(As + a_bytes, reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)(g * nst + st) * HEAD_BSTAGE_BYTES, HEAD_BSTAGE_BYTES,
+                         &full[s]);
             }
             __syncwarp();
             if (lane < 4)
@@ -151,7 +158,11 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
     const uint32_t lbo_a = P.rows_alloc * 16, lbo_b = HEAD_NCOLS * 16;
     int it = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int b = PER_BAND ? item / nbands : item;
+      const int g = WIDE ? item % ng : 0, fi = WIDE ? item / ng : item;
+      const int b = PER_BAND ? fi / nbands : fi;
+      const int o0 = HEAD_CLS * g;                                       // the group's first output channel
+      const int ncls = NPL ? NPL : (WIDE ? min(HEAD_CLS, P.cout - o0) : P.cout);  // planes handled by the unrolled loops
+      const float* bias = use_bias ? P.bias + o0 : nullptr;
       float mx[HEAD_CLS], sm[HEAD_CLS];
 #pragma unroll
       for (int o = 0; o < HEAD_CLS; ++o) {
@@ -163,7 +174,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
         asm volatile("bar.sync 1, 256;" ::: "memory");  // previous item's readers of fin are done
         if (tid - 64 < ncls) {
           const int o = tid - 64;
-          const float* pp = P.partials + ((size_t)b * nbands * HEAD_CLS + o) * 2;
+          const float* pp = P.partials + (((size_t)b * ng + g) * nbands * HEAD_CLS + o) * 2;
           float M = -1.0e30f;
           for (int j = 0; j < nbands; ++j) M = fmaxf(M, pp[(size_t)j * HEAD_CLS * 2]);
           float S = 0.f;
@@ -176,7 +187,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
       for (int pass = 0; pass < npass; ++pass) {
         const bool write = MODE == CONVT_ROWS_SOFTMAX_P0 ? false : (pass == npass - 1);
         for (int bi = 0; bi < bands_per_item; ++bi) {
-          const int band = PER_BAND ? item - b * nbands : bi;
+          const int band = PER_BAND ? fi - b * nbands : bi;
           const int y0 = band * R, rb = min(R, Hi - y0), tiles = (rb * Pp + 127) / 128;
           float acc[CR_TILES][2][6][4];
 #pragma unroll
@@ -237,7 +248,45 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             const int y = 2 * (y0 + ml) + e, x = 2 * n;
             auto body = [&](auto ec) {
               constexpr int E = decltype(ec)::value;
-              if constexpr (MODE == CONVT_ROWS_MID) {
+              if constexpr (MODE == CONVT_ROWS_MID && WIDE) {
+                // bf16 rows of the next layer, by 4-channel units (8-byte halves of a K-chunk): the group's five units
+                // 5g .. 5g + 4, and the last group also the units past the groups up to the end of the last K-chunk.
+                // Channel `cout` is the constant one, every other channel >= cout is 0.
+                if (valid) {
+                  const int u1 = g == ng - 1 ? 2 * P.mid_kc : 5 * g + 5;
+#pragma unroll
+                  for (int px = 0; px < 2; ++px) {
+                    const size_t row2 = (size_t)P.Lout.lead + (size_t)y * P.Lout.Pp + x + px;
+                    __nv_bfloat16* base = P.mid + ((size_t)b * P.mid_kc * P.Lout.rows + row2) * 8;
+#pragma unroll
+                    for (int i = 0; i < HEAD_CLS / 4; ++i) {
+                      const int u = 5 * g + i;
+                      uint32_t pk[2];
+#pragma unroll
+                      for (int e2 = 0; e2 < 2; ++e2) {
+                        float f[2];
+#pragma unroll
+                        for (int hh = 0; hh < 2; ++hh) {
+                          const int cl = 4 * i + 2 * e2 + hh;  // compile-time channel within the group
+                          const int ch = o0 + cl;
+                          f[hh] = ch < P.cout ? d[8 * E + px * HEAD_CLS + cl] + (use_bias ? __ldg(bias + cl) : 0.f) : (ch == P.cout ? 1.0f : 0.f);
+                        }
+                        __nv_bfloat162 h2 = __floats2bfloat162_rn(f[0], f[1]);
+                        pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
+                      }
+                      *reinterpret_cast<uint2*>(base + (size_t)(u >> 1) * P.Lout.rows * 8 + (u & 1) * 4) = make_uint2(pk[0], pk[1]);
+                    }
+                    for (int u = 5 * g + 5; u < u1; ++u) {
+                      const int c0 = 4 * u;
+                      const uint32_t one = 0x3f80u;  // bf16 1.0
+                      const uint32_t lo = (c0 == P.cout ? one : 0u) | (c0 + 1 == P.cout ? one << 16 : 0u);
+                      const uint32_t hi = (c0 + 2 == P.cout ? one : 0u) | (c0 + 3 == P.cout ? one << 16 : 0u);
+                      *reinterpret_cast<uint2*>(base + (size_t)(u >> 1) * P.Lout.rows * 8 + (u & 1) * 4) = make_uint2(lo, hi);
+                    }
+                  }
+                }
+                return;
+              } else if constexpr (MODE == CONVT_ROWS_MID) {
                 // bf16 rows of the next layer: channel `cout` is the constant one (carries that layer's bias)
                 if (valid) {
 #pragma unroll
@@ -270,7 +319,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                 }
                 return;
               }
-              float* dst = P.out + ((size_t)b * P.cout * Ho + y) * Wo + x;  // plane o adds o * Ho * Wo
+              float* dst = P.out + (((size_t)b * P.cout + o0) * Ho + y) * Wo + x;  // plane o0 + o adds o * Ho * Wo
               if constexpr (SOFTMAX) {
                 if (!write) {
                   // ---- pass 0: per-thread online (max, sum) per plane; the rescale is rare after the first tiles ----
@@ -318,7 +367,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 #pragma unroll
                 for (int o = 0; o < HEAD_CLS; ++o) {
                   if (o >= ncls) break;
-                  const float bo = use_bias ? __ldg(P.bias + o) : 0.f;
+                  const float bo = use_bias ? __ldg(bias + o) : 0.f;
                   const float l0 = d[8 * E + o] + bo, l1 = d[8 * E + HEAD_CLS + o] + bo;
                   if (valid) *reinterpret_cast<float2*>(dst + (size_t)o * plane_stride) = make_float2(l0, l1);
                 }
@@ -350,7 +399,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 #pragma unroll
             for (int i = 0; i < 8; ++i) S += stat[(HEAD_CLS + o) * 8 + i] * fast_exp2((stat[o * 8 + i] - M) * L2E);
             if constexpr (MODE == CONVT_ROWS_SOFTMAX_P0) {
-              float* pp = P.partials + (((size_t)b * nbands + (item - b * nbands)) * HEAD_CLS + o) * 2;
+              float* pp = P.partials + ((((size_t)b * ng + g) * nbands + (fi - b * nbands)) * HEAD_CLS + o) * 2;
               pp[0] = M;
               pp[1] = S;
             } else {
@@ -368,8 +417,8 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
   const int Pp = p.L.Pp;
   LPB_REQUIRE(Pp <= CR_TILES * 128, "head_fwd_bf16: image width %d too large for one band", p.L.Wi);
-  LPB_REQUIRE(p.cout >= 1 && p.cout <= HEAD_CLS && (p.mode != CONVT_ROWS_MID || p.cout < HEAD_CLS), "head_fwd_bf16: %d output channels exceed %d",
-              p.cout, HEAD_CLS);
+  LPB_REQUIRE(p.cout >= 1 && p.cout <= HEAD_MAX_CH, "head_fwd_bf16: %d output channels exceed %d", p.cout, HEAD_MAX_CH);
+  LPB_REQUIRE(p.mode != CONVT_ROWS_MID || p.mid_kc >= 4 * head_mid_stages(p.cout), "head_fwd_bf16: mid activations of %d K-chunks", p.mid_kc);
   p.R = (CR_TILES * 128) / Pp;
   if (p.R > p.L.Hi) p.R = p.L.Hi;
   const int tiles = (p.R * Pp + 127) / 128;
@@ -384,6 +433,22 @@ int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
     kern<<<grid, CR_THREADS, smem, s>>>(p);
     return LPB_OK;
   };
+  // wide layers (more than 20 output channels; 20 or more for the first of two, whose mid activations then take more
+  // than one K stage) run the keypoint-group instantiations
+  const bool wide = p.cout > HEAD_CLS || (p.mode == CONVT_ROWS_MID && p.cout >= HEAD_CLS);
+  p.ngroups = head_groups(p.cout);
+  if (wide) {
+    const long long per_group = (long long)p.B * nbands * p.ngroups;
+    if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<CONVT_ROWS_MID, 0, true>, per_group);
+    if (p.mode == CONVT_ROWS_PLANES) return run(convt_rows_kernel<CONVT_ROWS_PLANES, 0, true>, per_group);
+    // the split / fused choice of the narrow heads below, counting (frame, group) items
+    if (p.partials && (g_softmax_split == 2 || (g_softmax_split == 1 && (long long)p.B * p.ngroups < sms))) {
+      const int rc = run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 0, true>, per_group);
+      if (rc != LPB_OK) return rc;
+      return run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 0, true>, per_group);
+    }
+    return run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0, true>, (long long)p.B * p.ngroups);
+  }
   const bool k17 = p.cout == 17;
   const long long per_band = (long long)p.B * nbands;
   if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<CONVT_ROWS_MID, 0>, per_band);
