@@ -233,6 +233,20 @@ int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes, int ctx, 
 int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* mean3,
                          const float* std3, int layout, int out_bf16, void* out, void* stream);
 
+/* ---- multi-view video ingest: every camera's frames in one launch -----------------------------------------------
+ * replaces the multi-view tail of the DALI pipeline  lightning_pose/data/video/dali.py:301-330  (one reader per view,
+ * each through fn.resize -> / 255 -> fn.crop_mirror_normalize as in lpb_frames_normalize, then the views stacked into
+ * (seq, V, 3, H, W)).  frames_u8: HOST array of V device pointers, view v [F, H[v], W[v], 3] decoded RGB; H, W: HOST
+ * arrays of V ints (views may differ in size).  out [F, V, 3, out_h, out_w] (layout 0) or [F, V, out_h, out_w, 3]
+ * (layout 1), fp32 or bf16 (out_bf16): reshaped to [F * V, ...] it is the frame-major, view-minor batch the multi-view
+ * trackers read.  Every output image is bit-identical to lpb_frames_normalize on that view alone (a view already at
+ * out_h x out_w is copied and normalised without resampling).  1 <= V <= LPB_INGEST_MAX_VIEWS, F * V < 2^31; the
+ * output may pass 2^31 elements.  F = 0 is a no-op. */
+#define LPB_INGEST_MAX_VIEWS 16
+int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V, int F, const int* H, const int* W, int out_h,
+                               int out_w, const float* mean3, const float* std3, int layout, int out_bf16, void* out,
+                               void* stream);
+
 /* ---- augmented video ingest: the unlabeled branch's DALI augmentation ----------------------------------------
  * replaces  lightning_pose/data/video/dali.py:154-192  (training.imgaug "dlc" / "dlc-top-down") in front of the
  * normalisation of lpb_frames_normalize, one view, one draw per call.  Per frame of frames_u8 [F, H, W, 3]:

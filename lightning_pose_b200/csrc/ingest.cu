@@ -88,6 +88,42 @@ __global__ void __launch_bounds__(256) ingest_kernel(const __grid_constant__ Ing
   }
 }
 
+// ---- multi-view ingest: V views of F frames each in one launch ------------------------------------------------------
+// View v's frames are in[v] [F, H[v], W[v], 3]; the pointers travel by value in the kernel parameters, so a captured
+// graph reads the same buffers on every replay.  Output image fv = f * V + v (frame-major, view-minor) is frame f of
+// view v, computed with resized_pixel / store_pixel exactly as ingest_kernel computes it for that view alone; a view
+// already at the output size reads its source pixel directly.  F * V < 2^31 (checked by the host).  V = 1 keeps
+// ingest_kernel: this kernel's per-pixel view lookup costs 2-21 % on single-view ingest (DESIGN.md, K7).
+struct IngestViewsParams {
+  const uint8_t* in[LPB_INGEST_MAX_VIEWS];
+  void* out;
+  int F, V, OH, OW;
+  int H[LPB_INGEST_MAX_VIEWS], W[LPB_INGEST_MAX_VIEWS];
+  float ry[LPB_INGEST_MAX_VIEWS], rx[LPB_INGEST_MAX_VIEWS];  // H / OH, W / OW
+  float scale[3], shift[3];
+};
+
+template <int LAYOUT, bool BF16>
+__global__ void __launch_bounds__(256) ingest_views_kernel(const __grid_constant__ IngestViewsParams P) {
+  const int64_t total = (int64_t)P.F * P.V * P.OH * P.OW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % P.OW);
+    const int64_t r = i / P.OW;
+    const int y = (int)(r % P.OH), fv = (int)(r / P.OH);
+    const int view = fv % P.V, f = fv / P.V;
+    const int H = P.H[view], W = P.W[view];
+    const uint8_t* img = P.in[view] + (size_t)f * H * W * 3;
+    float v[3];
+    if (H != P.OH || W != P.OW)
+      resized_pixel<true>(img, H, W, P.ry[view], P.rx[view], y, x, v);
+    else
+      resized_pixel<false>(img, H, W, 0.f, 0.f, y, x, v);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = fmaf(v[c], P.scale[c], P.shift[c]);
+    store_pixel<LAYOUT, BF16>(P.out, P.OH, P.OW, fv, y, x, v);
+  }
+}
+
 // ---- augmented ingest: the DALI video augmentation of dali.py:156-178 ---------------------------------------------
 // Per output pixel (f, y, x) of one view, with M = [A | t] the rotate-scale matrix (source -> destination, (x, y)):
 //   warp     the resized image sampled bilinearly at  M^-1 (x + 0.5, y + 0.5) - 0.5, taps outside it read 0.
@@ -274,6 +310,45 @@ extern "C" int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int 
     case 5: ingest_kernel<1, false, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
     case 6: ingest_kernel<1, true, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
     default: ingest_kernel<1, true, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+  }
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V, int F, const int* H, const int* W, int out_h,
+                                          int out_w, const float* mean3, const float* std3, int layout, int out_bf16, void* out,
+                                          void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(frames_u8 && H && W && mean3 && std3 && out, "frames_normalize_views: null pointer");
+  LPB_REQUIRE(V >= 1 && V <= LPB_INGEST_MAX_VIEWS, "frames_normalize_views: view count %d outside 1..%d", V, LPB_INGEST_MAX_VIEWS);
+  LPB_REQUIRE(F >= 0 && out_h >= 1 && out_w >= 1 && (layout == 0 || layout == 1), "frames_normalize_views: bad shape/layout");
+  LPB_REQUIRE((int64_t)F * V <= INT32_MAX, "frames_normalize_views: F * V must be below 2^31");
+  IngestViewsParams p;
+  for (int v = 0; v < V; ++v) {  // frames_u8, H and W are HOST arrays
+    LPB_REQUIRE(frames_u8[v], "frames_normalize_views: null pointer");
+    LPB_REQUIRE(H[v] >= 1 && W[v] >= 1, "frames_normalize_views: bad shape/layout");
+    p.in[v] = frames_u8[v];
+    p.H[v] = H[v], p.W[v] = W[v];
+    p.ry[v] = (float)H[v] / (float)out_h;  // the ratios lpb_frames_normalize computes for this view
+    p.rx[v] = (float)W[v] / (float)out_w;
+  }
+  if (F == 0) return LPB_OK;
+  p.out = out;
+  p.F = F, p.V = V, p.OH = out_h, p.OW = out_w;
+  for (int c = 0; c < 3; ++c) {
+    LPB_REQUIRE(std3[c] > 0.f, "frames_normalize_views: std must be positive");
+    p.scale[c] = 1.0f / (255.0f * std3[c]);
+    p.shift[c] = -mean3[c] / std3[c];
+  }
+  const int64_t total = (int64_t)F * V * out_h * out_w;
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > 132 * 32) blocks = 132 * 32;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  switch (layout * 2 + (out_bf16 ? 1 : 0)) {
+    case 0: ingest_views_kernel<0, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 1: ingest_views_kernel<0, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 2: ingest_views_kernel<1, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    default: ingest_views_kernel<1, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
   }
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;

@@ -58,17 +58,19 @@ def frames_to_unlabeled_batch(frames_u8: torch.Tensor | Sequence[torch.Tensor], 
             raise ValueError("resize_dims is required when frames are cropped to bounding boxes")
         frames, boxes = ops.frames_crop_normalize(views[0], bbox, resize_dims, row0=bbox_row0, channels_last=channels_last, dtype=dtype)
         return {"frames": frames, "transforms": torch.tensor([-1.0], device=frames.device), "bbox": boxes, "is_multiview": False}
-    outs, boxes = [], []
-    for v in views:
-        outs.append(ops.frames_normalize(v, size=resize_dims, channels_last=channels_last, dtype=dtype))
-        boxes.append(torch.tensor([0.0, 0.0, float(v.shape[1]), float(v.shape[2])], device=v.device))
-    seq = outs[0].shape[0]
+    boxes = torch.tensor([[0.0, 0.0, float(v.shape[1]), float(v.shape[2])] for v in views], device=views[0].device).reshape(1, -1)
+    seq = views[0].shape[0]
     if len(views) == 1:
-        return {"frames": outs[0], "transforms": torch.tensor([-1.0], device=outs[0].device), "bbox": boxes[0].repeat(seq, 1), "is_multiview": False}
+        frames = ops.frames_normalize(views[0], size=resize_dims, channels_last=channels_last, dtype=dtype)
+        return {"frames": frames, "transforms": torch.tensor([-1.0], device=frames.device), "bbox": boxes.repeat(seq, 1), "is_multiview": False}
+    if resize_dims is None:  # each view at its own size: they can only be stacked when the sizes agree
+        if len({tuple(v.shape[1:3]) for v in views}) > 1:
+            raise ValueError("views of different sizes need resize_dims to be stacked")
+        resize_dims = tuple(views[0].shape[1:3])
     return {
-        "frames": torch.stack(outs, dim=1),
-        "transforms": torch.full((len(views), 1), -1.0, device=outs[0].device),
-        "bbox": torch.cat(boxes).repeat(seq, 1),
+        "frames": ops.frames_normalize_views(views, resize_dims, channels_last=channels_last, dtype=dtype),
+        "transforms": torch.full((len(views), 1), -1.0, device=views[0].device),
+        "bbox": boxes.repeat(seq, 1),
         "is_multiview": True,
     }
 

@@ -530,6 +530,41 @@ def frames_normalize(frames_u8, size=None, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     return out
 
 
+INGEST_MAX_VIEWS = 16  # LPB_INGEST_MAX_VIEWS (include/lpb200.h)
+
+
+def frames_normalize_views(views_u8, size, mean=IMAGENET_MEAN, std=IMAGENET_STD, channels_last=False, dtype=torch.float32):
+    """V synchronised views, uint8 (F, H_v, W_v, 3) each (sizes may differ), -> normalised (F, V, 3, h, w) [or
+    (F, V, h, w, 3)] fp32 / bf16 in one launch; view v of frame f is bit-identical to ``frames_normalize`` of that view.
+    ``reshape(F * V, ...)`` is the frame-major, view-minor batch of the multi-view trackers."""
+    views = list(views_u8)
+    if not 1 <= len(views) <= INGEST_MAX_VIEWS:
+        raise ValueError(f"frames_normalize_views takes 1..{INGEST_MAX_VIEWS} views; got {len(views)}")
+    for v in views:
+        if not isinstance(v, torch.Tensor) or not v.is_cuda:
+            raise RuntimeError("lpb200: `views` must be CUDA tensors (this package has no CPU fallback)")
+        if v.dtype != torch.uint8 or v.dim() != 4 or v.shape[-1] != 3:
+            raise ValueError(f"each view must be uint8 (F, H, W, 3); got {tuple(v.shape)} {v.dtype}")
+        if v.device != views[0].device:
+            raise ValueError("all views must be on one device")
+    f = views[0].shape[0]
+    if any(v.shape[0] != f for v in views):
+        raise ValueError(f"all views must have the same frame count; got {[v.shape[0] for v in views]}")
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError("dtype must be float32 or bfloat16")
+    xs = [v.contiguous() for v in views]
+    n = len(xs)
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((f, n, oh, ow, 3) if channels_last else (f, n, 3, oh, ow), device=xs[0].device, dtype=dtype)
+    ptrs = (C.c_void_p * n)(*[x.data_ptr() for x in xs])
+    hs, ws = (C.c_int * n)(*[x.shape[1] for x in xs]), (C.c_int * n)(*[x.shape[2] for x in xs])
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(xs[0].device):
+        check(lib.lpb_frames_normalize_views(ptrs, n, f, hs, ws, oh, ow, m3, s3, int(bool(channels_last)), int(dtype == torch.bfloat16),
+                                             _ptr(out), _stream()))
+    return out
+
+
 # training.imgaug "dlc" draw ranges (lightning_pose/data/video/dali.py:160-175) by column of the augment kernel's
 # params: angle (degrees), sx and sy, brightness and contrast, shot-noise factor
 DLC_PARAM_RANGES = ((slice(0, 1), -10.0, 10.0), (slice(1, 3), 0.8, 1.2), (slice(3, 5), 0.75, 1.25), (slice(5, 6), 0.0, 10.0))

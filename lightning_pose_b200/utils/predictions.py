@@ -43,14 +43,23 @@ class PredictionHandler:
     """Video-side mirror of the reference's ``PredictionHandler`` (:41-329): same column schema, same context fix-up.
 
     ``frame_count`` is given directly (the reference counts the video's frames with OpenCV; video I/O is out of scope).
+    ``view_names`` (the reference's ``cfg.data.view_names``) names the views of a multi-view video, in the order of the
+    prediction columns: view v owns keypoint columns ``[v K, (v + 1) K)`` (reference :296-315).
     """
 
-    def __init__(self, keypoint_names: Sequence[str], frame_count: int, model_type: str = "heatmap") -> None:
+    def __init__(self, keypoint_names: Sequence[str], frame_count: int, model_type: str = "heatmap",
+                 view_names: Sequence[str] | None = None) -> None:
         if keypoint_names is None:
             raise ValueError("must include `keypoint_names`")
         self.keypoint_names = list(keypoint_names)
         self.frame_count = int(frame_count)
         self.model_type = model_type
+        self.view_names = list(view_names) if view_names is not None else None
+
+    def _views(self) -> list[str]:
+        if not self.view_names:
+            raise ValueError("multi-view predictions need `view_names`")
+        return self.view_names
 
     @property
     def do_context(self) -> bool:
@@ -98,8 +107,16 @@ class PredictionHandler:
             arr = self.make_pred_arr_undo_resize(kp.numpy(), cf.numpy())
         return pd.DataFrame(arr, columns=make_dlc_pandas_index(self.model_type, self.keypoint_names))
 
-    def __call__(self, preds: Iterable[tuple[torch.Tensor, torch.Tensor]]):
-        """Reference call form: a list of per-batch (keypoints, confidences) tuples -> DataFrame."""
+    def dataframes(self, table: torch.Tensor | np.ndarray, frame_aligned: bool = False) -> dict:
+        """(N, 3 V K) multi-view prediction table -> ``{view_name: DataFrame}``, view v from columns [3 K v, 3 K (v + 1))."""
+        w = 3 * len(self.keypoint_names)
+        if table.shape[1] != w * len(self._views()):
+            raise ValueError(f"table has {table.shape[1]} columns; {len(self._views())} views of {w} expected")
+        return {name: self.dataframe(table[:, w * v : w * (v + 1)], frame_aligned) for v, name in enumerate(self._views())}
+
+    def __call__(self, preds: Iterable[tuple[torch.Tensor, torch.Tensor]], is_multiview_video: bool = False):
+        """Reference call form: a list of per-batch (keypoints, confidences) tuples -> DataFrame, or with
+        ``is_multiview_video`` the (N, 2 V K) / (N, V K) stack split into ``{view_name: DataFrame}`` (:287-315)."""
         preds = list(preds)
         kp = torch.vstack([p[0] for p in preds])[: self.frame_count]
         cf = torch.vstack([p[1] for p in preds])[: self.frame_count]
@@ -108,8 +125,16 @@ class PredictionHandler:
             cf = self.fix_context_preds_confs(cf, zero_pad_confidence=False)
         import pandas as pd
 
-        arr = self.make_pred_arr_undo_resize(kp.cpu().numpy(), cf.cpu().numpy())
-        return pd.DataFrame(arr, columns=make_dlc_pandas_index(self.model_type, self.keypoint_names))
+        columns = make_dlc_pandas_index(self.model_type, self.keypoint_names)
+        if not is_multiview_video:
+            return pd.DataFrame(self.make_pred_arr_undo_resize(kp.cpu().numpy(), cf.cpu().numpy()), columns=columns)
+        k = len(self.keypoint_names)
+        if cf.shape[1] != k * len(self._views()):
+            raise ValueError(f"predictions have {cf.shape[1]} keypoints; {len(self._views())} views of {k} expected")
+        kp_np, cf_np = kp.cpu().numpy(), cf.cpu().numpy()
+        return {name: pd.DataFrame(self.make_pred_arr_undo_resize(kp_np[:, 2 * k * v : 2 * k * (v + 1)], cf_np[:, k * v : k * (v + 1)]),
+                                   columns=columns)
+                for v, name in enumerate(self._views())}
 
 
 def _graph_kernel_count(graph: torch.cuda.CUDAGraph) -> int:
@@ -163,6 +188,18 @@ class BatchedPredictor:
     reference pads the tail with its first row).  Only when R = N - 1 does a row (N - 2) depend on frame N, the first
     padding frame of the last chunk; the reference reads the zero-filled frame its reader pads with there, so the
     caller's padding matters in that case only.  N < 5 raises (the reference has no window to predict from).
+
+    Multi-view mode (``head`` a ``HeatmapHead`` and ``num_views`` = V > 1: the multi-view transformer, or the heatmap
+    tracker with views folded into the batch; reference ``predict_video(video_file=[one per view])``,
+    ``utils/predictions.py:416-540``): ``chunk`` and ``sub_chunk`` count video frames, each of them V head items, and
+    ``features_of`` receives the (T V, 3, h, w) frame-major, view-minor batch (``model.forward_vit`` for the transformer,
+    the backbone for the folding tracker).  ``feed`` takes either V uint8 (T, H_v, W_v, 3) views (a list or tuple; sizes
+    may differ per view) - normalised to ``image_hw`` by one launch inside the chunk (``ops.frames_normalize_views``),
+    each view's box the whole frame ``[0, 0, H_v, W_v]``, fixed by the first chunk - or a (T, V, 3, h, w) frame tensor /
+    (T V, C, h', w') features with an optional (T, 4V) ``bbox`` (default: the whole model image of every view).  The
+    table is (N, 3 V K): view v owns columns [3 K v, 3 K (v + 1)), the reference's per-view split (``view_tables``,
+    ``PredictionHandler.dataframes``).  ``crop_dtype`` / ``crop_channels_last`` are the dtype and layout of the frames the
+    predictor's own ingest hands ``features_of``.
     """
 
     def __init__(self, head, num_keypoints: int, n_frames: int, chunk: int, image_hw: tuple[int, int],
@@ -185,7 +222,13 @@ class BatchedPredictor:
         self.image_hw = (int(image_hw[0]), int(image_hw[1]))
         self.features_of = features_of
         self.device = torch.device(device) if device is not None else next(head.parameters()).device
-        self.table = torch.zeros((self.n_frames, 3 * self.k), dtype=torch.float32, device=self.device)
+        self.num_views = int(num_views)
+        if self.num_views < 1:
+            raise ValueError(f"num_views must be >= 1; got {self.num_views}")
+        self.crop_dtype, self.crop_channels_last = crop_dtype, bool(crop_channels_last)
+        self._view_hw = None  # multi-view uint8 input: the views' frame sizes, fixed by the first chunk
+        self._view_bbox = None
+        self.table = torch.zeros((self.n_frames, 3 * self.k * self.num_views), dtype=torch.float32, device=self.device)
         self.cursor = torch.zeros((1,), dtype=torch.int64, device=self.device)
         self.use_graph = use_graph
         self._graph = None
@@ -202,7 +245,6 @@ class BatchedPredictor:
             if self.bboxes.shape[0] != self.n_frames:
                 raise ValueError(f"bboxes has {self.bboxes.shape[0]} rows but the video has {self.n_frames} frames")
             self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
-            self.crop_dtype, self.crop_channels_last = crop_dtype, bool(crop_channels_last)
         if self.context:
             # halo + chunk buffers: index b of the maps holds frame cursor - 4 + b, of the others frame cursor - 2 + b; the
             # maps' buffers are sized by the first chunk's maps
@@ -257,17 +299,25 @@ class BatchedPredictor:
         if self.context:
             self._context_chunk(x, bbox)
             return
+        v = self.num_views
+        if isinstance(x, list):  # V uint8 views -> (T V, 3, h, w), frame-major, view-minor
+            x = ops.frames_normalize_views(x, self.image_hw, channels_last=self.crop_channels_last, dtype=self.crop_dtype)
+        if x.dim() == 5:
+            x = x.reshape(-1, *x.shape[2:])
         feats = self.features_of(x) if self.features_of is not None else x
         with torch.no_grad():
             for i in range(0, self.chunk, self.sub_chunk):
-                heatmaps = self.head(feats[i : i + self.sub_chunk])
+                heatmaps = self.head(feats[i * v : (i + self.sub_chunk) * v])
                 kp, cf = self.head.run_subpixelmaxima(heatmaps)
-                kp = ops.remap_keypoints(kp, None, bbox[i : i + self.sub_chunk], self.image_hw[0], self.image_hw[1])  # model -> frame (bboxes.py:222-288)
+                if v > 1:  # (n V, 2K) -> (n, 2 V K): the views of a frame side by side, as the trackers fold them
+                    kp, cf = kp.reshape(-1, 2 * self.k * v), cf.reshape(-1, self.k * v)
+                kp = ops.remap_keypoints(kp, None, bbox[i : i + self.sub_chunk], self.image_hw[0], self.image_hw[1],
+                                         num_views=v)  # model -> frame (bboxes.py:222-288)
                 ops.pack_predictions(kp, cf, self.table, cursor=self.cursor)
 
-    def _capture(self, x: torch.Tensor, bbox: torch.Tensor) -> None:
-        self._static_in = torch.empty_like(x)
-        self._static_in.copy_(x)
+    def _capture(self, x: torch.Tensor | list[torch.Tensor], bbox: torch.Tensor) -> None:
+        self._static_in = [torch.empty_like(t) for t in x] if isinstance(x, list) else torch.empty_like(x)
+        self._copy_in(x)
         if bbox is not None:
             self._static_bbox = torch.empty_like(bbox)
             self._static_bbox.copy_(bbox)
@@ -286,10 +336,61 @@ class BatchedPredictor:
         self._graph.instantiate()
         self.cursor.zero_()  # the capture itself does not execute, but keep the invariant explicit
 
-    def feed(self, x: torch.Tensor, bbox: torch.Tensor | None = None) -> None:
+    def _copy_in(self, x: torch.Tensor | list[torch.Tensor]) -> None:
+        if isinstance(x, list):
+            for dst, src in zip(self._static_in, x):
+                dst.copy_(src, non_blocking=True)
+        else:
+            self._static_in.copy_(x, non_blocking=True)
+
+    def _is_views(self, x) -> bool:
+        return self.num_views > 1 and isinstance(x, (list, tuple)) and all(isinstance(t, torch.Tensor) and t.dtype == torch.uint8 for t in x)
+
+    def _check_views(self, x) -> tuple[list[torch.Tensor], torch.Tensor]:
+        """Multi-view uint8 input: V (T, H_v, W_v, 3) views of the sizes the first chunk fixed -> (views, their boxes)."""
+        views = list(x)
+        if len(views) != self.num_views:
+            raise ValueError(f"expected {self.num_views} views; got {len(views)}")
+        if self.features_of is None:
+            raise ValueError("uint8 views need features_of (frames -> features)")
+        for t in views:
+            if t.dim() != 4 or t.shape[-1] != 3:
+                raise ValueError(f"each view must be uint8 (T, H, W, 3); got {tuple(t.shape)}")
+        counts = [t.shape[0] for t in views]
+        if len(set(counts)) != 1:
+            raise ValueError(f"all views must have the same frame count; got {counts}")
+        if counts[0] != self.chunk:
+            raise ValueError(f"chunks are fixed-size ({self.chunk} frames); pad the last one (got {counts[0]})")
+        hw = [tuple(int(s) for s in t.shape[1:3]) for t in views]
+        if self._view_hw is None:
+            self._view_hw = hw
+            rows = [float(s) for h, w in hw for s in (0.0, 0.0, h, w)]
+            self._view_bbox = torch.tensor([rows], dtype=torch.float32, device=self.device).repeat(self.chunk, 1)
+        elif hw != self._view_hw:
+            raise ValueError(f"view sizes {hw} differ from the first chunk's {self._view_hw}")
+        return views, self._view_bbox
+
+    def feed(self, x: torch.Tensor | Sequence[torch.Tensor], bbox: torch.Tensor | None = None) -> None:
         """Process the next chunk (``x``: (T, ...) frames or features on the device; in crop mode uint8 (T, H, W, 3)
-        frames, and ``bbox`` must be None: the boxes come from the predictor's table)."""
-        if x.shape[0] != self.chunk:
+        frames, and ``bbox`` must be None: the boxes come from the predictor's table; in multi-view mode V uint8 views,
+        with ``bbox`` None, or (T, V, 3, h, w) frames / (T V, C, h', w') features)."""
+        if self.num_views > 1:
+            if isinstance(x, (list, tuple)):
+                if bbox is not None:
+                    raise ValueError("uint8 views take their boxes from the views' frame sizes")
+                x, bbox = self._check_views(x)
+            else:
+                n = x.shape[0] if x.dim() == 5 else x.shape[0] / self.num_views
+                if x.dim() == 5 and x.shape[1] != self.num_views:
+                    raise ValueError(f"expected (T, {self.num_views}, 3, h, w) frames; got {tuple(x.shape)}")
+                if n != self.chunk:
+                    raise ValueError(f"chunks are fixed-size ({self.chunk} frames of {self.num_views} views); got {tuple(x.shape)}")
+                if bbox is None:
+                    row = [0.0, 0.0, float(self.image_hw[0]), float(self.image_hw[1])] * self.num_views
+                    bbox = torch.tensor([row], device=self.device).repeat(self.chunk, 1)
+                elif tuple(bbox.shape) != (self.chunk, 4 * self.num_views):
+                    raise ValueError(f"bbox must be ({self.chunk}, {4 * self.num_views}); got {tuple(bbox.shape)}")
+        elif x.shape[0] != self.chunk:
             raise ValueError(f"chunks are fixed-size ({self.chunk} frames); pad the last one (got {x.shape[0]})")
         if self.bboxes is not None:
             if bbox is not None:
@@ -303,21 +404,29 @@ class BatchedPredictor:
             return
         if self._graph is None:
             self._capture(x, bbox)
-        self._static_in.copy_(x, non_blocking=True)
+        self._copy_in(x)
         if bbox is not None:
             self._static_bbox.copy_(bbox, non_blocking=True)
         self._graph.replay()
 
-    def run(self, chunks: Iterable[torch.Tensor | tuple[torch.Tensor, torch.Tensor]]) -> torch.Tensor:
-        """Feed every chunk of an iterable, return the (N, 3K) table (still on the device)."""
+    def run(self, chunks: Iterable[torch.Tensor | tuple[torch.Tensor, torch.Tensor] | Sequence[torch.Tensor]]) -> torch.Tensor:
+        """Feed every chunk of an iterable, return the (N, 3K) table (still on the device); in multi-view mode an item
+        may also be the chunk's V uint8 views."""
         for item in chunks:
-            if isinstance(item, tuple):
+            if isinstance(item, tuple) and not self._is_views(item):
                 self.feed(item[0], item[1])
             else:
                 self.feed(item)
         return self.table
 
     def results(self) -> tuple[torch.Tensor, torch.Tensor]:
-        """(keypoints (N, 2K), confidences (N, K)) views of the table - the reference's ``(preds, confs)`` pair."""
-        t = self.table.reshape(self.n_frames, self.k, 3)
-        return t[:, :, :2].reshape(self.n_frames, 2 * self.k), t[:, :, 2]
+        """(keypoints (N, 2K'), confidences (N, K')) views of the table - the reference's ``(preds, confs)`` pair, with
+        K' = V K in multi-view mode."""
+        kk = self.k * self.num_views
+        t = self.table.reshape(self.n_frames, kk, 3)
+        return t[:, :, :2].reshape(self.n_frames, 2 * kk), t[:, :, 2]
+
+    def view_tables(self) -> list[torch.Tensor]:
+        """The V (N, 3K) column blocks of the table, one per view (views, not copies)."""
+        w = 3 * self.k
+        return [self.table[:, w * v : w * (v + 1)] for v in range(self.num_views)]

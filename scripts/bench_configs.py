@@ -30,6 +30,24 @@ def head_for(arch, cin, gain=3.0):
     return head.to(dev)
 
 
+class Patch(torch.nn.Module):  # stand-in ViT patch embedding of the config-4 transformer
+    def __init__(self):
+        super().__init__()
+        self.proj = torch.nn.Conv2d(3, 384, 16, stride=16)
+
+    def forward(self, x):
+        return self.proj(x).flatten(2).transpose(1, 2)
+
+
+class Mix(torch.nn.Module):  # stand-in encoder: one token-mixing linear layer
+    def __init__(self):
+        super().__init__()
+        self.lin = torch.nn.Linear(384, 384)
+
+    def forward(self, t):
+        return (self.lin(t) + t.mean(1, keepdim=True)).bfloat16()
+
+
 def fwd_bwd(name, arch, shape, hm):
     b, c, fh, fw = shape
     head = head_for(arch, c)
@@ -179,6 +197,92 @@ def cfg3_context():
     res["cfg3_context_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
 
 
+def cfg4_predict():
+    """Multi-view video prediction with the config-4 transformer: 4 views of uint8 frames at mixed sizes (1024 x 1280 x 2,
+    720 x 1280 x 2) -> 384 x 384, the stand-in transformer at embedding 384 -> (T 4, 384, 24, 24) -> 96 x 96 heatmaps,
+    K = 17, T = 32 and 96 frames per chunk.  The ingest kernel against its bytes model (the source rows its bilinear taps
+    touch, read whole, plus the output) and against V x lpb_frames_normalize + torch.stack; the predictor's chunk (graph
+    replay and eager); the reference's form (per-view normalise + stack + predict_step + a host copy per batch + the host
+    per-view split)."""
+    import subprocess
+
+    import pandas  # noqa: F401  (imported here so that the handler's first call does not time the import)
+
+    from lightning_pose_b200 import ops
+    from lightning_pose_b200.models.heatmap_tracker_multiview import HeatmapTrackerMultiviewTransformer
+    from lightning_pose_b200.utils.predictions import PredictionHandler
+
+    shapes, side, k, v = ((1024, 1280), (1024, 1280), (720, 1280), (720, 1280)), 384, K, 4
+    torch.manual_seed(4)
+    model = HeatmapTrackerMultiviewTransformer(k, v, Patch(), Mix(), 384).to(dev).eval()
+
+    def touched_rows(h):  # distinct source rows read by the taps of the side output rows (y0 and y1 of resized_pixel)
+        sy = np.maximum((np.arange(side) + 0.5) * np.float32(h / side) - 0.5, 0)
+        y0 = np.minimum(sy.astype(np.int64), h - 1)
+        return len(set(y0) | set(np.minimum(y0 + 1, h - 1)))
+
+    def timed(fn, reps):
+        fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for i in range(reps):
+            fn(i)
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    for t in (32, 96):
+        gen = torch.Generator(device=dev).manual_seed(t)
+        pool = [[torch.randint(0, 256, (t, h, w, 3), dtype=torch.uint8, device=dev, generator=gen) for h, w in shapes] for _ in range(2)]
+        views = pool[0]
+        src = sum(t * touched_rows(h) * w * 3 for h, w in shapes)
+        for dtype, cl, form in ((torch.float32, False, "fchw_f32"), (torch.bfloat16, True, "fhwc_bf16")):
+            out_bytes = t * v * 3 * side * side * (4 if dtype == torch.float32 else 2)
+            ms, med = bench.time_stage(lambda: ops.frames_normalize_views(views, (side, side), channels_last=cl, dtype=dtype), flush)
+            ms_s, med_s = bench.time_stage(lambda: torch.stack([ops.frames_normalize(x, size=(side, side), channels_last=cl, dtype=dtype) for x in views], 1), flush)
+            res[f"cfg4_predict_T{t}_ingest_{form}"] = {
+                "frames": t, "views": v, "ms": ms, "ms_median": med, "bytes_model": src + out_bytes, "gbs": (src + out_bytes) / ms / 1e6,
+                "frac_hbm": (src + out_bytes) / ms / 1e6 / pk["hbm_gbs"], "per_view_normalize_plus_stack_ms": ms_s,
+                "per_view_normalize_plus_stack_ms_median": med_s}
+        n = t * 12
+        for mode in ("graph", "eager"):
+            bp = BatchedPredictor(model.head, k, n, t, (side, side), features_of=model.forward_vit, use_graph=mode == "graph", num_views=v)
+            ms = timed(lambda i=0: bp.feed(pool[i % 2]), 11)
+            res[f"cfg4_predict_T{t}_predictor_{mode}"] = {"video_frames_per_chunk": t, "ms_per_chunk": ms, "video_frames_per_s": 1e3 * t / ms,
+                                                         "launches_per_chunk": bp.launches_per_chunk}
+        ph = PredictionHandler([f"bp{i}" for i in range(k)], n, model_type="heatmap_multiview_transformer", view_names=["a", "b", "c", "d"])
+
+        def reference_form(i=0):  # one batch of the reference's loop, the handler's host split amortised over 4 batches
+            batch = {"frames": torch.stack([ops.frames_normalize(x, size=(side, side)) for x in pool[i % 2]], 1),
+                     "bbox": torch.tensor([[0.0, 0.0, float(h), float(w)] for h, w in shapes], device=dev).reshape(1, -1).repeat(t, 1),
+                     "is_multiview": True}
+            kp, cf = model.predict_step(batch, i)
+            preds.append((kp.cpu(), cf.cpu()))
+            if len(preds) == 4:
+                ph.frame_count = 4 * t
+                ph(preds, is_multiview_video=True)
+                preds.clear()
+
+        preds = []
+        ms = timed(reference_form, 8)
+        res[f"cfg4_predict_T{t}_reference_form"] = {"video_frames_per_batch": t, "ms_per_batch": ms, "video_frames_per_s": 1e3 * t / ms,
+                                                    "note": "eager; per-view normalise + stack + predict_step + host copy per batch + host per-view split"}
+        del pool, views
+    card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True).stdout.strip()
+    res["cfg4_predict_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0), "hbm_gbs_used": pk["hbm_gbs"]}
+
+
+if sys.argv[1:2] == ["cfg4_predict"]:  # only the multi-view prediction entries; an optional second argument names a JSON file
+    cfg4_predict()
+    if len(sys.argv) > 2:
+        os.makedirs(os.path.dirname(os.path.abspath(sys.argv[2])), exist_ok=True)
+        json.dump(res, open(sys.argv[2], "w"), indent=1)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
+
 if sys.argv[1:2] == ["cfg3_context"]:  # only the context-prediction entries; an optional second argument names a JSON file
     cfg3_context()
     if len(sys.argv) > 2:
@@ -294,24 +398,6 @@ ms, _ = bench.time_stage(lambda: torch.autograd.grad(stage3d(), kp_frame), flush
 res["cfg4_calibrated_3d_stage_fwd+bwd"] = {"frames": cb * cv, "ms": ms, "launches": 6, "note": "includes torch autograd bookkeeping and the small elementwise ops it adds"}
 
 
-class Patch(torch.nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.proj = torch.nn.Conv2d(3, 384, 16, stride=16)
-
-    def forward(self, x):
-        return self.proj(x).flatten(2).transpose(1, 2)
-
-
-class Mix(torch.nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.lin = torch.nn.Linear(384, 384)
-
-    def forward(self, t):
-        return (self.lin(t) + t.mean(1, keepdim=True)).bfloat16()
-
-
 kp_model = (torch.rand(cb, cv * K * 2, generator=gen) * img).to(dev)
 batch = {"images": torch.randn(cb, cv, 3, img, img, generator=gen).to(dev), "keypoints": kp_model.clone(),
          "heatmaps": ops.generate_heatmaps(kp_model.reshape(cb, cv * K, 2), img, img, (96, 96)), "bbox": bbox_c, "is_multiview": True,
@@ -400,6 +486,7 @@ for mode in ("on", "off"):
 card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 res["cfg5_crop_card"] = {"nvidia_smi": card, "torch_name": torch.cuda.get_device_name(0)}
 cfg3_context()
+cfg4_predict()
 cfg2_unlabeled_aug()
 
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
