@@ -159,47 +159,45 @@ def _graph_kernel_count(graph: torch.cuda.CUDAGraph) -> int:
 
 
 class BatchedPredictor:
-    """CUDA-graph chunk loop writing straight into a preallocated (N, 3K) device table.
+    """CUDA-graph chunk loop writing straight into a preallocated (N, 3 V K) device table, V = ``num_views``.
 
-    ``head``: a ``HeatmapHead`` (already on the device, eval).  ``features_of``: callable mapping a chunk's input (frames
-    or precomputed features) to backbone features ``(T, C, h, w)`` - identity when the caller streams features; a backbone
-    module otherwise (library convolutions; its kernels are captured into the same graph).  Chunks are fixed-size ``T``
-    (``dali.base.predict.sequence_length`` = 96 in the reference config); the last chunk is padded by the caller and its
-    surplus rows are dropped by the table writer.
+    ``head``: a ``HeatmapHead`` or ``HeatmapMHCRNNHead`` on the device, in eval mode.  Each ``feed`` is a chunk of
+    exactly T = ``chunk`` video frames (``dali.base.predict.sequence_length`` = 96 in the reference config): the caller
+    pads the last one and the table writer drops the surplus rows, at ``cursor``, a device int64 that each chunk
+    advances, so nothing returns to the host until the video is done.  ``features_of`` maps the chunk's T V frames (frame-major,
+    view-minor) to backbone features: None when the caller streams features, else a backbone, captured into the same
+    graph.  With ``use_graph`` the first chunk is captured (``launches_per_chunk`` counts its kernels) and every chunk
+    replays it, so every chunk must have the first one's form, shapes and dtypes.  The input forms:
 
-    Crop mode (crop-zoom pose models, reference ``predict_video(..., bbox_file=...)``, ``utils/predictions.py:455-470``
-    and ``data/video/dali.py:332-380``): ``bboxes`` is the video's (N, 4) [x, y, h, w] device table (``compute_bboxes``
-    / ``smooth_bboxes``) and ``frame_hw`` the full frame size.  ``feed`` then takes uint8 (T, H, W, 3) decoded frames;
-    inside the chunk (and its graph) one launch crops each frame to its box row at the table's device cursor (rows past
-    the end repeat the last), resizes the crop to ``image_hw`` and normalises it into ``crop_dtype`` (channels-last if
-    ``crop_channels_last``) for ``features_of``, and the clamped boxes it writes map the keypoints back to the frame.
-    ``launches_per_chunk``: kernel launches in one captured chunk (set at capture).
+    Tensor: (T V, ...) frames or features, or (T, V, 3, h, w) frames, and an optional (T, 4 V) ``bbox``, [x, y, h, w]
+    per view, that maps keypoints back to the frame (default: the whole model image ``image_hw``).
 
-    Context mode (``head`` a ``HeatmapMHCRNNHead``, reference ``HeatmapTrackerMHCRNN.predict_step`` over a reader of
-    windows of ``S = chunk + 4`` frames with step ``chunk``, ``dali.context.predict.sequence_length``): ``chunk`` is the
-    number of NEW frames per call, the caller feeds ``ceil(N / chunk)`` non-overlapping chunks (the last one padded) and
-    chunk j yields the predictions of frames ``j * chunk - 2 .. j * chunk + chunk - 3``.  The two / four frames before a
-    chunk stay on the device between calls (their single-frame decode, their boxes and their W_f / W_b maps), so every
-    frame passes through ``features_of``, ``head_sf`` and the maps once.  ``lpb_pack_context_predictions`` writes each
-    frame's selected, remapped prediction to every row the reference's ``fix_context_preds_confs`` gives it, so after
-    the last chunk ``table`` is the reference's final table for ``sequence_length = chunk + 4`` with no host fix-up (use
-    ``PredictionHandler.dataframe(table, frame_aligned=True)``).  With R = chunk * (ceil((N - S) / chunk) + 1):
-    R >= N: row f is frame clamp(f, 2, N - 3); R < N: row f is frame f for 2 <= f <= R - 1 and frame 2 otherwise (the
-    reference pads the tail with its first row).  Only when R = N - 1 does a row (N - 2) depend on frame N, the first
-    padding frame of the last chunk; the reference reads the zero-filled frame its reader pads with there, so the
-    caller's padding matters in that case only.  N < 5 raises (the reference has no window to predict from).
+    Views (reference ``predict_video(video_file=[one per view])``, ``utils/predictions.py:416-540``): V uint8
+    (T, H_v, W_v, 3) views in a list or tuple, sizes fixed by the first chunk, normalised by one launch inside the chunk
+    (``ops.frames_normalize_views``); each view's box is its whole frame.
 
-    Multi-view mode (``head`` a ``HeatmapHead`` and ``num_views`` = V > 1: the multi-view transformer, or the heatmap
-    tracker with views folded into the batch; reference ``predict_video(video_file=[one per view])``,
-    ``utils/predictions.py:416-540``): ``chunk`` and ``sub_chunk`` count video frames, each of them V head items, and
-    ``features_of`` receives the (T V, 3, h, w) frame-major, view-minor batch (``model.forward_vit`` for the transformer,
-    the backbone for the folding tracker).  ``feed`` takes either V uint8 (T, H_v, W_v, 3) views (a list or tuple; sizes
-    may differ per view) - normalised to ``image_hw`` by one launch inside the chunk (``ops.frames_normalize_views``),
-    each view's box the whole frame ``[0, 0, H_v, W_v]``, fixed by the first chunk - or a (T, V, 3, h, w) frame tensor /
-    (T V, C, h', w') features with an optional (T, 4V) ``bbox`` (default: the whole model image of every view).  The
-    table is (N, 3 V K): view v owns columns [3 K v, 3 K (v + 1)), the reference's per-view split (``view_tables``,
-    ``PredictionHandler.dataframes``).  ``crop_dtype`` / ``crop_channels_last`` are the dtype and layout of the frames the
-    predictor's own ingest hands ``features_of``.
+    Crop (crop-zoom models, reference ``predict_video(..., bbox_file=...)``, ``utils/predictions.py:455-470`` and
+    ``data/video/dali.py:332-380``): with ``bboxes``, the video's (N, 4) device table (``compute_bboxes`` /
+    ``smooth_bboxes``), and ``frame_hw``, uint8 (T, H, W, 3) full frames and no ``bbox``.  One launch inside the chunk
+    crops each frame to its row at the cursor (rows past the end repeat the last) and resizes it; the clamped boxes it
+    writes map the keypoints back.  Both ingests write ``crop_dtype``, channels-last if ``crop_channels_last``.
+
+    The body runs ``sub_chunk`` frames at a time.  Frame body (``HeatmapHead``; for V > 1 the multi-view transformer's,
+    ``features_of=model.forward_vit``, or a tracker's that folds views into the batch): head -> decode -> remap ->
+    ``lpb_pack_predictions``; view v owns columns [3 K v, 3 K (v + 1)), the reference's per-view split
+    (``view_tables``, ``PredictionHandler.dataframes``).
+
+    Context body (``HeatmapMHCRNNHead``, one view; reference ``HeatmapTrackerMHCRNN.predict_step`` over windows of
+    S = T + 4 frames with step T, ``dali.context.predict.sequence_length``): T counts NEW frames; chunk j yields frames
+    j T - 2 .. j T + T - 3.  The two / four frames before a chunk stay on the device (their single-frame decode, boxes
+    and W_f / W_b maps), so every frame passes through ``features_of``, ``head_sf`` and the maps once.
+    ``lpb_pack_context_predictions`` writes each frame's selected, remapped prediction to every row the reference's
+    ``fix_context_preds_confs`` gives it: after the last chunk ``table`` is the reference's final table
+    (``PredictionHandler.dataframe(table, frame_aligned=True)``).  With R = T (ceil((N - S) / T) + 1): R >= N: row f is
+    frame clamp(f, 2, N - 3); R < N: row f is frame f for 2 <= f <= R - 1 and frame 2 otherwise (the reference pads the
+    tail with its first row).  Only when R = N - 1 does a row (N - 2) depend on frame N, the first padding frame of the
+    last chunk; the reference reads the zero-filled frame its reader pads with there, so the caller's padding matters in
+    that case only.  N < 5 raises (the reference has no window to predict from).
     """
 
     def __init__(self, head, num_keypoints: int, n_frames: int, chunk: int, image_hw: tuple[int, int],
@@ -210,34 +208,32 @@ class BatchedPredictor:
 
         self.head, self.k, self.n_frames, self.chunk = head, int(num_keypoints), int(n_frames), int(chunk)
         self.context = isinstance(head, HeatmapMHCRNNHead)
-        if self.context and int(num_views) > 1:
+        self.num_views = int(num_views)
+        if self.context and self.num_views > 1:
             raise ValueError("context prediction is not supported for multiview models")
         if self.context and self.n_frames < 5:
             raise ValueError(f"a context model needs at least 5 frames to predict from; the video has {self.n_frames}")
         if self.chunk < 1:
             raise ValueError(f"chunk must be >= 1; got {self.chunk}")
+        if self.num_views < 1:
+            raise ValueError(f"num_views must be >= 1; got {self.num_views}")
         # frames per head / decode call inside a chunk: small enough that the heatmaps written by the head are still in
         # the 126 MB L2 when the decode reads them (None: the whole chunk at once)
         self.sub_chunk = int(sub_chunk) if sub_chunk else self.chunk
         self.image_hw = (int(image_hw[0]), int(image_hw[1]))
         self.features_of = features_of
         self.device = torch.device(device) if device is not None else next(head.parameters()).device
-        self.num_views = int(num_views)
-        if self.num_views < 1:
-            raise ValueError(f"num_views must be >= 1; got {self.num_views}")
         self.crop_dtype, self.crop_channels_last = crop_dtype, bool(crop_channels_last)
-        self._view_hw = None  # multi-view uint8 input: the views' frame sizes, fixed by the first chunk
-        self._view_bbox = None
         self.table = torch.zeros((self.n_frames, 3 * self.k * self.num_views), dtype=torch.float32, device=self.device)
         self.cursor = torch.zeros((1,), dtype=torch.int64, device=self.device)
         self.use_graph = use_graph
-        self._graph = None
-        self._static_in = None
-        self._static_bbox = None
+        self._graph = self._static = self._captured = None
         self.launches_per_chunk = None
+        self._image_bbox = self._whole_frames([self.image_hw] * self.num_views)
+        self._view_hw = self._view_bbox = None  # uint8 views: their frame sizes and boxes, fixed by the first chunk
         self.bboxes = None
         if bboxes is not None:
-            if int(num_views) > 1:
+            if self.num_views > 1:
                 raise ValueError("bbox cropping is not supported for multiview models")
             if frame_hw is None or features_of is None:
                 raise ValueError("crop mode needs frame_hw (the full frame size) and features_of (frames -> features)")
@@ -245,9 +241,7 @@ class BatchedPredictor:
             if self.bboxes.shape[0] != self.n_frames:
                 raise ValueError(f"bboxes has {self.bboxes.shape[0]} rows but the video has {self.n_frames} frames")
             self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
-        if self.context:
-            # halo + chunk buffers: index b of the maps holds frame cursor - 4 + b, of the others frame cursor - 2 + b; the
-            # maps' buffers are sized by the first chunk's maps
+        if self.context:  # the halo buffers; the maps' are sized by the first chunk's maps
             t, k, dev = self.chunk, self.k, self.device
             self._wf = self._wb = None
             self._kp_sf = torch.zeros((t + 2, 2 * k), dtype=torch.float32, device=dev)
@@ -255,166 +249,160 @@ class BatchedPredictor:
             self._box = torch.zeros((t + 2, 4), dtype=torch.float32, device=dev)
             self._idx = (torch.arange(t, device=dev)[:, None] + torch.arange(5, device=dev)[None, :]).to(torch.int32)
 
+    def _whole_frames(self, sizes: list[tuple[int, int]]) -> torch.Tensor:
+        """(T, 4 V) boxes [0, 0, h, w] of whole frames of the views' ``sizes``."""
+        row = [float(s) for h, w in sizes for s in (0, 0, h, w)]
+        return torch.tensor([row], dtype=torch.float32, device=self.device).repeat(self.chunk, 1)
+
+    def _halo(self) -> tuple[tuple[torch.Tensor, int], ...]:
+        """The context buffers and their halo rows: row b of the maps holds frame cursor - 4 + b, of the others frame
+        cursor - 2 + b."""
+        return ((self._wf, 4), (self._wb, 4), (self._kp_sf, 2), (self._cf_sf, 2), (self._box, 2))
+
     def _reset(self) -> None:
         self.cursor.zero_()
         self.table.zero_()
         if self.context:
-            for buf in (self._wf, self._wb, self._kp_sf, self._cf_sf, self._box):
-                if buf is not None:
-                    buf.zero_()
+            for buf, _ in self._halo():
+                buf.zero_()
 
-    def _context_chunk(self, x: torch.Tensor, bbox: torch.Tensor) -> None:
-        """One context chunk, eager: T new frames -> the predictions of frames cursor - 2 .. cursor + T - 3."""
-        head, mf = self.head, self.head.head_mf
+    def _inputs(self, x, bbox) -> tuple[str, tuple[torch.Tensor, ...]]:
+        """A chunk as fed -> (its form, its checked tensors): "crop" (frames,), "views" (*views, boxes) or
+        "tensor" (x, boxes)."""
+        t, v = self.chunk, self.num_views
+        if self.bboxes is not None:
+            if bbox is not None:
+                raise ValueError("crop mode takes its boxes from the `bboxes` table given at construction")
+            if x.dtype != torch.uint8 or tuple(x.shape) != (t, *self.frame_hw, 3):
+                raise ValueError(f"crop mode expects uint8 ({t}, {self.frame_hw[0]}, {self.frame_hw[1]}, 3) frames; got {tuple(x.shape)} {x.dtype}")
+            return "crop", (x,)
+        if isinstance(x, (list, tuple)):
+            if bbox is not None:
+                raise ValueError("uint8 views take their boxes from the views' frame sizes")
+            if len(x) != v:
+                raise ValueError(f"expected {v} views; got {len(x)}")
+            if self.features_of is None:
+                raise ValueError("uint8 views need features_of (frames -> features)")
+            for view in x:
+                if view.dtype != torch.uint8 or view.dim() != 4 or view.shape[-1] != 3:
+                    raise ValueError(f"each view must be uint8 (T, H, W, 3); got {tuple(view.shape)} {view.dtype}")
+            counts = [view.shape[0] for view in x]
+            if len(set(counts)) != 1:
+                raise ValueError(f"all views must have the same frame count; got {counts}")
+            if counts[0] != t:
+                raise ValueError(f"chunks are fixed-size ({t} frames); pad the last one (got {counts[0]})")
+            hw = [tuple(int(s) for s in view.shape[1:3]) for view in x]
+            if self._view_hw is None:
+                self._view_hw, self._view_bbox = hw, self._whole_frames(hw)
+            elif hw != self._view_hw:
+                raise ValueError(f"view sizes {hw} differ from the first chunk's {self._view_hw}")
+            return "views", (*x, self._view_bbox)
+        if x.dim() == 5 and x.shape[1] != v:
+            raise ValueError(f"expected (T, {v}, 3, h, w) frames; got {tuple(x.shape)}")
+        if x.shape[0] != (t if x.dim() == 5 else t * v):
+            raise ValueError(f"chunks are fixed-size, ({t * v}, ...) or ({t}, {v}, ...); pad the last one (got {tuple(x.shape)})")
+        if bbox is None:
+            bbox = self._image_bbox
+        elif tuple(bbox.shape) != (t, 4 * v):
+            raise ValueError(f"bbox must be ({t}, {4 * v}); got {tuple(bbox.shape)}")
+        return "tensor", (x, bbox)
+
+    def _ingest(self, form: str, xs) -> tuple[torch.Tensor, torch.Tensor]:
+        """A chunk's tensors -> (the (T V, ...) batch for ``features_of``, the (T, 4 V) boxes)."""
+        if form == "crop":  # crop to the rows at the cursor BEFORE the table writer advances it
+            x, bbox = ops.frames_crop_normalize(xs[0], self.bboxes, self.image_hw, cursor=self.cursor,
+                                                channels_last=self.crop_channels_last, dtype=self.crop_dtype)
+        elif form == "views":
+            x = ops.frames_normalize_views(xs[:-1], self.image_hw, channels_last=self.crop_channels_last, dtype=self.crop_dtype)
+            bbox = xs[-1]
+        else:
+            x, bbox = xs
+        return (x.reshape(-1, *x.shape[2:]) if x.dim() == 5 else x), bbox
+
+    @torch.no_grad()
+    def _chunk(self, form: str, xs) -> None:
+        """One chunk, enqueued on the current stream with no host sync: ingest, features, the body per sub-chunk."""
+        x, bbox = self._ingest(form, xs)
+        feats = self.features_of(x) if self.features_of is not None else x
+        emit = self._emit_context if self.context else self._emit_frames
+        for i in range(0, self.chunk, self.sub_chunk):
+            emit(feats, bbox, i, min(self.sub_chunk, self.chunk - i))
+
+    def _emit_frames(self, feats: torch.Tensor, bbox: torch.Tensor, i: int, n: int) -> None:
+        """Frames [i, i + n) of the chunk: head -> decode -> model->frame remap (bboxes.py:222-288) -> table rows."""
+        v = self.num_views
+        kp, cf = self.head.run_subpixelmaxima(self.head(feats[i * v : (i + n) * v]))
+        # (n V, 2K) -> (n, 2 V K): the views of a frame side by side, as the trackers fold them
+        kp = ops.remap_keypoints(kp.reshape(n, 2 * self.k * v), None, bbox[i : i + n], *self.image_hw, num_views=v)
+        ops.pack_predictions(kp, cf.reshape(n, self.k * v), self.table, cursor=self.cursor)
+
+    def _emit_context(self, feats: torch.Tensor, bbox: torch.Tensor, i: int, n: int) -> None:
+        """Frames [i, i + n) of a context chunk: the single-frame head and the W_f / W_b maps into the halo buffers, then
+        the predictions of frames cursor - 2 + i .. cursor - 3 + i + n.  The first sub-chunk stores the chunk's boxes,
+        the last one makes the chunk's final frames the next chunk's halo."""
+        head, mf, t = self.head, self.head.head_mf, self.chunk
+        if i == 0:
+            self._box[2:].copy_(bbox)
+        f = feats[i : i + n]
+        kp, cf = head.run_subpixelmaxima(head.head_sf(f))  # single-frame head, once per frame
+        self._kp_sf[2 + i : 2 + i + n].copy_(kp)
+        self._cf_sf[2 + i : 2 + i + n].copy_(cf)
+        wf, wb = mf._maps(f)  # W_f / W_b, once per frame
+        if self._wf is None:
+            self._wf = torch.zeros((t + 4, *wf.shape[1:]), dtype=torch.float32, device=self.device)
+            self._wb = torch.zeros_like(self._wf)
+        self._wf[4 + i : 4 + i + n].copy_(wf)
+        self._wb[4 + i : 4 + i + n].copy_(wb)
         hf = (mf.H_f[0].weight, mf.H_f[0].bias, mf.H_f[1].weight, mf.H_f[1].bias)
         hb = (mf.H_b[0].weight, mf.H_b[0].bias, mf.H_b[1].weight, mf.H_b[1].bias)
-        t = self.chunk
-        with torch.no_grad():
-            feats = self.features_of(x) if self.features_of is not None else x
-            self._box[2:].copy_(bbox)
-            for i in range(0, t, self.sub_chunk):
-                n = min(self.sub_chunk, t - i)
-                f = feats[i : i + n]
-                kp, cf = head.run_subpixelmaxima(head.head_sf(f))  # single-frame head, once per frame
-                self._kp_sf[2 + i : 2 + i + n].copy_(kp)
-                self._cf_sf[2 + i : 2 + i + n].copy_(cf)
-                wf, wb = mf._maps(f)  # W_f / W_b, once per frame
-                if self._wf is None:
-                    self._wf = torch.zeros((t + 4, *wf.shape[1:]), dtype=torch.float32, device=self.device)
-                    self._wb = torch.zeros_like(self._wf)
-                self._wf[4 + i : 4 + i + n].copy_(wf)
-                self._wb[4 + i : 4 + i + n].copy_(wb)
-                kp_mf, cf_mf = head.run_subpixelmaxima(ops.plane_softmax(ops.crnn_combine(self._wf, self._wb, self._idx[i : i + n], hf, hb)))
-                ops.pack_context_predictions(self._kp_sf[i : i + n], self._cf_sf[i : i + n], kp_mf, cf_mf, self._box[i : i + n],
-                                             self.image_hw[0], self.image_hw[1], self.table, t, cursor=self.cursor)
-            for buf, halo in ((self._wf, 4), (self._wb, 4), (self._kp_sf, 2), (self._cf_sf, 2), (self._box, 2)):
+        kp_mf, cf_mf = head.run_subpixelmaxima(ops.plane_softmax(ops.crnn_combine(self._wf, self._wb, self._idx[i : i + n], hf, hb)))
+        ops.pack_context_predictions(self._kp_sf[i : i + n], self._cf_sf[i : i + n], kp_mf, cf_mf, self._box[i : i + n],
+                                     *self.image_hw, self.table, t, cursor=self.cursor)
+        if i + n == t:
+            for buf, halo in self._halo():
                 tail = buf[t : t + halo]
-                buf[:halo].copy_(tail.clone() if t < halo else tail)  # the last frames become the next chunk's halo
+                buf[:halo].copy_(tail.clone() if t < halo else tail)
 
-    # one chunk, eager: everything below is enqueued on the current stream; no host sync
-    def _chunk(self, x: torch.Tensor, bbox: torch.Tensor | None) -> None:
-        if self.bboxes is not None:  # crop to the rows at the cursor BEFORE the table writer advances it
-            x, bbox = ops.frames_crop_normalize(x, self.bboxes, self.image_hw, cursor=self.cursor, channels_last=self.crop_channels_last,
-                                                dtype=self.crop_dtype)
-        if self.context:
-            self._context_chunk(x, bbox)
-            return
-        v = self.num_views
-        if isinstance(x, list):  # V uint8 views -> (T V, 3, h, w), frame-major, view-minor
-            x = ops.frames_normalize_views(x, self.image_hw, channels_last=self.crop_channels_last, dtype=self.crop_dtype)
-        if x.dim() == 5:
-            x = x.reshape(-1, *x.shape[2:])
-        feats = self.features_of(x) if self.features_of is not None else x
-        with torch.no_grad():
-            for i in range(0, self.chunk, self.sub_chunk):
-                heatmaps = self.head(feats[i * v : (i + self.sub_chunk) * v])
-                kp, cf = self.head.run_subpixelmaxima(heatmaps)
-                if v > 1:  # (n V, 2K) -> (n, 2 V K): the views of a frame side by side, as the trackers fold them
-                    kp, cf = kp.reshape(-1, 2 * self.k * v), cf.reshape(-1, self.k * v)
-                kp = ops.remap_keypoints(kp, None, bbox[i : i + self.sub_chunk], self.image_hw[0], self.image_hw[1],
-                                         num_views=v)  # model -> frame (bboxes.py:222-288)
-                ops.pack_predictions(kp, cf, self.table, cursor=self.cursor)
-
-    def _capture(self, x: torch.Tensor | list[torch.Tensor], bbox: torch.Tensor) -> None:
-        self._static_in = [torch.empty_like(t) for t in x] if isinstance(x, list) else torch.empty_like(x)
-        self._copy_in(x)
-        if bbox is not None:
-            self._static_bbox = torch.empty_like(bbox)
-            self._static_bbox.copy_(bbox)
+    def _capture(self, form: str, xs) -> None:
+        self._static = [x.clone() for x in xs]
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
             for _ in range(2):  # warm-up (per-shape tables, allocator pools); rewind the cursor afterwards
-                self._chunk(self._static_in, self._static_bbox)
+                self._chunk(form, self._static)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         self._reset()
         self._graph = torch.cuda.CUDAGraph(keep_graph=True)  # kept so that its kernel nodes can be counted
         with torch.cuda.graph(self._graph):
-            self._chunk(self._static_in, self._static_bbox)
+            self._chunk(form, self._static)
         self.launches_per_chunk = _graph_kernel_count(self._graph)
         self._graph.instantiate()
         self.cursor.zero_()  # the capture itself does not execute, but keep the invariant explicit
 
-    def _copy_in(self, x: torch.Tensor | list[torch.Tensor]) -> None:
-        if isinstance(x, list):
-            for dst, src in zip(self._static_in, x):
-                dst.copy_(src, non_blocking=True)
-        else:
-            self._static_in.copy_(x, non_blocking=True)
-
-    def _is_views(self, x) -> bool:
-        return self.num_views > 1 and isinstance(x, (list, tuple)) and all(isinstance(t, torch.Tensor) and t.dtype == torch.uint8 for t in x)
-
-    def _check_views(self, x) -> tuple[list[torch.Tensor], torch.Tensor]:
-        """Multi-view uint8 input: V (T, H_v, W_v, 3) views of the sizes the first chunk fixed -> (views, their boxes)."""
-        views = list(x)
-        if len(views) != self.num_views:
-            raise ValueError(f"expected {self.num_views} views; got {len(views)}")
-        if self.features_of is None:
-            raise ValueError("uint8 views need features_of (frames -> features)")
-        for t in views:
-            if t.dim() != 4 or t.shape[-1] != 3:
-                raise ValueError(f"each view must be uint8 (T, H, W, 3); got {tuple(t.shape)}")
-        counts = [t.shape[0] for t in views]
-        if len(set(counts)) != 1:
-            raise ValueError(f"all views must have the same frame count; got {counts}")
-        if counts[0] != self.chunk:
-            raise ValueError(f"chunks are fixed-size ({self.chunk} frames); pad the last one (got {counts[0]})")
-        hw = [tuple(int(s) for s in t.shape[1:3]) for t in views]
-        if self._view_hw is None:
-            self._view_hw = hw
-            rows = [float(s) for h, w in hw for s in (0.0, 0.0, h, w)]
-            self._view_bbox = torch.tensor([rows], dtype=torch.float32, device=self.device).repeat(self.chunk, 1)
-        elif hw != self._view_hw:
-            raise ValueError(f"view sizes {hw} differ from the first chunk's {self._view_hw}")
-        return views, self._view_bbox
-
     def feed(self, x: torch.Tensor | Sequence[torch.Tensor], bbox: torch.Tensor | None = None) -> None:
-        """Process the next chunk (``x``: (T, ...) frames or features on the device; in crop mode uint8 (T, H, W, 3)
-        frames, and ``bbox`` must be None: the boxes come from the predictor's table; in multi-view mode V uint8 views,
-        with ``bbox`` None, or (T, V, 3, h, w) frames / (T V, C, h', w') features)."""
-        if self.num_views > 1:
-            if isinstance(x, (list, tuple)):
-                if bbox is not None:
-                    raise ValueError("uint8 views take their boxes from the views' frame sizes")
-                x, bbox = self._check_views(x)
-            else:
-                n = x.shape[0] if x.dim() == 5 else x.shape[0] / self.num_views
-                if x.dim() == 5 and x.shape[1] != self.num_views:
-                    raise ValueError(f"expected (T, {self.num_views}, 3, h, w) frames; got {tuple(x.shape)}")
-                if n != self.chunk:
-                    raise ValueError(f"chunks are fixed-size ({self.chunk} frames of {self.num_views} views); got {tuple(x.shape)}")
-                if bbox is None:
-                    row = [0.0, 0.0, float(self.image_hw[0]), float(self.image_hw[1])] * self.num_views
-                    bbox = torch.tensor([row], device=self.device).repeat(self.chunk, 1)
-                elif tuple(bbox.shape) != (self.chunk, 4 * self.num_views):
-                    raise ValueError(f"bbox must be ({self.chunk}, {4 * self.num_views}); got {tuple(bbox.shape)}")
-        elif x.shape[0] != self.chunk:
-            raise ValueError(f"chunks are fixed-size ({self.chunk} frames); pad the last one (got {x.shape[0]})")
-        if self.bboxes is not None:
-            if bbox is not None:
-                raise ValueError("crop mode takes its boxes from the `bboxes` table given at construction")
-            if x.dtype != torch.uint8 or tuple(x.shape[1:]) != (*self.frame_hw, 3):
-                raise ValueError(f"crop mode expects uint8 ({self.chunk}, {self.frame_hw[0]}, {self.frame_hw[1]}, 3) frames; got {tuple(x.shape)} {x.dtype}")
-        elif bbox is None:
-            bbox = torch.tensor([[0.0, 0.0, float(self.image_hw[0]), float(self.image_hw[1])]], device=self.device).repeat(self.chunk, 1)
+        """Process the next chunk: a tensor with an optional ``bbox``, V uint8 views, or in crop mode uint8 full frames
+        (the forms of the class docstring)."""
+        form, xs = self._inputs(x, bbox)
         if not self.use_graph:
-            self._chunk(x, bbox)
+            self._chunk(form, xs)
             return
+        got = f"{form} " + ", ".join(f"{tuple(t.shape)} {t.dtype}" for t in xs)
         if self._graph is None:
-            self._capture(x, bbox)
-        self._copy_in(x)
-        if bbox is not None:
-            self._static_bbox.copy_(bbox, non_blocking=True)
+            self._capture(form, xs)
+            self._captured = got
+        if got != self._captured:  # a replay would cast or mis-read it
+            raise ValueError(f"the chunk's graph was captured for {self._captured}; this chunk is {got}")
+        for dst, src in zip(self._static, xs):
+            dst.copy_(src, non_blocking=True)
         self._graph.replay()
 
     def run(self, chunks: Iterable[torch.Tensor | tuple[torch.Tensor, torch.Tensor] | Sequence[torch.Tensor]]) -> torch.Tensor:
-        """Feed every chunk of an iterable, return the (N, 3K) table (still on the device); in multi-view mode an item
-        may also be the chunk's V uint8 views."""
+        """Feed every chunk of an iterable, return the (N, 3 V K) table (still on the device).  An item is a chunk, a
+        (chunk, bbox) pair, or a chunk's uint8 views."""
         for item in chunks:
-            if isinstance(item, tuple) and not self._is_views(item):
-                self.feed(item[0], item[1])
+            if isinstance(item, tuple) and not all(isinstance(t, torch.Tensor) and t.dtype == torch.uint8 for t in item):
+                self.feed(*item)
             else:
                 self.feed(item)
         return self.table

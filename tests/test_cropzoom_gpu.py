@@ -206,3 +206,5 @@ def test_batched_predictor_crop_mode_adds_one_launch():
     assert crop.launches_per_chunk == plain.launches_per_chunk + 1, (crop.launches_per_chunk, plain.launches_per_chunk)
     with pytest.raises(ValueError, match="uint8"):
         crop.feed(video.float())
+    with pytest.raises(ValueError, match="boxes from the `bboxes` table"):
+        crop.feed(video, boxes)

@@ -44,6 +44,54 @@ def test_context_shift_fixup_matches_reference_rule():
     assert h2.fix_context_preds_confs(stacked.clone()).flatten().tolist() == [0.0, 0.0, 0.0, 10.0, 20.0, 30.0, 0.0, 0.0]
 
 
+def test_batched_predictor_refuses_bad_single_view_chunks():
+    """One view takes the tensor form's checks of several: the chunk's length, the view count of (T, V, 3, h, w) frames
+    and the (T, 4) box, all refused before anything is enqueued (the head stays on the CPU)."""
+    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
+    from lightning_pose_b200.utils.predictions import BatchedPredictor
+
+    bp = BatchedPredictor(HeatmapHead("vits_dino", 64, 5), 5, 20, 4, (32, 32))
+    with pytest.raises(ValueError, match="fixed-size"):
+        bp.feed(torch.zeros(3, 64, 2, 2))
+    with pytest.raises(ValueError, match=r"expected \(T, 1, 3, h, w\)"):
+        bp.feed(torch.zeros(4, 2, 3, 32, 32))
+    with pytest.raises(ValueError, match=r"bbox must be \(4, 4\)"):
+        bp.feed(torch.zeros(4, 64, 2, 2), torch.zeros(4, 8))
+    with pytest.raises(ValueError, match=r"bbox must be \(4, 4\)"):
+        bp.feed(torch.zeros(4, 64, 2, 2), torch.zeros(3, 4))
+
+
+def test_context_predictor_refuses_a_chunk_of_the_wrong_length():
+    from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
+    from lightning_pose_b200.utils.predictions import BatchedPredictor
+
+    bp = BatchedPredictor(HeatmapMHCRNNHead("vits_dino", 64, 5), 5, 20, 4, (32, 32))
+    with pytest.raises(ValueError, match="fixed-size"):
+        bp.feed(torch.zeros(5, 64, 2, 2))
+
+
+@pytest.mark.gpu
+def test_batched_predictor_graph_refuses_a_chunk_unlike_its_capture():
+    """A replay copies the chunk into the captured input, which would cast fp32 features to the bf16 of the capture, so
+    graph mode refuses the chunk and names both forms; eager mode takes either."""
+    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
+    from lightning_pose_b200.utils.predictions import BatchedPredictor
+
+    dev = torch.device("cuda:0")
+    torch.manual_seed(5)
+    head = HeatmapHead("resnet50", 512, 17).to(dev).eval()
+    feats = torch.randn(8, 512, 4, 4, device=dev) * 0.5
+    graph = BatchedPredictor(head, 17, 16, 8, (128, 128))
+    graph.feed(feats.bfloat16())
+    with pytest.raises(ValueError, match=r"captured for tensor \(8, 512, 4, 4\) torch.bfloat16, .*; this chunk is tensor \(8, 512, 4, 4\) torch.float32"):
+        graph.feed(feats)
+    assert int(graph.cursor) == 8
+    eager = BatchedPredictor(head, 17, 16, 8, (128, 128), use_graph=False)
+    eager.feed(feats.bfloat16())
+    eager.feed(feats)
+    assert int(eager.cursor) == 16
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("use_graph", [True, False])
 def test_batched_predictor_matches_oracle(use_graph):
