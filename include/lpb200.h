@@ -125,6 +125,7 @@ int lpb_head_fwd_f32(const float* features, int B, int C, int H, int W, const fl
 
 /* The same stack one layer at a time (any number of deconvs: n_layers = log2(stride) - downsample_factor - 1,
  * heads/heatmap.py:192-193), with its native backward -- the fp32 reference precision path trains through these.
+ * Every convolution runs on the tensor cores in 3xTF32 (fp32 accuracy); any Cin, Cout, Hi, Wi (even with shuffle).
  *   lpb_convt_fwd_f32   in [B, Cin(*4 if shuffle), Hi(/2), Wi(/2)] -> out [B, Cout, 2Hi, 2Wi]; shuffle != 0 folds
  *                       PixelShuffle(2) into the load (Hi, Wi are the conv-input = shuffled sizes)
  *   lpb_plane_softmax_f32  in-place spatial softmax (T = 1) of [n_planes, hw]

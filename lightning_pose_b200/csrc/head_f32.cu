@@ -1,116 +1,209 @@
-// fp32 heatmap head: PixelShuffle(2) -> ConvTranspose2d(k3,s2,p1,op1) [x2] -> spatial softmax (T=1).
+// fp32 heatmap head: PixelShuffle(2) -> ConvTranspose2d(k3,s2,p1,op1) [x n] -> spatial softmax (T=1).
 // Reference: lightning_pose/models/heads/heatmap.py:20-71 (layer stack), :203-212 (forward).
 //
-// This is the full-precision path (reference training is fp32, lightning_pose/train.py:411-428):
-// CUDA-core FMA with fp32 accumulation, gather-form transposed convolution (each thread owns one
-// input pixel and produces its 2x2 output quad for a group of output channels, so there is no
-// scatter / atomics), PixelShuffle folded into the shared-memory staging of the first layer.
-// The bf16 tensor-core path lives in head_bf16.cu.
+// This is the full-precision path (reference training is fp32, lightning_pose/train.py:411-428).  Every convolution,
+// forward and both gradients, is a GEMM on the tensor cores in 3xTF32 (mma_sm90.cuh: each operand split into a tf32
+// big part and a tf32 residual, three mma.sync m16n8k8 per product, fp32 accumulate), which keeps fp32 accuracy;
+// 1xTF32 would not (its relative error is ~1e-3 at these K).  PixelShuffle is folded into the staging of the first
+// layer's input and its inverse into the store of the data gradient.  The bf16 tensor-core path lives in head_bf16.cu.
+//
+// Pixel blocks.  Every kernel works on blocks of at most 128 conv-input pixels of one frame: RB rows x CB columns,
+// RB = 128 / CB, with CB = ceil(Wi / k) for the k in 1..8 that fills the most slots (pixel slot p = (p / CB, p % CB);
+// slots outside the frame are masked).  So the shared-memory tiles are bounded for any Hi, Wi, Cin and Cout.
+#include <algorithm>
 #include <cstdint>
 
 #include "../../include/lpb200.h"
 #include "lpb_common.cuh"
+#include "mma_sm90.cuh"
 
 namespace lpb {
 
-constexpr int CT_CC = 8;        // input channels staged per iteration
-constexpr int CT_OG = 5;        // groups of 4 output channels per pass (20 >= 17 keypoints)
-constexpr int CT_KO = 4 * CT_OG;
-constexpr int CT_MAX_THREADS = 256;
+constexpr int TC_SLOTS = 128;    // pixel slots per block
+constexpr int TC_THREADS = 128;  // forward / data gradient: 4 warps x 32 pixel slots (two m16 tiles each)
+constexpr int FW_CC = 24;        // forward: input channels staged per pass (three k8 steps; a 17-keypoint input in one)
 
+struct PixBlocks {
+  int RB, CB, n;  // rows, columns per block; blocks per frame
+};
+static PixBlocks pix_blocks(int Hi, int Wi) {
+  PixBlocks best{0, 0, 0};
+  for (int k = (Wi + TC_SLOTS - 1) / TC_SLOTS; k <= std::max(8, (Wi + TC_SLOTS - 1) / TC_SLOTS); ++k) {
+    const int CB = (Wi + k - 1) / k, RB = TC_SLOTS / CB;
+    const int n = ((Hi + RB - 1) / RB) * ((Wi + CB - 1) / CB);
+    if (best.n == 0 || n < best.n) best = {RB, CB, n};  // fewest blocks = most slots filled
+  }
+  return best;
+}
+// a plane stride = 8 (mod 32) floats: the fragment pattern (g + 8 t) of a [k][m] operand falls on 32 distinct banks
+__host__ __device__ __forceinline__ int pad8_32(int n) { return ((n + 31) & ~31) + 8; }
+// n-stride of a pre-split [k][n] B operand (8 NT columns): = 8 or 24 (mod 32), so (g + t * stride) hits 32 banks
+template <int NT>
+__host__ __device__ constexpr int bstride() {
+  return (NT * 8) % 32 == 8 || (NT * 8) % 32 == 24 ? NT * 8 : NT * 8 + 8;
+}
+
+// Shared-memory staging with several global loads in flight per thread (a stage is latency-bound otherwise).
+// stage_rows: rows x cols elements, one warp per row and lanes along it, U rows per warp at a time.
+template <int U, typename Src, typename Dst>
+__device__ __forceinline__ void stage_rows(int rows, int cols, Src src, Dst dst) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int j = lane; j - lane < cols; j += 32)
+    for (int r0 = warp; r0 < rows; r0 += nw * U) {
+      float v[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int r = r0 + u * nw;
+        v[u] = (r < rows && j < cols) ? src(r, j) : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int r = r0 + u * nw;
+        if (r < rows && j < cols) dst(r, j, v[u]);
+      }
+    }
+}
+// stage_flat: n elements, U per thread at a time
+template <int U, typename Src, typename Dst>
+__device__ __forceinline__ void stage_flat(int n, Src src, Dst dst) {
+  for (int i0 = threadIdx.x; i0 < n; i0 += U * blockDim.x) {
+    float v[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int i = i0 + u * blockDim.x;
+      v[u] = i < n ? src(i) : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int i = i0 + u * blockDim.x;
+      if (i < n) dst(i, v[u]);
+    }
+  }
+}
+
+// x / d for 0 <= x, d < 2^16 without a division: (x * ceil(2^32 / d)) >> 32 is exact there (d = 1: no multiplier fits)
+struct FastDiv {
+  uint32_t m;
+  int d;
+  __device__ __forceinline__ explicit FastDiv(int d_) : m(d_ > 1 ? (uint32_t)((0x100000000ull + d_ - 1) / d_) : 0u), d(d_) {}
+  __device__ __forceinline__ int div(int x) const { return d > 1 ? (int)__umulhi((uint32_t)x, m) : x; }
+};
+
+// ---- forward ------------------------------------------------------------------------------------------------------
 // out[o, 2m+py, 2n+px] = bias[o] + sum_c sum_taps in[c, m+dm, n+dn] * Wt[c, o, ky, kx]
 //   py=0: (dm,ky)=(0,1);  py=1: (0,2),(1,0)     (y = 2*iy - 1 + ky), same along x.
 // SHUFFLE: in[c, m, n] = feat[4c + 2(m&1) + (n&1), m>>1, n>>1]   (PixelShuffle(2))
-template <bool SHUFFLE>
-__global__ void __launch_bounds__(CT_MAX_THREADS) convt3x3s2_kernel(const float* __restrict__ in, int Cin, int Hi, int Wi,
-                                                                    const float* __restrict__ wt,
-                                                                    const float* __restrict__ bias, int Cout, int TR,
-                                                                    float* __restrict__ out) {
-  // Hi, Wi: spatial size of the (shuffled) conv input; output is (Cout, 2Hi, 2Wi)
+// Each output parity class q = 2 py + px is a GEMM: M = pixels of the block, N = Cout (8 NT per CTA), K = Cin per
+// (shift, tap) pair; the 9 pairs below share four shifted A operands, which are constant offsets into the staged tile
+// (RB + 1 rows x CB + 1 columns, zero halo).
+__device__ constexpr int kFwdShift[9] = {0, 0, 0, 0, 1, 1, 2, 2, 3};  // shift s = 2 dm + dn
+__device__ constexpr int kFwdClass[9] = {0, 1, 2, 3, 1, 3, 2, 3, 3};  // output parity q = 2 py + px
+__device__ constexpr int kFwdTap[9] = {4, 5, 7, 8, 3, 6, 1, 2, 0};    // ky * 3 + kx
+
+template <bool SHUFFLE, int NT>
+__global__ void __launch_bounds__(TC_THREADS) convt3x3s2_kernel(const float* __restrict__ in, int Cin, int Hi, int Wi,
+                                                                const float* __restrict__ wt, const float* __restrict__ bias,
+                                                                int Cout, int RB, int CB, float* __restrict__ out) {
+  constexpr int S = bstride<NT>();
   extern __shared__ __align__(16) float sm[];
-  const int xs_row = Wi + 1;
-  const int xs_plane = (TR + 1) * xs_row;
-  float* xs = sm;                                   // [CT_CC][TR+1][Wi+1]
-  float* ws = sm + ((CT_CC * xs_plane + 3) & ~3);   // [CT_CC][CT_KO*9], 16-B aligned rows (180 floats)
-  const int tiles_per_img = (Hi + TR - 1) / TR;
-  const int b = blockIdx.x / tiles_per_img;
-  const int m0 = (blockIdx.x - b * tiles_per_img) * TR;
-  const int o0 = blockIdx.y * CT_KO;
-  const int nquad = TR * Wi;
-  const int q = threadIdx.x;
-  const int qm = q / Wi, qn = q - qm * Wi;
-  const bool active = (q < nquad) && (m0 + qm < Hi);
+  const int XR = CB + 1, XP = pad8_32((RB + 1) * XR);
+  float* xs = sm;                                                // [FW_CC][XP]: rows r0 .. r0+RB, cols n0 .. n0+CB
+  uint32_t* wb = reinterpret_cast<uint32_t*>(sm + FW_CC * XP);  // [9][FW_CC][S] tf32 big
+  uint32_t* wsm = wb + 9 * FW_CC * S;                            // [9][FW_CC][S] tf32 small
+  const int nbc = (Wi + CB - 1) / CB, nblk = ((Hi + RB - 1) / RB) * nbc;
+  const int b = blockIdx.x / nblk, blk = blockIdx.x - b * nblk;
+  const int r0 = (blk / nbc) * RB, n0 = (blk - (blk / nbc) * nbc) * CB;
+  const int o0 = blockIdx.y * (8 * NT);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 
-  float acc[CT_KO][4];
+  int off[2][2];  // staged offset of this lane's A rows (slots g, g + 8 of each m16 tile); 0 for masked slots
 #pragma unroll
-  for (int o = 0; o < CT_KO; ++o) acc[o][0] = acc[o][1] = acc[o][2] = acc[o][3] = 0.f;
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int p = warp * 32 + mt * 16 + h * 8 + g, pr = p / CB, pc = p - pr * CB;
+      off[mt][h] = (p < RB * CB && r0 + pr < Hi && n0 + pc < Wi) ? pr * XR + pc : 0;
+    }
+  float acc[2][4][NT][4];
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt) mma::zero(acc[mt]);
 
-  const size_t in_img = SHUFFLE ? (size_t)b * (4 * Cin) * (Hi / 2) * (Wi / 2) : (size_t)b * Cin * Hi * Wi;
-  for (int c0 = 0; c0 < Cin; c0 += CT_CC) {
+  const size_t in_img = (size_t)b * Cin * Hi * Wi;  // = b * 4Cin * (Hi/2) * (Wi/2) with SHUFFLE
+  const FastDiv rdiv(RB + 1);
+  for (int c0 = 0; c0 < Cin; c0 += FW_CC) {
     __syncthreads();
-    // ---- stage inputs (rows m0 .. m0+TR, cols 0 .. Wi; zero halo) ----
-    for (int i = threadIdx.x; i < CT_CC * xs_plane; i += blockDim.x) {
-      const int cc = i / xs_plane, r = (i - cc * xs_plane) / xs_row, n = i - cc * xs_plane - r * xs_row;
-      const int c = c0 + cc, m = m0 + r;
-      float v = 0.f;
-      if (c < Cin && m < Hi && n < Wi) {
-        if (SHUFFLE) {
-          const int ch = 4 * c + 2 * (m & 1) + (n & 1);
-          v = __ldg(in + in_img + ((size_t)ch * (Hi / 2) + (m >> 1)) * (Wi / 2) + (n >> 1));
-        } else {
-          v = __ldg(in + in_img + ((size_t)c * Hi + m) * Wi + n);
+    stage_rows<4>(
+        FW_CC * (RB + 1), XR,
+        [&](int cr, int j) {
+          const int cc = rdiv.div(cr), c = c0 + cc, m = r0 + cr - cc * (RB + 1), n = n0 + j;
+          if (c >= Cin || m >= Hi || n >= Wi) return 0.f;
+          if (SHUFFLE) return __ldg(in + in_img + ((size_t)(4 * c + 2 * (m & 1) + (n & 1)) * (Hi / 2) + (m >> 1)) * (Wi / 2) + (n >> 1));
+          return __ldg(in + in_img + ((size_t)c * Hi + m) * Wi + n);
+        },
+        [&](int cr, int j, float v) {
+          const int cc = rdiv.div(cr);
+          xs[cc * XP + (cr - cc * (RB + 1)) * XR + j] = v;
+        });
+    stage_flat<8>(  // weights, global order (c, o, tap) -> [tap][c][o]
+        FW_CC * 8 * NT * 9,
+        [&](int i) {
+          const int tap = i % 9, co = i / 9, ol = co % (8 * NT), cc = co / (8 * NT), c = c0 + cc, o = o0 + ol;
+          return (c < Cin && o < Cout) ? __ldg(wt + ((size_t)c * Cout + o) * 9 + tap) : 0.f;
+        },
+        [&](int i, float v) {
+          const int tap = i % 9, co = i / 9, ol = co % (8 * NT), cc = co / (8 * NT);
+          mma::split_tf32(v, wb[(tap * FW_CC + cc) * S + ol], wsm[(tap * FW_CC + cc) * S + ol]);
+        });
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < FW_CC / 8; ++kk) {
+      if (c0 + 8 * kk >= Cin) break;  // an all-zero k8 step (narrow inputs: a second layer's Cin is a keypoint count)
+      const float* xk = xs + (kk * 8 + t) * XP;
+      uint32_t ab[2][4], as[2][4];
+#pragma unroll
+      for (int pi = 0; pi < 9; ++pi) {
+        const int s = kFwdShift[pi], q = kFwdClass[pi], tap = kFwdTap[pi];
+        if (pi == 0 || pi == 4 || pi == 6 || pi == 8) {  // a new shift: its A fragments
+          const int so = (s >> 1) * XR + (s & 1);
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            mma::split_tf32(xk[off[mt][0] + so], ab[mt][0], as[mt][0]);
+            mma::split_tf32(xk[off[mt][1] + so], ab[mt][1], as[mt][1]);
+            mma::split_tf32(xk[4 * XP + off[mt][0] + so], ab[mt][2], as[mt][2]);
+            mma::split_tf32(xk[4 * XP + off[mt][1] + so], ab[mt][3], as[mt][3]);
+          }
         }
-      }
-      xs[i] = v;
-    }
-    // ---- stage weights for output channels o0 .. o0+CT_KO ----
-    for (int i = threadIdx.x; i < CT_CC * CT_KO * 9; i += blockDim.x) {
-      const int cc = i / (CT_KO * 9), r = i - cc * (CT_KO * 9);
-      const int o = o0 + r / 9, c = c0 + cc;
-      ws[i] = (c < Cin && o < Cout) ? __ldg(wt + ((size_t)c * Cout + o) * 9 + (r % 9)) : 0.f;
-    }
-    __syncthreads();
-    if (active) {
-#pragma unroll 2
-      for (int cc = 0; cc < CT_CC; ++cc) {
-        const float* xp = xs + cc * xs_plane + qm * xs_row + qn;
-        const float x00 = xp[0], x01 = xp[1], x10 = xp[xs_row], x11 = xp[xs_row + 1];
-        const float4* w4 = reinterpret_cast<const float4*>(ws + cc * (CT_KO * 9));
+        const int wo = (tap * FW_CC + kk * 8 + t) * S + g;
 #pragma unroll
-        for (int g = 0; g < CT_OG; ++g) {
-          float w[36];
+        for (int nt = 0; nt < NT; ++nt) {
+          const uint32_t bb0 = wb[wo + nt * 8], bb1 = wb[wo + 4 * S + nt * 8];
+          const uint32_t bs0 = wsm[wo + nt * 8], bs1 = wsm[wo + 4 * S + nt * 8];
 #pragma unroll
-          for (int k = 0; k < 9; ++k) {
-            const float4 t = w4[g * 9 + k];
-            w[4 * k] = t.x;
-            w[4 * k + 1] = t.y;
-            w[4 * k + 2] = t.z;
-            w[4 * k + 3] = t.w;
-          }
-#pragma unroll
-          for (int oo = 0; oo < 4; ++oo) {
-            const float* k9 = w + oo * 9;  // [ky][kx]
-            float* a = acc[g * 4 + oo];
-            a[0] = fmaf(x00, k9[4], a[0]);                                                      // (even, even)
-            a[1] = fmaf(x00, k9[5], fmaf(x01, k9[3], a[1]));                                    // (even, odd)
-            a[2] = fmaf(x00, k9[7], fmaf(x10, k9[1], a[2]));                                    // (odd, even)
-            a[3] = fmaf(x00, k9[8], fmaf(x01, k9[6], fmaf(x10, k9[2], fmaf(x11, k9[0], a[3]))));  // (odd, odd)
-          }
+          for (int mt = 0; mt < 2; ++mt) mma::mma_3xtf32(acc[mt][q][nt], ab[mt], as[mt], bb0, bb1, bs0, bs1);
         }
       }
     }
   }
-  if (!active) return;
+  // c (g [+8], 2t + j): the two x parities of one (pixel, channel, row parity) are one float2 of the output row
   const int Ho = 2 * Hi, Wo = 2 * Wi;
-  const int y = 2 * (m0 + qm), x = 2 * qn;
 #pragma unroll
-  for (int o = 0; o < CT_KO; ++o) {
-    if (o0 + o >= Cout) break;
-    const float bv = bias ? __ldg(bias + o0 + o) : 0.f;
-    float* dst = out + (((size_t)b * Cout + o0 + o) * Ho + y) * Wo + x;
-    *reinterpret_cast<float2*>(dst) = make_float2(acc[o][0] + bv, acc[o][1] + bv);
-    *reinterpret_cast<float2*>(dst + Wo) = make_float2(acc[o][2] + bv, acc[o][3] + bv);
-  }
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int p = warp * 32 + mt * 16 + h * 8 + g, pr = p / CB, pc = p - pr * CB, m = r0 + pr, n = n0 + pc;
+      if (p >= RB * CB || m >= Hi || n >= Wi) continue;
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int o = o0 + nt * 8 + 2 * t + j;
+          if (o >= Cout) continue;
+          const float bv = bias ? __ldg(bias + o) : 0.f;
+          float* dst = out + (((size_t)b * Cout + o) * Ho + 2 * m) * Wo + 2 * n;
+          *reinterpret_cast<float2*>(dst) = make_float2(acc[mt][0][nt][2 * h + j] + bv, acc[mt][1][nt][2 * h + j] + bv);
+          *reinterpret_cast<float2*>(dst + Wo) = make_float2(acc[mt][2][nt][2 * h + j] + bv, acc[mt][3][nt][2 * h + j] + bv);
+        }
+    }
 }
 
 // in-place softmax over each (b, k) plane: one HBM read + one write (plane staged in smem)
@@ -147,139 +240,311 @@ __global__ void __launch_bounds__(256) plane_softmax_kernel(float* __restrict__ 
   for (int i = threadIdx.x; i < hw; i += 256) p[i] = pl[i] * inv;
 }
 
-static int launch_convt(bool shuffle, const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias,
-                        int Cout, float* out, cudaStream_t s) {
-  int TR = CT_MAX_THREADS / Wi;
-  LPB_REQUIRE(TR >= 1, "head: conv input width %d > %d unsupported", Wi, CT_MAX_THREADS);
-  if (TR > Hi) TR = Hi;
-  const int threads = ((TR * Wi + 31) / 32) * 32;
-  const int tiles = (Hi + TR - 1) / TR;
-  const size_t smem = (size_t)(((CT_CC * (TR + 1) * (Wi + 1) + 3) & ~3) + CT_CC * CT_KO * 9) * sizeof(float);
-  dim3 grid((unsigned)(B * tiles), (unsigned)((Cout + CT_KO - 1) / CT_KO));
-  if (shuffle)
-    convt3x3s2_kernel<true><<<grid, threads, smem, s>>>(in, Cin, Hi, Wi, wt, bias, Cout, TR, out);
-  else
-    convt3x3s2_kernel<false><<<grid, threads, smem, s>>>(in, Cin, Hi, Wi, wt, bias, Cout, TR, out);
+
+template <bool SHUFFLE, int NT>
+static int launch_fwd_nt(const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias, int Cout, float* out,
+                          cudaStream_t s) {
+  const PixBlocks pb = pix_blocks(Hi, Wi);
+  const size_t smem = ((size_t)FW_CC * pad8_32((pb.RB + 1) * (pb.CB + 1)) + 2 * 9 * FW_CC * bstride<NT>()) * sizeof(float);
+  LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_kernel<SHUFFLE, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const dim3 grid((unsigned)((size_t)B * pb.n), (unsigned)((Cout + 8 * NT - 1) / (8 * NT)));
+  convt3x3s2_kernel<SHUFFLE, NT><<<grid, TC_THREADS, smem, s>>>(in, Cin, Hi, Wi, wt, bias, Cout, pb.RB, pb.CB, out);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
 
-// ---- backward of one transposed convolution (fp32, CUDA cores) --------------------------------------
+template <bool SHUFFLE>
+static int launch_fwd(const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias, int Cout, float* out,
+                      cudaStream_t s) {
+  // N tile = Cout rounded up to 8, at most 24 channels (wider heads: more CTAs along y)
+  if (Cout <= 8) return launch_fwd_nt<SHUFFLE, 1>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
+  if (Cout <= 16) return launch_fwd_nt<SHUFFLE, 2>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
+  return launch_fwd_nt<SHUFFLE, 3>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
+}
+
+static int launch_convt(bool shuffle, const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias,
+                        int Cout, float* out, cudaStream_t s) {
+  return shuffle ? launch_fwd<true>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s)
+                 : launch_fwd<false>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
+}
+
+// ---- backward of one transposed convolution -----------------------------------------------------------------------
 // In scatter form input pixel (m, n) feeds output pixel (2m - 1 + ky, 2n - 1 + kx), so
 //   d in[c, m, n]      = sum_o sum_{ky,kx} g[o, 2m-1+ky, 2n-1+kx] * W[c, o, ky, kx]           (data gradient)
 //   d W[c, o, ky, kx]  = sum_{b, m, n} in[c, m, n] * g[o, 2m-1+ky, 2n-1+kx]                   (weight gradient)
 //   d bias[o]          = sum g[o]  (= the taps (1..2, 1..2), which partition the output pixels)
-// Both kernels stage the gradient tile of a band of input rows (output rows 2m0-1 .. 2(m0+TR)-1, all Cout planes)
-// in shared memory.  SHUFFLE folds PixelShuffle(2) (and its inverse for d in) into the addressing.
-constexpr int CB_CG = 32;  // input channels per CTA (data gradient)
-constexpr int CB_WC = 8;   // input channels per CTA (weight gradient)
-
-__device__ __forceinline__ void stage_grad_tile(const float* __restrict__ g, int b, int Cout, int Hi, int Wi, int m0, int TR,
-                                                float* __restrict__ gs) {
-  const int Ho = 2 * Hi, Wo = 2 * Wi, gr = 2 * TR + 1, gc = 2 * Wi + 1;
-  for (int i = threadIdx.x; i < Cout * gr * gc; i += blockDim.x) {
-    const int o = i / (gr * gc), r = (i - o * gr * gc) / gc, cidx = i - o * gr * gc - r * gc;
-    const int y = 2 * m0 - 1 + r, x = cidx - 1;
-    gs[i] = (y >= 0 && y < Ho && x >= 0) ? __ldg(g + (((size_t)b * Cout + o) * Ho + y) * Wo + x) : 0.f;
-  }
+// Both kernels stage, per output channel, the gradient tile of a pixel block: output rows 2 r0 - 1 .. 2 (r0 + RB) - 1
+// (GR = 2 RB + 1) and columns 2 n0 - 1 .. 2 (n0 + CB) - 1 (GC = 2 CB + 1), zero outside the map.  A row is stored with
+// its even columns first (CB + 1 of them) and its odd columns after, so the taps of consecutive pixels are
+// consecutive words: tap (ky, kx) of pixel slot (pr, pc) sits at  2 pr GC + pc + ky GC + (kx == 1 ? CB + 1 : kx / 2).
+__device__ __forceinline__ int grad_tap_offset(int tap, int GC, int CB) {
+  const int ky = tap / 3, kx = tap - 3 * (tap / 3);
+  return ky * GC + (kx == 1 ? CB + 1 : kx >> 1);
 }
 
-template <bool SHUFFLE>
-__global__ void __launch_bounds__(CT_MAX_THREADS) convt3x3s2_dgrad_kernel(const float* __restrict__ g, int Cout, int Hi, int Wi,
-                                                                          const float* __restrict__ wt, int Cin, int TR,
-                                                                          float* __restrict__ din) {
+__device__ __forceinline__ void stage_grad_planes(const float* __restrict__ g, int b, int Cout, int Hi, int Wi, int o0, int np, int r0,
+                                                  int n0, int RB, int CB, int GP, float* __restrict__ gs) {
+  const int Ho = 2 * Hi, Wo = 2 * Wi, GR = 2 * RB + 1, GC = 2 * CB + 1;
+  const FastDiv rdiv(GR);
+  stage_rows<4>(
+      np * GR, GC,
+      [&](int orow, int j) {
+        const int ol = rdiv.div(orow), o = o0 + ol, y = 2 * r0 - 1 + orow - ol * GR, x = 2 * n0 - 1 + j;
+        return (o < Cout && y >= 0 && y < Ho && x >= 0 && x < Wo) ? __ldg(g + (((size_t)b * Cout + o) * Ho + y) * Wo + x) : 0.f;
+      },
+      [&](int orow, int j, float v) {
+        const int ol = rdiv.div(orow);
+        gs[ol * GP + (orow - ol * GR) * GC + ((j & 1) ? CB + 1 + (j >> 1) : (j >> 1))] = v;
+      });
+}
+
+// Data gradient: M = pixels of the block, N = Cin (8 NT per CTA), K = Cout x 9 in stages of 8 output channels
+// (72 = 9 k8 steps, k = o_local * 9 + tap; the weights [c][o][tap] are K-contiguous).
+template <bool SHUFFLE, int NT>
+__global__ void __launch_bounds__(TC_THREADS) convt3x3s2_dgrad_kernel(const float* __restrict__ g, int Cout, int Hi, int Wi,
+                                                                      const float* __restrict__ wt, int Cin, int RB, int CB,
+                                                                      float* __restrict__ din) {
+  constexpr int S = bstride<NT>();
   extern __shared__ __align__(16) float sm[];
-  const int gr = 2 * TR + 1, gc = 2 * Wi + 1;
-  float* gs = sm;                                        // [Cout][gr][gc]
-  float* ws = sm + ((Cout * gr * gc + 3) & ~3);          // [Cout*9][CB_CG]
-  const int tiles = (Hi + TR - 1) / TR;
-  const int b = blockIdx.x / tiles, m0 = (blockIdx.x - b * tiles) * TR, c0 = blockIdx.y * CB_CG;
-  stage_grad_tile(g, b, Cout, Hi, Wi, m0, TR, gs);
-  for (int i = threadIdx.x; i < Cout * 9 * CB_CG; i += blockDim.x) {
-    const int cc = i % CB_CG, ot = i / CB_CG;  // ot = o*9 + tap
-    ws[i] = (c0 + cc < Cin) ? __ldg(wt + (size_t)(c0 + cc) * Cout * 9 + ot) : 0.f;
-  }
-  __syncthreads();
-  const int q = threadIdx.x, qm = q / Wi, qn = q - qm * Wi;
-  if (q >= TR * Wi || m0 + qm >= Hi) return;
-  const int m = m0 + qm;
-  for (int cg = 0; cg < CB_CG; cg += 4) {
-    if (c0 + cg >= Cin) break;
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-    for (int o = 0; o < Cout; ++o) {
-      const float* gp = gs + (o * gr + 2 * qm) * gc + 2 * qn;
+  const int GC = 2 * CB + 1, GP = pad8_32((2 * RB + 1) * GC);
+  float* gs = sm;                                               // [8][GP]
+  uint32_t* wb = reinterpret_cast<uint32_t*>(sm + 8 * GP);     // [72][S] tf32 big
+  uint32_t* wsm = wb + 72 * S;                                  // [72][S] tf32 small
+  const int nbc = (Wi + CB - 1) / CB, nblk = ((Hi + RB - 1) / RB) * nbc;
+  const int b = blockIdx.x / nblk, blk = blockIdx.x - b * nblk;
+  const int r0 = (blk / nbc) * RB, n0 = (blk - (blk / nbc) * nbc) * CB;
+  const int c0 = blockIdx.y * (8 * NT);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g8 = lane >> 2, t = lane & 3;
+
+  int pbase[2][2];  // this lane's A rows: 2 pr GC + pc (0 for masked slots, whose results are never stored)
 #pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const float gv = gp[(t / 3) * gc + (t % 3)];
-        const float4 w = *reinterpret_cast<const float4*>(ws + (o * 9 + t) * CB_CG + cg);
-        a0 = fmaf(gv, w.x, a0);
-        a1 = fmaf(gv, w.y, a1);
-        a2 = fmaf(gv, w.z, a2);
-        a3 = fmaf(gv, w.w, a3);
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int p = warp * 32 + mt * 16 + h * 8 + g8, pr = p / CB, pc = p - pr * CB;
+      pbase[mt][h] = p < RB * CB ? 2 * pr * GC + pc : 0;
+    }
+  int koff[9][2];  // this lane's A columns k = 8 ks + t (+4) of a stage
+#pragma unroll
+  for (int ks = 0; ks < 9; ++ks)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int k = 8 * ks + t + 4 * h, ol = k / 9;
+      koff[ks][h] = ol * GP + grad_tap_offset(k - 9 * ol, GC, CB);
+    }
+  float acc[2][NT][4];
+  mma::zero(acc);
+
+  for (int o0 = 0; o0 < Cout; o0 += 8) {
+    __syncthreads();
+    stage_grad_planes(g, b, Cout, Hi, Wi, o0, 8, r0, n0, RB, CB, GP, gs);
+    stage_flat<8>(  // weights [c][o][tap]: K-contiguous per input channel -> [k][c]
+        8 * NT * 72,
+        [&](int i) {
+          const int k = i % 72, c = c0 + i / 72;
+          return (c < Cin && o0 + k / 9 < Cout) ? __ldg(wt + ((size_t)c * Cout + o0) * 9 + k) : 0.f;
+        },
+        [&](int i, float v) { mma::split_tf32(v, wb[(i % 72) * S + i / 72], wsm[(i % 72) * S + i / 72]); });
+    __syncthreads();
+    const int nks = min(9, ((Cout - o0) * 9 + 7) / 8);
+#pragma unroll
+    for (int ks = 0; ks < 9; ++ks) {
+      if (ks >= nks) break;
+      uint32_t ab[2][4], as[2][4];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        mma::split_tf32(gs[pbase[mt][0] + koff[ks][0]], ab[mt][0], as[mt][0]);
+        mma::split_tf32(gs[pbase[mt][1] + koff[ks][0]], ab[mt][1], as[mt][1]);
+        mma::split_tf32(gs[pbase[mt][0] + koff[ks][1]], ab[mt][2], as[mt][2]);
+        mma::split_tf32(gs[pbase[mt][1] + koff[ks][1]], ab[mt][3], as[mt][3]);
+      }
+      const int wo = (8 * ks + t) * S + g8;
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt) {
+        const uint32_t bb0 = wb[wo + nt * 8], bb1 = wb[wo + 4 * S + nt * 8];
+        const uint32_t bs0 = wsm[wo + nt * 8], bs1 = wsm[wo + 4 * S + nt * 8];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) mma::mma_3xtf32(acc[mt][nt], ab[mt], as[mt], bb0, bb1, bs0, bs1);
       }
     }
-    const float acc[4] = {a0, a1, a2, a3};
+  }
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int c = c0 + cg + k;
-      if (c >= Cin) break;
-      if (SHUFFLE)
-        din[(((size_t)b * 4 * Cin + 4 * c + 2 * (m & 1) + (qn & 1)) * (Hi / 2) + (m >> 1)) * (Wi / 2) + (qn >> 1)] = acc[k];
-      else
-        din[(((size_t)b * Cin + c) * Hi + m) * Wi + qn] = acc[k];
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int p = warp * 32 + mt * 16 + h * 8 + g8, pr = p / CB, pc = p - pr * CB, m = r0 + pr, n = n0 + pc;
+      if (p >= RB * CB || m >= Hi || n >= Wi) continue;
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int c = c0 + nt * 8 + 2 * t + j;
+          if (c >= Cin) continue;
+          const float v = acc[mt][nt][2 * h + j];
+          if (SHUFFLE)
+            din[(((size_t)b * 4 * Cin + 4 * c + 2 * (m & 1) + (n & 1)) * (Hi / 2) + (m >> 1)) * (Wi / 2) + (n >> 1)] = v;
+          else
+            din[(((size_t)b * Cin + c) * Hi + m) * Wi + n] = v;
+        }
+    }
+}
+
+// Weight gradient: M = Cin (32 WM per CTA), N = Cout x 9 (n = o * 9 + tap, 8 NT WN per CTA), K = pixels.  K is split
+// over gridDim.y CTAs, each looping over its share of the (frame, pixel block) units with the tile in registers; the
+// tile is added into grad_w with one float atomic per element.  A = the input [c][slot] (row stride 132 = 4 mod 32:
+// the (g, t) pattern on 32 banks), B = the staged gradient planes of the CTA's output channels.  The CTAs of the
+// first channel tile also sum the bias gradient (the four taps (1..2, 1..2)) of their channels.
+constexpr int WG_PS = TC_SLOTS + 4;
+
+template <bool SHUFFLE, int WM, int WN, int NT>
+__global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const float* __restrict__ in, const float* __restrict__ g,
+                                                                        int B, int Cin, int Cout, int Hi, int Wi, int RB, int CB,
+                                                                        float* __restrict__ dw, float* __restrict__ db) {
+  constexpr int CM = 32 * WM, CN = 8 * NT * WN, THREADS = 32 * WM * WN;
+  extern __shared__ __align__(16) float sm[];
+  const int GC = 2 * CB + 1, GP = pad8_32((2 * RB + 1) * GC);
+  const int nct = (Cin + CM - 1) / CM, ct = blockIdx.x % nct, c0 = ct * CM, n0 = (blockIdx.x / nct) * CN;
+  const int o_lo = n0 / 9, np = min(Cout, (n0 + CN - 1) / 9 + 1) - o_lo;
+  float* xs = sm;                                               // [CM][WG_PS]
+  float* gs = xs + CM * WG_PS;                                  // [np][GP]
+  int* pbt = reinterpret_cast<int*>(gs + np * GP);             // [TC_SLOTS]: slot -> 2 pr GC + pc
+  float* dbs = reinterpret_cast<float*>(pbt + TC_SLOTS);        // [np]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g8 = lane >> 2, t = lane & 3;
+  const int wm = warp % WM, wn = warp / WM;
+  const bool do_bias = db != nullptr && ct == 0;
+
+  for (int i = threadIdx.x; i < CM * WG_PS; i += THREADS) xs[i] = 0.f;  // slots past RB * CB stay zero
+  for (int p = threadIdx.x; p < TC_SLOTS; p += THREADS) pbt[p] = p < RB * CB ? 2 * (p / CB) * GC + p % CB : 0;
+  for (int i = threadIdx.x; i < np; i += THREADS) dbs[i] = 0.f;
+  int koff[NT];  // this lane's B column n = n0 + 8 (NT wn + nt) + g (clamped to plane 0 past Cout x 9: never stored)
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt) {
+    const int n = n0 + 8 * (NT * wn + nt) + g8, o = n / 9;
+    koff[nt] = n < Cout * 9 ? (o - o_lo) * GP + grad_tap_offset(n - 9 * o, GC, CB) : 0;
+  }
+  float acc[2][NT][4];
+  mma::zero(acc);
+
+  const int nbc = (Wi + CB - 1) / CB, nblk = ((Hi + RB - 1) / RB) * nbc;
+  const FastDiv rdiv(RB);
+  const long long units = (long long)B * nblk;
+  for (long long u = blockIdx.y; u < units; u += gridDim.y) {
+    const int b = (int)(u / nblk), blk = (int)(u - (long long)b * nblk);
+    const int r0 = (blk / nbc) * RB, q0 = (blk - (blk / nbc) * nbc) * CB;
+    __syncthreads();
+    stage_rows<4>(
+        CM * RB, CB,
+        [&](int cr, int pc) {
+          const int cc = rdiv.div(cr), c = c0 + cc, m = r0 + cr - cc * RB, n = q0 + pc;
+          if (c >= Cin || m >= Hi || n >= Wi) return 0.f;
+          if (SHUFFLE) return __ldg(in + (((size_t)b * 4 * Cin + 4 * c + 2 * (m & 1) + (n & 1)) * (Hi / 2) + (m >> 1)) * (Wi / 2) + (n >> 1));
+          return __ldg(in + (((size_t)b * Cin + c) * Hi + m) * Wi + n);
+        },
+        [&](int cr, int pc, float v) {
+          const int cc = rdiv.div(cr);
+          xs[cc * WG_PS + (cr - cc * RB) * CB + pc] = v;
+        });
+    stage_grad_planes(g, b, Cout, Hi, Wi, o_lo, np, r0, q0, RB, CB, GP, gs);
+    __syncthreads();
+    if (do_bias) {
+      const int hw = RB * CB;
+      for (int i = threadIdx.x; i < np * hw; i += THREADS) {
+        const int ol = i / hw, p = i - ol * hw, pr = p / CB, pc = p - pr * CB;
+        if (r0 + pr >= Hi || q0 + pc >= Wi) continue;
+        const float* gp = gs + ol * GP + pbt[p];
+        atomicAdd(dbs + ol, (gp[GC + CB + 1] + gp[GC + 1]) + (gp[2 * GC + CB + 1] + gp[2 * GC + 1]));  // taps 4, 5, 7, 8
+      }
+    }
+#pragma unroll 4
+    for (int ks = 0; ks < TC_SLOTS / 8; ++ks) {
+      uint32_t ab[2][4], as[2][4];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        const float* xa = xs + (32 * wm + 16 * mt + g8) * WG_PS + 8 * ks + t;
+        mma::split_tf32(xa[0], ab[mt][0], as[mt][0]);
+        mma::split_tf32(xa[8 * WG_PS], ab[mt][1], as[mt][1]);
+        mma::split_tf32(xa[4], ab[mt][2], as[mt][2]);
+        mma::split_tf32(xa[8 * WG_PS + 4], ab[mt][3], as[mt][3]);
+      }
+      const int p0 = pbt[8 * ks + t], p1 = pbt[8 * ks + t + 4];
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt) {
+        uint32_t bb0, bb1, bs0, bs1;
+        mma::split_tf32(gs[p0 + koff[nt]], bb0, bs0);
+        mma::split_tf32(gs[p1 + koff[nt]], bb1, bs1);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) mma::mma_3xtf32(acc[mt][nt], ab[mt], as[mt], bb0, bb1, bs0, bs1);
+      }
+    }
+  }
+  const int nk = Cout * 9;
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = c0 + 32 * wm + 16 * mt + 8 * h + g8;
+      if (c >= Cin) continue;
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int n = n0 + 8 * (NT * wn + nt) + 2 * t + j;
+          if (n < nk) atomicAdd(dw + (size_t)c * nk + n, acc[mt][nt][2 * h + j]);
+        }
+    }
+  if (do_bias) {
+    __syncthreads();
+    for (int ol = threadIdx.x; ol < np; ol += THREADS) {
+      const int o = o_lo + ol;
+      if (o * 9 >= n0) atomicAdd(db + o, dbs[ol]);  // channel o belongs to the n tile that holds its tap 0
     }
   }
 }
 
+template <bool SHUFFLE, int WM, int WN, int NT>
+static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cout, int Hi, int Wi, float* dw, float* db, cudaStream_t s) {
+  constexpr int CM = 32 * WM, CN = 8 * NT * WN;
+  const PixBlocks pb = pix_blocks(Hi, Wi);
+  const int nct = (Cin + CM - 1) / CM, nnt = (Cout * 9 + CN - 1) / CN;
+  const int np_max = CN / 9 + 2;
+  const size_t smem =
+      ((size_t)CM * WG_PS + (size_t)np_max * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1)) + TC_SLOTS + np_max) * sizeof(float);
+  LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // K split: about two CTAs per SM in all, each with as many units as that leaves (fewer atomics than one per unit)
+  int dev = 0, sms = 132;
+  LPB_CUDA(cudaGetDevice(&dev));
+  LPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const long long units = (long long)B * pb.n;
+  const long long ks = std::min<long long>(units, std::max<long long>(1, (2LL * sms + nct * nnt - 1) / (nct * nnt)));
+  const dim3 grid((unsigned)(nct * nnt), (unsigned)ks);
+  convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, dw, db);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
 template <bool SHUFFLE>
-__global__ void __launch_bounds__(CT_MAX_THREADS) convt3x3s2_wgrad_kernel(const float* __restrict__ in, const float* __restrict__ g,
-                                                                          int Cin, int Cout, int Hi, int Wi, int TR,
-                                                                          float* __restrict__ dw, float* __restrict__ db) {
-  extern __shared__ __align__(16) float sm[];
-  const int gr = 2 * TR + 1, gc = 2 * Wi + 1;
-  float* gs = sm;                                  // [Cout][gr][gc]
-  float* xs = sm + ((Cout * gr * gc + 3) & ~3);    // [TR*Wi][CB_WC]
-  const int tiles = (Hi + TR - 1) / TR;
-  const int b = blockIdx.x / tiles, m0 = (blockIdx.x - b * tiles) * TR, c0 = blockIdx.y * CB_WC;
-  stage_grad_tile(g, b, Cout, Hi, Wi, m0, TR, gs);
-  const int npix = TR * Wi;
-  for (int i = threadIdx.x; i < npix * CB_WC; i += blockDim.x) {
-    const int cc = i % CB_WC, pix = i / CB_WC, qm = pix / Wi, qn = pix - qm * Wi, c = c0 + cc, m = m0 + qm;
-    float v = 0.f;
-    if (c < Cin && m < Hi) {
-      if (SHUFFLE) v = __ldg(in + (((size_t)b * 4 * Cin + 4 * c + 2 * (m & 1) + (qn & 1)) * (Hi / 2) + (m >> 1)) * (Wi / 2) + (qn >> 1));
-      else v = __ldg(in + (((size_t)b * Cin + c) * Hi + m) * Wi + qn);
-    }
-    xs[i] = v;
-  }
-  __syncthreads();
-  const int ot = threadIdx.x;  // o*9 + tap
-  if (ot >= Cout * 9) return;
-  const int o = ot / 9, t = ot - o * 9;
-  const float* gp = gs + o * gr * gc + (t / 3) * gc + (t % 3);
-  float acc[CB_WC], gsum = 0.f;
-#pragma unroll
-  for (int k = 0; k < CB_WC; ++k) acc[k] = 0.f;
-  const int rows = min(TR, Hi - m0);
-  for (int qm = 0; qm < rows; ++qm)
-    for (int qn = 0; qn < Wi; ++qn) {
-      const float gv = gp[2 * qm * gc + 2 * qn];
-      gsum += gv;
-      const float4 x0 = *reinterpret_cast<const float4*>(xs + (qm * Wi + qn) * CB_WC);
-      const float4 x1 = *reinterpret_cast<const float4*>(xs + (qm * Wi + qn) * CB_WC + 4);
-      acc[0] = fmaf(gv, x0.x, acc[0]);
-      acc[1] = fmaf(gv, x0.y, acc[1]);
-      acc[2] = fmaf(gv, x0.z, acc[2]);
-      acc[3] = fmaf(gv, x0.w, acc[3]);
-      acc[4] = fmaf(gv, x1.x, acc[4]);
-      acc[5] = fmaf(gv, x1.y, acc[5]);
-      acc[6] = fmaf(gv, x1.z, acc[6]);
-      acc[7] = fmaf(gv, x1.w, acc[7]);
-    }
-#pragma unroll
-  for (int k = 0; k < CB_WC; ++k)
-    if (c0 + k < Cin && acc[k] != 0.f) atomicAdd(dw + (size_t)(c0 + k) * Cout * 9 + ot, acc[k]);
-  if (db && blockIdx.y == 0 && (t == 4 || t == 5 || t == 7 || t == 8) && gsum != 0.f) atomicAdd(db + o, gsum);
+static int launch_bwd(const float* in, const float* g, int B, int Cin, int Hi, int Wi, const float* wt, int Cout, float* din, float* dw,
+                      float* db, cudaStream_t s) {
+  // M tile: 128 input channels, or 32 for narrow inputs (a second layer's Cin is the first layer's keypoint count)
+  const int rc = Cin > 32 ? launch_wgrad<SHUFFLE, 4, 2, 10>(in, g, B, Cin, Cout, Hi, Wi, dw, db, s)
+                          : launch_wgrad<SHUFFLE, 1, 4, 5>(in, g, B, Cin, Cout, Hi, Wi, dw, db, s);
+  if (rc || !din) return rc;
+  const PixBlocks pb = pix_blocks(Hi, Wi);
+  const size_t gfl = (size_t)8 * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1));
+  auto go = [&](auto kernel, int nt, int stride) -> int {
+    const size_t smem = (gfl + (size_t)2 * 72 * stride) * sizeof(float);
+    LPB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const dim3 grid((unsigned)((size_t)B * pb.n), (unsigned)((Cin + 8 * nt - 1) / (8 * nt)));
+    kernel<<<grid, TC_THREADS, smem, s>>>(g, Cout, Hi, Wi, wt, Cin, pb.RB, pb.CB, din);
+    LPB_CUDA(cudaGetLastError());
+    return LPB_OK;
+  };
+  // N tile = Cin rounded up to 8, 16, 24, 32 or 64 channels
+  if (Cin <= 8) return go(convt3x3s2_dgrad_kernel<SHUFFLE, 1>, 1, bstride<1>());
+  if (Cin <= 16) return go(convt3x3s2_dgrad_kernel<SHUFFLE, 2>, 2, bstride<2>());
+  if (Cin <= 24) return go(convt3x3s2_dgrad_kernel<SHUFFLE, 3>, 3, bstride<3>());
+  if (Cin <= 32) return go(convt3x3s2_dgrad_kernel<SHUFFLE, 4>, 4, bstride<4>());
+  return go(convt3x3s2_dgrad_kernel<SHUFFLE, 8>, 8, bstride<8>());
 }
 
 }  // namespace lpb
@@ -310,42 +575,14 @@ extern "C" int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, 
                                  int Cout, float* grad_in, float* grad_w, float* grad_bias, void* stream) {
   using namespace lpb;
   LPB_REQUIRE(in && grad_out && w && grad_w, "convt_bwd_f32: null pointer");
-  LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Cout * 9 <= CT_MAX_THREADS && Hi >= 1 && Wi >= 1 && Wi <= CT_MAX_THREADS &&
-                  (!shuffle || (Hi % 2 == 0 && Wi % 2 == 0)),
-              "convt_bwd_f32: bad shape (Cout <= 28, Wi <= 256)");
+  LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Hi >= 1 && Wi >= 1 && (!shuffle || (Hi % 2 == 0 && Wi % 2 == 0)),
+              "convt_bwd_f32: bad shape");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   LPB_CUDA(cudaMemsetAsync(grad_w, 0, sizeof(float) * (size_t)Cin * Cout * 9, s));
   if (grad_bias) LPB_CUDA(cudaMemsetAsync(grad_bias, 0, sizeof(float) * Cout, s));
   if (B == 0) return LPB_OK;
-  int TR = CT_MAX_THREADS / Wi;
-  if (TR > Hi) TR = Hi;
-  // shrink the band until the staged gradient tile fits
-  auto tile_floats = [&](int tr) { return (size_t)((Cout * (2 * tr + 1) * (2 * Wi + 1) + 3) & ~3); };
-  while (TR > 1 && (tile_floats(TR) + (size_t)Cout * 9 * CB_CG) * sizeof(float) > 200 * 1024) --TR;
-  const int tiles = (Hi + TR - 1) / TR;
-  const size_t smem_w = (tile_floats(TR) + (size_t)TR * Wi * CB_WC) * sizeof(float);
-  const size_t smem_d = (tile_floats(TR) + (size_t)Cout * 9 * CB_CG) * sizeof(float);
-  LPB_REQUIRE(smem_w <= 220 * 1024 && smem_d <= 220 * 1024, "convt_bwd_f32: gradient tile too large (Wi = %d, Cout = %d)", Wi, Cout);
-  const int threads_w = ((max(Cout * 9, 32) + 31) / 32) * 32;
-  const int threads_d = ((TR * Wi + 31) / 32) * 32;
-  dim3 gw((unsigned)(B * tiles), (unsigned)((Cin + CB_WC - 1) / CB_WC)), gd((unsigned)(B * tiles), (unsigned)((Cin + CB_CG - 1) / CB_CG));
-  if (shuffle) {
-    LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));
-    convt3x3s2_wgrad_kernel<true><<<gw, threads_w, smem_w, s>>>(in, grad_out, Cin, Cout, Hi, Wi, TR, grad_w, grad_bias);
-    if (grad_in) {
-      LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_dgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_d));
-      convt3x3s2_dgrad_kernel<true><<<gd, threads_d, smem_d, s>>>(grad_out, Cout, Hi, Wi, w, Cin, TR, grad_in);
-    }
-  } else {
-    LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));
-    convt3x3s2_wgrad_kernel<false><<<gw, threads_w, smem_w, s>>>(in, grad_out, Cin, Cout, Hi, Wi, TR, grad_w, grad_bias);
-    if (grad_in) {
-      LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_dgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_d));
-      convt3x3s2_dgrad_kernel<false><<<gd, threads_d, smem_d, s>>>(grad_out, Cout, Hi, Wi, w, Cin, TR, grad_in);
-    }
-  }
-  LPB_CUDA(cudaGetLastError());
-  return LPB_OK;
+  return shuffle ? launch_bwd<true>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s)
+                 : launch_bwd<false>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s);
 }
 
 extern "C" int lpb_head_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {

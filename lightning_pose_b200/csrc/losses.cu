@@ -856,8 +856,9 @@ extern "C" int lpb_plane_softmax_bwd(const float* probs, const float* grad_probs
   if (n_planes == 0) return LPB_OK;
   const size_t smem = (size_t)2 * hw * sizeof(float);
   LPB_REQUIRE(smem <= 200 * 1024, "plane_softmax_bwd: plane of %d pixels too large", hw);
-  if (smem > 48 * 1024)
-    LPB_CUDA(cudaFuncSetAttribute(plane_softmax_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // opt in whatever the size: the kernel's static shared memory comes on top of the dynamic 2 * hw floats, so a
+  // plane of exactly 48 KiB (64 x 96 pixels) already needs it
+  LPB_CUDA(cudaFuncSetAttribute(plane_softmax_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   plane_softmax_bwd_kernel<<<(unsigned)n_planes, HL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(probs, grad_probs, hw,
                                                                                                       grad_logits);
   LPB_CUDA(cudaGetLastError());

@@ -29,6 +29,39 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// ---- 3xTF32 (fp32-accurate GEMMs on the tf32 tensor cores; the fp32 head, head_f32.cu) ----------------------------
+// x = big + small with big = tf32(x) and small = tf32(x - big); a*b ~ a_s*b_b + a_b*b_s + a_b*b_b (the small*small term
+// is below fp32 rounding), each product accumulated in fp32 by mma.sync m16n8k8.  Fragments (g = lane / 4, t = lane % 4):
+// a0 (g, t), a1 (g + 8, t), a2 (g, t + 4), a3 (g + 8, t + 4); b0 (k = t, n = g), b1 (k = t + 4, n = g); c as for bf16.
+__device__ __forceinline__ uint32_t tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return r & 0xffffe000u;
+}
+__device__ __forceinline__ void split_tf32(float x, uint32_t& big, uint32_t& small) {
+  big = tf32_rna(x);
+  small = tf32_rna(x - __uint_as_float(big));
+}
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// d += a * b for one k8 step.  The tensor cores' fp32 accumulation truncates, so a long-lived accumulator fed by
+// three MMAs per step drifts by up to an ulp of its own size per MMA (~2e-5 relative after K = 1152); the step's
+// products are summed in a fresh fragment (small products first) and added to d with a rounded FADD instead.
+__device__ __forceinline__ void mma_3xtf32(float (&d)[4], const uint32_t (&ab)[4], const uint32_t (&as)[4], uint32_t bb0, uint32_t bb1,
+                                           uint32_t bs0, uint32_t bs1) {
+  float p[4];
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%10,%10,%10};"
+               : "=f"(p[0]), "=f"(p[1]), "=f"(p[2]), "=f"(p[3])
+               : "r"(as[0]), "r"(as[1]), "r"(as[2]), "r"(as[3]), "r"(bb0), "r"(bb1), "f"(0.f));
+  mma_tf32(p, ab, bs0, bs1);
+  mma_tf32(p, ab, bb0, bb1);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) d[i] += p[i];
+}
+
 template <int MT, int NT>
 __device__ __forceinline__ void zero(float (&acc)[MT][NT][4]) {
 #pragma unroll

@@ -71,8 +71,8 @@ def _needs_grad(features: torch.Tensor, params) -> bool:
 class _HeadFunction(torch.autograd.Function):
     """Fused head, optionally with the soft-argmax decode riding along (``decode = (ds, temperature)``).
 
-    Forward: tensor-core head for bf16 features (one- or two-deconv heads inside the tensor-core tiling), the fp32
-    CUDA-core kernels otherwise (+ decode kernel).  Backward: native in both cases.  On the tensor-core path the gradient
+    Forward: bf16 tensor-core head for bf16 features (one- or two-deconv heads inside its tiling), the fp32 (3xTF32
+    tensor-core) kernels otherwise (+ decode kernel).  Backward: native in both cases.  On the tensor-core path the gradient
     w.r.t. the heatmaps is never materialised for the decode branch: the sparse decode windows, a dense heatmap-loss
     gradient if there is one, and the softmax backward are all folded into the kernel that writes the
     deconv-gradient operand.  Outputs: heatmaps [, keypoints (B, 2K), confidences (B, K)].

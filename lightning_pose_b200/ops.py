@@ -299,7 +299,7 @@ def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=
 
 # ---- fp32 precision path: one transposed convolution at a time (any number of layers), native backward ----------
 def convt_forward_f32(x, weight, bias, shuffle: bool):
-    """[PixelShuffle(2) +] ConvTranspose2d(k3, s2, p1, op1) in fp32 on CUDA cores."""
+    """[PixelShuffle(2) +] ConvTranspose2d(k3, s2, p1, op1) in fp32 (3xTF32 on the tensor cores); any Cin, Cout, size."""
     x = _cuda_f32(x, "input")
     wt = _cuda_f32(weight, "weight")
     bs = _cuda_f32(bias, "bias") if bias is not None else None
@@ -352,8 +352,9 @@ def head_forward_f32(features, weights, biases, final_softmax=True, keep_activat
 def head_forward(features, weights, biases, final_softmax=True):
     """PixelShuffle(2) + ConvTranspose2d stack + spatial softmax; forward only.
 
-    bf16 features take the tensor-core tensor-core kernels (fp32 accumulate, fp32 heatmaps) when the head is a one- or
-    two-deconv head the tiling covers; everything else takes the full-precision CUDA-core kernels.  Training uses
+    bf16 features take the bf16 tensor-core kernels (fp32 accumulate, fp32 heatmaps) when the head is a one- or
+    two-deconv head the tiling covers; everything else takes the full-precision kernels (3xTF32 on the tensor cores,
+    any depth and keypoint count).  Training uses
     ``HeatmapHead`` which adds the backward.
     """
     if not isinstance(features, torch.Tensor) or not features.is_cuda:

@@ -6,9 +6,8 @@ Timed per call with CUDA events, the L2 flushed before each call (a 256 MB write
   forward_decode   forward_with_keypoints without autograd (head + soft-argmax decode)
   train_backward   the training form's backward alone (forward_with_keypoints with autograd is set up untimed):
                    a dense heatmap-MSE-shaped gradient plus the decode's keypoint gradient (sparse windows on the bf16
-                   route).  On fp32 features the CUDA-core backward does not run at this shape (its plane-softmax
-                   backward fails at 768 x 51 planes, and lpb_convt_bwd_f32 serves at most 28 output channels per
-                   layer), so that entry records the error instead of a time.
+                   route; the dense decode backward on fp32 features).  An entry that fails records the error
+                   instead of a time.
 The card's name, power limit and SM clocks are read in the same call.  Usage:
     python scripts/bench_wide_head.py [out.json]
 """
@@ -82,7 +81,7 @@ def main():
         try:
             entry["tensor_core_backward"] = ops.head_bf16_supported(tuple(x.shape), [K, K], train=True) and x.dtype == torch.bfloat16
             entry["train_backward"] = timed(lambda st: torch.autograd.backward(list(st), [g_hm, g_kp]), setup)
-        except Exception as exc:  # noqa: BLE001  (recorded, not hidden: the fp32 route's limit)
+        except Exception as exc:  # noqa: BLE001  (recorded, not hidden)
             entry["train_backward"] = {"error": str(exc)[:200]}
         head.zero_grad(set_to_none=True)
         res[name] = entry
