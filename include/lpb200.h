@@ -164,6 +164,15 @@ int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const fl
  * otherwise, before anything is queued). */
 int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes);
 
+/* fp16 forward (inference under autocast(float16)): lpb_head_fwd_bf16 with fp16 features, the fp32 master weights and
+ * the bias that rides on the constant-one channel rounded to fp16 on device (round-to-nearest-even, subnormals kept,
+ * overflow to inf: torch's .half()), fp16 mid activations, fp32 accumulate, fp32 heatmaps.  Shapes, kernels and plan are
+ * those of the bf16 forward, and the layouts are identical with 2-byte elements: size it with lpb_head_bf16_plan,
+ * lpb_head_bf16_workspace_bytes and lpb_head_bf16_saved_bytes.  Same alignment rules.  There is no fp16 backward. */
+int lpb_head_fwd_f16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                     const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
+                     void* workspace, void* stream);
+
 /* backward of lpb_head_fwd_bf16 (replaces autograd through heatmap.py:203-212 and, fused into its front end,
  * through spatial_softmax2d :211 and run_subpixelmaxima :103-144).  Kernels: gradient front end (G2 writer),
  * layer-2 wgrad, layer-2 dgrad, layer-1 wgrad, layer-1 dgrad + inverse PixelShuffle (all tensor-core).
@@ -228,24 +237,29 @@ int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes, int ctx, 
  * replaces the tail of the DALI pipeline  lightning_pose/data/video/dali.py:157-197
  *   fn.resize -> / 255 -> fn.crop_mirror_normalize(output_layout="FCHW", mean, std)
  * frames_u8 [F, H, W, 3] decoded RGB (device) -> out [F, 3, out_h, out_w] (layout 0, the reference's FCHW) or
- * [F, out_h, out_w, 3] (layout 1, channels-last), fp32 or bf16 (out_bf16).  mean3 / std3: HOST arrays of three floats
- * in (0, 1) units (ImageNet statistics, dali.py:44-45).  Resize (when out size != input size): bilinear, half-pixel
- * centres, no antialiasing. */
+ * [F, out_h, out_w, 3] (layout 1, channels-last), in the element type of out_format: LPB_OUT_F32, LPB_OUT_BF16 or
+ * LPB_OUT_F16 (rounded to nearest even from the fp32 value, so bf16 / fp16 output is the fp32 output's .bfloat16() /
+ * .half() bit for bit); any other code is LPB_ERR_INVALID.  mean3 / std3: HOST arrays of three floats in (0, 1) units
+ * (ImageNet statistics, dali.py:44-45).  Resize (when out size != input size): bilinear, half-pixel centres, no
+ * antialiasing. */
+#define LPB_OUT_F32 0
+#define LPB_OUT_BF16 1
+#define LPB_OUT_F16 2
 int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* mean3,
-                         const float* std3, int layout, int out_bf16, void* out, void* stream);
+                         const float* std3, int layout, int out_format, void* out, void* stream);
 
 /* ---- multi-view video ingest: every camera's frames in one launch -----------------------------------------------
  * replaces the multi-view tail of the DALI pipeline  lightning_pose/data/video/dali.py:301-330  (one reader per view,
  * each through fn.resize -> / 255 -> fn.crop_mirror_normalize as in lpb_frames_normalize, then the views stacked into
  * (seq, V, 3, H, W)).  frames_u8: HOST array of V device pointers, view v [F, H[v], W[v], 3] decoded RGB; H, W: HOST
  * arrays of V ints (views may differ in size).  out [F, V, 3, out_h, out_w] (layout 0) or [F, V, out_h, out_w, 3]
- * (layout 1), fp32 or bf16 (out_bf16): reshaped to [F * V, ...] it is the frame-major, view-minor batch the multi-view
+ * (layout 1), in the element type of out_format (as for lpb_frames_normalize): reshaped to [F * V, ...] it is the frame-major, view-minor batch the multi-view
  * trackers read.  Every output image is bit-identical to lpb_frames_normalize on that view alone (a view already at
  * out_h x out_w is copied and normalised without resampling).  1 <= V <= LPB_INGEST_MAX_VIEWS, F * V < 2^31; the
  * output may pass 2^31 elements.  F = 0 is a no-op. */
 #define LPB_INGEST_MAX_VIEWS 16
 int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V, int F, const int* H, const int* W, int out_h,
-                               int out_w, const float* mean3, const float* std3, int layout, int out_bf16, void* out,
+                               int out_w, const float* mean3, const float* std3, int layout, int out_format, void* out,
                                void* stream);
 
 /* ---- augmented video ingest: the unlabeled branch's DALI augmentation ----------------------------------------
@@ -262,7 +276,7 @@ int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V, int F, co
  *   6. fn.noise.shot: Poisson(max(0, v / factor)) * factor, v when factor == 0; Philox4x32-10 keyed by *seed (DEVICE
  *      int64) and counted by (x, y, frame, channel): the noise does not depend on the launch shape;
  *   7. / 255 and mean3 / std3 (HOST arrays) to out, layout 0 [F, 3, out_h, out_w] or 1 [F, out_h, out_w, 3], fp32 or
- *      bf16 (out_bf16).
+ *      bf16 (out_bf16: LPB_OUT_F32 or LPB_OUT_BF16; this training-only entry refuses LPB_OUT_F16 with LPB_ERR_INVALID).
  * transform_out (DEVICE, 6 floats): M row-major [[a00, a01, t0], [a10, a11, t1]], the transform lpb_remap_keypoints
  * undoes.  Reading params and seed on the device lets draws made inside a captured graph take effect on replay.
  * F = 0 is a no-op. */
@@ -284,12 +298,13 @@ int lpb_frames_augment_normalize(const uint8_t* frames_u8, int F, int H, int W, 
  *               lpb_frames_normalize) on the way out;
  *   in_f32 = 1: frames fp32 [F, 3, H, W] already normalised (the reference function's own input); crop + resize only,
  *               mean3 / std3 ignored (may be NULL).
- * out: layout 0 [F, 3, out_h, out_w] or layout 1 [F, out_h, out_w, 3], fp32 or bf16 (out_bf16).
+ * out: layout 0 [F, 3, out_h, out_w] or layout 1 [F, out_h, out_w, 3], in the element type of out_format (as for
+ * lpb_frames_normalize).
  * boxes_out [F, 4]: the clamped boxes [x1, y1, y2 - y1, x2 - x1], the bbox that maps model coordinates back to the
  * frame (lpb_remap_keypoints).  F <= 65535. */
 int lpb_frames_crop_normalize(const void* frames, int in_f32, int F, int H, int W, const float* boxes, int64_t n_boxes,
                               const int64_t* cursor, int64_t row0, int out_h, int out_w, const float* mean3,
-                              const float* std3, int layout, int out_bf16, void* out, float* boxes_out, void* stream);
+                              const float* std3, int layout, int out_format, void* out, float* boxes_out, void* stream);
 
 /* replaces _calculate_bbox_size + _compute_bbox_df  lightning_pose/utils/cropzoom.py:31-143
  * keypoints: frame n, keypoint k at keypoints[n * row_stride + k * point_stride] (x) and + 1 (y): point_stride 2 reads

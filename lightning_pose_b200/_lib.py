@@ -57,6 +57,7 @@ SIGNATURES = {
     "lpb_head_bf16_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bf16_saved_bytes": (C.c_int, [_I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_fwd_bf16": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
+    "lpb_head_fwd_f16": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
     "lpb_head_bwd_bf16_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bwd_bf16": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_remap_keypoints": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),

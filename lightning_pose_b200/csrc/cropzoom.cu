@@ -59,7 +59,7 @@ __device__ __forceinline__ float load_px(const CropParams& P, int f, int c, int 
 }
 
 // grid (x-blocks, F): each block computes its frame's box, then strides over that frame's output pixels.
-template <bool IN_F32, int LAYOUT, bool BF16>
+template <bool IN_F32, int LAYOUT, int FMT>
 __global__ void __launch_bounds__(256) crop_kernel(const __grid_constant__ CropParams P) {
   const int f = blockIdx.y;
   int x1, y1, x2, y2;
@@ -92,17 +92,11 @@ __global__ void __launch_bounds__(256) crop_kernel(const __grid_constant__ CropP
     if (LAYOUT == 0) {  // FCHW
       const size_t o = (size_t)f * 3 * plane + i;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        if (BF16) static_cast<__nv_bfloat16*>(P.out)[o + c * plane] = __float2bfloat16_rn(v[c]);
-        else static_cast<float*>(P.out)[o + c * plane] = v[c];
-      }
+      for (int c = 0; c < 3; ++c) store_fmt<FMT>(P.out, o + c * plane, v[c]);
     } else {  // FHWC
       const size_t o = ((size_t)f * plane + i) * 3;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        if (BF16) static_cast<__nv_bfloat16*>(P.out)[o + c] = __float2bfloat16_rn(v[c]);
-        else static_cast<float*>(P.out)[o + c] = v[c];
-      }
+      for (int c = 0; c < 3; ++c) store_fmt<FMT>(P.out, o + c, v[c]);
     }
   }
 }
@@ -194,13 +188,14 @@ __global__ void __launch_bounds__(256) rolling_median_kernel(const float* __rest
 
 extern "C" int lpb_frames_crop_normalize(const void* frames, int in_f32, int F, int H, int W, const float* boxes,
                                          int64_t n_boxes, const int64_t* cursor, int64_t row0, int out_h, int out_w,
-                                         const float* mean3, const float* std3, int layout, int out_bf16, void* out,
+                                         const float* mean3, const float* std3, int layout, int out_format, void* out,
                                          float* boxes_out, void* stream) {
   using namespace lpb;
   LPB_REQUIRE(frames && boxes && out && boxes_out && (in_f32 || (mean3 && std3)), "frames_crop_normalize: null pointer");
   LPB_REQUIRE(F >= 0 && F <= 65535 && H >= 1 && W >= 1 && out_h >= 1 && out_w >= 1 && (int64_t)out_h * out_w < (1LL << 31) &&
                   n_boxes >= 1 && row0 >= 0 && (layout == 0 || layout == 1),
               "frames_crop_normalize: bad shape/layout");
+  LPB_REQUIRE(valid_out_format(out_format), "frames_crop_normalize: unknown output format %d", out_format);
   if (F == 0) return LPB_OK;
   CropParams p;
   p.in = frames, p.boxes = boxes, p.cursor = cursor, p.out = out, p.boxes_out = boxes_out;
@@ -216,17 +211,15 @@ extern "C" int lpb_frames_crop_normalize(const void* frames, int in_f32, int F, 
   const int64_t px_blocks = ((int64_t)out_h * out_w + 255) / 256;
   dim3 grid((unsigned)(px_blocks < 64 ? px_blocks : 64), (unsigned)F);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int key = (in_f32 ? 4 : 0) + layout * 2 + (out_bf16 ? 1 : 0);
-  switch (key) {
-    case 0: crop_kernel<false, 0, false><<<grid, 256, 0, s>>>(p); break;
-    case 1: crop_kernel<false, 0, true><<<grid, 256, 0, s>>>(p); break;
-    case 2: crop_kernel<false, 1, false><<<grid, 256, 0, s>>>(p); break;
-    case 3: crop_kernel<false, 1, true><<<grid, 256, 0, s>>>(p); break;
-    case 4: crop_kernel<true, 0, false><<<grid, 256, 0, s>>>(p); break;
-    case 5: crop_kernel<true, 0, true><<<grid, 256, 0, s>>>(p); break;
-    case 6: crop_kernel<true, 1, false><<<grid, 256, 0, s>>>(p); break;
-    default: crop_kernel<true, 1, true><<<grid, 256, 0, s>>>(p); break;
-  }
+  with_out_format(out_format, [&](auto fc) {
+    constexpr int FMT = decltype(fc)::value;
+    switch ((in_f32 ? 2 : 0) + layout) {
+      case 0: crop_kernel<false, 0, FMT><<<grid, 256, 0, s>>>(p); break;
+      case 1: crop_kernel<false, 1, FMT><<<grid, 256, 0, s>>>(p); break;
+      case 2: crop_kernel<true, 0, FMT><<<grid, 256, 0, s>>>(p); break;
+      default: crop_kernel<true, 1, FMT><<<grid, 256, 0, s>>>(p); break;
+    }
+  });
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

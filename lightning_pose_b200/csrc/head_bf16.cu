@@ -32,9 +32,10 @@
 namespace lpb {
 
 // ---- everything a head call prepares, in one launch (head_prep.cuh) -------------------------------------------
-// forward packs: W[Cin][Cout][3][3] (fp32) -> B[group][stage][shift][kchunk][80][8] bf16 (output channel
+// forward packs: W[Cin][Cout][3][3] (fp32) -> B[group][stage][shift][kchunk][80][8] of operand type T (output channel
 // o = HEAD_CLS * group + column % HEAD_CLS); a non-null bias rides on input channel `Cin` (the constant-one channel of the
-// mid activations; shift (0,0) only, which every output class uses once)
+// mid activations; shift (0,0) only, which every output class uses once) and is rounded to T like the weights
+template <typename T>
 __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ PrepJobs J) {
   const long long tid0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
 #pragma unroll
@@ -65,7 +66,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
       } else if (bias && c == Cin && o < Cout && sh == 0) {
         v = bias[o];
       }
-      J.fpack[j].out[i] = __float2bfloat16_rn(v);
+      static_cast<T*>(J.fpack[j].out)[i] = Operand<T>::from(v);
     }
   }
 #pragma unroll
@@ -112,7 +113,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
       if (e < L.lead) row = e;
       else if (e < L.lead + (L.rows - body1)) row = body1 + (e - L.lead);
       else row = body0 + (e - L.lead - (L.rows - body1)) * L.Pp + L.Wi;
-      *reinterpret_cast<uint4*>(J.pads[j].buf + ((size_t)slab * L.rows + row) * 8) = make_uint4(0, 0, 0, 0);
+      *reinterpret_cast<uint4*>(static_cast<unsigned char*>(J.pads[j].buf) + ((size_t)slab * L.rows + row) * 16) = make_uint4(0, 0, 0, 0);
     }
   }
 #pragma unroll
@@ -122,10 +123,13 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
   }
 }
 
+template <typename T>
 int launch_head_prep(const PrepJobs& jobs, cudaStream_t s) {
-  head_prep_kernel<<<132 * 2, 256, 0, s>>>(jobs);  // two CTAs per SM of an H100 SXM
+  head_prep_kernel<T><<<132 * 2, 256, 0, s>>>(jobs);  // two CTAs per SM of an H100 SXM
   return LPB_OK;
 }
+template int launch_head_prep<__nv_bfloat16>(const PrepJobs&, cudaStream_t);
+template int launch_head_prep<__half>(const PrepJobs&, cudaStream_t);
 
 // =====================================================================================================
 // k1a: PixelShuffle + first transposed convolution
@@ -194,12 +198,14 @@ __host__ inline K1aGeom make_k1a_geom(int H, int W) {
   return k;
 }
 
+// T: the operand element type (head_prep.cuh Operand) of the features, the packed weights and the mid activations
+template <typename T>
 struct K1aParams {
-  CUtensorMap feat;           // features [B * C][H * W] bf16, box {k.box, 128}: one stage's channels of an item's rows
-  const __nv_bfloat16* wpk;   // packed weights [nstages][HEAD_BSTAGE_BYTES]
+  CUtensorMap feat;           // features [B * C][H * W] of type T, box {k.box, 128}: one stage's channels of an item's rows
+  const T* wpk;               // packed weights [nstages][HEAD_BSTAGE_BYTES]
   const float* bias;          // [c1]
-  __nv_bfloat16* mid;         // [B][4][Lmid.rows][8]  padded row layout of the next layer's input (row_layout.cuh)
-  __nv_bfloat16* xs;          // [B][C/32][Lxs.rows][8] (training form): shuffled features in the padded row layout
+  T* mid;                     // [B][4][Lmid.rows][8]  padded row layout of the next layer's input (row_layout.cuh)
+  T* xs;                      // [B][C/32][Lxs.rows][8] (training form): shuffled features in the padded row layout
   RowLayout Lmid, Lxs;
   int B, C;                   // feature batch and channels (C = 4 * Cin)
   int c1, nstages;
@@ -215,10 +221,10 @@ __device__ __forceinline__ void k1a_band(const K1aGeom& k, int item, int& b, int
 }
 
 // One MMA warp's share of every item of its CTA: m16 tiles [m0, m0 + MT) of the band raster, all 80 columns, accumulated
-// over the item's stages; then + bias -> bf16 -> mid activations.  Per accumulator element
+// over the item's stages; then + bias -> T -> mid activations.  Per accumulator element
 // the MMA sequence is stages, then shifts, then k16, then the shift's non-zero n8 tiles.
-template <int MT>
-__device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* stage_base, int stage_bytes, int a_stage_bytes,
+template <int MT, typename T>
+__device__ __forceinline__ void k1a_mma_warp(const K1aParams<T>& P, unsigned char* stage_base, int stage_bytes, int a_stage_bytes,
                                              uint64_t* full, uint64_t* empty, int m0, int lane) {
   const K1aGeom& k = P.k;
   const uint32_t lbo_a = k.rows_alloc * 16, lbo_b = HEAD_NCOLS * 16;
@@ -240,14 +246,14 @@ __device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* 
           const int shift_rows = (sh >> 1) * k.P + (sh & 1);
 #pragma unroll
           for (int k16 = 0; k16 < 2; ++k16)
-            mma::kstep_nz<NZ_N8[sh]>(acc, a0 + (2 * k16) * lbo_a + (16 * m0 + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
+            mma::kstep_nz<NZ_N8[sh], T>(acc, a0 + (2 * k16) * lbo_a + (16 * m0 + shift_rows) * 16, lbo_a, b0 + (sh * 4 + 2 * k16) * lbo_b, lbo_b, lane);
         });
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);
     }
     if constexpr (MT > 0) {
-      // epilogue, 32 rows (two m16 tiles) at a time: (+bias) -> bf16 -> mid activations (A layout); channel c1 of the mid
+      // epilogue, 32 rows (two m16 tiles) at a time: (+bias) -> T -> mid activations (A layout); channel c1 of the mid
       // activations is the constant 1 (lets the next layer fold its bias into the GEMM)
       const int rows_mid = P.Lmid.rows;
       static_for<0, (MT + 1) / 2>([&](auto pc) {
@@ -281,8 +287,7 @@ __device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* 
                   }
                   f[hh] = val;
                 }
-                __nv_bfloat162 h2 = __floats2bfloat162_rn(f[0], f[1]);
-                pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
+                pk[e2] = Operand<T>::pack2(f[0], f[1]);
               }
               *reinterpret_cast<uint4*>(P.mid + ((((size_t)b * 4 + kc) * rows_mid + row2) * 8)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
             }
@@ -293,9 +298,9 @@ __device__ __forceinline__ void k1a_mma_warp(const K1aParams& P, unsigned char* 
   }
 }
 
-// XS = 1: training form, warp 13 writes the saved operand copy; XS = 0: inference
-template <int XS>
-__global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const __grid_constant__ K1aParams P) {
+// XS = 1: training form, warp 13 writes the saved operand copy; XS = 0: inference.  T: the operand element type.
+template <typename T, int XS>
+__global__ void __launch_bounds__(K1A_THREADS, 1) k1a_shuffle_convt_kernel(const __grid_constant__ K1aParams<T> P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const K1aGeom& k = P.k;
   const int a_stage_bytes = 4 * k.rows_alloc * 16;
@@ -473,7 +478,8 @@ static size_t k1a_smem_bytes(const K1aGeom& k) {
   return (size_t)K1A_STAGES * (4 * k.rows_alloc * 16 + HEAD_BSTAGE_BYTES) + (size_t)K1A_STAGES * 4 * HEAD_KSTAGE * k.box * 2 + 128 + K1A_ZROWS * 16;
 }
 
-// features [B][C][HW] bf16 viewed as [B * C][HW]; box = {box_px positions, 128 channels}, box_px <= HW (make_k1a_geom)
+// features [B][C][HW] of type T viewed as [B * C][HW]; box = {box_px positions, 128 channels}, box_px <= HW (make_k1a_geom)
+template <typename T>
 static bool make_feat_tensor_map(CUtensorMap* tm, const void* feat, int B, int C, int HW, int box_px) {
   const TensorMapEncodeFn encode = tensor_map_encoder();
   if (!encode || (HW * 2) % 16 != 0 || (box_px * 2) % 16 != 0 || box_px > 256 || box_px > HW) return false;
@@ -481,7 +487,8 @@ static bool make_feat_tensor_map(CUtensorMap* tm, const void* feat, int B, int C
   const cuuint64_t gstride[1] = {(cuuint64_t)HW * 2};  // bytes, dim 1
   const cuuint32_t box[2] = {(cuuint32_t)box_px, 4 * HEAD_KSTAGE};
   const cuuint32_t estr[2] = {1, 1};
-  return encode(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(feat), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  const CUtensorMapDataType dtype = std::is_same_v<T, __half> ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  return encode(tm, dtype, 2, const_cast<void*>(feat), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 }  // namespace lpb
@@ -547,20 +554,23 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
   return LPB_OK;
 }
 
-extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
-                                 const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
-                                 void* workspace, void* stream) {
+// lpb_head_fwd_bf16 (T = __nv_bfloat16) and lpb_head_fwd_f16 (T = __half): one plan, one workspace layout, one kernel
+// sequence; T is the element type of the features, the packed weights and the mid activations.
+template <typename T>
+static int head_fwd(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1, const float* w2,
+                    const float* b2, int c2, int final_softmax, float* out, void* saved_xs, void* workspace, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(features && w1 && b1 && out && workspace, "head_fwd_bf16: null pointer");
-  LPB_REQUIRE(c2 == 0 || (w2 && b2), "head_fwd_bf16: a two-deconv head needs w2 and b2");
-  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "head_fwd_bf16: bad feature shape C=%d H=%d W=%d", C, H, W);
-  LPB_REQUIRE((H * W) % 8 == 0, "head_fwd_bf16: H*W must be a multiple of 8 (got %d)", H * W);
-  LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "head_fwd_bf16: channel counts %d/%d outside this build's set (lpb200.h)", c1, c2);
+  const char* name = head_fwd_name<T>;
+  LPB_REQUIRE(features && w1 && b1 && out && workspace, "%s: null pointer", name);
+  LPB_REQUIRE(c2 == 0 || (w2 && b2), "%s: a two-deconv head needs w2 and b2", name);
+  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "%s: bad feature shape C=%d H=%d W=%d", name, C, H, W);
+  LPB_REQUIRE((H * W) % 8 == 0, "%s: H*W must be a multiple of 8 (got %d)", name, H * W);
+  LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "%s: channel counts %d/%d outside this build's set (lpb200.h)", name, c1, c2);
   // features: TMA or uint4 loads; saved_xs, workspace: bulk copies and uint4 stores; out: float2 stores
-  LPB_REQUIRE(aligned_to(features, 16), "head_fwd_bf16: features must be 16-byte aligned");
-  LPB_REQUIRE(aligned_to(saved_xs, 16), "head_fwd_bf16: saved_xs must be 16-byte aligned");
-  LPB_REQUIRE(aligned_to(workspace, 16), "head_fwd_bf16: workspace must be 16-byte aligned");
-  LPB_REQUIRE(aligned_to(out, 8), "head_fwd_bf16: out must be 8-byte aligned");
+  LPB_REQUIRE(aligned_to(features, 16), "%s: features must be 16-byte aligned", name);
+  LPB_REQUIRE(aligned_to(saved_xs, 16), "%s: saved_xs must be 16-byte aligned", name);
+  LPB_REQUIRE(aligned_to(workspace, 16), "%s: workspace must be 16-byte aligned", name);
+  LPB_REQUIRE(aligned_to(out, 8), "%s: out must be 8-byte aligned", name);
   if (B == 0) return LPB_OK;
   int max_smem = 0, sms = 0;
   device_limits(&max_smem, &sms);
@@ -571,17 +581,17 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   // a function of the shape (CPU-only callers size buffers with it); every driver that runs sm_90a code has the encoder,
   // and the features' alignment was checked with the arguments.
   CUtensorMap feat_map;
-  if (fast && !make_feat_tensor_map(&feat_map, features, B, C, H * W, k1.box)) {
-    set_error("head_fwd_bf16: cannot encode the feature tensor map");
+  if (fast && !make_feat_tensor_map<T>(&feat_map, features, B, C, H * W, k1.box)) {
+    set_error("%s: cannot encode the feature tensor map", name);
     return LPB_ERR_INVALID;
   }
   const int nst = C / 4 / HEAD_KSTAGE, nst2 = head_mid_stages(c1);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const RowLayout Lxs = make_row_layout(2 * H, 2 * W), Lmid = make_row_layout(4 * H, 4 * W);
   const HeadFwdLayout wl = head_fwd_layout(B, C, H, W, c1, c2);
-  __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.w1);
-  __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.w2);
-  __nv_bfloat16* mid = reinterpret_cast<__nv_bfloat16*>(ws + wl.mid);
+  T* wp1 = reinterpret_cast<T*>(ws + wl.w1);
+  T* wp2 = reinterpret_cast<T*>(ws + wl.w2);
+  T* mid = reinterpret_cast<T*>(ws + wl.mid);
   float* partials = reinterpret_cast<float*>(ws + wl.partials);
   {
     // one launch: both operand packs + the pad rows of the fresh row-layout buffers (k1a writes every row of the saved
@@ -594,16 +604,16 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
       jobs.fpack[1] = {w2, final_softmax ? nullptr : b2, c1, c2, nst2, head_groups(c2), wp2};
       jobs.pads[0] = {mid, Lmid, (long long)B * 4 * nst2};
     }
-    launch_head_prep(jobs, s);
+    launch_head_prep<T>(jobs, s);
   }
   if (!fast) {
     // ---- generic path: shuffle rows -> banded GEMM(s) ----
-    LPB_REQUIRE(saved_xs, "head_fwd_bf16: this shape takes the banded kernels (lpb_head_bf16_plan = 0): pass the "
-                          "lpb_head_bf16_saved_bytes() buffer as saved_xs");
-    __nv_bfloat16* xs = static_cast<__nv_bfloat16*>(saved_xs);
-    int rc = launch_rows_shuffle(static_cast<const __nv_bfloat16*>(features), B, C, H, W, xs, s);
+    LPB_REQUIRE(saved_xs, "%s: this shape takes the banded kernels (lpb_head_bf16_plan = 0): pass the "
+                          "lpb_head_bf16_saved_bytes() buffer as saved_xs", name);
+    T* xs = static_cast<T*>(saved_xs);
+    int rc = launch_rows_shuffle(static_cast<const T*>(features), B, C, H, W, xs, s);
     if (rc != LPB_OK) return rc;
-    ConvtRowsParams p{};
+    ConvtRowsParams<T> p{};
     p.X = xs;
     p.L = Lxs;
     p.wpk = wp1;
@@ -628,12 +638,12 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     if (rc != LPB_OK) return rc;
   } else {
     const size_t s1 = k1a_smem_bytes(k1);
-    K1aParams pa{};
+    K1aParams<T> pa{};
     pa.feat = feat_map;
     pa.wpk = wp1;
     pa.bias = b1;
     pa.mid = mid;
-    pa.xs = static_cast<__nv_bfloat16*>(saved_xs);
+    pa.xs = static_cast<T*>(saved_xs);
     pa.Lmid = Lmid;
     pa.Lxs = Lxs;
     pa.B = B;
@@ -641,7 +651,7 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     pa.c1 = c1;
     pa.nstages = nst;
     pa.k = k1;
-    auto kern = saved_xs ? k1a_shuffle_convt_kernel<1> : k1a_shuffle_convt_kernel<0>;
+    auto kern = saved_xs ? k1a_shuffle_convt_kernel<T, 1> : k1a_shuffle_convt_kernel<T, 0>;
     LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s1));
     // items are dealt round-robin (item = blockIdx.x + k gridDim.x), so with G = 2 and an even grid (132 SMs) a CTA always
     // takes the same band, and likewise with G = 3 and a grid divisible by 3: bands of equal size keep the CTAs even.
@@ -651,7 +661,7 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
     kern<<<items < sms ? items : sms, K1A_THREADS, s1, s>>>(pa);
   }
   // ---- layer 2 of a two-deconv head, on both paths: the banded kernel over the mid activations ----
-  ConvtRowsParams p2{};
+  ConvtRowsParams<T> p2{};
   p2.X = mid;
   p2.L = Lmid;
   p2.wpk = wp2;
@@ -666,4 +676,16 @@ extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int 
   if (rc != LPB_OK) return rc;
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
+}
+
+extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                                 const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
+                                 void* workspace, void* stream) {
+  return head_fwd<__nv_bfloat16>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, out, saved_xs, workspace, stream);
+}
+
+extern "C" int lpb_head_fwd_f16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                                const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
+                                void* workspace, void* stream) {
+  return head_fwd<__half>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, out, saved_xs, workspace, stream);
 }

@@ -1,13 +1,42 @@
-// One launch for everything a head call has to prepare: operand packing of the weights (fp32 master -> bf16 UMMA images),
+// One launch for everything a head call has to prepare: operand packing of the weights (fp32 master -> bf16 / fp16 images),
 // clearing the pad rows of freshly allocated row-layout buffers, zeroing gradient accumulators.  Eight tiny launches per
 // forward + backward pair became two (each used to cost a launch latency and a tail of its own).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
+
+#include <cstdint>
 
 #include "row_layout.cuh"
 
 namespace lpb {
+
+// The operand element type T of the forward: __nv_bfloat16 (the bf16 head) or __half (the fp16 forward).  Both are
+// 2-byte elements in the same layouts below, so packs, workspaces and kernels differ only in how an fp32 value is
+// rounded into T (round-to-nearest-even, subnormals kept, overflow to inf: torch's .bfloat16() / .half()), in the bits
+// of the constant-one channel that carries a bias, and in the MMA's operand type (mma_sm90.cuh mma16).  Every backward
+// operand is bf16.
+template <typename T>
+struct Operand;
+template <>
+struct Operand<__nv_bfloat16> {
+  static constexpr uint16_t one = 0x3f80;  // bf16 1.0
+  static __device__ __forceinline__ __nv_bfloat16 from(float v) { return __float2bfloat16_rn(v); }
+  static __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
+    __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&h2);
+  }
+};
+template <>
+struct Operand<__half> {
+  static constexpr uint16_t one = 0x3c00;  // fp16 1.0
+  static __device__ __forceinline__ __half from(float v) { return __float2half_rn(v); }
+  static __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
+    __half2 h2 = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&h2);
+  }
+};
 
 // A stride-2 3x3 transposed convolution in the 4-shift form (head_bf16.cu): output class cls = 2 py + px reads input
 // shift sh = 2 dm + dn through a real tap unless (py == 0 && dm == 1) or (px == 0 && dn == 1) -- 9 of the 16 pairs.  The
@@ -62,16 +91,19 @@ __host__ __device__ constexpr bool head_wide(int c1, int c2) {
 static_assert(head_groups(HEAD_CLS) == 1 && head_mid_stages(HEAD_CLS - 1) == 1, "narrow heads: one group, one mid stage");
 
 struct PrepJobs {
-  // forward operand packs: W[Cin][Cout][3][3] -> B[group][stage][shift][kchunk][80][8]   (head_bf16.cu)
-  struct { const float* w; const float* bias; int Cin, Cout, nstages, ngroups; __nv_bfloat16* out; } fpack[2];
+  // forward operand packs: W[Cin][Cout][3][3] -> B[group][stage][shift][kchunk][80][8] of the launch's operand type T
+  // (head_bf16.cu)
+  struct { const float* w; const float* bias; int Cin, Cout, nstages, ngroups; void* out; } fpack[2];
   // data-gradient operand packs: -> [kgroup][tile][shift][kchunk][rows_per_tile][8]    (head_bwd_bf16.cu): K is one
   // keypoint group of the layer's output channels (kgroups of them), row r of tile t is input channel tile_ch t + r
-  // (rows r >= tile_ch are zero)
+  // (rows r >= tile_ch are zero); always bf16
   struct { const float* w; int Cin, Cout, ntiles, rows_per_tile, tile_ch, kgroups; __nv_bfloat16* out; } dpack[2];
-  struct { __nv_bfloat16* buf; RowLayout L; long long nslabs; } pads[2];
+  // pad rows of row-layout buffers of 2-byte elements (zero in either type)
+  struct { void* buf; RowLayout L; long long nslabs; } pads[2];
   struct { float* p; long long n; } zero[4];
 };
 
+template <typename T = __nv_bfloat16>
 int launch_head_prep(const PrepJobs& jobs, cudaStream_t s);
 
 }  // namespace lpb

@@ -4,6 +4,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include <type_traits>
+
 #include "head_prep.cuh"
 #include "row_layout.cuh"
 
@@ -11,14 +13,16 @@ namespace lpb {
 
 enum { CONVT_ROWS_MID = 0, CONVT_ROWS_PLANES = 1, CONVT_ROWS_SOFTMAX = 2, CONVT_ROWS_SOFTMAX_P0 = 3, CONVT_ROWS_SOFTMAX_P1 = 4 };
 
+// T: the operand element type (head_prep.cuh Operand)
+template <typename T>
 struct ConvtRowsParams {
-  const __nv_bfloat16* X;    // [B][4*nst][L.rows][8] padded row layout of the conv input
+  const T* X;                // [B][4*nst][L.rows][8] padded row layout of the conv input
   RowLayout L;
-  const __nv_bfloat16* wpk;  // [ngroups][nst][4 shifts][4 kchunks][80][8] (head_prep_kernel)
+  const T* wpk;              // [ngroups][nst][4 shifts][4 kchunks][80][8] (head_prep_kernel)
   const float* bias;         // [cout] added in the epilogue, or null (bias folded into the GEMM / irrelevant)
   int nst;                   // 32-channel K stages
   int B, cout, mode;
-  __nv_bfloat16* mid;        // CONVT_ROWS_MID: [B][mid_kc][Lout.rows][8], channel `cout` = 1, the rest of the chunks 0
+  T* mid;                    // CONVT_ROWS_MID: [B][mid_kc][Lout.rows][8], channel `cout` = 1, the rest of the chunks 0
   RowLayout Lout;
   int mid_kc;                // CONVT_ROWS_MID: K-chunks of the next layer's input (4 * head_mid_stages(cout))
   float* out;                // planes [B][cout][2Hi][2Wi] (raw or softmaxed)
@@ -28,8 +32,14 @@ struct ConvtRowsParams {
   int ngroups;               // filled by launch_convt_rows: keypoint groups of the output channels (head_prep.cuh)
 };
 
-int launch_rows_shuffle(const __nv_bfloat16* feat, int B, int C, int H, int W, __nv_bfloat16* xs, cudaStream_t s);
-int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s);
+// the C-ABI entry of each operand type, named in its error messages
+template <typename T>
+constexpr const char* head_fwd_name = std::is_same_v<T, __half> ? "head_fwd_f16" : "head_fwd_bf16";
+
+template <typename T>
+int launch_rows_shuffle(const T* feat, int B, int C, int H, int W, T* xs, cudaStream_t s);
+template <typename T>
+int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s);
 
 // raster rows per band of the banded kernel (its M-tiles x 128)
 constexpr int CR_BAND_ROWS = 256;

@@ -1,4 +1,5 @@
-// Shape-generic bf16 heatmap head on the tensor cores: any feature map, one- or two-deconv heads (ViT / ResNet families).
+// Shape-generic bf16 / fp16 heatmap head on the tensor cores: any feature map, one- or two-deconv heads (ViT / ResNet
+// families).  The operand element type is a template parameter of the GEMM kernel (head_prep.cuh Operand).
 // Reference: lightning_pose/models/heads/heatmap.py:20-71 (layer stack; ViT stride 16 -> one deconv, :192-193),
 // :203-212 (forward).
 //
@@ -28,17 +29,18 @@ namespace lpb {
 
 // ---- PixelShuffle(2) + NCHW -> padded row layout ----------------------------------------------------------------
 // one CTA per (frame, K-chunk of 8 shuffled channels = 32 source channels): the slab is read with 16-byte loads,
-// transposed through shared memory and written as whole rows (pads included, so the buffer needs no clearing)
-__global__ void __launch_bounds__(256) rows_shuffle_kernel(const __nv_bfloat16* __restrict__ feat, int C, int H, int W,
-                                                           __nv_bfloat16* __restrict__ xs, RowLayout L) {
+// transposed through shared memory and written as whole rows (pads included, so the buffer needs no clearing).  It moves
+// 2-byte elements without looking at them, so bf16 and fp16 features share it.
+__global__ void __launch_bounds__(256) rows_shuffle_kernel(const uint16_t* __restrict__ feat, int C, int H, int W,
+                                                           uint16_t* __restrict__ xs, RowLayout L) {
   extern __shared__ __align__(16) unsigned char smraw[];
-  __nv_bfloat16* sl = reinterpret_cast<__nv_bfloat16*>(smraw);  // [32][H*W]
+  uint16_t* sl = reinterpret_cast<uint16_t*>(smraw);  // [32][H*W]
   const int HW = H * W, nkc = C / 32;
   const int b = blockIdx.x / nkc, kc = blockIdx.x - b * nkc;
   const uint4* src = reinterpret_cast<const uint4*>(feat + ((size_t)b * C + (size_t)kc * 32) * HW);
   for (int i = threadIdx.x; i < 32 * HW / 8; i += 256) reinterpret_cast<uint4*>(sl)[i] = __ldg(src + i);
   __syncthreads();
-  __nv_bfloat16* dst = xs + ((size_t)b * nkc + kc) * (size_t)L.rows * 8;
+  uint16_t* dst = xs + ((size_t)b * nkc + kc) * (size_t)L.rows * 8;
   const int body1 = L.lead + L.Hi * L.Pp;
   for (int r = threadIdx.x; r < L.rows; r += 256) {
     uint4 o = make_uint4(0, 0, 0, 0);
@@ -49,8 +51,8 @@ __global__ void __launch_bounds__(256) rows_shuffle_kernel(const __nv_bfloat16* 
         uint32_t pk[4];
 #pragma unroll
         for (int e2 = 0; e2 < 4; ++e2) {
-          const uint32_t lo = *reinterpret_cast<const unsigned short*>(sl + (size_t)(8 * e2 + q) * HW + pos);
-          const uint32_t hi = *reinterpret_cast<const unsigned short*>(sl + (size_t)(8 * e2 + 4 + q) * HW + pos);
+          const uint32_t lo = sl[(size_t)(8 * e2 + q) * HW + pos];
+          const uint32_t hi = sl[(size_t)(8 * e2 + 4 + q) * HW + pos];
           pk[e2] = lo | (hi << 16);
         }
         o = make_uint4(pk[0], pk[1], pk[2], pk[3]);
@@ -60,14 +62,17 @@ __global__ void __launch_bounds__(256) rows_shuffle_kernel(const __nv_bfloat16* 
   }
 }
 
-int launch_rows_shuffle(const __nv_bfloat16* feat, int B, int C, int H, int W, __nv_bfloat16* xs, cudaStream_t s) {
+template <typename T>
+int launch_rows_shuffle(const T* feat, int B, int C, int H, int W, T* xs, cudaStream_t s) {
   const RowLayout L = make_row_layout(2 * H, 2 * W);
   const size_t smem = (size_t)32 * H * W * 2;
-  LPB_REQUIRE(smem <= 200 * 1024, "head_fwd_bf16: feature map %dx%d too large for the shuffle stage", H, W);
+  LPB_REQUIRE(smem <= 200 * 1024, "%s: feature map %dx%d too large for the shuffle stage", head_fwd_name<T>, H, W);
   if (smem > 48 * 1024) LPB_CUDA(cudaFuncSetAttribute(rows_shuffle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  rows_shuffle_kernel<<<(unsigned)(B * (C / 32)), 256, smem, s>>>(feat, C, H, W, xs, L);
+  rows_shuffle_kernel<<<(unsigned)(B * (C / 32)), 256, smem, s>>>(reinterpret_cast<const uint16_t*>(feat), C, H, W, reinterpret_cast<uint16_t*>(xs), L);
   return LPB_OK;
 }
+template int launch_rows_shuffle<__nv_bfloat16>(const __nv_bfloat16*, int, int, int, int, __nv_bfloat16*, cudaStream_t);
+template int launch_rows_shuffle<__half>(const __half*, int, int, int, int, __half*, cudaStream_t);
 
 // ---- banded transposed-convolution GEMM ---------------------------------------------------------------------------
 constexpr int CR_THREADS = 320;  // warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue
@@ -83,8 +88,9 @@ constexpr int CR_STAGES = 2;
 // stages its rows, runs the group's 80-column GEMM and finishes the group's planes (or its mid channels [20g, 20g + 20),
 // written as 8-byte halves of the K-chunks, since two groups can share a chunk).  The per-warp accumulators are those of
 // a single group; a band is staged once per group and re-read from L2.
-template <int MODE, int NPL, bool WIDE = false>
-__global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_constant__ ConvtRowsParams P) {
+// T: the operand element type (head_prep.cuh Operand); the mid activations are written in it too.
+template <typename T, int MODE, int NPL, bool WIDE = false>
+__global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_constant__ ConvtRowsParams<T> P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Pp = P.L.Pp, Wi = P.L.Wi, Hi = P.L.Hi;
   const int a_bytes = 4 * P.rows_alloc * 16, stage_bytes = a_bytes + HEAD_BSTAGE_BYTES;
@@ -209,7 +215,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                   const int shift_rows = (sh >> 1) * Pp + (sh & 1);
 #pragma unroll
                   for (int k16 = 0; k16 < 2; ++k16)
-                    mma::kstep(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
+                    mma::kstep<T>(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
                                b0 + (sh * 4 + 2 * k16) * lbo_b + 32 * e * 16, lbo_b, lane);
                 }
               }
@@ -225,7 +231,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                     const int shift_rows = (sh >> 1) * Pp + (sh & 1);
 #pragma unroll
                     for (int k16 = 0; k16 < 2; ++k16)
-                      mma::kstep_nz<mask>(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
+                      mma::kstep_nz<mask, T>(acc[t], a0 + (2 * k16) * lbo_a + (t * 128 + 32 * q + shift_rows) * 16, lbo_a,
                                           b0 + (sh * 4 + 2 * k16) * lbo_b + 32 * E * 16, lbo_b, lane);
                   });
                 }
@@ -249,7 +255,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             auto body = [&](auto ec) {
               constexpr int E = decltype(ec)::value;
               if constexpr (MODE == CONVT_ROWS_MID && WIDE) {
-                // bf16 rows of the next layer, by 4-channel units (8-byte halves of a K-chunk): the group's five units
+                // T rows of the next layer, by 4-channel units (8-byte halves of a K-chunk): the group's five units
                 // 5g .. 5g + 4, and the last group also the units past the groups up to the end of the last K-chunk.
                 // Channel `cout` is the constant one, every other channel >= cout is 0.
                 if (valid) {
@@ -257,7 +263,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 #pragma unroll
                   for (int px = 0; px < 2; ++px) {
                     const size_t row2 = (size_t)P.Lout.lead + (size_t)y * P.Lout.Pp + x + px;
-                    __nv_bfloat16* base = P.mid + ((size_t)b * P.mid_kc * P.Lout.rows + row2) * 8;
+                    T* base = P.mid + ((size_t)b * P.mid_kc * P.Lout.rows + row2) * 8;
 #pragma unroll
                     for (int i = 0; i < HEAD_CLS / 4; ++i) {
                       const int u = 5 * g + i;
@@ -271,14 +277,13 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                           const int ch = o0 + cl;
                           f[hh] = ch < P.cout ? d[8 * E + px * HEAD_CLS + cl] + (use_bias ? __ldg(bias + cl) : 0.f) : (ch == P.cout ? 1.0f : 0.f);
                         }
-                        __nv_bfloat162 h2 = __floats2bfloat162_rn(f[0], f[1]);
-                        pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
+                        pk[e2] = Operand<T>::pack2(f[0], f[1]);
                       }
                       *reinterpret_cast<uint2*>(base + (size_t)(u >> 1) * P.Lout.rows * 8 + (u & 1) * 4) = make_uint2(pk[0], pk[1]);
                     }
                     for (int u = 5 * g + 5; u < u1; ++u) {
                       const int c0 = 4 * u;
-                      const uint32_t one = 0x3f80u;  // bf16 1.0
+                      const uint32_t one = Operand<T>::one;
                       const uint32_t lo = (c0 == P.cout ? one : 0u) | (c0 + 1 == P.cout ? one << 16 : 0u);
                       const uint32_t hi = (c0 + 2 == P.cout ? one : 0u) | (c0 + 3 == P.cout ? one << 16 : 0u);
                       *reinterpret_cast<uint2*>(base + (size_t)(u >> 1) * P.Lout.rows * 8 + (u & 1) * 4) = make_uint2(lo, hi);
@@ -287,7 +292,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                 }
                 return;
               } else if constexpr (MODE == CONVT_ROWS_MID) {
-                // bf16 rows of the next layer: channel `cout` is the constant one (carries that layer's bias)
+                // T rows of the next layer: channel `cout` is the constant one (carries that layer's bias)
                 if (valid) {
 #pragma unroll
                   for (int px = 0; px < 2; ++px) {
@@ -310,8 +315,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                           }
                           f[hh] = val;
                         }
-                        __nv_bfloat162 h2 = __floats2bfloat162_rn(f[0], f[1]);
-                        pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
+                        pk[e2] = Operand<T>::pack2(f[0], f[1]);
                       }
                       *reinterpret_cast<uint4*>(P.mid + ((((size_t)b * 4 + kc) * P.Lout.rows + row2) * 8)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
                     }
@@ -414,18 +418,20 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
   }
 }
 
-int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
+template <typename T>
+int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s) {
+  const char* name = head_fwd_name<T>;
   const int Pp = p.L.Pp;
-  LPB_REQUIRE(Pp <= CR_TILES * 128, "head_fwd_bf16: image width %d too large for one band", p.L.Wi);
-  LPB_REQUIRE(p.cout >= 1 && p.cout <= HEAD_MAX_CH, "head_fwd_bf16: %d output channels exceed %d", p.cout, HEAD_MAX_CH);
-  LPB_REQUIRE(p.mode != CONVT_ROWS_MID || p.mid_kc >= 4 * head_mid_stages(p.cout), "head_fwd_bf16: mid activations of %d K-chunks", p.mid_kc);
+  LPB_REQUIRE(Pp <= CR_TILES * 128, "%s: image width %d too large for one band", name, p.L.Wi);
+  LPB_REQUIRE(p.cout >= 1 && p.cout <= HEAD_MAX_CH, "%s: %d output channels exceed %d", name, p.cout, HEAD_MAX_CH);
+  LPB_REQUIRE(p.mode != CONVT_ROWS_MID || p.mid_kc >= 4 * head_mid_stages(p.cout), "%s: mid activations of %d K-chunks", name, p.mid_kc);
   p.R = (CR_TILES * 128) / Pp;
   if (p.R > p.L.Hi) p.R = p.L.Hi;
   const int tiles = (p.R * Pp + 127) / 128;
   p.rows_alloc = (tiles * 128 + Pp + 1 + 7) & ~7;
   if (p.rows_alloc < (p.R + 1) * Pp + 8) p.rows_alloc = ((p.R + 1) * Pp + 8 + 7) & ~7;
   const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + HEAD_BSTAGE_BYTES) + (2 * HEAD_CLS * 8 + 2 * HEAD_CLS) * sizeof(float) + 64;
-  LPB_REQUIRE(smem <= 113 * 1024, "head_fwd_bf16: band stages need %zu B shared memory", smem);
+  LPB_REQUIRE(smem <= 113 * 1024, "%s: band stages need %zu B shared memory", name, smem);
   const int nbands = (p.L.Hi + p.R - 1) / p.R;
   auto run = [&](auto kern, long long nitems) -> int {
     const int grid = (int)(nitems < sms ? nitems : sms);  // one CTA per SM: the accumulators take the register file
@@ -439,31 +445,33 @@ int launch_convt_rows(ConvtRowsParams p, int sms, cudaStream_t s) {
   p.ngroups = head_groups(p.cout);
   if (wide) {
     const long long per_group = (long long)p.B * nbands * p.ngroups;
-    if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<CONVT_ROWS_MID, 0, true>, per_group);
-    if (p.mode == CONVT_ROWS_PLANES) return run(convt_rows_kernel<CONVT_ROWS_PLANES, 0, true>, per_group);
+    if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<T, CONVT_ROWS_MID, 0, true>, per_group);
+    if (p.mode == CONVT_ROWS_PLANES) return run(convt_rows_kernel<T, CONVT_ROWS_PLANES, 0, true>, per_group);
     // the split / fused choice of the narrow heads below, counting (frame, group) items
     if (p.partials && (g_softmax_split == 2 || (g_softmax_split == 1 && (long long)p.B * p.ngroups < sms))) {
-      const int rc = run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 0, true>, per_group);
+      const int rc = run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX_P0, 0, true>, per_group);
       if (rc != LPB_OK) return rc;
-      return run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 0, true>, per_group);
+      return run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX_P1, 0, true>, per_group);
     }
-    return run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0, true>, (long long)p.B * p.ngroups);
+    return run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX, 0, true>, (long long)p.B * p.ngroups);
   }
   const bool k17 = p.cout == 17;
   const long long per_band = (long long)p.B * nbands;
-  if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<CONVT_ROWS_MID, 0>, per_band);
-  if (p.mode == CONVT_ROWS_PLANES) return k17 ? run(convt_rows_kernel<CONVT_ROWS_PLANES, 17>, per_band) : run(convt_rows_kernel<CONVT_ROWS_PLANES, 0>, per_band);
+  if (p.mode == CONVT_ROWS_MID) return run(convt_rows_kernel<T, CONVT_ROWS_MID, 0>, per_band);
+  if (p.mode == CONVT_ROWS_PLANES) return k17 ? run(convt_rows_kernel<T, CONVT_ROWS_PLANES, 17>, per_band) : run(convt_rows_kernel<T, CONVT_ROWS_PLANES, 0>, per_band);
   // split softmax (statistics launch + normalising launch, both parallel over (frame, band)) when one CTA per frame would
   // leave SMs idle (fewer frames than SMs); otherwise the single two-pass kernel is faster, because a frame's second pass
   // re-reads operands its first pass left in L2 (768-frame step 1.768 vs 1.802 ms; with the 256-frame labeled call fused
   // as well: step 1.565 vs 1.583 ms, forward-only 0.611 vs 0.635 ms).  Key value 2 forces the split.
   const int split_key = g_softmax_split;
   if (p.partials && (split_key == 2 || (split_key == 1 && p.B < sms))) {
-    int rc = k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 17>, per_band) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P0, 0>, per_band);
+    int rc = k17 ? run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX_P0, 17>, per_band) : run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX_P0, 0>, per_band);
     if (rc != LPB_OK) return rc;
-    return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 17>, per_band) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX_P1, 0>, per_band);
+    return k17 ? run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX_P1, 17>, per_band) : run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX_P1, 0>, per_band);
   }
-  return k17 ? run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 17>, p.B) : run(convt_rows_kernel<CONVT_ROWS_SOFTMAX, 0>, p.B);
+  return k17 ? run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX, 17>, p.B) : run(convt_rows_kernel<T, CONVT_ROWS_SOFTMAX, 0>, p.B);
 }
+template int launch_convt_rows<__nv_bfloat16>(ConvtRowsParams<__nv_bfloat16>, int, cudaStream_t);
+template int launch_convt_rows<__half>(ConvtRowsParams<__half>, int, cudaStream_t);
 
 }  // namespace lpb

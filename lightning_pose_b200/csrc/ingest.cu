@@ -44,36 +44,22 @@ __device__ __forceinline__ void resized_pixel(const uint8_t* img, int H, int W, 
   }
 }
 
-// Normalised output pixel (f, y, x) in the FCHW (LAYOUT 0) or FHWC (LAYOUT 1) layout, fp32 or bf16.
-template <int LAYOUT, bool BF16>
+// Normalised output pixel (f, y, x) in the FCHW (LAYOUT 0) or FHWC (LAYOUT 1) layout, in output format FMT (LPB_OUT_*).
+template <int LAYOUT, int FMT>
 __device__ __forceinline__ void store_pixel(void* out, int OH, int OW, int f, int y, int x, const float v[3]) {
   const size_t plane = (size_t)OH * OW;
   if (LAYOUT == 0) {  // FCHW
     const size_t o = (size_t)f * 3 * plane + (size_t)y * OW + x;
-    if (BF16) {
-      __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(out);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) dst[o + c * plane] = __float2bfloat16_rn(v[c]);
-    } else {
-      float* dst = static_cast<float*>(out);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) dst[o + c * plane] = v[c];
-    }
+    for (int c = 0; c < 3; ++c) store_fmt<FMT>(out, o + c * plane, v[c]);
   } else {  // FHWC
     const size_t o = ((size_t)f * plane + (size_t)y * OW + x) * 3;
-    if (BF16) {
-      __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(out);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) dst[o + c] = __float2bfloat16_rn(v[c]);
-    } else {
-      float* dst = static_cast<float*>(out);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) dst[o + c] = v[c];
-    }
+    for (int c = 0; c < 3; ++c) store_fmt<FMT>(out, o + c, v[c]);
   }
 }
 
-template <int LAYOUT, bool BF16, bool RESIZE>
+template <int LAYOUT, int FMT, bool RESIZE>
 __global__ void __launch_bounds__(256) ingest_kernel(const __grid_constant__ IngestParams P) {
   const int64_t total = (int64_t)P.F * P.OH * P.OW;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -84,7 +70,7 @@ __global__ void __launch_bounds__(256) ingest_kernel(const __grid_constant__ Ing
     resized_pixel<RESIZE>(P.in + (size_t)f * P.H * P.W * 3, P.H, P.W, P.ry, P.rx, y, x, v);
 #pragma unroll
     for (int c = 0; c < 3; ++c) v[c] = fmaf(v[c], P.scale[c], P.shift[c]);
-    store_pixel<LAYOUT, BF16>(P.out, P.OH, P.OW, f, y, x, v);
+    store_pixel<LAYOUT, FMT>(P.out, P.OH, P.OW, f, y, x, v);
   }
 }
 
@@ -103,7 +89,7 @@ struct IngestViewsParams {
   float scale[3], shift[3];
 };
 
-template <int LAYOUT, bool BF16>
+template <int LAYOUT, int FMT>
 __global__ void __launch_bounds__(256) ingest_views_kernel(const __grid_constant__ IngestViewsParams P) {
   const int64_t total = (int64_t)P.F * P.V * P.OH * P.OW;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -120,7 +106,7 @@ __global__ void __launch_bounds__(256) ingest_views_kernel(const __grid_constant
       resized_pixel<false>(img, H, W, 0.f, 0.f, y, x, v);
 #pragma unroll
     for (int c = 0; c < 3; ++c) v[c] = fmaf(v[c], P.scale[c], P.shift[c]);
-    store_pixel<LAYOUT, BF16>(P.out, P.OH, P.OW, fv, y, x, v);
+    store_pixel<LAYOUT, FMT>(P.out, P.OH, P.OW, fv, y, x, v);
   }
 }
 
@@ -211,7 +197,7 @@ __device__ float poisson_sample(float lam, uint4 ctr, uint2 key) {
   }
 }
 
-template <int LAYOUT, bool BF16, bool RESIZE>
+template <int LAYOUT, int FMT, bool RESIZE>
 __global__ void __launch_bounds__(256) augment_kernel(const __grid_constant__ AugmentParams P) {
   __shared__ float s_map[6];    // inverse map with the half-pixel shifts folded in: src = B (x, y) + d
   __shared__ float s_photo[3];  // brightness, contrast, factor
@@ -272,17 +258,18 @@ __global__ void __launch_bounds__(256) augment_kernel(const __grid_constant__ Au
         q = poisson_sample(fmaxf(q / factor, 0.f), make_uint4((uint32_t)x, (uint32_t)y, (uint32_t)f, (uint32_t)c << 24), key) * factor;
       v[c] = fmaf(q, P.scale[c], P.shift[c]);
     }
-    store_pixel<LAYOUT, BF16>(P.out, P.OH, P.OW, f, y, x, v);
+    store_pixel<LAYOUT, FMT>(P.out, P.OH, P.OW, f, y, x, v);
   }
 }
 
 }  // namespace lpb
 
 extern "C" int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* mean3,
-                                    const float* std3, int layout, int out_bf16, void* out, void* stream) {
+                                    const float* std3, int layout, int out_format, void* out, void* stream) {
   using namespace lpb;
   LPB_REQUIRE(frames_u8 && mean3 && std3 && out, "frames_normalize: null pointer");
   LPB_REQUIRE(F >= 0 && H >= 1 && W >= 1 && out_h >= 1 && out_w >= 1 && (layout == 0 || layout == 1), "frames_normalize: bad shape/layout");
+  LPB_REQUIRE(valid_out_format(out_format), "frames_normalize: unknown output format %d", out_format);
   if (F == 0) return LPB_OK;
   IngestParams p;
   p.in = frames_u8;
@@ -300,28 +287,27 @@ extern "C" int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int 
   int64_t blocks = (total + 255) / 256;
   if (blocks > 132 * 32) blocks = 132 * 32;  // 32 CTAs per SM of an H100 SXM
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int key = layout * 4 + (out_bf16 ? 2 : 0) + (resize ? 1 : 0);
-  switch (key) {
-    case 0: ingest_kernel<0, false, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 1: ingest_kernel<0, false, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 2: ingest_kernel<0, true, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 3: ingest_kernel<0, true, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 4: ingest_kernel<1, false, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 5: ingest_kernel<1, false, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 6: ingest_kernel<1, true, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    default: ingest_kernel<1, true, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-  }
+  with_out_format(out_format, [&](auto fc) {
+    constexpr int FMT = decltype(fc)::value;
+    switch (layout * 2 + (resize ? 1 : 0)) {
+      case 0: ingest_kernel<0, FMT, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+      case 1: ingest_kernel<0, FMT, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+      case 2: ingest_kernel<1, FMT, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+      default: ingest_kernel<1, FMT, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    }
+  });
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
 
 extern "C" int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V, int F, const int* H, const int* W, int out_h,
-                                          int out_w, const float* mean3, const float* std3, int layout, int out_bf16, void* out,
+                                          int out_w, const float* mean3, const float* std3, int layout, int out_format, void* out,
                                           void* stream) {
   using namespace lpb;
   LPB_REQUIRE(frames_u8 && H && W && mean3 && std3 && out, "frames_normalize_views: null pointer");
   LPB_REQUIRE(V >= 1 && V <= LPB_INGEST_MAX_VIEWS, "frames_normalize_views: view count %d outside 1..%d", V, LPB_INGEST_MAX_VIEWS);
   LPB_REQUIRE(F >= 0 && out_h >= 1 && out_w >= 1 && (layout == 0 || layout == 1), "frames_normalize_views: bad shape/layout");
+  LPB_REQUIRE(valid_out_format(out_format), "frames_normalize_views: unknown output format %d", out_format);
   LPB_REQUIRE((int64_t)F * V <= INT32_MAX, "frames_normalize_views: F * V must be below 2^31");
   IngestViewsParams p;
   for (int v = 0; v < V; ++v) {  // frames_u8, H and W are HOST arrays
@@ -344,12 +330,11 @@ extern "C" int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V
   int64_t blocks = (total + 255) / 256;
   if (blocks > 132 * 32) blocks = 132 * 32;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  switch (layout * 2 + (out_bf16 ? 1 : 0)) {
-    case 0: ingest_views_kernel<0, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 1: ingest_views_kernel<0, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 2: ingest_views_kernel<1, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    default: ingest_views_kernel<1, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-  }
+  with_out_format(out_format, [&](auto fc) {
+    constexpr int FMT = decltype(fc)::value;
+    if (layout == 0) ingest_views_kernel<0, FMT><<<(unsigned)blocks, 256, 0, s>>>(p);
+    else ingest_views_kernel<1, FMT><<<(unsigned)blocks, 256, 0, s>>>(p);
+  });
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
@@ -362,6 +347,8 @@ extern "C" int lpb_frames_augment_normalize(const uint8_t* frames_u8, int F, int
   LPB_REQUIRE(F >= 0 && H >= 1 && W >= 1 && out_h >= 1 && out_w >= 1 && (layout == 0 || layout == 1),
               "frames_augment_normalize: bad shape/layout");
   LPB_REQUIRE(F <= 16777215 && out_h <= 16777215 && out_w <= 16777215, "frames_augment_normalize: shape too large");
+  // training only: fp32 or bf16, as the training step reads
+  LPB_REQUIRE(out_bf16 == LPB_OUT_F32 || out_bf16 == LPB_OUT_BF16, "frames_augment_normalize: output format %d (0 = fp32, 1 = bf16)", out_bf16);
   if (F == 0) return LPB_OK;
   AugmentParams p;
   p.in = frames_u8;
@@ -384,14 +371,14 @@ extern "C" int lpb_frames_augment_normalize(const uint8_t* frames_u8, int F, int
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int key = layout * 4 + (out_bf16 ? 2 : 0) + (resize ? 1 : 0);
   switch (key) {
-    case 0: augment_kernel<0, false, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 1: augment_kernel<0, false, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 2: augment_kernel<0, true, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 3: augment_kernel<0, true, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 4: augment_kernel<1, false, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 5: augment_kernel<1, false, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    case 6: augment_kernel<1, true, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
-    default: augment_kernel<1, true, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 0: augment_kernel<0, LPB_OUT_F32, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 1: augment_kernel<0, LPB_OUT_F32, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 2: augment_kernel<0, LPB_OUT_BF16, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 3: augment_kernel<0, LPB_OUT_BF16, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 4: augment_kernel<1, LPB_OUT_F32, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 5: augment_kernel<1, LPB_OUT_F32, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    case 6: augment_kernel<1, LPB_OUT_BF16, false><<<(unsigned)blocks, 256, 0, s>>>(p); break;
+    default: augment_kernel<1, LPB_OUT_BF16, true><<<(unsigned)blocks, 256, 0, s>>>(p); break;
   }
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;

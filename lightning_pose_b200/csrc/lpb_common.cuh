@@ -3,6 +3,7 @@
 #include <type_traits>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cstdint>
 #include <cstdio>
 
@@ -33,6 +34,24 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
 inline bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
 
 extern int g_softmax_split;  // abi.cu: LPB_TUNE_SOFTMAX_SPLIT
+
+// ---- output element formats of the ingest entries (LPB_OUT_*, lpb200.h) ----------------------------------------
+// element i of `out` in format FMT: fp32 as is, bf16 / fp16 rounded to nearest even (torch's .bfloat16() / .half())
+template <int FMT>
+__device__ __forceinline__ void store_fmt(void* out, size_t i, float v) {
+  static_assert(FMT == LPB_OUT_F32 || FMT == LPB_OUT_BF16 || FMT == LPB_OUT_F16, "output format");
+  if constexpr (FMT == LPB_OUT_BF16) static_cast<__nv_bfloat16*>(out)[i] = __float2bfloat16_rn(v);
+  else if constexpr (FMT == LPB_OUT_F16) static_cast<__half*>(out)[i] = __float2half_rn(v);
+  else static_cast<float*>(out)[i] = v;
+}
+inline bool valid_out_format(int fmt) { return fmt == LPB_OUT_F32 || fmt == LPB_OUT_BF16 || fmt == LPB_OUT_F16; }
+// f(integral_constant<int, FMT>) for a run-time format the caller has checked
+template <typename F>
+inline void with_out_format(int fmt, F&& f) {
+  if (fmt == LPB_OUT_BF16) f(std::integral_constant<int, LPB_OUT_BF16>{});
+  else if (fmt == LPB_OUT_F16) f(std::integral_constant<int, LPB_OUT_F16>{});
+  else f(std::integral_constant<int, LPB_OUT_F32>{});
+}
 
 // ---- device helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float warp_max(float v) {

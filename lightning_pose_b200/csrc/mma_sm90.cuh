@@ -1,4 +1,4 @@
-// Warp-level bf16 tensor-core helpers for sm_90a: mma.sync m16n8k16 (fp32 accumulate) fed by ldmatrix straight from
+// Warp-level bf16 / fp16 tensor-core helpers for sm_90a: mma.sync m16n8k16 (fp32 accumulate) fed by ldmatrix straight from
 // the library's row layout (row_layout.cuh): 8-element K-chunks of 16 bytes per row, rows linear in memory, so an 8x8
 // ldmatrix block is 8 consecutive rows of one K-chunk and a row-shifted operand is just a different start address.
 //
@@ -6,6 +6,9 @@
 //   acc[mt][nt][0..3] = D(16 mt + g, 8 nt + 2 t + {0, 1}) and D(16 mt + g + 8, ...)   (g = lane / 4, t = lane % 4).
 // rows8() turns one n8 tile into "lane = accumulator row" form, the layout every epilogue of the head reads.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include <cstdint>
 #include <type_traits>
 
@@ -27,6 +30,18 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// m16n8k16 on 16-bit operands of type T (__nv_bfloat16 or __half): same fragments, same fp32 accumulators
+template <typename T>
+__device__ __forceinline__ void mma16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  static_assert(std::is_same_v<T, __nv_bfloat16> || std::is_same_v<T, __half>, "16-bit operands: bf16 or fp16");
+  if constexpr (std::is_same_v<T, __half>) mma_f16(d, a, b0, b1);
+  else mma_bf16(d, a, b0, b1);
 }
 
 // ---- 3xTF32 (fp32-accurate GEMMs on the tf32 tensor cores; the fp32 head, head_f32.cu) ----------------------------
@@ -73,8 +88,9 @@ __device__ __forceinline__ void zero(float (&acc)[MT][NT][4]) {
 }
 
 // One K = 16 step, both operands K-major: A row r at a + 16 r (K-chunk j at + j * lbo_a), B column n at b + 16 n
-// (K-chunk j at + j * lbo_b).  MT m16 tiles of A, NT n8 tiles of B (NT even).
-template <int MT, int NT>
+// (K-chunk j at + j * lbo_b).  MT m16 tiles of A, NT n8 tiles of B (NT even).  T: the operands' element type (the
+// forward's, head_prep.cuh Operand); the backward's operands are bf16.
+template <typename T = __nv_bfloat16, int MT, int NT>
 __device__ __forceinline__ void kstep(float (&acc)[MT][NT][4], uint32_t a, uint32_t lbo_a, uint32_t b, uint32_t lbo_b, int lane) {
   static_assert(NT % 2 == 0, "n8 tiles are loaded in pairs");
   uint32_t af[MT][4];
@@ -86,15 +102,15 @@ __device__ __forceinline__ void kstep(float (&acc)[MT][NT][4], uint32_t a, uint3
     ldsm_x4(bf, b + (uint32_t)(16 * np + (lane >> 4) * 8 + (lane & 7)) * 16 + (uint32_t)((lane >> 3) & 1) * lbo_b);
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
-      mma_bf16(acc[mt][2 * np], af[mt], bf[0], bf[1]);
-      mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
+      mma16<T>(acc[mt][2 * np], af[mt], bf[0], bf[1]);
+      mma16<T>(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
     }
   }
 }
 
 // kstep over the n8 tiles set in MASK only (compile time): the others keep their accumulators and cost no B load, and
 // a pair with one tile left is loaded with ldmatrix .x2.  MASK == 0 issues nothing, not even the A loads.
-template <unsigned MASK, int MT, int NT>
+template <unsigned MASK, typename T = __nv_bfloat16, int MT, int NT>
 __device__ __forceinline__ void kstep_nz(float (&acc)[MT][NT][4], uint32_t a, uint32_t lbo_a, uint32_t b, uint32_t lbo_b, int lane) {
   static_assert(NT % 2 == 0 && (MASK >> NT) == 0, "n8 tiles are loaded in pairs");
   if constexpr (MASK != 0) {
@@ -112,15 +128,15 @@ __device__ __forceinline__ void kstep_nz(float (&acc)[MT][NT][4], uint32_t a, ui
         ldsm_x4(bf, bl + (uint32_t)(16 * np) * 16);
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
-          mma_bf16(acc[mt][2 * np], af[mt], bf[0], bf[1]);
-          mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
+          mma16<T>(acc[mt][2 * np], af[mt], bf[0], bf[1]);
+          mma16<T>(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
         }
       } else if (lo || hi) {
         const int nt = 2 * np + (hi ? 1 : 0);
         uint32_t bf[2];
         ldsm_x2(bf, bl + (uint32_t)(8 * nt) * 16);
 #pragma unroll
-        for (int mt = 0; mt < MT; ++mt) mma_bf16(acc[mt][nt], af[mt], bf[0], bf[1]);
+        for (int mt = 0; mt < MT; ++mt) mma16<T>(acc[mt][nt], af[mt], bf[0], bf[1]);
       }
     }
   }

@@ -71,8 +71,9 @@ def _needs_grad(features: torch.Tensor, params) -> bool:
 class _HeadFunction(torch.autograd.Function):
     """Fused head, optionally with the soft-argmax decode riding along (``decode = (ds, temperature)``).
 
-    Forward: bf16 tensor-core head for bf16 features (one- or two-deconv heads inside its tiling), the fp32 (3xTF32
-    tensor-core) kernels otherwise (+ decode kernel).  Backward: native in both cases.  On the tensor-core path the gradient
+    Forward: bf16 tensor-core head for bf16 features and, when no backward follows, fp16 tensor-core head for fp16
+    features (one- or two-deconv heads inside its tiling), the fp32 (3xTF32 tensor-core) kernels otherwise (+ decode
+    kernel).  Backward: native in both cases.  On the tensor-core path the gradient
     w.r.t. the heatmaps is never materialised for the decode branch: the sparse decode windows, a dense heatmap-loss
     gradient if there is one, and the softmax backward are all folded into the kernel that writes the
     deconv-gradient operand.  Outputs: heatmaps [, keypoints (B, 2K), confidences (B, K)].
@@ -83,9 +84,11 @@ class _HeadFunction(torch.autograd.Function):
         n = len(params) // 2
         weights, biases = list(params[:n]), list(params[n:])
         saved = acts = None
-        if features.dtype == torch.bfloat16 and features.is_cuda and ops.head_bf16_supported(
-                tuple(features.shape), [w.shape[1] for w in weights], train=train):
-            res = ops._head_forward_bf16(features.contiguous(), weights, biases, final_softmax, train=train)
+        # fp16 features take the tensor cores for inference only (autocast(float16) in the reference); with a backward
+        # to follow they take the fp32 kernels, which train
+        sixteen = features.dtype == torch.bfloat16 or (features.dtype == torch.float16 and not train)
+        if sixteen and features.is_cuda and ops.head_bf16_supported(tuple(features.shape), [w.shape[1] for w in weights], train=train):
+            res = ops._head_forward_16(features.contiguous(), weights, biases, final_softmax, train=train)
             out, saved = res if train else (res, None)
         elif train:
             out, acts = ops.head_forward_f32(features, weights, biases, final_softmax, keep_activations=True)

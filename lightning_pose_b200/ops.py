@@ -219,12 +219,18 @@ def head_bf16_supported(shape, channels, train: bool) -> bool:
     return not train or lib.lpb_head_bwd_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)) == 0
 
 
-def _head_forward_bf16(f, weights, biases, final_softmax, train=False, want_hints=False):
-    """tensor-core path (one- or two-deconv heads); the caller checks ``head_bf16_supported`` first.
+def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=False):
+    """tensor-core path (one- or two-deconv heads) on 16-bit features: bf16 (``lpb_head_fwd_bf16``) or fp16
+    (``lpb_head_fwd_f16``), the weights rounded to the features' dtype on the device; the caller checks
+    ``head_bf16_supported`` first.  Both share the plan and the buffer sizes.
 
-    ``train=True`` returns ``(out, saved)`` where ``saved`` carries what ``head_backward_bf16`` needs
-    (the row-layout copy of the shuffled features and the forward workspace with the inter-layer activations).
+    ``train=True`` (bf16 only: there is no fp16 backward) returns ``(out, saved)`` where ``saved`` carries what
+    ``head_backward_bf16`` needs (the row-layout copy of the shuffled features and the forward workspace with the
+    inter-layer activations).
     """
+    entry = _HEAD_FWD_16.get(f.dtype)
+    if entry is None or (train and f.dtype != torch.bfloat16):
+        raise ValueError(f"the 16-bit head takes bf16 or (forward only) fp16 features; got {f.dtype}{' for training' if train else ''}")
     b, c, h, w = f.shape
     n = len(weights)
     w1 = _cuda_f32(weights[0], "weight")
@@ -244,12 +250,16 @@ def _head_forward_bf16(f, weights, biases, final_softmax, train=False, want_hint
         check(lib.lpb_head_bf16_saved_bytes(b, c, h, w, C.byref(nbytes)))
         xs = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
     with torch.cuda.device(f.device):
-        check(lib.lpb_head_fwd_bf16(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), _ptr(out), _ptr(xs), _ptr(ws), _stream()))
+        check(entry(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), _ptr(out), _ptr(xs), _ptr(ws), _stream()))
     if want_hints:  # kept for bench.py's call, which unpacks a decode-hints slot (always None)
         return (out, (xs, ws), None) if train else (out, None)
     if train:
         return out, (xs, ws)
     return out
+
+
+_HEAD_FWD_16 = {torch.bfloat16: lib.lpb_head_fwd_bf16, torch.float16: lib.lpb_head_fwd_f16}
+_head_forward_bf16 = _head_forward_16  # the name bench.py and the bf16 tests call
 
 
 def decode_backward_windows(heatmaps, stats, grad_xy, ds, temperature):
@@ -352,18 +362,18 @@ def head_forward_f32(features, weights, biases, final_softmax=True, keep_activat
 def head_forward(features, weights, biases, final_softmax=True):
     """PixelShuffle(2) + ConvTranspose2d stack + spatial softmax; forward only.
 
-    bf16 features take the bf16 tensor-core kernels (fp32 accumulate, fp32 heatmaps) when the head is a one- or
-    two-deconv head the tiling covers; everything else takes the full-precision kernels (3xTF32 on the tensor cores,
-    any depth and keypoint count).  Training uses
+    bf16 and fp16 features take the 16-bit tensor-core kernels (operands in the features' dtype, fp32 accumulate, fp32
+    heatmaps) when the head is a one- or two-deconv head the tiling covers; everything else takes the full-precision
+    kernels (3xTF32 on the tensor cores, any depth and keypoint count).  Training uses
     ``HeatmapHead`` which adds the backward.
     """
     if not isinstance(features, torch.Tensor) or not features.is_cuda:
         raise RuntimeError("lpb200: `features` must be a CUDA tensor (this package has no CPU fallback)")
     if len(weights) < 1:
         raise ValueError("head needs at least one deconv layer")
-    if features.dtype == torch.bfloat16 and all(b is not None for b in biases) and head_bf16_supported(
+    if features.dtype in _HEAD_FWD_16 and all(b is not None for b in biases) and head_bf16_supported(
             tuple(features.shape), [w.shape[1] for w in weights], train=False):
-        return _head_forward_bf16(features.contiguous(), weights, biases, final_softmax)
+        return _head_forward_16(features.contiguous(), weights, biases, final_softmax)
     return head_forward_f32(features, weights, biases, final_softmax)
 
 
@@ -512,22 +522,31 @@ def context_gather(seq: torch.Tensor, context_length: int = 5) -> torch.Tensor:
 IMAGENET_MEAN = (0.485, 0.456, 0.406)  # lightning_pose/data/__init__.py (_IMAGENET_MEAN / _IMAGENET_STD)
 IMAGENET_STD = (0.229, 0.224, 0.225)
 
+# output-format codes of the ingest entries (LPB_OUT_F32 / LPB_OUT_BF16 / LPB_OUT_F16, include/lpb200.h)
+_OUT_FORMATS = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+
+
+def _out_format(dtype) -> int:
+    if dtype not in _OUT_FORMATS:
+        raise ValueError("dtype must be float32, bfloat16 or float16")
+    return _OUT_FORMATS[dtype]
+
 
 def frames_normalize(frames_u8, size=None, mean=IMAGENET_MEAN, std=IMAGENET_STD, channels_last=False, dtype=torch.float32):
-    """uint8 (F, H, W, 3) decoded RGB frames -> normalised (F, 3, h, w) [or (F, h, w, 3)] fp32 / bf16 in one pass."""
+    """uint8 (F, H, W, 3) decoded RGB frames -> normalised (F, 3, h, w) [or (F, h, w, 3)] fp32 / bf16 / fp16 in one pass
+    (bf16 and fp16 are the fp32 result rounded to nearest even)."""
     if not isinstance(frames_u8, torch.Tensor) or not frames_u8.is_cuda:
         raise RuntimeError("lpb200: `frames` must be a CUDA tensor (this package has no CPU fallback)")
     if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[-1] != 3:
         raise ValueError(f"frames must be uint8 (F, H, W, 3); got {tuple(frames_u8.shape)} {frames_u8.dtype}")
-    if dtype not in (torch.float32, torch.bfloat16):
-        raise ValueError("dtype must be float32 or bfloat16")
+    fmt = _out_format(dtype)
     x = frames_u8.contiguous()
     f, h, w, _ = x.shape
     oh, ow = (int(size[0]), int(size[1])) if size is not None else (h, w)
     out = torch.empty((f, oh, ow, 3) if channels_last else (f, 3, oh, ow), device=x.device, dtype=dtype)
     m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
     with torch.cuda.device(x.device):
-        check(lib.lpb_frames_normalize(_ptr(x), f, h, w, oh, ow, m3, s3, int(bool(channels_last)), int(dtype == torch.bfloat16), _ptr(out), _stream()))
+        check(lib.lpb_frames_normalize(_ptr(x), f, h, w, oh, ow, m3, s3, int(bool(channels_last)), fmt, _ptr(out), _stream()))
     return out
 
 
@@ -536,7 +555,7 @@ INGEST_MAX_VIEWS = 16  # LPB_INGEST_MAX_VIEWS (include/lpb200.h)
 
 def frames_normalize_views(views_u8, size, mean=IMAGENET_MEAN, std=IMAGENET_STD, channels_last=False, dtype=torch.float32):
     """V synchronised views, uint8 (F, H_v, W_v, 3) each (sizes may differ), -> normalised (F, V, 3, h, w) [or
-    (F, V, h, w, 3)] fp32 / bf16 in one launch; view v of frame f is bit-identical to ``frames_normalize`` of that view.
+    (F, V, h, w, 3)] fp32 / bf16 / fp16 in one launch; view v of frame f is bit-identical to ``frames_normalize`` of that view.
     ``reshape(F * V, ...)`` is the frame-major, view-minor batch of the multi-view trackers."""
     views = list(views_u8)
     if not 1 <= len(views) <= INGEST_MAX_VIEWS:
@@ -551,8 +570,7 @@ def frames_normalize_views(views_u8, size, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     f = views[0].shape[0]
     if any(v.shape[0] != f for v in views):
         raise ValueError(f"all views must have the same frame count; got {[v.shape[0] for v in views]}")
-    if dtype not in (torch.float32, torch.bfloat16):
-        raise ValueError("dtype must be float32 or bfloat16")
+    fmt = _out_format(dtype)
     xs = [v.contiguous() for v in views]
     n = len(xs)
     oh, ow = int(size[0]), int(size[1])
@@ -561,7 +579,7 @@ def frames_normalize_views(views_u8, size, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     hs, ws = (C.c_int * n)(*[x.shape[1] for x in xs]), (C.c_int * n)(*[x.shape[2] for x in xs])
     m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
     with torch.cuda.device(xs[0].device):
-        check(lib.lpb_frames_normalize_views(ptrs, n, f, hs, ws, oh, ow, m3, s3, int(bool(channels_last)), int(dtype == torch.bfloat16),
+        check(lib.lpb_frames_normalize_views(ptrs, n, f, hs, ws, oh, ow, m3, s3, int(bool(channels_last)), fmt,
                                              _ptr(out), _stream()))
     return out
 
@@ -646,8 +664,7 @@ def frames_crop_normalize(frames, bboxes, size, cursor=None, row0: int = 0, mean
         f, _, h, w = frames.shape
     else:
         raise ValueError(f"frames must be uint8 (F, H, W, 3) or float32 (F, 3, H, W); got {tuple(frames.shape)} {frames.dtype}")
-    if dtype not in (torch.float32, torch.bfloat16):
-        raise ValueError("dtype must be float32 or bfloat16")
+    fmt = _out_format(dtype)
     if int(row0) < 0:
         raise ValueError(f"row0 must be >= 0; got {row0}")
     b = _bbox_table(bboxes, "bboxes")
@@ -660,7 +677,7 @@ def frames_crop_normalize(frames, bboxes, size, cursor=None, row0: int = 0, mean
     m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
     with torch.cuda.device(x.device):
         check(lib.lpb_frames_crop_normalize(_ptr(x), in_f32, f, h, w, _ptr(b), b.shape[0], _ptr(cursor), int(row0), oh, ow, m3, s3,
-                                            int(bool(channels_last)), int(dtype == torch.bfloat16), _ptr(out), _ptr(boxes_out), _stream()))
+                                            int(bool(channels_last)), fmt, _ptr(out), _ptr(boxes_out), _stream()))
     return out, boxes_out
 
 

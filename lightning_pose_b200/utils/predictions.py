@@ -180,7 +180,9 @@ class BatchedPredictor:
     ``data/video/dali.py:332-380``): with ``bboxes``, the video's (N, 4) device table (``compute_bboxes`` /
     ``smooth_bboxes``), and ``frame_hw``, uint8 (T, H, W, 3) full frames and no ``bbox``.  One launch inside the chunk
     crops each frame to its row at the cursor (rows past the end repeat the last) and resizes it; the clamped boxes it
-    writes map the keypoints back.  Both ingests write ``crop_dtype``, channels-last if ``crop_channels_last``.
+    writes map the keypoints back.  Both ingests write ``crop_dtype`` (float32, bfloat16 or float16), channels-last if
+    ``crop_channels_last``.  Features of the backbone's dtype pick the head's kernels: bf16, and fp16 (the reference's
+    ``precision="fp16"``, ``torch.autocast(float16)``) run on the 16-bit tensor-core head, fp32 on the 3xTF32 one.
 
     The body runs ``sub_chunk`` frames at a time.  Frame body (``HeatmapHead``; for V > 1 the multi-view transformer's,
     ``features_of=model.forward_vit``, or a tracker's that folds views into the batch): head -> decode -> remap ->
