@@ -284,6 +284,34 @@ int lpb_frames_augment_normalize(const uint8_t* frames_u8, int F, int H, int W, 
                                  const int64_t* seed, const float* mean3, const float* std3, int layout, int out_bf16,
                                  void* out, float* transform_out, void* stream);
 
+/* ---- curriculum patch masking of multi-view transformer training ----------------------------------------------
+ * replaces PatchMasker.apply_patch_masking  lightning_pose/callbacks.py:303-401  (the PatchMasking callback's
+ * on_train_batch_start, :222-263).  Images (B, V, C, H, W) are cut into LPB_PATCH_SIZE x LPB_PATCH_SIZE patches,
+ * P = (H / 16) * (W / 16) per view (integer division), patch p = (y / 16) * (W / 16) + x / 16; the H % 16 bottom rows
+ * and W % 16 right columns belong to no patch and are never masked, as in the reference.
+ *
+ * lpb_patch_mask_select: one CTA per (example, view).  step: DEVICE int64, read at run time (a captured graph replays
+ * with an advancing step).  The curriculum of callbacks.py:344-357, in fp64 without contractions, so that it equals
+ * Python's float64 result bit for bit:
+ *   ratio = 0 for step < init_step, else init_ratio + min((step - init_step) / (final_step - init_step), 1)
+ *           * (final_ratio - init_ratio);   m = clamp(int(ratio * P), 0, P)  (int() truncates toward zero).
+ * Each view masks exactly m of its P patches, a uniformly random subset: patch p gets a 52-bit Philox4x32-10 key,
+ * keyed by patch_seed and counted by (p, view, example, step); the m smallest keys (ties by patch index) are masked.
+ * The same (patch_seed, step, example, view) gives the same patches; this is not the reference's torch.randperm draw.
+ * mask [B, V, P] fp32: 1 = kept, 0 = masked (the reference's patch_mask).  Requires final_step > init_step,
+ * P <= LPB_PATCH_MAX, V <= 65535.  P = 0 or B * V = 0 is a no-op.
+ *
+ * lpb_patch_mask_apply: out[b, v, c, y, x] = mask[b, v, p(y, x)] != 0 ? images[b, v, c, y, x] : 0 for pixels inside a
+ * patch, images[...] elsewhere; bits are copied, not converted.  images, out: contiguous [B, V, C, H, W] in the element
+ * type of in_format, LPB_OUT_F32 or LPB_OUT_BF16 (anything else is LPB_ERR_INVALID); out must not alias images (the
+ * reference clones).  Accesses are 16 bytes wide where the row length and both pointers allow it. */
+#define LPB_PATCH_SIZE 16
+#define LPB_PATCH_MAX 4096
+int lpb_patch_mask_select(const int64_t* step, int B, int V, int H, int W, int64_t patch_seed, int64_t init_step,
+                          int64_t final_step, double init_ratio, double final_ratio, float* mask, void* stream);
+int lpb_patch_mask_apply(const void* images, int B, int V, int C, int H, int W, int in_format, const float* mask, void* out,
+                         void* stream);
+
 /* ---- crop-zoom inference (bbox mode of the video-ingest boundary) ------------------------------------------------
  * replaces crop_and_resize_frames  lightning_pose/data/bboxes.py:291-343  and the bbox-row slicing in front of it
  *   lightning_pose/data/video/dali.py:332-380, lightning_pose/data/video/pynvvc.py:266-283

@@ -70,7 +70,9 @@ SIGNATURES = {
     "lpb_frames_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
     "lpb_frames_normalize_views": (C.c_int, [C.POINTER(_P), _I, _I, C.POINTER(_I), C.POINTER(_I), _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
     "lpb_frames_augment_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
-    "lpb_frames_crop_normalize": (C.c_int, [_P, _I, _I, _I, _I, _P, _L, _P, _L, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
+    "lpb_patch_mask_select": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _L, C.c_double, C.c_double, _P, _P]),
+    "lpb_patch_mask_apply": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "lpb_frames_crop_normalize":(C.c_int, [_P, _I, _I, _I, _I, _P, _L, _P, _L, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
     "lpb_bboxes_from_keypoints": (C.c_int, [_P, _L, _I, _L, _I, C.POINTER(C.c_int32), _I, C.c_double, _I, _I, _P, _P]),
     "lpb_bboxes_rolling_median": (C.c_int, [_P, _L, _I, _P, _P]),
     "lpb_pack_predictions": (C.c_int, [_P, _P, _I, _I, _P, _L, _P, _L, _P]),

@@ -134,18 +134,6 @@ struct AugmentParams {
   float ry, rx;
 };
 
-// Philox4x32-10 (Salmon et al., SC'11): a counter-based generator, so a draw depends only on (key, counter).
-__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t lo0 = 0xD2511F53u * ctr.x, hi0 = __umulhi(0xD2511F53u, ctr.x);
-    const uint32_t lo1 = 0xCD9E8D57u * ctr.z, hi1 = __umulhi(0xCD9E8D57u, ctr.z);
-    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
-    key.x += 0x9E3779B9u, key.y += 0xBB67AE85u;
-  }
-  return ctr;
-}
-
 __device__ __forceinline__ float open_uniform(uint32_t r) { return ((float)(r >> 8) + 0.5f) * (1.0f / 16777216.0f); }  // (0, 1)
 
 // log k! for k < 16; above, Stirling's series to 1 / (360 k^3) (truncation error < 1e-12 at k = 16).

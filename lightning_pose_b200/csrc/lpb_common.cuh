@@ -80,6 +80,19 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
+// Philox4x32-10 (Salmon et al., SC'11): a counter-based generator, so a draw depends only on (key, counter).
+// Shared by the augmented ingest's shot noise (ingest.cu) and the patch-masking selection (patchmask.cu).
+__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t lo0 = 0xD2511F53u * ctr.x, hi0 = __umulhi(0xD2511F53u, ctr.x);
+    const uint32_t lo1 = 0xCD9E8D57u * ctr.z, hi1 = __umulhi(0xCD9E8D57u, ctr.z);
+    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
+    key.x += 0x9E3779B9u, key.y += 0xBB67AE85u;
+  }
+  return ctr;
+}
+
 // ---- fp32 pairs -------------------------------------------------------------------------------------
 // Code written against pairs of fp32 values (two positions per thread).  sm_90 has no packed fp32 instructions, so each
 // pair operation is two scalar IEEE fp32 operations: the same roundings a packed form would give.

@@ -13,6 +13,12 @@ kernels), the fold, and the loss inputs.  Calibrated batches (``keypoints_3d`` p
 distortions) also get the 3-D entries the pairwise-projection and reprojection losses read (:263-303), computed by the
 camera kernels without a host sync; uncalibrated batches get ``None`` there, as in the reference (:300-303).  Unlike
 the reference, malformed camera inputs raise instead of being logged and turned into ``None``.
+
+Training with curriculum patch masking (the reference's ``PatchMasking`` callback, ``callbacks.py:199-276``): pass a
+``PatchMasker`` as ``patch_masker``; ``training_step`` then masks ``batch_dict["images"]`` at the step held by the device
+counter ``global_step`` (0 at construction, one more after every ``training_step``, as Lightning's ``global_step``
+advances once per optimizer step) and stores the mask in ``current_patch_mask``.  The step never leaves the device, so
+a training step captured into a CUDA graph masks with a fresh step on every replay.
 """
 from __future__ import annotations
 
@@ -23,6 +29,7 @@ import torch
 from torch import nn
 
 from lightning_pose_b200 import ops
+from lightning_pose_b200.callbacks import PatchMasker
 from lightning_pose_b200.data.bboxes import model_to_frame_batch
 from lightning_pose_b200.data.cameras import project_camera_pairs_to_3d
 from lightning_pose_b200.losses.factory import LossFactory
@@ -50,10 +57,15 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         backbone_arch: str = "vits_dino",
         downsample_factor: Literal[1, 2, 3] = 2,
         torch_seed: int = 123,
+        patch_masker: PatchMasker | None = None,
         **kwargs: Any,
     ) -> None:
         super().__init__()
         torch.manual_seed(torch_seed)
+        self.patch_masker = patch_masker
+        self.current_patch_mask: torch.Tensor | None = None
+        # training steps taken (Lightning's global_step), on the device; not part of the state dict
+        self.register_buffer("global_step", torch.zeros(1, dtype=torch.int64), persistent=False)
         self.num_keypoints, self.num_views, self.downsample_factor = num_keypoints, num_views, downsample_factor
         self.num_fc_input_features = embedding_dim
         self.patch_embed, self.encoder = patch_embed, encoder
@@ -133,3 +145,31 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         loss, self.last_logs = self.loss_factory(stage=stage, anneal_weight=anneal_weight, **data_dict)
         self.last_rmse, _ = self.rmse_loss(stage=stage, **data_dict)
         return loss
+
+    def training_step(self, batch_dict: dict, batch_idx: int) -> dict[str, torch.Tensor]:
+        """One labeled training step: patch masking (with an enabled ``patch_masker``), forward, the supervised losses (the
+        3-D ones on calibrated batches), then ``global_step`` + 1.
+
+        The loss is ``evaluate_labeled``'s total, the sum over the loss factory of weight * loss in its order, computed
+        without the host: each weight is made on the device by a fill kernel instead of copied from the host, and the
+        RMSE diagnostic (a host-synchronising NaN filter) is left to ``evaluate_labeled``.  So the whole step captures
+        into one CUDA graph.  ``last_logs`` holds detached values (what Lightning's ``log`` keeps): a step's autograd
+        graph must not outlive it, or the next step's backward would meet the previous step's gradient nodes, whose
+        stream may be another than the one being captured."""
+        masker = self.patch_masker
+        if masker is not None and masker.use_patch_masking:  # PatchMasking.on_train_batch_start (callbacks.py:222-263)
+            batch_dict["images"], self.current_patch_mask = masker.apply_patch_masking(
+                batch_dict["images"], training_step=self.global_step, is_training=True)
+        data_dict = self.get_loss_inputs_labeled(batch_dict)
+        assert self.loss_factory is not None
+        total: torch.Tensor | None = None
+        logs: list[dict] = []
+        for name, inst in self.loss_factory.loss_instance_dict.items():
+            value, entries = inst(stage="train", **data_dict)
+            weighted = torch.full((), float(inst.weight), device=value.device) * value
+            total = weighted if total is None else total + weighted
+            logs += [{**e, "value": e["value"].detach()} if isinstance(e["value"], torch.Tensor) else e for e in entries]
+            logs.append({"name": f"train_{name}_loss_weighted", "value": weighted.detach()})
+        self.last_logs = logs
+        self.global_step.add_(1)
+        return {"loss": total}

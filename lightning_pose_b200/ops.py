@@ -640,6 +640,60 @@ def frames_augment_normalize(frames_u8, size, params, seed, mean=IMAGENET_MEAN, 
     return out, transform_out.view(2, 3)
 
 
+# curriculum patch masking (lpb_patch_mask_*, include/lpb200.h)
+PATCH_SIZE = 16  # LPB_PATCH_SIZE
+PATCH_MAX = 4096  # LPB_PATCH_MAX: patches per view
+
+
+def _patch_images(images) -> tuple[int, int, int, int, int]:
+    """Checks the (B, V, C, H, W) batch of the patch-masking entries; returns its shape."""
+    if not isinstance(images, torch.Tensor) or not images.is_cuda:
+        raise RuntimeError("lpb200: `images` must be a CUDA tensor (this package has no CPU fallback)")
+    if images.dim() != 5:
+        raise ValueError(f"images must be (batch, views, channels, height, width); got {tuple(images.shape)}")
+    if images.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"images must be float32 or bfloat16; got {images.dtype}")
+    if not images.is_contiguous():
+        raise ValueError("images must be contiguous")
+    b, v, c, h, w = images.shape
+    if (h // PATCH_SIZE) * (w // PATCH_SIZE) > PATCH_MAX:
+        raise ValueError(f"{h} x {w} images have {(h // PATCH_SIZE) * (w // PATCH_SIZE)} patches of {PATCH_SIZE} x {PATCH_SIZE} "
+                         f"per view; at most {PATCH_MAX}")
+    return b, v, c, h, w
+
+
+def patch_mask_select(images, step, patch_seed: int, init_step: int, final_step: int, init_ratio: float, final_ratio: float):
+    """The patch mask of one training step, drawn on the device: (B, V, P) fp32, 1 = kept, 0 = masked.
+
+    ``images``: (B, V, C, H, W) fp32 / bf16 CUDA batch (only its shape is read); ``step``: one-element int64 tensor on its
+    device, read by the kernel (so a captured graph replays with the step it holds).  Each view masks exactly
+    int(ratio(step) * P) of its P 16 x 16 patches, a uniformly random subset fixed by (patch_seed, step, example, view)."""
+    b, v, _, h, w = _patch_images(images)
+    if not isinstance(step, torch.Tensor) or step.device != images.device or step.dtype != torch.int64 or step.numel() != 1:
+        raise ValueError("step must be a one-element int64 tensor on the images' device")
+    p = (h // PATCH_SIZE) * (w // PATCH_SIZE)
+    mask = torch.empty((b, v, p), device=images.device, dtype=torch.float32)
+    seed = (int(patch_seed) + 2**63) % 2**64 - 2**63  # any integer, as torch.Generator.manual_seed takes it, to int64
+    with torch.cuda.device(images.device):
+        check(lib.lpb_patch_mask_select(_ptr(step.contiguous()), b, v, h, w, seed, int(init_step), int(final_step), float(init_ratio),
+                                        float(final_ratio), _ptr(mask), _stream()))
+    return mask
+
+
+def patch_mask_apply(images, mask):
+    """``images`` with every patch whose ``mask`` entry is 0 set to zero, out of place; the rows and columns past the last
+    whole patch are kept.  ``mask``: (B, V, P) fp32 on the images' device."""
+    b, v, c, h, w = _patch_images(images)
+    p = (h // PATCH_SIZE) * (w // PATCH_SIZE)
+    if not isinstance(mask, torch.Tensor) or mask.device != images.device or mask.dtype != torch.float32 or tuple(mask.shape) != (b, v, p):
+        raise ValueError(f"mask must be a float32 ({b}, {v}, {p}) tensor on the images' device")
+    m = mask.contiguous()
+    out = torch.empty_like(images)
+    with torch.cuda.device(images.device):
+        check(lib.lpb_patch_mask_apply(_ptr(images), b, v, c, h, w, _OUT_FORMATS[images.dtype], _ptr(m), _ptr(out), _stream()))
+    return out
+
+
 def _bbox_table(bboxes, name: str) -> torch.Tensor:
     b = _cuda_f32(bboxes, name)
     if b.dim() != 2 or b.shape[1] != 4 or b.shape[0] < 1:
