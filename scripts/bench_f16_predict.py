@@ -110,7 +110,7 @@ def main():
         d1.weight.copy_(w1), d1.bias.copy_(b1), d2.weight.copy_(w2), d2.bias.copy_(b2)
     head = head.to(dev).eval().requires_grad_(False)
     feats = prob["feats"].to(dev)
-    ref = S.head_ref_chunked(feats, [w1.to(dev), w2.to(dev)], [b1.to(dev), b2.to(dev)], softmax=True, bf16_operands=False)
+    ref = S.head_ref_chunked(feats, [w1.to(dev), w2.to(dev)], [b1.to(dev), b2.to(dev)], softmax=True, operands=None)
     kp_ref, cf_ref, _, _ = S.decode_ref(ref, 2)
     conf = (cf_ref > 0.5).flatten().cpu().numpy()
     acc = {"workload": f"config 2: {feats.shape[0]} frames of make_problem(regime='trained'), K = {bench.K_PTS}, image {bench.IMG} px",

@@ -107,17 +107,19 @@ def decode_grad_ref(hm: torch.Tensor, ds: int, temperature: float, grad_xy: torc
 # ------------------------------------------------------------------------------------------------
 # heatmap head
 # ------------------------------------------------------------------------------------------------
-def bf16_round(t: torch.Tensor) -> torch.Tensor:
-    """t rounded to bf16 (round to nearest even, from its float32 value), straight-through for autograd."""
-    return t + (t.detach().float().bfloat16().to(t.dtype) - t.detach())
+def operand_round(t: torch.Tensor, dtype) -> torch.Tensor:
+    """t rounded to the 16-bit ``dtype`` (round to nearest even, from its float32 value), straight-through for autograd."""
+    return t + (t.detach().float().to(dtype).to(t.dtype) - t.detach())
 
 
-def head_ref(feats: torch.Tensor, weights, biases, softmax: bool = True, bf16_operands: bool = True, mids: list | None = None):
+def head_ref(feats: torch.Tensor, weights, biases, softmax: bool = True, operands=torch.bfloat16, mids: list | None = None):
     """PixelShuffle(2) + ConvTranspose2d(k3, s2, p1, op1) per layer [+ spatial softmax], float64, on feats' device.
 
-    ``bf16_operands``: weights and the inputs of layers after the first are rounded to bf16 where the tensor-core kernels
-    round them (the features are taken as given).  Differentiable in every input.  ``mids``: if a list, the input of
-    every layer after the first is appended to it (with ``retain_grad``)."""
+    ``operands`` (None, ``torch.bfloat16`` or ``torch.float16``): the weights and the inputs of layers after the first are
+    rounded to that dtype where the tensor-core kernels round them (the features are taken as given).  The fp16 route
+    also rounds the biases of layers after the first, which ride on the constant-one channel as fp16 operands; the bf16
+    reference leaves them unrounded.  Differentiable in every input.  ``mids``: if a list, the input of every layer after
+    the first is appended to it (with ``retain_grad``)."""
     x = F.pixel_shuffle(feats.to(F64), 2)
     for i, (w, b) in enumerate(zip(weights, biases)):
         w = w.to(device=x.device, dtype=F64)
@@ -126,26 +128,28 @@ def head_ref(feats: torch.Tensor, weights, biases, softmax: bool = True, bf16_op
             if mids is not None:
                 x.retain_grad()
                 mids.append(x)
-            if bf16_operands:
-                x = bf16_round(x)
-        x = F.conv_transpose2d(x, bf16_round(w) if bf16_operands else w, b, stride=2, padding=1, output_padding=1)
+            if operands is not None:
+                x = operand_round(x, operands)
+            if operands == torch.float16:
+                b = operand_round(b, operands)
+        x = F.conv_transpose2d(x, w if operands is None else operand_round(w, operands), b, stride=2, padding=1, output_padding=1)
     if softmax:
         n, c, hh, ww = x.shape
         x = torch.softmax(x.reshape(n, c, -1), -1).reshape(n, c, hh, ww)
     return x
 
 
-def head_ref_chunked(feats: torch.Tensor, weights, biases, softmax: bool = True, bf16_operands: bool = True) -> torch.Tensor:
+def head_ref_chunked(feats: torch.Tensor, weights, biases, softmax: bool = True, operands=torch.bfloat16) -> torch.Tensor:
     """``head_ref`` without autograd, frame chunk by frame chunk."""
     out = []
     step = _chunk(feats[0].numel() * 8)
     with torch.no_grad():
         for i in range(0, feats.shape[0], step):
-            out.append(head_ref(feats[i : i + step], weights, biases, softmax, bf16_operands))
+            out.append(head_ref(feats[i : i + step], weights, biases, softmax, operands))
     return torch.cat(out)
 
 
-def head_grad_ref(feats, weights, biases, grad_out, softmax: bool = True, bf16_operands: bool = True, want_mid_grad=False):
+def head_grad_ref(feats, weights, biases, grad_out, softmax: bool = True, operands=torch.bfloat16, want_mid_grad=False):
     """float64 autograd of sum(head_ref(...) * grad_out), frame chunk by frame chunk.
 
     Returns (dfeat, [dw], [db][, per-channel L2 norm of d(input of the last layer)] )."""
@@ -157,7 +161,7 @@ def head_grad_ref(feats, weights, biases, grad_out, softmax: bool = True, bf16_o
     for i in range(0, feats.shape[0], step):
         f = feats[i : i + step].detach().to(F64).requires_grad_(True)
         mids: list = []
-        y = head_ref(f, ws, bs, softmax, bf16_operands, mids=mids if want_mid_grad else None)
+        y = head_ref(f, ws, bs, softmax, operands, mids=mids if want_mid_grad else None)
         (y * grad_out[i : i + step].to(F64)).sum().backward()
         dfeat[i : i + step] = f.grad
         if want_mid_grad:

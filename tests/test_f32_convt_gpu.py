@@ -6,9 +6,7 @@ import torch
 import torch.nn.functional as F
 
 import scale_oracle as S
-from test_head_shapes_gpu import _ref_grads, check_grads_f32
-
-F64 = torch.float64
+from head_support import F64, WORST, check_grads_f32, features, gen, head_params, make_head, ref_grads, report_headroom
 COUT = [1, 8, 17, 20, 21, 28, 29, 51, 64, 81, 128]
 CIN = [1, 3, 17, 51, 512]
 SIZES = [(1, 1), (3, 5), (6, 8), (16, 24), (48, 48), (4, 300)]
@@ -24,8 +22,11 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
+@pytest.fixture(scope="module", autouse=True)
+def _report_headroom():
+    WORST.clear()
+    yield
+    report_headroom()
 
 
 def _layer_ref(x, w, bias, shuffle):
@@ -40,9 +41,9 @@ def test_layer_against_float64(dev, cout, cin, hw, shuffle):
 
     hi, wi = hw
     b = 2
-    x = torch.randn((b, 4 * cin, hi // 2, wi // 2) if shuffle else (b, cin, hi, wi), device=dev, generator=_gen(cout * 131 + cin))
-    w = torch.randn(cin, cout, 3, 3, device=dev, generator=_gen(3)) / (cin * 2.25) ** 0.5
-    bias = torch.randn(cout, device=dev, generator=_gen(4))
+    x = torch.randn((b, 4 * cin, hi // 2, wi // 2) if shuffle else (b, cin, hi, wi), device=dev, generator=gen(cout * 131 + cin))
+    w = torch.randn(cin, cout, 3, 3, device=dev, generator=gen(3)) / (cin * 2.25) ** 0.5
+    bias = torch.randn(cout, device=dev, generator=gen(4))
     case = f"Cout={cout} Cin={cin} {hi}x{wi} shuffle={shuffle}"
 
     out = ops.convt_forward_f32(x, w, bias, shuffle)
@@ -53,31 +54,13 @@ def test_layer_against_float64(dev, cout, cin, hw, shuffle):
     ratio = float(((out.to(F64) - ref.detach()).abs() / (1e-5 * scale + 1e-30)).max())
     assert ratio < 1.0, (case, "forward", ratio)
 
-    g = torch.randn(ref.shape, device=dev, generator=_gen(5))
+    g = torch.randn(ref.shape, device=dev, generator=gen(5))
     dx, dw, db = ops.convt_backward_f32(x, g, w, shuffle)
     (ref * g.to(F64)).sum().backward()
     fscale = x64.grad.abs().flatten(1).amax(1).view(-1, *([1] * (x.dim() - 1)))
     ratio = float(((dx.to(F64) - x64.grad).abs() / (1e-5 * fscale + 1e-30)).max())
     assert ratio < 1.0, (case, "d input", ratio)
     check_grads_f32({"dw1": dw, "db1": db}, {"dw1": w64.grad, "db1": b64.grad}, {"db1": g.to(F64).pow(2).sum((0, 2, 3)).sqrt()}, case)
-
-
-def _head(c, ch, seed):
-    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
-
-    torch.manual_seed(seed)
-    head = HeatmapHead("resnet50", c, ch[1], deconv_out_channels=ch[0]) if len(ch) == 2 else HeatmapHead("vits_dino", c, ch[0])
-    deconvs = list(head.upsampling_layers)[1:]
-    assert [d.weight.shape[1] for d in deconvs] == list(ch)
-    for layer in deconvs:
-        torch.nn.init.xavier_uniform_(layer.weight, gain=3.0)
-        torch.nn.init.uniform_(layer.bias, -0.3, 0.3)
-    return head.cuda()
-
-
-def _params(head):
-    deconvs = list(head.upsampling_layers)[1:]
-    return deconvs, [d.weight.detach() for d in deconvs], [d.bias.detach() for d in deconvs]
 
 
 HEADS = {
@@ -95,22 +78,22 @@ def test_head_fp32_features_train(dev, name):
     from lightning_pose_b200 import ops
 
     (b, c, h, w), ch = HEADS[name]
-    head = _head(c, ch, seed=31)
-    deconvs, ws, bs = _params(head)
-    feats = torch.randn(b, c, h, w, device=dev, generator=_gen(9)) * 0.5
+    head = make_head(c, ch, seed=31)
+    deconvs, (ws, bs) = list(head.upsampling_layers)[1:], head_params(head)
+    feats = features(b, c, h, w, 9, torch.float32)
     f = feats.clone().requires_grad_(True)
     hm, kp, _ = head.forward_with_keypoints(f)
-    hm_ref = S.head_ref_chunked(feats, ws, bs, softmax=True, bf16_operands=False)
+    hm_ref = S.head_ref_chunked(feats, ws, bs, softmax=True, operands=None)
     err = (hm.detach().to(F64) - hm_ref).abs()
     assert bool((err <= 1e-4 * hm_ref + 1e-9).all()), (name, float((err / (1e-4 * hm_ref + 1e-9)).max()))
 
-    g_dense = torch.randn(hm.shape, device=dev, generator=_gen(10))
-    g_kp = torch.randn(kp.shape, device=dev, generator=_gen(11))
+    g_dense = torch.randn(hm.shape, device=dev, generator=gen(10))
+    g_kp = torch.randn(kp.shape, device=dev, generator=gen(11))
     ((hm * g_dense).sum() + (kp * g_kp).sum()).backward()
     k = hm.shape[1]
     _, _, stats = ops._decode_fwd(hm.detach(), 2, 1000.0)
     g_hm = g_dense + ops._decode_bwd(hm.detach(), stats, g_kp.reshape(b, k, 2).contiguous(), 2, 1000.0)
-    ref, gnorm = _ref_grads(feats, ws, bs, g_hm, True, hm_ref, bf16_operands=False)
+    ref, gnorm = ref_grads(feats, ws, bs, g_hm, True, hm_ref, operands=None)
     fscale = ref["dfeat"].abs().flatten(1).amax(1).view(-1, 1, 1, 1)
     ratio = float(((f.grad.to(F64) - ref["dfeat"]).abs() / (1e-4 * fscale + 1e-30)).max())
     assert ratio < 1.0, (name, "d features", ratio)
@@ -125,17 +108,17 @@ def test_head_fp32_several_waves_batch_independent(dev):
     """128 frames of a ResNet-50 head (forward: 640 CTAs, data gradients more) against float64, and each frame's
     heatmaps and d features bit-identical to the same frame run alone: neither has a cross-frame sum."""
     b, c, h, w = 128, 2048, 12, 12
-    head = _head(c, (17, 17), seed=41)
-    deconvs, ws, bs = _params(head)
-    feats = torch.randn(b, c, h, w, device=dev, generator=_gen(12)) * 0.5
+    head = make_head(c, (17, 17), seed=41)
+    deconvs, (ws, bs) = list(head.upsampling_layers)[1:], head_params(head)
+    feats = features(b, c, h, w, 12, torch.float32)
     f = feats.clone().requires_grad_(True)
     hm = head(f)
-    hm_ref = S.head_ref_chunked(feats, ws, bs, softmax=True, bf16_operands=False)
+    hm_ref = S.head_ref_chunked(feats, ws, bs, softmax=True, operands=None)
     err = (hm.detach().to(F64) - hm_ref).abs()
     assert bool((err <= 1e-4 * hm_ref + 1e-9).all()), float((err / (1e-4 * hm_ref + 1e-9)).max())
-    gout = torch.randn(hm.shape, device=dev, generator=_gen(13))
+    gout = torch.randn(hm.shape, device=dev, generator=gen(13))
     (hm * gout).sum().backward()
-    ref, gnorm = _ref_grads(feats, ws, bs, gout, True, hm_ref, bf16_operands=False)
+    ref, gnorm = ref_grads(feats, ws, bs, gout, True, hm_ref, operands=None)
     fscale = ref["dfeat"].abs().flatten(1).amax(1).view(-1, 1, 1, 1)
     ratio = float(((f.grad.to(F64) - ref["dfeat"]).abs() / (1e-4 * fscale + 1e-30)).max())
     assert ratio < 1.0, ("d features", ratio)

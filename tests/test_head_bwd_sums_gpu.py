@@ -12,6 +12,8 @@ import numpy as np
 import pytest
 import torch
 
+from head_support import head_params, make_head
+
 WG_MAX_CTAS, B2D_MAX_CTAS, GB_CLS = 132, 264, 20
 C_FEAT, H_FEAT, K_PTS = 2048, 12, 17
 
@@ -46,15 +48,8 @@ def seq_sum(rows: np.ndarray) -> np.ndarray:
 @pytest.mark.parametrize("b", [256, 512])
 def test_head_backward_sums_partials_in_fixed_order(lib, dev, b):
     from lightning_pose_b200 import ops
-    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
 
-    torch.manual_seed(101 + b)
-    head = HeatmapHead("resnet50", C_FEAT, K_PTS)
-    d1, d2 = list(head.upsampling_layers)[1:]
-    for layer in (d1, d2):
-        torch.nn.init.xavier_uniform_(layer.weight, gain=3.0)
-        torch.nn.init.uniform_(layer.bias, -0.3, 0.3)
-    w1, b1, w2, b2 = (t.detach().float().contiguous().to(dev) for t in (d1.weight, d1.bias, d2.weight, d2.bias))
+    (w1, w2), (b1, b2) = head_params(make_head(C_FEAT, (K_PTS, K_PTS), seed=101 + b))
     c4, c1, c2 = w1.shape[0], w1.shape[1], w2.shape[1]
     feats = (torch.randn(b, C_FEAT, H_FEAT, H_FEAT) * 0.5).bfloat16().to(dev)
     probs, (xs, fws) = ops._head_forward_bf16(feats, [w1, w2], [b1, b2], True, train=True)

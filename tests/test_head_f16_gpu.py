@@ -5,9 +5,9 @@ fp16 operands.  The fp16 forward is the bf16 forward's kernels instantiated on f
 that rides on the constant-one channel) rounded to fp16 on the device, fp16 mid activations, fp32 accumulators and fp32
 heatmaps.
 
-Oracle A is float64 on exactly those roundings.  Its bars are the bf16 head's (test_gpu_parity.py: 1e-2 relative, at
-most 0.01 % of the pixels up to 3e-2) scaled by the unit-roundoff ratio 2^-11 / 2^-8 = 1/8 and rounded up: 2e-3 relative,
-at most 0.01 % of the pixels up to 5e-3.  The pixels allowed past 2e-3 are those fed by a mid activation that sits on an
+Oracle A is float64 on exactly those roundings (``scale_oracle.head_ref`` with fp16 operands).  Its bars are the bf16
+head's (1e-2 relative, at most 0.01 % of the pixels up to 3e-2) scaled by the unit-roundoff ratio 2^-11 / 2^-8 = 1/8 and
+rounded up: 2e-3 relative, at most 0.01 % of the pixels up to 5e-3 (``head_support.BARS``).  The pixels allowed past 2e-3 are those fed by a mid activation that sits on an
 fp16 rounding boundary and rounds the other way than in the oracle (fp32 summation order).  Oracle B is the reference's own
 HeatmapHead and soft-argmax under autocast(float16), held to the reference's 1 px bar for swapping the compute behind a
 forward."""
@@ -15,11 +15,11 @@ import ctypes
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import scale_oracle as S
+from head_support import WORST, check_heatmaps, features, forward_checks, fwd_layout, head_params, make_head, report_headroom, softmax_split
 
-F64 = torch.float64
+F16 = torch.float16
 pytestmark = pytest.mark.gpu
 
 # (C, H, W, channels): fast path (cfg 2), banded two-deconv (cfg 5), one-deconv (cfgs 3 and 4), wide heads
@@ -39,128 +39,40 @@ def dev():
     return torch.device("cuda:0")
 
 
+@pytest.fixture(scope="module", autouse=True)
+def _report_headroom():
+    WORST.clear()
+    yield
+    report_headroom()
+
+
 def _lib():
     from lightning_pose_b200._lib import lib
 
     return lib
 
 
-def _gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _make_head(c, ch, seed=13, gain=3.0):
-    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
-
-    torch.manual_seed(seed)
-    head = HeatmapHead("resnet50", c, ch[1], deconv_out_channels=ch[0]) if len(ch) == 2 else HeatmapHead("vits_dino", c, ch[0])
-    for layer in list(head.upsampling_layers)[1:]:
-        torch.nn.init.xavier_uniform_(layer.weight, gain=gain)
-        torch.nn.init.uniform_(layer.bias, -0.3, 0.3)
-    return head.cuda().requires_grad_(False).eval()
-
-
-def _params(head):
-    deconvs = list(head.upsampling_layers)[1:]
-    return [d.weight for d in deconvs], [d.bias for d in deconvs]
-
-
-def _feats(b, c, h, w, seed=5):
-    return (torch.randn(b, c, h, w, device="cuda", generator=_gen(seed)) * 0.5).half()
-
-
-def oracle_a(feats, ws, bs, softmax):
-    """float64 on the fp16 route's roundings: fp16 features and weights, fp16 mid activations, the bias of a second layer
-    (it rides on the constant-one channel) in fp16; the first layer's bias is added to the fp32 accumulators as is."""
-    h = lambda t: t.detach().half().to(F64)  # noqa: E731
-    out = []
-    with torch.no_grad():
-        for i in range(0, feats.shape[0], 8):
-            x = F.pixel_shuffle(feats[i : i + 8].to(F64), 2)
-            for j, (w, b) in enumerate(zip(ws, bs)):
-                if j:
-                    x = h(x)
-                x = F.conv_transpose2d(x, h(w), h(b) if j else b.detach().to(F64), stride=2, padding=1, output_padding=1)
-            if softmax:
-                x = torch.softmax(x.flatten(2), -1).reshape(x.shape)
-            out.append(x)
-    return torch.cat(out)
-
-
-def check_heatmaps(out, ref, case):
-    out, ref = out.to(F64), ref.to(F64)
-    rel = (out - ref).abs() / (ref.abs() + 1e-7)
-    assert float(rel.max()) < 5e-3, (case, float(rel.max()))
-    assert float((rel > 2e-3).to(F64).mean()) < 1e-4, (case, float((rel > 2e-3).to(F64).mean()))
-    assert float((out.sum((-1, -2)) - 1).abs().max()) < 1e-5, case
-
-
-def check_logits(out, ref, case):
-    out, ref = out.to(F64), ref.to(F64)
-    allowed = 2e-3 * ref.abs().amax((-1, -2), keepdim=True) + 2e-3 * ref.abs() + 1e-12
-    assert float(((out - ref).abs() / allowed).max()) <= 1.0, case
-
-
-def check_keypoints(hm, hm_ref, ds, case, bar=0.1):
-    """The route's heatmaps and the oracle's, each decoded in float64: within ``bar`` px on confident planes."""
-    kp, _, _, _ = S.decode_ref(hm, ds)
-    kp_ref, cf_ref, _, _ = S.decode_ref(hm_ref, ds)
-    k = hm.shape[1]
-    d = (kp - kp_ref).abs().reshape(-1, k, 2).amax(-1)
-    conf = cf_ref > 0.5
-    if bool(conf.any()):
-        assert float(d[conf].max()) < bar, (case, float(d[conf].max()))
-    return float(d[conf].max()) if bool(conf.any()) else None
-
-
 @pytest.mark.parametrize("row", list(ROWS))
 def test_f16_forward_vs_oracle_a(dev, row):
     """Heatmaps (fused and split softmax), logits and decoded keypoints against oracle A."""
-    lib = _lib()
     c, h, w, ch = ROWS[row]
-    head = _make_head(c, ch)
-    feats = _feats(8, c, h, w)
-    ws, bs = _params(head)
-    hm_ref, logits_ref = oracle_a(feats, ws, bs, True), oracle_a(feats, ws, bs, False)
-    with torch.no_grad():
-        saved = lib.lpb_get_tuning(7)
-        try:
-            for split in (1, 0, 2):
-                assert lib.lpb_set_tuning(7, split) == 0
-                out = head(feats)
-                assert out.dtype == torch.float32 and out.shape == hm_ref.shape
-                check_heatmaps(out, hm_ref, f"{row} split={split}")
-        finally:
-            lib.lpb_set_tuning(7, saved)
-        head.final_softmax = False
-        check_logits(head(feats), logits_ref, row)
-        head.final_softmax = True
-    check_keypoints(out, hm_ref, head.downsample_factor, row)
+    head = make_head(c, ch, seed=13).requires_grad_(False).eval()
+    forward_checks(head, features(8, c, h, w, 5, F16), row, splits=(1, 0, 2), train=False, keypoint_bar=0.1)
 
 
 def test_f16_forward_past_one_wave(dev):
     """cfg 2 at B = 2 S + 7 (the persistent kernels run past one wave): oracle A, and with the fused softmax forced (a
     lone frame would otherwise take the split form) a frame alone gives the batch's bits."""
-    from test_head_shapes_gpu import softmax_unsplit
-
     c, h, w, ch = ROWS["cfg2_c2048_12x12"]
     b = 2 * torch.cuda.get_device_properties(dev).multi_processor_count + 7
-    head = _make_head(c, ch, seed=19)
-    feats = _feats(b, c, h, w, seed=9)
-    ws, bs = _params(head)
-    with torch.no_grad(), softmax_unsplit(_lib()):
+    head = make_head(c, ch, seed=19).requires_grad_(False).eval()
+    feats = features(b, c, h, w, 9, F16)
+    ws, bs = head_params(head)
+    with torch.no_grad(), softmax_split(_lib(), 0):
         out = head(feats)
         for i in (0, b // 2, b - 1):
             assert torch.equal(head(feats[i : i + 1])[0], out[i]), i
-    check_heatmaps(out, oracle_a(feats, ws, bs, True), f"cfg2 B={b}")
-
-
-def _ws_layout(b, c, h, w, c1, c2):
-    """head_fwd_layout (head_rows.cuh): byte offsets of the packed w1 / w2."""
-    stage = 4 * 4 * 80 * 16
-    groups = lambda k: -(-k // 20)  # noqa: E731
-    w2_at = groups(c1) * (c // 128) * stage
-    return 0, w2_at
+    check_heatmaps(out, S.head_ref_chunked(feats, ws, bs, True, operands=F16), f"cfg2 B={b}", dtype=F16)
 
 
 def _pack_ref(w, bias, nst, ngroups):
@@ -201,15 +113,15 @@ def test_f16_packs_equal_torch_half(dev):
 
     lib = _lib()
     b, c, h, w, c1, c2 = 2, 512, 8, 8, 17, 17
-    head = _make_head(c, (c1, c2), seed=3, gain=0.01)
-    ws, bs = _params(head)
+    head = make_head(c, (c1, c2), seed=3, gain=0.01).requires_grad_(False).eval()
+    ws, bs = head_params(head)
     with torch.no_grad():
         ws[0][0, 0, 0, 0] = 3e-8        # fp16 subnormal
         ws[0][1, 0, 1, 1] = -6.0e-5     # just below the smallest normal
         ws[1][2, 3, 1, 1] = 1e-7
         bs[1].copy_(torch.linspace(-1e-6, 70000.0, c2))  # subnormals, normals and an overflow to inf
     assert bool((ws[0].abs() < 6.1e-5).any())
-    feats = _feats(b, c, h, w)
+    feats = features(b, c, h, w, 5, F16)
     n = ctypes.c_size_t(0)
     assert lib.lpb_head_bf16_workspace_bytes(b, c, h, w, c1, c2, ctypes.byref(n)) == 0
     ws_buf = torch.zeros(n.value, dtype=torch.uint8, device=dev)
@@ -219,7 +131,7 @@ def test_f16_packs_equal_torch_half(dev):
                               ctypes.c_void_p(ws_buf.data_ptr()), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     assert rc == 0, lib.lpb_last_error()
     torch.cuda.synchronize()
-    w1_at, w2_at = _ws_layout(b, c, h, w, c1, c2)
+    w1_at, w2_at = 0, fwd_layout(b, c, h, w, c1, c2).w2_at
     stage = 4 * 4 * 80 * 16
     nst1, nst2 = c // 128, 1
     got1 = ws_buf[w1_at : w1_at + nst1 * stage].view(torch.int16)
@@ -251,17 +163,18 @@ def test_f16_routing(dev):
 
     for row, first in (("cfg2_c2048_12x12", "k1a_shuffle_convt_kernel<__half"), ("cfg5_c2048_16x16", "convt_rows_kernel<__half")):
         c, h, w, ch = ROWS[row]
-        head = _make_head(c, ch)
-        feats = _feats(4, c, h, w)
+        head = make_head(c, ch, seed=13).requires_grad_(False).eval()
+        feats = features(4, c, h, w, 5, F16)
         with torch.no_grad():
             names = _kernel_names(lambda: head.forward_with_keypoints(feats))
         assert any(first in k for k in names), (row, names)
         assert any("convt_rows_kernel<__half" in k for k in names), (row, names)
         assert not any("__nv_bfloat16" in k or "convt3x3" in k for k in names), (row, names)
     c, h, w, ch = ROWS["cfg2_c2048_12x12"]
-    head = _make_head(c, ch).requires_grad_(True)
-    feats = _feats(4, c, h, w).requires_grad_(True)
-    ws, bs = _params(head)
+    head = make_head(c, ch, seed=13).eval()
+    feats = features(4, c, h, w, 5, F16).requires_grad_(True)
+    ws = [d.weight for d in list(head.upsampling_layers)[1:]]
+    bs = [d.bias for d in list(head.upsampling_layers)[1:]]
     out = head(feats)
     ref = ops.head_forward_f32(feats.detach().float(), [x.detach() for x in ws], [x.detach() for x in bs], True)
     assert torch.equal(out.detach(), ref)
@@ -273,8 +186,8 @@ def test_f16_routing(dev):
 def test_f16_graph_replay_equals_eager(dev):
     """A captured CUDA graph of fp16 head + decode replays the eager bits."""
     c, h, w, ch = ROWS["cfg5_c2048_16x16"]
-    head = _make_head(c, ch, seed=7)
-    feats = _feats(16, c, h, w, seed=8)
+    head = make_head(c, ch, seed=7).requires_grad_(False).eval()
+    feats = features(16, c, h, w, 8, F16)
     static = feats.clone()
     with torch.no_grad():
         eager = head.forward_with_keypoints(feats)
@@ -286,7 +199,7 @@ def test_f16_graph_replay_equals_eager(dev):
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             outs = head.forward_with_keypoints(static)
-        static.copy_(_feats(16, c, h, w, seed=99))
+        static.copy_(features(16, c, h, w, 99, F16))
         g.replay()
         static.copy_(feats)
         g.replay()
@@ -308,22 +221,22 @@ def test_f16_context_head_vs_oracle_a(dev):
         if isinstance(m, torch.nn.ConvTranspose2d) and m.weight.shape[-1] == 3:
             torch.nn.init.xavier_uniform_(m.weight, gain=3.0)
             torch.nn.init.uniform_(m.bias, -0.3, 0.3)
-    feats = _feats(t, c, h, w, seed=22)
+    feats = features(t, c, h, w, 22, F16)
     with torch.no_grad():
         hm_sf, hm_mf = head.forward_sequence(feats)
-    ws, bs = _params(head.head_sf)
-    check_heatmaps(hm_sf, oracle_a(feats[2 : t - 2], ws, bs, True), "context head_sf")
+    ws, bs = head_params(head.head_sf)
+    check_heatmaps(hm_sf, S.head_ref_chunked(feats[2 : t - 2], ws, bs, True, operands=F16), "context head_sf", dtype=F16)
     mf = head.head_mf
     maps = []
     for last in (mf.W_f, mf.W_b):
         layers = ([mf.W_pre] if mf.upsampling_factor == 2 else []) + [last]
-        maps.append(oracle_a(feats, [m.weight for m in layers], [m.bias for m in layers], False).float())
+        maps.append(S.head_ref_chunked(feats, [m.weight for m in layers], [m.bias for m in layers], False, operands=F16).float())
     idx = (torch.arange(t - 4, device=dev)[:, None] + torch.arange(5, device=dev)[None, :]).to(torch.int32)
     hf = (mf.H_f[0].weight, mf.H_f[0].bias, mf.H_f[1].weight, mf.H_f[1].bias)
     hb = (mf.H_b[0].weight, mf.H_b[0].bias, mf.H_b[1].weight, mf.H_b[1].bias)
     with torch.no_grad():
         ref = ops.plane_softmax(ops.crnn_combine(maps[0], maps[1], idx, hf, hb))
-    check_heatmaps(hm_mf, ref, "context head_mf")
+    check_heatmaps(hm_mf, ref, "context head_mf", dtype=F16)
 
 
 def test_f16_vs_reference_under_autocast(dev):
@@ -339,10 +252,10 @@ def test_f16_vs_reference_under_autocast(dev):
     R.install()
     ref_mod = R.load("lightning_pose.models.heads.heatmap")
     c, h, w, ch = ROWS["cfg2_c2048_12x12"]
-    head = _make_head(c, ch, seed=29, gain=4.0)
+    head = make_head(c, ch, seed=29, gain=4.0).requires_grad_(False).eval()
     ref_head = ref_mod.HeatmapHead("resnet50", c, ch[1], deconv_out_channels=ch[0]).cuda().eval()
     ref_head.load_state_dict(head.state_dict())
-    feats = _feats(16, c, h, w, seed=30)
+    feats = features(16, c, h, w, 30, F16)
     with torch.no_grad():
         hm, kp, cf = head.forward_with_keypoints(feats)
         with torch.autocast("cuda", dtype=torch.float16):

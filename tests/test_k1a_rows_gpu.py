@@ -14,11 +14,11 @@ import torch
 import torch.nn.functional as F
 
 import scale_oracle as S
+from head_support import fwd_layout, gen, row_layout, softmax_split
 
 pytestmark = pytest.mark.gpu
 
 K = 17
-HB_BSTAGE_BYTES = 4 * 4 * 80 * 16  # packed weights of one 32-channel stage (head_prep.cuh)
 
 # (C, H, W) -> bands as (first feature row, rows): config 2 (0,6 6,6); W = 4 (0,16 16,16 32,16); W = 6, last band shorter
 # (0,12 12,12 24,8); one band in the training form with W = 6 and W = 7 (the frame's bottom edge is the only halo); H * W =
@@ -45,12 +45,6 @@ def lib():
     return lib
 
 
-def row_layout(hi, wi):
-    pp = wi + 1
-    lead = pp + 1
-    return pp, lead, (hi * pp + 2 * lead + 7) & ~7
-
-
 def head_call(lib, feats, w1, b1, w2, b2):
     """lpb_head_fwd_bf16 in the training form; returns (saved copy, mid activations) as int16 bit patterns."""
     b, c, h, w = feats.shape
@@ -66,9 +60,8 @@ def head_call(lib, feats, w1, b1, w2, b2):
                                ctypes.c_void_p(xs.data_ptr()), ctypes.c_void_p(ws.data_ptr()), stream)
     assert rc == 0, lib.lpb_last_error()
     torch.cuda.synchronize(feats.device)
-    nst = c // 4 // 32
-    _, _, rows_mid = row_layout(4 * h, 4 * w)
-    mid = ws[(nst + 1) * HB_BSTAGE_BYTES:(nst + 1) * HB_BSTAGE_BYTES + b * 4 * rows_mid * 16]
+    lay = fwd_layout(b, c, h, w, K, K)
+    mid = ws[lay.mid_at:lay.mid_at + b * 4 * lay.nst2 * lay.mid_rows * 16]
     return xs.view(torch.int16), mid.view(torch.int16)
 
 
@@ -108,15 +101,13 @@ def test_k1a_bands(lib, dev, shape):
     assert lib.lpb_head_bf16_plan(c, h, w, K, K, ctypes.byref(plan)) == 0 and plan.value == 1  # the fast path: k1a
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     b = 2 * sms + 7
-    g = torch.Generator(device="cuda").manual_seed(11)
+    g = gen(11)
     feats = (torch.randn(b, c, h, w, device=dev, generator=g) * 0.5).bfloat16()
     w1 = torch.randn(c // 4, K, 3, 3, device=dev, generator=g) * (2.0 / (c // 4)) ** 0.5
     b1 = torch.rand(K, device=dev, generator=g) - 0.5
     w2 = torch.randn(K, K, 3, 3, device=dev, generator=g) * 0.3
     b2 = torch.rand(K, device=dev, generator=g) - 0.5
-    saved = lib.lpb_get_tuning(7)
-    try:
-        lib.lpb_set_tuning(7, 0)
+    with softmax_split(lib, 0):
         xs, mid = head_call(lib, feats, w1, b1, w2, b2)
         assert torch.equal(xs, saved_copy_ref(feats))
 
@@ -138,5 +129,3 @@ def test_k1a_bands(lib, dev, shape):
             xs1, mid1 = head_call(lib, feats[j:j + 1].contiguous(), w1, b1, w2, b2)
             assert torch.equal(xs1, xs[j * nxs:(j + 1) * nxs])
             assert torch.equal(mid1, mid[j * nmid:(j + 1) * nmid])
-    finally:
-        lib.lpb_set_tuning(7, saved)

@@ -6,13 +6,14 @@ shared-memory buffers carry over from one item to the next.  Every test below pi
 the launch it exercises (restated in the ``*_launches`` helpers) and asserts that some CTA gets two or more items, so a
 later change to a launch's item count cannot quietly drop the test back to one item per CTA.  S is read from the
 device (H100 SXM: 132, PCIe: 114)."""
-import contextlib
 import ctypes
 
 import pytest
 import torch
 
 import scale_oracle as S
+from head_support import (WORST, check_grads, check_heatmaps, check_logits, features, gen, grads, head_params, make_head, ref_forward,
+                          ref_grads, report_headroom, softmax_split)
 
 pytestmark = pytest.mark.gpu
 
@@ -61,20 +62,11 @@ def assert_some_cta_loops(launches, at_least=2):
     assert any(items_per_cta(n, g) >= at_least for _, n, g in launches), launches
 
 
-@contextlib.contextmanager
-def tuning(lib, settings: dict):
-    saved = {k: lib.lpb_get_tuning(k) for k in settings}
-    try:
-        for k, v in settings.items():
-            assert lib.lpb_set_tuning(k, v) == 0
-        yield
-    finally:
-        for k, v in saved.items():
-            lib.lpb_set_tuning(k, v)
-
-
-def _gen(seed: int) -> torch.Generator:
-    return torch.Generator(device="cuda").manual_seed(seed)
+@pytest.fixture(scope="module", autouse=True)
+def _report_headroom():
+    WORST.clear()
+    yield
+    report_headroom()
 
 
 def close(a, b, atol, rtol):
@@ -94,8 +86,8 @@ B_KINDS = {"S-1": lambda s: s - 1, "S": lambda s: s, "S+1": lambda s: s + 1, "2S
 
 
 def _head_fwd_launches(cfg, b, s, split_key):
-    """(name, items, grid) of the persistent launches of lpb_head_fwd_bf16 (head_bf16.cu:931-932,
-    head_rows_bf16.cu:437-470)."""
+    """(name, items, grid) of the persistent launches of lpb_head_fwd_bf16: the k1a grid of head_fwd (head_bf16.cu), the
+    banded grid and the softmax split of launch_convt_rows (head_rows_bf16.cu)."""
     arch, _, h, w = HEAD_CFGS[cfg]
 
     def banded(hi, wi, mode):
@@ -114,7 +106,7 @@ def _head_fwd_launches(cfg, b, s, split_key):
 
 
 def _head_bwd_launches(cfg, b, s):
-    """(name, items, grid) of the frame loops of lpb_head_bwd_bf16 (head_bwd_bf16.cu:1049-1051, :1091-1096)."""
+    """(name, items, grid) of the frame loops of lpb_head_bwd_bf16 (head_bwd_bf16.cu): the b3a slots and the b2d grid."""
     _, c, _, _ = HEAD_CFGS[cfg]
     ntile1 = -(-(c // 4) // 128)
     slots = max(1, min(s // ntile1, b))
@@ -124,35 +116,14 @@ def _head_bwd_launches(cfg, b, s):
     return out
 
 
-def _rand_head(arch, cin, gain=3.0, seed=13, final_softmax=True):
-    from lightning_pose_b200.models.heads.heatmap import HeatmapHead
-
-    torch.manual_seed(seed)
-    head = HeatmapHead(arch, cin, K, final_softmax=final_softmax)
-    for layer in list(head.upsampling_layers)[1:]:
-        torch.nn.init.xavier_uniform_(layer.weight, gain=gain)
-        torch.nn.init.uniform_(layer.bias, -0.3, 0.3)
-    return head
+def _cfg_head(cfg, seed, gain=3.0):
+    arch, c, _, _ = HEAD_CFGS[cfg]
+    return make_head(c, (K, K) if arch == "resnet50" else (K,), seed=seed, gain=gain)
 
 
-def _head_params(head):
-    deconvs = list(head.upsampling_layers)[1:]
-    return [d.weight.detach() for d in deconvs], [d.bias.detach() for d in deconvs]
-
-
-def _feats(cfg, b, dev, seed=5, scale=0.5):
+def _cfg_feats(cfg, b, seed):
     _, c, h, w = HEAD_CFGS[cfg]
-    return (torch.randn(b, c, h, w, device=dev, generator=_gen(seed)) * scale).bfloat16()
-
-
-def _check_heatmaps(out, ref_hm):
-    """Acceptance rule of the bf16 head (test_head_bf16_real_config_shapes_forward): relative error below 3e-2 everywhere,
-    above 1e-2 on at most 0.01 % of the pixels (a mid activation on a bf16 rounding boundary may round the other way);
-    every plane sums to 1."""
-    rel = ((out.to(F64) - ref_hm).abs() / (ref_hm.abs() + 1e-7)).flatten()
-    assert float(rel.max()) < 3e-2 and float((rel > 1e-2).to(F64).mean()) < 1e-4, (float(rel.max()), float((rel > 1e-2).to(F64).mean()))
-    sums = out.sum((2, 3))
-    assert float((sums - 1).abs().max()) <= 1e-5
+    return features(b, c, h, w, seed, torch.bfloat16)
 
 
 @pytest.mark.parametrize("bkind", list(B_KINDS))
@@ -169,21 +140,19 @@ def test_head_forward_past_one_wave(lpb, lib, dev, sms, cfg, bkind):
     plan = ctypes.c_int(-1)
     assert lib.lpb_head_bf16_plan(c, h, w, K, K if two else 0, ctypes.byref(plan)) == 0
     assert plan.value == (1 if cfg == "cfg2" else 0)  # which kernels the launches above describe
-    head = _rand_head(arch, c).to(dev)
-    feats = _feats(cfg, 2 * sms + 7, dev)[:b]
-    ws, bs = _head_params(head)
-    logits_ref = S.head_ref_chunked(feats, ws, bs, softmax=False)
-    hm_ref = torch.softmax(logits_ref.flatten(2), -1).reshape(logits_ref.shape)
+    head = _cfg_head(cfg, seed=13)
+    feats = _cfg_feats(cfg, 2 * sms + 7, seed=5)[:b]
+    case = f"{cfg} B={bkind}"
+    logits_ref, hm_ref = ref_forward(head, feats)
     with torch.no_grad():
         out = head(feats)
     assert out.dtype == torch.float32 and out.shape == hm_ref.shape
-    _check_heatmaps(out, hm_ref)
+    check_heatmaps(out, hm_ref, case)
     del hm_ref
     head.final_softmax = False
     with torch.no_grad():
-        lg = head(feats)
-    close(lg, logits_ref, atol=1e-2 * float(logits_ref.abs().max()), rtol=1e-2)
-    del lg, logits_ref
+        check_logits(head(feats), logits_ref, case)
+    del logits_ref
     # the training route (saved operand copy, inter-layer activations kept) computes the same bits
     head.final_softmax = True
     out_train = head(feats.clone().requires_grad_(True))
@@ -196,7 +165,7 @@ def test_head_forward_past_one_wave(lpb, lib, dev, sms, cfg, bkind):
     with torch.no_grad():
         assert torch.equal(head(feats[perm]), out[perm])
     # with the fused softmax pinned (key 7 = 0: no split at any batch), a frame computes the same bits in a batch of one
-    with tuning(lib, {7: 0}):
+    with softmax_split(lib, 0):
         with torch.no_grad():
             big = head(feats)
             assert torch.equal(big, out)  # at B >= S the default never splits either
@@ -204,42 +173,26 @@ def test_head_forward_past_one_wave(lpb, lib, dev, sms, cfg, bkind):
                 assert torch.equal(head(feats[i : i + 1])[0], big[i]), i
 
 
-def _grads(head, feats, gout):
-    head.zero_grad(set_to_none=True)
-    f = feats.clone().requires_grad_(True)
-    (head(f) * gout).sum().backward()
-    return [f.grad.clone()] + [p.grad.clone() for p in head.parameters()]
-
-
 @pytest.mark.parametrize("cfg", ["cfg2", "cfg3"])
 def test_head_backward_past_one_wave(lpb, dev, sms, cfg):
     arch, c, h, w = HEAD_CFGS[cfg]
     b = 2 * sms + 7
     assert_some_cta_loops(_head_bwd_launches(cfg, b, sms))
-    head = _rand_head(arch, c, seed=31).to(dev)
-    feats = _feats(cfg, b, dev, seed=6)
+    head = _cfg_head(cfg, seed=31)
+    feats = _cfg_feats(cfg, b, seed=6)
     up = 8 if arch == "resnet50" else 4
-    gout = torch.randn(b, K, up * h, up * w, device=dev, generator=_gen(7))
-    run1 = _grads(head, feats, gout)
-    run2 = _grads(head, feats, gout)
-    for x, y in zip(run1, run2):  # fixed-order sums: bit-reproducible at this batch
-        assert torch.equal(x, y)
-    assert run1[0].dtype == torch.bfloat16
+    gout = torch.randn(b, K, up * h, up * w, device=dev, generator=gen(7))
+    run1 = grads(head, feats, gout)
+    run2 = grads(head, feats, gout)
+    for name in run1:  # fixed-order sums: bit-reproducible at this batch
+        assert torch.equal(run1[name], run2[name]), name
+    assert run1["dfeat"].dtype == torch.bfloat16
     perm = torch.randperm(b, generator=torch.Generator().manual_seed(2)).to(dev)
-    assert torch.equal(_grads(head, feats[perm], gout[perm])[0], run1[0][perm])
-    ws, bs = _head_params(head)
-    dfeat, dws, dbs = S.head_grad_ref(feats, ws, bs, gout, softmax=True)
-    deconvs = list(head.upsampling_layers)[1:]
-    got = {"dfeat": run1[0]}
-    for i, d in enumerate(deconvs):
-        got[f"dw{i}"], got[f"db{i}"] = d.weight.grad, d.bias.grad
-    ref = {"dfeat": dfeat, **{f"dw{i}": g for i, g in enumerate(dws)}, **{f"db{i}": g for i, g in enumerate(dbs)}}
-    wscale = float(dws[-1].abs().max())
-    for name in ref:
-        err, scale = float((got[name].to(F64) - ref[name]).abs().max()), float(ref[name].abs().max())
-        if name.startswith("db"):  # cancelling sums (exactly 0 behind a softmax): rounding noise, bounded by the dw scale
-            scale = max(scale, wscale)
-        assert err <= 1e-2 * scale + 1e-9, (name, err, scale)
+    assert torch.equal(grads(head, feats[perm], gout[perm])["dfeat"], run1["dfeat"][perm])
+    ws, bs = head_params(head)
+    _, hm_ref = ref_forward(head, feats)
+    ref, gnorm = ref_grads(feats, ws, bs, gout, True, hm_ref)
+    check_grads(run1, ref, gnorm, f"{cfg} B=2S+7 softmax=True", db_max_rule=True)
 
 
 def test_head_with_keypoints_past_one_wave(lpb, dev, sms):
@@ -247,11 +200,11 @@ def test_head_with_keypoints_past_one_wave(lpb, dev, sms):
     overflow the 32 x 32 decode windows into the dense backward route."""
     arch, c, h, w = HEAD_CFGS["cfg2"]
     b = 2 * sms + 7
-    head = _rand_head(arch, c, gain=4.0, seed=31).to(dev)
-    feats = _feats("cfg2", b, dev, seed=8)
+    head = _cfg_head("cfg2", seed=31, gain=4.0)
+    feats = _cfg_feats("cfg2", b, seed=8)
     flat_frames = [5, sms, b - 3]
     feats[flat_frames] = 0
-    g_kp = torch.randn(b, 2 * K, device=dev, generator=_gen(9))
+    g_kp = torch.randn(b, 2 * K, device=dev, generator=gen(9))
     f = feats.clone().requires_grad_(True)
     hm, kp, cf = head.forward_with_keypoints(f)
     (kp * g_kp).sum().backward()
@@ -267,7 +220,7 @@ def test_head_with_keypoints_past_one_wave(lpb, dev, sms):
     assert float(cerr.max()) <= 1e-4, float(cerr.max())
     # the fused backward against float64 autograd: the soft-argmax gradient taken at the kernel's heatmaps, then the head
     g_hm = S.decode_grad_ref(hm, 2, 1000.0, g_kp)
-    ws, bs = _head_params(head)
+    ws, bs = head_params(head)
     dfeat, dws, dbs, mid_norm = S.head_grad_ref(feats, ws, bs, g_hm, softmax=True, want_mid_grad=True)
     d1, d2 = list(head.upsampling_layers)[1:]
     # db1 only sees the image border and is left as rounding noise of the bf16 gradient operand, 2^-8 ||d mid||_2 per
@@ -314,7 +267,7 @@ def _decode_inputs(n, hw, n_diffuse, seed):
     """(B, 17, hw, hw) heatmaps: peaked planes (random centres, sigma 1.6, 5 % logit noise) with ``n_diffuse`` planes at
     random positions replaced by diffuse ones (logit noise 0.01, the bench's untrained regime); and the diffuse mask."""
     b = -(-n // K)
-    g = _gen(seed)
+    g = gen(seed)
     dev = torch.device("cuda")
     cy = torch.rand(b * K, 1, 1, device=dev, generator=g) * (hw - 1)
     cx = torch.rand(b * K, 1, 1, device=dev, generator=g) * (hw - 1)
@@ -450,7 +403,7 @@ def test_decode_backward_past_one_wave(lpb, props, sms, size, mix):
     hm, diffuse = _decode_inputs(n, hw, _n_diffuse(mix, n, props, sms), seed=hw + ds + 1)
     b = hm.shape[0]
     _, _, stats = lpb._decode_fwd(hm, ds, 1000.0)
-    gxy = torch.randn(b, K, 2, device=hm.device, generator=_gen(ds))
+    gxy = torch.randn(b, K, 2, device=hm.device, generator=gen(ds))
     ref = S.decode_grad_ref(hm, ds, 1000.0, gxy)
     _check_plane_grads(lpb._decode_bwd(hm, stats, gxy, ds, 1000.0), ref)
     win, meta, ov = lpb.decode_backward_windows(hm, stats, gxy, ds, 1000.0)
@@ -466,7 +419,7 @@ def test_decode_backward_past_one_wave(lpb, props, sms, size, mix):
 # e: losses and the CRNN combine
 # ------------------------------------------------------------------------------------------------
 def _peaked_planes(b, k, h, w, seed, sigma=1.6):
-    g = _gen(seed)
+    g = gen(seed)
     dev = torch.device("cuda")
     cy = torch.rand(b, k, 1, 1, device=dev, generator=g) * (h - 1)
     cx = torch.rand(b, k, 1, 1, device=dev, generator=g) * (w - 1)
@@ -492,7 +445,7 @@ def test_heatmap_losses_at_scale(lpb, dev, kind, layout):
     misaligned views take the scalar loop of heatmap_loss_plane_kernel (losses.cu:61-67), the bench batch the float4 one."""
     b, h, w = {"bench_768x17_96x96": (768, 96, 96), "odd_30x41": (64, 30, 41), "misaligned_96x96": (32, 96, 96)}[layout]
     targ = _peaked_planes(b, K, h, w, seed=11)
-    targ[torch.rand(b, K, device=dev, generator=_gen(12)) < 0.1] = 0.0
+    targ[torch.rand(b, K, device=dev, generator=gen(12)) < 0.1] = 0.0
     pred = _peaked_planes(b, K, h, w, seed=13, sigma=2.5)
     if layout.startswith("misaligned"):
         targ, pred = _misaligned(targ), _misaligned(pred)
@@ -507,7 +460,7 @@ def test_heatmap_losses_at_scale(lpb, dev, kind, layout):
 def test_heatmap_mse_from_keypoints_at_scale(lpb, dev):
     """Fused targets + MSE on 256 labeled frames: visibility 0 / 1 / 2, keypoints outside the frame and NaN."""
     b, img, oh = 256, 384, 96
-    g = _gen(14)
+    g = gen(14)
     kp = torch.rand(b, K, 2, device=dev, generator=g) * img
     sel = torch.rand(b, K, device=dev, generator=g)
     kp[sel < 0.05] = -12.0                            # left of / above the frame
@@ -534,7 +487,7 @@ def _pca_scratch_floats(n_sel, n_views, n_comp, t, bwd):
 
 def _unsup_check(lpb, kp, conf, eps, thr, sv, mv, sv_ref, mv_ref):
     n_clips = kp.shape[0]
-    wts = torch.rand(n_clips, 3, device=kp.device, generator=_gen(16)) + 0.5
+    wts = torch.rand(n_clips, 3, device=kp.device, generator=gen(16)) + 0.5
     x = kp.clone().requires_grad_(True)
     out = lpb.unsup_losses(x, conf, temporal_eps=eps, prob_threshold=thr, pca_singleview=sv, pca_multiview=mv)
     (out[:, :3] * wts).sum().backward()
@@ -555,8 +508,8 @@ def test_unsup_losses_bench_clips(lpb, dev, golden):
     """The bench's 16 clips x 32 frames: temporal + single-view PCA (median centring) + multi-view PCA per clip."""
     gl = golden("losses")
     base = torch.from_numpy(gl["pca_in_kp"]).to(dev)
-    kp = base[None] + 3.0 * torch.randn(16, *base.shape, device=dev, generator=_gen(17))
-    conf = torch.rand(16, base.shape[0], K, device=dev, generator=_gen(18))
+    kp = base[None] + 3.0 * torch.randn(16, *base.shape, device=dev, generator=gen(17))
+    conf = torch.rand(16, base.shape[0], K, device=dev, generator=gen(18))
     cols, mcm = gl["pca_sv_cols"], gl["pca_mv_mcm"]
     sv = lpb.PcaParams(cols.astype("int32"), len(cols), 0, "median", gl["pca_sv_mean"], gl["pca_sv_kept"], 2.5, dev)
     mv = lpb.PcaParams(mcm.reshape(-1).astype("int32"), mcm.shape[1], mcm.shape[0], None, gl["pca_mv_mean"], gl["pca_mv_kept"], 0.7, dev)
@@ -573,7 +526,7 @@ def test_unsup_losses_large_shared_memory_route(lpb, dev):
     fwd = (_pca_scratch_floats(K, views, nc, t, False) + 4) * 4
     bwd = (_pca_scratch_floats(K, views, nc, t, True) + t * kk * 2 + 4) * 4
     assert 48 * 1024 < fwd <= 200 * 1024 and 48 * 1024 < bwd <= 200 * 1024, (fwd, bwd)
-    g = _gen(19)
+    g = gen(19)
     mcm = torch.arange(kk).reshape(views, K)
     mean = torch.randn(2 * views, device=dev, generator=g) * 50 + 150
     kept = torch.linalg.qr(torch.randn(2 * views, nc, device=dev, generator=g))[0].T.contiguous()
@@ -594,7 +547,7 @@ def test_crnn_combine_grid_split(lpb, dev):
     n, h, w, hidden, m = 64, 4, 6, 16, 5000
     per = 65535 // K
     assert m * K >= 65536 and per * K < 65536 and -(-m // per) == 2  # two launches
-    g = _gen(20)
+    g = gen(20)
     wf = torch.randn(n, K, h, w, device=dev, generator=g)
     wb = torch.randn(n, K, h, w, device=dev, generator=g)
     idx = torch.randint(0, n, (m, 5), device=dev, generator=g, dtype=torch.int32)

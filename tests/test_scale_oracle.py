@@ -105,9 +105,9 @@ def test_head_ref_golden(golden, tag, nl):
     ws = [T(g[f"{tag}_w{i}"]) for i in range(nl)]
     bs = [T(g[f"{tag}_b{i}"]) for i in range(nl)]
     f = T(g[f"{tag}_in_features"])
-    close(S.head_ref(f, ws, bs, True, bf16_operands=False), g[f"{tag}_out_heatmaps"], atol=1e-8, rtol=1e-5)
-    close(S.head_ref(f, ws, bs, False, bf16_operands=False), g[f"{tag}_out_logits"], atol=2e-5, rtol=1e-5)
-    close(S.head_ref_chunked(f, ws, bs, True, bf16_operands=False), O.head_forward(f, ws, bs), atol=1e-8, rtol=1e-5)
+    close(S.head_ref(f, ws, bs, True, operands=None), g[f"{tag}_out_heatmaps"], atol=1e-8, rtol=1e-5)
+    close(S.head_ref(f, ws, bs, False, operands=None), g[f"{tag}_out_logits"], atol=2e-5, rtol=1e-5)
+    close(S.head_ref_chunked(f, ws, bs, True, operands=None), O.head_forward(f, ws, bs), atol=1e-8, rtol=1e-5)
 
 
 def _head_params(cin, c1, c2, seed):
@@ -135,8 +135,45 @@ def test_head_ref_bf16_operands(c2):
     close(got, x, atol=1e-2 * float(x.abs().max()), rtol=1e-2)
     assert float((got - x.double()).abs().max()) < 1e-4 * float(x.abs().max()) + 1e-2 * (c2 > 0)
     # rounded operands really differ from unrounded ones
-    assert not torch.allclose(got, S.head_ref(feats, ws, bs, softmax=False, bf16_operands=False), atol=1e-9, rtol=0)
+    assert not torch.allclose(got, S.head_ref(feats, ws, bs, softmax=False, operands=None), atol=1e-9, rtol=0)
     close(S.head_ref_chunked(feats, ws, bs, True), S.head_ref(feats, ws, bs, True), atol=1e-15)
+
+
+def _fp16_route_literal(feats, ws, bs, softmax):
+    """float64 on the fp16 route's roundings, written out: fp16 features and weights, fp16 mid activations, the bias of a
+    second layer (it rides on the constant-one channel) in fp16; the first layer's bias is added as is."""
+    h = lambda t: t.detach().half().to(torch.float64)  # noqa: E731
+    out = []
+    with torch.no_grad():
+        for i in range(0, feats.shape[0], 8):
+            x = F.pixel_shuffle(feats[i : i + 8].to(torch.float64), 2)
+            for j, (w, b) in enumerate(zip(ws, bs)):
+                if j:
+                    x = h(x)
+                x = F.conv_transpose2d(x, h(w), h(b) if j else b.detach().to(torch.float64), stride=2, padding=1, output_padding=1)
+            if softmax:
+                x = torch.softmax(x.flatten(2), -1).reshape(x.shape)
+            out.append(x)
+    return torch.cat(out)
+
+
+@pytest.mark.parametrize("c2", [0, 5])
+@pytest.mark.parametrize("softmax", [True, False])
+def test_head_ref_fp16_operands(c2, softmax):
+    """fp16 operands: head_ref / head_ref_chunked equal the written-out fp16 route bit for bit, layer-2 biases that
+    round included; with bf16 operands that bias stays unrounded."""
+    ws, bs = _head_params(64, 5, c2, seed=9)
+    if c2:
+        bs[1] = bs[1] + torch.tensor([1e-3 / 3, 0.1, -0.7, 1.0 / 3, 0.0])
+    feats = torch.randn(6, 64, 3, 4, generator=torch.Generator().manual_seed(10)).half()
+    want = _fp16_route_literal(feats, ws, bs, softmax)
+    assert torch.equal(S.head_ref(feats, ws, bs, softmax, operands=torch.float16), want)
+    assert torch.equal(S.head_ref_chunked(feats, ws, bs, softmax, operands=torch.float16), want)
+    if c2 and not softmax:
+        # the rounded layer-2 bias is what separates the two 16-bit forms' bias handling
+        moved = S.head_ref(feats, ws, bs, False, operands=torch.float16) - S.head_ref(feats, ws, [bs[0], bs[1].half().float()], False, operands=torch.float16)
+        assert float(moved.abs().max()) == 0.0
+        assert not torch.equal(S.head_ref(feats, ws, bs, False), S.head_ref(feats, ws, [bs[0], bs[1].bfloat16().float()], False))
 
 
 @pytest.mark.parametrize("c2,softmax", [(0, True), (5, True), (5, False)])
@@ -149,8 +186,8 @@ def test_head_grad_ref_vs_oracle_autograd(c2, softmax):
     wr = [w.clone().requires_grad_(True) for w in ws]
     br = [b.clone().requires_grad_(True) for b in bs]
     (O.head_forward(f, wr, br, softmax) * gout).sum().backward()
-    dfeat, dws, dbs, mid_norm = S.head_grad_ref(feats, ws, bs, gout, softmax, bf16_operands=False, want_mid_grad=c2 > 0) if c2 else (
-        *S.head_grad_ref(feats, ws, bs, gout, softmax, bf16_operands=False), None)
+    dfeat, dws, dbs, mid_norm = S.head_grad_ref(feats, ws, bs, gout, softmax, operands=None, want_mid_grad=c2 > 0) if c2 else (
+        *S.head_grad_ref(feats, ws, bs, gout, softmax, operands=None), None)
     close(dfeat, f.grad, atol=1e-6 * float(f.grad.abs().max()), rtol=1e-4)
     wscale = float(wr[-1].grad.abs().max())  # bias gradients behind a softmax cancel (the last one exactly): fp32 noise
     for a, b in zip(dws + dbs, [w.grad for w in wr] + [b.grad for b in br]):
