@@ -1089,15 +1089,9 @@ __global__ void __launch_bounds__(DEC_THREADS) upsample2x_kernel(const float* __
 }
 
 // ------------------------------------------------------------------------------------------------
-struct DecodeDevice {
-  int max_smem;  // opt-in shared memory per block
-  int sms;
-};
-
-// Fills what both directions share and queries the device.  lip (forward): Lipschitz bound of the 2-D upsampling.
+// Fills what both directions share.  lip (forward): Lipschitz bound of the 2-D upsampling.
 template <int DS>
-static int decode_geom(DecodeGeom<DS>& g, DecodeDevice& d, const float* heat, int64_t n_planes, int h, int w, float T,
-                       float* lip = nullptr) {
+static int decode_geom(DecodeGeom<DS>& g, const float* heat, int64_t n_planes, int h, int w, float T, float* lip = nullptr) {
   using G = UpsampleGeom<DS>;
   const DeviceTable* th = get_device_table(h, DS);
   const DeviceTable* tw = get_device_table(w, DS);
@@ -1122,10 +1116,6 @@ static int decode_geom(DecodeGeom<DS>& g, DecodeDevice& d, const float* heat, in
     for (int t = 0; t < G::W; ++t)
       g.phase2[q][t] = make_float2(th->host.phase[(size_t)(2 * q) * G::W + t], th->host.phase[(size_t)(2 * q + 1) * G::W + t]);
   if (lip) *lip = th->host.lip * tw->host.lip;
-  int dev = 0;
-  LPB_CUDA(cudaGetDevice(&dev));
-  LPB_CUDA(cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  LPB_CUDA(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
   return LPB_OK;
 }
 
@@ -1140,8 +1130,9 @@ static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, 
                              float* stats, void* workspace, cudaStream_t stream) {
   using G = UpsampleGeom<DS>;
   DecodeParams<DS> P;
-  DecodeDevice dev;
-  if (const int rc = decode_geom<DS>(P, dev, heat, n_planes, h, w, T, &P.lip); rc != LPB_OK) return rc;
+  DeviceLimits dev;
+  LPB_TRY(decode_geom<DS>(P, heat, n_planes, h, w, T, &P.lip));
+  LPB_TRY(device_limits(&dev));
   P.xy = xy;
   P.conf = conf;
   P.stats = stats;
@@ -1150,11 +1141,7 @@ static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, 
   P.qcounter = P.queue + 1 + n_planes;
   P.qscratch = reinterpret_cast<float*>(P.queue + 1 + 2 * n_planes);
   const size_t smem = ((size_t)(h + 2 * G::R) * P.pitch + DEC_FWD_SCRATCH) * sizeof(float) + 16;
-  if ((int64_t)smem > dev.max_smem) {
-    set_error("decode: plane %dx%d needs %zu B shared memory (> %d)", h, w, smem, dev.max_smem);
-    return LPB_ERR_UNSUPPORTED;
-  }
-  LPB_CUDA(cudaFuncSetAttribute(decode_fwd_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(decode_fwd_kernel<DS>, smem, "decode_fwd"));
   int per_sm = 0;
   LPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_fwd_kernel<DS>, DEC_THREADS, smem));
   const int64_t resident = (int64_t)dev.sms * (per_sm > 0 ? per_sm : 1);  // persistent CTAs: one wave
@@ -1174,8 +1161,9 @@ static int launch_decode_bwd(const float* heat, const float* stats, const float*
                              int* queue = nullptr) {
   using G = UpsampleGeom<DS>;
   DecodeBwdParams<DS> P;
-  DecodeDevice dev;
-  if (const int rc = decode_geom<DS>(P, dev, heat, n_planes, h, w, T); rc != LPB_OK) return rc;
+  DeviceLimits dev;
+  LPB_TRY(decode_geom<DS>(P, heat, n_planes, h, w, T));
+  LPB_TRY(device_limits(&dev));
   P.stats = stats;
   P.gxy = gxy;
   P.gheat = gheat;
@@ -1185,11 +1173,7 @@ static int launch_decode_bwd(const float* heat, const float* stats, const float*
     decode_bwd_window_kernel<DS><<<(unsigned)((n_planes + 3) / 4), 128, 0, stream>>>(P, win, meta, queue);
   }
   const size_t smem = ((size_t)2 * (h + 2 * G::R) * P.pitch + DEC_WARPS * 64) * sizeof(float) + 16;
-  if ((int64_t)smem > dev.max_smem) {
-    set_error("decode_bwd: plane %dx%d needs %zu B shared memory (> %d)", h, w, smem, dev.max_smem);
-    return LPB_ERR_UNSUPPORTED;
-  }
-  LPB_CUDA(cudaFuncSetAttribute(decode_bwd_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(decode_bwd_kernel<DS>, smem, "decode_bwd"));
   unsigned grid = (unsigned)n_planes;
   if (queue && grid > (unsigned)(2 * dev.sms)) grid = (unsigned)(2 * dev.sms);  // queue mode: one wave of resident CTAs
   decode_bwd_kernel<DS><<<grid, DEC_THREADS, smem, stream>>>(P);
@@ -1276,9 +1260,7 @@ extern "C" int lpb_upsample2x(const float* in, int64_t n_planes, int h, int w, f
   if (!th || !tw) return LPB_ERR_INVALID;
   const int padl = dec_padl(3), pitch = dec_pitch(w, 3);
   const size_t smem = (size_t)(h + 6) * pitch * sizeof(float);
-  LPB_REQUIRE(smem <= 200 * 1024, "upsample2x: plane %dx%d too large", h, w);
-  if (smem > 48 * 1024)
-    LPB_CUDA(cudaFuncSetAttribute(upsample2x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(upsample2x_kernel, smem, "upsample2x"));
   upsample2x_kernel<<<(unsigned)n_planes, DEC_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(in, h, w, pitch, padl,
                                                                                                  th->win, tw->win, out);
   LPB_CUDA(cudaGetLastError());

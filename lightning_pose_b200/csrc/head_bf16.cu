@@ -124,12 +124,12 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
 }
 
 template <typename T>
-int launch_head_prep(const PrepJobs& jobs, cudaStream_t s) {
-  head_prep_kernel<T><<<132 * 2, 256, 0, s>>>(jobs);  // two CTAs per SM of an H100 SXM
+int launch_head_prep(const PrepJobs& jobs, int sms, cudaStream_t s) {
+  head_prep_kernel<T><<<2 * sms, 256, 0, s>>>(jobs);  // two CTAs per SM
   return LPB_OK;
 }
-template int launch_head_prep<__nv_bfloat16>(const PrepJobs&, cudaStream_t);
-template int launch_head_prep<__half>(const PrepJobs&, cudaStream_t);
+template int launch_head_prep<__nv_bfloat16>(const PrepJobs&, int, cudaStream_t);
+template int launch_head_prep<__half>(const PrepJobs&, int, cudaStream_t);
 
 // =====================================================================================================
 // k1a: PixelShuffle + first transposed convolution
@@ -505,17 +505,6 @@ static bool head_fast_path(int C, int H, int W, int c2, int max_smem) {
   return k1.G > 0 && (int64_t)k1a_smem_bytes(k1) <= max_smem;
 }
 
-static int device_limits(int* max_smem, int* sms) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
-      cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
-    (void)cudaGetLastError();
-    *max_smem = 227 * 1024;  // sm_90a (also what a CPU-only caller sizing buffers should assume)
-    *sms = 132;
-  }
-  return 0;
-}
-
 static_assert(lpb::HEAD_MAX_CH == LPB_HEAD_MAX_CHANNELS, "the cap lpb200.h states is the keypoint groups' (head_prep.cuh)");
 
 // plan[0] = 1: fast path (saved_xs optional: training only); 0: generic path (saved_xs REQUIRED: it is the operand).
@@ -529,10 +518,8 @@ extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan
     return LPB_ERR_UNSUPPORTED;
   }
   LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "head_bf16_plan: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
-  int max_smem, sms;
-  device_limits(&max_smem, &sms);
-  plan[0] = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, max_smem) ? 1 : 0;
-  if (!plan[0] && ((size_t)32 * H * W * 2 > 200 * 1024 || (c2 > 0 ? 4 : 2) * W + 1 > CR_BAND_ROWS)) {
+  plan[0] = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, planning_limits().max_smem) ? 1 : 0;
+  if (!plan[0] && (rows_shuffle_smem_bytes(H, W) > HEAD_FEATURE_SMEM_BUDGET || (c2 > 0 ? 4 : 2) * W + 1 > CR_BAND_ROWS)) {
     set_error("head_bf16_plan: feature map %dx%d too large for this build", H, W);
     return LPB_ERR_UNSUPPORTED;
   }
@@ -572,10 +559,11 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
   LPB_REQUIRE(aligned_to(workspace, 16), "%s: workspace must be 16-byte aligned", name);
   LPB_REQUIRE(aligned_to(out, 8), "%s: out must be 8-byte aligned", name);
   if (B == 0) return LPB_OK;
-  int max_smem = 0, sms = 0;
-  device_limits(&max_smem, &sms);
+  DeviceLimits dev;
+  LPB_TRY(device_limits(&dev));
+  const int sms = dev.sms;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bool fast = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, max_smem);
+  const bool fast = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, dev.max_smem);
   const K1aGeom k1 = make_k1a_geom(H, W);
   // k1a's feature tensor map, encoded before anything is queued, so a failure leaves the stream untouched.  The plan stays
   // a function of the shape (CPU-only callers size buffers with it); every driver that runs sm_90a code has the encoder,
@@ -604,7 +592,7 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
       jobs.fpack[1] = {w2, final_softmax ? nullptr : b2, c1, c2, nst2, head_groups(c2), wp2};
       jobs.pads[0] = {mid, Lmid, (long long)B * 4 * nst2};
     }
-    launch_head_prep<T>(jobs, s);
+    launch_head_prep<T>(jobs, sms, s);
   }
   if (!fast) {
     // ---- generic path: shuffle rows -> banded GEMM(s) ----
@@ -652,7 +640,7 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
     pa.nstages = nst;
     pa.k = k1;
     auto kern = saved_xs ? k1a_shuffle_convt_kernel<T, 1> : k1a_shuffle_convt_kernel<T, 0>;
-    LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s1));
+    LPB_TRY(set_dynamic_smem(kern, s1, name));
     // items are dealt round-robin (item = blockIdx.x + k gridDim.x), so with G = 2 and an even grid (132 SMs) a CTA always
     // takes the same band, and likewise with G = 3 and a grid divisible by 3: bands of equal size keep the CTAs even.
     // Unequal bands (H % G != 0, e.g. 16 x 12 features: 6 / 5 / 5 rows) leave the CTAs of the larger bands one row pair

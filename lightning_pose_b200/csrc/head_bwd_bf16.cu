@@ -718,6 +718,9 @@ struct WgParams {
 // backward pass gives bit-identical results from run to run.
 constexpr int WG_MAX_CTAS = 132;   // weight-gradient CTAs per layer (one per SM of an H100 SXM; fewer on smaller devices)
 constexpr int B2D_MAX_CTAS = 264;  // b2d CTAs (two per SM)
+// Budget of the one-CTA-per-SM kernels (weight gradient, layer-1 data gradient b3a): an H100 SM's 227 KB less 2 KB.  It
+// picks the weight gradient's rows per unit R and whether b3a stages its d features for TMA stores.
+constexpr size_t HEAD_BWD_SMEM_BUDGET = 225 * 1024;
 __host__ __device__ inline size_t wgrad_part_stride(int Cin, int Cout) { return (size_t)Cin * Cout * 9 + 4 * (size_t)Cout; }
 // weight-gradient channel group (K-chunks of 8 channels per CTA) of a layer with nkc K-chunks of input
 inline int wgrad_kcx(int nkc) { return nkc % 8 == 0 ? 8 : 4; }
@@ -928,7 +931,7 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   for (int r = Hi < 8 ? Hi : 8; r >= 1; --r) {
     if (Hi % r) continue;
     const int kr = (r * (Wi + 1) + 15) & ~15, xr = (kr + Wi + 2 + 7) & ~7;
-    if ((size_t)2 * HEAD_KC * kr * 16 + (size_t)2 * kcx * xr * 16 + 64 <= 225 * 1024) {
+    if ((size_t)2 * HEAD_KC * kr * 16 + (size_t)2 * kcx * xr * 16 + 64 <= HEAD_BWD_SMEM_BUDGET) {
       R = r;
       break;
     }
@@ -953,8 +956,7 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   p.ones_c = ones_c;
   p.ngo = ngo;
   const size_t body = ((size_t)2 * HEAD_KC * p.KR * 16 + (size_t)2 * kcx * p.XR * 16 + 15) & ~(size_t)15;
-  p.smem_bytes = (int)(body + 64);
-  LPB_REQUIRE(p.smem_bytes <= 225 * 1024, "head_bwd_bf16: weight-gradient stages need %d B shared memory", p.smem_bytes);
+  p.smem_bytes = (int)(body + 64);  // within the budget: R was chosen so
   const int ngroups = kcx_total / kcx * ngo;  // CTA tiles
   const int nunits = B * (Hi / R);
   int slots = sms / ngroups;
@@ -962,7 +964,7 @@ static int launch_wgrad(const __nv_bfloat16* X, const __nv_bfloat16* G, float* d
   if (slots < 1) slots = 1;
   if (slots > nunits) slots = nunits;
   auto kern = kcx == 8 ? wgrad_kernel<4> : wgrad_kernel<2>;
-  LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, p.smem_bytes));
+  LPB_TRY(set_dynamic_smem(kern, p.smem_bytes, "head_bwd_bf16"));
   kern<<<slots * ngroups, WG_THREADS, p.smem_bytes, s>>>(p);
   const size_t stride = wgrad_part_stride(Cin, Cout);
   reduce_partials<1>(part, slots, stride, Cin * Cout * 9, dW, sms, s);
@@ -1127,9 +1129,9 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     set_error("head_bwd_bf16: feature map %dx%d outside this build's band tiling", H, W);
     return LPB_ERR_UNSUPPORTED;
   }
-  int dev = 0, sms = 0;
-  LPB_CUDA(cudaGetDevice(&dev));
-  LPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  DeviceLimits dev;
+  LPB_TRY(device_limits(&dev));
+  const int sms = dev.sms;
   const RowLayout L2 = make_row_layout(Hi2, Wi2), L1 = make_row_layout(Hi1, Wi1);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const int ntile1 = (C4 + 127) / 128;
@@ -1166,7 +1168,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
       jobs.zero[2] = {dw2, (long long)c1 * c2 * 9};
       jobs.zero[3] = {db2, (long long)c2};
     }
-    launch_head_prep(jobs, s);
+    launch_head_prep(jobs, sms, s);
   }
   {
     // gradient front end on the head's OUTPUT grid: G2 for a two-deconv head, G1 for a one-deconv head
@@ -1212,17 +1214,17 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     if (p.R2 > Hi2) p.R2 = Hi2;
     const int rows_alloc = (Wi2 + 2 + B2D_TILES * 128 + 7) & ~7;
     const size_t smem = (size_t)HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 32 * 16 + 64;
-    LPB_REQUIRE(smem <= 113 * 1024 && p.R2 >= 1, "head_bwd_bf16: layer-2 width %d too large", Wi2);
+    LPB_REQUIRE(smem <= HEAD_STAGE_SMEM_BUDGET && p.R2 >= 1, "head_bwd_bf16: layer-2 width %d too large", Wi2);
     int grid = B < 2 * sms ? B : 2 * sms;
     if (grid > B2D_MAX_CTAS) grid = B2D_MAX_CTAS;  // the bias partials' workspace
     if (!wide) {
-      LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      LPB_TRY(set_dynamic_smem(b2d_dgrad_kernel<false>, smem, "head_bwd_bf16"));
       b2d_dgrad_kernel<false><<<grid, B2D_THREADS, smem, s>>>(p);
       reduce_partials<1>(part_db1, grid * 4, HEAD_CLS, c1, db1, sms, s);
     } else {
       // keypoint groups: the mid activations' gradient in fp32 planes, the c2 groups added in order per c1 group, then
       // written as G1 by the front end's writer (a dense gradient, no softmax) and the bias gradient from G1's columns
-      LPB_CUDA(cudaFuncSetAttribute(b2d_dgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      LPB_TRY(set_dynamic_smem(b2d_dgrad_kernel<true>, smem, "head_bwd_bf16"));
       p.dmid = dmid;
       p.kc_frame = g2 * HEAD_KC;
       for (int t = 0; t < g1; ++t)
@@ -1266,7 +1268,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.acc_in = p.acc_out = p.kc0 = 0;
     const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
     size_t smem = (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
-    LPB_REQUIRE(smem <= 225 * 1024, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
+    LPB_REQUIRE(smem <= HEAD_BWD_SMEM_BUDGET, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
     // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit and the tensor map
     // encodes; otherwise direct 16-byte stores (dfeat's alignment was checked with the arguments)
     CUtensorMap tmap;
@@ -1274,7 +1276,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.tma_store = 0;
     if (!acc32) {  // (the groups' fp32 sums take the direct stores)
       const size_t stage = (size_t)2 * 4 * 128 * 4 * W + 128;
-      if (smem + stage <= 225 * 1024 && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
+      if (smem + stage <= HEAD_BWD_SMEM_BUDGET && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
         p.tma_store = 1;
         smem += stage;
       }
@@ -1284,12 +1286,12 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     if (slots > B) slots = B;
     auto run = [&](auto kern, auto kern_acc) -> int {
       if (!acc32) {
-        LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        LPB_TRY(set_dynamic_smem(kern, smem, "head_bwd_bf16"));
         kern<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap);
         return LPB_OK;
       }
       // keypoint groups of c1: one launch per group, in order, each adding its d features to the groups' fp32 sums
-      LPB_CUDA(cudaFuncSetAttribute(kern_acc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      LPB_TRY(set_dynamic_smem(kern_acc, smem, "head_bwd_bf16"));
       for (int g = 0; g < g1; ++g) {
         p.wpk = wp1 + (size_t)g * ntile1 * 4 * HEAD_KC * 128 * 8;
         p.kc0 = g * HEAD_KC;

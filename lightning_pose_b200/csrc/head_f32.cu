@@ -240,13 +240,22 @@ __global__ void __launch_bounds__(256) plane_softmax_kernel(float* __restrict__ 
   for (int i = threadIdx.x; i < hw; i += 256) p[i] = pl[i] * inv;
 }
 
+// n_planes >= 1 planes of hw pixels each, softmaxed in place; `entry` names the caller in errors
+static int launch_plane_softmax(float* x, int64_t n_planes, int hw, const char* entry, cudaStream_t s) {
+  const size_t smem = (size_t)hw * sizeof(float);
+  LPB_TRY(set_dynamic_smem(plane_softmax_kernel, smem, entry));
+  plane_softmax_kernel<<<(unsigned)n_planes, 256, smem, s>>>(x, hw);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
 
 template <bool SHUFFLE, int NT>
 static int launch_fwd_nt(const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias, int Cout, float* out,
                           cudaStream_t s) {
   const PixBlocks pb = pix_blocks(Hi, Wi);
   const size_t smem = ((size_t)FW_CC * pad8_32((pb.RB + 1) * (pb.CB + 1)) + 2 * 9 * FW_CC * bstride<NT>()) * sizeof(float);
-  LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_kernel<SHUFFLE, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(convt3x3s2_kernel<SHUFFLE, NT>, smem, "convt_fwd_f32"));
   const dim3 grid((unsigned)((size_t)B * pb.n), (unsigned)((Cout + 8 * NT - 1) / (8 * NT)));
   convt3x3s2_kernel<SHUFFLE, NT><<<grid, TC_THREADS, smem, s>>>(in, Cin, Hi, Wi, wt, bias, Cout, pb.RB, pb.CB, out);
   LPB_CUDA(cudaGetLastError());
@@ -509,13 +518,12 @@ static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cou
   const int np_max = CN / 9 + 2;
   const size_t smem =
       ((size_t)CM * WG_PS + (size_t)np_max * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1)) + TC_SLOTS + np_max) * sizeof(float);
-  LPB_CUDA(cudaFuncSetAttribute(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT>, smem, "convt_bwd_f32"));
   // K split: about two CTAs per SM in all, each with as many units as that leaves (fewer atomics than one per unit)
-  int dev = 0, sms = 132;
-  LPB_CUDA(cudaGetDevice(&dev));
-  LPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  DeviceLimits dev;
+  LPB_TRY(device_limits(&dev));
   const long long units = (long long)B * pb.n;
-  const long long ks = std::min<long long>(units, std::max<long long>(1, (2LL * sms + nct * nnt - 1) / (nct * nnt)));
+  const long long ks = std::min<long long>(units, std::max<long long>(1, (2LL * dev.sms + nct * nnt - 1) / (nct * nnt)));
   const dim3 grid((unsigned)(nct * nnt), (unsigned)ks);
   convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, dw, db);
   LPB_CUDA(cudaGetLastError());
@@ -533,7 +541,7 @@ static int launch_bwd(const float* in, const float* g, int B, int Cin, int Hi, i
   const size_t gfl = (size_t)8 * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1));
   auto go = [&](auto kernel, int nt, int stride) -> int {
     const size_t smem = (gfl + (size_t)2 * 72 * stride) * sizeof(float);
-    LPB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LPB_TRY(set_dynamic_smem(kernel, smem, "convt_bwd_f32"));
     const dim3 grid((unsigned)((size_t)B * pb.n), (unsigned)((Cin + 8 * nt - 1) / (8 * nt)));
     kernel<<<grid, TC_THREADS, smem, s>>>(g, Cout, Hi, Wi, wt, Cin, pb.RB, pb.CB, din);
     LPB_CUDA(cudaGetLastError());
@@ -563,12 +571,7 @@ extern "C" int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* s
   using namespace lpb;
   LPB_REQUIRE(x && n_planes >= 0 && hw >= 1, "plane_softmax_f32: bad arguments");
   if (n_planes == 0) return LPB_OK;
-  const size_t smem = (size_t)hw * sizeof(float);
-  LPB_REQUIRE(smem <= 200 * 1024, "plane_softmax_f32: plane of %d pixels too large for the softmax stage", hw);
-  if (smem > 48 * 1024) LPB_CUDA(cudaFuncSetAttribute(plane_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  plane_softmax_kernel<<<(unsigned)n_planes, 256, smem, static_cast<cudaStream_t>(stream)>>>(x, hw);
-  LPB_CUDA(cudaGetLastError());
-  return LPB_OK;
+  return launch_plane_softmax(x, n_planes, hw, "plane_softmax_f32", static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
@@ -620,14 +623,6 @@ extern "C" int lpb_head_fwd_f32(const float* features, int B, int C, int H, int 
     Ho = 4 * Hs;
     Wo = 4 * Ws;
   }
-  if (final_softmax) {
-    const int hw = Ho * Wo;
-    const size_t smem = (size_t)hw * sizeof(float);
-    LPB_REQUIRE(smem <= 200 * 1024, "head_fwd_f32: plane %dx%d too large for the softmax stage", Ho, Wo);
-    if (smem > 48 * 1024)
-      LPB_CUDA(cudaFuncSetAttribute(plane_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    plane_softmax_kernel<<<(unsigned)((size_t)B * K), 256, smem, s>>>(out, hw);
-    LPB_CUDA(cudaGetLastError());
-  }
+  if (final_softmax) return launch_plane_softmax(out, (int64_t)B * K, Ho * Wo, "head_fwd_f32", s);
   return LPB_OK;
 }

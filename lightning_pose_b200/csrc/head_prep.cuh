@@ -104,6 +104,6 @@ struct PrepJobs {
 };
 
 template <typename T = __nv_bfloat16>
-int launch_head_prep(const PrepJobs& jobs, cudaStream_t s);
+int launch_head_prep(const PrepJobs& jobs, int sms, cudaStream_t s);
 
 }  // namespace lpb

@@ -41,6 +41,14 @@ int launch_rows_shuffle(const T* feat, int B, int C, int H, int W, T* xs, cudaSt
 template <typename T>
 int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s);
 
+// The shuffle stage holds a CTA's 32 channels of one H x W feature map.  Its budget is the public feature-map limit of
+// the banded path (lpb_head_bf16_plan): maps up to 56 x 56.
+constexpr size_t HEAD_FEATURE_SMEM_BUDGET = 200 * 1024;
+inline size_t rows_shuffle_smem_bytes(int H, int W) { return (size_t)32 * H * W * 2; }
+// Stage budget of the banded kernel and of the backward's layer-2 data gradient (b2d, two CTAs per SM): half of an H100
+// SM's 227 KB.
+constexpr size_t HEAD_STAGE_SMEM_BUDGET = 113 * 1024;
+
 // raster rows per band of the banded kernel (its M-tiles x 128)
 constexpr int CR_BAND_ROWS = 256;
 // bands the banded kernel cuts an (Hi x Wi) conv input into (R = CR_BAND_ROWS / (Wi + 1) image rows each)

@@ -65,9 +65,9 @@ __global__ void __launch_bounds__(256) rows_shuffle_kernel(const uint16_t* __res
 template <typename T>
 int launch_rows_shuffle(const T* feat, int B, int C, int H, int W, T* xs, cudaStream_t s) {
   const RowLayout L = make_row_layout(2 * H, 2 * W);
-  const size_t smem = (size_t)32 * H * W * 2;
-  LPB_REQUIRE(smem <= 200 * 1024, "%s: feature map %dx%d too large for the shuffle stage", head_fwd_name<T>, H, W);
-  if (smem > 48 * 1024) LPB_CUDA(cudaFuncSetAttribute(rows_shuffle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const size_t smem = rows_shuffle_smem_bytes(H, W);
+  LPB_REQUIRE(smem <= HEAD_FEATURE_SMEM_BUDGET, "%s: feature map %dx%d too large for the shuffle stage", head_fwd_name<T>, H, W);
+  LPB_TRY(set_dynamic_smem(rows_shuffle_kernel, smem, head_fwd_name<T>));
   rows_shuffle_kernel<<<(unsigned)(B * (C / 32)), 256, smem, s>>>(reinterpret_cast<const uint16_t*>(feat), C, H, W, reinterpret_cast<uint16_t*>(xs), L);
   return LPB_OK;
 }
@@ -431,11 +431,11 @@ int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s) {
   p.rows_alloc = (tiles * 128 + Pp + 1 + 7) & ~7;
   if (p.rows_alloc < (p.R + 1) * Pp + 8) p.rows_alloc = ((p.R + 1) * Pp + 8 + 7) & ~7;
   const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + HEAD_BSTAGE_BYTES) + (2 * HEAD_CLS * 8 + 2 * HEAD_CLS) * sizeof(float) + 64;
-  LPB_REQUIRE(smem <= 113 * 1024, "%s: band stages need %zu B shared memory", name, smem);
+  LPB_REQUIRE(smem <= HEAD_STAGE_SMEM_BUDGET, "%s: band stages need %zu B shared memory", name, smem);
   const int nbands = (p.L.Hi + p.R - 1) / p.R;
   auto run = [&](auto kern, long long nitems) -> int {
     const int grid = (int)(nitems < sms ? nitems : sms);  // one CTA per SM: the accumulators take the register file
-    LPB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LPB_TRY(set_dynamic_smem(kern, smem, name));
     kern<<<grid, CR_THREADS, smem, s>>>(p);
     return LPB_OK;
   };

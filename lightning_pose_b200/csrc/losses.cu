@@ -750,9 +750,7 @@ extern "C" int lpb_unsup_losses_fwd(const float* keypoints, const float* confide
   const size_t fl2 = pca_scratch_floats(mv, T, false);
   fl = fl > fl2 ? fl : fl2;
   const size_t smem = (fl + 4) * sizeof(float);
-  LPB_REQUIRE(smem <= 200 * 1024, "unsup_losses_fwd: clip too large for shared memory (%zu B)", smem);
-  if (smem > 48 * 1024)
-    LPB_CUDA(cudaFuncSetAttribute(unsup_losses_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(unsup_losses_fwd_kernel, smem, "unsup_losses_fwd"));
   unsup_losses_fwd_kernel<<<(unsigned)n_clips, UL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
       keypoints, confidences, T, K, temporal_eps, prob_threshold, temporal_enabled, sv, mv, out);
   LPB_CUDA(cudaGetLastError());
@@ -776,9 +774,7 @@ extern "C" int lpb_unsup_losses_bwd(const float* keypoints, const float* confide
   const size_t fl2 = pca_scratch_floats(mv, T, true);
   fl = fl > fl2 ? fl : fl2;
   const size_t smem = (fl + (size_t)T * K * 2 + 4) * sizeof(float);
-  LPB_REQUIRE(smem <= 200 * 1024, "unsup_losses_bwd: clip too large for shared memory (%zu B)", smem);
-  if (smem > 48 * 1024)
-    LPB_CUDA(cudaFuncSetAttribute(unsup_losses_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(unsup_losses_bwd_kernel, smem, "unsup_losses_bwd"));
   unsup_losses_bwd_kernel<<<(unsigned)n_clips, UL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
       keypoints, confidences, T, K, temporal_eps, prob_threshold, temporal_enabled, sv, mv, grad_out, grad_keypoints);
   LPB_CUDA(cudaGetLastError());
@@ -855,10 +851,7 @@ extern "C" int lpb_plane_softmax_bwd(const float* probs, const float* grad_probs
   LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31) && hw >= 1, "plane_softmax_bwd: bad shape");
   if (n_planes == 0) return LPB_OK;
   const size_t smem = (size_t)2 * hw * sizeof(float);
-  LPB_REQUIRE(smem <= 200 * 1024, "plane_softmax_bwd: plane of %d pixels too large", hw);
-  // opt in whatever the size: the kernel's static shared memory comes on top of the dynamic 2 * hw floats, so a
-  // plane of exactly 48 KiB (64 x 96 pixels) already needs it
-  LPB_CUDA(cudaFuncSetAttribute(plane_softmax_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(plane_softmax_bwd_kernel, smem, "plane_softmax_bwd"));
   plane_softmax_bwd_kernel<<<(unsigned)n_planes, HL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(probs, grad_probs, hw,
                                                                                                       grad_logits);
   LPB_CUDA(cudaGetLastError());

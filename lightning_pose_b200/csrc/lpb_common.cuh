@@ -29,6 +29,37 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
     if (e__ != cudaSuccess) return ::lpb::cuda_fail(e__, #call, __FILE__, __LINE__); \
   } while (0)
 
+// an LPB_* status: returned as is unless it is LPB_OK
+#define LPB_TRY(call)                  \
+  do {                                 \
+    const int rc__ = (call);           \
+    if (rc__ != LPB_OK) return rc__;   \
+  } while (0)
+
+// ---- the current device (abi.cu) ----------------------------------------------------------------
+struct DeviceLimits {
+  int sms;       // streaming multiprocessors
+  int max_smem;  // opt-in shared memory per block, bytes (static plus dynamic)
+};
+// The current device's limits, queried once per device ordinal.  LPB_OK, or LPB_ERR_CUDA with the message set.
+int device_limits(DeviceLimits* d);
+// For shape planners that must answer without a GPU too: the current device's limits, or an H100 SXM's (132 SMs,
+// 227 KB) when there is no device to ask.
+DeviceLimits planning_limits();
+
+// ---- launches with dynamic shared memory --------------------------------------------------------
+// Every launch with dynamic shared memory first sets its kernel's limit to the bytes it requests.  CUDA refuses that when
+// the kernel's static plus dynamic memory exceeds the device's opt-in limit: LPB_ERR_UNSUPPORTED, naming the entry point
+// and the bytes, with the refusal cleared so that a later cudaGetLastError does not report it.
+int smem_refused(cudaError_t e, const char* entry, size_t bytes);
+template <typename Kernel>
+int set_dynamic_smem(Kernel* kernel, size_t bytes, const char* entry) {
+  const cudaError_t e = bytes <= (size_t)INT32_MAX
+                            ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes)
+                            : cudaErrorInvalidValue;
+  return e == cudaSuccess ? LPB_OK : smem_refused(e, entry, bytes);
+}
+
 // A caller's device pointer that is null or a multiple of `bytes`.  Entry points check the buffers their kernels move with
 // vector accesses, bulk copies or TMA up front: a misaligned one would otherwise fault on the device.
 inline bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }

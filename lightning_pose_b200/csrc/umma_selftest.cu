@@ -73,8 +73,7 @@ extern "C" int lpb_selftest_umma(const void* a, int kca, int rows_a, const void*
   P.row_shift = row_shift;
   (void)col_off;
   const size_t smem = (size_t)(kca * rows_a + kcb * rows_b) * 16 + 64;
-  LPB_REQUIRE(smem <= 200 * 1024, "selftest_umma: operands too large");
-  LPB_CUDA(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LPB_TRY(set_dynamic_smem(umma_selftest_kernel, smem, "selftest_umma"));
   umma_selftest_kernel<<<1, 128, smem, static_cast<cudaStream_t>(stream)>>>(P);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;

@@ -520,7 +520,8 @@ def test_unsup_losses_bench_clips(lpb, dev, golden):
 
 def test_unsup_losses_large_shared_memory_route(lpb, dev):
     """Multi-view PCA, 4 views x 17 keypoints, 3 components, T = 80: the clip needs more than the default 48 KB of shared
-    memory in both directions (losses.cu:753-755, :779-781) and stays under the 200 KB limit."""
+    memory in both directions, so both launches opt in to more (``set_dynamic_smem`` in lpb_common.cuh, called by
+    ``lpb_unsup_losses_fwd`` and ``lpb_unsup_losses_bwd``).  Both sizes stay well inside an H100's 227 KB."""
     views, t, nc, n_clips = 4, 80, 3, 3
     kk = views * K
     fwd = (_pca_scratch_floats(K, views, nc, t, False) + 4) * 4
