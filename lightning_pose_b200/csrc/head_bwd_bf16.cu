@@ -405,7 +405,10 @@ __global__ void __launch_bounds__(B2D_THREADS, 2) b2d_dgrad_kernel(const __grid_
 // =====================================================================================================
 // b3a: data gradient of the first deconv + inverse PixelShuffle:  G1 -> d features (NCHW bf16)
 // =====================================================================================================
-constexpr int B3A_THREADS = 320;  // warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue (lane = channel, two warps per 32-channel quarter)
+// 8 MMA + epilogue warps, two per 32-channel quarter of the CTA's 128 channels; lane 0-9 of warp 0 also issue the
+// operand copies.  Two warps per SM sub-partition leave each thread up to 255 registers (10 warps would cap it at 168),
+// which the weight fragments held in registers need.
+constexpr int B3A_THREADS = 256;
 
 struct B3aParams {
   const __nv_bfloat16* G1;   // [B][10][L.rows][8] padded row layout
@@ -423,22 +426,70 @@ struct B3aParams {
   int acc_in, acc_out, kc_frame, kc0;
 };
 
-// TMA tensor store of d features.  The tensor map views the NCHW gradient as [b][c'][pl][px] (source plane 4c' + pl,
-// px = H*W pixels); a box is {2 feature rows, one pl, 128 c', one frame}: in shared memory 128 rows of 4*WS2 bytes, so
-// thread c' writes at a 4*WS2-byte stride (conflict-free for WS2 = 12) and the copy engine does the 1152-byte-strided
-// scatter that cost the epilogue 32 half-used sectors per store instruction.
+// TMA tensor store of d features.  The tensor maps view the NCHW gradient as [b][c'][pl][px] (source plane 4c' + pl,
+// px = H*W pixels); a box is {2 or 4 feature rows, one pl, 128 c', one frame}: in shared memory 128 rows of 4*WS2 or
+// 8*WS2 bytes, and the copy engine does the plane-strided scatter.
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, const void* smem_src, int x0, int x1, int x2, int x3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tm), "r"(smem_u32(smem_src)), "r"(x0),
                "r"(x1), "r"(x2), "r"(x3)
                : "memory");
 }
-__device__ __forceinline__ void bulk_wait_group_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// A frame is processed in bands of Hh image rows (N = Hh * (Wi + 1) accumulator columns per band; the band's gradient
-// rows plus the halo row above are double-buffered in shared memory).
+// Column tiling of b3a (W = WS2, the feature width).  A work item is (di, pair of feature rows i, i + 1) of one frame:
+// shuffled rows m = 2i + di and m + 2 of the band.  Its columns go in plane order: for dj = 0, 1, the 2W pixels
+// (2i' + di, 2j + dj), i' = i, i + 1, j < W, which are 2W consecutive elements of source plane 4c + 2di + dj in NCHW.
+// So an item is B3aCols::NTI = W / 2 n8 tiles (W / 4 per dj) with no padding or wasted column, and the accumulator pair
+// (2t, 2t + 1) of a thread is two adjacent pixels of one plane.  ldmatrix takes one row address per lane, so the G1 rows
+// of a tile can be any 8 raster rows.  The tiles are computed in chunks of NT, with the chunk sized from W so that the
+// accumulators fit beside the 112 registers of weights without spilling (larger chunks spill at W = 32).
+template <int WS2>
+struct B3aCols {
+  static constexpr int TPD = WS2 / 4;  // n8 tiles per dj
+  static constexpr int NTI = 2 * TPD;  // n8 tiles per item
+  static constexpr int NT_MAX = 6;
+  static constexpr int nt() {
+    int n = 2;
+    for (int d = 2; d <= NT_MAX && d <= NTI; d += 2)
+      if (NTI % d == 0) n = d;
+    return n;
+  }
+  static constexpr int NT = nt();  // n8 tiles per chunk: the largest even divisor of NTI up to NT_MAX
+  static constexpr int NCHUNK = NTI / NT;
+  static_assert(WS2 % 4 == 0 && NTI % NT == 0 && NT % 2 == 0, "b3a column tiling");
+  // band column of tile T's column n (T < NTI, n < 8), relative to the item's first accumulator row
+  __device__ static int col(int T, int n) {
+    const int dj = T / TPD, x = 8 * (T % TPD) + n;  // x: index into the plane's 2W run
+    return (x / WS2) * 2 * (2 * WS2 + 1) + 2 * (x % WS2) + dj;
+  }
+};
+// the 14 non-zero (shift, k16) steps in issue order: shift 0..3, k16 = shift..4
+__host__ __device__ constexpr int b3a_kstep(int sh, int k16) { return 5 * sh - sh * (sh - 1) / 2 + k16 - sh; }
+constexpr int B3A_KSTEPS = b3a_kstep(3, 4) + 1;
+static_assert(B3A_KSTEPS == 14, "b3a: 14 non-zero (shift, k16) weight steps");
+
+// f(channel row within the warp, dj, x, D(x), D(x + 1)) for every accumulator pair of chunk ch: x indexes the plane's
+// 2W run, and the pair is two adjacent pixels of it
+template <int WS2, typename F>
+__device__ __forceinline__ void b3a_each_pair(int ch, const float (&acc)[2][B3aCols<WS2>::NT][4], int lane, F&& f) {
+  constexpr int NT = B3aCols<WS2>::NT, TPD = B3aCols<WS2>::TPD;
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      const int T = ch * NT + t, dj = T / TPD, x = 8 * (T % TPD) + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) f(16 * m + 8 * h + (lane >> 2), dj, x, acc[m][t][2 * h], acc[m][t][2 * h + 1]);
+    }
+}
+
+// A frame is processed in bands of Hh image rows (the band's gradient rows plus the halo row above are double-buffered
+// in shared memory).
 template <int WS2, bool ACC = false>
-__global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_constant__ B3aParams P, const __grid_constant__ CUtensorMap TM) {
+__global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_constant__ B3aParams P, const __grid_constant__ CUtensorMap TM,
+                                                                   const __grid_constant__ CUtensorMap TM_PAIR) {
+  using Cols = B3aCols<WS2>;
+  constexpr int NT = Cols::NT;
   extern __shared__ __align__(1024) unsigned char smem[];
   const int Wi = P.Wi, Hi = P.Hi, Pp = Wi + 1, LEAD = Pp + 1;
   const int Hh = P.Hh, nbands = (Hi + Hh - 1) / Hh;
@@ -451,7 +502,7 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
   uint64_t* g_full = bars;       // [2]
   uint64_t* g_empty = bars + 2;  // [2]
   uint64_t* w_full = bars + 4;
-  // staging slices of the TMA store: [ip & 1][pl][128 lanes][4 * WS2 bytes]
+  // staging slices of the TMA store: [pl][128 channels][2 items][4 * WS2 bytes]
   unsigned char* Ss = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(bars + 12) + 127) & ~(uintptr_t)127);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntile = (P.C4 + 127) / 128;
@@ -469,183 +520,155 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
   fence_proxy_async();
   __syncthreads();
 
+  // operand copies, issued by warp 0: the weights once, then the bands in (frame, band) order, each into stage j % 2 once
+  // every warp has arrived on that stage's g_empty for band j - 2
+  int lb = slot, lband = 0;  // the next band to copy
+  auto load_next = [&](int j) {
+    const int st = j & 1, y0 = lband * Hh, hb = min(Hh, Hi - y0);
+    // one copy per K-chunk: the zero entry before image row y0 - 1, that row (zero lead rows of the layout when
+    // y0 = 0), and the band's rows, zero columns included
+    const uint32_t nbytes = (uint32_t)((1 + (hb + 1) * Pp) * 16);
+    if (lane < HEAD_KC) {
+      if (lane == 0) mbar_expect_tx(&g_full[st], HEAD_KC * nbytes);
+      __syncwarp((1u << HEAD_KC) - 1);
+      bulk_g2s(Gs + (size_t)st * g_bytes + (size_t)lane * rows_alloc * 16,
+               P.G1 + (((size_t)lb * (ACC ? P.kc_frame : HEAD_KC) + (ACC ? P.kc0 : 0) + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8,
+               nbytes, &g_full[st]);
+    }
+    if (++lband == nbands) lband = 0, lb += nslot;
+  };
   if (warp == 0) {
     if (lane == 0) {
       mbar_expect_tx(w_full, (uint32_t)w_bytes);
       bulk_g2s(Ws, reinterpret_cast<const unsigned char*>(P.wpk) + (size_t)mt * w_bytes, (uint32_t)w_bytes, w_full);
     }
+    for (int j = 0; j < 2 && lb < P.B; ++j) load_next(j);
+  }
+  {
+    // MMA + epilogue: D[c][pixel] = sum_{shift, k} W1[shift][c][k] * G1[pixel - shift][k], M = channels, N = pixels.  Warp
+    // (q, e) owns the 32 channels 32 q .. 32 q + 31 of the CTA's 128-channel tile (two m16 tiles) and the items with di = e;
+    // the band's whole K is resident, and the warp's weight fragments sit in registers for the whole launch.
+    const int q = warp & 3, e = warp >> 2;
+    const int HW = (Hi / 2) * WS2;
+    const uint32_t lbo_g = rows_alloc * 16, lbo_w = 128 * 16;
+    mbar_wait(w_full, 0);
+    uint32_t af[B3A_KSTEPS][2][4];  // A fragments of the 14 non-zero (shift, k16) steps x 2 m16 tiles
+#pragma unroll
+    for (int sh = 0; sh < 4; ++sh)
+#pragma unroll
+      for (int k16 = sh; k16 < HEAD_NCOLS / 16; ++k16)
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+          mma::ldsm_x4(af[b3a_kstep(sh, k16)][m], smem_u32(Ws) + ((sh * HEAD_KC + 2 * k16) * 128 + 32 * q + 16 * m + ((lane >> 3) & 1) * 8 + (lane & 7)) * 16 +
+                                                     (lane >> 4) * lbo_w);
+    // this lane's ldmatrix row of tile pair np of chunk ch: tile 2 np + lane / 16 of the chunk, column lane % 8, K-chunk
+    // (lane / 8) % 2 of the k16 step
+    auto b_row = [&](int ch, int np) { return (uint32_t)(LEAD + Cols::col(ch * NT + 2 * np + (lane >> 4), lane & 7)) * 16 + ((lane >> 3) & 1) * lbo_g; };
+    // one chunk of an item: each element is the same mma.sync sequence from zero, shift 0..3, k16 ascending, the
+    // all-zero k16 < shift steps skipped (K = (cls, o), cls = 2 py + px at stride 20: shift (dm, dn) has no tap for the
+    // classes with py < dm or px < dn, so its packed weights are zero for k < 20 (dn), k < 40 (dm), k < 60 (both))
+    auto mma_chunk = [&](uint32_t g_item, int ch, float (&acc)[2][NT][4]) {
+      mma::zero(acc);
+#pragma unroll
+      for (int sh = 0; sh < 4; ++sh) {
+        const int shift_rows = (sh >> 1) * Pp + (sh & 1);
+#pragma unroll
+        for (int k16 = sh; k16 < HEAD_NCOLS / 16; ++k16) {
+          const uint32_t g_k = g_item + (2 * k16) * lbo_g - shift_rows * 16;
+#pragma unroll
+          for (int np = 0; np < NT / 2; ++np) {
+            uint32_t bf[4];
+            mma::ldsm_x4(bf, g_k + b_row(ch, np));
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {
+              mma::mma_bf16(acc[m][2 * np], af[b3a_kstep(sh, k16)][m], bf[0], bf[1]);
+              mma::mma_bf16(acc[m][2 * np + 1], af[b3a_kstep(sh, k16)][m], bf[2], bf[3]);
+            }
+          }
+        }
+      }
+    };
     int it = 0;
     for (int b = slot; b < P.B; b += nslot)
       for (int band = 0; band < nbands; ++band, ++it) {
         const int st = it & 1, y0 = band * Hh, hb = min(Hh, Hi - y0);
-        mbar_wait(&g_empty[st], ((it >> 1) & 1) ^ 1);
-        // one copy per K-chunk: the zero entry before image row y0 - 1, that row (zero lead rows of the layout when
-        // y0 = 0), and the band's rows, zero columns included
-        const uint32_t nbytes = (uint32_t)((1 + (hb + 1) * Pp) * 16);
-        if (lane < HEAD_KC) {
-          if (lane == 0) mbar_expect_tx(&g_full[st], HEAD_KC * nbytes);
-          __syncwarp((1u << HEAD_KC) - 1);
-          bulk_g2s(Gs + (size_t)st * g_bytes + (size_t)lane * rows_alloc * 16,
-                   P.G1 + (((size_t)b * (ACC ? P.kc_frame : HEAD_KC) + (ACC ? P.kc0 : 0) + lane) * P.L.rows + P.L.lead + (size_t)(y0 - 1) * Pp - 1) * 8,
-                   nbytes, &g_full[st]);
-        }
-      }
-  } else if (warp >= 2) {
-    // MMA + epilogue.  The band's whole K (4 shifts x 80) is resident, so a warp computes each 16-pixel block of its 32
-    // channels (accumulator rows) when the epilogue needs it.  Thread = shuffled channel c (accumulator row); shuffled pixel (m, n) = (2i + di, 2j + dj) belongs to source
-    // plane 4c + 2di + dj.  A work item is (di, pair of feature rows i, i+1): two accumulator rows m = 2i + di and m + 2,
-    // i.e. 2 * WS2 consecutive elements of each of the planes dj = 0, 1 -> aligned 16-byte stores.  The two warps of a
-    // lane quarter take alternate items.
-    const int q = warp & 3, e = (warp - 2) >> 2;
-    const int c = mt * 128 + 32 * q + lane;
-    const int HW = (Hi / 2) * WS2;
-    constexpr int NCH = (2 * WS2 + 15) / 16;  // 16-column blocks per accumulator row
-    const uint32_t lbo_g = rows_alloc * 16, lbo_w = 128 * 16;
-    const uint32_t w0 = smem_u32(Ws);
-    mbar_wait(w_full, 0);
-    int it = 0, tma_cnt = 0;
-    for (int b = slot; b < P.B; b += nslot)
-      for (int band = 0; band < nbands; ++band, ++it) {
-        const int st = it & 1, y0 = band * Hh, hb = min(Hh, Hi - y0);
-        const int npairs = hb / 4;  // feature-row pairs in this band
+        const int nitems = 2 * (hb / 4);  // (di, feature-row pair) items of this band
         mbar_wait_idle(&g_full[st], (it >> 1) & 1);
         const uint32_t g0 = smem_u32(Gs + (size_t)st * g_bytes);
-        auto issue = [&](int item, float (&buf)[2][NCH * 16]) {
-          const int ml = 4 * (item >> 1) + (item & 1);  // first accumulator row of the item within this band
+        for (int item = e; item < nitems; item += 2) {
+          const int ip = item >> 1, ml = 4 * ip + e;  // ml: the item's first accumulator row within the band
+          const uint32_t g_item = g0 + (uint32_t)(ml * Pp) * 16;
+          if (!ACC && P.tma_store) {
+            // The 4 warps of this e form a group of 128 channels that owns the slices pl = 2e, 2e + 1.  Items go out in
+            // pairs (ip even, ip + 1): a slice row holds both items' 2W pixels of a channel's plane, 8W consecutive bytes
+            // of d features, and one tensor store per plane class writes them.  Single items' 4W-byte rows (48 bytes at
+            // W = 12) split 32-byte sectors between two stores, which made the stores take twice as long on an H100
+            // (DESIGN.md K4).  A band's last item without a partner (odd pair count) is stored alone, from a dense
+            // [128][4W bytes] slice.
+            constexpr int PB = 4 * WS2, SLICE = 128 * 2 * PB;  // bytes per channel and item / per slice
+            const bool issuer = (q == 0 && lane == 0);
+            const bool alone = ip + 1 == nitems / 2 && (ip & 1) == 0, last = alone || (ip & 1);
+            // row stride and offset of this item in the slice
+            const int rs = alone ? PB : 2 * PB, ro = (ip & 1) * PB;
+            unsigned char* sl = Ss + (size_t)(2 * e) * SLICE + (size_t)(32 * q) * rs + ro;
 #pragma unroll
-          for (int r = 0; r < 2; ++r)
-#pragma unroll
-            for (int k = 0; k < NCH; ++k) {
-              const int col0 = (ml + 2 * r) * Pp + 16 * k;  // first accumulator column (band pixel) of the block
-              float acc[2][2][4];
-              mma::zero(acc);
-#pragma unroll
-              for (int sh = 0; sh < 4; ++sh) {
-                const int shift_rows = (sh >> 1) * Pp + (sh & 1);
-#pragma unroll
-                for (int k16 = 0; k16 < HEAD_NCOLS / 16; ++k16) {
-                  // K = (cls, o), cls = 2 py + px at stride 20: shift (dm, dn) has no tap for classes with py < dm or px < dn,
-                  // so its packed weights are zero for k < 20 (dn), k < 40 (dm), k < 60 (both): the 16-wide chunks k16 < sh
-                  // are all-zero and skipped (14 of 20 remain)
-                  if (k16 < sh) continue;
-                  mma::kstep(acc, w0 + ((sh * HEAD_KC + 2 * k16) * 128 + 32 * q) * 16, lbo_w,
-                             g0 + (2 * k16) * lbo_g + (LEAD - shift_rows + col0) * 16, lbo_g, lane);
-                }
+            for (int ch = 0; ch < Cols::NCHUNK; ++ch) {
+              float acc[2][NT][4];
+              mma_chunk(g_item, ch, acc);
+              if (ch == 0 && (ip & 1) == 0) {
+                if (issuer) bulk_wait_group_read0();  // the group's last stores have read the slices
+                named_bar_sync(1 + e, 128);
               }
-              mma::rows8(acc, 0, &buf[r][16 * k], lane);
-              mma::rows8(acc, 1, &buf[r][16 * k + 8], lane);
+              b3a_each_pair<WS2>(ch, acc, lane, [&](int r, int dj, int x, float v0, float v1) {
+                *reinterpret_cast<__nv_bfloat162*>(sl + dj * SLICE + r * rs + 2 * x) = __floats2bfloat162_rn(v0, v1);
+              });
             }
-        };
-        auto emit = [&](int item, const float (&v)[2][NCH * 16]) {
-          if (c >= P.C4) return;
-          const int di = item & 1, ip = item >> 1;
-          const int i0 = y0 / 2 + 2 * ip;  // first feature row of the pair
-#pragma unroll
-          for (int dj = 0; dj < 2; ++dj) {
-            const size_t off = ((size_t)b * 4 * P.C4 + 4 * c + 2 * di + dj) * HW + (size_t)i0 * WS2;
-            __nv_bfloat16* dst = P.dfeat + off;
-            if constexpr (ACC) {
-              float* a32 = P.acc32 + off;
-#pragma unroll
-              for (int s4 = 0; s4 < (2 * WS2) / 8; ++s4) {
-                float f[8];
-#pragma unroll
-                for (int x = 0; x < 8; ++x) f[x] = v[(8 * s4 + x) / WS2][2 * ((8 * s4 + x) % WS2) + dj];
-                if (P.acc_in) {
-                  const float4 p0 = *reinterpret_cast<const float4*>(a32 + 8 * s4), p1 = *reinterpret_cast<const float4*>(a32 + 8 * s4 + 4);
-                  f[0] = p0.x + f[0], f[1] = p0.y + f[1], f[2] = p0.z + f[2], f[3] = p0.w + f[3];
-                  f[4] = p1.x + f[4], f[5] = p1.y + f[5], f[6] = p1.z + f[6], f[7] = p1.w + f[7];
-                }
-                if (P.acc_out) {
-                  *reinterpret_cast<float4*>(a32 + 8 * s4) = make_float4(f[0], f[1], f[2], f[3]);
-                  *reinterpret_cast<float4*>(a32 + 8 * s4 + 4) = make_float4(f[4], f[5], f[6], f[7]);
-                } else {
-                  uint32_t pk[4];
-#pragma unroll
-                  for (int e2 = 0; e2 < 4; ++e2) {
-                    __nv_bfloat162 h2 = __floats2bfloat162_rn(f[2 * e2], f[2 * e2 + 1]);
-                    pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
+            if (last) {
+              fence_proxy_async();
+              named_bar_sync(1 + e, 128);
+              if (issuer) {
+                const int px0 = (y0 / 2 + 2 * (ip & ~1)) * WS2;
+                const CUtensorMap* tm = alone ? &TM : &TM_PAIR;
+                tma_store_4d(tm, Ss + (size_t)(2 * e) * SLICE, px0, 2 * e, mt * 128, b);
+                tma_store_4d(tm, Ss + (size_t)(2 * e + 1) * SLICE, px0, 2 * e + 1, mt * 128, b);
+                bulk_commit_group();
+              }
+            }
+          } else {
+            const int c0 = mt * 128 + 32 * q, i0 = y0 / 2 + 2 * ip;  // the warp's first channel, the pair's first feature row
+            const size_t base = ((size_t)b * 4 * P.C4 + 4 * c0 + 2 * e) * HW + (size_t)i0 * WS2;
+            // (not unrolled: the chunks' operand addresses would stay live together and spill at W >= 24)
+#pragma unroll 1
+            for (int ch = 0; ch < Cols::NCHUNK; ++ch) {
+              float acc[2][NT][4];
+              mma_chunk(g_item, ch, acc);
+              b3a_each_pair<WS2>(ch, acc, lane, [&](int r, int dj, int x, float v0, float v1) {
+                if (c0 + r >= P.C4) return;
+                const size_t off = base + (size_t)((4 * r + dj) * HW + x);
+                __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(P.dfeat + off);
+                if constexpr (ACC) {
+                  float2* a32 = reinterpret_cast<float2*>(P.acc32 + off);
+                  if (P.acc_in) {
+                    const float2 p = *a32;
+                    v0 = p.x + v0, v1 = p.y + v1;
                   }
-                  *reinterpret_cast<uint4*>(dst + 8 * s4) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                  if (P.acc_out) *a32 = make_float2(v0, v1);
+                  else *dst = __floats2bfloat162_rn(v0, v1);
+                } else {
+                  *dst = __floats2bfloat162_rn(v0, v1);
                 }
-              }
-              continue;
+              });
             }
-#pragma unroll
-            for (int s4 = 0; s4 < (2 * WS2) / 8; ++s4) {  // 8 consecutive elements of [row r][j]
-              uint32_t pk[4];
-#pragma unroll
-              for (int e2 = 0; e2 < 4; ++e2) {
-                const int x0 = 8 * s4 + 2 * e2, x1 = x0 + 1;  // index into the 2*WS2 run
-                const float f0 = v[x0 / WS2][2 * (x0 % WS2) + dj];
-                const float f1 = v[x1 / WS2][2 * (x1 % WS2) + dj];
-                __nv_bfloat162 h2 = __floats2bfloat162_rn(f0, f1);
-                pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
-              }
-              *reinterpret_cast<uint4*>(dst + 8 * s4) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
-          }
-        };
-        const int nitems = 2 * npairs;
-        if (P.tma_store) {
-          // warps with the same e (= di) form a group of 128 lanes that owns the slices pl = 2e, 2e + 1; per item:
-          //   the group's issuer makes sure the copy that last read these slices is done, the group writes its
-          //   2 x (2 * WS2 / 8) 16-byte pieces per lane, and the issuer launches one tensor store per plane class
-          constexpr int PB = 4 * WS2, SLICE = 128 * PB;  // bytes per lane and slice / per slice
-          const bool issuer = (q == 0 && lane == 0);
-          float va[2][NCH * 16];
-          for (int item = e; item < nitems; item += 2, ++tma_cnt) {
-            issue(item, va);
-            const int ip = item >> 1, par = tma_cnt & 1;  // the group's slices alternate item by item
-            unsigned char* sl = Ss + (size_t)(par * 4 + 2 * e) * SLICE + (size_t)(32 * q + lane) * PB;
-            if (issuer) bulk_wait_group_read1();  // at most the previous item's stores (the other ip parity) still read smem
-            named_bar_sync(1 + e, 128);
-#pragma unroll
-            for (int dj = 0; dj < 2; ++dj) {
-#pragma unroll
-              for (int s4 = 0; s4 < (2 * WS2) / 8; ++s4) {
-                uint32_t pk[4];
-#pragma unroll
-                for (int e2 = 0; e2 < 4; ++e2) {
-                  const int x0 = 8 * s4 + 2 * e2, x1 = x0 + 1;
-                  __nv_bfloat162 h2 = __floats2bfloat162_rn(va[x0 / WS2][2 * (x0 % WS2) + dj], va[x1 / WS2][2 * (x1 % WS2) + dj]);
-                  pk[e2] = *reinterpret_cast<uint32_t*>(&h2);
-                }
-                *reinterpret_cast<uint4*>(sl + dj * SLICE + 16 * s4) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              }
-            }
-            fence_proxy_async();
-            named_bar_sync(1 + e, 128);
-            if (issuer) {
-              const int px0 = (y0 / 2 + 2 * ip) * WS2;
-              tma_store_4d(&TM, Ss + (size_t)(par * 4 + 2 * e) * SLICE, px0, 2 * e, mt * 128, b);
-              tma_store_4d(&TM, Ss + (size_t)(par * 4 + 2 * e + 1) * SLICE, px0, 2 * e + 1, mt * 128, b);
-              bulk_commit_group();
-            }
-          }
-        } else if (NCH <= 2) {
-          // the next item's blocks are computed before the current item is converted and stored
-          float va[2][NCH * 16], vb[2][NCH * 16];
-          if (e < nitems) issue(e, va);
-          for (int item = e; item < nitems; item += 4) {
-            if (item + 2 < nitems) issue(item + 2, vb);
-            emit(item, va);
-            if (item + 2 < nitems) {
-              if (item + 4 < nitems) issue(item + 4, va);
-              emit(item + 2, vb);
-            }
-          }
-        } else {
-          for (int item = e; item < nitems; item += 2) {
-            float v[2][NCH * 16];
-            issue(item, v);
-            emit(item, v);
           }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&g_empty[st]);  // this warp's reads of the band are done
+        if (warp == 0 && lb < P.B) {
+          mbar_wait(&g_empty[st], (it >> 1) & 1);  // every warp's are: band it + 2 may overwrite the stage
+          load_next(it + 2);
+        }
       }
-    if (P.tma_store && q == 0 && lane == 0) bulk_wait_group0();  // the stores have landed before the kernel ends
+    if (!ACC && P.tma_store && q == 0 && lane == 0) bulk_wait_group0();  // the stores have landed before the kernel ends
   }
 }
 
@@ -1269,14 +1292,17 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
     size_t smem = (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
     LPB_REQUIRE(smem <= HEAD_BWD_SMEM_BUDGET, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
-    // TMA tensor store of d features when its staging slices (2 x 4 x 128 lanes x 4W bytes) still fit and the tensor map
-    // encodes; otherwise direct 16-byte stores (dfeat's alignment was checked with the arguments)
-    CUtensorMap tmap;
+    // TMA tensor stores of d features when their staging slices (4 x 128 channels x 2 items x 4W bytes) still fit and the
+    // tensor maps (boxes of one item and of an item pair) encode; otherwise direct stores (dfeat's alignment was checked
+    // with the arguments)
+    CUtensorMap tmap, tmap_pair;
     memset(&tmap, 0, sizeof(tmap));
+    memset(&tmap_pair, 0, sizeof(tmap_pair));
     p.tma_store = 0;
     if (!acc32) {  // (the groups' fp32 sums take the direct stores)
-      const size_t stage = (size_t)2 * 4 * 128 * 4 * W + 128;
-      if (smem + stage <= HEAD_BWD_SMEM_BUDGET && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W)) {
+      const size_t stage = (size_t)4 * 128 * 2 * 4 * W + 128;
+      if (smem + stage <= HEAD_BWD_SMEM_BUDGET && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W) &&
+          make_dfeat_tensor_map(&tmap_pair, dfeat, B, C4, H * W, 4 * W)) {
         p.tma_store = 1;
         smem += stage;
       }
@@ -1287,7 +1313,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     auto run = [&](auto kern, auto kern_acc) -> int {
       if (!acc32) {
         LPB_TRY(set_dynamic_smem(kern, smem, "head_bwd_bf16"));
-        kern<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap);
+        kern<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap, tmap_pair);
         return LPB_OK;
       }
       // keypoint groups of c1: one launch per group, in order, each adding its d features to the groups' fp32 sums
@@ -1297,7 +1323,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
         p.kc0 = g * HEAD_KC;
         p.acc_in = g > 0;
         p.acc_out = g < g1 - 1;
-        kern_acc<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap);
+        kern_acc<<<slots * ntile1, B3A_THREADS, smem, s>>>(p, tmap, tmap_pair);
       }
       return LPB_OK;
     };

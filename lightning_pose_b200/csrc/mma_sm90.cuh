@@ -4,7 +4,8 @@
 //
 // A warp owns a block of 32 accumulator rows (two m16 tiles) x 8*NT columns (NT n8 tiles):
 //   acc[mt][nt][0..3] = D(16 mt + g, 8 nt + 2 t + {0, 1}) and D(16 mt + g + 8, ...)   (g = lane / 4, t = lane % 4).
-// rows8() turns one n8 tile into "lane = accumulator row" form, the layout every epilogue of the head reads.
+// rows8() turns one n8 tile into "lane = accumulator row" form, the layout the head's epilogues read (all but b3a's,
+// which stores the fragments as they are).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

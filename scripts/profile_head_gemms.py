@@ -8,6 +8,8 @@ prints two counts of mma.sync m16n8k16 FLOPs and the rate each implies over the 
   non-zero   -- only the tiles whose weights hold one of the 9 real (class, shift) taps of 16 (head_prep.cuh NZ_N8 /
                 NZ_M16; for the banded kernel, of the columns its epilogue reads).
 Kernels that skip the zero tiles issue the non-zero count; kernels that do not, the all-tiles count.  The card's name, power limit and SM clocks are read in the same run.
+For b3a_dgrad_kernel (layer-1 data gradient) it prints the FLOPs it issues and the useful ones (2 x 9 taps x c1 per d
+feature), with the rate each implies.
 It also prints the head backward's fixed-order gradient sums (every reduce_partials* launch) as one row: µs and launches per step.
 
     python scripts/profile_head_gemms.py [--clips 16] [--steps 10] [--warmup 3] [--json OUT]
@@ -78,6 +80,14 @@ def wgrad_flops(frames: int, hi: int, wi: int, nkc: int) -> tuple[float, float]:
     return all_t * MMA_FLOP, nonzero * MMA_FLOP
 
 
+def b3a_flops(frames: int, c: int, h: int, w: int, c1: int) -> tuple[float, float]:
+    """b3a: per (frame, 128-channel tile, (di, feature-row pair) item), 4 warps x W / 2 n8 tiles x 2 m16 tiles x the 14
+    non-zero (shift, k16) steps; useful: 9 taps x c1 multiply-adds per d feature"""
+    tiles = -(-c // 4 // 128)
+    issued = frames * tiles * h * 4 * (w // 2) * 2 * 14
+    return issued * MMA_FLOP, frames * c * h * w * 2 * 9 * c1
+
+
 def gpu_info() -> dict:
     q = "name,power.limit,clocks.sm,clocks.max.sm"
     try:
@@ -131,6 +141,10 @@ def main():
         "convt_rows_kernel": rows_flops(nf, 4 * h, 4 * h, 2),
         "wgrad_kernel": tuple(a + b for a, b in zip(wgrad_flops(nf, 2 * h, 2 * h, c4 // 8), wgrad_flops(nf, 4 * h, 4 * h, 4))),
     }
+    b3a_us = sum(v for k, v in per.items() if "b3a_dgrad_kernel" in k)
+    issued, useful = b3a_flops(nf, bench.FEAT_C, h, h, bench.K_PTS)
+    b3a = {"kernel": "b3a_dgrad_kernel", "us_per_step": round(b3a_us, 1), "issued_tflop": round(issued / 1e12, 4), "useful_tflop": round(useful / 1e12, 4),
+           "issued_tflops": round(issued / b3a_us / 1e6, 1) if b3a_us else None, "useful_tflops": round(useful / b3a_us / 1e6, 1) if b3a_us else None}
     rows = []
     for name, (all_t, nz) in gemms.items():
         us = sum(v for k, v in per.items() if name in k)
@@ -138,13 +152,15 @@ def main():
                      "all_tiles_tflops": round(all_t / us / 1e6, 1) if us else None, "nonzero_tflops": round(nz / us / 1e6, 1) if us else None})
     top = sorted(per.items(), key=lambda kv: -kv[1])[:15]
     res = {"gpu": info, "clocks_during_profile": clocks, "frames_per_step": nf, "steps": args.steps,
-           "kernel_us_per_step_total": round(total, 1), "head_gemms": rows, "fixed_order_sums": fixed_sums,
+           "kernel_us_per_step_total": round(total, 1), "head_gemms": rows, "b3a": b3a, "fixed_order_sums": fixed_sums,
            "top_kernels": [{"kernel": k[:90], "us_per_step": round(v, 1)} for k, v in top]}
     print(f"{info.get('name')}  power limit {info.get('power.limit')}  SM clock {clocks.get('sm_mhz')} MHz (max {clocks.get('sm_max_mhz')})  "
           f"{nf} frames/step, {args.steps} steps")
     print(f"{'kernel':28s} {'us/step':>9s} {'all-tiles TFLOP':>16s} {'non-zero TFLOP':>15s} {'all-tiles TFLOP/s':>18s} {'non-zero TFLOP/s':>17s}")
     for r in rows:
         print(f"{r['kernel']:28s} {r['us_per_step']:9.1f} {r['all_tiles_tflop']:16.4f} {r['nonzero_tflop']:15.4f} {r['all_tiles_tflops'] or 0:18.1f} {r['nonzero_tflops'] or 0:17.1f}")
+    print(f"{'b3a_dgrad_kernel':28s} {b3a['us_per_step']:9.1f}  issued {b3a['issued_tflop']:.4f} TFLOP ({b3a['issued_tflops'] or 0:.1f} TFLOP/s), "
+          f"useful {b3a['useful_tflop']:.4f} TFLOP ({b3a['useful_tflops'] or 0:.1f} TFLOP/s)")
     print(f"{'fixed-order sums':28s} {fixed_sums['us_per_step']:9.1f} us/step in {fixed_sums['launches_per_step']:g} launches/step (reduce_partials*)")
     print(f"all kernels: {total:.1f} us/step (summed over both streams)")
     for t in res["top_kernels"]:
