@@ -127,10 +127,16 @@ int lpb_head_fwd_f32(const float* features, int B, int C, int H, int W, const fl
  * heads/heatmap.py:192-193), with its native backward -- the fp32 reference precision path trains through these.
  * Every convolution runs on the tensor cores in 3xTF32 (fp32 accuracy); any Cin, Cout, Hi, Wi (even with shuffle).
  *   lpb_convt_fwd_f32   in [B, Cin(*4 if shuffle), Hi(/2), Wi(/2)] -> out [B, Cout, 2Hi, 2Wi]; shuffle != 0 folds
- *                       PixelShuffle(2) into the load (Hi, Wi are the conv-input = shuffled sizes)
+ *                       PixelShuffle(2) into the load (Hi, Wi are the conv-input = shuffled sizes).  shuffle =
+ *                       LPB_SHUFFLE_NHWC: the same with `in` channels-last, [B, Hi/2, Wi/2, 4 Cin] in memory (and so
+ *                       grad_in of lpb_convt_bwd_f32); results are bit-identical to LPB_SHUFFLE_NCHW (= 1) on the same
+ *                       logical tensor.
  *   lpb_plane_softmax_f32  in-place spatial softmax (T = 1) of [n_planes, hw]
  *   lpb_convt_bwd_f32   autograd of lpb_convt_fwd_f32: grad_in (same shape as `in`, may be NULL), grad_w [Cin,Cout,3,3],
  *                       grad_bias [Cout] (may be NULL); all overwritten. */
+#define LPB_SHUFFLE_NONE 0
+#define LPB_SHUFFLE_NCHW 1
+#define LPB_SHUFFLE_NHWC 2
 int lpb_convt_fwd_f32(const float* in, int B, int Cin, int Hi, int Wi, int shuffle, const float* w, const float* bias,
                       int Cout, float* out, void* stream);
 int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* stream);
@@ -193,6 +199,35 @@ int lpb_head_bwd_bf16(const float* g_out, const float* probs, const float* win, 
                       const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H,
                       int W, const float* w1, int c1, const float* w2, int c2, void* dfeat, float* dw1, float* db1,
                       float* dw2, float* db2, void* workspace, void* stream);
+
+/* Channels-last features (torch.channels_last; a transformer encoder's tokens (B, H*W, C) viewed as (B, C, H, W)):
+ * the same head on features whose memory is [B, H, W, C], read and, for d features, written where they lie -- no NCHW
+ * copy on either side (the reference permutes the tokens, lightning_pose/models/heatmap_tracker_multiview.py forward_vit;
+ * heads/heatmap.py:203-212 is the forward these stand for).  The _layout entries are the entries above with a
+ * feature_layout argument, and LPB_FEATURES_NCHW makes them exactly those.  With LPB_FEATURES_NHWC:
+ *   lpb_head_bf16_plan_layout   plan[0] = 0 for every shape: the banded kernels serve all of them, so saved_xs is always
+ *                        REQUIRED by the forward (inference: scratch), and the NCHW shuffle stage's feature-map limit
+ *                        does not apply.
+ *   lpb_head_fwd_bf16_layout / lpb_head_fwd_f16_layout   features [B, H, W, C]; everything else as above.  saved_xs
+ *                        receives byte for byte what the NCHW entry writes for the same logical tensor.
+ *   lpb_head_bwd_bf16_workspace_bytes_layout   the NCHW shapes except W = 32 (LPB_ERR_UNSUPPORTED), same size.
+ *   lpb_head_bwd_bf16_layout   dfeat [B, H, W, C] bf16; saved_xs / fwd_workspace from either forward layout.
+ * lpb_head_bf16_workspace_bytes and lpb_head_bf16_saved_bytes do not depend on the layout and serve both.  Alignment:
+ * the same buffers, 16 bytes. */
+#define LPB_FEATURES_NCHW 0
+#define LPB_FEATURES_NHWC 1
+int lpb_head_bf16_plan_layout(int C, int H, int W, int c1, int c2, int feature_layout, int* plan);
+int lpb_head_fwd_bf16_layout(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                             const float* w2, const float* b2, int c2, int final_softmax, int feature_layout, float* out,
+                             void* saved_xs, void* workspace, void* stream);
+int lpb_head_fwd_f16_layout(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                            const float* w2, const float* b2, int c2, int final_softmax, int feature_layout, float* out,
+                            void* saved_xs, void* workspace, void* stream);
+int lpb_head_bwd_bf16_workspace_bytes_layout(int B, int C, int H, int W, int c1, int c2, int feature_layout, size_t* bytes);
+int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, const float* win, const int32_t* win_meta,
+                             const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H,
+                             int W, const float* w1, int c1, const float* w2, int c2, int feature_layout, void* dfeat,
+                             float* dw1, float* db1, float* dw2, float* db2, void* workspace, void* stream);
 
 /* ---- coordinate remap -------------------------------------------------------------------------
  * replaces undo_affine_transform_batch + model_to_frame_batch

@@ -60,6 +60,11 @@ SIGNATURES = {
     "lpb_head_fwd_f16": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
     "lpb_head_bwd_bf16_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bwd_bf16": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "lpb_head_bf16_plan_layout": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_I)]),
+    "lpb_head_fwd_bf16_layout": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
+    "lpb_head_fwd_f16_layout": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
+    "lpb_head_bwd_bf16_workspace_bytes_layout": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
+    "lpb_head_bwd_bf16_layout": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_remap_keypoints": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
     "lpb_remap_keypoints_bwd": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
     "lpb_crnn_prepare": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P]),

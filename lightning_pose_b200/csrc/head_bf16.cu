@@ -509,21 +509,29 @@ static_assert(lpb::HEAD_MAX_CH == LPB_HEAD_MAX_CHANNELS, "the cap lpb200.h state
 
 // plan[0] = 1: fast path (saved_xs optional: training only); 0: generic path (saved_xs REQUIRED: it is the operand).
 // Wide heads (more than HEAD_CLS keypoints, head_prep.cuh) always take the generic path.
-extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan) {
+// Channels-last features always take the banded kernels: k1a's TMA loader and transposer warps read NCHW slabs, while
+// rows_shuffle_nhwc_kernel needs no shared memory, so the shuffle stage's feature-map limit does not apply either.
+extern "C" int lpb_head_bf16_plan_layout(int C, int H, int W, int c1, int c2, int feature_layout, int* plan) {
   using namespace lpb;
   LPB_REQUIRE(plan, "head_bf16_plan: null pointer");
+  LPB_REQUIRE(feature_layout == LPB_FEATURES_NCHW || feature_layout == LPB_FEATURES_NHWC, "head_bf16_plan: unknown feature layout %d", feature_layout);
+  const bool nhwc = feature_layout == LPB_FEATURES_NHWC;
   LPB_REQUIRE(C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && (H * W) % 8 == 0 && c1 >= 1 && c2 >= 0, "head_bf16_plan: bad shape");
   if ((c2 > 0 ? c2 : c1) > HEAD_CLS && !head_wide(c1, c2)) {
     set_error("head_bf16_plan: channel counts %d/%d exceed the keypoint groups of this build (%d channels per layer)", c1, c2, HEAD_MAX_CH);
     return LPB_ERR_UNSUPPORTED;
   }
   LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "head_bf16_plan: channel counts %d/%d exceed %d", c1, c2, HEAD_CLS);
-  plan[0] = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, planning_limits().max_smem) ? 1 : 0;
-  if (!plan[0] && (rows_shuffle_smem_bytes(H, W) > HEAD_FEATURE_SMEM_BUDGET || (c2 > 0 ? 4 : 2) * W + 1 > CR_BAND_ROWS)) {
+  plan[0] = !nhwc && !head_wide(c1, c2) && head_fast_path(C, H, W, c2, planning_limits().max_smem) ? 1 : 0;
+  if (!plan[0] && ((!nhwc && rows_shuffle_smem_bytes(H, W) > HEAD_FEATURE_SMEM_BUDGET) || (c2 > 0 ? 4 : 2) * W + 1 > CR_BAND_ROWS)) {
     set_error("head_bf16_plan: feature map %dx%d too large for this build", H, W);
     return LPB_ERR_UNSUPPORTED;
   }
   return LPB_OK;
+}
+
+extern "C" int lpb_head_bf16_plan(int C, int H, int W, int c1, int c2, int* plan) {
+  return lpb_head_bf16_plan_layout(C, H, W, c1, c2, LPB_FEATURES_NCHW, plan);
 }
 
 extern "C" int lpb_head_bf16_saved_bytes(int B, int C, int H, int W, size_t* bytes) {
@@ -545,9 +553,12 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
 // sequence; T is the element type of the features, the packed weights and the mid activations.
 template <typename T>
 static int head_fwd(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1, const float* w2,
-                    const float* b2, int c2, int final_softmax, float* out, void* saved_xs, void* workspace, void* stream) {
+                    const float* b2, int c2, int final_softmax, int feature_layout, float* out, void* saved_xs, void* workspace,
+                    void* stream) {
   using namespace lpb;
   const char* name = head_fwd_name<T>;
+  LPB_REQUIRE(feature_layout == LPB_FEATURES_NCHW || feature_layout == LPB_FEATURES_NHWC, "%s: unknown feature layout %d", name, feature_layout);
+  const bool nhwc = feature_layout == LPB_FEATURES_NHWC;
   LPB_REQUIRE(features && w1 && b1 && out && workspace, "%s: null pointer", name);
   LPB_REQUIRE(c2 == 0 || (w2 && b2), "%s: a two-deconv head needs w2 and b2", name);
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "%s: bad feature shape C=%d H=%d W=%d", name, C, H, W);
@@ -563,7 +574,7 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
   LPB_TRY(device_limits(&dev));
   const int sms = dev.sms;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bool fast = !head_wide(c1, c2) && head_fast_path(C, H, W, c2, dev.max_smem);
+  const bool fast = !nhwc && !head_wide(c1, c2) && head_fast_path(C, H, W, c2, dev.max_smem);
   const K1aGeom k1 = make_k1a_geom(H, W);
   // k1a's feature tensor map, encoded before anything is queued, so a failure leaves the stream untouched.  The plan stays
   // a function of the shape (CPU-only callers size buffers with it); every driver that runs sm_90a code has the encoder,
@@ -599,7 +610,8 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
     LPB_REQUIRE(saved_xs, "%s: this shape takes the banded kernels (lpb_head_bf16_plan = 0): pass the "
                           "lpb_head_bf16_saved_bytes() buffer as saved_xs", name);
     T* xs = static_cast<T*>(saved_xs);
-    int rc = launch_rows_shuffle(static_cast<const T*>(features), B, C, H, W, xs, s);
+    int rc = nhwc ? launch_rows_shuffle_nhwc(static_cast<const T*>(features), B, C, H, W, xs, s)
+                  : launch_rows_shuffle(static_cast<const T*>(features), B, C, H, W, xs, s);
     if (rc != LPB_OK) return rc;
     ConvtRowsParams<T> p{};
     p.X = xs;
@@ -666,14 +678,26 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
   return LPB_OK;
 }
 
+extern "C" int lpb_head_fwd_bf16_layout(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                                        const float* w2, const float* b2, int c2, int final_softmax, int feature_layout, float* out,
+                                        void* saved_xs, void* workspace, void* stream) {
+  return head_fwd<__nv_bfloat16>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, feature_layout, out, saved_xs, workspace, stream);
+}
+
+extern "C" int lpb_head_fwd_f16_layout(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                                       const float* w2, const float* b2, int c2, int final_softmax, int feature_layout, float* out,
+                                       void* saved_xs, void* workspace, void* stream) {
+  return head_fwd<__half>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, feature_layout, out, saved_xs, workspace, stream);
+}
+
 extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
                                  const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
                                  void* workspace, void* stream) {
-  return head_fwd<__nv_bfloat16>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, out, saved_xs, workspace, stream);
+  return lpb_head_fwd_bf16_layout(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, LPB_FEATURES_NCHW, out, saved_xs, workspace, stream);
 }
 
 extern "C" int lpb_head_fwd_f16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
                                 const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
                                 void* workspace, void* stream) {
-  return head_fwd<__half>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, out, saved_xs, workspace, stream);
+  return lpb_head_fwd_f16_layout(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, LPB_FEATURES_NCHW, out, saved_xs, workspace, stream);
 }

@@ -7,7 +7,8 @@
 //   d in[c, m', n'] = sum_{cls, (dm,dn) valid} G[(m'-dm, n'-dn)][(cls, o)] * W[c, o, ky, kx]
 // is again a 4-shift GEMM (negative row shifts of the same smem operand, mma_sm90.cuh), K = 80:
 //   b2d: G2 (48x48 rows)  x W2  -> d mid (48x48 x 17)  written straight into G1 (24x24 rows) for the next stage
-//   b3a: W1 (M = 128 channels) x G1^T -> d Xs[c][row]   un-shuffled in the epilogue into d features (NCHW bf16)
+//   b3a: W1 (M = 128 channels) x G1^T -> d Xs[c][row]   un-shuffled in the epilogue into d features (bf16, NCHW or
+//        channels-last [B][H][W][C])
 #include <cuda_bf16.h>
 
 #include <cstdint>
@@ -414,7 +415,7 @@ struct B3aParams {
   const __nv_bfloat16* G1;   // [B][10][L.rows][8] padded row layout
   RowLayout L;
   const __nv_bfloat16* wpk;  // [ceil(C4/128)][4][10][128][8]
-  __nv_bfloat16* dfeat;      // [B][4*C4][(Hi/2)*(Wi/2)]
+  __nv_bfloat16* dfeat;      // [B][4*C4][(Hi/2)*(Wi/2)], or [B][Hi/2][Wi/2][4*C4] in the NHWC instantiations
   int B, C4, Hi, Wi;         // shuffled-image geometry (Hi = 2H, Wi = 2W)
   int Hh;                    // image rows per band (multiple of 4)
   int ncols;                 // accumulator columns per band = Hh * (Wi + 1) rounded up to 16 (<= 304)
@@ -483,9 +484,19 @@ __device__ __forceinline__ void b3a_each_pair(int ch, const float (&acc)[2][B3aC
     }
 }
 
+// Channels-last d features (NHWC): [B][H][W][C] with C = 4 C4.  The accumulator rows are channels and the columns pixels,
+// so the store transposes through shared memory.  The two items (di = 0, 1) of a feature-row pair, which the two warp
+// groups e = 0, 1 compute side by side, cover every source channel 4c + 2 di + dj of the CTA's 128 shuffled channels at the
+// pair's 2W feature pixels: both groups round their values into one staging tile [2W pixels][128 c][4 planes] bf16, and
+// after a CTA barrier all threads copy it out with 16-byte vectors -- per pixel one contiguous run of up to 1024 bytes
+// (the tile's 512 channels), whole 32-byte sectors.  B3A_NHWC_PX is the tile's pixel stride: 16 bytes past the 1024 so
+// that the 2-byte staging stores of a warp (8 channels x 4 pixel pairs) spread over the banks.
+constexpr int B3A_NHWC_PX = 1024 + 16;
+inline size_t b3a_nhwc_stage_bytes(int W) { return (size_t)2 * W * B3A_NHWC_PX + 128; }
+
 // A frame is processed in bands of Hh image rows (the band's gradient rows plus the halo row above are double-buffered
 // in shared memory).
-template <int WS2, bool ACC = false>
+template <int WS2, bool ACC = false, bool NHWC = false>
 __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_constant__ B3aParams P, const __grid_constant__ CUtensorMap TM,
                                                                    const __grid_constant__ CUtensorMap TM_PAIR) {
   using Cols = B3aCols<WS2>;
@@ -598,7 +609,38 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
         for (int item = e; item < nitems; item += 2) {
           const int ip = item >> 1, ml = 4 * ip + e;  // ml: the item's first accumulator row within the band
           const uint32_t g_item = g0 + (uint32_t)(ml * Pp) * 16;
-          if (!ACC && P.tma_store) {
+          if (NHWC && !(ACC && P.acc_out)) {
+            // (keypoint groups: only the last group's rounding store is channels-last; the fp32 partial sums keep their
+            // plane layout)
+            const int c0 = mt * 128 + 32 * q, i0 = y0 / 2 + 2 * ip;
+            const size_t base = ((size_t)b * 4 * P.C4 + 4 * c0 + 2 * e) * HW + (size_t)i0 * WS2;
+            uint16_t* st = reinterpret_cast<uint16_t*>(Ss) + (32 * q) * 4 + 2 * e;
+#pragma unroll 1
+            for (int ch = 0; ch < Cols::NCHUNK; ++ch) {
+              float acc[2][NT][4];
+              mma_chunk(g_item, ch, acc);
+              b3a_each_pair<WS2>(ch, acc, lane, [&](int r, int dj, int x, float v0, float v1) {
+                if (c0 + r >= P.C4) return;
+                if constexpr (ACC) {
+                  if (P.acc_in) {
+                    const float2 p = *reinterpret_cast<const float2*>(P.acc32 + base + (size_t)((4 * r + dj) * HW + x));
+                    v0 = p.x + v0, v1 = p.y + v1;
+                  }
+                }
+                uint16_t* d = st + (size_t)x * (B3A_NHWC_PX / 2) + 4 * r + dj;
+                d[0] = __bfloat16_as_ushort(__float2bfloat16_rn(v0));
+                d[B3A_NHWC_PX / 2] = __bfloat16_as_ushort(__float2bfloat16_rn(v1));
+              });
+            }
+            named_bar_sync(3, B3A_THREADS);  // both groups' halves of the tile are staged
+            const int nv = min(128, P.C4 - mt * 128) / 2;  // 16-byte vectors per pixel: this tile's channels
+            unsigned char* out = reinterpret_cast<unsigned char*>(P.dfeat + (((size_t)b * (Hi / 2) + i0) * WS2) * 4 * P.C4 + (size_t)mt * 512);
+            for (int idx = tid; idx < 2 * WS2 * nv; idx += B3A_THREADS) {
+              const int px = idx / nv, v = idx - px * nv;
+              *reinterpret_cast<uint4*>(out + (size_t)px * 8 * P.C4 + v * 16) = *reinterpret_cast<const uint4*>(Ss + (size_t)px * B3A_NHWC_PX + v * 16);
+            }
+            named_bar_sync(3, B3A_THREADS);  // the tile may be overwritten
+          } else if (!ACC && P.tma_store) {
             // The 4 warps of this e form a group of 128 channels that owns the slices pl = 2e, 2e + 1.  Items go out in
             // pairs (ip even, ip + 1): a slice row holds both items' 2W pixels of a channel's plane, 8W consecutive bytes
             // of d features, and one tensor store per plane class writes them.  Single items' 4W-byte rows (48 bytes at
@@ -1042,6 +1084,12 @@ static int b3a_band_rows(int Hi1, int Wi1) {
   return hh;
 }
 
+// shared memory of b3a's operands: two band stages of G1 and the CTA's weights
+static size_t b3a_operand_smem_bytes(int Hi1, int Wi1) {
+  const int ncols = (b3a_band_rows(Hi1, Wi1) * (Wi1 + 1) + 15) & ~15, rows_alloc = (Wi1 + 2 + ncols + 7) & ~7;
+  return (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
+}
+
 // d features [B][4*C4][HW] bf16 viewed as [b][c'][pl][px]; box = {box_px pixels, one pl, 128 c', one frame}.
 static bool make_dfeat_tensor_map(CUtensorMap* tm, void* dfeat, int B, int C4, int HW, int box_px) {
   const TensorMapEncodeFn encode = tensor_map_encoder();
@@ -1056,8 +1104,17 @@ static bool make_dfeat_tensor_map(CUtensorMap* tm, void* dfeat, int B, int C4, i
 
 // The shapes the backward serves (lpb200.h): H even, W one of the widths b3a_dgrad_kernel is instantiated for, and the
 // forward's channel limits.  LPB_OK, or LPB_ERR_UNSUPPORTED with the message set.
-static int head_bwd_covers(const char* who, int H, int W, int c1, int c2) {
+static int head_bwd_covers(const char* who, int H, int W, int c1, int c2, int feature_layout) {
   const bool width = W == 4 || W == 8 || W == 12 || W == 16 || W == 24 || W == 32;
+  if (feature_layout != LPB_FEATURES_NCHW && feature_layout != LPB_FEATURES_NHWC) {
+    set_error("%s: unknown feature layout %d", who, feature_layout);
+    return LPB_ERR_INVALID;
+  }
+  if (feature_layout == LPB_FEATURES_NHWC && width && b3a_operand_smem_bytes(2 * H, 2 * W) + b3a_nhwc_stage_bytes(W) > HEAD_BWD_SMEM_BUDGET) {
+    // (W = 32: the operands leave no room for the transposing tile; such features train through an NCHW copy)
+    set_error("%s: channels-last d features of width %d do not fit the data gradient's shared memory", who, W);
+    return LPB_ERR_UNSUPPORTED;
+  }
   if (H % 2 == 0 && width && (head_narrow(c1, c2) || head_wide(c1, c2))) return LPB_OK;
   set_error("%s: head %dx%d with %d/%d channels outside this build's set (H even, W in {4, 8, 12, 16, 24, 32}, the "
             "forward's channel counts)", who, H, W, c1, c2);
@@ -1108,26 +1165,38 @@ static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2)
 }  // namespace lpb
 
 extern "C" int lpb_head_bwd_bf16_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {
-  using namespace lpb;
-  LPB_REQUIRE(bytes, "head_bwd_bf16_workspace_bytes: null pointer");
-  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_bwd_bf16_workspace_bytes: bad shape");
-  if (const int rc = head_bwd_covers("head_bwd_bf16_workspace_bytes", H, W, c1, c2); rc != LPB_OK) return rc;
-  *bytes = head_bwd_layout(B, C, H, W, c1, c2).total;
-  return LPB_OK;
+  return lpb_head_bwd_bf16_workspace_bytes_layout(B, C, H, W, c1, c2, LPB_FEATURES_NCHW, bytes);
 }
 
 extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const float* win, const int32_t* win_meta,
                                  const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H,
                                  int W, const float* w1, int c1, const float* w2, int c2, void* dfeat, float* dw1, float* db1,
                                  float* dw2, float* db2, void* workspace, void* stream) {
+  return lpb_head_bwd_bf16_layout(g_out, probs, win, win_meta, g_overflow, saved_xs, fwd_workspace, B, C, H, W, w1, c1, w2, c2,
+                                  LPB_FEATURES_NCHW, dfeat, dw1, db1, dw2, db2, workspace, stream);
+}
+
+extern "C" int lpb_head_bwd_bf16_workspace_bytes_layout(int B, int C, int H, int W, int c1, int c2, int feature_layout, size_t* bytes) {
   using namespace lpb;
-  const bool two = c2 > 0;
+  LPB_REQUIRE(bytes, "head_bwd_bf16_workspace_bytes: null pointer");
+  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_bwd_bf16_workspace_bytes: bad shape");
+  if (const int rc = head_bwd_covers("head_bwd_bf16_workspace_bytes", H, W, c1, c2, feature_layout); rc != LPB_OK) return rc;
+  *bytes = head_bwd_layout(B, C, H, W, c1, c2).total;
+  return LPB_OK;
+}
+
+extern "C" int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, const float* win, const int32_t* win_meta,
+                                        const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C,
+                                        int H, int W, const float* w1, int c1, const float* w2, int c2, int feature_layout,
+                                        void* dfeat, float* dw1, float* db1, float* dw2, float* db2, void* workspace, void* stream) {
+  using namespace lpb;
+  const bool two = c2 > 0, nhwc = feature_layout == LPB_FEATURES_NHWC;
   LPB_REQUIRE(saved_xs && fwd_workspace && w1 && dw1 && db1 && workspace, "head_bwd_bf16: null pointer");
   LPB_REQUIRE(!two || (w2 && dw2 && db2), "head_bwd_bf16: a two-deconv head needs w2, dw2, db2");
   LPB_REQUIRE(g_out || win, "head_bwd_bf16: neither a dense gradient nor decode windows given");
   LPB_REQUIRE(!win || (win_meta && g_overflow), "head_bwd_bf16: windows need their meta and overflow buffers");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1, "head_bwd_bf16: bad shape C=%d H=%d W=%d c1=%d", C, H, W, c1);
-  if (const int rc = head_bwd_covers("head_bwd_bf16", H, W, c1, c2); rc != LPB_OK) return rc;
+  if (const int rc = head_bwd_covers("head_bwd_bf16", H, W, c1, c2, feature_layout); rc != LPB_OK) return rc;
   {
     // read or written with 16-byte vectors (g_out, probs, g_overflow: float4 plane dots; win_meta: int4; dfeat: uint4 or
     // TMA stores) or bulk copies (saved_xs, fwd_workspace, workspace)
@@ -1289,8 +1358,7 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     p.acc32 = acc32;
     p.kc_frame = g1 * HEAD_KC;
     p.acc_in = p.acc_out = p.kc0 = 0;
-    const int rows_alloc = (Wi1 + 2 + p.ncols + 7) & ~7;
-    size_t smem = (size_t)2 * HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 128 * 16 + 160;
+    size_t smem = b3a_operand_smem_bytes(Hi1, Wi1);
     LPB_REQUIRE(smem <= HEAD_BWD_SMEM_BUDGET, "head_bwd_bf16: layer-1 operands need %zu B shared memory", smem);
     // TMA tensor stores of d features when their staging slices (4 x 128 channels x 2 items x 4W bytes) still fit and the
     // tensor maps (boxes of one item and of an item pair) encode; otherwise direct stores (dfeat's alignment was checked
@@ -1299,7 +1367,10 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     memset(&tmap, 0, sizeof(tmap));
     memset(&tmap_pair, 0, sizeof(tmap_pair));
     p.tma_store = 0;
-    if (!acc32) {  // (the groups' fp32 sums take the direct stores)
+    if (nhwc) {
+      smem += b3a_nhwc_stage_bytes(W);
+      LPB_REQUIRE(smem <= HEAD_BWD_SMEM_BUDGET, "head_bwd_bf16: the channels-last d-feature tile of width %d needs %zu B shared memory", W, smem);
+    } else if (!acc32) {  // (the groups' fp32 sums take the direct stores)
       const size_t stage = (size_t)4 * 128 * 2 * 4 * W + 128;
       if (smem + stage <= HEAD_BWD_SMEM_BUDGET && make_dfeat_tensor_map(&tmap, dfeat, B, C4, H * W, 2 * W) &&
           make_dfeat_tensor_map(&tmap_pair, dfeat, B, C4, H * W, 4 * W)) {
@@ -1329,12 +1400,17 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
     };
     int rc = LPB_ERR_UNSUPPORTED;
     switch (W) {
-      case 4: rc = run(b3a_dgrad_kernel<4>, b3a_dgrad_kernel<4, true>); break;
-      case 8: rc = run(b3a_dgrad_kernel<8>, b3a_dgrad_kernel<8, true>); break;
-      case 12: rc = run(b3a_dgrad_kernel<12>, b3a_dgrad_kernel<12, true>); break;
-      case 16: rc = run(b3a_dgrad_kernel<16>, b3a_dgrad_kernel<16, true>); break;
-      case 24: rc = run(b3a_dgrad_kernel<24>, b3a_dgrad_kernel<24, true>); break;
-      case 32: rc = run(b3a_dgrad_kernel<32>, b3a_dgrad_kernel<32, true>); break;
+#define LPB_B3A_CASE(WS2) \
+  case WS2: \
+    rc = nhwc ? run(b3a_dgrad_kernel<WS2, false, true>, b3a_dgrad_kernel<WS2, true, true>) : run(b3a_dgrad_kernel<WS2>, b3a_dgrad_kernel<WS2, true>); \
+    break;
+      LPB_B3A_CASE(4)
+      LPB_B3A_CASE(8)
+      LPB_B3A_CASE(12)
+      LPB_B3A_CASE(16)
+      LPB_B3A_CASE(24)
+      LPB_B3A_CASE(32)
+#undef LPB_B3A_CASE
       default: set_error("head_bwd_bf16: feature width %d not in this build's epilogue set", W);
     }
     if (rc != LPB_OK) return rc;

@@ -89,10 +89,40 @@ struct FastDiv {
   __device__ __forceinline__ int div(int x) const { return d > 1 ? (int)__umulhi((uint32_t)x, m) : x; }
 };
 
+// Channels-last staging of a PixelShuffle(2) source tile.  `feat` is one frame [H][W][C] (C = 4 Cin): the channels
+// 4 c0 .. 4 (c0 + ncc) - 1 of a feature pixel are one contiguous run and hold the four sub-pixels (2i + di, 2j + dj) of the
+// shuffled channels c0 .. c0 + ncc - 1, so consecutive threads walk that run (coalesced) over the feature pixels that
+// cover shuffled rows m0 .. m0 + nm - 1 and columns n0 .. n0 + nn - 1.  dst(cc, m - m0, n - n0, v) receives every element
+// of that window, zero outside the frame or past Cin.
+template <typename Dst>
+__device__ __forceinline__ void stage_shuffled_nhwc(const float* __restrict__ feat, int Cin, int Hi, int Wi, int c0, int ncc, int m0, int nm,
+                                                    int n0, int nn, Dst dst) {
+  const int i0 = m0 >> 1, ni = ((m0 + nm - 1) >> 1) - i0 + 1, j0 = n0 >> 1, nj = ((n0 + nn - 1) >> 1) - j0 + 1;
+  const int run = 4 * ncc, total = ni * nj * run;
+  const FastDiv rund(run), jd(nj);
+  constexpr int U = 4;
+  for (int e0 = threadIdx.x; e0 < total; e0 += U * blockDim.x) {
+    float v[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int e = e0 + u * blockDim.x, px = rund.div(e), k = e - px * run, ii = jd.div(px), i = i0 + ii, j = j0 + px - ii * nj;
+      const bool ok = e < total && 4 * c0 + k < 4 * Cin && 2 * i < Hi && 2 * j < Wi;
+      v[u] = ok ? __ldg(feat + ((size_t)i * (Wi / 2) + j) * (4 * Cin) + 4 * c0 + k) : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int e = e0 + u * blockDim.x, px = rund.div(e), k = e - px * run, ii = jd.div(px);
+      const int m = 2 * (i0 + ii) + ((k >> 1) & 1) - m0, n = 2 * (j0 + px - ii * nj) + (k & 1) - n0;
+      if (e < total && m >= 0 && m < nm && n >= 0 && n < nn) dst(k >> 2, m, n, v[u]);
+    }
+  }
+}
+
 // ---- forward ------------------------------------------------------------------------------------------------------
 // out[o, 2m+py, 2n+px] = bias[o] + sum_c sum_taps in[c, m+dm, n+dn] * Wt[c, o, ky, kx]
 //   py=0: (dm,ky)=(0,1);  py=1: (0,2),(1,0)     (y = 2*iy - 1 + ky), same along x.
-// SHUFFLE: in[c, m, n] = feat[4c + 2(m&1) + (n&1), m>>1, n>>1]   (PixelShuffle(2))
+// SHUFFLE: in[c, m, n] = feat[4c + 2(m&1) + (n&1), m>>1, n>>1]   (PixelShuffle(2)); LPB_SHUFFLE_NHWC: feat is channels-last
+// in memory (the staged tile, and so every MMA and every result bit, is the same)
 // Each output parity class q = 2 py + px is a GEMM: M = pixels of the block, N = Cout (8 NT per CTA), K = Cin per
 // (shift, tap) pair; the 9 pairs below share four shifted A operands, which are constant offsets into the staged tile
 // (RB + 1 rows x CB + 1 columns, zero halo).
@@ -100,7 +130,7 @@ __device__ constexpr int kFwdShift[9] = {0, 0, 0, 0, 1, 1, 2, 2, 3};  // shift s
 __device__ constexpr int kFwdClass[9] = {0, 1, 2, 3, 1, 3, 2, 3, 3};  // output parity q = 2 py + px
 __device__ constexpr int kFwdTap[9] = {4, 5, 7, 8, 3, 6, 1, 2, 0};    // ky * 3 + kx
 
-template <bool SHUFFLE, int NT>
+template <int SHUFFLE, int NT>
 __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_kernel(const float* __restrict__ in, int Cin, int Hi, int Wi,
                                                                 const float* __restrict__ wt, const float* __restrict__ bias,
                                                                 int Cout, int RB, int CB, float* __restrict__ out) {
@@ -132,6 +162,9 @@ __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_kernel(const float* __r
   const FastDiv rdiv(RB + 1);
   for (int c0 = 0; c0 < Cin; c0 += FW_CC) {
     __syncthreads();
+    if constexpr (SHUFFLE == LPB_SHUFFLE_NHWC)
+      stage_shuffled_nhwc(in + in_img, Cin, Hi, Wi, c0, FW_CC, r0, RB + 1, n0, XR, [&](int cc, int m, int n, float v) { xs[cc * XP + m * XR + n] = v; });
+    else
     stage_rows<4>(
         FW_CC * (RB + 1), XR,
         [&](int cr, int j) {
@@ -250,7 +283,7 @@ static int launch_plane_softmax(float* x, int64_t n_planes, int hw, const char* 
 }
 
 
-template <bool SHUFFLE, int NT>
+template <int SHUFFLE, int NT>
 static int launch_fwd_nt(const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias, int Cout, float* out,
                           cudaStream_t s) {
   const PixBlocks pb = pix_blocks(Hi, Wi);
@@ -262,7 +295,7 @@ static int launch_fwd_nt(const float* in, int B, int Cin, int Hi, int Wi, const 
   return LPB_OK;
 }
 
-template <bool SHUFFLE>
+template <int SHUFFLE>
 static int launch_fwd(const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias, int Cout, float* out,
                       cudaStream_t s) {
   // N tile = Cout rounded up to 8, at most 24 channels (wider heads: more CTAs along y)
@@ -271,10 +304,11 @@ static int launch_fwd(const float* in, int B, int Cin, int Hi, int Wi, const flo
   return launch_fwd_nt<SHUFFLE, 3>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
 }
 
-static int launch_convt(bool shuffle, const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias,
+static int launch_convt(int shuffle, const float* in, int B, int Cin, int Hi, int Wi, const float* wt, const float* bias,
                         int Cout, float* out, cudaStream_t s) {
-  return shuffle ? launch_fwd<true>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s)
-                 : launch_fwd<false>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
+  if (shuffle == LPB_SHUFFLE_NHWC) return launch_fwd<LPB_SHUFFLE_NHWC>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
+  return shuffle ? launch_fwd<LPB_SHUFFLE_NCHW>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s)
+                 : launch_fwd<LPB_SHUFFLE_NONE>(in, B, Cin, Hi, Wi, wt, bias, Cout, out, s);
 }
 
 // ---- backward of one transposed convolution -----------------------------------------------------------------------
@@ -309,7 +343,7 @@ __device__ __forceinline__ void stage_grad_planes(const float* __restrict__ g, i
 
 // Data gradient: M = pixels of the block, N = Cin (8 NT per CTA), K = Cout x 9 in stages of 8 output channels
 // (72 = 9 k8 steps, k = o_local * 9 + tap; the weights [c][o][tap] are K-contiguous).
-template <bool SHUFFLE, int NT>
+template <int SHUFFLE, int NT>
 __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_dgrad_kernel(const float* __restrict__ g, int Cout, int Hi, int Wi,
                                                                       const float* __restrict__ wt, int Cin, int RB, int CB,
                                                                       float* __restrict__ din) {
@@ -390,7 +424,9 @@ __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_dgrad_kernel(const floa
           const int c = c0 + nt * 8 + 2 * t + j;
           if (c >= Cin) continue;
           const float v = acc[mt][nt][2 * h + j];
-          if (SHUFFLE)
+          if (SHUFFLE == LPB_SHUFFLE_NHWC)
+            din[(((size_t)b * (Hi / 2) + (m >> 1)) * (Wi / 2) + (n >> 1)) * (4 * Cin) + 4 * c + 2 * (m & 1) + (n & 1)] = v;
+          else if (SHUFFLE)
             din[(((size_t)b * 4 * Cin + 4 * c + 2 * (m & 1) + (n & 1)) * (Hi / 2) + (m >> 1)) * (Wi / 2) + (n >> 1)] = v;
           else
             din[(((size_t)b * Cin + c) * Hi + m) * Wi + n] = v;
@@ -405,7 +441,7 @@ __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_dgrad_kernel(const floa
 // first channel tile also sum the bias gradient (the four taps (1..2, 1..2)) of their channels.
 constexpr int WG_PS = TC_SLOTS + 4;
 
-template <bool SHUFFLE, int WM, int WN, int NT>
+template <int SHUFFLE, int WM, int WN, int NT>
 __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const float* __restrict__ in, const float* __restrict__ g,
                                                                         int B, int Cin, int Cout, int Hi, int Wi, int RB, int CB,
                                                                         float* __restrict__ dw, float* __restrict__ db) {
@@ -441,6 +477,9 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
     const int b = (int)(u / nblk), blk = (int)(u - (long long)b * nblk);
     const int r0 = (blk / nbc) * RB, q0 = (blk - (blk / nbc) * nbc) * CB;
     __syncthreads();
+    if constexpr (SHUFFLE == LPB_SHUFFLE_NHWC)
+      stage_shuffled_nhwc(in + (size_t)b * Cin * Hi * Wi, Cin, Hi, Wi, c0, CM, r0, RB, q0, CB, [&](int cc, int m, int n, float v) { xs[cc * WG_PS + m * CB + n] = v; });
+    else
     stage_rows<4>(
         CM * RB, CB,
         [&](int cr, int pc) {
@@ -510,7 +549,7 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
   }
 }
 
-template <bool SHUFFLE, int WM, int WN, int NT>
+template <int SHUFFLE, int WM, int WN, int NT>
 static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cout, int Hi, int Wi, float* dw, float* db, cudaStream_t s) {
   constexpr int CM = 32 * WM, CN = 8 * NT * WN;
   const PixBlocks pb = pix_blocks(Hi, Wi);
@@ -530,7 +569,7 @@ static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cou
   return LPB_OK;
 }
 
-template <bool SHUFFLE>
+template <int SHUFFLE>
 static int launch_bwd(const float* in, const float* g, int B, int Cin, int Hi, int Wi, const float* wt, int Cout, float* din, float* dw,
                       float* db, cudaStream_t s) {
   // M tile: 128 input channels, or 32 for narrow inputs (a second layer's Cin is the first layer's keypoint count)
@@ -564,7 +603,7 @@ extern "C" int lpb_convt_fwd_f32(const float* in, int B, int Cin, int Hi, int Wi
   LPB_REQUIRE(in && w && out, "convt_fwd_f32: null pointer");
   LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Hi >= 1 && Wi >= 1 && (!shuffle || (Hi % 2 == 0 && Wi % 2 == 0)), "convt_fwd_f32: bad shape");
   if (B == 0) return LPB_OK;
-  return launch_convt(shuffle != 0, in, B, Cin, Hi, Wi, w, bias, Cout, out, static_cast<cudaStream_t>(stream));
+  return launch_convt(shuffle, in, B, Cin, Hi, Wi, w, bias, Cout, out, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* stream) {
@@ -584,8 +623,9 @@ extern "C" int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, 
   LPB_CUDA(cudaMemsetAsync(grad_w, 0, sizeof(float) * (size_t)Cin * Cout * 9, s));
   if (grad_bias) LPB_CUDA(cudaMemsetAsync(grad_bias, 0, sizeof(float) * Cout, s));
   if (B == 0) return LPB_OK;
-  return shuffle ? launch_bwd<true>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s)
-                 : launch_bwd<false>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s);
+  if (shuffle == LPB_SHUFFLE_NHWC) return launch_bwd<LPB_SHUFFLE_NHWC>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s);
+  return shuffle ? launch_bwd<LPB_SHUFFLE_NCHW>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s)
+                 : launch_bwd<LPB_SHUFFLE_NONE>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s);
 }
 
 extern "C" int lpb_head_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {
@@ -608,16 +648,16 @@ extern "C" int lpb_head_fwd_f32(const float* features, int B, int C, int H, int 
   const int Hs = 2 * H, Ws = 2 * W;  // after PixelShuffle(2)
   int K, Ho, Wo;
   if (c2 == 0) {
-    int rc = launch_convt(true, features, B, C / 4, Hs, Ws, w1, b1, c1, out, s);
+    int rc = launch_convt(LPB_SHUFFLE_NCHW, features, B, C / 4, Hs, Ws, w1, b1, c1, out, s);
     if (rc) return rc;
     K = c1;
     Ho = 2 * Hs;
     Wo = 2 * Ws;
   } else {
     float* mid = static_cast<float*>(workspace);
-    int rc = launch_convt(true, features, B, C / 4, Hs, Ws, w1, b1, c1, mid, s);
+    int rc = launch_convt(LPB_SHUFFLE_NCHW, features, B, C / 4, Hs, Ws, w1, b1, c1, mid, s);
     if (rc) return rc;
-    rc = launch_convt(false, mid, B, c1, 2 * Hs, 2 * Ws, w2, b2, c2, out, s);
+    rc = launch_convt(LPB_SHUFFLE_NONE, mid, B, c1, 2 * Hs, 2 * Ws, w2, b2, c2, out, s);
     if (rc) return rc;
     K = c2;
     Ho = 4 * Hs;

@@ -39,6 +39,8 @@ constexpr const char* head_fwd_name = std::is_same_v<T, __half> ? "head_fwd_f16"
 template <typename T>
 int launch_rows_shuffle(const T* feat, int B, int C, int H, int W, T* xs, cudaStream_t s);
 template <typename T>
+int launch_rows_shuffle_nhwc(const T* feat, int B, int C, int H, int W, T* xs, cudaStream_t s);
+template <typename T>
 int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s);
 
 // The shuffle stage holds a CTA's 32 channels of one H x W feature map.  Its budget is the public feature-map limit of

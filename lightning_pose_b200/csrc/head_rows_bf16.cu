@@ -6,6 +6,7 @@
 // head_bf16.cu keeps a whole frame's operands in shared memory and therefore stops at 12x12 feature maps.  Here a
 // transposed convolution is a *banded* 4-shift GEMM on the padded row layout (row_layout.cuh):
 //   rows_shuffle_kernel   features (NCHW bf16) -> pixel-shuffled rows X[b][kchunk][row][8]      (one pass, HBM-bound)
+//   rows_shuffle_nhwc_kernel   the same rows from channels-last features [B][H][W][C], without the transpose
 //   convt_rows_kernel     X rows --TMA bulk, one copy per K-chunk--> smem stages (K streamed 32 channels at a time)
 //                         --mma.sync, 4 shifted views--> register accumulators (<= 2 M-tiles = one band of image rows)
 //                         --epilogue--> bf16 rows of the next layer | fp32 planes | two-pass plane softmax
@@ -73,6 +74,63 @@ int launch_rows_shuffle(const T* feat, int B, int C, int H, int W, T* xs, cudaSt
 }
 template int launch_rows_shuffle<__nv_bfloat16>(const __nv_bfloat16*, int, int, int, int, __nv_bfloat16*, cudaStream_t);
 template int launch_rows_shuffle<__half>(const __half*, int, int, int, int, __half*, cudaStream_t);
+
+// ---- PixelShuffle(2) + channels-last [B][H][W][C] -> padded row layout ---------------------------------------------
+// In this layout the 32 source channels of a K-chunk at one feature pixel are 64 contiguous bytes, and the fold needs no
+// transpose: row entry q = 2 di + dj of the pixel's 2 x 2 sub-pixels holds source channels q, 4 + q, .., 28 + q of the
+// chunk, picked out of the four 16-byte loads with byte permutes.  One CTA per (frame, feature row); a thread takes one
+// (K-chunk, pixel) with the pixels along the lanes, so a warp's stores are the 32-byte (dj = 0, 1) entry pairs of
+// consecutive pixels -- one contiguous run of rows per di -- and every load is two whole 32-byte sectors.  The CTA also
+// writes the pads its rows touch (the zero column; the lead / trail rows from the first / last feature row), so the
+// buffer needs no clearing and is byte-identical to rows_shuffle_kernel's for the same logical tensor.
+// Bytes: C * H * W * 2 read, lpb_head_bf16_saved_bytes written.
+__global__ void __launch_bounds__(256) rows_shuffle_nhwc_kernel(const uint16_t* __restrict__ feat, int C, int H, int W,
+                                                                uint16_t* __restrict__ xs, RowLayout L) {
+  const int nkc = C / 32;
+  const int b = blockIdx.x / H, i = blockIdx.x - b * H;
+  const uint16_t* src = feat + ((size_t)b * H + i) * W * C;
+  uint16_t* dst = xs + (size_t)b * nkc * L.rows * 8;
+  for (int idx = threadIdx.x; idx < nkc * W; idx += 256) {
+    const int kc = idx / W, j = idx - kc * W;
+    const uint4* p = reinterpret_cast<const uint4*>(src + (size_t)j * C + kc * 32);
+    uint32_t w[16];
+#pragma unroll
+    for (int v = 0; v < 4; ++v) {
+      const uint4 u = __ldg(p + v);
+      w[4 * v] = u.x, w[4 * v + 1] = u.y, w[4 * v + 2] = u.z, w[4 * v + 3] = u.w;
+    }
+    // element k of entry q is channel 4 k + q of the chunk: 32-bit word 2 k + q / 2, half q % 2
+    uint4 o[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t sel = (q & 1) ? 0x7632u : 0x5410u;
+      const int h = q >> 1;
+      o[q] = make_uint4(__byte_perm(w[h], w[2 + h], sel), __byte_perm(w[4 + h], w[6 + h], sel), __byte_perm(w[8 + h], w[10 + h], sel),
+                        __byte_perm(w[12 + h], w[14 + h], sel));
+    }
+    uint16_t* d0 = dst + ((size_t)kc * L.rows + L.lead + (size_t)(2 * i) * L.Pp + 2 * j) * 8;
+    *reinterpret_cast<uint4*>(d0) = o[0];
+    *reinterpret_cast<uint4*>(d0 + 8) = o[1];
+    *reinterpret_cast<uint4*>(d0 + (size_t)L.Pp * 8) = o[2];
+    *reinterpret_cast<uint4*>(d0 + (size_t)L.Pp * 8 + 8) = o[3];
+  }
+  const int body1 = L.lead + L.Hi * L.Pp;
+  const int r_lo = i == 0 ? 0 : L.lead + 2 * i * L.Pp, r_hi = i == H - 1 ? L.rows : L.lead + (2 * i + 2) * L.Pp, nr = r_hi - r_lo;
+  for (int idx = threadIdx.x; idx < nkc * nr; idx += 256) {
+    const int kc = idx / nr, r = r_lo + idx - kc * nr;
+    if (r < L.lead || r >= body1 || (r - L.lead) % L.Pp == L.Wi)
+      *reinterpret_cast<uint4*>(dst + ((size_t)kc * L.rows + r) * 8) = make_uint4(0, 0, 0, 0);
+  }
+}
+
+template <typename T>
+int launch_rows_shuffle_nhwc(const T* feat, int B, int C, int H, int W, T* xs, cudaStream_t s) {
+  const RowLayout L = make_row_layout(2 * H, 2 * W);
+  rows_shuffle_nhwc_kernel<<<(unsigned)(B * H), 256, 0, s>>>(reinterpret_cast<const uint16_t*>(feat), C, H, W, reinterpret_cast<uint16_t*>(xs), L);
+  return LPB_OK;
+}
+template int launch_rows_shuffle_nhwc<__nv_bfloat16>(const __nv_bfloat16*, int, int, int, int, __nv_bfloat16*, cudaStream_t);
+template int launch_rows_shuffle_nhwc<__half>(const __half*, int, int, int, int, __half*, cudaStream_t);
 
 // ---- banded transposed-convolution GEMM ---------------------------------------------------------------------------
 constexpr int CR_THREADS = 320;  // warp 0 loader, warp 1 idle, warps 2-9 MMA + epilogue

@@ -87,8 +87,13 @@ class _HeadFunction(torch.autograd.Function):
         # fp16 features take the tensor cores for inference only (autocast(float16) in the reference); with a backward
         # to follow they take the fp32 kernels, which train
         sixteen = features.dtype == torch.bfloat16 or (features.dtype == torch.float16 and not train)
-        if sixteen and features.is_cuda and ops.head_bf16_supported(tuple(features.shape), [w.shape[1] for w in weights], train=train):
-            res = ops._head_forward_16(features.contiguous(), weights, biases, final_softmax, train=train)
+        # channels-last features (a ViT's tokens, a convnet run in torch.channels_last) are read where they lie, and
+        # their gradient is written in the same format
+        operand = ops.head_16_operand(features, [w.shape[1] for w in weights], train) if sixteen and features.is_cuda else None
+        ctx.layout = ops.FEATURES_NCHW
+        if operand is not None:
+            f16, ctx.layout = operand
+            res = ops._head_forward_16(f16, weights, biases, final_softmax, train=train, layout=ctx.layout)
             out, saved = res if train else (res, None)
         elif train:
             out, acts = ops.head_forward_f32(features, weights, biases, final_softmax, keep_activations=True)
@@ -126,7 +131,7 @@ class _HeadFunction(torch.autograd.Function):
                 windows = ops.decode_backward_windows(out, stats, g_xy.contiguous().float(), int(ctx.decode[0]), float(ctx.decode[1]))
             dfeat, dw1, db1, dw2, db2 = ops.head_backward_bf16(
                 g, ctx.saved, tuple(features.shape), weights[0], weights[1] if n == 2 else None, need_dfeat=need_dfeat,
-                probs=out if ctx.final_softmax else None, windows=windows,
+                probs=out if ctx.final_softmax else None, windows=windows, layout=ctx.layout,
             )
             dws, dbs = ([dw1, dw2], [db1, db2]) if n == 2 else ([dw1], [db1])
             return (dfeat, None, None, None, *[d.to(w.dtype) for d, w in zip(dws, weights)], *[d.to(b.dtype) for d, b in zip(dbs, biases)])

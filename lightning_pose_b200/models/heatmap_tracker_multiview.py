@@ -34,6 +34,7 @@ from lightning_pose_b200.data.bboxes import model_to_frame_batch
 from lightning_pose_b200.data.cameras import project_camera_pairs_to_3d
 from lightning_pose_b200.losses.factory import LossFactory
 from lightning_pose_b200.losses.losses import RegressionRMSELoss
+from lightning_pose_b200.models.backbones import tokens_to_feature_map
 from lightning_pose_b200.models.heads.heatmap import HeatmapHead
 
 __all__: list[str] = []
@@ -75,8 +76,11 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         self.loss_factory = loss_factory
         self.rmse_loss = RegressionRMSELoss()
 
-    def forward_vit(self, images: torch.Tensor) -> torch.Tensor:
-        """(view * batch, 3, H, W) -> (view * batch, D, h, w), views attending to each other (reference :143-232)."""
+    def forward_vit(self, images: torch.Tensor, channels_last: bool = False) -> torch.Tensor:
+        """(view * batch, 3, H, W) -> (view * batch, D, h, w), views attending to each other (reference :143-232).
+
+        Contiguous NCHW, as the reference returns it; with ``channels_last`` the same values as a view of the encoder's
+        tokens (``tokens_to_feature_map``), which is what the head is fed: it reads them in place."""
         tokens = self.patch_embed(images)  # (view * batch, N, D)
         vb, n, d = tokens.shape
         batch = vb // self.num_views
@@ -84,17 +88,17 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         tokens = tokens + self.view_embeddings[view_idx].to(tokens.dtype).unsqueeze(1)
         seq = self.encoder(tokens.reshape(batch, self.num_views * n, d))  # all views of an example in one sequence
         side = math.isqrt(n)
-        out = seq.reshape(batch, self.num_views, side, side, d).permute(0, 1, 4, 2, 3)
-        return out.reshape(vb, d, side, side).contiguous()
+        features = tokens_to_feature_map(seq.reshape(vb, n, d), (side, side))
+        return features if channels_last else features.contiguous()
 
     def forward(self, images: torch.Tensor) -> torch.Tensor:
         batch, views, c, h, w = images.shape
-        heatmaps = self.head(self.forward_vit(images.reshape(-1, c, h, w)))
+        heatmaps = self.head(self.forward_vit(images.reshape(-1, c, h, w), channels_last=True))
         return heatmaps.reshape(batch, -1, heatmaps.shape[-2], heatmaps.shape[-1])
 
     def forward_with_keypoints(self, images: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         batch, views, c, h, w = images.shape
-        hm, kp, cf = self.head.forward_with_keypoints(self.forward_vit(images.reshape(-1, c, h, w)))
+        hm, kp, cf = self.head.forward_with_keypoints(self.forward_vit(images.reshape(-1, c, h, w), channels_last=True))
         return hm.reshape(batch, -1, hm.shape[-2], hm.shape[-1]), kp.reshape(batch, -1), cf.reshape(batch, -1)
 
     def get_loss_inputs_labeled(self, batch_dict: dict) -> dict:

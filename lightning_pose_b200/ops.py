@@ -203,26 +203,55 @@ def evaluate_heatmaps_at_location(heatmaps, locs, radius: int = 2):
 # =====================================================================================
 # heatmap head
 # =====================================================================================
-def head_bf16_supported(shape, channels, train: bool) -> bool:
-    """Whether the tensor-core kernels cover this head: feature shape (B, C, H, W), deconv output channels (c1[, c2]).
+FEATURES_NCHW, FEATURES_NHWC = 0, 1  # LPB_FEATURES_* (lpb200.h)
+_SHUFFLE_NHWC = 2                    # LPB_SHUFFLE_NHWC
 
-    The library owns the shape rules: the forward's in ``lpb_head_bf16_plan``, the backward's (``train``) in
-    ``lpb_head_bwd_bf16_workspace_bytes``.  Neither needs a GPU."""
+
+def feature_layout(features: torch.Tensor) -> int:
+    """The memory format the head's kernels can read ``features`` (B, C, H, W) in without a copy: ``FEATURES_NHWC`` for
+    a dense channels-last tensor (``torch.channels_last``, or a token tensor seen through
+    ``models.backbones.tokens_to_feature_map``), ``FEATURES_NCHW`` otherwise.  A tensor that is both (C = 1, or
+    H = W = 1) counts as NCHW, and so does one with any other strides: its caller makes it contiguous."""
+    if features.dim() == 4 and not features.is_contiguous() and features.is_contiguous(memory_format=torch.channels_last):
+        return FEATURES_NHWC
+    return FEATURES_NCHW
+
+
+def head_bf16_supported(shape, channels, train: bool, layout: int = FEATURES_NCHW) -> bool:
+    """Whether the tensor-core kernels cover this head: feature shape (B, C, H, W), deconv output channels (c1[, c2]),
+    memory format of the features (``feature_layout``).
+
+    The library owns the shape rules: the forward's in ``lpb_head_bf16_plan_layout``, the backward's (``train``) in
+    ``lpb_head_bwd_bf16_workspace_bytes_layout``.  Neither needs a GPU."""
     b, c, h, w = shape
     if len(channels) not in (1, 2):
         return False
     c1, c2 = channels[0], (channels[1] if len(channels) == 2 else 0)
     plan = C.c_int(0)
-    if lib.lpb_head_bf16_plan(c, h, w, c1, c2, C.byref(plan)) != 0:
+    if lib.lpb_head_bf16_plan_layout(c, h, w, c1, c2, layout, C.byref(plan)) != 0:
         return False
     nbytes = C.c_size_t(0)
-    return not train or lib.lpb_head_bwd_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)) == 0
+    return not train or lib.lpb_head_bwd_bf16_workspace_bytes_layout(b, c, h, w, c1, c2, layout, C.byref(nbytes)) == 0
 
 
-def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=False):
+def head_16_operand(features, channels, train: bool):
+    """``(features as the 16-bit head reads them, layout)`` or None when the tensor-core kernels do not cover the head.
+
+    Channels-last features are read in place where the kernels take them.  Where only the NCHW kernels cover the shape
+    (training at W = 32), and for every tensor that is neither format, this is the NCHW copy."""
+    layout = feature_layout(features)
+    if layout == FEATURES_NHWC and head_bf16_supported(tuple(features.shape), channels, train, FEATURES_NHWC):
+        return features, FEATURES_NHWC
+    if head_bf16_supported(tuple(features.shape), channels, train):
+        return features.contiguous(), FEATURES_NCHW
+    return None
+
+
+def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=False, layout=FEATURES_NCHW):
     """tensor-core path (one- or two-deconv heads) on 16-bit features: bf16 (``lpb_head_fwd_bf16``) or fp16
     (``lpb_head_fwd_f16``), the weights rounded to the features' dtype on the device; the caller checks
-    ``head_bf16_supported`` first.  Both share the plan and the buffer sizes.
+    ``head_bf16_supported`` first.  Both share the plan and the buffer sizes.  ``layout``: the memory format ``f`` is
+    dense in (``FEATURES_NCHW``: contiguous; ``FEATURES_NHWC``: channels-last, read in place).
 
     ``train=True`` (bf16 only: there is no fp16 backward) returns ``(out, saved)`` where ``saved`` carries what
     ``head_backward_bf16`` needs (the row-layout copy of the shuffled features and the forward workspace with the
@@ -239,7 +268,7 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
     b2 = _cuda_f32(biases[1], "bias") if n == 2 else None
     c1, c2 = w1.shape[1], (w2.shape[1] if n == 2 else 0)
     plan = C.c_int(0)
-    check(lib.lpb_head_bf16_plan(c, h, w, c1, c2, C.byref(plan)))
+    check(lib.lpb_head_bf16_plan_layout(c, h, w, c1, c2, layout, C.byref(plan)))
     nbytes = C.c_size_t(0)
     check(lib.lpb_head_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)))
     ws = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
@@ -250,7 +279,7 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
         check(lib.lpb_head_bf16_saved_bytes(b, c, h, w, C.byref(nbytes)))
         xs = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
     with torch.cuda.device(f.device):
-        check(entry(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), _ptr(out), _ptr(xs), _ptr(ws), _stream()))
+        check(entry(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), layout, _ptr(out), _ptr(xs), _ptr(ws), _stream()))
     if want_hints:  # kept for bench.py's call, which unpacks a decode-hints slot (always None)
         return (out, (xs, ws), None) if train else (out, None)
     if train:
@@ -258,7 +287,7 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
     return out
 
 
-_HEAD_FWD_16 = {torch.bfloat16: lib.lpb_head_fwd_bf16, torch.float16: lib.lpb_head_fwd_f16}
+_HEAD_FWD_16 = {torch.bfloat16: lib.lpb_head_fwd_bf16_layout, torch.float16: lib.lpb_head_fwd_f16_layout}
 _head_forward_bf16 = _head_forward_16  # the name bench.py and the bf16 tests call
 
 
@@ -276,8 +305,9 @@ def decode_backward_windows(heatmaps, stats, grad_xy, ds, temperature):
     return win, meta, overflow
 
 
-def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None):
-    """Gradients of the bf16 head: returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None).
+def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None, layout=FEATURES_NCHW):
+    """Gradients of the bf16 head: returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None).  ``dfeat`` is dense in
+    ``layout``, the memory format the forward read the features in.
 
     ``g_out``: dense gradient w.r.t. the head output or None; ``probs``: the head output when it ends in the
     spatial softmax (its backward is fused in), None for a logits head; ``windows``: result of
@@ -293,24 +323,34 @@ def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=
     c1, c2 = w1.shape[1], (w2.shape[1] if w2 is not None else 0)
     dev = w1.device
     nbytes = C.c_size_t(0)
-    check(lib.lpb_head_bwd_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)))
+    check(lib.lpb_head_bwd_bf16_workspace_bytes_layout(b, c, h, w, c1, c2, layout, C.byref(nbytes)))
     ws = torch.empty((nbytes.value,), device=dev, dtype=torch.uint8)
-    dfeat = torch.empty((b, c, h, w), device=dev, dtype=torch.bfloat16) if need_dfeat else None
+    fmt = torch.channels_last if layout == FEATURES_NHWC else torch.contiguous_format
+    dfeat = torch.empty((b, c, h, w), device=dev, dtype=torch.bfloat16, memory_format=fmt) if need_dfeat else None
     dw1 = torch.empty_like(w1)
     db1 = torch.empty((c1,), device=dev, dtype=torch.float32)
     dw2 = torch.empty_like(w2) if w2 is not None else None
     db2 = torch.empty((c2,), device=dev, dtype=torch.float32) if w2 is not None else None
     win, meta, ov = windows if windows is not None else (None, None, None)
     with torch.cuda.device(dev):
-        check(lib.lpb_head_bwd_bf16(_ptr(g), _ptr(probs), _ptr(win), _ptr(meta), _ptr(ov), _ptr(xs), _ptr(fws), b, c, h, w, _ptr(w1), c1, _ptr(w2), c2,
-                                    _ptr(dfeat), _ptr(dw1), _ptr(db1), _ptr(dw2), _ptr(db2), _ptr(ws), _stream()))
+        check(lib.lpb_head_bwd_bf16_layout(_ptr(g), _ptr(probs), _ptr(win), _ptr(meta), _ptr(ov), _ptr(xs), _ptr(fws), b, c, h, w, _ptr(w1), c1, _ptr(w2), c2,
+                                    layout, _ptr(dfeat), _ptr(dw1), _ptr(db1), _ptr(dw2), _ptr(db2), _ptr(ws), _stream()))
     return dfeat, dw1, db1, dw2, db2
 
 
 # ---- fp32 precision path: one transposed convolution at a time (any number of layers), native backward ----------
+def _f32_conv_input(x, shuffle: bool):
+    """``(x as fp32 the kernels can read, the entries' shuffle argument)``: the PixelShuffle-folding layer reads
+    channels-last features in place, everything else is made contiguous."""
+    if shuffle and isinstance(x, torch.Tensor) and x.is_cuda and feature_layout(x) == FEATURES_NHWC:
+        return x.float(), _SHUFFLE_NHWC  # (.float() keeps the strides)
+    return _cuda_f32(x, "input"), int(shuffle)
+
+
 def convt_forward_f32(x, weight, bias, shuffle: bool):
-    """[PixelShuffle(2) +] ConvTranspose2d(k3, s2, p1, op1) in fp32 (3xTF32 on the tensor cores); any Cin, Cout, size."""
-    x = _cuda_f32(x, "input")
+    """[PixelShuffle(2) +] ConvTranspose2d(k3, s2, p1, op1) in fp32 (3xTF32 on the tensor cores); any Cin, Cout, size.
+    With ``shuffle``, channels-last ``x`` is read in place (same result bits as from its NCHW copy)."""
+    x, mode = _f32_conv_input(x, shuffle)
     wt = _cuda_f32(weight, "weight")
     bs = _cuda_f32(bias, "bias") if bias is not None else None
     b, c, h, w = x.shape
@@ -319,13 +359,13 @@ def convt_forward_f32(x, weight, bias, shuffle: bool):
         raise ValueError(f"weight expects {wt.shape[0]} input channels, got {cin}")
     out = torch.empty((b, wt.shape[1], 2 * hi, 2 * wi), device=x.device, dtype=torch.float32)
     with torch.cuda.device(x.device):
-        check(lib.lpb_convt_fwd_f32(_ptr(x), b, cin, hi, wi, int(shuffle), _ptr(wt), _ptr(bs), wt.shape[1], _ptr(out), _stream()))
+        check(lib.lpb_convt_fwd_f32(_ptr(x), b, cin, hi, wi, mode, _ptr(wt), _ptr(bs), wt.shape[1], _ptr(out), _stream()))
     return out
 
 
 def convt_backward_f32(x, grad_out, weight, shuffle: bool, need_dx: bool = True, need_db: bool = True):
-    """Autograd of ``convt_forward_f32``: (dx | None, dw, db | None)."""
-    x = _cuda_f32(x, "input")
+    """Autograd of ``convt_forward_f32``: (dx | None, dw, db | None); ``dx`` has the memory format of ``x``."""
+    x, mode = _f32_conv_input(x, shuffle)
     g = _cuda_f32(grad_out, "grad_out")
     wt = _cuda_f32(weight, "weight")
     b, c, h, w = x.shape
@@ -334,7 +374,7 @@ def convt_backward_f32(x, grad_out, weight, shuffle: bool, need_dx: bool = True,
     dw = torch.empty_like(wt)
     db = torch.empty((wt.shape[1],), device=x.device, dtype=torch.float32) if need_db else None
     with torch.cuda.device(x.device):
-        check(lib.lpb_convt_bwd_f32(_ptr(x), _ptr(g), b, cin, hi, wi, int(shuffle), _ptr(wt), wt.shape[1], _ptr(dx), _ptr(dw), _ptr(db), _stream()))
+        check(lib.lpb_convt_bwd_f32(_ptr(x), _ptr(g), b, cin, hi, wi, mode, _ptr(wt), wt.shape[1], _ptr(dx), _ptr(dw), _ptr(db), _stream()))
     return dx, dw, db
 
 
@@ -349,7 +389,7 @@ def plane_softmax_(x: torch.Tensor) -> torch.Tensor:
 def head_forward_f32(features, weights, biases, final_softmax=True, keep_activations=False):
     """fp32 head: PixelShuffle(2) + any number of deconvs + spatial softmax.  Returns ``out`` or, with
     ``keep_activations``, ``(out, inputs_of_each_layer)`` for ``convt_backward_f32``."""
-    x = _cuda_f32(features, "features")
+    x, _ = _f32_conv_input(features, True)
     acts = []
     for i, (wt, bs) in enumerate(zip(weights, biases)):
         acts.append(x)
@@ -371,9 +411,11 @@ def head_forward(features, weights, biases, final_softmax=True):
         raise RuntimeError("lpb200: `features` must be a CUDA tensor (this package has no CPU fallback)")
     if len(weights) < 1:
         raise ValueError("head needs at least one deconv layer")
-    if features.dtype in _HEAD_FWD_16 and all(b is not None for b in biases) and head_bf16_supported(
-            tuple(features.shape), [w.shape[1] for w in weights], train=False):
-        return _head_forward_16(features.contiguous(), weights, biases, final_softmax)
+    operand = None
+    if features.dtype in _HEAD_FWD_16 and all(b is not None for b in biases):
+        operand = head_16_operand(features, [w.shape[1] for w in weights], train=False)
+    if operand is not None:
+        return _head_forward_16(operand[0], weights, biases, final_softmax, layout=operand[1])
     return head_forward_f32(features, weights, biases, final_softmax)
 
 
