@@ -256,7 +256,9 @@ int lpb_remap_keypoints_bwd(const float* grad_out, int64_t n, int K, const float
  * -> out_logits [M, K, H, W] = (x_f + x_b) / 2 before the spatial softmax.  lpb_crnn_combine_bwd: its autograd
  * (dWF, dWB [N,K,H,W], dLf/dLb [K,4,4], dhf/dhb [K,4]; all overwritten).  M * K < 65536 per call.
  * lpb_context_gather: the materialised window tensor out[i][s] = seq[clamp(i + s - ctx/2)] for API parity
- * (n items of item_bytes, a multiple of 16). */
+ * (n items of item_bytes, a multiple of 16).  lpb_context_gather_bwd: its adjoint, d_seq [n, elems] = for each frame
+ * the sum of the grad [n, ctx, elems] slots that read it (the repeated edge frames included), in a fixed order without
+ * atomics; elements in the LPB_OUT_* format `format` (see the ingest entries below), summed in fp32. */
 int lpb_crnn_prepare(const float* conv_w, const float* conv_b, const float* convt_w, const float* convt_b, int K, int F,
                      float* L, float* h, void* stream);
 int lpb_crnn_prepare_bwd(const float* conv_w, const float* conv_b, const float* convt_w, const float* dL, const float* dh,
@@ -267,6 +269,7 @@ int lpb_crnn_combine_bwd(const float* WF, const float* WB, const int32_t* idx, c
                          int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb, float* dWF,
                          float* dWB, float* dLf, float* dhf, float* dLb, float* dhb, void* stream);
 int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes, int ctx, void* out, void* stream);
+int lpb_context_gather_bwd(const void* grad, int64_t n, int64_t elems, int ctx, int format, void* d_seq, void* stream);
 
 /* ---- video-ingest boundary (SURVEY 8f-4) ----------------------------------------------------------------
  * replaces the tail of the DALI pipeline  lightning_pose/data/video/dali.py:157-197

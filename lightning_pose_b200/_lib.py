@@ -72,6 +72,7 @@ SIGNATURES = {
     "lpb_crnn_combine_fwd": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "lpb_crnn_combine_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_context_gather": (C.c_int, [_P, _L, _L, _I, _P, _P]),
+    "lpb_context_gather_bwd": (C.c_int, [_P, _L, _L, _I, _I, _P, _P]),
     "lpb_frames_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
     "lpb_frames_normalize_views": (C.c_int, [C.POINTER(_P), _I, _I, C.POINTER(_I), C.POINTER(_I), _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
     "lpb_frames_augment_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),

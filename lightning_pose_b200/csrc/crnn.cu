@@ -216,6 +216,34 @@ __global__ void context_gather_kernel(const uint4* __restrict__ seq, int64_t n, 
   }
 }
 
+template <int FMT>
+__device__ __forceinline__ float load_fmt(const void* p, int64_t i) {
+  if constexpr (FMT == LPB_OUT_BF16) return __bfloat162float(static_cast<const __nv_bfloat16*>(p)[i]);
+  else if constexpr (FMT == LPB_OUT_F16) return __half2float(static_cast<const __half*>(p)[i]);
+  else return static_cast<const float*>(p)[i];
+}
+
+// adjoint of context_gather_kernel: d_seq[f] = sum of grad[i][s] over the slots with clamp(i + s - ctx/2) == f.  Only the
+// windows i in [f - ctx/2, f + ctx/2] can read frame f (the edge frames' repeats included); they are summed in ascending
+// (i, s) order in fp32, one thread per element of d_seq, so the result does not depend on the launch.
+template <int FMT>
+__global__ void context_gather_bwd_kernel(const void* __restrict__ grad, int64_t n, int64_t elems, int ctx, void* __restrict__ d_seq) {
+  const int half = ctx / 2;
+  const int64_t total = n * elems;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t f = i / elems, e = i - f * elems;
+    const int64_t lo = f - half < 0 ? 0 : f - half, hi = f + half > n - 1 ? n - 1 : f + half;
+    float acc = 0.f;
+    for (int64_t w = lo; w <= hi; ++w)
+      for (int s = 0; s < ctx; ++s) {
+        int64_t src = w + s - half;
+        src = src < 0 ? 0 : (src > n - 1 ? n - 1 : src);
+        if (src == f) acc += load_fmt<FMT>(grad, (w * ctx + s) * elems + e);
+      }
+    store_fmt<FMT>(d_seq, (size_t)i, acc);
+  }
+}
+
 }  // namespace lpb
 
 extern "C" int lpb_crnn_prepare(const float* conv_w, const float* conv_b, const float* convt_w, const float* convt_b, int K, int F,
@@ -292,6 +320,21 @@ extern "C" int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes
   if (blocks > 132 * 32) blocks = 132 * 32;  // 32 CTAs per SM of an H100 SXM
   context_gather_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint4*>(seq), n, item_bytes / 16, ctx,
                                                                                         static_cast<uint4*>(out));
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_context_gather_bwd(const void* grad, int64_t n, int64_t elems, int ctx, int format, void* d_seq, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(grad && d_seq && n >= 1 && elems >= 1 && ctx >= 1 && (ctx & 1) && valid_out_format(format),
+              "context_gather_bwd: bad arguments (odd context length, element format LPB_OUT_F32 / BF16 / F16)");
+  DeviceLimits dev;
+  LPB_TRY(device_limits(&dev));
+  int64_t blocks = (n * elems + 255) / 256;
+  if (blocks > (int64_t)dev.sms * 16) blocks = (int64_t)dev.sms * 16;
+  with_out_format(format, [&](auto fmt) {
+    context_gather_bwd_kernel<decltype(fmt)::value><<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(grad, n, elems, ctx, d_seq);
+  });
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

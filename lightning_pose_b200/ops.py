@@ -546,19 +546,39 @@ def plane_softmax(logits: torch.Tensor) -> torch.Tensor:
     return _PlaneSoftmax.apply(_cuda_f32(logits, "logits"))
 
 
+class _ContextGather(torch.autograd.Function):
+    """The window tensor and its adjoint: a frame's gradient is the sum of the window slots that read it."""
+
+    @staticmethod
+    def forward(ctx, x, context_length):
+        n = x.shape[0]
+        out = torch.empty((n, context_length, *x.shape[1:]), device=x.device, dtype=x.dtype)
+        with torch.cuda.device(x.device):
+            check(lib.lpb_context_gather(_ptr(x), n, x[0].numel() * x.element_size(), context_length, _ptr(out), _stream()))
+        ctx.shape, ctx.context_length = x.shape, context_length
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.contiguous()
+        d = torch.empty(ctx.shape, device=g.device, dtype=g.dtype)
+        with torch.cuda.device(g.device):
+            check(lib.lpb_context_gather_bwd(_ptr(g), ctx.shape[0], d[0].numel(), ctx.context_length, _OUT_FORMATS[g.dtype], _ptr(d), _stream()))
+        return d, None
+
+
 def context_gather(seq: torch.Tensor, context_length: int = 5) -> torch.Tensor:
-    """get_context_from_sequence (base.py:159-196): (n, ...) -> (n, ctx, ...) windows with replicated edges."""
+    """get_context_from_sequence (base.py:159-196): (n, ...) -> (n, ctx, ...) windows with replicated edges;
+    differentiable in ``seq`` for fp32, bf16 and fp16 sequences."""
     if not isinstance(seq, torch.Tensor) or not seq.is_cuda:
         raise RuntimeError("lpb200: `img_seq` must be a CUDA tensor (this package has no CPU fallback)")
     x = seq.contiguous()
-    n = x.shape[0]
     item = x[0].numel() * x.element_size()
     if item % 16:
         raise ValueError(f"items of {item} bytes: the gather moves 16-byte vectors")
-    out = torch.empty((n, context_length, *x.shape[1:]), device=x.device, dtype=x.dtype)
-    with torch.cuda.device(x.device):
-        check(lib.lpb_context_gather(_ptr(x), n, item, int(context_length), _ptr(out), _stream()))
-    return out
+    if x.requires_grad and torch.is_grad_enabled() and x.dtype not in _OUT_FORMATS:
+        raise ValueError(f"the window gradient is summed for float32, bfloat16 and float16 sequences; got {x.dtype}")
+    return _ContextGather.apply(x, int(context_length))
 
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)  # lightning_pose/data/__init__.py (_IMAGENET_MEAN / _IMAGENET_STD)

@@ -281,6 +281,27 @@ def crnn_ref(features: torch.Tensor, params: dict, upsampling_factor: int, softm
     return crnn_combine_ref(wf, wb, idx, p["H_f"], p["H_b"])
 
 
+def context_ref(feats: torch.Tensor, params: dict, upsampling_factor: int, idx: torch.Tensor, operands=torch.bfloat16,
+                mids: list | None = None):
+    """The context head as its kernels compute it, in float64: the W_f and W_b maps of every frame (N, C, h, w) by two
+    ``head_ref`` logit heads, W_pre + W_f and W_pre + W_b (``upsampling_factor`` 2) or W_f and W_b alone, with the
+    tensor-core kernels' operand roundings (``operands``; None: none); then ``crnn_combine_ref`` over the (M, 5) window
+    table ``idx`` and the plane softmax.  Returns ``(heatmaps (M, K, H, W), wf, wb)``, the maps (N, K, H, W) with
+    ``retain_grad`` where they need a gradient, so that their per-channel gradient norms can bound the W_f / W_b bias
+    gradients.  ``mids``: as ``head_ref``'s (the W_pre outputs of the W_f run, then of the W_b run).  Differentiable in
+    every input."""
+    maps = []
+    for key in ("W_f", "W_b"):
+        layers = ([params["W_pre"]] if upsampling_factor == 2 else []) + [params[key]]
+        m = head_ref(feats, [w for w, _ in layers], [b for _, b in layers], softmax=False, operands=operands, mids=mids)
+        if m.requires_grad:
+            m.retain_grad()
+        maps.append(m)
+    logits = crnn_combine_ref(maps[0], maps[1], idx, params["H_f"], params["H_b"])
+    n, k, hh, ww = logits.shape
+    return torch.softmax(logits.reshape(n, k, -1), -1).reshape(n, k, hh, ww), maps[0], maps[1]
+
+
 def crnn_combine_ref(wf, wb, idx, h_f_params, h_b_params) -> torch.Tensor:
     """(x_f + x_b) / 2 of the bidirectional recurrence over the five context slots of every window, float64.
 

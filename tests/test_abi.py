@@ -247,6 +247,9 @@ def test_round2_entry_points_validate_arguments_without_gpu():
     ):
         assert rc == -1, (rc, L.lpb_last_error())
     assert L.lpb_context_gather(C.c_void_p(16), 4, 24, 5, C.c_void_p(16), None) == -1  # items must be 16-byte multiples
+    assert L.lpb_context_gather_bwd(None, 4, 64, 5, 0, None, None) == -1
+    assert L.lpb_context_gather_bwd(C.c_void_p(16), 4, 64, 4, 0, C.c_void_p(16), None) == -1  # odd context length
+    assert L.lpb_context_gather_bwd(C.c_void_p(16), 4, 64, 5, 3, C.c_void_p(16), None) == -1  # no such element format
 
 
 def test_tuning_switch_takes_only_softmax_split():

@@ -814,7 +814,7 @@ def test_mhcrnn_backward_vs_oracle_autograd(lpb, dev, golden, tag, arch, uf):
 
 
 def test_mhcrnn_bf16_real_shape_and_tracker(lpb, dev):
-    """config 3: ViT-S features (384, 16, 16) of a 256x256 clip, bf16, through the tensor-core deconv maps + recurrence kernel."""
+    """config 3: ViT-S features (384, 16, 16) of a 256x256 clip, bf16: the video form's shapes, one semi-supervised step and predict_step."""
     from lightning_pose_b200.models.heatmap_tracker_mhcrnn import SemiSupervisedHeatmapTrackerMHCRNN
     from lightning_pose_b200.losses.factory import LossFactory
 
@@ -837,14 +837,7 @@ def test_mhcrnn_bf16_real_shape_and_tracker(lpb, dev):
     with torch.no_grad():
         feats = tr.backbone(frames)
         sf, mf = tr.head.forward_sequence(feats)
-    assert sf.shape == mf.shape == (t - 4, k, 64, 64)
-    p = _mhcrnn_oracle_params(tr.head)
-    r = lambda x: x.bfloat16().float()
-    p_r = {key: tuple(r(x) if x.dim() == 4 and key.startswith("W") else x for x in tup) for key, tup in p.items()}
-    win = O.context_windows(feats.float().cpu(), 5)[2:-2]
-    mf_ref = O.mhcrnn_multiframe(win.permute(1, 0, 2, 3, 4), p_r, 1)
-    rel = ((mf.cpu() - mf_ref).abs() / (mf_ref.abs() + 1e-7)).flatten()
-    assert float(rel.max()) < 3e-2 and float((rel > 1e-2).float().mean()) < 1e-4
+    assert sf.shape == mf.shape == (t - 4, k, 64, 64)  # the heatmaps against float64: test_context_train_gpu.py
     # one semi-supervised step runs end to end and reaches the backbone
     bbox = torch.tensor([[0.0, 0.0, 256.0, 256.0]], device=dev).repeat(t, 1)
     loss = tr.evaluate_unlabeled({"frames": frames, "transforms": torch.tensor([-1.0], device=dev), "bbox": bbox, "is_multiview": False}, "train", 1.0)

@@ -298,3 +298,33 @@ def test_crnn_refs_golden(golden, tag, uf):
     close(mf, O.mhcrnn_multiframe(feats, p, uf), atol=1e-7, rtol=1e-5)
     logits = S.crnn_ref(feats, p, uf, softmax=False)
     close(O.spatial_softmax2d(logits, 1.0), mf, atol=1e-12)
+
+
+@pytest.mark.parametrize("tag,uf", [("vit", 1), ("resnet", 2)])
+def test_context_ref_golden(golden, tag, uf):
+    """context_ref without operand roundings is crnn_ref (the reference module's recurrence) on the call form's window
+    table, value and float64 gradient in every input; its maps are the W_f / W_b logit heads of every frame; the
+    bf16 roundings move it by a bf16-sized step only."""
+    g = golden("mhcrnn")
+    p = {key: tuple(t.double().requires_grad_(True) for t in tup) for key, tup in _golden_crnn_params(g, tag, uf).items()}
+    feats = T(g[f"{tag}_in_features"]).permute(4, 0, 1, 2, 3).double()  # (frames, batch, C, h, w)
+    frames, batch = feats.shape[:2]
+    idx = torch.arange(frames)[None, :] * batch + torch.arange(batch)[:, None]  # window b, slot s -> frame s * batch + b
+    f1 = feats.clone().requires_grad_(True)
+    hm, wf, wb = S.context_ref(f1.flatten(0, 1), p, uf, idx, operands=None)
+    close(hm, g[f"{tag}_out_mf"], atol=1e-7, rtol=1e-5)
+    gout = torch.randn(hm.shape, generator=torch.Generator().manual_seed(4), dtype=torch.float64)
+    leaves = [f1] + [t for tup in p.values() for t in tup]
+    got = torch.autograd.grad((hm * gout).sum(), leaves)
+    f2 = feats.clone().requires_grad_(True)
+    ref = S.crnn_ref(f2, p, uf)
+    close(hm, ref, atol=1e-12)
+    want = torch.autograd.grad((ref * gout).sum(), [f2] + leaves[1:])
+    for a, b in zip(got, want):
+        close(a, b, atol=1e-12 * float(b.abs().max()) + 1e-15)
+    layers = lambda key: ([p["W_pre"]] if uf == 2 else []) + [p[key]]
+    for m, key in ((wf, "W_f"), (wb, "W_b")):
+        close(m, S.head_ref(feats.flatten(0, 1), [w for w, _ in layers(key)], [b for _, b in layers(key)], softmax=False, operands=None), atol=0)
+    hm16, _, _ = S.context_ref(feats.flatten(0, 1), p, uf, idx)
+    close(hm16, hm, atol=3e-2 * float(hm.detach().abs().max()))
+    assert float((hm16 - hm).detach().abs().max()) > 0
