@@ -229,6 +229,29 @@ int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, const float
                              int W, const float* w1, int c1, const float* w2, int c2, int feature_layout, void* dfeat,
                              float* dw1, float* db1, float* dw2, float* db2, void* workspace, void* stream);
 
+/* Keypoint-target source of the head backward: the gradient of lpb_heatmap_mse_from_keypoints_fwd w.r.t. its preds
+ * (which must be the head output, probs), rebuilt inside the backward's front end from the keypoints instead of read
+ * from a dense g_out.  The per-pixel values are those lpb_heatmap_mse_from_keypoints_bwd writes, bit for bit; the
+ * [n_planes, 8H, 8W] fp32 gradient never exists.  Fields are the arguments of the two loss entries (device pointers):
+ * keypoints [B*C][2], visibility [B*C] or NULL, fwd_out the forward's out (out[1] = kept planes), grad_out the scalar
+ * upstream gradient. */
+typedef struct lpb_mse_targets {
+  const float* keypoints;
+  const int32_t* visibility;
+  float img_height, img_width, sigma;
+  const float* fwd_out;
+  const float* grad_out;
+} lpb_mse_targets;
+/* lpb_head_bwd_bf16_layout with a keypoint-target source: mse NULL makes it exactly that entry.  With mse, g_out must be
+ * NULL (the targets stand for it), probs non-NULL, and the workspace is lpb_head_bwd_bf16_workspace_bytes_targets(...,
+ * with_targets = 1) bytes (a per-plane row of target factors more); with_targets = 0 gives the _layout size. */
+int lpb_head_bwd_bf16_workspace_bytes_targets(int B, int C, int H, int W, int c1, int c2, int feature_layout, int with_targets,
+                                              size_t* bytes);
+int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win,
+                              const int32_t* win_meta, const float* g_overflow, const void* saved_xs, const void* fwd_workspace,
+                              int B, int C, int H, int W, const float* w1, int c1, const float* w2, int c2, int feature_layout,
+                              void* dfeat, float* dw1, float* db1, float* dw2, float* db2, void* workspace, void* stream);
+
 /* ---- coordinate remap -------------------------------------------------------------------------
  * replaces undo_affine_transform_batch + model_to_frame_batch
  *   lightning_pose/data/utils.py:142-234, lightning_pose/data/bboxes.py:74-105,222-288

@@ -29,6 +29,20 @@ class PcaDesc(C.Structure):
     ]
 
 
+class MseTargets(C.Structure):
+    """mirror of ``lpb_mse_targets`` (include/lpb200.h)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p),
+        ("visibility", C.c_void_p),
+        ("img_height", C.c_float),
+        ("img_width", C.c_float),
+        ("sigma", C.c_float),
+        ("fwd_out", C.c_void_p),
+        ("grad_out", C.c_void_p),
+    ]
+
+
 _P, _I, _L, _F, _Z = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
 
 # symbol -> (restype, argtypes); this table is also what tests/test_abi.py checks against the header
@@ -65,6 +79,9 @@ SIGNATURES = {
     "lpb_head_fwd_f16_layout": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
     "lpb_head_bwd_bf16_workspace_bytes_layout": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bwd_bf16_layout": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "lpb_head_bwd_bf16_workspace_bytes_targets": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
+    "lpb_head_bwd_bf16_targets": (C.c_int, [_P, C.POINTER(MseTargets), _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P, _P,
+                                            _P, _P, _P, _P]),
     "lpb_remap_keypoints": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
     "lpb_remap_keypoints_bwd": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
     "lpb_crnn_prepare": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P]),

@@ -22,6 +22,7 @@
 #include "tensor_map.cuh"
 #include "row_layout.cuh"
 #include "mma_sm90.cuh"
+#include "targets.cuh"
 
 namespace lpb {
 
@@ -32,14 +33,30 @@ namespace lpb {
 // and, when the head ends in the spatial softmax, is pulled back through it on the fly:
 //   g_logit = p * (g - dot),  dot = sum_plane(g * p) = ddot (dense part, plane_dot_kernel) + window dot (meta).
 // Neither the dense decode gradient, nor its sum with g_out, nor g_logit ever exist in memory.
+// The dense part may instead come from keypoint targets (lpb_mse_targets): the fused target + MSE loss's gradient
+// (p - t) * scale, rebuilt per pixel from each plane's target mode and axis factors.  plane_dot_targets_kernel computes
+// those once per plane into fac, and the G2 writers (TGT forms) read them with the probabilities, so that gradient is
+// never in memory either.
 struct G2Src {
   const float* g_out;   // or null
   const float* probs;   // head output when it ends in softmax, else null
   const float* win;     // [planes][32*32] or null
   const int* meta;      // [planes][4] {row0, col0, flag, bits(dot)}
   const float* gov;     // dense fallback planes (flag 2)
-  const float* ddot;    // [planes] dense part of the softmax dot (valid when probs && (g_out || win))
+  const float* ddot;    // [planes] dense part of the softmax dot (valid when probs && (g_out || win || kp))
+  // keypoint targets (kp non-null): the MSE's keypoints / visibility, target geometry, its forward's out (out[1] =
+  // kept planes) and upstream gradient, and fac [planes][fac_stride] = {mode, 3 unused, ex[Wo], er[Ho]}
+  const float* kp;
+  const int32_t* vis;
+  float sx, sy, two_s2;
+  const float* mse_out;
+  const float* mse_gout;
+  float* fac;
+  int fac_stride;
 };
+
+// floats per plane of the target factors: {mode, 3 unused} + ex[ow] + er[oh], a multiple of 4 (16-byte rows)
+inline int mse_fac_stride(int oh, int ow) { return (4 + ow + oh + 3) & ~3; }
 
 // ddot[plane] = sum(p * (g_out + [flag == 2] gov)); one CTA per plane
 __global__ void __launch_bounds__(256) plane_dot_kernel(G2Src S, int hw, float* __restrict__ ddot) {
@@ -67,6 +84,63 @@ __global__ void __launch_bounds__(256) plane_dot_kernel(G2Src S, int hw, float* 
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[i];
+    ddot[plane] = t;
+  }
+}
+
+// Keypoint-target form: the dense gradient is rebuilt per element as heatmap_mse_from_kp_bwd_kernel (losses.cu) computes
+// it -- the same 256-thread axis factors, so norm has the same bits, and the same mse_target_grad -- and ddot sums it in
+// plane_dot_kernel's loop and expression order, so the result is what that kernel gives on the materialised gradient.
+// Also writes the plane's mode and factor rows (ex[c], er[r] = ey[r] * norm; uniform planes 1/n and 1) to S.fac.
+// ow % 4 == 0 (the head's output widths): a float4 of pixels lies in one row.
+__global__ void __launch_bounds__(256) plane_dot_targets_kernel(G2Src S, int oh, int ow, float* __restrict__ ddot) {
+  extern __shared__ float sm[];  // ex[ow], ey[oh] (then er), red[16]
+  float* ex = sm;
+  float* ey = sm + ow;
+  float* red = ey + oh;
+  __shared__ float dred[8];
+  const size_t plane = blockIdx.x;
+  const int hw = oh * ow;
+  const TargetPlane tp = classify_target(S.kp[2 * plane], S.kp[2 * plane + 1], S.vis ? S.vis[plane] : -1, S.sx, S.sy, oh, ow);
+  float* fac = S.fac + plane * S.fac_stride;
+  if (threadIdx.x == 0) reinterpret_cast<int*>(fac)[0] = tp.mode;
+  if (tp.mode != TARGET_ZERO) {
+    const float norm = tp.mode == TARGET_GAUSS ? target_axis_factors(tp, oh, ow, S.two_s2, ex, ey, red, 256) : 1.f;
+    const float u = mse_target_uniform(hw);
+    for (int c = threadIdx.x; c < ow; c += 256) {
+      if (tp.mode == TARGET_UNIFORM) ex[c] = u;
+      fac[4 + c] = ex[c];
+    }
+    for (int r = threadIdx.x; r < oh; r += 256) {
+      const float er = tp.mode == TARGET_UNIFORM ? 1.f : ey[r] * norm;
+      ey[r] = er;
+      fac[4 + ow + r] = er;
+    }
+    __syncthreads();
+  }
+  const float scale = mse_target_scale(S.mse_gout[0], S.mse_out[1]);
+  const bool ov = S.meta && S.meta[4 * plane + 2] == 2;
+  const float4* p4 = reinterpret_cast<const float4*>(S.probs + plane * hw);
+  const float4* o4 = ov ? reinterpret_cast<const float4*>(S.gov + plane * hw) : nullptr;
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < hw / 4; i += 256) {
+    const float4 p = __ldg(p4 + i);
+    const int r = (4 * i) / ow, c = 4 * i - r * ow;
+    const float er = ey[r];
+    float4 g = make_float4(mse_target_grad(tp.mode, p.x, ex[c], er, scale), mse_target_grad(tp.mode, p.y, ex[c + 1], er, scale),
+                           mse_target_grad(tp.mode, p.z, ex[c + 2], er, scale), mse_target_grad(tp.mode, p.w, ex[c + 3], er, scale));
+    if (o4) {
+      const float4 o = __ldg(o4 + i);
+      g.x += o.x, g.y += o.y, g.z += o.z, g.w += o.w;
+    }
+    acc += p.x * g.x + p.y * g.y + p.z * g.z + p.w * g.w;
+  }
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) dred[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int i = 0; i < 8; ++i) t += dred[i];
     ddot[plane] = t;
   }
 }
@@ -109,17 +183,22 @@ constexpr int G2B_THREADS = 128;
 // HAS_OV (pass ahead of the patch kernel): planes whose decode gradient is dense (flag 2, the decode's overflow buffer) are
 // added here, in the streaming pass -- in the fresh-init regime that is every plane.  blockIdx.y is the keypoint group
 // (head_prep.cuh): planes [20 g, 20 g + 20) of the C, written to the group's 10 K-chunks of the frame's gridDim.y * 10.
-template <bool HAS_G, bool HAS_P, bool HAS_OV>
+// TGT (with HAS_G, HAS_P): the dense gradient is the keypoint targets' (G2Src), from the probabilities and the factor rows.
+template <bool HAS_G, bool HAS_P, bool HAS_OV, bool TGT>
 __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B, int C, int Hi, int Wi, int ctas_per_frame,
                                                                __nv_bfloat16* __restrict__ G, RowLayout L) {
+  static_assert(!TGT || (HAS_G && HAS_P), "the keypoint-target source is a dense gradient of a softmax head");
   const int b = blockIdx.x / ctas_per_frame, t0 = (blockIdx.x - b * ctas_per_frame) * G2B_THREADS, t = t0 + threadIdx.x;
   const int Wo = 2 * Wi, Ho = 2 * Hi;
   const int g = blockIdx.y, o0 = HEAD_CLS * g, cg = min(HEAD_CLS, C - o0);
   __shared__ float sdot[HEAD_CLS];
+  __shared__ int smode[HEAD_CLS];
+  __shared__ float sscale;
   __shared__ unsigned sov;
   if (threadIdx.x < HEAD_CLS) {
     float d = 0.f;
     int4 mt = make_int4(0, 0, 0, 0);
+    int mode = TARGET_ZERO;
     if (threadIdx.x < cg) {
       const size_t plane = (size_t)b * C + o0 + threadIdx.x;
       if (S.meta) mt = reinterpret_cast<const int4*>(S.meta)[plane];
@@ -127,8 +206,13 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
         if (mt.z == 1) d = __int_as_float(mt.w);
         if (S.ddot) d += S.ddot[plane];
       }
+      if (TGT) mode = reinterpret_cast<const int*>(S.fac + plane * S.fac_stride)[0];
     }
     sdot[threadIdx.x] = d;
+    if (TGT) {
+      smode[threadIdx.x] = mode;
+      if (threadIdx.x == 0) sscale = mse_target_scale(S.mse_gout[0], S.mse_out[1]);
+    }
     if (HAS_OV) {
       const unsigned bov = __ballot_sync((1u << HEAD_CLS) - 1, mt.z == 2);
       if (threadIdx.x == 0) sov = bov;
@@ -149,10 +233,31 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
       gv[o] = make_float2(0.f, 0.f);
       if (o < cg) {
         if (HAS_P) pv[o] = __ldg(reinterpret_cast<const float2*>(S.probs + off0 + o * pstride));
-        if (HAS_G) gv[o] = __ldg(reinterpret_cast<const float2*>(S.g_out + off0 + o * pstride));
+        if (HAS_G && !TGT) gv[o] = __ldg(reinterpret_cast<const float2*>(S.g_out + off0 + o * pstride));
       }
     }
-    if (HAS_OV && sov) {  // uniform per frame
+    if (TGT) {
+      // plane by plane to the softmax term, so that each plane's operands die at once (the same operations in the same
+      // order as the three passes below)
+      const float scale = sscale;
+      const unsigned ovm = HAS_OV ? sov : 0u;
+      const float* f0 = S.fac + ((size_t)b * C + o0) * S.fac_stride + 4;
+#pragma unroll
+      for (int o = 0; o < HEAD_CLS; ++o) {
+        if (o < cg) {
+          const float* f = f0 + (size_t)o * S.fac_stride;
+          const float2 e = __ldg(reinterpret_cast<const float2*>(f + x));
+          const float er = __ldg(f + Wo + y);
+          float2 gt = make_float2(mse_target_grad(smode[o], pv[o].x, e.x, er, scale), mse_target_grad(smode[o], pv[o].y, e.y, er, scale));
+          if (HAS_OV && ((ovm >> o) & 1u)) {
+            const float2 u = __ldg(reinterpret_cast<const float2*>(S.gov + off0 + o * pstride));
+            gt.x += u.x, gt.y += u.y;
+          }
+          const float d = sdot[o];
+          gv[o] = make_float2(pv[o].x * (gt.x - d), pv[o].y * (gt.y - d));
+        }
+      }
+    } else if (HAS_OV && sov) {  // uniform per frame
       const unsigned ovm = sov;
 #pragma unroll
       for (int o = 0; o < HEAD_CLS; ++o) {
@@ -162,7 +267,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
         }
       }
     }
-    if (HAS_P) {
+    if (HAS_P && !TGT) {
 #pragma unroll
       for (int o = 0; o < HEAD_CLS; ++o) {
         const float d = sdot[o];
@@ -193,7 +298,7 @@ __global__ void __launch_bounds__(G2B_THREADS, 4) g2_build_kernel(G2Src S, int B
 // bf16 entries.  The streaming pass then runs at the DRAM roofline with no look-ups in it, and this pass touches 4 KB of
 // probabilities per plane (a ninth of it).
 // Window rows go eight at a time: 8 independent window loads, then 8 independent probability loads per lane.
-template <bool HAS_G, bool HAS_P>
+template <bool HAS_G, bool HAS_P, bool TGT>
 __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_planes, int C, int Hi, int Wi,
                                                       __nv_bfloat16* __restrict__ G, RowLayout L) {
   const int lane = threadIdx.x & 31;
@@ -206,6 +311,10 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
       const int b = (int)(plane / C), oc = (int)(plane - (long long)b * C), g = oc / HEAD_CLS, o = oc - g * HEAD_CLS;
       float dot = 0.f;
       if (HAS_P) dot = __int_as_float(mt.w) + (S.ddot ? S.ddot[plane] : 0.f);
+      // keypoint targets: this plane's mode and factor rows, the loss's scale
+      const float* fac = TGT ? S.fac + (size_t)plane * S.fac_stride : nullptr;
+      const int tmode = TGT ? reinterpret_cast<const int*>(fac)[0] : TARGET_ZERO;
+      const float tscale = TGT ? mse_target_scale(S.mse_gout[0], S.mse_out[1]) : 0.f;
       const size_t poff = (size_t)plane * Ho * Wo;
       const float* wp = S.win + (size_t)plane * 1024 + lane;
       const int x = mt.y + lane;
@@ -223,7 +332,8 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
           const int y = mt.x + r0 + k;
           const bool ok = xin && gw[k] != 0.f && (unsigned)y < (unsigned)Ho;
           pv[k] = (HAS_P && ok) ? __ldg(S.probs + poff + (size_t)y * Wo + x) : 0.f;
-          go[k] = (HAS_G && ok) ? __ldg(S.g_out + poff + (size_t)y * Wo + x) : 0.f;
+          if (TGT) go[k] = ok ? mse_target_grad(tmode, pv[k], __ldg(fac + 4 + x), __ldg(fac + 4 + Wo + y), tscale) : 0.f;
+          else go[k] = (HAS_G && ok) ? __ldg(S.g_out + poff + (size_t)y * Wo + x) : 0.f;
         }
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
@@ -239,17 +349,17 @@ __global__ void __launch_bounds__(128) g2_patch_kernel(G2Src S, long long n_plan
   }
 }
 
-template <bool HAS_G, bool HAS_P>
+template <bool HAS_G, bool HAS_P, bool TGT = false>
 static void launch_g2_build(const G2Src& S, int B, int C, int Hi, int Wi, __nv_bfloat16* G, RowLayout L, cudaStream_t s) {
   const int cpf = (Hi * Wi + G2B_THREADS - 1) / G2B_THREADS;
   const dim3 grid((unsigned)(B * cpf), (unsigned)head_groups(C));
   if (!S.win) {
-    g2_build_kernel<HAS_G, HAS_P, false><<<grid, G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
+    g2_build_kernel<HAS_G, HAS_P, false, TGT><<<grid, G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
     return;
   }
-  g2_build_kernel<HAS_G, HAS_P, true><<<grid, G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
+  g2_build_kernel<HAS_G, HAS_P, true, TGT><<<grid, G2B_THREADS, 0, s>>>(S, B, C, Hi, Wi, cpf, G, L);
   const long long np = (long long)B * C;
-  g2_patch_kernel<HAS_G, HAS_P><<<(unsigned)((np + 3) / 4), 128, 0, s>>>(S, np, C, Hi, Wi, G, L);
+  g2_patch_kernel<HAS_G, HAS_P, TGT><<<(unsigned)((np + 3) / 4), 128, 0, s>>>(S, np, C, Hi, Wi, G, L);
 }
 
 // (the data-gradient operand packs  out[tile][shift][kchunk][r][8]: element (r, k) = W[tile*rows_per_tile + r][o][ky][kx]
@@ -1130,10 +1240,11 @@ static int head_bwd_covers(const char* who, int H, int W, int c1, int c2, int fe
 // group of c2 / c1, and two fp32 buffers follow the narrow layout: dmid [B][c1][4H * 4W] (the mid activations' gradient,
 // summed over the c2 groups, two-deconv heads) and acc32 [B][C][H * W] (the d features of the c1 groups before the last,
 // when c1 has more than one group).  Narrow heads have one group everywhere and neither buffer.
+// With keypoint targets, the per-plane target factors (mse_fac_stride floats per output plane) come last.
 struct HeadBwdLayout {
-  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, dmid, acc32, total;
+  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, dmid, acc32, fac, total;
 };
-static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2) {
+static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2, bool targets) {
   const int C4 = C / 4;
   const bool two = c2 > 0, wide = head_wide(c1, c2);
   const int g1 = head_groups(c1), g2 = two ? head_groups(c2) : 1, nst2 = two ? head_mid_stages(c1) : 1;
@@ -1159,6 +1270,11 @@ static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2)
     l.acc32 = l.dmid + (two ? (size_t)B * c1 * 16 * H * W * sizeof(float) : 0);
     l.total = l.acc32 + (g1 > 1 ? (size_t)B * C * H * W * sizeof(float) : 0);
   }
+  if (targets) {
+    const int up = two ? 8 : 4;  // output grid: (up H) x (up W)
+    l.fac = (l.total + 255) & ~(size_t)255;
+    l.total = l.fac + (size_t)B * (two ? c2 : c1) * mse_fac_stride(up * H, up * W) * sizeof(float);
+  }
   return l;
 }
 
@@ -1177,11 +1293,16 @@ extern "C" int lpb_head_bwd_bf16(const float* g_out, const float* probs, const f
 }
 
 extern "C" int lpb_head_bwd_bf16_workspace_bytes_layout(int B, int C, int H, int W, int c1, int c2, int feature_layout, size_t* bytes) {
+  return lpb_head_bwd_bf16_workspace_bytes_targets(B, C, H, W, c1, c2, feature_layout, 0, bytes);
+}
+
+extern "C" int lpb_head_bwd_bf16_workspace_bytes_targets(int B, int C, int H, int W, int c1, int c2, int feature_layout, int with_targets,
+                                                         size_t* bytes) {
   using namespace lpb;
   LPB_REQUIRE(bytes, "head_bwd_bf16_workspace_bytes: null pointer");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_bwd_bf16_workspace_bytes: bad shape");
   if (const int rc = head_bwd_covers("head_bwd_bf16_workspace_bytes", H, W, c1, c2, feature_layout); rc != LPB_OK) return rc;
-  *bytes = head_bwd_layout(B, C, H, W, c1, c2).total;
+  *bytes = head_bwd_layout(B, C, H, W, c1, c2, with_targets != 0).total;
   return LPB_OK;
 }
 
@@ -1189,11 +1310,26 @@ extern "C" int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, 
                                         const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C,
                                         int H, int W, const float* w1, int c1, const float* w2, int c2, int feature_layout,
                                         void* dfeat, float* dw1, float* db1, float* dw2, float* db2, void* workspace, void* stream) {
+  return lpb_head_bwd_bf16_targets(g_out, nullptr, probs, win, win_meta, g_overflow, saved_xs, fwd_workspace, B, C, H, W, w1, c1, w2, c2,
+                                   feature_layout, dfeat, dw1, db1, dw2, db2, workspace, stream);
+}
+
+extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win,
+                                         const int32_t* win_meta, const float* g_overflow, const void* saved_xs,
+                                         const void* fwd_workspace, int B, int C, int H, int W, const float* w1, int c1,
+                                         const float* w2, int c2, int feature_layout, void* dfeat, float* dw1, float* db1,
+                                         float* dw2, float* db2, void* workspace, void* stream) {
   using namespace lpb;
   const bool two = c2 > 0, nhwc = feature_layout == LPB_FEATURES_NHWC;
   LPB_REQUIRE(saved_xs && fwd_workspace && w1 && dw1 && db1 && workspace, "head_bwd_bf16: null pointer");
   LPB_REQUIRE(!two || (w2 && dw2 && db2), "head_bwd_bf16: a two-deconv head needs w2, dw2, db2");
-  LPB_REQUIRE(g_out || win, "head_bwd_bf16: neither a dense gradient nor decode windows given");
+  LPB_REQUIRE(g_out || mse || win, "head_bwd_bf16: neither a dense gradient nor decode windows given");
+  if (mse) {
+    LPB_REQUIRE(!g_out, "head_bwd_bf16: keypoint targets stand for the dense gradient; g_out must be null");
+    LPB_REQUIRE(probs, "head_bwd_bf16: keypoint targets need the softmax head's output (probs)");
+    LPB_REQUIRE(mse->keypoints && mse->fwd_out && mse->grad_out, "head_bwd_bf16: keypoint targets: null pointer");
+    LPB_REQUIRE(mse->img_height > 0.f && mse->img_width > 0.f && mse->sigma > 0.f, "head_bwd_bf16: keypoint targets: bad image size or sigma");
+  }
   LPB_REQUIRE(!win || (win_meta && g_overflow), "head_bwd_bf16: windows need their meta and overflow buffers");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1, "head_bwd_bf16: bad shape C=%d H=%d W=%d c1=%d", C, H, W, c1);
   if (const int rc = head_bwd_covers("head_bwd_bf16", H, W, c1, c2, feature_layout); rc != LPB_OK) return rc;
@@ -1227,7 +1363,7 @@ extern "C" int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, 
   const RowLayout L2 = make_row_layout(Hi2, Wi2), L1 = make_row_layout(Hi1, Wi1);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const int ntile1 = (C4 + 127) / 128;
-  const HeadBwdLayout wl = head_bwd_layout(B, C, H, W, c1, c2);
+  const HeadBwdLayout wl = head_bwd_layout(B, C, H, W, c1, c2, mse != nullptr);
   __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.wp1);
   __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.wp2);
   __nv_bfloat16* G2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.G2);
@@ -1267,25 +1403,40 @@ extern "C" int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, 
     const int Hio = two ? Hi2 : Hi1, Wio = two ? Wi2 : Wi1;
     __nv_bfloat16* Gout = two ? G2 : G1;
     const RowLayout Lo = two ? L2 : L1;
-    G2Src src;
+    G2Src src{};
     src.g_out = g_out;
     src.probs = probs;
     src.win = win;
     src.meta = win ? win_meta : nullptr;
     src.gov = g_overflow;
     src.ddot = nullptr;
-    if (probs) {
-      LPB_REQUIRE(((4 * Hio * Wio) % 4) == 0, "head_bwd_bf16: plane size");
-      if (!g_out && win)
-        plane_dot_sparse_kernel<<<(unsigned)(((long long)B * kout + 7) / 8), 256, 0, s>>>(src, (long long)B * kout, 4 * Hio * Wio, ddot);
-      else
-        plane_dot_kernel<<<(unsigned)(B * kout), 256, 0, s>>>(src, 4 * Hio * Wio, ddot);
+    if (mse) {
+      const int oh = 2 * Hio, ow = 2 * Wio;  // ow is a multiple of 4 (W even)
+      const TargetGeom tg = target_geom(mse->img_height, mse->img_width, oh, ow, mse->sigma);
+      src.kp = mse->keypoints;
+      src.vis = mse->visibility;
+      src.sx = tg.sx, src.sy = tg.sy, src.two_s2 = tg.two_s2;
+      src.mse_out = mse->fwd_out;
+      src.mse_gout = mse->grad_out;
+      src.fac = reinterpret_cast<float*>(ws + wl.fac);
+      src.fac_stride = mse_fac_stride(oh, ow);
+      plane_dot_targets_kernel<<<(unsigned)(B * kout), 256, (size_t)(oh + ow + 16) * sizeof(float), s>>>(src, oh, ow, ddot);
       src.ddot = ddot;
+      launch_g2_build<true, true, true>(src, B, kout, Hio, Wio, Gout, Lo, s);
+    } else {
+      if (probs) {
+        LPB_REQUIRE(((4 * Hio * Wio) % 4) == 0, "head_bwd_bf16: plane size");
+        if (!g_out && win)
+          plane_dot_sparse_kernel<<<(unsigned)(((long long)B * kout + 7) / 8), 256, 0, s>>>(src, (long long)B * kout, 4 * Hio * Wio, ddot);
+        else
+          plane_dot_kernel<<<(unsigned)(B * kout), 256, 0, s>>>(src, 4 * Hio * Wio, ddot);
+        src.ddot = ddot;
+      }
+      if (g_out && probs) launch_g2_build<true, true>(src, B, kout, Hio, Wio, Gout, Lo, s);
+      else if (g_out) launch_g2_build<true, false>(src, B, kout, Hio, Wio, Gout, Lo, s);
+      else if (probs) launch_g2_build<false, true>(src, B, kout, Hio, Wio, Gout, Lo, s);
+      else launch_g2_build<false, false>(src, B, kout, Hio, Wio, Gout, Lo, s);
     }
-    if (g_out && probs) launch_g2_build<true, true>(src, B, kout, Hio, Wio, Gout, Lo, s);
-    else if (g_out) launch_g2_build<true, false>(src, B, kout, Hio, Wio, Gout, Lo, s);
-    else if (probs) launch_g2_build<false, true>(src, B, kout, Hio, Wio, Gout, Lo, s);
-    else launch_g2_build<false, false>(src, B, kout, Hio, Wio, Gout, Lo, s);
   }
   if (two) {
     // layer 2: weight + bias gradient (bias from the all-ones channel c1 of mid), then data gradient -> G1 (+ db1)

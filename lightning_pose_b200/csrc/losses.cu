@@ -186,18 +186,18 @@ __global__ void __launch_bounds__(HL_THREADS) heatmap_mse_from_kp_bwd_kernel(con
     for (int i = threadIdx.x; i < n; i += HL_THREADS) g[i] = 0.f;
     return;
   }
-  const float scale = 2.f * gout[0] / fwd_out[1];
+  const float scale = mse_target_scale(gout[0], fwd_out[1]);
   const float* __restrict__ p = pred + plane * (size_t)n;
   if (tp.mode == TARGET_UNIFORM) {
-    const float u = 1.0f / (float)n;
-    for (int i = threadIdx.x; i < n; i += HL_THREADS) g[i] = (__ldg(p + i) - u) * scale;
+    const float u = mse_target_uniform(n);
+    for (int i = threadIdx.x; i < n; i += HL_THREADS) g[i] = mse_target_grad(TARGET_UNIFORM, __ldg(p + i), u, 1.f, scale);
     return;
   }
   const float norm = target_axis_factors(tp, oh, ow, two_s2, ex, ey, red, HL_THREADS);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int r = warp; r < oh; r += HL_THREADS / 32) {
     const float er = ey[r] * norm;
-    for (int c = lane; c < ow; c += 32) g[(size_t)r * ow + c] = (__ldg(p + (size_t)r * ow + c) - ex[c] * er) * scale;
+    for (int c = lane; c < ow; c += 32) g[(size_t)r * ow + c] = mse_target_grad(TARGET_GAUSS, __ldg(p + (size_t)r * ow + c), ex[c], er, scale);
   }
 }
 
@@ -706,9 +706,9 @@ extern "C" int lpb_heatmap_mse_from_keypoints_fwd(const float* keypoints, const 
   LPB_REQUIRE(n_planes >= 1 && n_planes < (1ll << 31), "heatmap_mse_from_keypoints_fwd: bad n_planes");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t smem = (size_t)(oh + ow + 16) * sizeof(float);
-  heatmap_mse_from_kp_kernel<<<(unsigned)n_planes, HL_THREADS, smem, s>>>(
-      keypoints, visibility, preds, (float)((double)ow / (double)img_width), (float)((double)oh / (double)img_height), oh,
-      ow, (float)(2.0 * (double)sigma * (double)sigma), workspace);
+  const TargetGeom tg = target_geom(img_height, img_width, oh, ow, sigma);
+  heatmap_mse_from_kp_kernel<<<(unsigned)n_planes, HL_THREADS, smem, s>>>(keypoints, visibility, preds, tg.sx, tg.sy, oh, ow,
+                                                                          tg.two_s2, workspace);
   heatmap_loss_final_kernel<<<1, HL_THREADS, 0, s>>>(workspace, n_planes, out);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
@@ -820,9 +820,9 @@ extern "C" int lpb_heatmap_mse_from_keypoints_bwd(const float* keypoints, const 
               "heatmap_mse_from_keypoints_bwd: bad shape");
   LPB_REQUIRE(n_planes >= 1 && n_planes < (1ll << 31), "heatmap_mse_from_keypoints_bwd: bad n_planes");
   const size_t smem = (size_t)(oh + ow + 16) * sizeof(float);
+  const TargetGeom tg = target_geom(img_height, img_width, oh, ow, sigma);
   heatmap_mse_from_kp_bwd_kernel<<<(unsigned)n_planes, HL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
-      keypoints, visibility, preds, (float)((double)ow / (double)img_width), (float)((double)oh / (double)img_height), oh,
-      ow, (float)(2.0 * (double)sigma * (double)sigma), fwd_out, grad_out, grad_preds);
+      keypoints, visibility, preds, tg.sx, tg.sy, oh, ow, tg.two_s2, fwd_out, grad_out, grad_preds);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

@@ -65,4 +65,25 @@ __device__ __forceinline__ float target_axis_factors(const TargetPlane& tp, int 
   return 1.0f / (sxs * sys);
 }
 
+// grid scale (sx, sy) and 2 sigma^2 of the targets, from the image size and sigma the loss entries take
+struct TargetGeom {
+  float sx, sy, two_s2;
+};
+inline TargetGeom target_geom(float img_height, float img_width, int oh, int ow, float sigma) {
+  return {(float)((double)ow / (double)img_width), (float)((double)oh / (double)img_height), (float)(2.0 * (double)sigma * (double)sigma)};
+}
+
+// ---- gradient of the fused target + MSE (lpb_heatmap_mse_from_keypoints_bwd, and the head backward's target source) --
+// d loss / d pred = 2 (pred - target) / n_kept * grad_out = (pred - target) * scale on kept planes, 0 on dropped ones.
+__device__ __forceinline__ float mse_target_scale(float grad_out, float n_kept) { return 2.f * grad_out / n_kept; }
+// the uniform target of a plane of n pixels
+__device__ __forceinline__ float mse_target_uniform(int n) { return 1.0f / (float)n; }
+// One pixel: target = exc * er with exc = ex[column], er = ey[row] * norm for a Gaussian plane, and exc = 1/n, er = 1 for a
+// uniform one (the fma is then exactly pred - 1/n).  The intrinsics pin the rounding: one fused multiply-add, then a
+// separate multiply that no caller may fuse with what it does next, so every user gets the same bits.
+__device__ __forceinline__ float mse_target_grad(int mode, float p, float exc, float er, float scale) {
+  if (mode == TARGET_ZERO) return 0.f;
+  return __fmul_rn(__fmaf_rn(-exc, er, p), scale);
+}
+
 }  // namespace lpb

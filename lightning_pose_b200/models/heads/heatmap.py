@@ -123,6 +123,14 @@ class _HeadFunction(torch.autograd.Function):
         need_dfeat = ctx.needs_input_grad[0]
         if g is None and g_xy is None:
             return (None,) * (4 + 2 * n)
+        # the keypoint-target MSE's gradient on this node's own softmax output stays implicit: the tensor-core backward
+        # rebuilds it where it reads it; every other case takes the dense gradient
+        mse = None
+        if isinstance(g, ops.MseKeypointGrad):
+            if ctx.saved is not None and ctx.final_softmax and g.implicit_for(out):
+                mse, g = g, None
+            else:
+                g = g.materialize()
         if g is not None:
             g = g.contiguous().float()
         if ctx.saved is not None:
@@ -131,7 +139,7 @@ class _HeadFunction(torch.autograd.Function):
                 windows = ops.decode_backward_windows(out, stats, g_xy.contiguous().float(), int(ctx.decode[0]), float(ctx.decode[1]))
             dfeat, dw1, db1, dw2, db2 = ops.head_backward_bf16(
                 g, ctx.saved, tuple(features.shape), weights[0], weights[1] if n == 2 else None, need_dfeat=need_dfeat,
-                probs=out if ctx.final_softmax else None, windows=windows, layout=ctx.layout,
+                probs=out if ctx.final_softmax else None, windows=windows, layout=ctx.layout, mse=mse,
             )
             dws, dbs = ([dw1, dw2], [db1, db2]) if n == 2 else ([dw1], [db1])
             return (dfeat, None, None, None, *[d.to(w.dtype) for d, w in zip(dws, weights)], *[d.to(b.dtype) for d, b in zip(dbs, biases)])

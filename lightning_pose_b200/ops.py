@@ -10,7 +10,9 @@ import ctypes as C
 
 import torch
 
-from ._lib import PcaDesc, check, lib
+import torch.utils._pytree
+
+from ._lib import MseTargets, PcaDesc, check, lib
 
 __all__ = [
     "decode_softargmax",
@@ -45,12 +47,16 @@ def _stream() -> C.c_void_p:
 
 
 def _ptr(t: torch.Tensor | None) -> C.c_void_p:
+    if isinstance(t, MseKeypointGrad):
+        t = t.materialize()
     return C.c_void_p(0 if t is None else t.data_ptr())
 
 
 def _cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
         raise RuntimeError(f"lpb200: `{name}` must be a CUDA tensor (this package has no CPU fallback)")
+    if isinstance(t, MseKeypointGrad):
+        t = t.materialize()
     if t.dtype != torch.float32:
         t = t.float()
     return t.contiguous()
@@ -305,25 +311,28 @@ def decode_backward_windows(heatmaps, stats, grad_xy, ds, temperature):
     return win, meta, overflow
 
 
-def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None, layout=FEATURES_NCHW):
+def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None, layout=FEATURES_NCHW, mse=None):
     """Gradients of the bf16 head: returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None).  ``dfeat`` is dense in
     ``layout``, the memory format the forward read the features in.
 
     ``g_out``: dense gradient w.r.t. the head output or None; ``probs``: the head output when it ends in the
     spatial softmax (its backward is fused in), None for a logits head; ``windows``: result of
-    ``decode_backward_windows`` or None; ``w2`` None for a one-deconv head.
+    ``decode_backward_windows`` or None; ``w2`` None for a one-deconv head.  ``mse``: instead of ``g_out``, a
+    ``MseKeypointGrad`` of the loss on ``probs``, rebuilt inside the kernels (``lpb_head_bwd_bf16_targets``).
     """
     xs, fws = saved
     b, c, h, w = feat_shape
     g = _cuda_f32(g_out, "g_out") if g_out is not None else None
-    if g is None and windows is None:
+    if g is None and windows is None and mse is None:
         raise ValueError("head_backward_bf16 needs a dense gradient and/or decode windows")
+    if mse is not None and (g is not None or probs is None or not mse.implicit_for(probs)):
+        raise ValueError("head_backward_bf16: `mse` stands for the dense gradient of a loss on `probs`")
     w1 = _cuda_f32(w1, "w1")
     w2 = _cuda_f32(w2, "w2") if w2 is not None else None
     c1, c2 = w1.shape[1], (w2.shape[1] if w2 is not None else 0)
     dev = w1.device
     nbytes = C.c_size_t(0)
-    check(lib.lpb_head_bwd_bf16_workspace_bytes_layout(b, c, h, w, c1, c2, layout, C.byref(nbytes)))
+    check(lib.lpb_head_bwd_bf16_workspace_bytes_targets(b, c, h, w, c1, c2, layout, int(mse is not None), C.byref(nbytes)))
     ws = torch.empty((nbytes.value,), device=dev, dtype=torch.uint8)
     fmt = torch.channels_last if layout == FEATURES_NHWC else torch.contiguous_format
     dfeat = torch.empty((b, c, h, w), device=dev, dtype=torch.bfloat16, memory_format=fmt) if need_dfeat else None
@@ -332,9 +341,10 @@ def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=
     dw2 = torch.empty_like(w2) if w2 is not None else None
     db2 = torch.empty((c2,), device=dev, dtype=torch.float32) if w2 is not None else None
     win, meta, ov = windows if windows is not None else (None, None, None)
+    targets = C.byref(mse.targets()) if mse is not None else None
     with torch.cuda.device(dev):
-        check(lib.lpb_head_bwd_bf16_layout(_ptr(g), _ptr(probs), _ptr(win), _ptr(meta), _ptr(ov), _ptr(xs), _ptr(fws), b, c, h, w, _ptr(w1), c1, _ptr(w2), c2,
-                                    layout, _ptr(dfeat), _ptr(dw1), _ptr(db1), _ptr(dw2), _ptr(db2), _ptr(ws), _stream()))
+        check(lib.lpb_head_bwd_bf16_targets(_ptr(g), targets, _ptr(probs), _ptr(win), _ptr(meta), _ptr(ov), _ptr(xs), _ptr(fws), b, c, h, w, _ptr(w1), c1,
+                                            _ptr(w2), c2, layout, _ptr(dfeat), _ptr(dw1), _ptr(db1), _ptr(dw2), _ptr(db2), _ptr(ws), _stream()))
     return dfeat, dw1, db1, dw2, db2
 
 
@@ -932,13 +942,55 @@ class _HeatmapMseFromKeypoints(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         kp, vis, preds, out = ctx.saved_tensors
-        height, width, sigma = ctx.meta
-        b, k, oh, ow = preds.shape
-        gp = torch.empty_like(preds)
-        gg = g.reshape(1).contiguous().float()
-        with torch.cuda.device(preds.device):
-            check(lib.lpb_heatmap_mse_from_keypoints_bwd(_ptr(kp), _ptr(vis), _ptr(preds), b * k, height, width, oh, ow, sigma, _ptr(out), _ptr(gg), _ptr(gp), _stream()))
-        return None, None, gp, None, None, None
+        return None, None, MseKeypointGrad(kp, vis, preds, out, g.reshape(1).contiguous().float(), ctx.meta), None, None, None
+
+
+class MseKeypointGrad(torch.Tensor):
+    """d loss / d preds of ``heatmap_mse_from_keypoints``, held as what it is computed from (keypoints, visibility, the
+    preds, the forward's out, the upstream gradient) rather than as a dense (B, K, h, w) fp32 tensor.
+
+    The bf16 head's backward consumes it as it is when ``preds`` is that head's own output: its kernels rebuild the values
+    where they read them (``lpb_head_bwd_bf16_targets``), so the dense gradient is never written.  Any other use -- a
+    torch op, autograd adding a second gradient, ``record_stream``, a hook, the tensor ``torch.autograd.grad`` hands back,
+    the fp32 head -- goes through ``__torch_dispatch__`` (or ``materialize``), which writes the dense gradient once with
+    ``lpb_heatmap_mse_from_keypoints_bwd``, keeps it, and runs the op on it: the same values bit for bit."""
+
+    __torch_function__ = torch._C._disabled_torch_function_impl
+
+    @staticmethod
+    def __new__(cls, kp, vis, preds, fwd_out, grad_out, meta):
+        t = torch.Tensor._make_wrapper_subclass(cls, preds.shape, strides=preds.stride(), dtype=preds.dtype, device=preds.device)
+        t.src = (kp, vis, preds, fwd_out, grad_out, meta)
+        t.dense = None
+        return t
+
+    def materialize(self) -> torch.Tensor:
+        """The dense gradient (written on the current stream at the first call)."""
+        if self.dense is None:
+            kp, vis, preds, out, gg, (height, width, sigma) = self.src
+            b, k, oh, ow = preds.shape
+            gp = torch.empty_like(preds)
+            with torch.cuda.device(preds.device):
+                check(lib.lpb_heatmap_mse_from_keypoints_bwd(_ptr(kp), _ptr(vis), _ptr(preds), b * k, height, width, oh, ow, sigma, _ptr(out), _ptr(gg), _ptr(gp), _stream()))
+            self.dense = gp
+        return self.dense
+
+    def implicit_for(self, heatmaps: torch.Tensor) -> bool:
+        """Whether a backward that owns ``heatmaps`` may take this gradient implicitly: not yet materialised, and the loss
+        read exactly ``heatmaps`` (same memory, shape and strides)."""
+        preds = self.src[2]
+        return (self.dense is None and preds.data_ptr() == heatmaps.data_ptr() and preds.shape == heatmaps.shape
+                and preds.stride() == heatmaps.stride() and preds.dtype == heatmaps.dtype)
+
+    def targets(self) -> MseTargets:
+        """The ``lpb_mse_targets`` descriptor of this gradient (device pointers; the tensors stay alive with ``self``)."""
+        kp, vis, _, out, gg, (height, width, sigma) = self.src
+        return MseTargets(kp.data_ptr(), vis.data_ptr() if vis is not None else None, height, width, sigma, out.data_ptr(), gg.data_ptr())
+
+    @classmethod
+    def __torch_dispatch__(cls, func, types, args=(), kwargs=None):
+        dense = lambda x: x.materialize() if isinstance(x, MseKeypointGrad) else x
+        return func(*torch.utils._pytree.tree_map(dense, args), **torch.utils._pytree.tree_map(dense, kwargs or {}))
 
 
 def heatmap_mse_from_keypoints(keypoints, preds, height, width, sigma=1.25, visibility=None):
