@@ -8,7 +8,8 @@
 H100 specifics: the running total never touches the host (the reference starts it as a CPU
 tensor and ``.to(device)``s it every iteration, :250,273), and when a factory holds more than one
 of {temporal, pca_singleview, pca_multiview} they are evaluated by ONE kernel launch whose result
-is handed to each loss object.
+is handed to each loss object.  ``LossFactory.total_on_device`` is the same sum with device-made
+weights and a device-held anneal weight, for training steps captured into a CUDA graph.
 """
 from __future__ import annotations
 
@@ -142,7 +143,7 @@ class LossFactory(_FactoryBase):
         args: dict[str, Any] = {}
         if "temporal" in names:
             t = self.loss_instance_dict["temporal"]
-            args.update(temporal_eps=t.epsilon, prob_threshold=float(t.prob_threshold), confidences=kwargs.get("confidences"))
+            args.update(temporal_eps=t.device_epsilon(kp.device), prob_threshold=float(t.prob_threshold), confidences=kwargs.get("confidences"))
         for n in ("pca_singleview", "pca_multiview"):
             if n in names:
                 args[n] = self.loss_instance_dict[n].kernel_params(kp.shape[1] // 2)
@@ -168,4 +169,33 @@ class LossFactory(_FactoryBase):
             logs += entries + [{"name": f"{stage}_{name}_loss_weighted", "value": weighted}]
         if total is None:
             total = torch.tensor(0.0)
+        return total, logs
+
+    def total_on_device(
+        self,
+        stage: Literal["train", "val", "test"] | None = None,
+        anneal_weight: torch.Tensor | None = None,
+        **kwargs: Any,
+    ) -> tuple[torch.Tensor, list[dict]]:
+        """``__call__``'s total and logs without the host, so that a training step captures into one CUDA graph.
+
+        Each weight is made on the device by a fill kernel instead of copied from the host.  ``anneal_weight`` is a
+        device scalar read by the multiply (a replay sees its value at replay time), or None for no annealing; the
+        ``_ANNEAL_EXEMPT`` losses keep weight 1 either way.  The logged values are detached (what Lightning's ``log``
+        keeps): a step's autograd graph must not outlive it, or the next step's backward would meet the previous
+        step's gradient nodes, whose stream may be another than the one being captured."""
+        fused = self._fused_unsupervised(kwargs)
+        if fused is not None:
+            kwargs = {**kwargs, L._FUSED_KEY: fused}
+        total: torch.Tensor | None = None
+        logs: list[dict] = []
+        for name, inst in self.loss_instance_dict.items():
+            value, entries = inst(stage=stage, **kwargs)
+            weighted = torch.full((), float(inst.weight), device=value.device) * value
+            scaled = weighted if (anneal_weight is None or name in _ANNEAL_EXEMPT) else anneal_weight * weighted
+            total = scaled if total is None else total + scaled
+            logs += [{**e, "value": e["value"].detach()} if isinstance(e["value"], torch.Tensor) else e for e in entries]
+            logs.append({"name": f"{stage}_{name}_loss_weighted", "value": weighted.detach()})
+        if total is None:
+            raise ValueError("the loss factory holds no losses")
         return total, logs

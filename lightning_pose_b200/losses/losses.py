@@ -67,6 +67,16 @@ class Loss:
         """``1 / (2 exp(log_weight))`` (reference :89-100)."""
         return 1.0 / (2.0 * torch.exp(self.log_weight))
 
+    def device_epsilon(self, device: torch.device) -> torch.Tensor:
+        """``epsilon`` on ``device``, copied there once (again only when ``epsilon`` is replaced): the kernels read it
+        without a copy from pageable host memory in the step, so the loss launch captures into a CUDA graph."""
+        cache = self.__dict__.setdefault("_device_epsilon", {})
+        key = (torch.device(device), id(self.epsilon))
+        if key not in cache:
+            cache.clear()
+            cache[key] = self.epsilon.to(device)
+        return cache[key]
+
     def remove_nans(self, **kwargs: Any) -> Any:
         raise NotImplementedError
 
@@ -286,7 +296,7 @@ class TemporalLoss(Loss):
         fused = kwargs.get(_FUSED_KEY)
         if fused is None:
             fused = ops.unsup_losses(
-                keypoints_pred, confidences, temporal_eps=self.epsilon, prob_threshold=float(self.prob_threshold)
+                keypoints_pred, confidences, temporal_eps=self.device_epsilon(keypoints_pred.device), prob_threshold=float(self.prob_threshold)
             )
         scalar_loss = fused[0]
         return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
@@ -335,7 +345,7 @@ class TemporalHeatmapLoss(Loss):
         **kwargs: Any,
     ) -> LossOutput:
         scalar_loss = ops.temporal_heatmap_loss(
-            heatmaps_pred, confidences, self._kind, self.epsilon, float(self.prob_threshold)
+            heatmaps_pred, confidences, self._kind, self.device_epsilon(heatmaps_pred.device), float(self.prob_threshold)
         )
         return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
 

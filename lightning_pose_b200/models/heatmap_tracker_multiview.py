@@ -19,6 +19,10 @@ Training with curriculum patch masking (the reference's ``PatchMasking`` callbac
 counter ``global_step`` (0 at construction, one more after every ``training_step``, as Lightning's ``global_step``
 advances once per optimizer step) and stores the mask in ``current_patch_mask``.  The step never leaves the device, so
 a training step captured into a CUDA graph masks with a fresh step on every replay.
+
+``SemiSupervisedHeatmapTrackerMultiviewTransformer`` (reference :370-484) adds the unlabeled multi-view video branch
+and its unsupervised losses (``pca_multiview``, ``pca_singleview``, ``temporal``, ``temporal_heatmap_*``) with the anneal
+weight held on the device, so its semi-supervised step captures into one CUDA graph as the labeled step does.
 """
 from __future__ import annotations
 
@@ -87,8 +91,9 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         view_idx = torch.arange(self.num_views, device=tokens.device).repeat(batch)  # [0..V-1, 0..V-1, ...]
         tokens = tokens + self.view_embeddings[view_idx].to(tokens.dtype).unsqueeze(1)
         seq = self.encoder(tokens.reshape(batch, self.num_views * n, d))  # all views of an example in one sequence
-        side = math.isqrt(n)
-        features = tokens_to_feature_map(seq.reshape(vb, n, d), (side, side))
+        h_img, w_img = images.shape[-2:]
+        patch = math.isqrt(h_img * w_img // n)  # square patches: n = (H / patch) * (W / patch), so H != W works too
+        features = tokens_to_feature_map(seq.reshape(vb, n, d), (h_img // patch, w_img // patch))
         return features if channels_last else features.contiguous()
 
     def forward(self, images: torch.Tensor) -> torch.Tensor:
@@ -159,21 +164,118 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
         RMSE diagnostic (a host-synchronising NaN filter) is left to ``evaluate_labeled``.  So the whole step captures
         into one CUDA graph.  ``last_logs`` holds detached values (what Lightning's ``log`` keeps): a step's autograd
         graph must not outlive it, or the next step's backward would meet the previous step's gradient nodes, whose
-        stream may be another than the one being captured."""
+        stream may be another than the one being captured (``LossFactory.total_on_device``)."""
+        total = self._labeled_step_loss(batch_dict, anneal_weight=None)
+        self.global_step.add_(1)
+        return {"loss": total}
+
+    def _labeled_step_loss(self, batch_dict: dict, anneal_weight: torch.Tensor | None) -> torch.Tensor:
+        """Patch masking of ``batch_dict["images"]`` at ``global_step`` (with an enabled ``patch_masker``), forward and
+        the labeled losses summed on the device; ``last_logs`` holds their detached values."""
         masker = self.patch_masker
         if masker is not None and masker.use_patch_masking:  # PatchMasking.on_train_batch_start (callbacks.py:222-263)
             batch_dict["images"], self.current_patch_mask = masker.apply_patch_masking(
                 batch_dict["images"], training_step=self.global_step, is_training=True)
-        data_dict = self.get_loss_inputs_labeled(batch_dict)
         assert self.loss_factory is not None
-        total: torch.Tensor | None = None
-        logs: list[dict] = []
-        for name, inst in self.loss_factory.loss_instance_dict.items():
-            value, entries = inst(stage="train", **data_dict)
-            weighted = torch.full((), float(inst.weight), device=value.device) * value
-            total = weighted if total is None else total + weighted
-            logs += [{**e, "value": e["value"].detach()} if isinstance(e["value"], torch.Tensor) else e for e in entries]
-            logs.append({"name": f"train_{name}_loss_weighted", "value": weighted.detach()})
-        self.last_logs = logs
+        total, self.last_logs = self.loss_factory.total_on_device("train", anneal_weight, **self.get_loss_inputs_labeled(batch_dict))
+        return total
+
+
+def view_transforms(transforms: torch.Tensor, num_views: int) -> torch.Tensor | None:
+    """The augmentation matrices of a multi-view unlabeled batch as (views, 2, 3), or None for an unaugmented batch
+    (a last dimension other than 3, e.g. the (views, 1) sentinel of ``frames_to_unlabeled_batch``).
+
+    Accepts the shapes the reference squeezes (``heatmap_tracker_multiview.py:449-462``): (views, 1, 2, 3) as
+    ``frames_to_unlabeled_batch`` returns it, (1, views, 2, 3) and (views, 2, 3).  Any other shape raises (the reference
+    logs a warning and undoes the wrong matrices)."""
+    if transforms.shape[-1] != 3:
+        return None
+    if transforms.dim() == 4:
+        if transforms.shape[1] == 1:
+            transforms = transforms.squeeze(1)
+        elif transforms.shape[0] == 1:
+            transforms = transforms.squeeze(0)
+    if tuple(transforms.shape) != (num_views, 2, 3):
+        raise ValueError(f"expected transforms (views, 2, 3) with views = {num_views}, (views, 1, 2, 3) or (1, views, 2, 3); "
+                         f"got {tuple(transforms.shape)}")
+    return transforms
+
+
+class SemiSupervisedHeatmapTrackerMultiviewTransformer(HeatmapTrackerMultiviewTransformer):
+    """Adds the unlabeled multi-view video branch and its unsupervised loss factory (reference :370-484).
+
+    An unlabeled batch holds frames (T, views, 3, H, W), one sequence per camera, as ``frames_to_unlabeled_batch``
+    returns them.  Its heatmaps are folded like the labeled ones, (T, views * K, h, w), so the temporal losses compare
+    consecutive frames of each view and ``pca_multiview`` reads the views of a frame side by side.
+
+    ``total_unsupervised_importance`` (the reference's attribute, which its ``AnnealWeight`` callback sets) is a device
+    scalar buffer here: a schedule changes it in place, ``model.total_unsupervised_importance.fill_(w)``, and a
+    ``training_step`` captured into a CUDA graph then uses the new value on its next replay.  Assigning a new tensor to
+    the attribute instead works eagerly but is not seen by a captured graph."""
+
+    def __init__(
+        self,
+        num_keypoints: int,
+        num_views: int,
+        patch_embed: nn.Module | Callable,
+        encoder: nn.Module | Callable,
+        embedding_dim: int,
+        loss_factory: LossFactory | None = None,
+        loss_factory_unsupervised: LossFactory | None = None,
+        backbone_arch: str = "vits_dino",
+        downsample_factor: Literal[1, 2, 3] = 2,
+        torch_seed: int = 123,
+        patch_masker: PatchMasker | None = None,
+        **kwargs: Any,
+    ) -> None:
+        super().__init__(
+            num_keypoints, num_views, patch_embed, encoder, embedding_dim, loss_factory=loss_factory,
+            backbone_arch=backbone_arch, downsample_factor=downsample_factor, torch_seed=torch_seed,
+            patch_masker=patch_masker, **kwargs,
+        )
+        self.loss_factory_unsup = loss_factory_unsupervised
+        # not part of the state dict, as the reference's plain attribute is not
+        self.register_buffer("total_unsupervised_importance", torch.ones(()), persistent=False)
+
+    def get_loss_inputs_unlabeled(self, batch_dict: dict) -> dict:
+        """Frames (T, views, 3, H, W) -> heatmaps (T, views * K, h, w), keypoints and confidences; the per-view affine
+        undo and the model -> frame map in one launch (reference :434-484)."""
+        frames = batch_dict["frames"]
+        if frames.dim() != 5 or frames.shape[1] != self.num_views:
+            raise ValueError(f"expected frames (T, {self.num_views}, 3, H, W); got {tuple(frames.shape)}")
+        pred_heatmaps, pred_keypoints_augmented, confidence = self.forward_with_keypoints(frames)
+        pred_keypoints = ops.remap_keypoints(
+            pred_keypoints_augmented, view_transforms(batch_dict["transforms"], self.num_views), batch_dict["bbox"],
+            frames.shape[-2], frames.shape[-1], is_multiview=True, num_views=self.num_views,
+        )
+        return {
+            "heatmaps_pred": pred_heatmaps,
+            "keypoints_pred": pred_keypoints,
+            "keypoints_pred_augmented": pred_keypoints_augmented,
+            "confidences": confidence,
+        }
+
+    def evaluate_unlabeled(self, batch_dict: dict, stage=None, anneal_weight=1.0) -> torch.Tensor:
+        data_dict = self.get_loss_inputs_unlabeled(batch_dict)
+        assert self.loss_factory_unsup is not None
+        loss, self.last_logs_unsup = self.loss_factory_unsup(stage=stage, anneal_weight=anneal_weight, **data_dict)
+        return loss
+
+    def training_step(self, batch_dict: dict, batch_idx: int) -> dict[str, torch.Tensor]:
+        """One semi-supervised step on ``{"labeled": ..., "unlabeled": ...}`` (the reference's mixin,
+        ``models/base.py:660-701``), then ``global_step`` + 1.
+
+        Labeled branch: the parent's ``training_step`` (patch masking of ``labeled["images"]``, the 3-D losses on
+        calibrated batches).  The unlabeled frames are not masked; the reference's ``PatchMasking`` callback looks for
+        top-level ``images`` / ``frames`` keys only (``callbacks.py:233-243``), so it masks neither branch of a
+        semi-supervised batch, while the labeled branch here is masked as a labeled step is.  Both branches' losses are scaled by ``total_unsupervised_importance`` except the
+        heatmap losses, which keep weight 1, as the reference's loss factory does.  Both sums run on the device
+        (``LossFactory.total_on_device``), so the whole step captures into one CUDA graph; ``last_logs`` and
+        ``last_logs_unsup`` hold detached values."""
+        anneal = self.total_unsupervised_importance
+        loss_super = self._labeled_step_loss(batch_dict["labeled"], anneal_weight=anneal)
+        assert self.loss_factory_unsup is not None
+        loss_unsuper, self.last_logs_unsup = self.loss_factory_unsup.total_on_device(
+            "train", anneal, **self.get_loss_inputs_unlabeled(batch_dict["unlabeled"]))
         self.global_step.add_(1)
-        return {"loss": total}
+        return {"loss": loss_super + loss_unsuper}
