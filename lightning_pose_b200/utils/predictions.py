@@ -10,8 +10,12 @@ Here one *chunk* of ``T`` frames is one CUDA-graph replay: head -> soft-argmax d
 rows of a preallocated ``(N, 3K)`` device table at a device-resident cursor (``lpb_pack_predictions``).  Nothing
 returns to the host until the video is done; then ONE device->host copy of the table.  The table's column order is the
 reference's, so ``PredictionHandler.make_pred_arr_undo_resize`` / ``make_dlc_pandas_index`` below produce the same CSV.
-Multi-GPU: replicas over contiguous frame ranges (``frame_range_for_rank``), no communication (the reference itself
-never predicts on more than one device).
+Multi-GPU (the reference itself never predicts on more than one device): ``BatchedPredictor(..., shard=(rank, world))``
+predicts rank ``rank``'s contiguous rows ``frame_range_for_rank(N, rank, world)`` into a full-length table at global rows,
+feeding ``feed_range``: its own frames, plus for a context model a 2-frame halo at each edge.  ``gather()`` is one
+all-gather of every rank's rows into the full table on every rank, then the context edge fill
+(``fill_context_edges``): each edge row whose source frame lies in another shard is copied from that frame's own row.
+The gathered table equals the one-GPU table bit for bit.
 """
 from __future__ import annotations
 
@@ -22,13 +26,67 @@ import torch
 
 from lightning_pose_b200 import ops
 
-__all__ = ["BatchedPredictor", "PredictionHandler", "make_dlc_pandas_index", "frame_range_for_rank"]
+__all__ = ["BatchedPredictor", "PredictionHandler", "make_dlc_pandas_index", "frame_range_for_rank", "shard_feed_range",
+           "context_edge_fill", "fill_context_edges"]
 
 
 def frame_range_for_rank(n_frames: int, rank: int, world: int) -> tuple[int, int]:
     """Contiguous, near-equal frame ranges: [start, stop) of ``rank`` (cfg 5: 100,000 frames -> 12,500 per GPU)."""
     per = -(-n_frames // max(world, 1))
     return min(rank * per, n_frames), min((rank + 1) * per, n_frames)
+
+
+def _context_rows(n_frames: int, chunk: int) -> int:
+    """R, the rows the reference's context reader produces for windows of S = T + 4 frames with step T (one window per
+    frame when T = 1): ``context_source_row`` in csrc/predict.cu."""
+    t = chunk
+    return n_frames if t == 1 else t * (-(-(n_frames - t - 4) // t) + 1)
+
+
+def _context_source(row: int, n_frames: int, r_rows: int) -> int:
+    """The frame whose prediction row ``row`` of the final context table holds (the rule of ``pack_context_kernel``)."""
+    if r_rows >= n_frames:
+        return min(max(row, 2), n_frames - 3)
+    return row if 2 <= row <= r_rows - 1 else 2
+
+
+def shard_feed_range(n_frames: int, chunk: int, rank: int, world: int, context: bool = False) -> tuple[int, int]:
+    """[lo, hi): the frames shard ``rank`` of ``world`` feeds, in chunks of ``chunk`` from frame lo, the last chunk padded
+    past hi as the one-GPU caller pads the video's end.  A frame model feeds its own rows' frames.  A context model's
+    row f needs frames f - 2 .. f + 2, so its shard feeds a 2-frame halo on each side, clamped to the video.  When
+    R = N - 1, row N - 2 reads the first padding frame N: a shard that owns that row starts one frame earlier if its
+    chunks would otherwise end exactly at frame N, so that frame N is fed and frame N - 2 is predicted."""
+    a, b = frame_range_for_rank(n_frames, rank, world)
+    if not context or a == b:
+        return a, b
+    lo, hi = max(a - 2, 0), min(b + 2, n_frames)
+    if _context_rows(n_frames, chunk) == n_frames - 1 and a <= n_frames - 2 < b and (n_frames - lo) % chunk == 0:
+        lo -= 1  # lo >= 1 here: lo = 0 would need N = 0 and N = 1 (mod T), so T = 1, where R = N
+    return lo, hi
+
+
+def context_edge_fill(n_frames: int, chunk: int, world: int) -> list[tuple[int, int]]:
+    """(row, source row) pairs that complete a context table gathered from ``world`` shards: every edge row (0, 1, the
+    last four) whose source frame's own row belongs to another shard.  The kernel writes a frame's prediction to all
+    its rows, but only the shard that owns the frame's row computes it from the right window; another shard's rows
+    hold a halo frame's prediction (or none) there.  Empty for one shard."""
+    n, per = n_frames, -(-n_frames // max(world, 1))
+    r_rows = _context_rows(n, chunk)
+    pairs = []
+    for row in sorted({0, 1, *range(max(n - 4, 0), n)}):
+        src = _context_source(row, n, r_rows)
+        if row // per != src // per:
+            pairs.append((row, src))
+    return pairs
+
+
+def fill_context_edges(table: torch.Tensor, chunk: int, world: int) -> torch.Tensor:
+    """Apply ``context_edge_fill`` to an (N, 3K) context table on its device, in place (one gather, one scatter)."""
+    pairs = context_edge_fill(table.shape[0], chunk, world)
+    if pairs:
+        dst, src = (torch.tensor(rows, dtype=torch.int64, device=table.device) for rows in zip(*pairs))
+        table.index_copy_(0, dst, table.index_select(0, src))
+    return table
 
 
 def make_dlc_pandas_index(model_type: str, keypoint_names: Sequence[str]):
@@ -200,12 +258,22 @@ class BatchedPredictor:
     tail with its first row).  Only when R = N - 1 does a row (N - 2) depend on frame N, the first padding frame of the
     last chunk; the reference reads the zero-filled frame its reader pads with there, so the caller's padding matters in
     that case only.  N < 5 raises (the reference has no window to predict from).
+
+    Shards (``shard=(rank, world)``; the default (0, 1) is the whole video): the predictor owns rows
+    ``rows = frame_range_for_rank(N, rank, world)`` of the full-length table and is fed ``feed_range``
+    (``shard_feed_range``), in chunks starting at its first frame, the last one padded as above.  The device cursor
+    starts there, so every writer and the crop ingest work in global rows unchanged.  A context shard's first two output
+    frames come from the zero halo.  They land in rows of other shards, which the gather overwrites, and in edge rows
+    whose source frame lies in another shard (when R < N frame 2's tail rows [R, N) may be the shard's own), which
+    the edge fill overwrites: the fill, not row ownership, is what discards them.  ``gather()`` assembles the table on
+    every rank.
     """
 
     def __init__(self, head, num_keypoints: int, n_frames: int, chunk: int, image_hw: tuple[int, int],
                  features_of: Callable[[torch.Tensor], torch.Tensor] | None = None, device=None, use_graph: bool = True,
                  sub_chunk: int | None = None, bboxes: torch.Tensor | None = None, frame_hw: tuple[int, int] | None = None,
-                 crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False, num_views: int = 1) -> None:
+                 crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False, num_views: int = 1,
+                 shard: tuple[int, int] = (0, 1)) -> None:
         from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
 
         self.head, self.k, self.n_frames, self.chunk = head, int(num_keypoints), int(n_frames), int(chunk)
@@ -219,6 +287,12 @@ class BatchedPredictor:
             raise ValueError(f"chunk must be >= 1; got {self.chunk}")
         if self.num_views < 1:
             raise ValueError(f"num_views must be >= 1; got {self.num_views}")
+        rank, world = (int(v) for v in shard)
+        if world < 1 or not 0 <= rank < world:
+            raise ValueError(f"shard must be (rank, world) with 0 <= rank < world; got {tuple(shard)}")
+        self.shard = (rank, world)
+        self.rows = frame_range_for_rank(self.n_frames, rank, world)
+        self.feed_range = shard_feed_range(self.n_frames, self.chunk, rank, world, self.context)
         # frames per head / decode call inside a chunk: small enough that the heatmaps written by the head are still in
         # the 126 MB L2 when the decode reads them (None: the whole chunk at once)
         self.sub_chunk = int(sub_chunk) if sub_chunk else self.chunk
@@ -226,8 +300,11 @@ class BatchedPredictor:
         self.features_of = features_of
         self.device = torch.device(device) if device is not None else next(head.parameters()).device
         self.crop_dtype, self.crop_channels_last = crop_dtype, bool(crop_channels_last)
-        self.table = torch.zeros((self.n_frames, 3 * self.k * self.num_views), dtype=torch.float32, device=self.device)
-        self.cursor = torch.zeros((1,), dtype=torch.int64, device=self.device)
+        # the table is the first N rows of ``world`` equal blocks, the all-gather's outputs (the last one padded)
+        per = -(-self.n_frames // world)
+        self._blocks = torch.zeros((per * world, 3 * self.k * self.num_views), dtype=torch.float32, device=self.device)
+        self.table = self._blocks[: self.n_frames]
+        self.cursor = torch.full((1,), self.feed_range[0], dtype=torch.int64, device=self.device)
         self.use_graph = use_graph
         self._graph = self._static = self._captured = None
         self.launches_per_chunk = None
@@ -262,7 +339,7 @@ class BatchedPredictor:
         return ((self._wf, 4), (self._wb, 4), (self._kp_sf, 2), (self._cf_sf, 2), (self._box, 2))
 
     def _reset(self) -> None:
-        self.cursor.zero_()
+        self.cursor.fill_(self.feed_range[0])
         self.table.zero_()
         if self.context:
             for buf, _ in self._halo():
@@ -380,7 +457,7 @@ class BatchedPredictor:
             self._chunk(form, self._static)
         self.launches_per_chunk = _graph_kernel_count(self._graph)
         self._graph.instantiate()
-        self.cursor.zero_()  # the capture itself does not execute, but keep the invariant explicit
+        self.cursor.fill_(self.feed_range[0])  # the capture itself does not execute, but keep the invariant explicit
 
     def feed(self, x: torch.Tensor | Sequence[torch.Tensor], bbox: torch.Tensor | None = None) -> None:
         """Process the next chunk: a tensor with an optional ``bbox``, V uint8 views, or in crop mode uint8 full frames
@@ -407,6 +484,23 @@ class BatchedPredictor:
                 self.feed(*item)
             else:
                 self.feed(item)
+        return self.table
+
+    def gather(self) -> torch.Tensor:
+        """The full (N, 3 V K) table on every rank, equal to the one-GPU table: one ``all_gather`` of each rank's block
+        of ``ceil(N / world)`` rows (its own rows, padded), then ``fill_context_edges`` on the device.  Every rank of
+        the default process group calls it, those without rows too; one shard needs no collective."""
+        rank, world = self.shard
+        if world > 1:
+            import torch.distributed as dist
+
+            if dist.get_world_size() != world or dist.get_rank() != rank:
+                raise ValueError(f"shard {self.shard} does not match the process group (rank {dist.get_rank()} of "
+                                 f"{dist.get_world_size()})")
+            blocks = list(self._blocks.split(self._blocks.shape[0] // world))
+            dist.all_gather(blocks, blocks[rank].clone())
+        if self.context:
+            fill_context_edges(self.table, self.chunk, world)
         return self.table
 
     def results(self) -> tuple[torch.Tensor, torch.Tensor]:
