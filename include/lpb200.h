@@ -83,7 +83,11 @@ int lpb_upsample2x(const float* in, int64_t n_planes, int h, int w, float* out, 
 
 /* ---- Gaussian target generation --------------------------------------------------------------
  * replaces generate_heatmaps  lightning_pose/data/heatmaps.py:11-87
- * keypoints [n_planes, 2] fp32 image pixels; visibility [n_planes] int32 {0,1,2} or NULL.
+ * keypoints [n_planes, 2] fp32 image pixels; visibility [n_planes] int32 or NULL (the reference's None: a NaN x or
+ * a point outside [-1, size + 1] on the grid gives a zero plane).  With a visibility, 0 -> zero plane, 1 -> uniform
+ * 1/(oh ow), 2 -> Gaussian (zero plane when NaN x / outside), any other value (3, -1, ...) -> the clamped Gaussian
+ * (NaN plane for a NaN coordinate), as the reference's masks leave it.  The same rule holds for every entry that
+ * takes a visibility (lpb_heatmap_mse_from_keypoints_*, lpb_mse_targets).
  * out [n_planes, oh, ow] fp32.
  */
 int lpb_generate_heatmaps(const float* keypoints, const int32_t* visibility, int64_t n_planes,
@@ -233,7 +237,7 @@ int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, const float
  * (which must be the head output, probs), rebuilt inside the backward's front end from the keypoints instead of read
  * from a dense g_out.  The per-pixel values are those lpb_heatmap_mse_from_keypoints_bwd writes, bit for bit; the
  * [n_planes, 8H, 8W] fp32 gradient never exists.  Fields are the arguments of the two loss entries (device pointers):
- * keypoints [B*C][2], visibility [B*C] or NULL, fwd_out the forward's out (out[1] = kept planes), grad_out the scalar
+ * keypoints [B*C][2], visibility [B*C] or NULL (the rule of lpb_generate_heatmaps), fwd_out the forward's out (out[1] = kept planes), grad_out the scalar
  * upstream gradient. */
 typedef struct lpb_mse_targets {
   const float* keypoints;

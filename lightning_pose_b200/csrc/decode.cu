@@ -848,6 +848,8 @@ __device__ __forceinline__ void decode_bwd_strip(const DecodeGeom<DS>& P, const 
 
 // Dense form: one CTA per plane (grid = n_planes), or -- queue mode -- per (plane, row segment) unit of the planes
 // the window kernel could not take; a unit adds its rows into the plane's pre-zeroed gradient with global atomics.
+// Those adds, and the shared-memory adds of overlapping strips (scatter_row<DS, true>), meet in no fixed order, so this
+// gradient (and the windows' overflow planes, which it writes) can differ in the last bits from call to call.
 constexpr int DEC_BWD_SEGS = 8;
 
 template <int DS>

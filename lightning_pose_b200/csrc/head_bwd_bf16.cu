@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(256) plane_dot_targets_kernel(G2Src S, int oh,
   __shared__ float dred[8];
   const size_t plane = blockIdx.x;
   const int hw = oh * ow;
-  const TargetPlane tp = classify_target(S.kp[2 * plane], S.kp[2 * plane + 1], S.vis ? S.vis[plane] : -1, S.sx, S.sy, oh, ow);
+  const TargetPlane tp = classify_target(S.kp, S.vis, plane, S.sx, S.sy, oh, ow);
   float* fac = S.fac + plane * S.fac_stride;
   if (threadIdx.x == 0) reinterpret_cast<int*>(fac)[0] = tp.mode;
   if (tp.mode != TARGET_ZERO) {

@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(HL_THREADS) heatmap_mse_from_kp_kernel(const f
   float* red = ey + oh;
   const size_t plane = blockIdx.x;
   const int n = oh * ow;
-  const TargetPlane tp = classify_target(kp[2 * plane], kp[2 * plane + 1], vis ? vis[plane] : -1, sx, sy, oh, ow);
+  const TargetPlane tp = classify_target(kp, vis, plane, sx, sy, oh, ow);
   if (tp.mode == TARGET_ZERO) {  // dropped plane: the prediction is not even read
     if (threadIdx.x == 0) {
       ws[2 * plane] = 0.f;
@@ -180,7 +180,7 @@ __global__ void __launch_bounds__(HL_THREADS) heatmap_mse_from_kp_bwd_kernel(con
   float* red = ey + oh;
   const size_t plane = blockIdx.x;
   const int n = oh * ow;
-  const TargetPlane tp = classify_target(kp[2 * plane], kp[2 * plane + 1], vis ? vis[plane] : -1, sx, sy, oh, ow);
+  const TargetPlane tp = classify_target(kp, vis, plane, sx, sy, oh, ow);
   float* __restrict__ g = gpred + plane * (size_t)n;
   if (tp.mode == TARGET_ZERO) {
     for (int i = threadIdx.x; i < n; i += HL_THREADS) g[i] = 0.f;

@@ -20,7 +20,7 @@ __global__ void __launch_bounds__(TGT_THREADS) generate_heatmaps_kernel(const fl
   float* ey = sm + ow;
   float* red = ey + oh;
   const size_t plane = blockIdx.x;
-  const TargetPlane tp = classify_target(kp[2 * plane], kp[2 * plane + 1], vis ? vis[plane] : -1, sx, sy, oh, ow);
+  const TargetPlane tp = classify_target(kp, vis, plane, sx, sy, oh, ow);
   float* __restrict__ dst = out + plane * (size_t)oh * ow;
   const int n = oh * ow;
   if (tp.mode != TARGET_GAUSS) {
@@ -39,6 +39,9 @@ __global__ void __launch_bounds__(TGT_THREADS) generate_heatmaps_kernel(const fl
 // d loss / d keypoints of the normalised Gaussian:  d g_rc / d x = g_rc (c - xbar) / sigma^2 with
 // xbar = sum g c  (softmax-like Jacobian); chain through the clamp (zero outside [-1, size+1]) and the
 // image->grid scale.  Used by keep_gradients=True (lightning_pose/data/heatmaps.py:37-40).
+// The sums take c and r relative to the grid point (c0, r0) nearest the centre: sum G g (c - xbar) is unchanged by the
+// shift, and its two terms stay of the size of the result instead of c times larger (in fp32, sum G g c - xbar sum G g
+// at c ~ 190 loses the gradient of a sharp target, and most of it when the centre is clamped off the grid's edge).
 __global__ void __launch_bounds__(TGT_THREADS) generate_heatmaps_bwd_kernel(const float* __restrict__ kp,
                                                                             const int32_t* __restrict__ vis,
                                                                             const float* __restrict__ gout, float sx,
@@ -50,23 +53,26 @@ __global__ void __launch_bounds__(TGT_THREADS) generate_heatmaps_bwd_kernel(cons
   float* red = ey + oh;  // 16 floats
   const size_t plane = blockIdx.x;
   const float xr = kp[2 * plane], yr = kp[2 * plane + 1];
-  const TargetPlane tp = classify_target(xr, yr, vis ? vis[plane] : -1, sx, sy, oh, ow);
+  const TargetPlane tp = classify_target(kp, vis, plane, sx, sy, oh, ow);
   if (tp.mode != TARGET_GAUSS) {
     if (threadIdx.x == 0) gkp[2 * plane] = gkp[2 * plane + 1] = 0.f;
     return;
   }
   const float norm = target_axis_factors(tp, oh, ow, two_s2, ex, ey, red, TGT_THREADS);
   const float* __restrict__ g = gout + plane * (size_t)oh * ow;
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f, m1 = 0.f, m2 = 0.f;  // sum G g, sum G g c, sum G g r, sum g c, sum g r
+  // (a NaN centre gives NaN sums whatever c0, r0 are)
+  const int c0 = (int)fminf(fmaxf(rintf(tp.x), 0.f), (float)(ow - 1)), r0 = (int)fminf(fmaxf(rintf(tp.y), 0.f), (float)(oh - 1));
+  // sum G g, sum G g (c - c0), sum G g (r - r0), sum g (c - c0), sum g (r - r0)
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f, m1 = 0.f, m2 = 0.f;
   for (int i = threadIdx.x; i < oh * ow; i += TGT_THREADS) {
     const int r = i / ow, c = i - r * ow;
     const float gv = ex[c] * ey[r] * norm;
     const float Gg = g[i] * gv;
     s0 += Gg;
-    s1 = fmaf(Gg, (float)c, s1);
-    s2 = fmaf(Gg, (float)r, s2);
-    m1 = fmaf(gv, (float)c, m1);
-    m2 = fmaf(gv, (float)r, m2);
+    s1 = fmaf(Gg, (float)(c - c0), s1);
+    s2 = fmaf(Gg, (float)(r - r0), s2);
+    m1 = fmaf(gv, (float)(c - c0), m1);
+    m2 = fmaf(gv, (float)(r - r0), m2);
   }
   float vals[5] = {s0, s1, s2, m1, m2};
   __shared__ float acc[5][TGT_THREADS / 32];

@@ -12,22 +12,27 @@ struct TargetPlane {
   float x, y;  // clamped heatmap-grid coordinates (NaN propagates, as torch.clamp does)
 };
 
-// vis < 0 means "visibility is None".
-__device__ __forceinline__ TargetPlane classify_target(float xr, float yr, int vis, float sx, float sy, int oh, int ow) {
+// Plane `plane` of keypoints kp (x, y image pixels); vis null means "visibility is None".  With a visibility, only 0, 1 and
+// 2 change the plane: any other value (3, -1, ...) keeps the clamped Gaussian, NaN included.
+__device__ __forceinline__ TargetPlane classify_target(const float* kp, const int32_t* vis, size_t plane, float sx, float sy,
+                                                       int oh, int ow) {
   TargetPlane t;
-  const float x = xr * sx, y = yr * sy;  // :41-42
+  const float x = kp[2 * plane] * sx, y = kp[2 * plane + 1] * sy;  // :41-42
   // :43-49 - only x is tested for NaN; NaN comparisons are false
   const bool bad = isnan(x) || (x < -1.f) || (x > (float)(ow + 1)) || (y < -1.f) || (y > (float)(oh + 1));
   t.x = isnan(x) ? x : fminf(fmaxf(x, -1.f), (float)(ow + 1));  // :52-53
   t.y = isnan(y) ? y : fminf(fmaxf(y, -1.f), (float)(oh + 1));
-  if (vis < 0) {
+  if (!vis) {
     t.mode = bad ? TARGET_ZERO : TARGET_GAUSS;  // :78-79
-  } else if (vis == 0) {
+    return t;
+  }
+  const int v = vis[plane];
+  if (v == 0) {
     t.mode = TARGET_ZERO;  // :81
-  } else if (vis == 1) {
+  } else if (v == 1) {
     t.mode = TARGET_UNIFORM;  // :82
   } else {
-    t.mode = (vis == 2 && bad) ? TARGET_ZERO : TARGET_GAUSS;  // :83
+    t.mode = (v == 2 && bad) ? TARGET_ZERO : TARGET_GAUSS;  // :83
   }
   return t;
 }

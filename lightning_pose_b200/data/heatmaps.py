@@ -29,7 +29,8 @@ def generate_heatmaps(
     """(batch, num_keypoints, 2) image-pixel keypoints -> normalised Gaussian heatmaps.
 
     NaN / out-of-bounds keypoints give all-zero planes; with ``visibility``: 0 -> zeros,
-    1 -> uniform, 2 -> Gaussian (zeros if also out of bounds).  ``keep_gradients=True`` makes the
+    1 -> uniform, 2 -> Gaussian (zeros if also out of bounds), any other value (3, -1, ...) ->
+    the clamped Gaussian, as the reference's masks leave it.  ``keep_gradients=True`` makes the
     result differentiable with respect to ``keypoints``.
     """
     return ops.generate_heatmaps(keypoints, height, width, output_shape, sigma, keep_gradients, visibility)
