@@ -47,9 +47,11 @@ int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s);
 // the banded path (lpb_head_bf16_plan): maps up to 56 x 56.
 constexpr size_t HEAD_FEATURE_SMEM_BUDGET = 200 * 1024;
 inline size_t rows_shuffle_smem_bytes(int H, int W) { return (size_t)32 * H * W * 2; }
-// Stage budget of the banded kernel and of the backward's layer-2 data gradient (b2d, two CTAs per SM): half of an H100
-// SM's 227 KB.
+// Stage budget of the backward's layer-2 data gradient (b2d, two CTAs per SM): half of an H100 SM's 227 KB.
 constexpr size_t HEAD_STAGE_SMEM_BUDGET = 113 * 1024;
+// The banded kernel runs one CTA per SM (its accumulators take the register file): stages, statistics and the epilogue
+// warps' scratch share an H100 SM's 227 KB.
+constexpr size_t CR_SMEM_BUDGET = 227 * 1024;
 
 // raster rows per band of the banded kernel (its M-tiles x 128)
 constexpr int CR_BAND_ROWS = 256;

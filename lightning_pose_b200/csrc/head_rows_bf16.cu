@@ -138,6 +138,16 @@ constexpr int CR_EPI = 256;
 constexpr int CR_TILES = 2;      // M-tiles per band: a warp's accumulators (CR_TILES x 32 rows x 48 columns) stay in registers
 static_assert(CR_TILES * 128 == CR_BAND_ROWS, "head_rows.cuh sizes the per-band softmax statistics with CR_BAND_ROWS");
 constexpr int CR_STAGES = 2;
+// after the stages: the softmax statistics [2][HEAD_CLS][8 warps], fin [HEAD_CLS][2] and the four barriers (+ slack), then
+// each MMA warp's epilogue scratch (mma_sm90.cuh rows_store)
+constexpr size_t CR_STAT_BYTES = (2 * HEAD_CLS * 8 + 2 * HEAD_CLS) * sizeof(float) + 64;
+constexpr size_t CR_SCRATCH_BYTES = (size_t)(CR_EPI / 32) * mma::ROWS_SCRATCH * sizeof(float);
+inline size_t convt_rows_smem_bytes(int rows_alloc) {
+  return (size_t)CR_STAGES * (4 * rows_alloc * 16 + HEAD_BSTAGE_BYTES) + CR_STAT_BYTES + CR_SCRATCH_BYTES;
+}
+// the widest band the kernel takes (Pp = CR_BAND_ROWS: one image row and its halo row, launch_convt_rows' rows_alloc)
+static_assert(CR_STAGES * (4 * ((2 * CR_BAND_ROWS + 8 + 7) & ~7) * 16 + HEAD_BSTAGE_BYTES) + CR_STAT_BYTES + CR_SCRATCH_BYTES <= CR_SMEM_BUDGET,
+              "the banded kernel's stages and scratch fit one CTA per SM at every accepted width");
 
 // NPL: compile-time plane count (17 = the usual keypoint count) or 0 for a run-time count <= 20.
 // The softmax modes' epilogue takes one warp vote per tile (instead of one per plane), keeps the running-max rescale out
@@ -157,6 +167,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
   uint64_t* bars = reinterpret_cast<uint64_t*>(fin + 2 * HEAD_CLS);
   uint64_t* full = bars;       // [2]
   uint64_t* empty = bars + 2;  // [2]
+  float* scratch = reinterpret_cast<float*>(smem + CR_STAGES * stage_bytes + CR_STAT_BYTES);  // [8 warps][ROWS_SCRATCH]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < CR_STAGES * stage_bytes / 16; i += CR_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
@@ -216,6 +227,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
     // classes (py = e, px = 0 | 1) = accumulator columns [40e, 40e + 40); the warp accumulates [32e, 32e + 48) over the
     // stages and reads them out in "lane = row" form
     const int q = warp & 3, e = (warp - 2) >> 2, ew = warp - 2;
+    float* scr = scratch + ew * mma::ROWS_SCRATCH;
     const float L2E = 1.4426950408889634f;
     const size_t plane_stride = (size_t)Ho * Wo;
     const bool use_bias = P.bias && (MODE == CONVT_ROWS_MID || MODE == CONVT_ROWS_PLANES);  // a per-plane constant does not change a softmax
@@ -303,15 +315,18 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 #pragma unroll
           for (int t = 0; t < CR_TILES; ++t) {
             if (t >= tiles) break;
-            float d[48];
-#pragma unroll
-            for (int nt = 0; nt < 6; ++nt) mma::rows8(acc[t], nt, &d[8 * nt], lane);
             const int row = t * 128 + 32 * q + lane;
             const int ml = row / Pp, n = row - ml * Pp;
             const bool valid = (ml < rb) && (n < Wi);
             const int y = 2 * (y0 + ml) + e, x = 2 * n;
             auto body = [&](auto ec) {
               constexpr int E = decltype(ec)::value;
+              // the epilogue reads columns [8E, 8E + 20 + ncls) of the warp's 48: n8 tiles E .. E + 4, the last one
+              // only for more than 12 planes.  rl[c] = accumulator column 8E + c of row `lane`.
+              __syncwarp();  // the previous block's reads of the scratch are done
+              mma::rows_store<E, 5>(scr, acc[t], (HEAD_CLS + ncls + 7) / 8, lane);
+              __syncwarp();
+              const float* rl = mma::rows_lane(scr, lane);
               if constexpr (MODE == CONVT_ROWS_MID && WIDE) {
                 // T rows of the next layer, by 4-channel units (8-byte halves of a K-chunk): the group's five units
                 // 5g .. 5g + 4, and the last group also the units past the groups up to the end of the last K-chunk.
@@ -333,7 +348,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                         for (int hh = 0; hh < 2; ++hh) {
                           const int cl = 4 * i + 2 * e2 + hh;  // compile-time channel within the group
                           const int ch = o0 + cl;
-                          f[hh] = ch < P.cout ? d[8 * E + px * HEAD_CLS + cl] + (use_bias ? __ldg(bias + cl) : 0.f) : (ch == P.cout ? 1.0f : 0.f);
+                          f[hh] = ch < P.cout ? rl[px * HEAD_CLS + cl] + (use_bias ? __ldg(bias + cl) : 0.f) : (ch == P.cout ? 1.0f : 0.f);
                         }
                         pk[e2] = Operand<T>::pack2(f[0], f[1]);
                       }
@@ -366,7 +381,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                           const int ch = kc * 8 + 2 * e2 + hh;  // compile-time
                           float val = 0.f;
                           if (ch < HEAD_CLS) {
-                            if (ch < P.cout) val = d[8 * E + px * HEAD_CLS + ch] + (use_bias ? __ldg(P.bias + ch) : 0.f);
+                            if (ch < P.cout) val = rl[px * HEAD_CLS + ch] + (use_bias ? __ldg(P.bias + ch) : 0.f);
                             else if (ch == P.cout) val = 1.0f;
                           } else if (ch == P.cout) {
                             val = 1.0f;
@@ -389,14 +404,14 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
 #pragma unroll
                   for (int o = 0; o < HEAD_CLS; ++o) {
                     if (o >= ncls) break;
-                    need |= fmaxf(d[8 * E + o], d[8 * E + HEAD_CLS + o]) > mx[o];
+                    need |= fmaxf(rl[o], rl[HEAD_CLS + o]) > mx[o];
                   }
                   if (__any_sync(0xffffffffu, need && valid)) {
                     if (valid) {
 #pragma unroll
                       for (int o = 0; o < HEAD_CLS; ++o) {
                         if (o >= ncls) break;
-                        const float tm = fmaxf(d[8 * E + o], d[8 * E + HEAD_CLS + o]);
+                        const float tm = fmaxf(rl[o], rl[HEAD_CLS + o]);
                         if (tm > mx[o]) {
                           sm[o] *= fast_exp2((mx[o] - tm) * L2E);
                           mx[o] = tm;
@@ -409,7 +424,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                     for (int o = 0; o < HEAD_CLS; ++o) {
                       if (o >= ncls) break;
                       const float mL = mx[o] * L2E;
-                      sm[o] += fast_exp2(fmaf(d[8 * E + o], L2E, -mL)) + fast_exp2(fmaf(d[8 * E + HEAD_CLS + o], L2E, -mL));
+                      sm[o] += fast_exp2(fmaf(rl[o], L2E, -mL)) + fast_exp2(fmaf(rl[HEAD_CLS + o], L2E, -mL));
                     }
                   }
                 } else if (valid) {
@@ -418,8 +433,8 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                   for (int o = 0; o < HEAD_CLS; ++o) {
                     if (o >= ncls) break;
                     const float2 f = reinterpret_cast<const float2*>(fin)[o];
-                    const float p0 = fast_exp2(fmaf(d[8 * E + o], L2E, -f.x)) * f.y;
-                    const float p1 = fast_exp2(fmaf(d[8 * E + HEAD_CLS + o], L2E, -f.x)) * f.y;
+                    const float p0 = fast_exp2(fmaf(rl[o], L2E, -f.x)) * f.y;
+                    const float p1 = fast_exp2(fmaf(rl[HEAD_CLS + o], L2E, -f.x)) * f.y;
                     *reinterpret_cast<float2*>(dst) = make_float2(p0, p1);
                     dst += plane_stride;
                   }
@@ -430,7 +445,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                 for (int o = 0; o < HEAD_CLS; ++o) {
                   if (o >= ncls) break;
                   const float bo = use_bias ? __ldg(bias + o) : 0.f;
-                  const float l0 = d[8 * E + o] + bo, l1 = d[8 * E + HEAD_CLS + o] + bo;
+                  const float l0 = rl[o] + bo, l1 = rl[HEAD_CLS + o] + bo;
                   if (valid) *reinterpret_cast<float2*>(dst + (size_t)o * plane_stride) = make_float2(l0, l1);
                 }
               }
@@ -488,8 +503,8 @@ int launch_convt_rows(ConvtRowsParams<T> p, int sms, cudaStream_t s) {
   const int tiles = (p.R * Pp + 127) / 128;
   p.rows_alloc = (tiles * 128 + Pp + 1 + 7) & ~7;
   if (p.rows_alloc < (p.R + 1) * Pp + 8) p.rows_alloc = ((p.R + 1) * Pp + 8 + 7) & ~7;
-  const size_t smem = (size_t)CR_STAGES * (4 * p.rows_alloc * 16 + HEAD_BSTAGE_BYTES) + (2 * HEAD_CLS * 8 + 2 * HEAD_CLS) * sizeof(float) + 64;
-  LPB_REQUIRE(smem <= HEAD_STAGE_SMEM_BUDGET, "%s: band stages need %zu B shared memory", name, smem);
+  const size_t smem = convt_rows_smem_bytes(p.rows_alloc);
+  LPB_REQUIRE(smem <= CR_SMEM_BUDGET, "%s: band stages need %zu B shared memory", name, smem);
   const int nbands = (p.L.Hi + p.R - 1) / p.R;
   auto run = [&](auto kern, long long nitems) -> int {
     const int grid = (int)(nitems < sms ? nitems : sms);  // one CTA per SM: the accumulators take the register file

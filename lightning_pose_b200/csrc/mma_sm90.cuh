@@ -4,8 +4,8 @@
 //
 // A warp owns a block of 32 accumulator rows (two m16 tiles) x 8*NT columns (NT n8 tiles):
 //   acc[mt][nt][0..3] = D(16 mt + g, 8 nt + 2 t + {0, 1}) and D(16 mt + g + 8, ...)   (g = lane / 4, t = lane % 4).
-// rows8() turns one n8 tile into "lane = accumulator row" form, the layout the head's epilogues read (all but b3a's,
-// which stores the fragments as they are).
+// rows8() turns one n8 tile into "lane = accumulator row" form with shuffles, the layout the head's epilogues read
+// (b3a's stores the fragments as they are; the banded kernel's goes through shared memory, rows_store() below).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -197,6 +197,41 @@ template <int NT>
 __device__ __forceinline__ void rows8(const float (&acc)[2][NT][4], int nt, float* v, int lane) {
   rows8_at<0>(acc, nt, v, lane);
 }
+
+// ---- "lane = row" through shared memory (the banded kernel's epilogue; it reads ~34 of a row's 40 columns) --------
+// A warp writes n8 tiles NT0 .. NT0 + NTS - 1 of its 32-row block (m16 tiles 0, 1) into its own scratch of ROWS_SCRATCH
+// floats with 64-bit stores of the fragment pairs as they lie, then reads D(lane, 8 NT0 + c) at rows_lane(s, lane)[c].
+// The scratch is the warp's alone, so a __syncwarp orders its writes before its reads, and its reads before the next
+// block's writes.  Element (row r, column c) is at float r * ROWS_STRIDE + 2 (r / 4) + c.  Banks, with
+// ROWS_STRIDE = 56 = 24 (mod 32): row r starts at bank 8 (3 r mod 4) + 2 (r / 4) (mod 32), always even, so every pair
+// is 8-byte aligned.
+//  * st.shared.v2.f32, a wavefront per half-warp: its lanes (g, t) hold rows r0 + g (r0 = 0 mod 4, g / 4 fixed) and
+//    columns 8 nt + 2 t, i.e. banks 8 (3 g mod 4) + 2 t + {0, 1} + const: four rows 8 banks apart, four pairs each within
+//    8 banks -- 32 distinct banks, conflict-free.
+//  * ld.shared.f32, one row per lane: the starts 8 (3 r mod 4) + 2 (r / 4) of rows 0..31 hit each even bank exactly
+//    twice, so a column read is 2-way -- the least possible with even (pair-aligned) row starts.
+// A row spans 2 * 7 + 8 NTS <= ROWS_STRIDE floats: NTS <= 5.
+constexpr int ROWS_STRIDE = 56;
+constexpr int ROWS_SCRATCH = 32 * ROWS_STRIDE;
+
+// the tiles j < ntiles (a warp-uniform run-time bound) of NT0 .. NT0 + NTS - 1
+template <int NT0, int NTS, int NT>
+__device__ __forceinline__ void rows_store(float* s, const float (&acc)[2][NT][4], int ntiles, int lane) {
+  static_assert(NT0 + NTS <= NT && 2 * 7 + 8 * NTS <= ROWS_STRIDE, "scratch rows hold 8 NTS columns after the skew");
+  const int g = lane >> 2, t = lane & 3;
+  float* p = s + g * ROWS_STRIDE + 2 * (g >> 2) + 2 * t;
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r0 = 16 * mt + 8 * h;  // compile-time after unrolling; (r0 + g) / 4 = r0 / 4 + g / 4
+#pragma unroll
+      for (int j = 0; j < NTS; ++j)
+        if (j < ntiles)
+          *reinterpret_cast<float2*>(p + r0 * ROWS_STRIDE + 2 * (r0 >> 2) + 8 * j) = make_float2(acc[mt][NT0 + j][2 * h], acc[mt][NT0 + j][2 * h + 1]);
+    }
+}
+__device__ __forceinline__ const float* rows_lane(const float* s, int lane) { return s + lane * ROWS_STRIDE + 2 * (lane >> 2); }
 
 }  // namespace mma
 }  // namespace lpb
