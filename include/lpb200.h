@@ -349,6 +349,32 @@ int lpb_frames_augment_normalize(const uint8_t* frames_u8, int F, int H, int W, 
                                  const int64_t* seed, const float* mean3, const float* std3, int layout, int out_bf16,
                                  void* out, float* transform_out, void* stream);
 
+/* ---- single-frame ingest: crop, OpenCV resize and numpy normalisation, bit for bit --------------------------------
+ * replaces the preprocessing of Model.predict_frame  lightning_pose/api/model.py:388-430 (a numpy-slice crop,
+ * cv2.resize(..., INTER_LINEAR) on uint8, then (u8 / 255.0 - mean) / std in fp32 numpy), for all F frames in one launch.
+ * frames_u8 [F, H, W, 3] RGB (device), F >= 1 (1 frame, or the 5 frames of a context window).
+ * box: DEVICE int32 [x, y, w, h], read at run time (one captured graph serves every box), or NULL for the whole frame.
+ * It is cut as frame[y:y+h, x:x+w]: the crop is actual_h = min(H, y + h) - y rows by actual_w = min(W, x + w) - x
+ * columns.  The caller refuses what the reference refuses (x or y < 0, w or h <= 0, an empty crop); a box outside those
+ * rules is clamped into the frame, never read out of bounds.
+ * bbox_out (DEVICE, 4 floats): [x, y, actual_h, actual_w], or [0, 0, H, W] without a box: the bbox of
+ * lpb_remap_keypoints that maps model pixels back to the frame.
+ * Resize to out_h x out_w: OpenCV 4.x INTER_LINEAR on 8-bit images (imgproc resize.cpp, the fixed-point path).  Per
+ * output axis, scale = 1.0 / ((double)dst / src), f = (float)((d + 0.5) * scale - 0.5) in double then rounded to
+ * float, s = floor(f), f -= s, s0 = clamp(s, 0, src - 1), s1 = clamp(s + 1, 0, src - 1), a1 = rint(f * 2048),
+ * a0 = rint((1 - f) * 2048); the vertical weights are NOT zeroed where a row index is clamped.  Per channel
+ * S(y, x) = a0[x] img[y, x0] + a1[x] img[y, x1] (int32) and
+ *   u = clamp((((b0 (S(y0) >> 4)) >> 16) + ((b1 (S(y1) >> 4)) >> 16) + 2) >> 2, 0, 255),
+ * the rule of OpenCV's vectorised vertical pass, used for every pixel (its scalar tail, (b0 S0 + b1 S1 + 2^21) >> 22,
+ * differs in the last bit on about 10 % of pixels; cv2.resize 4.13 matched the vector rule on every tested shape).
+ * An exact 2x downscale equals OpenCV's INTER_AREA switch under this rule; out size == crop size copies the crop.
+ * Normalisation: (u / 255.0f - mean) / std, three correctly rounded fp32 operations without contraction; mean3 / std3
+ * HOST arrays of three floats.  out: layout 0 [F, 3, out_h, out_w] or 1 [F, out_h, out_w, 3], LPB_OUT_F32 / BF16 /
+ * F16 (bf16 / fp16 are the fp32 value rounded to nearest even). */
+int lpb_frames_crop_resize_cv2(const uint8_t* frames_u8, int F, int H, int W, const int32_t* box, int out_h, int out_w,
+                               const float* mean3, const float* std3, int layout, int out_format, void* out,
+                               float* bbox_out, void* stream);
+
 /* ---- curriculum patch masking of multi-view transformer training ----------------------------------------------
  * replaces PatchMasker.apply_patch_masking  lightning_pose/callbacks.py:303-401  (the PatchMasking callback's
  * on_train_batch_start, :222-263).  Images (B, V, C, H, W) are cut into LPB_PATCH_SIZE x LPB_PATCH_SIZE patches,

@@ -250,7 +250,102 @@ __global__ void __launch_bounds__(256) augment_kernel(const __grid_constant__ Au
   }
 }
 
+// ---- single-frame ingest: numpy-slice crop, OpenCV INTER_LINEAR on uint8, numpy's fp32 normalisation -----------------
+// The preprocessing of the reference's Model.predict_frame (lightning_pose/api/model.py:388-430), bit for bit: the rule
+// is restated in lpb200.h and tests/frame_resize_oracle.py.  The box is read from device memory, so one captured graph
+// serves every box.  Every weight is recomputed per output pixel from the crop size (a few fp64 operations): the crop
+// size changes with the box, and a 384 x 384 output is small enough that tables would only add a launch.
+struct CropCv2Params {
+  const uint8_t* in;
+  const int32_t* box;  // [x, y, w, h] or NULL (the whole frame)
+  void* out;
+  float* bbox_out;     // [x, y, actual_h, actual_w]
+  int F, H, W, OH, OW;
+  float mean[3], std[3];
+};
+
+// Taps of output index d on one axis (src -> dst): the source indices and their 11-bit fixed-point weights, as
+// OpenCV's resize computes them (f in double, rounded to float, then split and scaled by 2^11 with rint).  The
+// intrinsics keep every operation correctly rounded and uncontracted.
+__device__ __forceinline__ void cv2_linear_taps(int d, int src, int dst, int& i0, int& i1, int& w0, int& w1) {
+  const double scale = __ddiv_rn(1.0, __ddiv_rn((double)dst, (double)src));
+  const float fx = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
+  const float s = floorf(fx);
+  const float fr = __fsub_rn(fx, s);
+  const int si = (int)s;
+  i0 = min(max(si, 0), src - 1);
+  i1 = min(max(si + 1, 0), src - 1);
+  w1 = __float2int_rn(__fmul_rn(fr, 2048.f));
+  w0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fr), 2048.f));
+}
+
+template <int LAYOUT, int FMT>
+__global__ void __launch_bounds__(256) crop_resize_cv2_kernel(const __grid_constant__ CropCv2Params P) {
+  // the host refuses the boxes numpy would reject; the clamps only keep a bad box inside the frame
+  int bx = 0, by = 0, cw = P.W, ch = P.H;
+  if (P.box) {
+    bx = min(max(P.box[0], 0), P.W - 1), by = min(max(P.box[1], 0), P.H - 1);
+    cw = min(max(P.box[2], 1), P.W - bx), ch = min(max(P.box[3], 1), P.H - by);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    P.bbox_out[0] = (float)bx, P.bbox_out[1] = (float)by, P.bbox_out[2] = (float)ch, P.bbox_out[3] = (float)cw;
+  }
+  const int64_t total = (int64_t)P.F * P.OH * P.OW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % P.OW);
+    const int64_t r = i / P.OW;
+    const int y = (int)(r % P.OH), f = (int)(r / P.OH);
+    int x0, x1, a0, a1, y0, y1, b0, b1;
+    cv2_linear_taps(x, cw, P.OW, x0, x1, a0, a1);
+    cv2_linear_taps(y, ch, P.OH, y0, y1, b0, b1);
+    const uint8_t* img = P.in + (size_t)f * P.H * P.W * 3;
+    const uint8_t* r0 = img + ((size_t)(by + y0) * P.W + bx) * 3;
+    const uint8_t* r1 = img + ((size_t)(by + y1) * P.W + bx) * 3;
+    float v[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      // horizontal pass in int32, then the vertical pass of OpenCV's vector path: (b * (S >> 4)) >> 16 per row
+      const int s0 = a0 * r0[x0 * 3 + c] + a1 * r0[x1 * 3 + c];
+      const int s1 = a0 * r1[x0 * 3 + c] + a1 * r1[x1 * 3 + c];
+      const int u = min(max((((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2, 0), 255);
+      v[c] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), P.mean[c]), P.std[c]);
+    }
+    store_pixel<LAYOUT, FMT>(P.out, P.OH, P.OW, f, y, x, v);
+  }
+}
+
 }  // namespace lpb
+
+extern "C" int lpb_frames_crop_resize_cv2(const uint8_t* frames_u8, int F, int H, int W, const int32_t* box, int out_h,
+                                          int out_w, const float* mean3, const float* std3, int layout, int out_format,
+                                          void* out, float* bbox_out, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(frames_u8 && mean3 && std3 && out && bbox_out, "frames_crop_resize_cv2: null pointer");
+  LPB_REQUIRE(F >= 1 && H >= 1 && W >= 1 && out_h >= 1 && out_w >= 1 && (layout == 0 || layout == 1),
+              "frames_crop_resize_cv2: bad shape/layout");
+  LPB_REQUIRE(valid_out_format(out_format), "frames_crop_resize_cv2: unknown output format %d", out_format);
+  CropCv2Params p;
+  p.in = frames_u8;
+  p.box = box;
+  p.out = out;
+  p.bbox_out = bbox_out;
+  p.F = F, p.H = H, p.W = W, p.OH = out_h, p.OW = out_w;
+  for (int c = 0; c < 3; ++c) {  // HOST arrays, as for lpb_frames_normalize
+    LPB_REQUIRE(std3[c] > 0.f, "frames_crop_resize_cv2: std must be positive");
+    p.mean[c] = mean3[c], p.std[c] = std3[c];
+  }
+  const int64_t total = (int64_t)F * out_h * out_w;
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > 132 * 32) blocks = 132 * 32;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  with_out_format(out_format, [&](auto fc) {
+    constexpr int FMT = decltype(fc)::value;
+    if (layout == 0) crop_resize_cv2_kernel<0, FMT><<<(unsigned)blocks, 256, 0, s>>>(p);
+    else crop_resize_cv2_kernel<1, FMT><<<(unsigned)blocks, 256, 0, s>>>(p);
+  });
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
 
 extern "C" int lpb_frames_normalize(const uint8_t* frames_u8, int F, int H, int W, int out_h, int out_w, const float* mean3,
                                     const float* std3, int layout, int out_format, void* out, void* stream) {

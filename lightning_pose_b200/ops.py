@@ -622,6 +622,43 @@ def frames_normalize(frames_u8, size=None, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     return out
 
 
+def frames_crop_resize_cv2(frames_u8, size, box=None, mean=IMAGENET_MEAN, std=IMAGENET_STD, channels_last=False,
+                           dtype=torch.float32, out=None, bbox_out=None):
+    """uint8 (F, H, W, 3) frames -> the preprocessing of the reference's ``Model.predict_frame`` in one launch: the
+    numpy-slice crop ``frame[y:y+h, x:x+w]``, ``cv2.resize(INTER_LINEAR)`` on uint8 and ``(u8 / 255 - mean) / std`` in
+    fp32, bit for bit (``lpb_frames_crop_resize_cv2``).
+
+    ``box``: None (the whole frame) or a 4-element int32 CUDA tensor [x, y, w, h], read by the kernel (the caller has
+    refused a negative origin, a non-positive size and an empty crop).  Returns (frames (F, 3, h, w) [or (F, h, w, 3)],
+    bbox (1, 4) fp32 [x, y, actual_h, actual_w]), written into ``out`` / ``bbox_out`` when given."""
+    if not isinstance(frames_u8, torch.Tensor) or not frames_u8.is_cuda:
+        raise RuntimeError("lpb200: `frames` must be a CUDA tensor (this package has no CPU fallback)")
+    if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[-1] != 3 or frames_u8.shape[0] < 1:
+        raise ValueError(f"frames must be uint8 (F >= 1, H, W, 3); got {tuple(frames_u8.shape)} {frames_u8.dtype}")
+    fmt = _out_format(dtype)
+    dev = frames_u8.device
+    if box is not None and (not isinstance(box, torch.Tensor) or box.device != dev or box.dtype != torch.int32
+                            or box.numel() != 4 or not box.is_contiguous()):
+        raise ValueError("box must be a contiguous 4-element int32 tensor [x, y, w, h] on the frames' device")
+    x = frames_u8.contiguous()
+    f, h, w, _ = x.shape
+    oh, ow = int(size[0]), int(size[1])
+    shape = (f, oh, ow, 3) if channels_last else (f, 3, oh, ow)
+    if out is None:
+        out = torch.empty(shape, device=dev, dtype=dtype)
+    elif tuple(out.shape) != shape or out.dtype != dtype or out.device != dev or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous {dtype} {shape} tensor on the frames' device")
+    if bbox_out is None:
+        bbox_out = torch.empty((1, 4), device=dev, dtype=torch.float32)
+    elif bbox_out.dtype != torch.float32 or bbox_out.device != dev or bbox_out.numel() != 4 or not bbox_out.is_contiguous():
+        raise ValueError("bbox_out must be a contiguous 4-element float32 tensor on the frames' device")
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(dev):
+        check(lib.lpb_frames_crop_resize_cv2(_ptr(x), f, h, w, _ptr(box), oh, ow, m3, s3, int(bool(channels_last)), fmt,
+                                             _ptr(out), _ptr(bbox_out), _stream()))
+    return out, bbox_out.view(1, 4)
+
+
 INGEST_MAX_VIEWS = 16  # LPB_INGEST_MAX_VIEWS (include/lpb200.h)
 
 

@@ -19,6 +19,7 @@ The gathered table equals the one-GPU table bit for bit.
 """
 from __future__ import annotations
 
+import operator
 from typing import Callable, Iterable, Sequence
 
 import numpy as np
@@ -26,8 +27,8 @@ import torch
 
 from lightning_pose_b200 import ops
 
-__all__ = ["BatchedPredictor", "PredictionHandler", "make_dlc_pandas_index", "frame_range_for_rank", "shard_feed_range",
-           "context_edge_fill", "fill_context_edges"]
+__all__ = ["BatchedPredictor", "FramePredictor", "PredictionHandler", "make_dlc_pandas_index", "frame_range_for_rank",
+           "shard_feed_range", "context_edge_fill", "fill_context_edges"]
 
 
 def frame_range_for_rank(n_frames: int, rank: int, world: int) -> tuple[int, int]:
@@ -514,3 +515,171 @@ class BatchedPredictor:
         """The V (N, 3K) column blocks of the table, one per view (views, not copies)."""
         w = 3 * self.k
         return [self.table[:, w * v : w * (v + 1)] for v in range(self.num_views)]
+
+
+class FramePredictor:
+    """One frame in, its keypoints out, with one CUDA-graph replay per call: the reference's ``Model.predict_frame``
+    (``lightning_pose/api/model.py:298-509``) for loops that need each answer before the next camera frame.
+
+    ``head``: a ``HeatmapHead`` or ``HeatmapMHCRNNHead`` on the device, in eval mode; ``features_of`` maps the ingested
+    (F, 3, h, w) images (channels-last memory with ``channels_last``) to backbone features, e.g. the tracker's
+    ``backbone``.  ``image_hw`` is the model's input size (``image_resize_dims``); ``dtype`` / ``channels_last`` the
+    ingest's output, what ``features_of`` takes; ``mean`` / ``std`` the normalisation.
+
+    ``predict_frame(frame_rgb, bbox=None)`` keeps the reference's contract: ``frame_rgb`` is uint8 (H, W, 3), or
+    (5, H, W, 3) for a context model (the T = 5 frames its labeled batches use; other T raise), as a host numpy array or
+    a CUDA tensor already on the device; ``bbox`` an optional (x, y, w, h) crop, cut as ``frame[y:y+h, x:x+w]`` (the far
+    edges clip to the frame).  Returns ``{"keypoints": (K, 2), "confidence": (K,)}`` float32 numpy arrays in
+    original-frame pixels, and raises ``ValueError`` where the reference does.
+
+    Body: ``ops.frames_crop_resize_cv2`` (the reference's cv2 resize and numpy normalisation, bit for bit, with the box
+    read on the device) -> ``features_of`` -> head -> soft-argmax decode -> model -> frame remap -> one (K, 3) row.  A
+    context head runs ``HeatmapTrackerMHCRNN``'s labeled form on (1, 5, 3, h, w) and keeps, per keypoint, the
+    multi-frame prediction where its confidence is greater than the single-frame one (a NaN keeps single-frame).
+
+    With ``use_graph`` the first call of each input form (host or device frame, frame shape) is captured; a new form
+    captures anew and replaces the old graph.  The images' dtype, and with it the features', is fixed per predictor.
+    The box changes on every call without a capture.  A host frame and the box are written to pinned staging buffers whose
+    host -> device copies are nodes of the graph, and the result comes back by a device -> host copy inside it; a
+    device frame is copied into the graph's input buffer on the device.  A call is: write the staging buffers, replay,
+    synchronise once, return copies.  ``launches_per_call`` counts the captured kernels.  ``use_graph=False`` runs the
+    same body eagerly.
+    """
+
+    CONTEXT_FRAMES = 5
+
+    def __init__(self, head, num_keypoints: int, image_hw: tuple[int, int], features_of: Callable[[torch.Tensor], torch.Tensor],
+                 device=None, use_graph: bool = True, dtype: torch.dtype = torch.float32, channels_last: bool = False,
+                 mean: Sequence[float] = ops.IMAGENET_MEAN, std: Sequence[float] = ops.IMAGENET_STD) -> None:
+        from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
+
+        if features_of is None:
+            raise ValueError("features_of (images -> backbone features) is required")
+        ops._out_format(dtype)
+        self.head, self.k = head, int(num_keypoints)
+        self.context = isinstance(head, HeatmapMHCRNNHead)
+        self.image_hw = (int(image_hw[0]), int(image_hw[1]))
+        self.features_of = features_of
+        self.device = torch.device(device) if device is not None else next(head.parameters()).device
+        self.use_graph = bool(use_graph)
+        self.dtype, self.channels_last = dtype, bool(channels_last)
+        self.mean, self.std = tuple(float(v) for v in mean), tuple(float(v) for v in std)
+        # the (K, 3) result: a context call writes the one frame of a five-row window to all five rows
+        # (lpb_pack_context_predictions with frame0 = 4, step 1), a frame call writes row 0
+        self._table = torch.zeros((self.CONTEXT_FRAMES if self.context else 1, 3 * self.k), dtype=torch.float32, device=self.device)
+        self._box = torch.zeros(4, dtype=torch.int32, device=self.device)
+        self._pin_box = torch.zeros(4, dtype=torch.int32).pin_memory()
+        self._pin_out = torch.zeros((self.k, 3), dtype=torch.float32).pin_memory()
+        self._key = self._graph = self._frames = self._pin_frames = None
+        self.launches_per_call = None
+
+    def _check(self, frame_rgb, bbox) -> tuple[np.ndarray | torch.Tensor, tuple[int, int, int, int]]:
+        """The reference's input checks (api/model.py:353-407) -> (frames (F, H, W, 3), box [x, y, w, h])."""
+        if isinstance(frame_rgb, torch.Tensor):
+            if frame_rgb.dtype != torch.uint8:
+                raise ValueError(f"frame_rgb must be uint8, got {frame_rgb.dtype}")
+            if not frame_rgb.is_cuda:
+                frame_rgb = frame_rgb.numpy()
+            elif frame_rgb.device != self.device:
+                raise ValueError(f"frame_rgb is on {frame_rgb.device}; the model is on {self.device}")
+        else:
+            frame_rgb = np.asarray(frame_rgb)
+            if frame_rgb.dtype != np.uint8:
+                raise ValueError(f"frame_rgb must be uint8, got {frame_rgb.dtype}")
+        shape = tuple(frame_rgb.shape)
+        if len(shape) not in (3, 4) or shape[-1] != 3:
+            raise ValueError(f"frame_rgb must be (H, W, 3) or (T, H, W, 3), got shape {shape}")
+        if int(np.prod(shape)) == 0:
+            raise ValueError("frame_rgb is empty")
+        if self.context and len(shape) == 3:
+            raise ValueError(f"a context model requires frame_rgb of shape ({self.CONTEXT_FRAMES}, H, W, 3); got a single frame "
+                             f"{shape}. Use BatchedPredictor for video input.")
+        if self.context and shape[0] != self.CONTEXT_FRAMES:
+            raise ValueError(f"a context model takes {self.CONTEXT_FRAMES} frames, the context length of its labeled batches; "
+                             f"got {shape[0]}")
+        if not self.context and len(shape) == 4:
+            raise ValueError(f"a single-frame model takes one (H, W, 3) frame; got shape {shape}")
+        h, w = shape[-3], shape[-2]
+        if bbox is None:
+            return frame_rgb, (0, 0, w, h)
+        bx, by, bw, bh = (operator.index(v) for v in bbox)
+        if bx < 0 or by < 0:
+            raise ValueError(f"bbox origin must be non-negative, got x={bx}, y={by}")
+        if bw <= 0 or bh <= 0:
+            raise ValueError(f"bbox width and height must be positive, got w={bw}, h={bh}")
+        if bx >= w or by >= h:
+            raise ValueError(f"bbox (x={bx}, y={by}, w={bw}, h={bh}) produces an empty crop on frame of shape {shape}")
+        return frame_rgb, (bx, by, min(bw, w), min(bh, h))  # sizes past the frame clip as the numpy slice does
+
+    def _body(self) -> torch.Tensor:
+        """Ingest -> features -> head -> decode -> remap into ``_table``; returns the (K, 3) result row (device)."""
+        head, (mh, mw) = self.head, self.image_hw
+        x, bbox = ops.frames_crop_resize_cv2(self._frames, self.image_hw, self._box, self.mean, self.std,
+                                             channels_last=self.channels_last, dtype=self.dtype)
+        if self.channels_last:
+            x = x.permute(0, 3, 1, 2)
+        feats = self.features_of(x)
+        if not self.context:
+            _, kp, cf = head.forward_with_keypoints(feats)
+            kp = ops.remap_keypoints(kp, None, bbox, mh, mw)
+            ops.pack_predictions(kp, cf, self._table, row0=0)
+            return self._table.view(self.k, 3)
+        t = self.CONTEXT_FRAMES
+        # HeatmapTrackerMHCRNN.forward on a (1, 5, 3, h, w) labeled batch
+        reps = torch.permute(feats.reshape(1, t, *feats.shape[1:]), (0, 2, 3, 4, 1))
+        sf, mf = head(reps, (1, t, 3, mh, mw), False)
+        kp_sf, cf_sf = head.run_subpixelmaxima(sf)
+        kp_mf, cf_mf = head.run_subpixelmaxima(mf)
+        # a table of five rows, fed frame0 = 4: output frame 2, which is every row's source
+        ops.pack_context_predictions(kp_sf, cf_sf, kp_mf, cf_mf, bbox, mh, mw, self._table, 1, frame0=t - 1)
+        return self._table[2].view(self.k, 3)
+
+    @torch.no_grad()
+    def _call(self, from_host: bool) -> None:
+        """One call's device work on the current stream: staging -> device, the body, result -> pinned buffer."""
+        if from_host:
+            self._frames.copy_(self._pin_frames, non_blocking=True)
+        self._box.copy_(self._pin_box, non_blocking=True)
+        self._pin_out.copy_(self._body(), non_blocking=True)
+
+    def _prepare(self, key) -> None:
+        """Buffers (and with ``use_graph`` the graph) of an input form: (host?, frame shape)."""
+        self._key, self._graph = key, None
+        from_host, shape = key
+        self._frames = torch.zeros(shape, dtype=torch.uint8, device=self.device)
+        self._pin_frames = torch.zeros(shape, dtype=torch.uint8).pin_memory() if from_host else None
+        if not self.use_graph:
+            return
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(side):
+            for _ in range(2):  # warm-up: per-shape tables, allocator pools
+                self._call(from_host)
+        torch.cuda.current_stream(self.device).wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        graph = torch.cuda.CUDAGraph(keep_graph=True)  # kept so that its kernel nodes can be counted
+        with torch.cuda.graph(graph):
+            self._call(from_host)
+        self.launches_per_call = _graph_kernel_count(graph)
+        graph.instantiate()
+        self._graph = graph
+
+    def predict_frame(self, frame_rgb, bbox: tuple[int, int, int, int] | None = None) -> dict[str, np.ndarray]:
+        """The reference's ``predict_frame``: ``{"keypoints": (K, 2), "confidence": (K,)}`` float32, frame pixels."""
+        frames, box = self._check(frame_rgb, bbox)
+        from_host = not isinstance(frames, torch.Tensor)
+        shape = tuple(frames.shape) if frames.ndim == 4 else (1, *frames.shape)
+        if self._key != (from_host, shape):
+            self._prepare((from_host, shape))
+        self._pin_box.numpy()[:] = box
+        if from_host:
+            np.copyto(self._pin_frames.numpy(), frames.reshape(shape))
+        else:
+            self._frames.copy_(frames.reshape(shape))
+        if self._graph is not None:
+            self._graph.replay()
+        else:
+            self._call(from_host)
+        torch.cuda.current_stream(self.device).synchronize()
+        out = self._pin_out.numpy()
+        return {"keypoints": out[:, :2].copy(), "confidence": out[:, 2].copy()}
