@@ -68,6 +68,9 @@ int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds
 int lpb_decode_bwd(const float* heatmaps, const float* stats, const float* grad_xy, int64_t n_planes,
                    int h, int w, int ds, float temperature, float* grad_heatmaps, void* stream);
 
+/* Both decode backward entries are bit-reproducible: every element of grad_heatmaps / g_overflow is a sum in an order
+ * fixed by the shapes and the inputs (no float atomics), so identical inputs give identical bits on the same device
+ * model. */
 /* sparse form of lpb_decode_bwd for the fused head backward: per plane a 32x32 window of d loss / d heatmap
  * (win [n_planes, 32, 32]) and meta [n_planes, 4] = {window row0, col0, flag, float bits of sum(win * heatmap)};
  * flag 0: zero gradient, 1: window valid, 2: the support does not fit a window -- that plane's dense
@@ -137,7 +140,14 @@ int lpb_head_fwd_f32(const float* features, int B, int C, int H, int W, const fl
  *                       logical tensor.
  *   lpb_plane_softmax_f32  in-place spatial softmax (T = 1) of [n_planes, hw]
  *   lpb_convt_bwd_f32   autograd of lpb_convt_fwd_f32: grad_in (same shape as `in`, may be NULL), grad_w [Cin,Cout,3,3],
- *                       grad_bias [Cout] (may be NULL); all overwritten. */
+ *                       grad_bias [Cout] (may be NULL); all overwritten.  NOT bit-reproducible: grad_w and grad_bias are
+ *                       summed over the K-split CTAs with float atomics, so their last bits can change from call to call.
+ *   lpb_convt_bwd_f32_ws   the same gradients, bit-reproducible: each K-split CTA ("slot") stores its grad_w tile and
+ *                       bias sums as a partial in `workspace`, and the slots are added in slot order.  The slot count
+ *                       follows the device's SM count (at most 264), so the order -- and the bits -- are fixed per device
+ *                       model and shape.  workspace: lpb_convt_bwd_f32_workspace_bytes(B, Cin, Hi, Wi, Cout) bytes (the
+ *                       conv-input sizes, as above), 4-byte aligned; NULL only when that is 0.  workspace_bytes is its
+ *                       size (LPB_ERR_INVALID if smaller, before anything is queued).  Only the call's own kernels use it. */
 #define LPB_SHUFFLE_NONE 0
 #define LPB_SHUFFLE_NCHW 1
 #define LPB_SHUFFLE_NHWC 2
@@ -146,6 +156,10 @@ int lpb_convt_fwd_f32(const float* in, int B, int Cin, int Hi, int Wi, int shuff
 int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* stream);
 int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
                       int Cout, float* grad_in, float* grad_w, float* grad_bias, void* stream);
+int lpb_convt_bwd_f32_workspace_bytes(int B, int Cin, int Hi, int Wi, int Cout, size_t* bytes);
+int lpb_convt_bwd_f32_ws(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
+                         int Cout, float* grad_in, float* grad_w, float* grad_bias, void* workspace, size_t workspace_bytes,
+                         void* stream);
 
 /* bf16 tensor-core path (tensor-core mma): features bf16 NCHW, fp32 master weights (rounded to bf16 on device, as
  * autocast does), fp32 accumulate, fp32 heatmaps.  One-deconv heads (ViT family, heads/heatmap.py:192-193: pass
@@ -281,7 +295,12 @@ int lpb_remap_keypoints_bwd(const float* grad_out, int64_t n, int K, const float
  * lpb_crnn_combine_fwd: WF, WB [N, K, H, W] = W_f / W_b applied to each of N frames ONCE (head kernels), idx [M, 5] =
  * frame index of each context slot of each of M outputs (overlapping windows share frames: no 5x feature tiling)
  * -> out_logits [M, K, H, W] = (x_f + x_b) / 2 before the spatial softmax.  lpb_crnn_combine_bwd: its autograd
- * (dWF, dWB [N,K,H,W], dLf/dLb [K,4,4], dhf/dhb [K,4]; all overwritten).  M * K < 65536 per call.
+ * (dWF, dWB [N,K,H,W], dLf/dLb [K,4,4], dhf/dhb [K,4]; all overwritten).  M * K < 65536 per call.  It sums with
+ * float atomics and is NOT bit-reproducible.  lpb_crnn_combine_bwd_ws: the same gradients, bit-reproducible for any idx:
+ * each element of dWF / dWB is one sum over the (window, slot) pairs that read its frame, window ascending then slot
+ * (a pair list built on the device, no host sync), and dL / dh are per-CTA partials added in a fixed order.  workspace:
+ * lpb_crnn_combine_bwd_workspace_bytes(M, N, K, H, W) bytes, 16-byte aligned, workspace_bytes its size (LPB_ERR_INVALID
+ * if smaller or NULL, before anything is queued).
  * lpb_context_gather: the materialised window tensor out[i][s] = seq[clamp(i + s - ctx/2)] for API parity
  * (n items of item_bytes, a multiple of 16).  lpb_context_gather_bwd: its adjoint, d_seq [n, elems] = for each frame
  * the sum of the grad [n, ctx, elems] slots that read it (the repeated edge frames included), in a fixed order without
@@ -295,6 +314,11 @@ int lpb_crnn_combine_fwd(const float* WF, const float* WB, const int32_t* idx, i
 int lpb_crnn_combine_bwd(const float* WF, const float* WB, const int32_t* idx, const float* grad_logits, int M, int N, int K,
                          int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb, float* dWF,
                          float* dWB, float* dLf, float* dhf, float* dLb, float* dhb, void* stream);
+int lpb_crnn_combine_bwd_workspace_bytes(int M, int N, int K, int H, int W, size_t* bytes);
+int lpb_crnn_combine_bwd_ws(const float* WF, const float* WB, const int32_t* idx, const float* grad_logits, int M, int N, int K,
+                            int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb, float* dWF,
+                            float* dWB, float* dLf, float* dhf, float* dLb, float* dhb, void* workspace, size_t workspace_bytes,
+                            void* stream);
 int lpb_context_gather(const void* seq, int64_t n, int64_t item_bytes, int ctx, void* out, void* stream);
 int lpb_context_gather_bwd(const void* grad, int64_t n, int64_t elems, int ctx, int format, void* d_seq, void* stream);
 

@@ -67,6 +67,8 @@ SIGNATURES = {
     "lpb_convt_fwd_f32": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P]),
     "lpb_plane_softmax_f32": (C.c_int, [_P, _L, _I, _P]),
     "lpb_convt_bwd_f32": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
+    "lpb_convt_bwd_f32_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, C.POINTER(_Z)]),
+    "lpb_convt_bwd_f32_ws": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P, _P, _Z, _P]),
     "lpb_head_bf16_plan": (C.c_int, [_I, _I, _I, _I, _I, C.POINTER(_I)]),
     "lpb_head_bf16_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bf16_saved_bytes": (C.c_int, [_I, _I, _I, _I, C.POINTER(_Z)]),
@@ -88,6 +90,8 @@ SIGNATURES = {
     "lpb_crnn_prepare_bwd": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "lpb_crnn_combine_fwd": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "lpb_crnn_combine_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "lpb_crnn_combine_bwd_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, C.POINTER(_Z)]),
+    "lpb_crnn_combine_bwd_ws": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
     "lpb_context_gather": (C.c_int, [_P, _L, _L, _I, _P, _P]),
     "lpb_context_gather_bwd": (C.c_int, [_P, _L, _L, _I, _I, _P, _P]),
     "lpb_frames_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),

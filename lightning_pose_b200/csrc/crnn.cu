@@ -17,6 +17,7 @@
 
 #include "../../include/lpb200.h"
 #include "lpb_common.cuh"
+#include "reduce_partials.cuh"
 
 namespace lpb {
 
@@ -122,12 +123,18 @@ __global__ void __launch_bounds__(256) crnn_combine_fwd_kernel(const __grid_cons
   *reinterpret_cast<float2*>(dst + (size_t)(2 * by + 1) * P.W + 2 * bx) = make_float2(0.5f * (xf[2] + xb[2]), 0.5f * (xf[3] + xb[3]));
 }
 
-// backward: recompute the two chains, then walk them in reverse.  dWF / dWB are accumulated with atomics (a frame can sit
-// in several windows); dL / dh are reduced per warp first.
+// Backward: recompute the two chains, then walk them in reverse.
+// FIXED = false (lpb_crnn_combine_bwd): dWF / dWB are accumulated with atomics (a frame can sit in several windows); dL /
+//   dh are reduced per warp, then added with atomics.  The order of those adds is not fixed.
+// FIXED = true (lpb_crnn_combine_bwd_ws): dWF / dWB are left to crnn_dmaps_kernel; each CTA sums dL / dh over its warps
+//   in warp order and stores them as partial row m * gridDim.x + blockIdx.x of `part` ([dLf | dhf | dLb | dhb], 40 K
+//   floats a row; the CTA writes its keypoint's 40), which reduce_partials adds in row order.
+template <bool FIXED>
 __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_constant__ CrnnParams P, const float* __restrict__ g,
                                                                float* __restrict__ dWF, float* __restrict__ dWB,
                                                                float* __restrict__ dLf, float* __restrict__ dhf,
-                                                               float* __restrict__ dLb, float* __restrict__ dhb) {
+                                                               float* __restrict__ dLb, float* __restrict__ dhb, float* __restrict__ part) {
+  __shared__ float red[8][40];  // FIXED: [warp][dLf 16 | dhf 4 | dLb 16 | dhb 4]
   const int plane = blockIdx.y, m = plane / P.K, k = plane - m * P.K;
   const int Wb = P.W / 2, nblk = (P.H / 2) * Wb;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -168,11 +175,13 @@ __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_cons
       gg[0] = 0.5f * r0.x, gg[1] = 0.5f * r0.y, gg[2] = 0.5f * r1.x, gg[3] = 0.5f * r1.y;
 #pragma unroll
       for (int s = CRNN_CTX - 1; s >= 0; --s) {
-        float* dp = dWm + ((size_t)fr[dir ? CRNN_CTX - 1 - s : s] * P.K + k) * hw;
-        atomicAdd(dp + (size_t)(2 * by) * P.W + 2 * bx, gg[0]);
-        atomicAdd(dp + (size_t)(2 * by) * P.W + 2 * bx + 1, gg[1]);
-        atomicAdd(dp + (size_t)(2 * by + 1) * P.W + 2 * bx, gg[2]);
-        atomicAdd(dp + (size_t)(2 * by + 1) * P.W + 2 * bx + 1, gg[3]);
+        if constexpr (!FIXED) {
+          float* dp = dWm + ((size_t)fr[dir ? CRNN_CTX - 1 - s : s] * P.K + k) * hw;
+          atomicAdd(dp + (size_t)(2 * by) * P.W + 2 * bx, gg[0]);
+          atomicAdd(dp + (size_t)(2 * by) * P.W + 2 * bx + 1, gg[1]);
+          atomicAdd(dp + (size_t)(2 * by + 1) * P.W + 2 * bx, gg[2]);
+          atomicAdd(dp + (size_t)(2 * by + 1) * P.W + 2 * bx + 1, gg[3]);
+        }
         if (s == 0) break;
         float gn[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -188,19 +197,148 @@ __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_cons
         for (int i = 0; i < 4; ++i) gg[i] = gn[i];
       }
     }
-    float* dLg = (dir ? dLb : dLf) + k * 16;
-    float* dhg = (dir ? dhb : dhf) + k * 4;
+    if constexpr (FIXED) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float v = warp_sum(dL[i]);
-      if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dLg + i, v);
-    }
+      for (int i = 0; i < 20; ++i) {
+        const float v = warp_sum(i < 16 ? dL[i] : dh[i - 16]);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][20 * dir + i] = v;
+      }
+    } else {
+      float* dLg = (dir ? dLb : dLf) + k * 16;
+      float* dhg = (dir ? dhb : dhf) + k * 4;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float v = warp_sum(dh[i]);
-      if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dhg + i, v);
+      for (int i = 0; i < 16; ++i) {
+        const float v = warp_sum(dL[i]);
+        if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dLg + i, v);
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float v = warp_sum(dh[i]);
+        if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dhg + i, v);
+      }
     }
   }
+  if constexpr (FIXED) {
+    __syncthreads();
+    if (threadIdx.x < 40) {
+      const int i = threadIdx.x, dir = i / 20, j = i - 20 * dir;
+      float v = 0.f;
+      for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) v += red[wp][i];
+      // section offsets in a row: dLf 0, dhf 16 K, dLb 20 K, dhb 36 K
+      const size_t col = (size_t)20 * P.K * dir + (j < 16 ? (size_t)k * 16 + j : (size_t)16 * P.K + k * 4 + (j - 16));
+      part[((size_t)m * gridDim.x + blockIdx.x) * 40 * P.K + col] = v;
+    }
+  }
+}
+
+// The (window, slot) pairs that read each frame, in ascending window-then-slot order: pairs[start[f] .. start[f + 1]) holds
+// e = 5 m + s for every idx[m][s] == f.  One CTA: counts (integer atomics), exclusive scan, placement (integer atomics),
+// then each frame's list is sorted, so the result does not depend on the order of the placements.  Entries outside
+// [0, N) belong to no frame.
+__global__ void __launch_bounds__(1024) crnn_pairs_kernel(const int32_t* __restrict__ idx, int M, int N, int* __restrict__ start,
+                                                          int* __restrict__ cnt, int* __restrict__ pairs) {
+  __shared__ int wsum[32];
+  __shared__ int carry;
+  const int t = threadIdx.x, E = M * CRNN_CTX;
+  for (int f = t; f < N; f += blockDim.x) cnt[f] = 0;
+  if (t == 0) carry = 0, start[0] = 0;
+  __syncthreads();
+  for (int e = t; e < E; e += blockDim.x) {
+    const int f = __ldg(idx + e);
+    if ((unsigned)f < (unsigned)N) atomicAdd(cnt + f, 1);
+  }
+  __syncthreads();
+  for (int base = 0; base < N; base += blockDim.x) {  // start[f + 1] = sum of cnt[0 .. f]
+    const int f = base + t;
+    int v = f < N ? cnt[f] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, o);
+      if ((t & 31) >= o) v += u;
+    }
+    if ((t & 31) == 31) wsum[t >> 5] = v;
+    __syncthreads();
+    int pre = carry;
+    for (int wp = 0; wp < (t >> 5); ++wp) pre += wsum[wp];
+    if (f < N) start[f + 1] = pre + v;
+    __syncthreads();
+    if (t == blockDim.x - 1) carry = pre + v;
+    __syncthreads();
+  }
+  for (int f = t; f < N; f += blockDim.x) cnt[f] = 0;
+  __syncthreads();
+  for (int e = t; e < E; e += blockDim.x) {
+    const int f = __ldg(idx + e);
+    if ((unsigned)f < (unsigned)N) pairs[start[f] + atomicAdd(cnt + f, 1)] = e;
+  }
+  __syncthreads();
+  for (int f = t; f < N; f += blockDim.x) {
+    int* l = pairs + start[f];
+    const int n = start[f + 1] - start[f];
+    for (int i = 1; i < n; ++i) {
+      const int v = l[i];
+      int j = i - 1;
+      for (; j >= 0 && l[j] > v; --j) l[j + 1] = l[j];
+      l[j + 1] = v;
+    }
+  }
+}
+
+// dWF / dWB of lpb_crnn_combine_bwd_ws, one thread per 2x2 block of one (frame, keypoint) plane: the sum over the frame's
+// (window, slot) pairs, in pair order, of the slot's chain gradient.  That gradient needs no chain state: at chain step
+// q it is (L^T)^(4 - q) 0.5 g[m], computed here with the backward kernel's own fma sequence, so each term has the bits
+// of the term the atomic form adds.  Window slot s is chain step s forward and 4 - s backward.
+__global__ void __launch_bounds__(256) crnn_dmaps_kernel(const __grid_constant__ CrnnParams P, const float* __restrict__ g,
+                                                         const int* __restrict__ start, const int* __restrict__ pairs,
+                                                         float* __restrict__ dWF, float* __restrict__ dWB) {
+  const int Wb = P.W / 2, nblk = (P.H / 2) * Wb;
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)P.N * P.K * nblk) return;
+  const int64_t fk = t / nblk;
+  const int blk = (int)(t - fk * nblk), k = (int)(fk % P.K), f = (int)(fk / P.K);
+  const int by = blk / Wb, bx = blk - by * Wb;
+  const size_t hw = (size_t)P.H * P.W, o0 = (size_t)(2 * by) * P.W + 2 * bx, o1 = o0 + P.W;
+  const int p0 = __ldg(start + f), p1 = __ldg(start + f + 1);
+#pragma unroll
+  for (int dir = 0; dir < 2; ++dir) {
+    float L[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) L[i] = __ldg((dir ? P.Lb : P.Lf) + k * 16 + i);
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int p = p0; p < p1; ++p) {
+      const int e = __ldg(pairs + p), m = e / CRNN_CTX, s = e - m * CRNN_CTX;
+      const float* gp = g + ((size_t)m * P.K + k) * hw;
+      const float2 r0 = __ldg(reinterpret_cast<const float2*>(gp + o0)), r1 = __ldg(reinterpret_cast<const float2*>(gp + o1));
+      float gg[4] = {0.5f * r0.x, 0.5f * r0.y, 0.5f * r1.x, 0.5f * r1.y};
+      for (int q = CRNN_CTX - 1; q > (dir ? CRNN_CTX - 1 - s : s); --q) {
+        float gn[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int o = 0; o < 4; ++o)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) gn[i] = fmaf(L[o * 4 + i], gg[o], gn[i]);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) gg[i] = gn[i];
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[i] += gg[i];
+    }
+    float* dp = (dir ? dWB : dWF) + ((size_t)f * P.K + k) * hw;
+    *reinterpret_cast<float2*>(dp + o0) = make_float2(acc[0], acc[1]);
+    *reinterpret_cast<float2*>(dp + o1) = make_float2(acc[2], acc[3]);
+  }
+}
+
+// workspace of lpb_crnn_combine_bwd_ws: start [N + 1], cnt [N], pairs [5 M] (ints), then at a 16-byte boundary the
+// dL / dh partials [M * ceil(blocks / 256)][40 K] (floats)
+struct CrnnWs {
+  size_t ints, rows, bytes;
+};
+static CrnnWs crnn_ws(int M, int N, int K, int H, int W) {
+  CrnnWs w;
+  w.ints = (((size_t)2 * N + 1 + (size_t)CRNN_CTX * M) + 3) & ~(size_t)3;
+  w.rows = (size_t)M * (((size_t)(H / 2) * (W / 2) + 255) / 256);
+  w.bytes = w.ints * sizeof(int) + w.rows * 40 * (size_t)K * sizeof(float);
+  return w;
 }
 
 // get_context_from_sequence: out[i][s] = seq[clamp(i + s - ctx/2, 0, n - 1)]   (16-byte vectors)
@@ -306,7 +444,60 @@ extern "C" int lpb_crnn_combine_bwd(const float* WF, const float* WB, const int3
   CrnnParams p{WF, WB, idx, Lf, hf, Lb, hb, M, N, K, H, W};
   const int nblk = (H / 2) * (W / 2);
   dim3 grid((unsigned)((nblk + 255) / 256), (unsigned)(M * K));
-  crnn_combine_bwd_kernel<<<grid, 256, 0, s>>>(p, grad_logits, dWF, dWB, dLf, dhf, dLb, dhb);
+  crnn_combine_bwd_kernel<false><<<grid, 256, 0, s>>>(p, grad_logits, dWF, dWB, dLf, dhf, dLb, dhb, nullptr);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_crnn_combine_bwd_workspace_bytes(int M, int N, int K, int H, int W, size_t* bytes) {
+  using namespace lpb;
+  LPB_REQUIRE(bytes, "crnn_combine_bwd_workspace_bytes: null pointer");
+  LPB_REQUIRE(M >= 0 && N >= 1 && K >= 1 && H >= 2 && W >= 2 && H % 2 == 0 && W % 2 == 0 && (int64_t)M * K < 65536,
+              "crnn_combine_bwd_workspace_bytes: bad shape (even H, W; M * K < 65536 per call)");
+  *bytes = crnn_ws(M, N, K, H, W).bytes;
+  return LPB_OK;
+}
+
+extern "C" int lpb_crnn_combine_bwd_ws(const float* WF, const float* WB, const int32_t* idx, const float* grad_logits, int M, int N,
+                                       int K, int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb,
+                                       float* dWF, float* dWB, float* dLf, float* dhf, float* dLb, float* dhb, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  using namespace lpb;
+  if (int rc = crnn_check(WF, WB, idx, M, N, K, H, W)) return rc;
+  LPB_REQUIRE(grad_logits && Lf && hf && Lb && hb && dWF && dWB && dLf && dhf && dLb && dhb, "crnn_combine_bwd_ws: null pointer");
+  const CrnnWs ws = crnn_ws(M, N, K, H, W);
+  LPB_REQUIRE(workspace && aligned_to(workspace, 16), "crnn_combine_bwd_ws: null or unaligned workspace (16 bytes)");
+  LPB_REQUIRE(workspace_bytes >= ws.bytes, "crnn_combine_bwd_ws: workspace of %zu bytes, %zu needed", workspace_bytes, ws.bytes);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (M == 0) {
+    const size_t nmap = (size_t)N * K * H * W * sizeof(float);
+    LPB_CUDA(cudaMemsetAsync(dWF, 0, nmap, s));
+    LPB_CUDA(cudaMemsetAsync(dWB, 0, nmap, s));
+    LPB_CUDA(cudaMemsetAsync(dLf, 0, sizeof(float) * K * 16, s));
+    LPB_CUDA(cudaMemsetAsync(dLb, 0, sizeof(float) * K * 16, s));
+    LPB_CUDA(cudaMemsetAsync(dhf, 0, sizeof(float) * K * 4, s));
+    LPB_CUDA(cudaMemsetAsync(dhb, 0, sizeof(float) * K * 4, s));
+    return LPB_OK;
+  }
+  DeviceLimits dev;
+  LPB_TRY(device_limits(&dev));
+  int* start = static_cast<int*>(workspace);
+  int* cnt = start + N + 1;
+  int* pairs = cnt + N;
+  float* part = reinterpret_cast<float*>(start + ws.ints);
+  CrnnParams p{WF, WB, idx, Lf, hf, Lb, hb, M, N, K, H, W};
+  const int nblk = (H / 2) * (W / 2);
+  crnn_pairs_kernel<<<1, 1024, 0, s>>>(idx, M, N, start, cnt, pairs);
+  const dim3 grid((unsigned)((nblk + 255) / 256), (unsigned)(M * K));
+  crnn_combine_bwd_kernel<true><<<grid, 256, 0, s>>>(p, grad_logits, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, part);
+  const int64_t nthreads = (int64_t)N * K * nblk;
+  crnn_dmaps_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, s>>>(p, grad_logits, start, pairs, dWF, dWB);
+  const size_t stride = (size_t)40 * K;
+  const int rows = (int)ws.rows;
+  reduce_partials<1>(part, rows, stride, 16 * K, dLf, dev.sms, s);
+  reduce_partials<1>(part + (size_t)16 * K, rows, stride, 4 * K, dhf, dev.sms, s);
+  reduce_partials<1>(part + (size_t)20 * K, rows, stride, 16 * K, dLb, dev.sms, s);
+  reduce_partials<1>(part + (size_t)36 * K, rows, stride, 4 * K, dhb, dev.sms, s);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

@@ -745,7 +745,7 @@ struct ScatterPlan {
   }
 };
 
-template <int DS, bool ATOMIC>
+template <int DS>
 __device__ __forceinline__ void scatter_row(float* grow0, float gv, const ScatterPlan<DS>& sp, float* srow, int lane, int maxcols) {
   srow[lane] = gv;
   __syncwarp();
@@ -761,16 +761,13 @@ __device__ __forceinline__ void scatter_row(float* grow0, float gv, const Scatte
   unpack2(acc2, lo, hi);
   float acc = lo + hi;
   if (ScatterPlan<DS>::SPLIT == 2) acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-  if (sp.writer && sp.oc < maxcols && acc != 0.f) {
-    if (ATOMIC) atomicAdd(grow0 + sp.oc, acc);
-    else grow0[sp.oc] += acc;
-  }
+  if (sp.writer && sp.oc < maxcols && acc != 0.f) grow0[sp.oc] += acc;
 }
 
 // One strip (32 fine columns starting at fine column jf0, a multiple of F) over coarse rows [r0, r1): evaluates the
 // softmax weights of the fine field and accumulates U_H^T G U_W into gt.  `tile` / `gt` are addressed as
 // row * pitch + column with (trow0, tcol0) the tile coordinates of coarse row r0 - R and of coarse column jf0/F - R.
-template <int DS, bool ATOMIC>
+template <int DS>
 __device__ __forceinline__ void decode_bwd_strip(const DecodeGeom<DS>& P, const float* tile, float* gt, int pitch,
                                                  int trow0, int tcol0, int maxcols, int jf0, int J1, int r0, int r1, float M,
                                                  float c, float kscale, float xhat, float yhat, float gx, float gy, int lane,
@@ -839,7 +836,7 @@ __device__ __forceinline__ void decode_bwd_strip(const DecodeGeom<DS>& P, const 
       // coarse row r0 + la - R is complete for this lane's column
       float lo, hi;
       unpack2(gacc[rot], lo, hi);
-      scatter_row<DS, ATOMIC>(gt + (trow0 + la) * pitch + tcol0, lo + hi, sp, srow + 32 * (la & 1), lane, maxcols);
+      scatter_row<DS>(gt + (trow0 + la) * pitch + tcol0, lo + hi, sp, srow + 32 * (la & 1), lane, maxcols);
       gacc[rot] = pack2(0.f, 0.f);
       tmp[rot] = (la + 1 < nrows) ? dot_w<W>(colbase + (trow0 + la + 1 + 2 * R) * pitch, wc) : 0.f;
     });
@@ -847,9 +844,12 @@ __device__ __forceinline__ void decode_bwd_strip(const DecodeGeom<DS>& P, const 
 }
 
 // Dense form: one CTA per plane (grid = n_planes), or -- queue mode -- per (plane, row segment) unit of the planes
-// the window kernel could not take; a unit adds its rows into the plane's pre-zeroed gradient with global atomics.
-// Those adds, and the shared-memory adds of overlapping strips (scatter_row<DS, true>), meet in no fixed order, so this
-// gradient (and the windows' overflow planes, which it writes) can differ in the last bits from call to call.
+// the window kernel could not take.  Every gradient element is a sum in a fixed order, with no atomics, so this gradient
+// (and the windows' overflow planes, which it writes) has the same bits from call to call:
+//   * inside a CTA, the work items (32-column strip, row group) run in phases of a barrier each, and the items of one
+//     phase touch disjoint gradient elements; so each element receives its items' adds in phase order;
+//   * a queue-mode segment owns a band of gradient rows, evaluates the R coarse rows either side of the band as well
+//     (the rows whose taps reach it), and stores only its band: one writer per element, no scratch.
 constexpr int DEC_BWD_SEGS = 8;
 
 template <int DS>
@@ -871,9 +871,8 @@ __global__ void __launch_bounds__(DEC_THREADS) decode_bwd_kernel(const __grid_co
     __syncthreads();
   }
   uint32_t phase = 0;
-  // queue mode: a few left-over planes are split into row segments so that every resident CTA has work (their partial
-  // rows meet through global atomics in the gradient the window kernel cleared); when the queue alone fills the grid
-  // (flat heatmaps of a freshly initialised network: every plane is dense) a unit is a whole plane and stores plainly
+  // queue mode: a few left-over planes are split into row segments so that every resident CTA has work; when the queue
+  // alone fills the grid (flat heatmaps of a freshly initialised network: every plane is dense) a unit is a whole plane
   const int nseg = P.queue ? max(1, min(DEC_BWD_SEGS, (int)gridDim.x / max(P.queue[0], 1))) : 1;
   const long long nunits = P.queue ? (long long)P.queue[0] * nseg : P.n_planes;
   for (long long unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
@@ -883,12 +882,15 @@ __global__ void __launch_bounds__(DEC_THREADS) decode_bwd_kernel(const __grid_co
     const int A0 = (int)st[4], A1 = (int)st[5], B0 = (int)st[6], B1 = (int)st[7];
     const float gx = P.gxy[2 * plane], gy = P.gxy[2 * plane + 1];
     const int nrows = A1 - A0 + 1;
-    int useg0 = A0, useg1 = A1 + 1;  // coarse rows this unit evaluates
-    if (nseg > 1) {
-      const int sg = (nrows + nseg - 1) / nseg;
-      useg0 = A0 + (int)(unit % nseg) * sg;
-      useg1 = min(useg0 + sg, A1 + 1);
-      if (useg0 >= useg1) continue;  // uniform per CTA
+    int own0 = 0, own1 = h;          // gradient rows this unit stores
+    int useg0 = A0, useg1 = A1 + 1;  // coarse rows it evaluates
+    if (nseg > 1) {  // segment k owns the rows from the start of its share of [A0, A1] to the next share's start
+      const int sg = (nrows + nseg - 1) / nseg, k = (int)(unit % nseg);
+      if (k * sg >= nrows) continue;  // uniform per CTA; an empty share owns no rows (nor does a plane with none)
+      own0 = k == 0 ? 0 : A0 + k * sg;
+      own1 = (k + 1) * sg >= nrows ? h : A0 + (k + 1) * sg;
+      useg0 = max(A0, own0 - R);
+      useg1 = min(A1 + 1, own1 + R);
     }
     const float* __restrict__ src = P.heat + plane * (size_t)h * w;
     if (P.bulk) {
@@ -925,44 +927,50 @@ __global__ void __launch_bounds__(DEC_THREADS) decode_bwd_kernel(const __grid_co
       const int J0 = B0 * F, J1 = (B1 + 1) * F;
       const int nstrips = (J1 - J0 + 31) >> 5;
       const int urows = useg1 - useg0;
-      int G = 1, seg = urows;  // split the rows further so that all warps have an item
+      // Items (strip, row group): a strip adds into 32/F + 2R coarse columns, 32/F apart, so strips NCS apart are
+      // disjoint; a group of sg rows adds into sg + 2R rows, so groups ncg apart are.  Phase (cs, cg) runs the strips
+      // cs (mod NCS) of the groups cg (mod ncg), and a barrier ends it.  The rows are split into G groups so that all
+      // warps have items, at the least cost over the phases.
+      constexpr int NG = 32 / F, NCS = (NG + 2 * R + NG - 1) / NG;
+      auto ncolours = [&](int g, int sg) { return min(g, 1 + (2 * R + sg - 1) / sg); };
+      auto phase_items = [&](int n, int nc, int c) { return (n - c + nc - 1) / nc; };
+      int G = 1, seg = urows, ncg = 1;
       {
         int bestcost = 0x7fffffff;
         for (int g = 1; g <= 8; ++g) {
-          const int sg = (urows + g - 1) / g;
-          const int cost = ((nstrips * g + DEC_WARPS - 1) / DEC_WARPS) * (sg + 2 * R);
+          const int sg = (urows + g - 1) / g, nc = ncolours(g, sg);
+          int rounds = 0;
+          for (int cs = 0; cs < NCS; ++cs)
+            for (int cg = 0; cg < nc; ++cg) rounds += (phase_items(nstrips, NCS, cs) * phase_items(g, nc, cg) + DEC_WARPS - 1) / DEC_WARPS;
+          const int cost = rounds * (sg + 2 * R);
           if (cost < bestcost) {
             bestcost = cost;
             G = g;
             seg = sg;
+            ncg = nc;
           }
         }
       }
-      const int nitems = nstrips * G;
-      for (int item = warp; item < nitems; item += DEC_WARPS) {
-        const int sidx = item % nstrips, g = item / nstrips;
-        const int r0 = useg0 + g * seg, r1 = min(r0 + seg, useg1);
-        if (r0 >= r1) continue;
-        const int jf0 = J0 + sidx * 32;
-        const int tcol0 = padl + (jf0 / F - R);
-        decode_bwd_strip<DS, true>(P, tile, gtile, pitch, r0, tcol0, pitch - tcol0, jf0, J1, r0, r1, M, c, kscale, xhat, yhat, gx, gy,
-                                   lane, srows + warp * 64);
-      }
+      for (int cs = 0; cs < NCS; ++cs)
+        for (int cg = 0; cg < ncg; ++cg) {
+          const int ns = phase_items(nstrips, NCS, cs), nitems = ns * phase_items(G, ncg, cg);
+          for (int item = warp; item < nitems; item += DEC_WARPS) {
+            const int sidx = cs + NCS * (item % ns), g = cg + ncg * (item / ns);
+            const int r0 = useg0 + g * seg, r1 = min(r0 + seg, useg1);
+            if (r0 >= r1) continue;
+            const int jf0 = J0 + sidx * 32;
+            const int tcol0 = padl + (jf0 / F - R);
+            decode_bwd_strip<DS>(P, tile, gtile, pitch, r0, tcol0, pitch - tcol0, jf0, J1, r0, r1, M, c, kscale, xhat, yhat, gx, gy, lane,
+                                 srows + warp * 64);
+          }
+          __syncthreads();
+        }
     }
     __syncthreads();
     float* __restrict__ dst = P.gheat + plane * (size_t)h * w;
-    if (nseg > 1) {  // rows this unit touched: [useg0 - R, useg1 + R)
-      const int a0 = max(useg0 - R, 0), a1 = min(useg1 + R, h);
-      for (int a = a0 + warp; a < a1; a += DEC_WARPS) {
-        const float* row = gtile + (a + R) * pitch + padl;
-        for (int b = lane; b < w; b += 32)
-          if (row[b] != 0.f) atomicAdd(dst + (size_t)a * w + b, row[b]);
-      }
-    } else {
-      for (int a = warp; a < h; a += DEC_WARPS) {
-        const float* row = gtile + (a + R) * pitch + padl;
-        for (int b = lane; b < w; b += 32) dst[(size_t)a * w + b] = row[b];
-      }
+    for (int a = own0 + warp; a < own1; a += DEC_WARPS) {
+      const float* row = gtile + (a + R) * pitch + padl;
+      for (int b = lane; b < w; b += 32) dst[(size_t)a * w + b] = row[b];
     }
     __syncthreads();  // tile / gtile are reused by the next unit
   }
@@ -1053,7 +1061,7 @@ __global__ void __launch_bounds__(128) decode_bwd_window_kernel(const __grid_con
   for (int sidx = 0; sidx < nstrips; ++sidx) {
     const int jf0 = J0 + sidx * 32;
     const int tcol0 = jf0 / F - B0;  // window column of coarse column jf0/F - R
-    decode_bwd_strip<DS, false>(P, tile, gt, DEC_WP, ra0 - A0, tcol0, DEC_WIN - tcol0, jf0, J1, ra0, ra1 + 1, M, c, kscale, xhat, yhat, gx,
+    decode_bwd_strip<DS>(P, tile, gt, DEC_WP, ra0 - A0, tcol0, DEC_WIN - tcol0, jf0, J1, ra0, ra1 + 1, M, c, kscale, xhat, yhat, gx,
                                 gy, lane, srow_s[warp]);
     __syncwarp();
   }

@@ -16,6 +16,7 @@
 #include "../../include/lpb200.h"
 #include "lpb_common.cuh"
 #include "mma_sm90.cuh"
+#include "reduce_partials.cuh"
 
 namespace lpb {
 
@@ -435,16 +436,20 @@ __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_dgrad_kernel(const floa
 }
 
 // Weight gradient: M = Cin (32 WM per CTA), N = Cout x 9 (n = o * 9 + tap, 8 NT WN per CTA), K = pixels.  K is split
-// over gridDim.y CTAs, each looping over its share of the (frame, pixel block) units with the tile in registers; the
-// tile is added into grad_w with one float atomic per element.  A = the input [c][slot] (row stride 132 = 4 mod 32:
-// the (g, t) pattern on 32 banks), B = the staged gradient planes of the CTA's output channels.  The CTAs of the
-// first channel tile also sum the bias gradient (the four taps (1..2, 1..2)) of their channels.
+// over gridDim.y CTAs ("slots"), each looping over its share of the (frame, pixel block) units with the tile in
+// registers.  A = the input [c][slot] (row stride 132 = 4 mod 32: the (g, t) pattern on 32 banks), B = the staged
+// gradient planes of the CTA's output channels.  The CTAs of the first channel tile also sum the bias gradient (the four
+// taps (1..2, 1..2)) of their channels: warp w takes channels w, w + warps, ...; its lanes sum the unit's pixels and
+// the warp's shuffle sum is added to the channel's running total, so that sum has a fixed order too.
+// PART: the tile and bias sums are stored into the slot's partial, dw / db + blockIdx.y * slot_stride, one writer per
+// element, and reduce_partials adds the slots in slot order (bit-reproducible).  Otherwise they are added into grad_w /
+// grad_b with float atomics (lpb_convt_bwd_f32: the order of the slots' adds is not fixed).
 constexpr int WG_PS = TC_SLOTS + 4;
 
-template <int SHUFFLE, int WM, int WN, int NT>
+template <int SHUFFLE, int WM, int WN, int NT, bool PART>
 __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const float* __restrict__ in, const float* __restrict__ g,
                                                                         int B, int Cin, int Cout, int Hi, int Wi, int RB, int CB,
-                                                                        float* __restrict__ dw, float* __restrict__ db) {
+                                                                        float* __restrict__ dw, float* __restrict__ db, size_t slot_stride) {
   constexpr int CM = 32 * WM, CN = 8 * NT * WN, THREADS = 32 * WM * WN;
   extern __shared__ __align__(16) float sm[];
   const int GC = 2 * CB + 1, GP = pad8_32((2 * RB + 1) * GC);
@@ -457,6 +462,10 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g8 = lane >> 2, t = lane & 3;
   const int wm = warp % WM, wn = warp / WM;
   const bool do_bias = db != nullptr && ct == 0;
+  if constexpr (PART) {
+    dw += blockIdx.y * slot_stride;
+    if (db) db += blockIdx.y * slot_stride;
+  }
 
   for (int i = threadIdx.x; i < CM * WG_PS; i += THREADS) xs[i] = 0.f;  // slots past RB * CB stay zero
   for (int p = threadIdx.x; p < TC_SLOTS; p += THREADS) pbt[p] = p < RB * CB ? 2 * (p / CB) * GC + p % CB : 0;
@@ -496,11 +505,16 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
     __syncthreads();
     if (do_bias) {
       const int hw = RB * CB;
-      for (int i = threadIdx.x; i < np * hw; i += THREADS) {
-        const int ol = i / hw, p = i - ol * hw, pr = p / CB, pc = p - pr * CB;
-        if (r0 + pr >= Hi || q0 + pc >= Wi) continue;
-        const float* gp = gs + ol * GP + pbt[p];
-        atomicAdd(dbs + ol, (gp[GC + CB + 1] + gp[GC + 1]) + (gp[2 * GC + CB + 1] + gp[2 * GC + 1]));  // taps 4, 5, 7, 8
+      for (int ol = warp; ol < np; ol += WM * WN) {
+        float sb = 0.f;
+        for (int p = lane; p < hw; p += 32) {
+          const int pr = p / CB, pc = p - pr * CB;
+          if (r0 + pr >= Hi || q0 + pc >= Wi) continue;
+          const float* gp = gs + ol * GP + pbt[p];
+          sb += (gp[GC + CB + 1] + gp[GC + 1]) + (gp[2 * GC + CB + 1] + gp[2 * GC + 1]);  // taps 4, 5, 7, 8
+        }
+        sb = warp_sum(sb);
+        if (lane == 0) dbs[ol] += sb;  // only this warp touches dbs[ol]; the units follow one another
       }
     }
 #pragma unroll 4
@@ -537,44 +551,72 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
           const int n = n0 + 8 * (NT * wn + nt) + 2 * t + j;
-          if (n < nk) atomicAdd(dw + (size_t)c * nk + n, acc[mt][nt][2 * h + j]);
+          if (n >= nk) continue;
+          if constexpr (PART) dw[(size_t)c * nk + n] = acc[mt][nt][2 * h + j];
+          else atomicAdd(dw + (size_t)c * nk + n, acc[mt][nt][2 * h + j]);
         }
     }
   if (do_bias) {
     __syncthreads();
     for (int ol = threadIdx.x; ol < np; ol += THREADS) {
       const int o = o_lo + ol;
-      if (o * 9 >= n0) atomicAdd(db + o, dbs[ol]);  // channel o belongs to the n tile that holds its tap 0
+      if (o * 9 < n0) continue;  // channel o belongs to the n tile that holds its tap 0
+      if constexpr (PART) db[o] = dbs[ol];
+      else atomicAdd(db + o, dbs[ol]);
     }
   }
 }
 
+// K split of the weight gradient: about `ctas` CTAs in all, each with as many units as that leaves (one tile row of
+// partials or atomics per CTA).  The reproducible form caps `ctas` at F32_WG_MAX_CTAS, which bounds its workspace
+// without a device query; on an H100 SXM (132 SMs) both forms split alike.
+constexpr int F32_WG_MAX_CTAS = 264;
+constexpr int F32_WG_CN = 160;  // N tile of both tilings below: 8 NT WN
+static long long wgrad_f32_slots(int B, int Cin, int Cout, int Hi, int Wi, int ctas) {
+  const int CM = Cin > 32 ? 128 : 32;
+  const PixBlocks pb = pix_blocks(Hi, Wi);
+  const long long tiles = (long long)((Cin + CM - 1) / CM) * ((Cout * 9 + F32_WG_CN - 1) / F32_WG_CN);
+  const long long units = (long long)B * pb.n;
+  return std::min<long long>(units, std::max<long long>(1, (ctas + tiles - 1) / tiles));
+}
+// one slot of the partials: its grad_w tile sums [Cin * Cout * 9], then its bias sums [Cout]
+static size_t wgrad_f32_part_stride(int Cin, int Cout) { return (size_t)Cin * Cout * 9 + Cout; }
+
 template <int SHUFFLE, int WM, int WN, int NT>
-static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cout, int Hi, int Wi, float* dw, float* db, cudaStream_t s) {
+static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cout, int Hi, int Wi, float* dw, float* db, float* part,
+                        cudaStream_t s) {
   constexpr int CM = 32 * WM, CN = 8 * NT * WN;
+  static_assert(CN == F32_WG_CN && (CM == 128) == (WM == 4), "wgrad_f32_slots assumes this tiling");
   const PixBlocks pb = pix_blocks(Hi, Wi);
   const int nct = (Cin + CM - 1) / CM, nnt = (Cout * 9 + CN - 1) / CN;
   const int np_max = CN / 9 + 2;
   const size_t smem =
       ((size_t)CM * WG_PS + (size_t)np_max * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1)) + TC_SLOTS + np_max) * sizeof(float);
-  LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT>, smem, "convt_bwd_f32"));
-  // K split: about two CTAs per SM in all, each with as many units as that leaves (fewer atomics than one per unit)
   DeviceLimits dev;
   LPB_TRY(device_limits(&dev));
-  const long long units = (long long)B * pb.n;
-  const long long ks = std::min<long long>(units, std::max<long long>(1, (2LL * dev.sms + nct * nnt - 1) / (nct * nnt)));
+  const long long ks = wgrad_f32_slots(B, Cin, Cout, Hi, Wi, part ? std::min(2 * dev.sms, F32_WG_MAX_CTAS) : 2 * dev.sms);
   const dim3 grid((unsigned)(nct * nnt), (unsigned)ks);
-  convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, dw, db);
+  if (part) {
+    const size_t stride = wgrad_f32_part_stride(Cin, Cout), nw = (size_t)Cin * Cout * 9;
+    LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, true>, smem, "convt_bwd_f32"));
+    convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, true><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, part,
+                                                                                        db ? part + nw : nullptr, stride);
+    reduce_partials<1>(part, (int)ks, stride, (int)nw, dw, dev.sms, s);
+    if (db) reduce_partials<1>(part + nw, (int)ks, stride, Cout, db, dev.sms, s);
+  } else {
+    LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, false>, smem, "convt_bwd_f32"));
+    convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, false><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, dw, db, 0);
+  }
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
 
 template <int SHUFFLE>
 static int launch_bwd(const float* in, const float* g, int B, int Cin, int Hi, int Wi, const float* wt, int Cout, float* din, float* dw,
-                      float* db, cudaStream_t s) {
+                      float* db, float* part, cudaStream_t s) {
   // M tile: 128 input channels, or 32 for narrow inputs (a second layer's Cin is the first layer's keypoint count)
-  const int rc = Cin > 32 ? launch_wgrad<SHUFFLE, 4, 2, 10>(in, g, B, Cin, Cout, Hi, Wi, dw, db, s)
-                          : launch_wgrad<SHUFFLE, 1, 4, 5>(in, g, B, Cin, Cout, Hi, Wi, dw, db, s);
+  const int rc = Cin > 32 ? launch_wgrad<SHUFFLE, 4, 2, 10>(in, g, B, Cin, Cout, Hi, Wi, dw, db, part, s)
+                          : launch_wgrad<SHUFFLE, 1, 4, 5>(in, g, B, Cin, Cout, Hi, Wi, dw, db, part, s);
   if (rc || !din) return rc;
   const PixBlocks pb = pix_blocks(Hi, Wi);
   const size_t gfl = (size_t)8 * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1));
@@ -592,6 +634,19 @@ static int launch_bwd(const float* in, const float* g, int B, int Cin, int Hi, i
   if (Cin <= 24) return go(convt3x3s2_dgrad_kernel<SHUFFLE, 3>, 3, bstride<3>());
   if (Cin <= 32) return go(convt3x3s2_dgrad_kernel<SHUFFLE, 4>, 4, bstride<4>());
   return go(convt3x3s2_dgrad_kernel<SHUFFLE, 8>, 8, bstride<8>());
+}
+
+// part == NULL: lpb_convt_bwd_f32 (atomics); otherwise the workspace of lpb_convt_bwd_f32_ws
+static int convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w, int Cout,
+                         float* grad_in, float* grad_w, float* grad_bias, float* part, cudaStream_t s) {
+  if (!part || B == 0) {  // the partials' sums overwrite grad_w and grad_bias
+    LPB_CUDA(cudaMemsetAsync(grad_w, 0, sizeof(float) * (size_t)Cin * Cout * 9, s));
+    if (grad_bias) LPB_CUDA(cudaMemsetAsync(grad_bias, 0, sizeof(float) * Cout, s));
+  }
+  if (B == 0) return LPB_OK;
+  if (shuffle == LPB_SHUFFLE_NHWC) return launch_bwd<LPB_SHUFFLE_NHWC>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, part, s);
+  return shuffle ? launch_bwd<LPB_SHUFFLE_NCHW>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, part, s)
+                 : launch_bwd<LPB_SHUFFLE_NONE>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, part, s);
 }
 
 }  // namespace lpb
@@ -619,13 +674,30 @@ extern "C" int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, 
   LPB_REQUIRE(in && grad_out && w && grad_w, "convt_bwd_f32: null pointer");
   LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Hi >= 1 && Wi >= 1 && (!shuffle || (Hi % 2 == 0 && Wi % 2 == 0)),
               "convt_bwd_f32: bad shape");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  LPB_CUDA(cudaMemsetAsync(grad_w, 0, sizeof(float) * (size_t)Cin * Cout * 9, s));
-  if (grad_bias) LPB_CUDA(cudaMemsetAsync(grad_bias, 0, sizeof(float) * Cout, s));
-  if (B == 0) return LPB_OK;
-  if (shuffle == LPB_SHUFFLE_NHWC) return launch_bwd<LPB_SHUFFLE_NHWC>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s);
-  return shuffle ? launch_bwd<LPB_SHUFFLE_NCHW>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s)
-                 : launch_bwd<LPB_SHUFFLE_NONE>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, s);
+  return convt_bwd_f32(in, grad_out, B, Cin, Hi, Wi, shuffle, w, Cout, grad_in, grad_w, grad_bias, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int lpb_convt_bwd_f32_workspace_bytes(int B, int Cin, int Hi, int Wi, int Cout, size_t* bytes) {
+  using namespace lpb;
+  LPB_REQUIRE(bytes, "convt_bwd_f32_workspace_bytes: null pointer");
+  LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Hi >= 1 && Wi >= 1, "convt_bwd_f32_workspace_bytes: bad shape");
+  *bytes = B == 0 ? 0 : (size_t)wgrad_f32_slots(B, Cin, Cout, Hi, Wi, F32_WG_MAX_CTAS) * wgrad_f32_part_stride(Cin, Cout) * sizeof(float);
+  return LPB_OK;
+}
+
+extern "C" int lpb_convt_bwd_f32_ws(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
+                                    int Cout, float* grad_in, float* grad_w, float* grad_bias, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(in && grad_out && w && grad_w, "convt_bwd_f32_ws: null pointer");
+  LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Hi >= 1 && Wi >= 1 && (!shuffle || (Hi % 2 == 0 && Wi % 2 == 0)),
+              "convt_bwd_f32_ws: bad shape");
+  size_t need = 0;
+  LPB_TRY(lpb_convt_bwd_f32_workspace_bytes(B, Cin, Hi, Wi, Cout, &need));
+  LPB_REQUIRE(B == 0 || (workspace && aligned_to(workspace, 4)), "convt_bwd_f32_ws: null or unaligned workspace");
+  LPB_REQUIRE(workspace_bytes >= need, "convt_bwd_f32_ws: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  return convt_bwd_f32(in, grad_out, B, Cin, Hi, Wi, shuffle, w, Cout, grad_in, grad_w, grad_bias, static_cast<float*>(workspace),
+                       static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int lpb_head_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {

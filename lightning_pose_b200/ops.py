@@ -374,7 +374,8 @@ def convt_forward_f32(x, weight, bias, shuffle: bool):
 
 
 def convt_backward_f32(x, grad_out, weight, shuffle: bool, need_dx: bool = True, need_db: bool = True):
-    """Autograd of ``convt_forward_f32``: (dx | None, dw, db | None); ``dx`` has the memory format of ``x``."""
+    """Autograd of ``convt_forward_f32``: (dx | None, dw, db | None); ``dx`` has the memory format of ``x``.  ``dw`` and
+    ``db`` are fixed-order sums (the same bits from run to run on one device model)."""
     x, mode = _f32_conv_input(x, shuffle)
     g = _cuda_f32(grad_out, "grad_out")
     wt = _cuda_f32(weight, "weight")
@@ -383,8 +384,12 @@ def convt_backward_f32(x, grad_out, weight, shuffle: bool, need_dx: bool = True,
     dx = torch.empty_like(x) if need_dx else None
     dw = torch.empty_like(wt)
     db = torch.empty((wt.shape[1],), device=x.device, dtype=torch.float32) if need_db else None
+    nbytes = C.c_size_t(0)
+    check(lib.lpb_convt_bwd_f32_workspace_bytes(b, cin, hi, wi, wt.shape[1], C.byref(nbytes)))
+    ws = torch.empty((nbytes.value,), device=x.device, dtype=torch.uint8)
     with torch.cuda.device(x.device):
-        check(lib.lpb_convt_bwd_f32(_ptr(x), _ptr(g), b, cin, hi, wi, mode, _ptr(wt), wt.shape[1], _ptr(dx), _ptr(dw), _ptr(db), _stream()))
+        check(lib.lpb_convt_bwd_f32_ws(_ptr(x), _ptr(g), b, cin, hi, wi, mode, _ptr(wt), wt.shape[1], _ptr(dx), _ptr(dw), _ptr(db), _ptr(ws),
+                                       nbytes.value, _stream()))
     return dx, dw, db
 
 
@@ -511,9 +516,12 @@ class _CrnnCombine(torch.autograd.Function):
         dwf, dwb = torch.empty_like(wf), torch.empty_like(wb)
         dLf, dhf, dLb, dhb = torch.empty_like(Lf), torch.empty_like(hf), torch.empty_like(Lb), torch.empty_like(hb)
         outs = [torch.empty_like(t) for t in (cwf, cbf, twf)] + [torch.empty((k,), device=dev)] + [torch.empty_like(t) for t in (cwb, cbb, twb)] + [torch.empty((k,), device=dev)]
+        nbytes = C.c_size_t(0)
+        check(lib.lpb_crnn_combine_bwd_workspace_bytes(m, n, k, h, w, C.byref(nbytes)))
+        ws = torch.empty((nbytes.value,), device=dev, dtype=torch.uint8)
         with torch.cuda.device(dev):
-            check(lib.lpb_crnn_combine_bwd(_ptr(wf), _ptr(wb), _ptr(idx), _ptr(g), m, n, k, h, w, _ptr(Lf), _ptr(hf), _ptr(Lb), _ptr(hb),
-                                           _ptr(dwf), _ptr(dwb), _ptr(dLf), _ptr(dhf), _ptr(dLb), _ptr(dhb), _stream()))
+            check(lib.lpb_crnn_combine_bwd_ws(_ptr(wf), _ptr(wb), _ptr(idx), _ptr(g), m, n, k, h, w, _ptr(Lf), _ptr(hf), _ptr(Lb), _ptr(hb),
+                                              _ptr(dwf), _ptr(dwb), _ptr(dLf), _ptr(dhf), _ptr(dLb), _ptr(dhb), _ptr(ws), nbytes.value, _stream()))
             check(lib.lpb_crnn_prepare_bwd(_ptr(cwf), _ptr(cbf), _ptr(twf), _ptr(dLf), _ptr(dhf), k, f, _ptr(outs[0]), _ptr(outs[1]), _ptr(outs[2]), _ptr(outs[3]), _stream()))
             check(lib.lpb_crnn_prepare_bwd(_ptr(cwb), _ptr(cbb), _ptr(twb), _ptr(dLb), _ptr(dhb), k, f, _ptr(outs[4]), _ptr(outs[5]), _ptr(outs[6]), _ptr(outs[7]), _stream()))
         return (dwf, dwb, None, *outs)
