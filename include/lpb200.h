@@ -63,6 +63,16 @@ int lpb_decode_prepare(int h, int w, int ds);
 int lpb_decode_fwd_workspace_bytes(int64_t n_planes, size_t* bytes);
 int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
                    float* xy, float* conf, float* stats, void* workspace, void* stream);
+/* lpb_decode_fwd on heatmaps whose per-band maxima the head's softmax wrote (lpb_head_fwd_bf16_band_max): the same
+ * outputs, bit for bit, from fewer bytes.  band_max [n_planes][nbands][8] uint32, 4-byte aligned: the bits of the
+ * largest value in each band's rows, in 8 slots whose maximum is the band's; heatmap rows [2 b band_rows,
+ * 2 (b + 1) band_rows) form band b (lpb_head_band_max_dims).  Every value of a plane must be >= 0 or NaN, and the
+ * largest of a band's slots must be the largest non-NaN value of its rows (the softmax writes exactly that).  Refused: nbands < 0, a
+ * null or misaligned band_max with nbands > 0, an odd h, and band counts that do not cut h / 2 rows into bands of
+ * band_rows.  nbands = 0 is lpb_decode_fwd. */
+int lpb_decode_fwd_banded(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
+                          const uint32_t* band_max, int band_rows, int nbands, float* xy, float* conf, float* stats,
+                          void* workspace, void* stream);
 /* d loss / d heatmaps given d loss / d xy (confidence carries no gradient: it only feeds `<`
  * comparisons, lightning_pose/losses/losses.py:636). grad_heatmaps [n_planes,h,w] is overwritten. */
 int lpb_decode_bwd(const float* heatmaps, const float* stats, const float* grad_xy, int64_t n_planes,
@@ -241,6 +251,19 @@ int lpb_head_fwd_bf16_layout(const void* features, int B, int C, int H, int W, c
 int lpb_head_fwd_f16_layout(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
                             const float* w2, const float* b2, int c2, int final_softmax, int feature_layout, float* out,
                             void* saved_xs, void* workspace, void* stream);
+/* The forwards above with final_softmax = 1 that also write the per-band maxima of the heatmaps for
+ * lpb_decode_fwd_banded: band_max [B][c_out][nbands][8] uint32 (4-byte aligned, REQUIRED), for an h x w heatmap
+ * (h = 8 H, w = 8 W for two deconvs, 4 H / 4 W for one) band_rows and nbands from lpb_head_band_max_dims(h, w).
+ * Slot [b][k][j][e] holds the bits of the largest value the softmax's epilogue warp e stored in rows
+ * [2 j band_rows, 2 (j + 1) band_rows) of plane k (0 where it stored none).  The heatmaps are those of the plain
+ * entries, bit for bit. */
+int lpb_head_band_max_dims(int h, int w, int* band_rows, int* nbands);
+int lpb_head_fwd_bf16_band_max(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                               const float* w2, const float* b2, int c2, int feature_layout, float* out,
+                               uint32_t* band_max, void* saved_xs, void* workspace, void* stream);
+int lpb_head_fwd_f16_band_max(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                              const float* w2, const float* b2, int c2, int feature_layout, float* out,
+                              uint32_t* band_max, void* saved_xs, void* workspace, void* stream);
 int lpb_head_bwd_bf16_workspace_bytes_layout(int B, int C, int H, int W, int c1, int c2, int feature_layout, size_t* bytes);
 int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, const float* win, const int32_t* win_meta,
                              const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H,

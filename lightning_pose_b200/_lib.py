@@ -55,6 +55,7 @@ SIGNATURES = {
     "lpb_decode_prepare": (C.c_int, [_I, _I, _I]),
     "lpb_decode_fwd_workspace_bytes": (C.c_int, [_L, C.POINTER(_Z)]),
     "lpb_decode_fwd": (C.c_int, [_P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
+    "lpb_decode_fwd_banded": (C.c_int, [_P, _L, _I, _I, _I, _F, _P, _I, _I, _P, _P, _P, _P, _P]),
     "lpb_decode_bwd": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _F, _P, _P]),
     "lpb_decode_bwd_windows": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
     "lpb_upsample2x": (C.c_int, [_P, _L, _I, _I, _P, _P]),
@@ -79,6 +80,9 @@ SIGNATURES = {
     "lpb_head_bf16_plan_layout": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_I)]),
     "lpb_head_fwd_bf16_layout": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
     "lpb_head_fwd_f16_layout": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
+    "lpb_head_band_max_dims": (C.c_int, [_I, _I, C.POINTER(_I), C.POINTER(_I)]),
+    "lpb_head_fwd_bf16_band_max": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
+    "lpb_head_fwd_f16_band_max": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "lpb_head_bwd_bf16_workspace_bytes_layout": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bwd_bf16_layout": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_head_bwd_bf16_workspace_bytes_targets": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),

@@ -53,6 +53,8 @@ struct DecodeParams : DecodeGeom<DS> {
   float* stats;
   float lip, offset;
   int* queue;         // {count, plane ids ...}: the planes the warp kernel leaves for the CTA kernel
+  const uint32_t* band_max;  // or null: [n_planes][bm_nbands][8] the bits of each band's maxima (lpb_decode_fwd_banded)
+  int bm_rows, bm_nbands;    // heatmap rows per band (the last band may be shorter), bands per plane
   int* qcounter;      // [n_planes] arrival counters (zeroed) and
   float* qscratch;    // [n_planes][DEC_MAX_PARTS][4] partial softmax states of a plane split over several CTAs
 };
@@ -506,11 +508,35 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
     if (lane == 0) queue[1 + atomicAdd(queue, 1)] = (int)plane;
   };
 
+  // ---- band maxima (lpb_decode_fwd_banded): the bands of rows that can hold the arg max and the hull ----------
+  // With a positive finite maximum gmax over the slots, the lowest flat index holding the plane's maximum lies in the
+  // first band (in row order) whose maximum equals gmax, and a band whose maximum is below theta holds no candidate of
+  // pass 2: both passes sweep only those rows and find what the full sweeps find.  Otherwise the full sweeps decide.
+  const uint32_t* bm = nullptr;
+  const int nslots = P.bm_nbands * 8, band_groups = 2 * P.bm_rows * w4;
+  int i0 = 0, i1 = n4;  // pass 1's 4-column groups
+  if (P.band_max) {
+    const uint32_t* slots = P.band_max + (size_t)plane * nslots;
+    uint32_t g = 0u;
+    for (int k = lane; k < nslots; k += 32) g = max(g, __ldg(slots + k));
+    g = __reduce_max_sync(0xffffffffu, g);
+    if (g > 0u && g < 0x7f800000u) {  // bits of a positive finite float
+      int first = -1;  // the lowest slot holding gmax: its band is the first whose maximum is gmax
+      for (int k0 = 0; k0 < nslots && first < 0; k0 += 32) {
+        const unsigned hit = __ballot_sync(0xffffffffu, k0 + lane < nslots && __ldg(slots + k0 + lane) == g);
+        if (hit) first = k0 + __ffs(hit) - 1;
+      }
+      bm = slots;
+      i0 = (first >> 3) * band_groups;
+      i1 = min(i0 + band_groups, n4);
+    }
+  }
+
   // ---- pass 1: arg max of |h| ----------------------------------------------------------------------------
   float best = -1.f;
   int bidx = 0;
 #pragma unroll 8
-  for (int idx = lane; idx < n4; idx += 32) {
+  for (int idx = i0 + lane; idx < i1; idx += 32) {
     const float4 x = ld4h(idx, pol_keep);
     const float m4 = fmaxf(fmaxf(fabsf(x.x), fabsf(x.y)), fmaxf(fabsf(x.z), fabsf(x.w)));
     if (m4 > best) {
@@ -550,14 +576,14 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
 
   // ---- pass 2: hull of the candidates (|h| >= theta), 4-column granularity ---------------------------------
   int amin = h, amax = -1, bmin = w, bmax = -1;
-  {
-    int a = 0, g = lane;  // idx = a * w4 + g
+  auto hull = [&](int j0, int j1) {  // the candidates among groups [j0, j1)
+    int a = j0 / w4, g = j0 - a * w4 + lane;  // idx = a * w4 + g
     while (g >= w4) {
       g -= w4;
       ++a;
     }
 #pragma unroll 4
-    for (int idx = lane; idx < n4; idx += 32) {
+    for (int idx = j0 + lane; idx < j1; idx += 32) {
       const float4 x = ld4h(idx, pol_drop);
       const bool c = (fabsf(x.x) >= theta) || (fabsf(x.y) >= theta) || (fabsf(x.z) >= theta) || (fabsf(x.w) >= theta);
       if (c) {
@@ -570,6 +596,20 @@ __device__ void decode_plane_warp(const DecodeParams<DS>& P, long long plane, co
       while (g >= w4) {
         g -= w4;
         ++a;
+      }
+    }
+  };
+  if (!bm) {
+    hull(0, n4);
+  } else {
+    // the bands whose maximum reaches theta, 4 bands (32 slots) per ballot
+    for (int k0 = 0; k0 < nslots; k0 += 32) {
+      unsigned hit = __ballot_sync(0xffffffffu, k0 + lane < nslots && __uint_as_float(__ldg(bm + k0 + lane)) >= theta);
+      while (hit) {
+        const int j = (__ffs(hit) - 1) >> 3;  // band (k0 >> 3) + j
+        hit &= ~(0xffu << (8 * j));
+        const int j0 = ((k0 >> 3) + j) * band_groups;
+        hull(j0, min(j0 + band_groups, n4));
       }
     }
   }
@@ -1137,7 +1177,8 @@ static size_t decode_fwd_workspace_bytes(int64_t n_planes) {
 
 template <int DS>
 static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, float T, float* xy, float* conf,
-                             float* stats, void* workspace, cudaStream_t stream) {
+                             float* stats, void* workspace, cudaStream_t stream, const uint32_t* band_max = nullptr,
+                             int bm_rows = 0, int bm_nbands = 0) {
   using G = UpsampleGeom<DS>;
   DecodeParams<DS> P;
   DeviceLimits dev;
@@ -1148,6 +1189,9 @@ static int launch_decode_fwd(const float* heat, int64_t n_planes, int h, int w, 
   P.stats = stats;
   P.offset = (DS == 1) ? 0.5f : (DS == 2 ? 1.5f : 2.5f);  // lightning_pose/models/heads/heatmap.py:131-136
   P.queue = static_cast<int*>(workspace);
+  P.band_max = band_max;
+  P.bm_rows = bm_rows;
+  P.bm_nbands = bm_nbands;
   P.qcounter = P.queue + 1 + n_planes;
   P.qscratch = reinterpret_cast<float*>(P.queue + 1 + 2 * n_planes);
   const size_t smem = ((size_t)(h + 2 * G::R) * P.pitch + DEC_FWD_SCRATCH) * sizeof(float) + 16;
@@ -1208,25 +1252,47 @@ extern "C" int lpb_decode_fwd_workspace_bytes(int64_t n_planes, size_t* bytes) {
   return LPB_OK;
 }
 
-extern "C" int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
-                              float* xy, float* conf, float* stats, void* workspace, void* stream) {
+static int decode_fwd_entry(const char* name, const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
+                            const uint32_t* band_max, int band_rows, int nbands, float* xy, float* conf, float* stats,
+                            void* workspace, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(heatmaps && xy && conf, "decode_fwd: null pointer");
-  LPB_REQUIRE(h >= 1 && w >= 1 && ds >= 1 && ds <= 3, "decode_fwd: bad shape h=%d w=%d ds=%d", h, w, ds);
-  LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "decode_fwd: bad n_planes");
-  LPB_REQUIRE(workspace || n_planes == 0, "decode_fwd: null workspace");
-  LPB_REQUIRE(aligned_to(workspace, 4), "decode_fwd: workspace must be 4-byte aligned");
+  LPB_REQUIRE(heatmaps && xy && conf, "%s: null pointer", name);
+  LPB_REQUIRE(h >= 1 && w >= 1 && ds >= 1 && ds <= 3, "%s: bad shape h=%d w=%d ds=%d", name, h, w, ds);
+  LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "%s: bad n_planes", name);
+  LPB_REQUIRE(workspace || n_planes == 0, "%s: null workspace", name);
+  LPB_REQUIRE(aligned_to(workspace, 4), "%s: workspace must be 4-byte aligned", name);
   if (((int64_t)w << ds) > 1024 || w > 256) {
-    lpb::set_error("decode_fwd: heatmap width %d (x%d) exceeds this build's 1024-column field limit", w, 1 << ds);
+    lpb::set_error("%s: heatmap width %d (x%d) exceeds this build's 1024-column field limit", name, w, 1 << ds);
     return LPB_ERR_UNSUPPORTED;
+  }
+  LPB_REQUIRE(nbands >= 0, "%s: %d bands", name, nbands);
+  if (nbands > 0) {
+    // the band cut of the softmax that wrote the maxima: bands of band_rows input rows = 2 band_rows heatmap rows
+    LPB_REQUIRE(band_max, "%s: null band_max with %d bands", name, nbands);
+    LPB_REQUIRE(aligned_to(band_max, 4), "%s: band_max must be 4-byte aligned", name);
+    LPB_REQUIRE(h % 2 == 0 && band_rows >= 1 && (int64_t)(nbands - 1) * band_rows < h / 2 && (int64_t)nbands * band_rows >= h / 2,
+                "%s: %d bands of %d rows do not cut the %d input rows of a %d-row heatmap", name, nbands, band_rows, h / 2, h);
   }
   if (n_planes == 0) return LPB_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const uint32_t* bm = nbands > 0 ? band_max : nullptr;
   switch (ds) {
-    case 1: return launch_decode_fwd<1>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s);
-    case 2: return launch_decode_fwd<2>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s);
-    default: return launch_decode_fwd<3>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s);
+    case 1: return launch_decode_fwd<1>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s, bm, band_rows, nbands);
+    case 2: return launch_decode_fwd<2>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s, bm, band_rows, nbands);
+    default: return launch_decode_fwd<3>(heatmaps, n_planes, h, w, temperature, xy, conf, stats, workspace, s, bm, band_rows, nbands);
   }
+}
+
+extern "C" int lpb_decode_fwd(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
+                              float* xy, float* conf, float* stats, void* workspace, void* stream) {
+  return decode_fwd_entry("decode_fwd", heatmaps, n_planes, h, w, ds, temperature, nullptr, 0, 0, xy, conf, stats, workspace, stream);
+}
+
+extern "C" int lpb_decode_fwd_banded(const float* heatmaps, int64_t n_planes, int h, int w, int ds, float temperature,
+                                     const uint32_t* band_max, int band_rows, int nbands, float* xy, float* conf,
+                                     float* stats, void* workspace, void* stream) {
+  return decode_fwd_entry("decode_fwd_banded", heatmaps, n_planes, h, w, ds, temperature, band_max, band_rows, nbands, xy, conf,
+                          stats, workspace, stream);
 }
 
 extern "C" int lpb_decode_bwd(const float* heatmaps, const float* stats, const float* grad_xy, int64_t n_planes, int h,

@@ -554,7 +554,7 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
 template <typename T>
 static int head_fwd(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1, const float* w2,
                     const float* b2, int c2, int final_softmax, int feature_layout, float* out, void* saved_xs, void* workspace,
-                    void* stream) {
+                    void* stream, uint32_t* band_max = nullptr) {
   using namespace lpb;
   const char* name = head_fwd_name<T>;
   LPB_REQUIRE(feature_layout == LPB_FEATURES_NCHW || feature_layout == LPB_FEATURES_NHWC, "%s: unknown feature layout %d", name, feature_layout);
@@ -569,6 +569,7 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
   LPB_REQUIRE(aligned_to(saved_xs, 16), "%s: saved_xs must be 16-byte aligned", name);
   LPB_REQUIRE(aligned_to(workspace, 16), "%s: workspace must be 16-byte aligned", name);
   LPB_REQUIRE(aligned_to(out, 8), "%s: out must be 8-byte aligned", name);
+  LPB_REQUIRE(aligned_to(band_max, 4), "%s: band_max must be 4-byte aligned", name);
   if (B == 0) return LPB_OK;
   DeviceLimits dev;
   LPB_TRY(device_limits(&dev));
@@ -625,6 +626,7 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
     p.partials = partials;
     if (c2 == 0) {
       p.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
+      p.band_max = final_softmax ? band_max : nullptr;
       rc = launch_convt_rows(p, sms, s);
       if (rc != LPB_OK) return rc;
       LPB_CUDA(cudaGetLastError());
@@ -672,6 +674,7 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
   p2.out = out;
   p2.partials = partials;
   p2.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
+  p2.band_max = final_softmax ? band_max : nullptr;
   const int rc = launch_convt_rows(p2, sms, s);
   if (rc != LPB_OK) return rc;
   LPB_CUDA(cudaGetLastError());
@@ -688,6 +691,33 @@ extern "C" int lpb_head_fwd_f16_layout(const void* features, int B, int C, int H
                                        const float* w2, const float* b2, int c2, int final_softmax, int feature_layout, float* out,
                                        void* saved_xs, void* workspace, void* stream) {
   return head_fwd<__half>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, feature_layout, out, saved_xs, workspace, stream);
+}
+
+extern "C" int lpb_head_band_max_dims(int h, int w, int* band_rows, int* nbands) {
+  using namespace lpb;
+  LPB_REQUIRE(band_rows && nbands, "head_band_max_dims: null pointer");
+  LPB_REQUIRE(h >= 2 && w >= 2 && h % 2 == 0 && w % 2 == 0, "head_band_max_dims: bad heatmap size %dx%d", h, w);
+  // launch_convt_rows' cut of the softmax layer's (h / 2) x (w / 2) input
+  const int Hi = h / 2, Wi = w / 2;
+  int R = CR_BAND_ROWS / (Wi + 1);
+  R = R > Hi ? Hi : (R < 1 ? 1 : R);
+  *band_rows = R;
+  *nbands = convt_rows_bands(Hi, Wi);
+  return LPB_OK;
+}
+
+extern "C" int lpb_head_fwd_bf16_band_max(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                                          const float* w2, const float* b2, int c2, int feature_layout, float* out,
+                                          uint32_t* band_max, void* saved_xs, void* workspace, void* stream) {
+  LPB_REQUIRE(band_max, "head_fwd_bf16: null band_max");
+  return head_fwd<__nv_bfloat16>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, 1, feature_layout, out, saved_xs, workspace, stream, band_max);
+}
+
+extern "C" int lpb_head_fwd_f16_band_max(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,
+                                         const float* w2, const float* b2, int c2, int feature_layout, float* out,
+                                         uint32_t* band_max, void* saved_xs, void* workspace, void* stream) {
+  LPB_REQUIRE(band_max, "head_fwd_f16: null band_max");
+  return head_fwd<__half>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, 1, feature_layout, out, saved_xs, workspace, stream, band_max);
 }
 
 extern "C" int lpb_head_fwd_bf16(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1,

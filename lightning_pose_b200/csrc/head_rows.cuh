@@ -28,6 +28,9 @@ struct ConvtRowsParams {
   float* out;                // planes [B][cout][2Hi][2Wi] (raw or softmaxed)
   float* partials;           // split softmax: [B][ngroups][nbands][20][2] (max, sum) per (frame, group, band, plane), or
                              // null (fused two-pass form)
+  unsigned* band_max;        // softmax modes that write planes: [B][cout][nbands][8 epilogue warps] the bits of the
+                             // largest value each warp stored per (plane, band), or null (not written); see
+                             // lpb_head_band_max_dims
   int R, rows_alloc;         // filled by launch_convt_rows
   int ngroups;               // filled by launch_convt_rows: keypoint groups of the output channels (head_prep.cuh)
 };

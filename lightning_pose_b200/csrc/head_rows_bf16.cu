@@ -268,6 +268,12 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
           float acc[CR_TILES][2][6][4];
 #pragma unroll
           for (int t = 0; t < CR_TILES; ++t) mma::zero(acc[t]);
+          // writing pass: the largest value this thread stores per plane in this band (the values are >= 0; fmaxf drops
+          // NaNs).  17 more live registers cost ptxas 12 bytes of spill loads, and the kernel ran faster in
+          // situ than with one redux per plane and tile folded into a single register.
+          float bmx[HEAD_CLS];
+#pragma unroll
+          for (int o = 0; o < HEAD_CLS; ++o) bmx[o] = 0.f;
           for (int st = 0; st < nst; ++st, ++it) {
             const int s = it % CR_STAGES;
             mbar_wait_idle(&full[s], (it / CR_STAGES) & 1);
@@ -437,6 +443,7 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
                     const float p1 = fast_exp2(fmaf(rl[HEAD_CLS + o], L2E, -f.x)) * f.y;
                     *reinterpret_cast<float2*>(dst) = make_float2(p0, p1);
                     dst += plane_stride;
+                    bmx[o] = fmaxf(bmx[o], fmaxf(p0, p1));
                   }
                 }
               } else {
@@ -452,6 +459,18 @@ __global__ void __launch_bounds__(CR_THREADS, 1) convt_rows_kernel(const __grid_
             };
             if (e == 0) body(std::integral_constant<int, 0>{});
             else body(std::integral_constant<int, 1>{});
+          }
+          if (SOFTMAX && write && P.band_max) {
+            // the band maxima: one redux per plane over the warp's rows (unsigned order of non-negative floats' bits is
+            // float order), lane o stores plane o's into this warp's slot -- per-warp slots need no atomics or barrier
+            unsigned bm_lane = 0u;
+#pragma unroll
+            for (int o = 0; o < HEAD_CLS; ++o) {
+              if (o >= ncls) break;
+              const unsigned v = __reduce_max_sync(0xffffffffu, __float_as_uint(bmx[o]));
+              if (lane == o) bm_lane = v;
+            }
+            if (lane < ncls) P.band_max[(((size_t)b * P.cout + o0 + lane) * nbands + band) * 8 + ew] = bm_lane;
           }
         }
         if ((npass == 2 && pass == 0) || MODE == CONVT_ROWS_SOFTMAX_P0) {

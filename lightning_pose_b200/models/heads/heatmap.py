@@ -91,10 +91,15 @@ class _HeadFunction(torch.autograd.Function):
         # their gradient is written in the same format
         operand = ops.head_16_operand(features, [w.shape[1] for w in weights], train) if sixteen and features.is_cuda else None
         ctx.layout = ops.FEATURES_NCHW
+        band_max = None  # the softmax's per-band maxima: the decode sweeps only the bands that can matter
         if operand is not None:
             f16, ctx.layout = operand
-            res = ops._head_forward_16(f16, weights, biases, final_softmax, train=train, layout=ctx.layout)
-            out, saved = res if train else (res, None)
+            if decode is not None:
+                res = ops._head_forward_16(f16, weights, biases, final_softmax, train=train, want_hints=True, layout=ctx.layout)
+                out, saved, band_max = res if train else (res[0], None, res[1])
+            else:
+                res = ops._head_forward_16(f16, weights, biases, final_softmax, train=train, layout=ctx.layout)
+                out, saved = res if train else (res, None)
         elif train:
             out, acts = ops.head_forward_f32(features, weights, biases, final_softmax, keep_activations=True)
         else:
@@ -107,7 +112,7 @@ class _HeadFunction(torch.autograd.Function):
             ctx.save_for_backward(features, out, *params, *extra)
             return out
         ds, temperature = decode
-        xy, conf, stats = ops.decode_forward(out, int(ds), float(temperature))
+        xy, conf, stats = ops.decode_forward(out, int(ds), float(temperature), band_max=band_max)
         ctx.save_for_backward(features, out, *params, *extra, stats)
         ctx.mark_non_differentiable(conf)
         return out, xy.reshape(-1, out.shape[1] * 2), conf

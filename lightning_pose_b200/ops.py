@@ -7,6 +7,7 @@ no CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+from typing import NamedTuple
 
 import torch
 
@@ -65,9 +66,19 @@ def _cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
 # =====================================================================================
 # soft-argmax decode
 # =====================================================================================
-def decode_forward(heatmaps: torch.Tensor, ds: int, temperature: float):
+class BandMax(NamedTuple):
+    """Per-band maxima of softmax heatmaps, written by the 16-bit head's softmax (``lpb_head_fwd_bf16_band_max``):
+    ``bits`` int32 [B, K, nbands, 8], the float bits of the largest value in heatmap rows [2 j rows, 2 (j + 1) rows) of
+    band j, one slot per epilogue warp.  ``lpb_decode_fwd_banded`` sweeps only the bands that can matter."""
+
+    bits: torch.Tensor
+    rows: int
+    nbands: int
+
+
+def decode_forward(heatmaps: torch.Tensor, ds: int, temperature: float, band_max: BandMax | None = None):
     """soft-argmax decode -> (xy, conf, stats).  No autograd node of its own (``_decode_fwd`` and ``_HeadFunction`` own
-    the backward)."""
+    the backward).  ``band_max``: the head's band maxima of exactly these heatmaps (same outputs, fewer bytes read)."""
     b, k, h, w = heatmaps.shape
     xy = torch.empty((b, k, 2), device=heatmaps.device, dtype=torch.float32)
     conf = torch.empty((b, k), device=heatmaps.device, dtype=torch.float32)
@@ -76,7 +87,13 @@ def decode_forward(heatmaps: torch.Tensor, ds: int, temperature: float):
     check(lib.lpb_decode_fwd_workspace_bytes(b * k, C.byref(nbytes)))
     workspace = torch.empty((nbytes.value,), device=heatmaps.device, dtype=torch.uint8)
     with torch.cuda.device(heatmaps.device):
-        check(lib.lpb_decode_fwd(_ptr(heatmaps), b * k, h, w, ds, temperature, _ptr(xy), _ptr(conf), _ptr(stats), _ptr(workspace), _stream()))
+        if band_max is None:
+            check(lib.lpb_decode_fwd(_ptr(heatmaps), b * k, h, w, ds, temperature, _ptr(xy), _ptr(conf), _ptr(stats), _ptr(workspace), _stream()))
+        else:
+            if band_max.bits.shape != (b, k, band_max.nbands, 8) or band_max.bits.dtype != torch.int32 or not band_max.bits.is_contiguous():
+                raise ValueError(f"decode_forward: band maxima {tuple(band_max.bits.shape)} {band_max.bits.dtype} do not belong to heatmaps {tuple(heatmaps.shape)}")
+            check(lib.lpb_decode_fwd_banded(_ptr(heatmaps), b * k, h, w, ds, temperature, _ptr(band_max.bits), band_max.rows, band_max.nbands,
+                                            _ptr(xy), _ptr(conf), _ptr(stats), _ptr(workspace), _stream()))
     return xy, conf, stats
 
 
@@ -85,11 +102,10 @@ def _decode_fwd(heatmaps: torch.Tensor, ds: int, temperature: float) -> tuple[to
     return decode_forward(heatmaps, ds, temperature)
 
 
-def decode_forward_hinted(heatmaps: torch.Tensor, ds: int, temperature: float, hints):
-    # kept for bench.py's call, which passes what _head_forward_bf16(..., want_hints=True) returned: always None
-    if hints is not None:
-        raise ValueError("decode_forward_hinted: the head produces no decode hints; pass hints=None")
-    return decode_forward(heatmaps, ds, temperature)
+def decode_forward_hinted(heatmaps: torch.Tensor, ds: int, temperature: float, hints: BandMax | None):
+    """``decode_forward`` with the hints ``_head_forward_16(..., want_hints=True)`` returned: the band maxima of a
+    softmax head, or None (full sweeps)."""
+    return decode_forward(heatmaps, ds, temperature, band_max=hints)
 
 
 @_decode_fwd.register_fake
@@ -262,6 +278,9 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
     ``train=True`` (bf16 only: there is no fp16 backward) returns ``(out, saved)`` where ``saved`` carries what
     ``head_backward_bf16`` needs (the row-layout copy of the shuffled features and the forward workspace with the
     inter-layer activations).
+
+    ``want_hints=True`` appends the decode hints: with ``final_softmax`` the heatmaps' band maxima (``BandMax``, written
+    by the softmax pass for ``decode_forward``), otherwise None.
     """
     entry = _HEAD_FWD_16.get(f.dtype)
     if entry is None or (train and f.dtype != torch.bfloat16):
@@ -284,16 +303,25 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
     if train or plan.value == 0:  # row-layout copy of the shuffled features: the banded path's operand / the wgrad's input
         check(lib.lpb_head_bf16_saved_bytes(b, c, h, w, C.byref(nbytes)))
         xs = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
+    hints = None
     with torch.cuda.device(f.device):
-        check(entry(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), layout, _ptr(out), _ptr(xs), _ptr(ws), _stream()))
-    if want_hints:  # kept for bench.py's call, which unpacks a decode-hints slot (always None)
-        return (out, (xs, ws), None) if train else (out, None)
+        if want_hints and final_softmax:
+            rows, nbands = C.c_int(0), C.c_int(0)
+            check(lib.lpb_head_band_max_dims(out.shape[2], out.shape[3], C.byref(rows), C.byref(nbands)))
+            hints = BandMax(torch.empty((b, out.shape[1], nbands.value, 8), device=f.device, dtype=torch.int32), rows.value, nbands.value)
+            check(_HEAD_FWD_16_BAND_MAX[f.dtype](_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, layout, _ptr(out),
+                                                 _ptr(hints.bits), _ptr(xs), _ptr(ws), _stream()))
+        else:
+            check(entry(_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, int(bool(final_softmax)), layout, _ptr(out), _ptr(xs), _ptr(ws), _stream()))
+    if want_hints:
+        return (out, (xs, ws), hints) if train else (out, hints)
     if train:
         return out, (xs, ws)
     return out
 
 
 _HEAD_FWD_16 = {torch.bfloat16: lib.lpb_head_fwd_bf16_layout, torch.float16: lib.lpb_head_fwd_f16_layout}
+_HEAD_FWD_16_BAND_MAX = {torch.bfloat16: lib.lpb_head_fwd_bf16_band_max, torch.float16: lib.lpb_head_fwd_f16_band_max}
 _head_forward_bf16 = _head_forward_16  # the name bench.py and the bf16 tests call
 
 
