@@ -565,6 +565,25 @@ int lpb_heatmap_mse_from_keypoints_bwd(const float* keypoints, const int32_t* vi
                                        float sigma, const float* fwd_out, const float* grad_out, float* grad_preds,
                                        void* stream);
 
+/* fused target generation + HeatmapMSELoss / HeatmapKLLoss / HeatmapJSLoss (kind LPB_HM_*): replaces generate_heatmaps
+ * on the labeled keypoints (lightning_pose/data/heatmaps.py:37-87, called at data/datasets.py:516) followed by the loss
+ * (lightning_pose/losses/losses.py:229-289, :314-335, :338-378, :381-423).  No target plane is written.
+ * keypoints [n_planes, 2] image pixels, visibility [n_planes] or null (the plane rule of lpb_generate_heatmaps); preds
+ * [n_planes, oh, ow].  A plane whose target is all-zero is dropped without reading its prediction; uniform planes
+ * (visibility 1) use 1/(oh*ow); NaN planes are kept, so the loss is NaN as in the reference.  KL and JS add 1e-10 to
+ * both operands (:375-376, :420-421).  out[0] = mean over kept planes of the per-plane sum of terms, out[1] = the kept
+ * count; out[0] is NaN when nothing is kept.  workspace: n_planes * 2 floats.
+ * LPB_HM_MSE runs lpb_heatmap_mse_from_keypoints_fwd / _bwd (same bits, same refusals). */
+int lpb_heatmap_loss_from_keypoints_fwd(const float* keypoints, const int32_t* visibility, const float* preds,
+                                        int64_t n_planes, float img_height, float img_width, int oh, int ow,
+                                        float sigma, int kind, float* out, float* workspace, void* stream);
+/* d loss/d preds of the call above, written dense (zeros on dropped planes, and everywhere when nothing is kept);
+ * fwd_out is its out, grad_out the upstream scalar gradient (device pointers). */
+int lpb_heatmap_loss_from_keypoints_bwd(const float* keypoints, const int32_t* visibility, const float* preds,
+                                        int64_t n_planes, float img_height, float img_width, int oh, int ow,
+                                        float sigma, int kind, const float* fwd_out, const float* grad_out,
+                                        float* grad_preds, void* stream);
+
 /* replaces TemporalHeatmapLoss.__call__  lightning_pose/losses/losses.py:793-854
  * heatmaps [T,K,h,w], confidences [T,K], eps [K]; kind LPB_HM_MSE | LPB_HM_KL; out[0] = scalar loss;
  * workspace (T-1)*K floats. */

@@ -115,6 +115,8 @@ SIGNATURES = {
     "lpb_heatmap_loss_bwd": (C.c_int, [_P, _P, _L, _I, _I, _I, _P, _P, _P, _P, _P]),
     "lpb_heatmap_mse_from_keypoints_fwd": (C.c_int, [_P, _P, _P, _L, _F, _F, _I, _I, _F, _P, _P, _P]),
     "lpb_heatmap_mse_from_keypoints_bwd": (C.c_int, [_P, _P, _P, _L, _F, _F, _I, _I, _F, _P, _P, _P, _P]),
+    "lpb_heatmap_loss_from_keypoints_fwd": (C.c_int, [_P, _P, _P, _L, _F, _F, _I, _I, _F, _I, _P, _P, _P]),
+    "lpb_heatmap_loss_from_keypoints_bwd": (C.c_int, [_P, _P, _P, _L, _F, _F, _I, _I, _F, _I, _P, _P, _P, _P]),
     "lpb_temporal_heatmap_loss_fwd": (C.c_int, [_P, _P, _L, _I, _I, _I, _I, _P, _F, _P, _P, _P]),
     "lpb_temporal_heatmap_loss_bwd": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _I, _P, _F, _P, _P, _P]),
     "lpb_selftest_umma": (C.c_int, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),

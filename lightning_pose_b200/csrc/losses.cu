@@ -41,6 +41,12 @@ __device__ __forceinline__ float hm_term(int kind, float t, float p) {
   return 0.5f * (tt * (logf(tt) - lm) + pp * (logf(pp) - lm));
 }
 
+// d hm_term / d p for KL and JS (losses.py:375-376, :420-421 through autograd)
+__device__ __forceinline__ float hm_div_grad(int kind, float t, float p) {
+  const float tt = t + 1e-10f, pp = p + 1e-10f;
+  return (kind == LPB_HM_KL) ? -tt / pp : 0.5f * (logf(pp) - logf(0.5f * (tt + pp)));
+}
+
 // stage 1: one CTA per plane -> ws[2*plane] = sum of terms, ws[2*plane+1] = 1 if target not all-zero
 __global__ void __launch_bounds__(HL_THREADS) heatmap_loss_plane_kernel(const float* __restrict__ targ,
                                                                         const float* __restrict__ pred, int hw,
@@ -111,8 +117,7 @@ __global__ void __launch_bounds__(HL_THREADS) heatmap_loss_bwd_kernel(const floa
     } else if (kind == LPB_HM_MSE) {
       d = 2.f * (p[i] - t[i]);
     } else {
-      const float tt = t[i] + 1e-10f, pp = p[i] + 1e-10f;
-      d = (kind == LPB_HM_KL) ? -tt / pp : 0.5f * (logf(pp) - logf(0.5f * (tt + pp)));
+      d = hm_div_grad(kind, t[i], p[i]);
     }
     g[i] = d * scale;
   }
@@ -198,6 +203,84 @@ __global__ void __launch_bounds__(HL_THREADS) heatmap_mse_from_kp_bwd_kernel(con
   for (int r = warp; r < oh; r += HL_THREADS / 32) {
     const float er = ey[r] * norm;
     for (int c = lane; c < ow; c += 32) g[(size_t)r * ow + c] = mse_target_grad(TARGET_GAUSS, __ldg(p + (size_t)r * ow + c), ex[c], er, scale);
+  }
+}
+
+// fused target generation + KL / JS: each target value is made in registers where the prediction is read
+// (losses.py:338-423 on the planes of data/heatmaps.py:37-87).  A dropped plane's prediction is not read.
+__global__ void __launch_bounds__(HL_THREADS) heatmap_div_from_kp_kernel(const float* __restrict__ kp,
+                                                                         const int32_t* __restrict__ vis,
+                                                                         const float* __restrict__ pred, float sx,
+                                                                         float sy, int oh, int ow, float two_s2,
+                                                                         int kind, float* __restrict__ ws) {
+  extern __shared__ float sm[];  // ex[ow], ey[oh], red[16]
+  float* ex = sm;
+  float* ey = sm + ow;
+  float* red = ey + oh;
+  const size_t plane = blockIdx.x;
+  const int n = oh * ow;
+  const TargetPlane tp = classify_target(kp, vis, plane, sx, sy, oh, ow);
+  if (tp.mode == TARGET_ZERO) {
+    if (threadIdx.x == 0) {
+      ws[2 * plane] = 0.f;
+      ws[2 * plane + 1] = 0.f;
+    }
+    return;
+  }
+  const float* __restrict__ p = pred + plane * (size_t)n;
+  float acc = 0.f;
+  if (tp.mode == TARGET_UNIFORM) {
+    const float u = mse_target_uniform(n);
+    for (int i = threadIdx.x; i < n; i += HL_THREADS) acc += hm_term(kind, u, __ldg(p + i));
+  } else {
+    const float norm = target_axis_factors(tp, oh, ow, two_s2, ex, ey, red, HL_THREADS);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int r = warp; r < oh; r += HL_THREADS / 32) {
+      const float er = ey[r] * norm;
+      const float* __restrict__ pr = p + (size_t)r * ow;
+      for (int c = lane; c < ow; c += 32) acc += hm_term(kind, ex[c] * er, __ldg(pr + c));
+    }
+  }
+  acc = block_sum_256(acc, red + 8);
+  if (threadIdx.x == 0) {
+    ws[2 * plane] = acc;
+    ws[2 * plane + 1] = 1.f;  // a Gaussian / uniform target is never all-zero (NaN planes are kept too)
+  }
+}
+
+// backward of the kernel above: d loss / d pred = hm_div_grad(target, pred) * grad_out / n_kept on kept planes, 0 on
+// dropped ones (and everywhere when the scale is 0, as heatmap_loss_bwd_kernel does)
+__global__ void __launch_bounds__(HL_THREADS) heatmap_div_from_kp_bwd_kernel(const float* __restrict__ kp,
+                                                                             const int32_t* __restrict__ vis,
+                                                                             const float* __restrict__ pred, float sx,
+                                                                             float sy, int oh, int ow, float two_s2,
+                                                                             int kind, const float* __restrict__ fwd_out,
+                                                                             const float* __restrict__ gout,
+                                                                             float* __restrict__ gpred) {
+  extern __shared__ float sm[];  // ex[ow], ey[oh], red[16]
+  float* ex = sm;
+  float* ey = sm + ow;
+  float* red = ey + oh;
+  const size_t plane = blockIdx.x;
+  const int n = oh * ow;
+  const TargetPlane tp = classify_target(kp, vis, plane, sx, sy, oh, ow);
+  float* __restrict__ g = gpred + plane * (size_t)n;
+  const float scale = tp.mode == TARGET_ZERO ? 0.f : gout[0] / fwd_out[1];
+  if (scale == 0.f) {
+    for (int i = threadIdx.x; i < n; i += HL_THREADS) g[i] = 0.f;
+    return;
+  }
+  const float* __restrict__ p = pred + plane * (size_t)n;
+  if (tp.mode == TARGET_UNIFORM) {
+    const float u = mse_target_uniform(n);
+    for (int i = threadIdx.x; i < n; i += HL_THREADS) g[i] = hm_div_grad(kind, u, __ldg(p + i)) * scale;
+    return;
+  }
+  const float norm = target_axis_factors(tp, oh, ow, two_s2, ex, ey, red, HL_THREADS);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int r = warp; r < oh; r += HL_THREADS / 32) {
+    const float er = ey[r] * norm;
+    for (int c = lane; c < ow; c += 32) g[(size_t)r * ow + c] = hm_div_grad(kind, ex[c] * er, __ldg(p + (size_t)r * ow + c)) * scale;
   }
 }
 
@@ -823,6 +906,49 @@ extern "C" int lpb_heatmap_mse_from_keypoints_bwd(const float* keypoints, const 
   const TargetGeom tg = target_geom(img_height, img_width, oh, ow, sigma);
   heatmap_mse_from_kp_bwd_kernel<<<(unsigned)n_planes, HL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
       keypoints, visibility, preds, tg.sx, tg.sy, oh, ow, tg.two_s2, fwd_out, grad_out, grad_preds);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_heatmap_loss_from_keypoints_fwd(const float* keypoints, const int32_t* visibility, const float* preds,
+                                                   int64_t n_planes, float img_height, float img_width, int oh, int ow,
+                                                   float sigma, int kind, float* out, float* workspace, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(kind >= 0 && kind <= 2, "heatmap_loss_from_keypoints_fwd: bad kind %d", kind);
+  if (kind == LPB_HM_MSE)
+    return lpb_heatmap_mse_from_keypoints_fwd(keypoints, visibility, preds, n_planes, img_height, img_width, oh, ow, sigma,
+                                              out, workspace, stream);
+  LPB_REQUIRE(keypoints && preds && out && workspace, "heatmap_loss_from_keypoints_fwd: null pointer");
+  LPB_REQUIRE(oh >= 1 && ow >= 1 && oh + ow < 8000 && sigma > 0.f && img_height > 0.f && img_width > 0.f,
+              "heatmap_loss_from_keypoints_fwd: bad shape");
+  LPB_REQUIRE(n_planes >= 1 && n_planes < (1ll << 31), "heatmap_loss_from_keypoints_fwd: bad n_planes");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t smem = (size_t)(oh + ow + 16) * sizeof(float);
+  const TargetGeom tg = target_geom(img_height, img_width, oh, ow, sigma);
+  heatmap_div_from_kp_kernel<<<(unsigned)n_planes, HL_THREADS, smem, s>>>(keypoints, visibility, preds, tg.sx, tg.sy, oh, ow,
+                                                                          tg.two_s2, kind, workspace);
+  heatmap_loss_final_kernel<<<1, HL_THREADS, 0, s>>>(workspace, n_planes, out);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_heatmap_loss_from_keypoints_bwd(const float* keypoints, const int32_t* visibility, const float* preds,
+                                                   int64_t n_planes, float img_height, float img_width, int oh, int ow,
+                                                   float sigma, int kind, const float* fwd_out, const float* grad_out,
+                                                   float* grad_preds, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(kind >= 0 && kind <= 2, "heatmap_loss_from_keypoints_bwd: bad kind %d", kind);
+  if (kind == LPB_HM_MSE)
+    return lpb_heatmap_mse_from_keypoints_bwd(keypoints, visibility, preds, n_planes, img_height, img_width, oh, ow, sigma,
+                                              fwd_out, grad_out, grad_preds, stream);
+  LPB_REQUIRE(keypoints && preds && fwd_out && grad_out && grad_preds, "heatmap_loss_from_keypoints_bwd: null pointer");
+  LPB_REQUIRE(oh >= 1 && ow >= 1 && oh + ow < 8000 && sigma > 0.f && img_height > 0.f && img_width > 0.f,
+              "heatmap_loss_from_keypoints_bwd: bad shape");
+  LPB_REQUIRE(n_planes >= 1 && n_planes < (1ll << 31), "heatmap_loss_from_keypoints_bwd: bad n_planes");
+  const size_t smem = (size_t)(oh + ow + 16) * sizeof(float);
+  const TargetGeom tg = target_geom(img_height, img_width, oh, ow, sigma);
+  heatmap_div_from_kp_bwd_kernel<<<(unsigned)n_planes, HL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+      keypoints, visibility, preds, tg.sx, tg.sy, oh, ow, tg.two_s2, kind, fwd_out, grad_out, grad_preds);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

@@ -48,10 +48,12 @@ class GaussianTargets:
 
     The reference's DataLoader workers render ``(K, h, w)`` target planes on the CPU
     (``data/datasets.py:486-525``) and ship 627 KB per frame to the device.  Here the batch ships only
-    ``(keypoints, visibility)``; the supervised loss consumes this object: ``HeatmapMSELoss`` evaluates targets and
-    loss in one kernel without ever writing the planes (``ops.heatmap_mse_from_keypoints``), the other heatmap losses
-    call ``materialize()``.  ``keypoints`` are model-image pixels AFTER augmentation; the out-of-frame -> NaN rule of
-    ``compute_heatmap`` (:496-508) is applied on the device at construction.
+    ``(keypoints, visibility)``; the supervised loss consumes this object: ``HeatmapMSELoss``, ``HeatmapKLLoss``,
+    ``HeatmapJSLoss`` and ``ReprojectionHeatmapLoss`` evaluate targets and loss in one kernel without ever writing the
+    planes (``ops.heatmap_loss_from_keypoints``); ``materialize()`` renders them for any other consumer.  ``keypoints``
+    are model-image pixels AFTER augmentation; the out-of-frame -> NaN rule of ``compute_heatmap`` (:496-508) is applied
+    on the device at construction unless ``ignore_nans`` (the reference's flag: calibrated multi-view validation
+    batches skip the rule, ``datasets.py:1161-1164``).
     """
 
     def __init__(self, keypoints: torch.Tensor, height: int, width: int, output_shape: tuple[int, int], sigma: float = 1.25,

@@ -9,10 +9,12 @@ Every class keeps the reference's constructor keywords, attributes (``loss_name`
 staged pipeline (boolean-mask gathers, python loops over frames, a dozen tiny launches) each loss
 is one fused CUDA reduction (``csrc/losses.cu``) that produces the same scalar:
 
-* ``HeatmapMSELoss/KLLoss/JSLoss``  -> ``ops.heatmap_loss`` (all-zero target planes dropped on device)
+* ``HeatmapMSELoss/KLLoss/JSLoss``  -> ``ops.heatmap_loss`` (all-zero target planes dropped on device), or
+                                       ``ops.heatmap_loss_from_keypoints`` given ``GaussianTargets``
 * ``TemporalLoss`` / ``PCALoss``     -> ``ops.unsup_losses`` (one launch; the factory shares it)
 * ``TemporalHeatmapLoss``           -> ``ops.temporal_heatmap_loss``
-* ``ReprojectionHeatmapLoss``       -> ``ops.generate_heatmaps`` (differentiable) + ``ops.heatmap_loss``
+* ``ReprojectionHeatmapLoss``       -> ``ops.generate_heatmaps`` (differentiable) + ``ops.heatmap_loss``, or
+                                       ``ops.heatmap_loss_from_keypoints("mse")`` given ``GaussianTargets``
 * ``PairwiseProjectionsLoss``       -> ``ops.pairwise_projections_loss`` (NaN entries dropped on device)
 
 The staged methods remain as small tensor utilities for callers/tests that use them directly; the
@@ -122,12 +124,10 @@ class HeatmapLoss(Loss):
         stage: Literal["train", "val", "test"] | None = None,
         **kwargs: Any,
     ) -> LossOutput:
-        if isinstance(heatmaps_targ, GaussianTargets):  # targets made on the GPU from (keypoints, visibility)
-            if self._kind == "mse":  # one kernel, target planes never written
-                scalar_loss = ops.heatmap_mse_from_keypoints(heatmaps_targ.keypoints, heatmaps_pred, heatmaps_targ.height, heatmaps_targ.width,
-                                                             sigma=heatmaps_targ.sigma, visibility=heatmaps_targ.visibility)
-                return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
-            heatmaps_targ = heatmaps_targ.materialize()
+        if isinstance(heatmaps_targ, GaussianTargets):  # targets made on the GPU from (keypoints, visibility), never written
+            scalar_loss = ops.heatmap_loss_from_keypoints(self._kind, heatmaps_targ.keypoints, heatmaps_pred, heatmaps_targ.height,
+                                                          heatmaps_targ.width, sigma=heatmaps_targ.sigma, visibility=heatmaps_targ.visibility)
+            return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
         scalar_loss = ops.heatmap_loss(heatmaps_targ, heatmaps_pred, self._kind)
         return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
 
@@ -480,7 +480,11 @@ class ReprojectionHeatmapLoss(Loss):
             (self.downsampled_image_height, self.downsampled_image_width),
             keep_gradients=True,
         )
-        mse, n_kept = ops.heatmap_loss(heatmaps_targ, heatmaps_pred, "mse", return_count=True)
+        if isinstance(heatmaps_targ, GaussianTargets):  # targets evaluated where the predictions are read, never written
+            mse, n_kept = ops.heatmap_loss_from_keypoints("mse", heatmaps_targ.keypoints, heatmaps_pred, heatmaps_targ.height, heatmaps_targ.width,
+                                                          sigma=heatmaps_targ.sigma, visibility=heatmaps_targ.visibility, return_count=True)
+        else:
+            mse, n_kept = ops.heatmap_loss(heatmaps_targ, heatmaps_pred, "mse", return_count=True)
         # sum((t-p)^2) / n_kept  ->  mean over kept pixels of (t-p)^2 * (K*h)
         scale = heatmaps_targ.shape[1] / heatmaps_targ.shape[3]
         scalar_loss = torch.where(n_kept > 0, mse * scale, torch.zeros_like(mse))

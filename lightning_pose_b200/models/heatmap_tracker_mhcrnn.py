@@ -18,6 +18,7 @@ from torch import nn
 
 from lightning_pose_b200 import ops
 from lightning_pose_b200.data.bboxes import model_to_frame_batch
+from lightning_pose_b200.data.heatmaps import GaussianTargets
 from lightning_pose_b200.losses.factory import LossFactory
 from lightning_pose_b200.losses.losses import RegressionRMSELoss
 from lightning_pose_b200.models.backbones import BACKBONE_STRIDES
@@ -81,16 +82,36 @@ class HeatmapTrackerMHCRNN(nn.Module):
         sf, mf = self.forward(batch_dict["images"])
         kp_sf, cf_sf = self.head.run_subpixelmaxima(sf)
         kp_mf, cf_mf = self.head.run_subpixelmaxima(mf)
-        target = model_to_frame_batch(batch_dict, batch_dict["keypoints"])
+        if "heatmaps" in batch_dict:  # reference flow: DataLoader workers rendered the centre frame's targets
+            heatmaps_targ = torch.cat([batch_dict["heatmaps"], batch_dict["heatmaps"]], dim=0)
+            target = model_to_frame_batch(batch_dict, batch_dict["keypoints"])
+        else:
+            heatmaps_targ, keypoints = self._keypoint_targets(batch_dict)
+            target = model_to_frame_batch(batch_dict, keypoints, in_place=False)
         kp_sf = model_to_frame_batch(batch_dict, kp_sf)
         kp_mf = model_to_frame_batch(batch_dict, kp_mf)
         return {
-            "heatmaps_targ": torch.cat([batch_dict["heatmaps"], batch_dict["heatmaps"]], dim=0),
+            "heatmaps_targ": heatmaps_targ,
             "heatmaps_pred": torch.cat([sf, mf], dim=0),
             "keypoints_targ": torch.cat([target, target], dim=0),
             "keypoints_pred": torch.cat([kp_sf, kp_mf], dim=0),
             "confidences": torch.cat([cf_sf, cf_mf], dim=0),
         }
+
+    def _keypoint_targets(self, batch_dict: dict) -> tuple[GaussianTargets, torch.Tensor]:
+        """Targets of a labeled batch that ships the centre frame's ``keypoints`` (and ``visibility``) without
+        ``heatmaps``: ``GaussianTargets`` standing for ``torch.cat([heatmaps, heatmaps])``, one copy per head (reference
+        :158-173), and the keypoints after the out-of-frame -> NaN rule, which the reference's ``compute_heatmap``
+        applies in place on the example's keypoints (``datasets.py:486-508``), so it reaches the RMSE targets too.
+        ``images`` is (B, 5, 3, H, W) or (B, V, 5, 3, H, W); the heatmaps are (H, W) / 2**downsample_factor."""
+        images, keypoints = batch_dict["images"], batch_dict["keypoints"]
+        h_img, w_img = images.shape[-2], images.shape[-1]
+        shape_hm = (h_img // 2**self.downsample_factor, w_img // 2**self.downsample_factor)
+        centre = GaussianTargets(keypoints, h_img, w_img, shape_hm, sigma=1.25, visibility=batch_dict.get("visibility"))
+        kp, vis = centre.keypoints, centre.visibility
+        both = GaussianTargets(torch.cat([kp, kp], dim=0), h_img, w_img, shape_hm, sigma=1.25,
+                               visibility=None if vis is None else torch.cat([vis, vis], dim=0), ignore_nans=True)
+        return both, kp.reshape(keypoints.shape)
 
     def predict_step(self, batch_dict: dict, batch_idx: int, return_heatmaps: bool | None = False):
         images = batch_dict["images"] if "images" in batch_dict else batch_dict["frames"]

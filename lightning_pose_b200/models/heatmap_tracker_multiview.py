@@ -36,6 +36,7 @@ from lightning_pose_b200 import ops
 from lightning_pose_b200.callbacks import PatchMasker
 from lightning_pose_b200.data.bboxes import model_to_frame_batch
 from lightning_pose_b200.data.cameras import project_camera_pairs_to_3d
+from lightning_pose_b200.data.heatmaps import GaussianTargets
 from lightning_pose_b200.losses.factory import LossFactory
 from lightning_pose_b200.losses.losses import RegressionRMSELoss
 from lightning_pose_b200.models.backbones import tokens_to_feature_map
@@ -108,7 +109,12 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
 
     def get_loss_inputs_labeled(self, batch_dict: dict) -> dict:
         pred_heatmaps, pred_keypoints, confidence = self.forward_with_keypoints(batch_dict["images"])
-        target_keypoints = model_to_frame_batch(batch_dict, batch_dict["keypoints"])
+        if "heatmaps" in batch_dict:  # reference flow: DataLoader workers rendered the targets
+            heatmaps_targ = batch_dict["heatmaps"]
+            target_keypoints = model_to_frame_batch(batch_dict, batch_dict["keypoints"])
+        else:
+            heatmaps_targ = self._keypoint_targets(batch_dict)
+            target_keypoints = model_to_frame_batch(batch_dict, heatmaps_targ.keypoints.reshape(batch_dict["keypoints"].shape), in_place=False)
         pred_keypoints = model_to_frame_batch(batch_dict, pred_keypoints)
         keypoints_targ_3d = keypoints_pred_3d = keypoints_pred_2d_reprojected = None
         # calibrated batches (reference :263-303): triangulate every camera pair; with the reprojection loss registered,
@@ -126,7 +132,7 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
                     keypoints_pred_3d, *cameras, mean_over_pairs=True, bbox=batch_dict["bbox"], model_size=images.shape[-2:],
                 ).reshape(-1, num_views * num_keypoints, 2)
         return {
-            "heatmaps_targ": batch_dict["heatmaps"],
+            "heatmaps_targ": heatmaps_targ,
             "heatmaps_pred": pred_heatmaps,
             "keypoints_targ": target_keypoints,
             "keypoints_pred": pred_keypoints,
@@ -135,6 +141,24 @@ class HeatmapTrackerMultiviewTransformer(nn.Module):
             "keypoints_pred_3d": keypoints_pred_3d,  # (batch, cam_pairs, num_keypoints, 3)
             "keypoints_pred_2d_reprojected": keypoints_pred_2d_reprojected,  # (batch, num_views * num_keypoints, 2)
         }
+
+    def _keypoint_targets(self, batch_dict: dict) -> GaussianTargets:
+        """Targets of a labeled batch that ships ``keypoints`` (B, V * K * 2) model pixels (and ``visibility``
+        (B, V * K)) without ``heatmaps``: planes view-major, v * K + k, the order of the reference's ``fusion``
+        (``datasets.py:1129-1148``), each (H, W) / 2**downsample_factor.
+
+        The out-of-frame -> NaN rule applies unless the batch carries ``"ignore_nans": True``, a Python bool (a
+        tensor would cost a host sync): the reference's dataset skips the rule for calibrated batches
+        (``datasets.py:1161-1164``) and recomputes the targets of calibrated training batches after the 3-D
+        augmentation with the rule applied (:1094-1101), so pass True for calibrated validation batches only.  As
+        there (the rule writes NaN into the example's keypoints), the masked keypoints are also the RMSE targets.
+        Building the targets is one kernel launch and no host sync, so a labeled step still captures into a CUDA
+        graph."""
+        images = batch_dict["images"]
+        h_img, w_img = images.shape[-2], images.shape[-1]
+        shape_hm = (h_img // 2**self.downsample_factor, w_img // 2**self.downsample_factor)
+        return GaussianTargets(batch_dict["keypoints"], h_img, w_img, shape_hm, sigma=1.25, visibility=batch_dict.get("visibility"),
+                               ignore_nans=bool(batch_dict.get("ignore_nans", False)))
 
     def predict_step(self, batch_dict: dict, batch_idx: int, return_heatmaps: bool = False):
         images = batch_dict["images"] if "images" in batch_dict else batch_dict["frames"]

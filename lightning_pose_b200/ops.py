@@ -31,6 +31,7 @@ __all__ = [
     "remap_keypoints",
     "heatmap_loss",
     "heatmap_mse_from_keypoints",
+    "heatmap_loss_from_keypoints",
     "temporal_heatmap_loss",
     "unsup_losses",
     "PcaParams",
@@ -1072,6 +1073,54 @@ def heatmap_mse_from_keypoints(keypoints, preds, height, width, sigma=1.25, visi
     p = _cuda_f32(preds, "heatmaps_pred")
     vis = visibility.to(torch.int32).contiguous() if visibility is not None else None
     return _HeatmapMseFromKeypoints.apply(kp, vis, p, float(height), float(width), float(sigma))
+
+
+class _HeatmapLossFromKeypoints(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, kp, vis, preds, height, width, sigma, kind):
+        b, k, oh, ow = preds.shape
+        out = torch.empty((2,), device=preds.device, dtype=torch.float32)
+        ws = torch.empty((b * k * 2,), device=preds.device, dtype=torch.float32)
+        with torch.cuda.device(preds.device):
+            check(lib.lpb_heatmap_loss_from_keypoints_fwd(_ptr(kp), _ptr(vis), _ptr(preds), b * k, height, width, oh, ow, sigma, kind,
+                                                          _ptr(out), _ptr(ws), _stream()))
+        ctx.save_for_backward(kp, vis, preds, out)
+        ctx.meta = (height, width, sigma, kind)
+        loss, count = out[0].clone(), out[1].clone()
+        ctx.mark_non_differentiable(count)
+        return loss, count
+
+    @staticmethod
+    def backward(ctx, g, _g_count):
+        kp, vis, preds, out = ctx.saved_tensors
+        height, width, sigma, kind = ctx.meta
+        b, k, oh, ow = preds.shape
+        gp = torch.empty_like(preds)
+        gg = g.reshape(1).contiguous().float()
+        with torch.cuda.device(preds.device):
+            check(lib.lpb_heatmap_loss_from_keypoints_bwd(_ptr(kp), _ptr(vis), _ptr(preds), b * k, height, width, oh, ow, sigma, kind,
+                                                          _ptr(out), _ptr(gg), _ptr(gp), _stream()))
+        return None, None, gp, None, None, None, None
+
+
+def heatmap_loss_from_keypoints(kind: str, keypoints, preds, height, width, sigma=1.25, visibility=None, return_count: bool = False):
+    """Fused target generation + HeatmapMSELoss / KLLoss / JSLoss (``kind`` "mse" | "kl" | "js"): the Gaussian targets of
+    ``keypoints`` (B, K, 2) image pixels are made where ``preds`` (B, K, oh, ow) is read and never written; differentiable
+    in ``preds``.  With ``return_count`` also the number of kept planes (a non-differentiable device scalar).
+
+    "mse" without the count is ``heatmap_mse_from_keypoints`` (whose gradient the bf16 head takes implicitly); the other
+    kinds, and "mse" with the count, write the dense gradient once in the backward."""
+    if kind == "mse" and not return_count:
+        return heatmap_mse_from_keypoints(keypoints, preds, height, width, sigma, visibility)
+    kp = _cuda_f32(keypoints, "keypoints").detach()
+    p = _cuda_f32(preds, "heatmaps_pred")
+    vis = visibility.to(torch.int32).contiguous() if visibility is not None else None
+    planes = p.shape[0] * p.shape[1] if p.dim() == 4 else -1
+    if planes < 0 or kp.numel() != 2 * planes or (vis is not None and vis.numel() != planes):
+        raise ValueError(f"heatmap_loss_from_keypoints: keypoints {tuple(kp.shape)}, visibility "
+                         f"{None if vis is None else tuple(vis.shape)} do not match preds {tuple(p.shape)} (B, K, h, w)")
+    loss, count = _HeatmapLossFromKeypoints.apply(kp, vis, p, float(height), float(width), float(sigma), _KIND[kind])
+    return (loss, count) if return_count else loss
 
 
 class _TemporalHeatmapLoss(torch.autograd.Function):
