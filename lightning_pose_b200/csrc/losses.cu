@@ -29,6 +29,9 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
   return t;
 }
 
+// F.relu as torch computes it: NaN stays NaN (fmaxf would return the 0), every other value gets fmaxf's bits
+__device__ __forceinline__ float relu_keep_nan(float x) { return isnan(x) ? x : fmaxf(x, 0.f); }
+
 __device__ __forceinline__ float hm_term(int kind, float t, float p) {
   if (kind == LPB_HM_MSE) {
     const float d = t - p;
@@ -318,7 +321,7 @@ __global__ void __launch_bounds__(HL_THREADS) temporal_heatmap_final_kernel(cons
     const int t = i / K, k = i - t * K;
     float d = ws[i];
     if (conf[(size_t)t * K + k] < thr || conf[(size_t)(t + 1) * K + k] < thr) d = 0.f;
-    acc += fmaxf(d - eps[k], 0.f);
+    acc += relu_keep_nan(d - eps[k]);
   }
   acc = block_sum_256(acc, red);
   if (threadIdx.x == 0) out[0] = acc / (float)((T - 1) * K);
@@ -328,7 +331,9 @@ __global__ void __launch_bounds__(HL_THREADS) temporal_heatmap_final_kernel(cons
 //   MSE  d = mean((a-b)^2):                 dd/da = 2(a-b)/hw,          dd/db = -2(a-b)/hw
 //   KL   d = sum p (log p - log q), q = a + 1e-10, p = b + 1e-10:   dd/da = -p/q,   dd/db = log p - log q + 1
 // a pair (t, k) carries gradient iff neither confidence is below the threshold (the reference zeroes those
-// entries in place, losses.py:789) and d > eps_k (F.relu, :761); the mean runs over all (T-1)*K entries (:851).
+// entries in place, losses.py:789) and d > eps_k or d is NaN (F.relu, :761, passes the gradient of a NaN); the mean
+// runs over all (T-1)*K entries (:851).  A pair without gradient whose d is NaN still gives NaN where either of its
+// pixels is NaN, as autograd's 0 * NaN does in the per-pixel backward; its other pixels get 0.
 __global__ void __launch_bounds__(HL_THREADS) temporal_heatmap_bwd_kernel(const float* __restrict__ hm,
                                                                           const float* __restrict__ conf,
                                                                           const float* __restrict__ ws, int T, int K,
@@ -337,27 +342,33 @@ __global__ void __launch_bounds__(HL_THREADS) temporal_heatmap_bwd_kernel(const 
                                                                           float* __restrict__ grad) {
   const int t = blockIdx.x / K, k = blockIdx.x - t * K;
   const float scale = __ldg(gout) / (float)((T - 1) * K);
-  auto active = [&](int tt) {  // pair (tt, tt + 1)
-    if (tt < 0 || tt >= T - 1) return false;
-    if (conf[(size_t)tt * K + k] < thr || conf[(size_t)(tt + 1) * K + k] < thr) return false;
-    return ws[(size_t)tt * K + k] - eps[k] > 0.f;
+  enum { PAIR_OFF, PAIR_GRAD, PAIR_NAN_ONLY };
+  auto state = [&](int tt) {  // pair (tt, tt + 1)
+    if (tt < 0 || tt >= T - 1) return PAIR_OFF;
+    const float d = ws[(size_t)tt * K + k];
+    if (conf[(size_t)tt * K + k] < thr || conf[(size_t)(tt + 1) * K + k] < thr) return isnan(d) ? PAIR_NAN_ONLY : PAIR_OFF;
+    return d - eps[k] > 0.f || isnan(d) ? PAIR_GRAD : PAIR_OFF;
   };
-  const bool fwd = active(t), bwd = active(t - 1);  // this plane is `a` of pair t and `b` of pair t - 1
+  const int fwd = state(t), bwd = state(t - 1);  // this plane is `a` of pair t and `b` of pair t - 1
   const float* __restrict__ cur = hm + ((size_t)t * K + k) * hw;
-  const float* __restrict__ nxt = fwd ? hm + ((size_t)(t + 1) * K + k) * hw : cur;
-  const float* __restrict__ prv = bwd ? hm + ((size_t)(t - 1) * K + k) * hw : cur;
+  const float* __restrict__ nxt = fwd != PAIR_OFF ? hm + ((size_t)(t + 1) * K + k) * hw : cur;
+  const float* __restrict__ prv = bwd != PAIR_OFF ? hm + ((size_t)(t - 1) * K + k) * hw : cur;
   float* __restrict__ g = grad + ((size_t)t * K + k) * hw;
   const float inv_hw = 1.0f / (float)hw;
   for (int i = threadIdx.x; i < hw; i += HL_THREADS) {
     const float x = __ldg(cur + i);
     float acc = 0.f;
-    if (fwd) {
+    if (fwd == PAIR_GRAD) {
       const float y = __ldg(nxt + i);
       acc += kind == LPB_HM_MSE ? 2.f * (x - y) * inv_hw : -(y + 1e-10f) / (x + 1e-10f);
+    } else if (fwd == PAIR_NAN_ONLY) {
+      acc += 0.f * (x - __ldg(nxt + i));
     }
-    if (bwd) {
+    if (bwd == PAIR_GRAD) {
       const float z = __ldg(prv + i);
       acc += kind == LPB_HM_MSE ? -2.f * (z - x) * inv_hw : logf(x + 1e-10f) - logf(z + 1e-10f) + 1.f;
+    } else if (bwd == PAIR_NAN_ONLY) {
+      acc += 0.f * (__ldg(prv + i) - x);
     }
     g[i] = acc * scale;
   }
@@ -459,9 +470,19 @@ __device__ __forceinline__ float block_sum_ul(float v, float* red) {
 }
 
 // quantile(0.5) with linear interpolation over n values read through `get(i)`; also returns the
-// two ranks' source positions and the interpolation fraction (for the backward pass)
+// two ranks' source positions and the interpolation fraction (for the backward pass).  Ties rank by position, as a
+// stable sort orders them.  Any NaN makes the median NaN, as torch.quantile does: it sorts NaN last and takes the last
+// sorted value, so both positions are the last NaN's and the fraction is 0.
 template <typename Get>
 __device__ float median_interp(int n, Get get, int* lo_src, int* hi_src, float* frac) {
+  for (int i = n - 1; i >= 0; --i) {
+    const float vi = get(i);
+    if (isnan(vi)) {
+      *lo_src = *hi_src = i;
+      *frac = 0.f;
+      return vi;
+    }
+  }
   const float pos = 0.5f * (float)(n - 1);
   const int lo = (int)floorf(pos), hi = (int)ceilf(pos);
   float vlo = 0.f, vhi = 0.f;
@@ -566,7 +587,7 @@ __device__ float pca_loss_clip(const float* __restrict__ kp, int T, int K, const
     const int row = i / (D / 2), pr = i - row * (D / 2);
     const float rx = pca_residual(X, proj, row, 2 * pr, D, d);
     const float ry = pca_residual(X, proj, row, 2 * pr + 1, D, d);
-    acc += fmaxf(sqrtf(rx * rx + ry * ry) - d.eps, 0.f);  // rectify_epsilon, losses.py:125-136
+    acc += relu_keep_nan(sqrtf(rx * rx + ry * ry) - d.eps);  // rectify_epsilon, losses.py:125-136
   }
   acc = block_sum_ul(acc, red);
   return acc / (float)npairs;
@@ -592,7 +613,7 @@ __global__ void __launch_bounds__(UL_THREADS) unsup_losses_fwd_kernel(const floa
       const float dy = kp[((size_t)(t + 1) * K + k) * 2 + 1] - kp[((size_t)t * K + k) * 2 + 1];
       float d = sqrtf(dx * dx + dy * dy);
       if (cf && (cf[(size_t)t * K + k] < thr || cf[(size_t)(t + 1) * K + k] < thr)) d = 0.f;  // losses.py:636-649
-      acc += fmaxf(d - teps[k], 0.f);
+      acc += relu_keep_nan(d - teps[k]);
     }
     acc = block_sum_ul(acc, red);
     lt = acc / (float)((T - 1) * K);
@@ -630,7 +651,9 @@ __device__ void pca_loss_clip_bwd(const float* __restrict__ kp, int T, int K, co
     const float rx = pca_residual(X, proj, row, 2 * pr, D, d);
     const float ry = pca_residual(X, proj, row, 2 * pr + 1, D, d);
     const float e = sqrtf(rx * rx + ry * ry);
-    const float s = (e > d.eps && e > 0.f) ? g / e : 0.f;
+    // autograd: relu passes the gradient where e > eps and where e is NaN, and the norm's backward (r / e) g is 0 at
+    // e == 0; a NaN e makes both entries NaN (not only the NaN coordinate's)
+    const float s = (isnan(e) || (e > d.eps && e > 0.f)) ? g / e : 0.f;
     gr[(size_t)row * D + 2 * pr] = rx * s;
     gr[(size_t)row * D + 2 * pr + 1] = ry * s;
   }
@@ -703,7 +726,15 @@ __global__ void __launch_bounds__(UL_THREADS) unsup_losses_bwd_kernel(const floa
       const float dy = kp[((size_t)(t + 1) * K + k) * 2 + 1] - kp[((size_t)t * K + k) * 2 + 1];
       const float d = sqrtf(dx * dx + dy * dy);
       const bool masked = cf && (cf[(size_t)t * K + k] < thr || cf[(size_t)(t + 1) * K + k] < thr);
-      if (!masked && d > teps[k] && d > 0.f) {
+      if (isnan(d)) {
+        // autograd: the norm's backward (dx, dy) * (g / d) is NaN in both coordinates, whatever the mask and the
+        // rectification pass on (a masked pair gets 0 * NaN)
+        const float nan = __int_as_float(0x7fc00000);
+        atomicAdd(&gkp[((size_t)(t + 1) * K + k) * 2], nan);
+        atomicAdd(&gkp[((size_t)(t + 1) * K + k) * 2 + 1], nan);
+        atomicAdd(&gkp[((size_t)t * K + k) * 2], nan);
+        atomicAdd(&gkp[((size_t)t * K + k) * 2 + 1], nan);
+      } else if (!masked && d > teps[k] && d > 0.f) {
         const float sx = g * dx / d, sy = g * dy / d;
         atomicAdd(&gkp[((size_t)(t + 1) * K + k) * 2], sx);
         atomicAdd(&gkp[((size_t)(t + 1) * K + k) * 2 + 1], sy);
@@ -723,7 +754,8 @@ __global__ void __launch_bounds__(UL_THREADS) unsup_losses_bwd_kernel(const floa
 static int make_pca_dev(const lpb_pca_desc* d, int K, PcaDev* out, const char* name) {
   PcaDev p{};
   if (d && d->n_sel > 0) {
-    LPB_REQUIRE(d->kp_index && d->mean && d->kept, "%s: null pointer in pca desc", name);
+    // no components: the reprojection is the mean and `kept` (0 x D, an empty tensor's null pointer) is never read
+    LPB_REQUIRE(d->kp_index && d->mean && (d->kept || d->n_components == 0), "%s: null pointer in pca desc", name);
     LPB_REQUIRE(d->n_sel <= UL_MAX_SEL * 4 && d->n_components >= 0 && d->n_views >= 0 && d->n_views <= 32,
                 "%s: bad pca desc n_sel=%d n_components=%d n_views=%d", name, d->n_sel, d->n_components, d->n_views);
     LPB_REQUIRE(d->centering >= 0 && d->centering <= 2 && !(d->n_views > 0 && d->centering != 0),

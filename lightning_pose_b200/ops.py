@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import NamedTuple
 
+import numpy as np
 import torch
 
 import torch.utils._pytree
@@ -1165,6 +1166,10 @@ class PcaParams:
     """Device-side parameters of one PCA loss (mirror of ``lpb_pca_desc``)."""
 
     def __init__(self, kp_index, n_sel, n_views, centering, mean, kept, epsilon, device):
+        # the index range stays on the host, so that unsup_losses can check it against K without a device sync
+        idx = np.asarray(kp_index).reshape(-1)
+        self.kp_index_min = int(idx.min()) if idx.size else 0
+        self.kp_index_max = int(idx.max()) if idx.size else -1
         self.kp_index = torch.as_tensor(kp_index, dtype=torch.int32, device=device).contiguous()
         self.mean = torch.as_tensor(mean, dtype=torch.float32, device=device).contiguous()
         self.kept = torch.as_tensor(kept, dtype=torch.float32, device=device).contiguous().reshape(-1, self.mean.numel())
@@ -1214,7 +1219,13 @@ def unsup_losses(keypoints, confidences=None, temporal_eps=None, prob_threshold=
     """One launch for the unsupervised loss stack.  keypoints (n_clips, T, 2K) or (T, 2K).
 
     Returns (n_clips, 4) = [temporal, pca_singleview, pca_multiview, 0] per clip (or (4,) for 2-D input).
+    A NaN keypoint makes the losses that read it NaN, as in the reference.
     """
+    k = keypoints.shape[-1] // 2
+    for name, p in (("pca_singleview", pca_singleview), ("pca_multiview", pca_multiview)):
+        if p is not None and p.n_sel > 0 and (p.kp_index_min < 0 or p.kp_index_max >= k):
+            raise ValueError(f"{name}: keypoint indices span [{p.kp_index_min}, {p.kp_index_max}], outside [0, {k}) "
+                             f"for {k} keypoints")
     kp = _cuda_f32(keypoints, "keypoints_pred")
     squeeze = kp.dim() == 2
     if squeeze:
