@@ -556,10 +556,10 @@ inline unsigned n_blocks(int64_t n, int threads) { return (unsigned)((n + thread
 extern "C" int lpb_triangulate_pairs_fwd(const float* points, const float* intrinsics, const float* extrinsics, const float* dist,
                                          int B, int V, int K, int P, float* out, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(points && intrinsics && extrinsics && dist && out, "triangulate_pairs_fwd: null pointer");
   CAM_CHECK_SHAPE("triangulate_pairs_fwd", V, K, P, 2);
   const int64_t n = (int64_t)B * (V * (V - 1) / 2) * K;
-  if (n == 0) return LPB_OK;
+  if (n == 0) return LPB_OK;  // an empty batch reads and writes nothing: its tensors may have no storage
+  LPB_REQUIRE(points && intrinsics && extrinsics && dist && out, "triangulate_pairs_fwd: null pointer");
   triangulate_fwd_kernel<<<n_blocks(n, CAM_THREADS), CAM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(points, intrinsics, extrinsics,
                                                                                                            dist, B, V, K, P, out);
   LPB_CUDA(cudaGetLastError());
@@ -569,10 +569,10 @@ extern "C" int lpb_triangulate_pairs_fwd(const float* points, const float* intri
 extern "C" int lpb_triangulate_pairs_bwd(const float* points, const float* intrinsics, const float* extrinsics, const float* dist,
                                          const float* grad_out, int B, int V, int K, int P, float* grad_points, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(points && intrinsics && extrinsics && dist && grad_out && grad_points, "triangulate_pairs_bwd: null pointer");
   CAM_CHECK_SHAPE("triangulate_pairs_bwd", V, K, P, 2);
   const int64_t n = (int64_t)B * V * K;
   if (n == 0) return LPB_OK;
+  LPB_REQUIRE(points && intrinsics && extrinsics && dist && grad_out && grad_points, "triangulate_pairs_bwd: null pointer");
   triangulate_bwd_kernel<<<n_blocks(n, CAM_THREADS), CAM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       points, intrinsics, extrinsics, dist, grad_out, B, V, K, P, grad_points);
   LPB_CUDA(cudaGetLastError());
@@ -583,11 +583,11 @@ extern "C" int lpb_project_points_fwd(const float* points3d, int n_pairs, const 
                                       const float* dist, const float* bbox, float model_height, float model_width, int B, int V,
                                       int K, int P, float* out, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(points3d && intrinsics && extrinsics && dist && out, "project_points_fwd: null pointer");
   CAM_CHECK_SHAPE("project_points_fwd", V, K, P, 1);
   LPB_REQUIRE(n_pairs >= 0 && (!bbox || (model_height > 0.f && model_width > 0.f)), "project_points_fwd: bad n_pairs or model size");
   const int64_t n = (int64_t)B * V * K;
   if (n == 0) return LPB_OK;
+  LPB_REQUIRE(points3d && intrinsics && extrinsics && dist && out, "project_points_fwd: null pointer");
   project_fwd_kernel<<<n_blocks(n, CAM_THREADS), CAM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       points3d, n_pairs, intrinsics, extrinsics, dist, bbox, model_height, model_width, B, V, K, P, out);
   LPB_CUDA(cudaGetLastError());
@@ -598,11 +598,11 @@ extern "C" int lpb_project_points_bwd(const float* points3d, int n_pairs, const 
                                       const float* dist, const float* bbox, float model_height, float model_width,
                                       const float* grad_out, int B, int V, int K, int P, float* grad_points3d, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(points3d && intrinsics && extrinsics && dist && grad_out && grad_points3d, "project_points_bwd: null pointer");
   CAM_CHECK_SHAPE("project_points_bwd", V, K, P, 1);
   LPB_REQUIRE(n_pairs >= 0 && (!bbox || (model_height > 0.f && model_width > 0.f)), "project_points_bwd: bad n_pairs or model size");
   const int64_t n = (int64_t)B * K;
   if (n == 0) return LPB_OK;
+  LPB_REQUIRE(points3d && intrinsics && extrinsics && dist && grad_out && grad_points3d, "project_points_bwd: null pointer");
   project_bwd_kernel<<<n_blocks(n, CAM_THREADS), CAM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       points3d, n_pairs, intrinsics, extrinsics, dist, bbox, model_height, model_width, grad_out, B, V, K, P, grad_points3d);
   LPB_CUDA(cudaGetLastError());
@@ -612,10 +612,10 @@ extern "C" int lpb_project_points_bwd(const float* points3d, int n_pairs, const 
 extern "C" int lpb_frame_to_model(const float* keypoints, int B, int V, int K, const float* bbox, float model_height, float model_width,
                                   int grad, float* out, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(keypoints && bbox && out, "frame_to_model: null pointer");
   LPB_REQUIRE(B >= 0 && V >= 1 && K >= 1 && model_height > 0.f && model_width > 0.f, "frame_to_model: bad shape");
   const int64_t n = (int64_t)B * V * K;
   if (n == 0) return LPB_OK;
+  LPB_REQUIRE(keypoints && bbox && out, "frame_to_model: null pointer");
   frame_to_model_kernel<<<n_blocks(n, CAM_THREADS), CAM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(keypoints, B, V, K, bbox,
                                                                                                           model_height, model_width, grad, out);
   LPB_CUDA(cudaGetLastError());
@@ -625,9 +625,10 @@ extern "C" int lpb_frame_to_model(const float* keypoints, int B, int V, int K, c
 extern "C" int lpb_pairwise_projections_loss_fwd(const float* targets, const float* preds, int B, int n_pairs, int K, float* out,
                                                  void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(targets && preds && out, "pairwise_projections_loss_fwd: null pointer");
   LPB_REQUIRE(B >= 0 && n_pairs >= 1 && K >= 1, "pairwise_projections_loss_fwd: bad shape");
-  ppl_fwd_kernel<<<1, PPL_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(targets, preds, (int64_t)B * n_pairs * K, n_pairs, K, out);
+  const int64_t n = (int64_t)B * n_pairs * K;
+  LPB_REQUIRE(out && (n == 0 || (targets && preds)), "pairwise_projections_loss_fwd: null pointer");  // B = 0: writes 0, 0
+  ppl_fwd_kernel<<<1, PPL_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(targets, preds, n, n_pairs, K, out);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
@@ -635,10 +636,10 @@ extern "C" int lpb_pairwise_projections_loss_fwd(const float* targets, const flo
 extern "C" int lpb_pairwise_projections_loss_bwd(const float* targets, const float* preds, int B, int n_pairs, int K, const float* fwd_out,
                                                  const float* grad_out, float* grad_preds, void* stream) {
   using namespace lpb;
-  LPB_REQUIRE(targets && preds && fwd_out && grad_out && grad_preds, "pairwise_projections_loss_bwd: null pointer");
   LPB_REQUIRE(B >= 0 && n_pairs >= 1 && K >= 1, "pairwise_projections_loss_bwd: bad shape");
   const int64_t n = (int64_t)B * n_pairs * K;
   if (n == 0) return LPB_OK;
+  LPB_REQUIRE(targets && preds && fwd_out && grad_out && grad_preds, "pairwise_projections_loss_bwd: null pointer");
   ppl_bwd_kernel<<<n_blocks(n, CAM_THREADS), CAM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(targets, preds, n, n_pairs, K, fwd_out,
                                                                                                    grad_out, grad_preds);
   LPB_CUDA(cudaGetLastError());

@@ -1326,6 +1326,9 @@ def project_points(points_3d, intrinsics, extrinsics, dist, mean_over_pairs=Fals
     ``mean_over_pairs``: ``points_3d`` is (B, pairs, K, 3) and is averaged over the pair axis first (NaN-propagating, as
     ``torch.mean(dim=1)``).  ``bbox`` (B, 4V) with ``model_size`` (height, width): the result is in model coordinates
     (``frame_to_model``).  One launch each way; differentiable in ``points_3d``."""
+    if mean_over_pairs and points_3d.dim() == 4 and points_3d.shape[1] == 0:
+        # the kernels read n_pairs = 0 as "no pair axis": a zero-width slice would project its parent's first points
+        raise ValueError(f"points_3d has no pairs to average over: {tuple(points_3d.shape)}")
     p3 = _cuda_f32(points_3d, "points_3d")
     if p3.shape[-1] != 3 or p3.dim() != (4 if mean_over_pairs else 3):
         raise ValueError(f"points_3d must be {'(batch, pairs, num_keypoints, 3)' if mean_over_pairs else '(batch, num_keypoints, 3)'}; got {tuple(p3.shape)}")
