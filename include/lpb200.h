@@ -678,6 +678,38 @@ int lpb_pairwise_projections_loss_fwd(const float* targets, const float* preds, 
 int lpb_pairwise_projections_loss_bwd(const float* targets, const float* preds, int B, int n_pairs, int K, const float* fwd_out,
                                       const float* grad_out, float* grad_preds, void* stream);
 
+/* ---- coordinate-regression models (csrc/regression.cu) -------------------------------------------
+ * replaces LinearRegressionHead.forward  lightning_pose/models/heads/regression.py:29-43, with the backbone's avgpool in
+ * front of it (lightning_pose/models/backbones/factory.py:324 keeps torchvision's pool for regression)
+ *   features [B, C, H, W] in the LPB_OUT_* element format `format` (fp32, bf16 or fp16), layout LPB_FEATURES_NCHW or
+ *   LPB_FEATURES_NHWC (channels-last, [B, H, W, C] in memory); weight [n_out, C] fp32, bias [n_out] fp32.
+ *   pooled [B, C] fp32: the mean over the H W pixels, summed in fp32 in a fixed order (the backward reads it);
+ *   out [B, n_out] fp32 = pooled weight^T + bias.  Each feature byte is read once.  With H = W = 1 this is the
+ *   reference's head exactly (features.reshape(B, C), then nn.Linear). */
+int lpb_regression_head_fwd(const void* features, int format, int layout, int B, int C, int H, int W, const float* weight,
+                            const float* bias, int n_out, float* pooled, float* out, void* stream);
+/* grad_out [B, n_out] fp32.  dweight [n_out, C] and dbias [n_out] (both or neither) are overwritten with fixed-order sums
+ * over the frames (no float atomics: the same bits from run to run).  dfeatures (NULL: not wanted) is overwritten with
+ * (grad_out weight) / (H W) broadcast over the pixels, in the format and layout of the features, each element written
+ * once; it needs workspace, B x C floats of device scratch. */
+int lpb_regression_head_bwd(const float* grad_out, const float* pooled, const float* weight, int format, int layout, int B, int C,
+                            int H, int W, int n_out, void* dfeatures, float* dweight, float* dbias, float* workspace,
+                            void* stream);
+
+/* replaces RegressionMSELoss.__call__ and RegressionRMSELoss.__call__ (remove_nans + compute_loss + mean)
+ *   lightning_pose/losses/losses.py:880-996
+ * targets, preds [n] fp32 (the (B, 2K) keypoint tensors), one CTA, no host sync.  out[4] =
+ *   {mse, kept, rmse, pairs}: mse = mean of (t - p)^2 over the entries whose target is not NaN (NaN when none is);
+ *   rmse = the reference's diagnostic: the kept squared errors compacted in order, paired as (x, y) (so an entry with
+ *   only x NaN shifts the pairing of every later one, as reshape(-1, 2) does there), mean over the pairs of
+ *   sqrt(pair mean); NaN when no entry is kept or their number is odd (where the reference's reshape raises).
+ *   kept / pairs are the counts, exact up to 2^24.  A NaN prediction at a kept entry makes both losses NaN. */
+int lpb_regression_losses_fwd(const float* targets, const float* preds, int64_t n, float* out, void* stream);
+/* d mse / d preds given grad_out [1] (the rmse is a diagnostic: it gets no gradient); fwd_out = the forward's out;
+ * grad_preds [n] is overwritten, 0 at the dropped entries. */
+int lpb_regression_losses_bwd(const float* targets, const float* preds, int64_t n, const float* fwd_out, const float* grad_out,
+                              float* grad_preds, void* stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * Tensor-core operand self-test (bring-up aid): one-CTA GEMM over operands in the library's row layout
  * [kchunk][row][8] bf16; mode 0 = K-major view, 1 = MN-major view; d [128][n] fp32.  col_off has no effect

@@ -129,6 +129,10 @@ SIGNATURES = {
     "lpb_frame_to_model": (C.c_int, [_P, _I, _I, _I, _P, _F, _F, _I, _P, _P]),
     "lpb_pairwise_projections_loss_fwd": (C.c_int, [_P, _P, _I, _I, _I, _P, _P]),
     "lpb_pairwise_projections_loss_bwd": (C.c_int, [_P, _P, _I, _I, _I, _P, _P, _P, _P]),
+    "lpb_regression_head_fwd": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _P]),
+    "lpb_regression_head_bwd": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "lpb_regression_losses_fwd": (C.c_int, [_P, _P, _L, _P, _P]),
+    "lpb_regression_losses_bwd": (C.c_int, [_P, _P, _L, _P, _P, _P, _P]),
 }
 
 

@@ -16,9 +16,11 @@ is one fused CUDA reduction (``csrc/losses.cu``) that produces the same scalar:
 * ``ReprojectionHeatmapLoss``       -> ``ops.generate_heatmaps`` (differentiable) + ``ops.heatmap_loss``, or
                                        ``ops.heatmap_loss_from_keypoints("mse")`` given ``GaussianTargets``
 * ``PairwiseProjectionsLoss``       -> ``ops.pairwise_projections_loss`` (NaN entries dropped on device)
+* ``RegressionMSELoss``             -> ``ops.regression_losses`` on CUDA inputs (NaN targets dropped on device, one
+                                       launch with the RMSE diagnostic; the regression trackers share it)
 
-The staged methods remain as small tensor utilities for callers/tests that use them directly; the
-coordinate-regression losses (not on the heatmap path) are plain tensor code.
+The staged methods remain as small tensor utilities for callers/tests that use them directly.
+``RegressionRMSELoss``, the always-on diagnostic of the heatmap trackers, keeps the staged tensor code.
 """
 from __future__ import annotations
 
@@ -351,9 +353,16 @@ class TemporalHeatmapLoss(Loss):
 
 
 # --------------------------------------------------------------------------------------
-# coordinate-regression losses: not on the heatmap hot path, kept as surface (SURVEY 2 row 3)
+# coordinate-regression losses (reference :857-996)
 # --------------------------------------------------------------------------------------
+FUSED_REGRESSION_KEY = "_lpb_fused_regression"  # a regression tracker passes its one-launch (mse, kept, rmse, pairs)
+
+
 class RegressionMSELoss(Loss):
+    """Mean of (t - p)^2 over the non-NaN target entries.  ``__call__`` on CUDA tensors is one device reduction
+    (``ops.regression_losses``: no data-dependent shapes, no host sync, capturable); on CPU tensors it is the staged
+    ``remove_nans`` / ``compute_loss`` / ``reduce_loss`` pipeline."""
+
     loss_name = "regression"
 
     def __init__(self, data_module=None, epsilon: float = 0.0, log_weight: float = 0.0, **kwargs: Any) -> None:
@@ -373,19 +382,38 @@ class RegressionMSELoss(Loss):
         stage: Literal["train", "val", "test"] | None = None,
         **kwargs: Any,
     ) -> LossOutput:
+        fused = kwargs.get(FUSED_REGRESSION_KEY)
+        if fused is None and keypoints_pred.is_cuda:
+            fused = ops.regression_losses(keypoints_targ, keypoints_pred)
+        if fused is not None:
+            scalar_loss = fused[0]
+            return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
+        return self._staged_call(keypoints_targ, keypoints_pred, stage)
+
+    def _staged_call(self, keypoints_targ: torch.Tensor, keypoints_pred: torch.Tensor, stage) -> LossOutput:
         t, p = self.remove_nans(targets=keypoints_targ, predictions=keypoints_pred)
         scalar_loss = self.reduce_loss(self.compute_loss(targets=t, predictions=p), method="mean")
         return scalar_loss, self.log_loss(loss=scalar_loss, stage=stage)
 
 
 class RegressionRMSELoss(RegressionMSELoss):
-    """Per-keypoint Euclidean pixel error; the always-on diagnostic of every tracker."""
+    """Per-keypoint Euclidean pixel error; the always-on diagnostic of every tracker.  Staged tensor code on every
+    device (a regression tracker reads the same value from its one-launch ``ops.regression_losses`` instead)."""
 
     loss_name = "rmse"
 
     def compute_loss(self, targets: torch.Tensor, predictions: torch.Tensor) -> torch.Tensor:
         d2 = (targets.reshape(-1, 2) - predictions.reshape(-1, 2)) ** 2
         return torch.sqrt(d2.mean(dim=1))
+
+    def __call__(
+        self,
+        keypoints_targ: torch.Tensor,
+        keypoints_pred: torch.Tensor,
+        stage: Literal["train", "val", "test"] | None = None,
+        **kwargs: Any,
+    ) -> LossOutput:
+        return self._staged_call(keypoints_targ, keypoints_pred, stage)
 
 
 class PairwiseProjectionsLoss(Loss):

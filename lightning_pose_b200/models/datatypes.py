@@ -9,7 +9,8 @@ from typing import TypedDict
 
 import torch
 
-__all__ = ["HeatmapTrackerLabeledOutputsDict", "HeatmapTrackerUnlabeledOutputsDict"]
+__all__ = ["HeatmapTrackerLabeledOutputsDict", "HeatmapTrackerUnlabeledOutputsDict", "RegressionTrackerLabeledOutputsDict",
+           "RegressionTrackerUnlabeledOutputsDict"]
 
 
 class HeatmapTrackerLabeledOutputsDict(TypedDict):
@@ -25,3 +26,12 @@ class HeatmapTrackerUnlabeledOutputsDict(TypedDict):
     keypoints_pred: torch.Tensor  # (seq, 2K) in frame coordinates, augmentation undone
     keypoints_pred_augmented: torch.Tensor  # (seq, 2K) matching heatmaps_pred
     confidences: torch.Tensor  # (seq, K)
+
+
+class RegressionTrackerLabeledOutputsDict(TypedDict):
+    keypoints_targ: torch.Tensor  # (batch, 2K) model pixels
+    keypoints_pred: torch.Tensor  # (batch, 2K) model pixels
+
+
+class RegressionTrackerUnlabeledOutputsDict(TypedDict):
+    keypoints_pred: torch.Tensor  # (seq, 2K), augmentation undone

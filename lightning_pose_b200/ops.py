@@ -40,6 +40,8 @@ __all__ = [
     "project_points",
     "frame_to_model",
     "pairwise_projections_loss",
+    "regression_head",
+    "regression_losses",
 ]
 
 _KIND = {"mse": 0, "kl": 1, "js": 2}
@@ -1409,3 +1411,94 @@ def pairwise_projections_loss(targets, preds, return_count=False):
         raise ValueError(f"targets (batch, num_keypoints, 3) vs predictions (batch, pairs, num_keypoints, 3): {tuple(t.shape)} / {tuple(p.shape)}")
     loss, count = _PairwiseProjectionsLoss.apply(t, p)
     return (loss, count) if return_count else loss
+
+
+# =====================================================================================
+# coordinate-regression models (csrc/regression.cu)
+# =====================================================================================
+_FEATURE_FORMAT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}  # LPB_OUT_* (lpb200.h)
+
+
+class _RegressionHead(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, features, layout, weight, bias):
+        b, c, h, w = features.shape
+        n = weight.shape[0]
+        pooled = torch.empty((b, c), device=features.device, dtype=torch.float32)
+        out = torch.empty((b, n), device=features.device, dtype=torch.float32)
+        fmt = _FEATURE_FORMAT[features.dtype]
+        with torch.cuda.device(features.device):
+            check(lib.lpb_regression_head_fwd(_ptr(features), fmt, layout, b, c, h, w, _ptr(weight), _ptr(bias), n, _ptr(pooled),
+                                              _ptr(out), _stream()))
+        ctx.save_for_backward(pooled, weight)
+        ctx.meta = (fmt, layout, tuple(features.shape), features.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        pooled, weight = ctx.saved_tensors
+        fmt, layout, (b, c, h, w), dtype = ctx.meta
+        n = weight.shape[0]
+        g = g.contiguous().float()
+        dfeat = dw = db = ws = None
+        if ctx.needs_input_grad[0]:
+            memory = torch.channels_last if layout == FEATURES_NHWC else torch.contiguous_format
+            dfeat = torch.empty((b, c, h, w), device=g.device, dtype=dtype, memory_format=memory)
+            ws = torch.empty((b, c), device=g.device, dtype=torch.float32)
+        if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+            dw, db = torch.empty_like(weight), torch.empty((n,), device=g.device, dtype=torch.float32)
+        with torch.cuda.device(g.device):
+            check(lib.lpb_regression_head_bwd(_ptr(g), _ptr(pooled), _ptr(weight), fmt, layout, b, c, h, w, n, _ptr(dfeat), _ptr(dw),
+                                              _ptr(db), _ptr(ws), _stream()))
+        return dfeat, None, dw, db
+
+
+def regression_head(features, weight, bias):
+    """``mean over (h, w) of features`` then ``nn.Linear``: (B, C, h, w) -> (B, N) fp32, forward and both gradients in
+    ``liblpb200.so``.  Features in bf16, fp16 or fp32, NCHW or channels-last (read in place, ``feature_layout``); the
+    gradient comes back in the same dtype and layout.  Differentiable in features, weight and bias."""
+    if not isinstance(features, torch.Tensor) or not features.is_cuda:
+        raise RuntimeError("lpb200: `features` must be a CUDA tensor (this package has no CPU fallback)")
+    if features.dim() != 4:
+        raise ValueError(f"features must be (batch, channels, height, width); got {tuple(features.shape)}")
+    if features.dtype not in _FEATURE_FORMAT:
+        raise ValueError(f"features must be float32, bfloat16 or float16; got {features.dtype}")
+    if weight.dim() != 2 or weight.shape[1] != features.shape[1] or bias.shape != (weight.shape[0],):
+        raise ValueError(f"weight (N, C) / bias (N,) for C = {features.shape[1]}: {tuple(weight.shape)} / {tuple(bias.shape)}")
+    layout = feature_layout(features)
+    f = features if layout == FEATURES_NHWC else features.contiguous()
+    return _RegressionHead.apply(f, layout, _cuda_f32(weight, "weight"), _cuda_f32(bias, "bias"))
+
+
+class _RegressionLosses(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, targ, pred):
+        out = torch.empty((4,), device=pred.device, dtype=torch.float32)
+        with torch.cuda.device(pred.device):
+            check(lib.lpb_regression_losses_fwd(_ptr(targ), _ptr(pred), pred.numel(), _ptr(out), _stream()))
+        ctx.save_for_backward(targ, pred, out)
+        mse, kept, rmse, pairs = (out[i].clone() for i in range(4))
+        ctx.mark_non_differentiable(kept, rmse, pairs)
+        return mse, kept, rmse, pairs
+
+    @staticmethod
+    def backward(ctx, g, _g_kept, _g_rmse, _g_pairs):
+        targ, pred, out = ctx.saved_tensors
+        gp = torch.empty_like(pred)
+        gg = g.reshape(1).contiguous().float()
+        with torch.cuda.device(pred.device):
+            check(lib.lpb_regression_losses_bwd(_ptr(targ), _ptr(pred), pred.numel(), _ptr(out), _ptr(gg), _ptr(gp), _stream()))
+        return None, gp
+
+
+def regression_losses(targets, preds):
+    """``(mse, kept, rmse, pairs)`` of (B, 2K) keypoint targets and predictions in one launch, with no host sync.
+
+    ``mse``: mean of (t - p)^2 over the entries whose target is not NaN (NaN when there is none), differentiable in
+    ``preds``.  ``rmse``: the reference's diagnostic, the kept squared errors compacted in order and paired as (x, y),
+    mean of sqrt(pair mean); NaN when nothing is kept or an odd number is.  ``kept`` / ``pairs``: the counts."""
+    t = _cuda_f32(targets, "keypoints_targ").detach()
+    p = _cuda_f32(preds, "keypoints_pred")
+    if t.shape != p.shape:
+        raise ValueError(f"keypoint targets {tuple(t.shape)} and predictions {tuple(p.shape)} differ in shape")
+    return _RegressionLosses.apply(t, p)

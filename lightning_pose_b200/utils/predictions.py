@@ -248,6 +248,10 @@ class BatchedPredictor:
     ``lpb_pack_predictions``; view v owns columns [3 K v, 3 K (v + 1)), the reference's per-view split
     (``view_tables``, ``PredictionHandler.dataframes``).
 
+    Regression body (``LinearRegressionHead``, one view; reference ``RegressionTracker.predict_step``): head ->
+    ``lpb_pack_predictions`` with a likelihood of 0.0, the reference's zeros, and the keypoints in model pixels as
+    ``predict_step`` returns them (it has no model -> frame remap).  A ``bbox``, crop mode and more than one view raise.
+
     Context body (``HeatmapMHCRNNHead``, one view; reference ``HeatmapTrackerMHCRNN.predict_step`` over windows of
     S = T + 4 frames with step T, ``dali.context.predict.sequence_length``): T counts NEW frames; chunk j yields frames
     j T - 2 .. j T + T - 3.  The two / four frames before a chunk stay on the device (their single-frame decode, boxes
@@ -276,10 +280,16 @@ class BatchedPredictor:
                  crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False, num_views: int = 1,
                  shard: tuple[int, int] = (0, 1)) -> None:
         from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
+        from lightning_pose_b200.models.heads.regression import LinearRegressionHead
 
         self.head, self.k, self.n_frames, self.chunk = head, int(num_keypoints), int(n_frames), int(chunk)
         self.context = isinstance(head, HeatmapMHCRNNHead)
+        self.regression = isinstance(head, LinearRegressionHead)
         self.num_views = int(num_views)
+        if self.regression and self.num_views > 1:
+            raise ValueError("multiview prediction is not supported for regression models")
+        if self.regression and bboxes is not None:
+            raise ValueError("bbox cropping is not supported for regression models")
         if self.context and self.num_views > 1:
             raise ValueError("context prediction is not supported for multiview models")
         if self.context and self.n_frames < 5:
@@ -321,6 +331,8 @@ class BatchedPredictor:
             if self.bboxes.shape[0] != self.n_frames:
                 raise ValueError(f"bboxes has {self.bboxes.shape[0]} rows but the video has {self.n_frames} frames")
             self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
+        if self.regression:  # the likelihood column
+            self._zero_conf = torch.zeros((self.chunk, self.k), dtype=torch.float32, device=self.device)
         if self.context:  # the halo buffers; the maps' are sized by the first chunk's maps
             t, k, dev = self.chunk, self.k, self.device
             self._wf = self._wb = None
@@ -383,6 +395,8 @@ class BatchedPredictor:
             raise ValueError(f"chunks are fixed-size, ({t * v}, ...) or ({t}, {v}, ...); pad the last one (got {tuple(x.shape)})")
         if bbox is None:
             bbox = self._image_bbox
+        elif self.regression:
+            raise ValueError("a regression model predicts in model pixels (RegressionTracker.predict_step has no bbox remap)")
         elif tuple(bbox.shape) != (t, 4 * v):
             raise ValueError(f"bbox must be ({t}, {4 * v}); got {tuple(bbox.shape)}")
         return "tensor", (x, bbox)
@@ -404,7 +418,7 @@ class BatchedPredictor:
         """One chunk, enqueued on the current stream with no host sync: ingest, features, the body per sub-chunk."""
         x, bbox = self._ingest(form, xs)
         feats = self.features_of(x) if self.features_of is not None else x
-        emit = self._emit_context if self.context else self._emit_frames
+        emit = self._emit_context if self.context else self._emit_regression if self.regression else self._emit_frames
         for i in range(0, self.chunk, self.sub_chunk):
             emit(feats, bbox, i, min(self.sub_chunk, self.chunk - i))
 
@@ -415,6 +429,10 @@ class BatchedPredictor:
         # (n V, 2K) -> (n, 2 V K): the views of a frame side by side, as the trackers fold them
         kp = ops.remap_keypoints(kp.reshape(n, 2 * self.k * v), None, bbox[i : i + n], *self.image_hw, num_views=v)
         ops.pack_predictions(kp, cf.reshape(n, self.k * v), self.table, cursor=self.cursor)
+
+    def _emit_regression(self, feats: torch.Tensor, bbox: torch.Tensor, i: int, n: int) -> None:
+        """Frames [i, i + n) of a regression chunk: pooled linear head -> table rows, likelihood 0.0."""
+        ops.pack_predictions(self.head(feats[i : i + n]), self._zero_conf[:n], self.table, cursor=self.cursor)
 
     def _emit_context(self, feats: torch.Tensor, bbox: torch.Tensor, i: int, n: int) -> None:
         """Frames [i, i + n) of a context chunk: the single-frame head and the W_f / W_b maps into the halo buffers, then
@@ -521,7 +539,8 @@ class FramePredictor:
     """One frame in, its keypoints out, with one CUDA-graph replay per call: the reference's ``Model.predict_frame``
     (``lightning_pose/api/model.py:298-509``) for loops that need each answer before the next camera frame.
 
-    ``head``: a ``HeatmapHead`` or ``HeatmapMHCRNNHead`` on the device, in eval mode; ``features_of`` maps the ingested
+    ``head``: a ``HeatmapHead``, ``HeatmapMHCRNNHead`` or ``LinearRegressionHead`` on the device, in eval mode;
+    ``features_of`` maps the ingested
     (F, 3, h, w) images (channels-last memory with ``channels_last``) to backbone features, e.g. the tracker's
     ``backbone``.  ``image_hw`` is the model's input size (``image_resize_dims``); ``dtype`` / ``channels_last`` the
     ingest's output, what ``features_of`` takes; ``mean`` / ``std`` the normalisation.
@@ -535,7 +554,9 @@ class FramePredictor:
     Body: ``ops.frames_crop_resize_cv2`` (the reference's cv2 resize and numpy normalisation, bit for bit, with the box
     read on the device) -> ``features_of`` -> head -> soft-argmax decode -> model -> frame remap -> one (K, 3) row.  A
     context head runs ``HeatmapTrackerMHCRNN``'s labeled form on (1, 5, 3, h, w) and keeps, per keypoint, the
-    multi-frame prediction where its confidence is greater than the single-frame one (a NaN keeps single-frame).
+    multi-frame prediction where its confidence is greater than the single-frame one (a NaN keeps single-frame).  A
+    regression head maps its model-pixel keypoints to the frame and reports a confidence of 1.0, as the reference's
+    ``predict_frame`` does for regression models (``api/model.py:495-500``; its ``predict_step`` gives zeros instead).
 
     With ``use_graph`` the first call of each input form (host or device frame, frame shape) is captured; a new form
     captures anew and replaces the old graph.  The images' dtype, and with it the features', is fixed per predictor.
@@ -552,12 +573,14 @@ class FramePredictor:
                  device=None, use_graph: bool = True, dtype: torch.dtype = torch.float32, channels_last: bool = False,
                  mean: Sequence[float] = ops.IMAGENET_MEAN, std: Sequence[float] = ops.IMAGENET_STD) -> None:
         from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
+        from lightning_pose_b200.models.heads.regression import LinearRegressionHead
 
         if features_of is None:
             raise ValueError("features_of (images -> backbone features) is required")
         ops._out_format(dtype)
         self.head, self.k = head, int(num_keypoints)
         self.context = isinstance(head, HeatmapMHCRNNHead)
+        self.regression = isinstance(head, LinearRegressionHead)
         self.image_hw = (int(image_hw[0]), int(image_hw[1]))
         self.features_of = features_of
         self.device = torch.device(device) if device is not None else next(head.parameters()).device
@@ -567,6 +590,7 @@ class FramePredictor:
         # the (K, 3) result: a context call writes the one frame of a five-row window to all five rows
         # (lpb_pack_context_predictions with frame0 = 4, step 1), a frame call writes row 0
         self._table = torch.zeros((self.CONTEXT_FRAMES if self.context else 1, 3 * self.k), dtype=torch.float32, device=self.device)
+        self._ones = torch.ones((1, self.k), dtype=torch.float32, device=self.device)  # a regression head's confidence
         self._box = torch.zeros(4, dtype=torch.int32, device=self.device)
         self._pin_box = torch.zeros(4, dtype=torch.int32).pin_memory()
         self._pin_out = torch.zeros((self.k, 3), dtype=torch.float32).pin_memory()
@@ -619,6 +643,9 @@ class FramePredictor:
         if self.channels_last:
             x = x.permute(0, 3, 1, 2)
         feats = self.features_of(x)
+        if self.regression:
+            ops.pack_predictions(ops.remap_keypoints(head(feats), None, bbox, mh, mw), self._ones, self._table, row0=0)
+            return self._table.view(self.k, 3)
         if not self.context:
             _, kp, cf = head.forward_with_keypoints(feats)
             kp = ops.remap_keypoints(kp, None, bbox, mh, mw)
