@@ -58,6 +58,8 @@ int lpb_get_tuning(int key);
  * workspace lpb_decode_fwd_workspace_bytes(n_planes) bytes of device scratch, 4-byte aligned; NULL only when
  *           n_planes == 0.  Only the call's own kernels use it, so one buffer can serve every call on a stream.
  * ds in {1,2,3}.  Evaluation is exact up to a dropped softmax mass < 1e-12 (see DESIGN.md).
+ * temperature >= 0 (0: the uniform softmax); a negative or NaN temperature is LPB_ERR_INVALID here and in both
+ * backward entries, before anything is queued.
  */
 int lpb_decode_prepare(int h, int w, int ds);
 int lpb_decode_fwd_workspace_bytes(int64_t n_planes, size_t* bytes);

@@ -1222,12 +1222,14 @@ static int launch_decode_bwd(const float* heat, const float* stats, const float*
   P.gxy = gxy;
   P.gheat = gheat;
   P.queue = queue;
+  // the dense kernel's shared memory is checked before anything is queued: a refused plane size leaves win, meta,
+  // queue and the gradient untouched
+  const size_t smem = ((size_t)2 * (h + 2 * G::R) * P.pitch + DEC_WARPS * 64) * sizeof(float) + 16;
+  LPB_TRY(set_dynamic_smem(decode_bwd_kernel<DS>, smem, "decode_bwd"));
   if (win) {  // sparse windows first; the dense kernel below then only runs the planes they queued
     LPB_CUDA(cudaMemsetAsync(queue, 0, sizeof(int), stream));
     decode_bwd_window_kernel<DS><<<(unsigned)((n_planes + 3) / 4), 128, 0, stream>>>(P, win, meta, queue);
   }
-  const size_t smem = ((size_t)2 * (h + 2 * G::R) * P.pitch + DEC_WARPS * 64) * sizeof(float) + 16;
-  LPB_TRY(set_dynamic_smem(decode_bwd_kernel<DS>, smem, "decode_bwd"));
   unsigned grid = (unsigned)n_planes;
   if (queue && grid > (unsigned)(2 * dev.sms)) grid = (unsigned)(2 * dev.sms);  // queue mode: one wave of resident CTAs
   decode_bwd_kernel<DS><<<grid, DEC_THREADS, smem, stream>>>(P);
@@ -1261,6 +1263,8 @@ static int decode_fwd_entry(const char* name, const float* heatmaps, int64_t n_p
   LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "%s: bad n_planes", name);
   LPB_REQUIRE(workspace || n_planes == 0, "%s: null workspace", name);
   LPB_REQUIRE(aligned_to(workspace, 4), "%s: workspace must be 4-byte aligned", name);
+  // the online softmax of the CTA kernel starts from a running maximum that assumes T >= 0
+  LPB_REQUIRE(temperature >= 0.f, "%s: temperature %g must be >= 0", name, (double)temperature);
   if (((int64_t)w << ds) > 1024 || w > 256) {
     lpb::set_error("%s: heatmap width %d (x%d) exceeds this build's 1024-column field limit", name, w, 1 << ds);
     return LPB_ERR_UNSUPPORTED;
@@ -1301,6 +1305,7 @@ extern "C" int lpb_decode_bwd(const float* heatmaps, const float* stats, const f
   LPB_REQUIRE(heatmaps && stats && grad_xy && grad_heatmaps, "decode_bwd: null pointer");
   LPB_REQUIRE(h >= 1 && w >= 1 && ds >= 1 && ds <= 3, "decode_bwd: bad shape h=%d w=%d ds=%d", h, w, ds);
   LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "decode_bwd: bad n_planes");
+  LPB_REQUIRE(temperature >= 0.f, "decode_bwd: temperature %g must be >= 0", (double)temperature);
   if (n_planes == 0) return LPB_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   switch (ds) {
@@ -1317,6 +1322,7 @@ extern "C" int lpb_decode_bwd_windows(const float* heatmaps, const float* stats,
   LPB_REQUIRE(heatmaps && stats && grad_xy && win && meta && g_overflow && queue, "decode_bwd_windows: null pointer");
   LPB_REQUIRE(h >= 1 && w >= 1 && ds >= 1 && ds <= 3, "decode_bwd_windows: bad shape h=%d w=%d ds=%d", h, w, ds);
   LPB_REQUIRE(n_planes >= 0 && n_planes < (1ll << 31), "decode_bwd_windows: bad n_planes");
+  LPB_REQUIRE(temperature >= 0.f, "decode_bwd_windows: temperature %g must be >= 0", (double)temperature);
   if (n_planes == 0) return LPB_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   switch (ds) {
