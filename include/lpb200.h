@@ -526,6 +526,28 @@ int lpb_pack_context_predictions(const float* kp_sf, const float* conf_sf, const
                                  float* table, int64_t n_rows, int64_t* cursor, int64_t frame0, int64_t step,
                                  void* stream);
 
+/* ---- batched inference with context (MHCRNN) models over a list of videos ----------------------------------------
+ * replaces, per video, the host stacking / shift of PredictionHandler.unpack_preds + fix_context_preds_confs
+ *   lightning_pose/utils/predictions.py:146-177 (and the selection / model -> frame step as above), for videos fed back
+ *   to back as one frame stream (litpose predict over a video directory, cli/commands/predict.py:236-294).
+ * table [n_rows, 3K] holds the videos back to back: segments [n_segments][3] (device, int64, 8-byte aligned) is
+ * (row0, N, R) per video, R the rows its reader produces at this step (as for lpb_pack_context_predictions);
+ * segments_host is the same table on the host, checked here: row0 of video 0 is 0, each video starts where the previous
+ * one ends, the last ends at n_rows, N >= 5 and R = T * (ceil((N - S) / T) + 1) (N when T = 1).
+ * Output frame i of the call is global frame g = c - 2 + i, c = *cursor (required; advanced by n_frames), frame
+ * f = g - row0 of its video: its selected, remapped prediction goes to every row row0 + r of its video whose source
+ * (the one-video rule with that video's N and R) is f.  Frames 0, 1 and N - 1 of a video, and N - 2 unless R = N - 1,
+ * own no row and are not written: their windows cross into a neighbouring video.
+ * window_index: optional device int32 [step][5], the window table lpb_crnn_combine_fwd reads; when given, the cursor
+ * advance also writes it for the chunk that starts at the new cursor: window i reads map rows i .. i + 4, except that
+ * the window of frame N - 2 of a video with R = N - 1 reads map row step + 4 (the padding frame's maps, which the
+ * caller keeps there) in place of frame N, which is the next video's frame 0.  Pass it on a chunk's last call. */
+int lpb_pack_context_predictions_segments(const float* kp_sf, const float* conf_sf, const float* kp_mf,
+                                          const float* conf_mf, int n_frames, int K, const float* bbox,
+                                          float model_height, float model_width, float* table, int64_t n_rows,
+                                          int64_t* cursor, const int64_t* segments, const int64_t* segments_host,
+                                          int n_segments, int64_t step, int32_t* window_index, void* stream);
+
 /* ---- optimizer step (the tail of a training step) ---------------------------------------------------
  * replaces torch.optim.Adam / AdamW as configured by configure_optimizers  lightning_pose/models/base.py:458-477
  * (no amsgrad).  One launch over up to 16 fp32 tensors; params / grads / exp_avg / exp_avg_sq / numel are HOST arrays

@@ -956,6 +956,51 @@ def pack_context_predictions(kp_sf, conf_sf, kp_mf, conf_mf, bbox, model_height,
     return table
 
 
+def context_segments(lengths, step: int) -> torch.Tensor:
+    """(S, 3) int64 host table (row0, N, R) of videos of ``lengths`` frames back to back, R the rows a context reader of
+    step ``step`` produces for each (what ``lpb_pack_context_predictions_segments`` reads)."""
+    t, rows, row0 = int(step), [], 0
+    for n in (int(v) for v in lengths):
+        rows.append((row0, n, n if t == 1 else t * (-(-(n - t - 4) // t) + 1)))
+        row0 += n
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 3)
+
+
+def pack_context_predictions_segments(kp_sf, conf_sf, kp_mf, conf_mf, bbox, model_height, model_width, table, step, cursor,
+                                      segments, segments_host, window_index=None):
+    """``pack_context_predictions`` for a list of videos back to back in ``table``: ``segments`` is the (S, 3) device
+    copy of ``segments_host`` (``context_segments``).  Each output frame goes to the rows of its own video; frames whose
+    windows cross a video boundary write nothing.  With ``window_index`` ((step, 5) int32 device tensor) the cursor
+    advance also writes the next chunk's window table (see ``lpb_pack_context_predictions_segments``).  Mutates
+    ``table``, ``cursor`` (advanced by T) and ``window_index``."""
+    kps, cfs = _cuda_f32(kp_sf, "kp_sf"), _cuda_f32(conf_sf, "conf_sf")
+    kpm, cfm = _cuda_f32(kp_mf, "kp_mf"), _cuda_f32(conf_mf, "conf_mf")
+    bb = _cuda_f32(bbox, "bbox")
+    t, k = cfs.shape
+    if kps.shape != (t, 2 * k) or kpm.shape != (t, 2 * k) or cfm.shape != (t, k) or bb.shape != (t, 4):
+        raise ValueError(f"shapes: kp_sf {tuple(kps.shape)}, kp_mf {tuple(kpm.shape)} (T, 2K); conf_sf {tuple(cfs.shape)}, "
+                         f"conf_mf {tuple(cfm.shape)} (T, K); bbox {tuple(bb.shape)} (T, 4)")
+    if not isinstance(table, torch.Tensor) or not table.is_cuda:
+        raise RuntimeError("lpb200: `table` must be a CUDA tensor (this package has no CPU fallback)")
+    if table.dtype != torch.float32 or not table.is_contiguous() or table.dim() != 2 or table.shape[1] != 3 * k:
+        raise ValueError(f"table must be contiguous fp32 (N, {3 * k}); got {tuple(table.shape)} {table.dtype}")
+    if cursor is None or not cursor.is_cuda or cursor.dtype != torch.int64 or cursor.numel() != 1:
+        raise ValueError("cursor must be a one-element int64 CUDA tensor")
+    seg_host = segments_host.contiguous()
+    if (not segments.is_cuda or segments.dtype != torch.int64 or not segments.is_contiguous() or seg_host.is_cuda
+            or seg_host.dtype != torch.int64 or segments.dim() != 2 or segments.shape[1] != 3 or seg_host.shape != segments.shape):
+        raise ValueError("segments must be an (S, 3) int64 CUDA tensor and segments_host its (S, 3) int64 host copy")
+    if window_index is not None and (not window_index.is_cuda or window_index.dtype != torch.int32
+                                     or not window_index.is_contiguous() or tuple(window_index.shape) != (int(step), 5)):
+        raise ValueError(f"window_index must be a contiguous ({int(step)}, 5) int32 CUDA tensor")
+    with torch.cuda.device(kps.device):
+        check(lib.lpb_pack_context_predictions_segments(
+            _ptr(kps), _ptr(cfs), _ptr(kpm), _ptr(cfm), t, k, _ptr(bb), float(model_height), float(model_width), _ptr(table),
+            table.shape[0], _ptr(cursor), _ptr(segments), _ptr(seg_host), segments.shape[0], int(step), _ptr(window_index),
+            _stream()))
+    return table
+
+
 def plane_softmax_backward(probs: torch.Tensor, grad_probs: torch.Tensor) -> torch.Tensor:
     p = _cuda_f32(probs, "probs")
     g = _cuda_f32(grad_probs, "grad_probs")

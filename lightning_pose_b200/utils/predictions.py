@@ -16,9 +16,16 @@ feeding ``feed_range``: its own frames, plus for a context model a 2-frame halo 
 all-gather of every rank's rows into the full table on every rank, then the context edge fill
 (``fill_context_edges``): each edge row whose source frame lies in another shard is copied from that frame's own row.
 The gathered table equals the one-GPU table bit for bit.
+
+A list of videos (``n_frames=[N_0, N_1, ...]``, ``litpose predict <model_dir> <video_dir>``) is one frame stream: the
+videos sit back to back in one table and in one chunk sequence, a chunk may hold the end of one video and the start of
+the next, and only the last chunk of the whole list is padded.  ``video_tables()`` gives each video's rows, equal to
+the table a one-video predictor gives that video.
 """
 from __future__ import annotations
 
+import bisect
+import numbers
 import operator
 from typing import Callable, Iterable, Sequence
 
@@ -51,12 +58,54 @@ def _context_source(row: int, n_frames: int, r_rows: int) -> int:
     return row if 2 <= row <= r_rows - 1 else 2
 
 
-def shard_feed_range(n_frames: int, chunk: int, rank: int, world: int, context: bool = False) -> tuple[int, int]:
+def _video_starts(lengths: Sequence[int]) -> list[int]:
+    """row0 of every video of a list, back to back, and the total as the last entry."""
+    starts = [0]
+    for n in lengths:
+        starts.append(starts[-1] + int(n))
+    return starts
+
+
+def _context_window_index(start: int, chunk: int, lengths: Sequence[int]) -> list[list[int]]:
+    """The (T, 5) window table of the context chunk that starts at global frame ``start`` of a list: window i reads map
+    rows i .. i + 4, except that the window of frame N - 2 of a video with R = N - 1 reads the padding frame's maps at
+    row T + 4 in place of frame N, the next video's frame 0 (what the cursor advance of
+    ``lpb_pack_context_predictions_segments`` writes for every later chunk)."""
+    starts, t = _video_starts(lengths), chunk
+    out = []
+    for i in range(t):
+        g, row = start - 2 + i, [i, i + 1, i + 2, i + 3, i + 4]
+        if 0 <= g < starts[-1]:
+            v = bisect.bisect_right(starts, g) - 1
+            n = starts[v + 1] - starts[v]
+            if _context_rows(n, t) == n - 1 and g - starts[v] == n - 2:
+                row[4] = t + 4
+        out.append(row)
+    return out
+
+
+def shard_feed_range(n_frames: int | Sequence[int], chunk: int, rank: int, world: int,
+                     context: bool = False) -> tuple[int, int]:
     """[lo, hi): the frames shard ``rank`` of ``world`` feeds, in chunks of ``chunk`` from frame lo, the last chunk padded
     past hi as the one-GPU caller pads the video's end.  A frame model feeds its own rows' frames.  A context model's
     row f needs frames f - 2 .. f + 2, so its shard feeds a 2-frame halo on each side, clamped to the video.  When
     R = N - 1, row N - 2 reads the first padding frame N: a shard that owns that row starts one frame earlier if its
-    chunks would otherwise end exactly at frame N, so that frame N is fed and frame N - 2 is predicted."""
+    chunks would otherwise end exactly at frame N, so that frame N is fed and frame N - 2 is predicted.
+
+    A list of video lengths: shard ``rank``'s rows of the concatenated table.  A context shard's halo stops at the
+    first frame of the video holding its first row (frames of the previous video reach no row of this one), and at the
+    end of the video holding its last row, plus one frame when that video has R = N - 1: frame N - 2 is then predicted
+    from the padding frame's maps, in the chunk that holds position N, so that position is fed (it may be the list's
+    end: hi is then one past the last frame, a padding frame).  Feed ``ceil((hi - lo) / chunk)`` chunks."""
+    if not isinstance(n_frames, numbers.Integral):
+        starts = _video_starts(n_frames)
+        a, b = frame_range_for_rank(starts[-1], rank, world)
+        if not context or a == b:
+            return a, b
+        first = starts[bisect.bisect_right(starts, a) - 1]
+        v = bisect.bisect_right(starts, b - 1) - 1
+        n = starts[v + 1] - starts[v]
+        return max(a - 2, first), min(b + 2, starts[v + 1] + (_context_rows(n, chunk) == n - 1))
     a, b = frame_range_for_rank(n_frames, rank, world)
     if not context or a == b:
         return a, b
@@ -66,24 +115,30 @@ def shard_feed_range(n_frames: int, chunk: int, rank: int, world: int, context: 
     return lo, hi
 
 
-def context_edge_fill(n_frames: int, chunk: int, world: int) -> list[tuple[int, int]]:
+def context_edge_fill(n_frames: int | Sequence[int], chunk: int, world: int) -> list[tuple[int, int]]:
     """(row, source row) pairs that complete a context table gathered from ``world`` shards: every edge row (0, 1, the
     last four) whose source frame's own row belongs to another shard.  The kernel writes a frame's prediction to all
     its rows, but only the shard that owns the frame's row computes it from the right window; another shard's rows
-    hold a halo frame's prediction (or none) there.  Empty for one shard."""
-    n, per = n_frames, -(-n_frames // max(world, 1))
-    r_rows = _context_rows(n, chunk)
+    hold a halo frame's prediction (or none) there.  Empty for one shard.  A list of video lengths: the edge rows of
+    every video, in rows of the concatenated table."""
+    lengths = [n_frames] if isinstance(n_frames, numbers.Integral) else list(n_frames)
+    starts = _video_starts(lengths)
+    per = -(-starts[-1] // max(world, 1))
     pairs = []
-    for row in sorted({0, 1, *range(max(n - 4, 0), n)}):
-        src = _context_source(row, n, r_rows)
-        if row // per != src // per:
-            pairs.append((row, src))
+    for row0, n in zip(starts, lengths):
+        r_rows = _context_rows(n, chunk)
+        for row in sorted({0, 1, *range(max(n - 4, 0), n)}):
+            src = _context_source(row, n, r_rows)
+            if (row0 + row) // per != (row0 + src) // per:
+                pairs.append((row0 + row, row0 + src))
     return pairs
 
 
-def fill_context_edges(table: torch.Tensor, chunk: int, world: int) -> torch.Tensor:
-    """Apply ``context_edge_fill`` to an (N, 3K) context table on its device, in place (one gather, one scatter)."""
-    pairs = context_edge_fill(table.shape[0], chunk, world)
+def fill_context_edges(table: torch.Tensor, chunk: int, world: int,
+                       lengths: Sequence[int] | None = None) -> torch.Tensor:
+    """Apply ``context_edge_fill`` to an (N, 3K) context table on its device, in place (one gather, one scatter).
+    ``lengths``: the videos of a list table (default: one video of N frames)."""
+    pairs = context_edge_fill(table.shape[0] if lengths is None else lengths, chunk, world)
     if pairs:
         dst, src = (torch.tensor(rows, dtype=torch.int64, device=table.device) for rows in zip(*pairs))
         table.index_copy_(0, dst, table.index_select(0, src))
@@ -172,6 +227,18 @@ class PredictionHandler:
         if table.shape[1] != w * len(self._views()):
             raise ValueError(f"table has {table.shape[1]} columns; {len(self._views())} views of {w} expected")
         return {name: self.dataframe(table[:, w * v : w * (v + 1)], frame_aligned) for v, name in enumerate(self._views())}
+
+    def video_dataframes(self, tables: Sequence[torch.Tensor | np.ndarray], frame_aligned: bool = False) -> list:
+        """One result per video of a list (``BatchedPredictor.video_tables()``): ``dataframe`` of each video's own
+        (N_i, 3K) rows, or with ``view_names`` its ``{view_name: DataFrame}``.  ``frame_count`` is each table's rows."""
+        import copy
+
+        out = []
+        for table in tables:
+            handler = copy.copy(self)
+            handler.frame_count = int(table.shape[0])
+            out.append(handler.dataframes(table, frame_aligned) if self.view_names else handler.dataframe(table, frame_aligned))
+        return out
 
     def __call__(self, preds: Iterable[tuple[torch.Tensor, torch.Tensor]], is_multiview_video: bool = False):
         """Reference call form: a list of per-batch (keypoints, confidences) tuples -> DataFrame, or with
@@ -272,16 +339,37 @@ class BatchedPredictor:
     whose source frame lies in another shard (when R < N frame 2's tail rows [R, N) may be the shard's own), which
     the edge fill overwrites: the fill, not row ownership, is what discards them.  ``gather()`` assembles the table on
     every rank.
+
+    A list of videos (``n_frames`` a sequence ``[N_0, N_1, ...]``; an int is one video): ``table`` has sum(N_i) rows,
+    the videos back to back, and ``video_tables()`` gives each video's (N_i, 3 V K) rows.  The caller feeds the
+    concatenated frame stream (and in crop mode passes the concatenated (sum(N_i), 4) ``bboxes``) in chunks of T, only
+    the last chunk padded: ``n_chunks`` chunks of the stream from ``feed_range[0]``.  One capture serves the whole list.
+    Frame, regression, multi-view and crop bodies follow the cursor as for one video.  The context body writes through
+    ``lpb_pack_context_predictions_segments``, which reads a device table of (row0, N, R) per video: each frame goes to
+    the rows of its own video, frames whose windows cross a video boundary write nothing.  The one window that needs the
+    frame after a video's end (frame N - 2 when R = N - 1) reads the padding frame's W_f / W_b maps, kept in a row after
+    the halo buffers' and pointed to by the window table the writer builds for each chunk: ``pad``, one (...) item of
+    the tensor form (a feature when the caller streams features), or with uint8 views and in crop mode a zero frame.
+    Each video's rows then equal the table of a one-video predictor fed that video with ``pad`` as its padding.  Shards
+    split the concatenated rows (``shard_feed_range`` and ``context_edge_fill`` take the list of lengths).
     """
 
-    def __init__(self, head, num_keypoints: int, n_frames: int, chunk: int, image_hw: tuple[int, int],
+    def __init__(self, head, num_keypoints: int, n_frames: int | Sequence[int], chunk: int, image_hw: tuple[int, int],
                  features_of: Callable[[torch.Tensor], torch.Tensor] | None = None, device=None, use_graph: bool = True,
                  sub_chunk: int | None = None, bboxes: torch.Tensor | None = None, frame_hw: tuple[int, int] | None = None,
                  crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False, num_views: int = 1,
-                 shard: tuple[int, int] = (0, 1)) -> None:
+                 shard: tuple[int, int] = (0, 1), pad: torch.Tensor | None = None) -> None:
         from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
         from lightning_pose_b200.models.heads.regression import LinearRegressionHead
 
+        self.lengths = None  # one video; a list of videos: their frame counts
+        if not isinstance(n_frames, numbers.Integral):
+            self.lengths = [operator.index(n) for n in n_frames]
+            if not self.lengths:
+                raise ValueError("the list of videos is empty")
+            if min(self.lengths) < 1:
+                raise ValueError(f"every video needs at least one frame; got lengths {self.lengths}")
+            n_frames = sum(self.lengths)
         self.head, self.k, self.n_frames, self.chunk = head, int(num_keypoints), int(n_frames), int(chunk)
         self.context = isinstance(head, HeatmapMHCRNNHead)
         self.regression = isinstance(head, LinearRegressionHead)
@@ -294,6 +382,9 @@ class BatchedPredictor:
             raise ValueError("context prediction is not supported for multiview models")
         if self.context and self.n_frames < 5:
             raise ValueError(f"a context model needs at least 5 frames to predict from; the video has {self.n_frames}")
+        if self.context and self.lengths is not None and min(self.lengths) < 5:
+            short = [i for i, n in enumerate(self.lengths) if n < 5]
+            raise ValueError(f"a context model needs at least 5 frames to predict from; videos {short} have fewer")
         if self.chunk < 1:
             raise ValueError(f"chunk must be >= 1; got {self.chunk}")
         if self.num_views < 1:
@@ -303,7 +394,9 @@ class BatchedPredictor:
             raise ValueError(f"shard must be (rank, world) with 0 <= rank < world; got {tuple(shard)}")
         self.shard = (rank, world)
         self.rows = frame_range_for_rank(self.n_frames, rank, world)
-        self.feed_range = shard_feed_range(self.n_frames, self.chunk, rank, world, self.context)
+        self.feed_range = shard_feed_range(self.n_frames if self.lengths is None else self.lengths, self.chunk, rank,
+                                           world, self.context)
+        self.n_chunks = -(-(self.feed_range[1] - self.feed_range[0]) // self.chunk)
         # frames per head / decode call inside a chunk: small enough that the heatmaps written by the head are still in
         # the 126 MB L2 when the decode reads them (None: the whole chunk at once)
         self.sub_chunk = int(sub_chunk) if sub_chunk else self.chunk
@@ -340,7 +433,14 @@ class BatchedPredictor:
             self._cf_sf = torch.zeros((t + 2, k), dtype=torch.float32, device=dev)
             self._box = torch.zeros((t + 2, 4), dtype=torch.float32, device=dev)
             self._idx = (torch.arange(t, device=dev)[:, None] + torch.arange(5, device=dev)[None, :]).to(torch.int32)
-
+            self._segments = self._pad = None
+            if self.lengths is not None:  # the writer's (row0, N, R) table, and the window table of the first chunk
+                self._segments_host = ops.context_segments(self.lengths, t)
+                self._segments = self._segments_host.to(dev)
+                self._idx.copy_(torch.tensor(_context_window_index(self.feed_range[0], t, self.lengths), dtype=torch.int32))
+                # the padding frame's maps are needed when a video has R = N - 1 (computed at the first feed)
+                self._pad = (None if not any(r == n - 1 for _, n, r in self._segments_host.tolist()) else
+                             pad if pad is not None else False)
     def _whole_frames(self, sizes: list[tuple[int, int]]) -> torch.Tensor:
         """(T, 4 V) boxes [0, 0, h, w] of whole frames of the views' ``sizes``."""
         row = [float(s) for h, w in sizes for s in (0, 0, h, w)]
@@ -355,8 +455,42 @@ class BatchedPredictor:
         self.cursor.fill_(self.feed_range[0])
         self.table.zero_()
         if self.context:
-            for buf, _ in self._halo():
-                buf.zero_()
+            for buf, halo in self._halo():
+                buf[: self.chunk + halo].zero_()  # not the padding frame's maps after a list's halo rows
+            if self.lengths is not None:
+                self._idx.copy_(torch.tensor(_context_window_index(self.feed_range[0], self.chunk, self.lengths), dtype=torch.int32))
+
+    def _alloc_maps(self, wf: torch.Tensor) -> None:
+        """The W_f / W_b halo buffers, sized by a chunk's maps: T + 4 rows, and for a list one more for the padding
+        frame's maps."""
+        rows = self.chunk + 4 + (self.lengths is not None)
+        self._wf = torch.zeros((rows, *wf.shape[1:]), dtype=torch.float32, device=self.device)
+        self._wb = torch.zeros_like(self._wf)
+
+    @torch.no_grad()
+    def _pad_maps(self, form: str, xs) -> None:
+        """W_f / W_b of the padding frame into map row T + 4, from a chunk made of that frame alone so that every
+        kernel runs at a chunk's shapes: ``pad`` in the tensor form, else a zero uint8 frame."""
+        t, pad = self.chunk, self._pad
+        if form == "tensor":
+            x = xs[0]
+            if x.dim() == 5 or tuple(pad.shape) != tuple(x.shape[1:]) or pad.dtype != x.dtype:
+                raise ValueError(f"pad must be one ({', '.join(map(str, x.shape[1:]))}) {x.dtype} item of the chunk's form; "
+                                 f"got {tuple(pad.shape)} {pad.dtype}")
+            x = pad.to(x.device)[None].expand(t, *pad.shape).contiguous()
+        elif form == "crop":
+            x, _ = ops.frames_crop_normalize(torch.zeros_like(xs[0]), self.bboxes, self.image_hw, row0=0,
+                                             channels_last=self.crop_channels_last, dtype=self.crop_dtype)
+        else:
+            x = ops.frames_normalize_views([torch.zeros_like(v) for v in xs[:-1]], self.image_hw,
+                                           channels_last=self.crop_channels_last, dtype=self.crop_dtype)
+        feats = self.features_of(x) if self.features_of is not None else x
+        wf, wb = self.head.head_mf._maps(feats[: self.sub_chunk])
+        if self._wf is None:
+            self._alloc_maps(wf)
+        self._wf[t + 4].copy_(wf[0])
+        self._wb[t + 4].copy_(wb[0])
+        self._pad = True
 
     def _inputs(self, x, bbox) -> tuple[str, tuple[torch.Tensor, ...]]:
         """A chunk as fed -> (its form, its checked tensors): "crop" (frames,), "views" (*views, boxes) or
@@ -447,15 +581,20 @@ class BatchedPredictor:
         self._cf_sf[2 + i : 2 + i + n].copy_(cf)
         wf, wb = mf._maps(f)  # W_f / W_b, once per frame
         if self._wf is None:
-            self._wf = torch.zeros((t + 4, *wf.shape[1:]), dtype=torch.float32, device=self.device)
-            self._wb = torch.zeros_like(self._wf)
+            self._alloc_maps(wf)
         self._wf[4 + i : 4 + i + n].copy_(wf)
         self._wb[4 + i : 4 + i + n].copy_(wb)
         hf = (mf.H_f[0].weight, mf.H_f[0].bias, mf.H_f[1].weight, mf.H_f[1].bias)
         hb = (mf.H_b[0].weight, mf.H_b[0].bias, mf.H_b[1].weight, mf.H_b[1].bias)
         kp_mf, cf_mf = head.run_subpixelmaxima(ops.plane_softmax(ops.crnn_combine(self._wf, self._wb, self._idx[i : i + n], hf, hb)))
-        ops.pack_context_predictions(self._kp_sf[i : i + n], self._cf_sf[i : i + n], kp_mf, cf_mf, self._box[i : i + n],
-                                     *self.image_hw, self.table, t, cursor=self.cursor)
+        if self.lengths is None:
+            ops.pack_context_predictions(self._kp_sf[i : i + n], self._cf_sf[i : i + n], kp_mf, cf_mf, self._box[i : i + n],
+                                         *self.image_hw, self.table, t, cursor=self.cursor)
+        else:  # the chunk's last call also writes the next chunk's window table
+            ops.pack_context_predictions_segments(self._kp_sf[i : i + n], self._cf_sf[i : i + n], kp_mf, cf_mf,
+                                                  self._box[i : i + n], *self.image_hw, self.table, t, self.cursor,
+                                                  self._segments, self._segments_host,
+                                                  window_index=self._idx if i + n == t else None)
         if i + n == t:
             for buf, halo in self._halo():
                 tail = buf[t : t + halo]
@@ -482,6 +621,11 @@ class BatchedPredictor:
         """Process the next chunk: a tensor with an optional ``bbox``, V uint8 views, or in crop mode uint8 full frames
         (the forms of the class docstring)."""
         form, xs = self._inputs(x, bbox)
+        if self.context and self._pad is not None and self._pad is not True:
+            if self._pad is False and form == "tensor":
+                raise ValueError("a video of this list has R = N - 1 rows, so its frame N - 2 is predicted from the "
+                                 "padding frame: pass `pad`, one item of the chunk's form (a zero frame's features)")
+            self._pad_maps(form, xs)
         if not self.use_graph:
             self._chunk(form, xs)
             return
@@ -519,7 +663,7 @@ class BatchedPredictor:
             blocks = list(self._blocks.split(self._blocks.shape[0] // world))
             dist.all_gather(blocks, blocks[rank].clone())
         if self.context:
-            fill_context_edges(self.table, self.chunk, world)
+            fill_context_edges(self.table, self.chunk, world, self.lengths)
         return self.table
 
     def results(self) -> tuple[torch.Tensor, torch.Tensor]:
@@ -528,6 +672,13 @@ class BatchedPredictor:
         kk = self.k * self.num_views
         t = self.table.reshape(self.n_frames, kk, 3)
         return t[:, :, :2].reshape(self.n_frames, 2 * kk), t[:, :, 2]
+
+    def video_tables(self) -> list[torch.Tensor]:
+        """The (N_i, 3 V K) rows of each video of a list (views, not copies); ``[table]`` for one video."""
+        if self.lengths is None:
+            return [self.table]
+        starts = _video_starts(self.lengths)
+        return [self.table[a:b] for a, b in zip(starts, starts[1:])]
 
     def view_tables(self) -> list[torch.Tensor]:
         """The V (N, 3K) column blocks of the table, one per view (views, not copies)."""
