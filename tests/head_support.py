@@ -293,6 +293,62 @@ def forward_checks(head, feats, case, splits=(None,), train=True, keypoint_bar=N
     return hm_ref
 
 
+# ------------------------------------------------------------------------------------------------
+# the band maxima of the 16-bit softmax and the decode that reads them
+# ------------------------------------------------------------------------------------------------
+def bits(t):
+    return t.contiguous().view(torch.int32)
+
+
+def band_max_of(hm, rows, nbands):
+    """per (frame, plane, band) maximum of the non-NaN values in heatmap rows [2 j rows, 2 (j + 1) rows)"""
+    b, k, h, w = hm.shape
+    pad = torch.zeros((b, k, nbands * 2 * rows - h, w), device=hm.device)
+    x = torch.cat([torch.nan_to_num(hm, nan=0.0), pad], dim=2)
+    return x.reshape(b, k, nbands, 2 * rows * w).amax(dim=3)
+
+
+def band_dims(h, w):
+    """(rows, bands) of ``lpb_head_band_max_dims`` for h x w heatmaps"""
+    import ctypes
+
+    r, n = ctypes.c_int(0), ctypes.c_int(0)
+    assert _lib().lpb_head_band_max_dims(h, w, ctypes.byref(r), ctypes.byref(n)) == 0
+    return r.value, n.value
+
+
+def assert_same_decode(hm, bm, ds, case, temperature=1000.0):
+    """The decode on the band maxima ``bm`` gives ``ops.decode_forward``'s full-sweep xy, confidence and stats, bit for
+    bit; returns the full sweep's."""
+    from lightning_pose_b200 import ops
+
+    full = ops.decode_forward(hm, ds, temperature)
+    banded = ops.decode_forward(hm, ds, temperature, band_max=bm)
+    for name, a, b in zip(("xy", "conf", "stats"), full, banded):
+        assert torch.equal(bits(a), bits(b)), f"{case} ds={ds}: {name} differs in {int((bits(a) != bits(b)).sum())} elements"
+    return full
+
+
+def head_run(feats, weights, biases, split):
+    """The 16-bit softmax head with its band maxima under softmax form ``split``, on features in either memory format
+    (``ops.feature_layout``): the heatmaps equal the plain call's bits, and the maxima equal the heatmaps' own per band.
+    Returns (heatmaps, ``ops.BandMax``)."""
+    from lightning_pose_b200 import ops
+
+    layout = ops.feature_layout(feats)
+    with softmax_split(_lib(), split):
+        hm, hints = ops._head_forward_16(feats, weights, biases, True, want_hints=True, layout=layout)
+        plain = ops._head_forward_16(feats, weights, biases, True, layout=layout)
+    torch.cuda.synchronize()
+    assert torch.equal(bits(hm), bits(plain)), "writing the band maxima changed the heatmaps"
+    rows, nbands = band_dims(hm.shape[2], hm.shape[3])
+    assert (hints.rows, hints.nbands) == (rows, nbands) and hints.bits.shape == (*hm.shape[:2], nbands, 8)
+    want = band_max_of(hm, rows, nbands)
+    got = hints.bits.view(torch.float32).amax(dim=3)
+    assert torch.equal(bits(got), bits(want)), "band maxima differ from the heatmaps' own"
+    return hm, hints
+
+
 def backward_checks(head, feats, softmax, hm_ref, case, seed=7, frozen=False, db_max_rule=False):
     """bf16 gradients of sum(head(feats) * gout), gout random, against float64 (``check_grads``); with ``frozen`` also
     the weight gradients of a frozen backbone's call (no feature gradient requested)."""

@@ -16,21 +16,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from head_support import _lib, features, head_params, make_head, softmax_split  # noqa: E402
+from head_support import assert_same_decode, band_dims as dims, bits, features, head_params, head_run, make_head  # noqa: E402
 
 T = 1000.0
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def band_max_of(hm, rows, nbands):
-    """per (frame, plane, band) maximum of the non-NaN values in heatmap rows [2 j rows, 2 (j + 1) rows)"""
-    b, k, h, w = hm.shape
-    pad = torch.zeros((b, k, nbands * 2 * rows - h, w), device=hm.device)
-    x = torch.cat([torch.nan_to_num(hm, nan=0.0), pad], dim=2)
-    return x.reshape(b, k, nbands, 2 * rows * w).amax(dim=3)
 
 
 def slots_of(hm, rows, nbands):
@@ -44,40 +32,6 @@ def slots_of(hm, rows, nbands):
         if part.shape[3]:
             out[..., e] = part.amax(dim=(3, 4))
     return out.view(torch.int32).contiguous()
-
-
-def dims(h, w):
-    import ctypes
-
-    r, n = ctypes.c_int(0), ctypes.c_int(0)
-    assert _lib().lpb_head_band_max_dims(h, w, ctypes.byref(r), ctypes.byref(n)) == 0
-    return r.value, n.value
-
-
-def assert_same_decode(hm, bm, ds, case):
-    from lightning_pose_b200 import ops
-
-    full = ops.decode_forward(hm, ds, T)
-    banded = ops.decode_forward(hm, ds, T, band_max=bm)
-    for name, a, b in zip(("xy", "conf", "stats"), full, banded):
-        assert torch.equal(bits(a), bits(b)), f"{case} ds={ds}: {name} differs in {int((bits(a) != bits(b)).sum())} elements"
-    return full
-
-
-def head_run(feats, weights, biases, split):
-    from lightning_pose_b200 import ops
-
-    with softmax_split(_lib(), split):
-        hm, hints = ops._head_forward_16(feats, weights, biases, True, want_hints=True)
-        plain = ops._head_forward_16(feats, weights, biases, True)
-    torch.cuda.synchronize()
-    assert torch.equal(bits(hm), bits(plain)), "writing the band maxima changed the heatmaps"
-    rows, nbands = dims(hm.shape[2], hm.shape[3])
-    assert (hints.rows, hints.nbands) == (rows, nbands) and hints.bits.shape == (*hm.shape[:2], nbands, 8)
-    want = band_max_of(hm, rows, nbands)
-    got = hints.bits.view(torch.float32).amax(dim=3)
-    assert torch.equal(bits(got), bits(want)), "band maxima differ from the heatmaps' own"
-    return hm, hints
 
 
 @pytest.fixture(scope="module")
