@@ -131,43 +131,35 @@ int lpb_evaluate_heatmaps_at_location(const float* heatmaps, const float* locs, 
  * replaces HeatmapHead.forward  lightning_pose/models/heads/heatmap.py:203-212
  * (PixelShuffle(2) -> ConvTranspose2d(k3,s2,p1,op1) x n_layers [:20-71] -> spatial_softmax2d(T=1)).
  *
- * features  [B, C, H, W]   fp32 (lpb_head_fwd_f32) or bf16 (lpb_head_fwd_bf16), NCHW contiguous
- * w1 [C/4, c1, 3, 3], b1 [c1]   first deconv (ConvTranspose2d layout, fp32 or bf16 to match)
+ * features  [B, C, H, W]   bf16 (lpb_head_fwd_bf16) or fp16 (lpb_head_fwd_f16), NCHW contiguous
+ * w1 [C/4, c1, 3, 3], b1 [c1]   first deconv (ConvTranspose2d layout, fp32 master weights)
  * w2 [c1, c2, 3, 3],  b2 [c2]   second deconv, or NULL/NULL for a one-layer head (then c2 = 0)
  * out [B, K, Ho, Wo] fp32 with K = c2 ? c2 : c1, Ho = 4H*(n_layers==2?2:1) ...
- * workspace: lpb_head_workspace_bytes() bytes of scratch (device), may be NULL if that is 0.
- */
-int lpb_head_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes);
-int lpb_head_fwd_f32(const float* features, int B, int C, int H, int W, const float* w1, const float* b1,
-                     int c1, const float* w2, const float* b2, int c2, int final_softmax, float* out,
-                     void* workspace, void* stream);
-
-/* The same stack one layer at a time (any number of deconvs: n_layers = log2(stride) - downsample_factor - 1,
+ * workspace: lpb_head_bf16_workspace_bytes() bytes of scratch (device).
+ *
+ * fp32 heads run the stack one layer at a time (any number of deconvs: n_layers = log2(stride) - downsample_factor - 1,
  * heads/heatmap.py:192-193), with its native backward -- the fp32 reference precision path trains through these.
  * Every convolution runs on the tensor cores in 3xTF32 (fp32 accuracy); any Cin, Cout, Hi, Wi (even with shuffle).
  *   lpb_convt_fwd_f32   in [B, Cin(*4 if shuffle), Hi(/2), Wi(/2)] -> out [B, Cout, 2Hi, 2Wi]; shuffle != 0 folds
  *                       PixelShuffle(2) into the load (Hi, Wi are the conv-input = shuffled sizes).  shuffle =
  *                       LPB_SHUFFLE_NHWC: the same with `in` channels-last, [B, Hi/2, Wi/2, 4 Cin] in memory (and so
- *                       grad_in of lpb_convt_bwd_f32); results are bit-identical to LPB_SHUFFLE_NCHW (= 1) on the same
- *                       logical tensor.
+ *                       grad_in of lpb_convt_bwd_f32_ws); results are bit-identical to LPB_SHUFFLE_NCHW (= 1) on the
+ *                       same logical tensor.
  *   lpb_plane_softmax_f32  in-place spatial softmax (T = 1) of [n_planes, hw]
- *   lpb_convt_bwd_f32   autograd of lpb_convt_fwd_f32: grad_in (same shape as `in`, may be NULL), grad_w [Cin,Cout,3,3],
- *                       grad_bias [Cout] (may be NULL); all overwritten.  NOT bit-reproducible: grad_w and grad_bias are
- *                       summed over the K-split CTAs with float atomics, so their last bits can change from call to call.
- *   lpb_convt_bwd_f32_ws   the same gradients, bit-reproducible: each K-split CTA ("slot") stores its grad_w tile and
- *                       bias sums as a partial in `workspace`, and the slots are added in slot order.  The slot count
- *                       follows the device's SM count (at most 264), so the order -- and the bits -- are fixed per device
- *                       model and shape.  workspace: lpb_convt_bwd_f32_workspace_bytes(B, Cin, Hi, Wi, Cout) bytes (the
- *                       conv-input sizes, as above), 4-byte aligned; NULL only when that is 0.  workspace_bytes is its
- *                       size (LPB_ERR_INVALID if smaller, before anything is queued).  Only the call's own kernels use it. */
+ *   lpb_convt_bwd_f32_ws   autograd of lpb_convt_fwd_f32: grad_in (same shape as `in`, may be NULL), grad_w
+ *                       [Cin,Cout,3,3], grad_bias [Cout] (may be NULL); all overwritten.  Bit-reproducible: each K-split
+ *                       CTA ("slot") stores its grad_w tile and bias sums as a partial in `workspace`, and the slots
+ *                       are added in slot order.  The slot count follows the device's SM count (at most 264), so the
+ *                       order -- and the bits -- are fixed per device model and shape.  workspace:
+ *                       lpb_convt_bwd_f32_workspace_bytes(B, Cin, Hi, Wi, Cout) bytes (the conv-input sizes, as above),
+ *                       4-byte aligned; NULL only when that is 0.  workspace_bytes is its size (LPB_ERR_INVALID if
+ *                       smaller, before anything is queued).  Only the call's own kernels use it. */
 #define LPB_SHUFFLE_NONE 0
 #define LPB_SHUFFLE_NCHW 1
 #define LPB_SHUFFLE_NHWC 2
 int lpb_convt_fwd_f32(const float* in, int B, int Cin, int Hi, int Wi, int shuffle, const float* w, const float* bias,
                       int Cout, float* out, void* stream);
 int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* stream);
-int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
-                      int Cout, float* grad_in, float* grad_w, float* grad_bias, void* stream);
 int lpb_convt_bwd_f32_workspace_bytes(int B, int Cin, int Hi, int Wi, int Cout, size_t* bytes);
 int lpb_convt_bwd_f32_ws(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
                          int Cout, float* grad_in, float* grad_w, float* grad_bias, void* workspace, size_t workspace_bytes,
@@ -319,13 +311,12 @@ int lpb_remap_keypoints_bwd(const float* grad_out, int64_t n, int K, const float
  * [K*F,1,2,2], convt_b [K] into L [K,4,4], h [K,4];  lpb_crnn_prepare_bwd maps (dL, dh) back to their gradients.
  * lpb_crnn_combine_fwd: WF, WB [N, K, H, W] = W_f / W_b applied to each of N frames ONCE (head kernels), idx [M, 5] =
  * frame index of each context slot of each of M outputs (overlapping windows share frames: no 5x feature tiling)
- * -> out_logits [M, K, H, W] = (x_f + x_b) / 2 before the spatial softmax.  lpb_crnn_combine_bwd: its autograd
- * (dWF, dWB [N,K,H,W], dLf/dLb [K,4,4], dhf/dhb [K,4]; all overwritten).  M * K < 65536 per call.  It sums with
- * float atomics and is NOT bit-reproducible.  lpb_crnn_combine_bwd_ws: the same gradients, bit-reproducible for any idx:
- * each element of dWF / dWB is one sum over the (window, slot) pairs that read its frame, window ascending then slot
- * (a pair list built on the device, no host sync), and dL / dh are per-CTA partials added in a fixed order.  workspace:
- * lpb_crnn_combine_bwd_workspace_bytes(M, N, K, H, W) bytes, 16-byte aligned, workspace_bytes its size (LPB_ERR_INVALID
- * if smaller or NULL, before anything is queued).
+ * -> out_logits [M, K, H, W] = (x_f + x_b) / 2 before the spatial softmax.  lpb_crnn_combine_bwd_ws: its autograd
+ * (dWF, dWB [N,K,H,W], dLf/dLb [K,4,4], dhf/dhb [K,4]; all overwritten).  M * K < 65536 per call.  Bit-reproducible
+ * for any idx: each element of dWF / dWB is one sum over the (window, slot) pairs that read its frame, window ascending
+ * then slot (a pair list built on the device, no host sync), and dL / dh are per-CTA partials added in a fixed order.
+ * workspace: lpb_crnn_combine_bwd_workspace_bytes(M, N, K, H, W) bytes, 16-byte aligned, workspace_bytes its size
+ * (LPB_ERR_INVALID if smaller or NULL, before anything is queued).
  * lpb_context_gather: the materialised window tensor out[i][s] = seq[clamp(i + s - ctx/2)] for API parity
  * (n items of item_bytes, a multiple of 16).  lpb_context_gather_bwd: its adjoint, d_seq [n, elems] = for each frame
  * the sum of the grad [n, ctx, elems] slots that read it (the repeated edge frames included), in a fixed order without
@@ -336,9 +327,6 @@ int lpb_crnn_prepare_bwd(const float* conv_w, const float* conv_b, const float* 
                          int K, int F, float* d_conv_w, float* d_conv_b, float* d_convt_w, float* d_convt_b, void* stream);
 int lpb_crnn_combine_fwd(const float* WF, const float* WB, const int32_t* idx, int M, int N, int K, int H, int W,
                          const float* Lf, const float* hf, const float* Lb, const float* hb, float* out_logits, void* stream);
-int lpb_crnn_combine_bwd(const float* WF, const float* WB, const int32_t* idx, const float* grad_logits, int M, int N, int K,
-                         int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb, float* dWF,
-                         float* dWB, float* dLf, float* dhf, float* dLb, float* dhb, void* stream);
 int lpb_crnn_combine_bwd_workspace_bytes(int M, int N, int K, int H, int W, size_t* bytes);
 int lpb_crnn_combine_bwd_ws(const float* WF, const float* WB, const int32_t* idx, const float* grad_logits, int M, int N, int K,
                             int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb, float* dWF,
@@ -733,13 +721,6 @@ int lpb_regression_losses_fwd(const float* targets, const float* preds, int64_t 
  * grad_preds [n] is overwritten, 0 at the dropped entries. */
 int lpb_regression_losses_bwd(const float* targets, const float* preds, int64_t n, const float* fwd_out, const float* grad_out,
                               float* grad_preds, void* stream);
-
-/* ---- diagnostics ------------------------------------------------------------------------------
- * Tensor-core operand self-test (bring-up aid): one-CTA GEMM over operands in the library's row layout
- * [kchunk][row][8] bf16; mode 0 = K-major view, 1 = MN-major view; d [128][n] fp32.  col_off has no effect
- * (kept for ABI compatibility). */
-int lpb_selftest_umma(const void* a, int kca, int rows_a, const void* b, int kcb, int rows_b, int mode, int n, int k,
-                      int row_shift, int col_off, float* d, void* stream);
 
 #ifdef __cplusplus
 }

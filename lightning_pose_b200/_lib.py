@@ -63,11 +63,8 @@ SIGNATURES = {
     "lpb_keypoints_mask_oob": (C.c_int, [_P, _L, _F, _F, _P, _P]),
     "lpb_generate_heatmaps_bwd": (C.c_int, [_P, _P, _P, _L, _F, _F, _I, _I, _F, _P, _P]),
     "lpb_evaluate_heatmaps_at_location": (C.c_int, [_P, _P, _L, _I, _I, _I, _P, _P]),
-    "lpb_head_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
-    "lpb_head_fwd_f32": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P]),
     "lpb_convt_fwd_f32": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P]),
     "lpb_plane_softmax_f32": (C.c_int, [_P, _L, _I, _P]),
-    "lpb_convt_bwd_f32": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
     "lpb_convt_bwd_f32_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_convt_bwd_f32_ws": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P, _P, _Z, _P]),
     "lpb_head_bf16_plan": (C.c_int, [_I, _I, _I, _I, _I, C.POINTER(_I)]),
@@ -93,7 +90,6 @@ SIGNATURES = {
     "lpb_crnn_prepare": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P]),
     "lpb_crnn_prepare_bwd": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "lpb_crnn_combine_fwd": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
-    "lpb_crnn_combine_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "lpb_crnn_combine_bwd_workspace_bytes": (C.c_int, [_I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_crnn_combine_bwd_ws": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
     "lpb_context_gather": (C.c_int, [_P, _L, _L, _I, _P, _P]),
@@ -120,7 +116,6 @@ SIGNATURES = {
     "lpb_heatmap_loss_from_keypoints_bwd": (C.c_int, [_P, _P, _P, _L, _F, _F, _I, _I, _F, _I, _P, _P, _P, _P]),
     "lpb_temporal_heatmap_loss_fwd": (C.c_int, [_P, _P, _L, _I, _I, _I, _I, _P, _F, _P, _P, _P]),
     "lpb_temporal_heatmap_loss_bwd": (C.c_int, [_P, _P, _P, _L, _I, _I, _I, _I, _P, _F, _P, _P, _P]),
-    "lpb_selftest_umma": (C.c_int, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "lpb_unsup_losses_fwd": (C.c_int, [_P, _P, _L, _I, _I, _P, _F, _I, C.POINTER(PcaDesc), C.POINTER(PcaDesc), _P, _P]),
     "lpb_unsup_losses_bwd": (C.c_int, [_P, _P, _L, _I, _I, _P, _F, _I, C.POINTER(PcaDesc), C.POINTER(PcaDesc), _P, _P, _P]),
     "lpb_triangulate_pairs_fwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),

@@ -10,7 +10,7 @@ namespace lpb {
 const char* last_error_cstr();
 }
 
-extern "C" int lpb_version(void) { return 100; }
+extern "C" int lpb_version(void) { return 200; }
 extern "C" const char* lpb_last_error(void) { return lpb::last_error_cstr(); }
 extern "C" const char* lpb_build_arch(void) { return "sm_90a"; }
 

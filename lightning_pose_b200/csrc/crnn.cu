@@ -123,18 +123,13 @@ __global__ void __launch_bounds__(256) crnn_combine_fwd_kernel(const __grid_cons
   *reinterpret_cast<float2*>(dst + (size_t)(2 * by + 1) * P.W + 2 * bx) = make_float2(0.5f * (xf[2] + xb[2]), 0.5f * (xf[3] + xb[3]));
 }
 
-// Backward: recompute the two chains, then walk them in reverse.
-// FIXED = false (lpb_crnn_combine_bwd): dWF / dWB are accumulated with atomics (a frame can sit in several windows); dL /
-//   dh are reduced per warp, then added with atomics.  The order of those adds is not fixed.
-// FIXED = true (lpb_crnn_combine_bwd_ws): dWF / dWB are left to crnn_dmaps_kernel; each CTA sums dL / dh over its warps
-//   in warp order and stores them as partial row m * gridDim.x + blockIdx.x of `part` ([dLf | dhf | dLb | dhb], 40 K
-//   floats a row; the CTA writes its keypoint's 40), which reduce_partials adds in row order.
-template <bool FIXED>
+// Backward of the L / h parameters (lpb_crnn_combine_bwd_ws): recompute the two chains, then walk them in reverse.
+// dWF / dWB are left to crnn_dmaps_kernel (a frame can sit in several windows).  Each CTA sums dL / dh over its warps
+// in warp order and stores them as partial row m * gridDim.x + blockIdx.x of `part` ([dLf | dhf | dLb | dhb], 40 K
+// floats a row; the CTA writes its keypoint's 40), which reduce_partials adds in row order.
 __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_constant__ CrnnParams P, const float* __restrict__ g,
-                                                               float* __restrict__ dWF, float* __restrict__ dWB,
-                                                               float* __restrict__ dLf, float* __restrict__ dhf,
-                                                               float* __restrict__ dLb, float* __restrict__ dhb, float* __restrict__ part) {
-  __shared__ float red[8][40];  // FIXED: [warp][dLf 16 | dhf 4 | dLb 16 | dhb 4]
+                                                               float* __restrict__ part) {
+  __shared__ float red[8][40];  // [warp][dLf 16 | dhf 4 | dLb 16 | dhb 4]
   const int plane = blockIdx.y, m = plane / P.K, k = plane - m * P.K;
   const int Wb = P.W / 2, nblk = (P.H / 2) * Wb;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -147,7 +142,6 @@ __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_cons
 #pragma unroll
   for (int dir = 0; dir < 2; ++dir) {
     const float* Wm = dir ? P.WB : P.WF;
-    float* dWm = dir ? dWB : dWF;
     float L[16], h[4];
 #pragma unroll
     for (int i = 0; i < 16; ++i) L[i] = __ldg((dir ? P.Lb : P.Lf) + k * 16 + i);
@@ -174,15 +168,7 @@ __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_cons
       const float2 r1 = __ldg(reinterpret_cast<const float2*>(gp + (size_t)(2 * by + 1) * P.W + 2 * bx));
       gg[0] = 0.5f * r0.x, gg[1] = 0.5f * r0.y, gg[2] = 0.5f * r1.x, gg[3] = 0.5f * r1.y;
 #pragma unroll
-      for (int s = CRNN_CTX - 1; s >= 0; --s) {
-        if constexpr (!FIXED) {
-          float* dp = dWm + ((size_t)fr[dir ? CRNN_CTX - 1 - s : s] * P.K + k) * hw;
-          atomicAdd(dp + (size_t)(2 * by) * P.W + 2 * bx, gg[0]);
-          atomicAdd(dp + (size_t)(2 * by) * P.W + 2 * bx + 1, gg[1]);
-          atomicAdd(dp + (size_t)(2 * by + 1) * P.W + 2 * bx, gg[2]);
-          atomicAdd(dp + (size_t)(2 * by + 1) * P.W + 2 * bx + 1, gg[3]);
-        }
-        if (s == 0) break;
+      for (int s = CRNN_CTX - 1; s > 0; --s) {
         float gn[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int o = 0; o < 4; ++o) {
@@ -197,37 +183,20 @@ __global__ void __launch_bounds__(256) crnn_combine_bwd_kernel(const __grid_cons
         for (int i = 0; i < 4; ++i) gg[i] = gn[i];
       }
     }
-    if constexpr (FIXED) {
 #pragma unroll
-      for (int i = 0; i < 20; ++i) {
-        const float v = warp_sum(i < 16 ? dL[i] : dh[i - 16]);
-        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][20 * dir + i] = v;
-      }
-    } else {
-      float* dLg = (dir ? dLb : dLf) + k * 16;
-      float* dhg = (dir ? dhb : dhf) + k * 4;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float v = warp_sum(dL[i]);
-        if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dLg + i, v);
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float v = warp_sum(dh[i]);
-        if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dhg + i, v);
-      }
+    for (int i = 0; i < 20; ++i) {
+      const float v = warp_sum(i < 16 ? dL[i] : dh[i - 16]);
+      if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][20 * dir + i] = v;
     }
   }
-  if constexpr (FIXED) {
-    __syncthreads();
-    if (threadIdx.x < 40) {
-      const int i = threadIdx.x, dir = i / 20, j = i - 20 * dir;
-      float v = 0.f;
-      for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) v += red[wp][i];
-      // section offsets in a row: dLf 0, dhf 16 K, dLb 20 K, dhb 36 K
-      const size_t col = (size_t)20 * P.K * dir + (j < 16 ? (size_t)k * 16 + j : (size_t)16 * P.K + k * 4 + (j - 16));
-      part[((size_t)m * gridDim.x + blockIdx.x) * 40 * P.K + col] = v;
-    }
+  __syncthreads();
+  if (threadIdx.x < 40) {
+    const int i = threadIdx.x, dir = i / 20, j = i - 20 * dir;
+    float v = 0.f;
+    for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) v += red[wp][i];
+    // section offsets in a row: dLf 0, dhf 16 K, dLb 20 K, dhb 36 K
+    const size_t col = (size_t)20 * P.K * dir + (j < 16 ? (size_t)k * 16 + j : (size_t)16 * P.K + k * 4 + (j - 16));
+    part[((size_t)m * gridDim.x + blockIdx.x) * 40 * P.K + col] = v;
   }
 }
 
@@ -286,8 +255,9 @@ __global__ void __launch_bounds__(1024) crnn_pairs_kernel(const int32_t* __restr
 
 // dWF / dWB of lpb_crnn_combine_bwd_ws, one thread per 2x2 block of one (frame, keypoint) plane: the sum over the frame's
 // (window, slot) pairs, in pair order, of the slot's chain gradient.  That gradient needs no chain state: at chain step
-// q it is (L^T)^(4 - q) 0.5 g[m], computed here with the backward kernel's own fma sequence, so each term has the bits
-// of the term the atomic form adds.  Window slot s is chain step s forward and 4 - s backward.
+// q it is (L^T)^(4 - q) 0.5 g[m], computed here with the same fma sequence as crnn_combine_bwd_kernel's walk back
+// along the chain, so each term has the bits of the chain gradient that kernel carries at that step.  Window slot s is
+// chain step s forward and 4 - s backward.
 __global__ void __launch_bounds__(256) crnn_dmaps_kernel(const __grid_constant__ CrnnParams P, const float* __restrict__ g,
                                                          const int* __restrict__ start, const int* __restrict__ pairs,
                                                          float* __restrict__ dWF, float* __restrict__ dWB) {
@@ -426,29 +396,6 @@ extern "C" int lpb_crnn_combine_fwd(const float* WF, const float* WB, const int3
   return LPB_OK;
 }
 
-extern "C" int lpb_crnn_combine_bwd(const float* WF, const float* WB, const int32_t* idx, const float* grad_logits, int M, int N, int K,
-                                    int H, int W, const float* Lf, const float* hf, const float* Lb, const float* hb, float* dWF,
-                                    float* dWB, float* dLf, float* dhf, float* dLb, float* dhb, void* stream) {
-  using namespace lpb;
-  if (int rc = crnn_check(WF, WB, idx, M, N, K, H, W)) return rc;
-  LPB_REQUIRE(grad_logits && Lf && hf && Lb && hb && dWF && dWB && dLf && dhf && dLb && dhb, "crnn_combine_bwd: null pointer");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const size_t nmap = (size_t)N * K * H * W * sizeof(float);
-  LPB_CUDA(cudaMemsetAsync(dWF, 0, nmap, s));
-  LPB_CUDA(cudaMemsetAsync(dWB, 0, nmap, s));
-  LPB_CUDA(cudaMemsetAsync(dLf, 0, sizeof(float) * K * 16, s));
-  LPB_CUDA(cudaMemsetAsync(dLb, 0, sizeof(float) * K * 16, s));
-  LPB_CUDA(cudaMemsetAsync(dhf, 0, sizeof(float) * K * 4, s));
-  LPB_CUDA(cudaMemsetAsync(dhb, 0, sizeof(float) * K * 4, s));
-  if (M == 0) return LPB_OK;
-  CrnnParams p{WF, WB, idx, Lf, hf, Lb, hb, M, N, K, H, W};
-  const int nblk = (H / 2) * (W / 2);
-  dim3 grid((unsigned)((nblk + 255) / 256), (unsigned)(M * K));
-  crnn_combine_bwd_kernel<false><<<grid, 256, 0, s>>>(p, grad_logits, dWF, dWB, dLf, dhf, dLb, dhb, nullptr);
-  LPB_CUDA(cudaGetLastError());
-  return LPB_OK;
-}
-
 extern "C" int lpb_crnn_combine_bwd_workspace_bytes(int M, int N, int K, int H, int W, size_t* bytes) {
   using namespace lpb;
   LPB_REQUIRE(bytes, "crnn_combine_bwd_workspace_bytes: null pointer");
@@ -489,7 +436,7 @@ extern "C" int lpb_crnn_combine_bwd_ws(const float* WF, const float* WB, const i
   const int nblk = (H / 2) * (W / 2);
   crnn_pairs_kernel<<<1, 1024, 0, s>>>(idx, M, N, start, cnt, pairs);
   const dim3 grid((unsigned)((nblk + 255) / 256), (unsigned)(M * K));
-  crnn_combine_bwd_kernel<true><<<grid, 256, 0, s>>>(p, grad_logits, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, part);
+  crnn_combine_bwd_kernel<<<grid, 256, 0, s>>>(p, grad_logits, part);
   const int64_t nthreads = (int64_t)N * K * nblk;
   crnn_dmaps_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, s>>>(p, grad_logits, start, pairs, dWF, dWB);
   const size_t stride = (size_t)40 * K;

@@ -831,8 +831,8 @@ __global__ void __launch_bounds__(B3A_THREADS, 1) b3a_dgrad_kernel(const __grid_
 // =====================================================================================================
 //   dW[c, o, ky, kx] = sum_{frames, rows} X[row + shift][c] * G[row][(cls, o)]      ((cls, shift) -> tap)
 // a GEMM whose K dimension is the pixel raster.  Both operands are the row layout read TRANSPOSED (ldmatrix .trans,
-// mma_sm90.cuh kstep_mn / umma_selftest.cu mode 1): A = G (M = the 80 (cls, o) rows), B = X at a row offset (the
-// shift), N = this CTA's channel group.  Of the 4 shifts x 5 m16 tiles of A, 14 hold a real tap (NZ_M16, head_prep.cuh);
+// mma_sm90.cuh ldsm_x4_t): A = G (M = the 80 (cls, o) rows), B = X at a row offset (the shift), N = this CTA's channel
+// group.  Of the 4 shifts x 5 m16 tiles of A, 14 hold a real tap (NZ_M16, head_prep.cuh);
 // MMA warp w takes half w / 4 of the channel group and the (shift, m16 tile) units of role w % 4 (wg_unit) of it -- at most 4 each,
 // where one warp per shift would carry 5.  Its accumulators stay in registers across every (frame, row-chunk) unit of
 // the CTA, and one epilogue at the end writes them to the CTA's slot of the partials.  An all-ones input channel (the

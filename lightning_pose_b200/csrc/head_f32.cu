@@ -441,12 +441,11 @@ __global__ void __launch_bounds__(TC_THREADS) convt3x3s2_dgrad_kernel(const floa
 // gradient planes of the CTA's output channels.  The CTAs of the first channel tile also sum the bias gradient (the four
 // taps (1..2, 1..2)) of their channels: warp w takes channels w, w + warps, ...; its lanes sum the unit's pixels and
 // the warp's shuffle sum is added to the channel's running total, so that sum has a fixed order too.
-// PART: the tile and bias sums are stored into the slot's partial, dw / db + blockIdx.y * slot_stride, one writer per
-// element, and reduce_partials adds the slots in slot order (bit-reproducible).  Otherwise they are added into grad_w /
-// grad_b with float atomics (lpb_convt_bwd_f32: the order of the slots' adds is not fixed).
+// The tile and bias sums are stored into the slot's partial, dw / db + blockIdx.y * slot_stride, one writer per
+// element, and reduce_partials adds the slots in slot order (bit-reproducible).
 constexpr int WG_PS = TC_SLOTS + 4;
 
-template <int SHUFFLE, int WM, int WN, int NT, bool PART>
+template <int SHUFFLE, int WM, int WN, int NT>
 __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const float* __restrict__ in, const float* __restrict__ g,
                                                                         int B, int Cin, int Cout, int Hi, int Wi, int RB, int CB,
                                                                         float* __restrict__ dw, float* __restrict__ db, size_t slot_stride) {
@@ -462,10 +461,8 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g8 = lane >> 2, t = lane & 3;
   const int wm = warp % WM, wn = warp / WM;
   const bool do_bias = db != nullptr && ct == 0;
-  if constexpr (PART) {
-    dw += blockIdx.y * slot_stride;
-    if (db) db += blockIdx.y * slot_stride;
-  }
+  dw += blockIdx.y * slot_stride;
+  if (db) db += blockIdx.y * slot_stride;
 
   for (int i = threadIdx.x; i < CM * WG_PS; i += THREADS) xs[i] = 0.f;  // slots past RB * CB stay zero
   for (int p = threadIdx.x; p < TC_SLOTS; p += THREADS) pbt[p] = p < RB * CB ? 2 * (p / CB) * GC + p % CB : 0;
@@ -552,8 +549,7 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
         for (int j = 0; j < 2; ++j) {
           const int n = n0 + 8 * (NT * wn + nt) + 2 * t + j;
           if (n >= nk) continue;
-          if constexpr (PART) dw[(size_t)c * nk + n] = acc[mt][nt][2 * h + j];
-          else atomicAdd(dw + (size_t)c * nk + n, acc[mt][nt][2 * h + j]);
+          dw[(size_t)c * nk + n] = acc[mt][nt][2 * h + j];
         }
     }
   if (do_bias) {
@@ -561,15 +557,14 @@ __global__ void __launch_bounds__(32 * WM * WN) convt3x3s2_wgrad_kernel(const fl
     for (int ol = threadIdx.x; ol < np; ol += THREADS) {
       const int o = o_lo + ol;
       if (o * 9 < n0) continue;  // channel o belongs to the n tile that holds its tap 0
-      if constexpr (PART) db[o] = dbs[ol];
-      else atomicAdd(db + o, dbs[ol]);
+      db[o] = dbs[ol];
     }
   }
 }
 
 // K split of the weight gradient: about `ctas` CTAs in all, each with as many units as that leaves (one tile row of
-// partials or atomics per CTA).  The reproducible form caps `ctas` at F32_WG_MAX_CTAS, which bounds its workspace
-// without a device query; on an H100 SXM (132 SMs) both forms split alike.
+// partials per CTA).  `ctas` is capped at F32_WG_MAX_CTAS, which bounds the workspace without a device query; on an
+// H100 SXM (132 SMs) the cap equals the 2 CTAs per SM asked for, so it does not bind.
 constexpr int F32_WG_MAX_CTAS = 264;
 constexpr int F32_WG_CN = 160;  // N tile of both tilings below: 8 NT WN
 static long long wgrad_f32_slots(int B, int Cin, int Cout, int Hi, int Wi, int ctas) {
@@ -594,19 +589,14 @@ static int launch_wgrad(const float* in, const float* g, int B, int Cin, int Cou
       ((size_t)CM * WG_PS + (size_t)np_max * pad8_32((2 * pb.RB + 1) * (2 * pb.CB + 1)) + TC_SLOTS + np_max) * sizeof(float);
   DeviceLimits dev;
   LPB_TRY(device_limits(&dev));
-  const long long ks = wgrad_f32_slots(B, Cin, Cout, Hi, Wi, part ? std::min(2 * dev.sms, F32_WG_MAX_CTAS) : 2 * dev.sms);
+  const long long ks = wgrad_f32_slots(B, Cin, Cout, Hi, Wi, std::min(2 * dev.sms, F32_WG_MAX_CTAS));
   const dim3 grid((unsigned)(nct * nnt), (unsigned)ks);
-  if (part) {
-    const size_t stride = wgrad_f32_part_stride(Cin, Cout), nw = (size_t)Cin * Cout * 9;
-    LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, true>, smem, "convt_bwd_f32"));
-    convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, true><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, part,
-                                                                                        db ? part + nw : nullptr, stride);
-    reduce_partials<1>(part, (int)ks, stride, (int)nw, dw, dev.sms, s);
-    if (db) reduce_partials<1>(part + nw, (int)ks, stride, Cout, db, dev.sms, s);
-  } else {
-    LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, false>, smem, "convt_bwd_f32"));
-    convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT, false><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, dw, db, 0);
-  }
+  const size_t stride = wgrad_f32_part_stride(Cin, Cout), nw = (size_t)Cin * Cout * 9;
+  LPB_TRY(set_dynamic_smem(convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT>, smem, "convt_bwd_f32"));
+  convt3x3s2_wgrad_kernel<SHUFFLE, WM, WN, NT><<<grid, 32 * WM * WN, smem, s>>>(in, g, B, Cin, Cout, Hi, Wi, pb.RB, pb.CB, part,
+                                                                                db ? part + nw : nullptr, stride);
+  reduce_partials<1>(part, (int)ks, stride, (int)nw, dw, dev.sms, s);
+  if (db) reduce_partials<1>(part + nw, (int)ks, stride, Cout, db, dev.sms, s);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
@@ -636,14 +626,14 @@ static int launch_bwd(const float* in, const float* g, int B, int Cin, int Hi, i
   return go(convt3x3s2_dgrad_kernel<SHUFFLE, 8>, 8, bstride<8>());
 }
 
-// part == NULL: lpb_convt_bwd_f32 (atomics); otherwise the workspace of lpb_convt_bwd_f32_ws
+// part: the workspace of lpb_convt_bwd_f32_ws (the weight gradient's per-slot partials)
 static int convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w, int Cout,
                          float* grad_in, float* grad_w, float* grad_bias, float* part, cudaStream_t s) {
-  if (!part || B == 0) {  // the partials' sums overwrite grad_w and grad_bias
+  if (B == 0) {  // no partials to sum: the gradients of an empty batch are zero
     LPB_CUDA(cudaMemsetAsync(grad_w, 0, sizeof(float) * (size_t)Cin * Cout * 9, s));
     if (grad_bias) LPB_CUDA(cudaMemsetAsync(grad_bias, 0, sizeof(float) * Cout, s));
+    return LPB_OK;
   }
-  if (B == 0) return LPB_OK;
   if (shuffle == LPB_SHUFFLE_NHWC) return launch_bwd<LPB_SHUFFLE_NHWC>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, part, s);
   return shuffle ? launch_bwd<LPB_SHUFFLE_NCHW>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, part, s)
                  : launch_bwd<LPB_SHUFFLE_NONE>(in, grad_out, B, Cin, Hi, Wi, w, Cout, grad_in, grad_w, grad_bias, part, s);
@@ -668,15 +658,6 @@ extern "C" int lpb_plane_softmax_f32(float* x, int64_t n_planes, int hw, void* s
   return launch_plane_softmax(x, n_planes, hw, "plane_softmax_f32", static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int lpb_convt_bwd_f32(const float* in, const float* grad_out, int B, int Cin, int Hi, int Wi, int shuffle, const float* w,
-                                 int Cout, float* grad_in, float* grad_w, float* grad_bias, void* stream) {
-  using namespace lpb;
-  LPB_REQUIRE(in && grad_out && w && grad_w, "convt_bwd_f32: null pointer");
-  LPB_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1 && Hi >= 1 && Wi >= 1 && (!shuffle || (Hi % 2 == 0 && Wi % 2 == 0)),
-              "convt_bwd_f32: bad shape");
-  return convt_bwd_f32(in, grad_out, B, Cin, Hi, Wi, shuffle, w, Cout, grad_in, grad_w, grad_bias, nullptr, static_cast<cudaStream_t>(stream));
-}
-
 extern "C" int lpb_convt_bwd_f32_workspace_bytes(int B, int Cin, int Hi, int Wi, int Cout, size_t* bytes) {
   using namespace lpb;
   LPB_REQUIRE(bytes, "convt_bwd_f32_workspace_bytes: null pointer");
@@ -698,43 +679,4 @@ extern "C" int lpb_convt_bwd_f32_ws(const float* in, const float* grad_out, int 
   LPB_REQUIRE(workspace_bytes >= need, "convt_bwd_f32_ws: workspace of %zu bytes, %zu needed", workspace_bytes, need);
   return convt_bwd_f32(in, grad_out, B, Cin, Hi, Wi, shuffle, w, Cout, grad_in, grad_w, grad_bias, static_cast<float*>(workspace),
                        static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int lpb_head_workspace_bytes(int B, int C, int H, int W, int c1, int c2, size_t* bytes) {
-  using namespace lpb;
-  LPB_REQUIRE(bytes, "head_workspace_bytes: null pointer");
-  LPB_REQUIRE(B >= 0 && C >= 4 && C % 4 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_workspace_bytes: bad shape");
-  *bytes = c2 > 0 ? (size_t)B * c1 * (4 * H) * (4 * W) * sizeof(float) : 0;
-  return LPB_OK;
-}
-
-extern "C" int lpb_head_fwd_f32(const float* features, int B, int C, int H, int W, const float* w1, const float* b1,
-                                int c1, const float* w2, const float* b2, int c2, int final_softmax, float* out,
-                                void* workspace, void* stream) {
-  using namespace lpb;
-  LPB_REQUIRE(features && w1 && out, "head_fwd_f32: null pointer");
-  LPB_REQUIRE(B >= 0 && C >= 4 && C % 4 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 0, "head_fwd_f32: bad shape");
-  LPB_REQUIRE(c2 == 0 || (w2 && workspace), "head_fwd_f32: two-layer head needs w2 and workspace");
-  if (B == 0) return LPB_OK;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int Hs = 2 * H, Ws = 2 * W;  // after PixelShuffle(2)
-  int K, Ho, Wo;
-  if (c2 == 0) {
-    int rc = launch_convt(LPB_SHUFFLE_NCHW, features, B, C / 4, Hs, Ws, w1, b1, c1, out, s);
-    if (rc) return rc;
-    K = c1;
-    Ho = 2 * Hs;
-    Wo = 2 * Ws;
-  } else {
-    float* mid = static_cast<float*>(workspace);
-    int rc = launch_convt(LPB_SHUFFLE_NCHW, features, B, C / 4, Hs, Ws, w1, b1, c1, mid, s);
-    if (rc) return rc;
-    rc = launch_convt(LPB_SHUFFLE_NONE, mid, B, c1, 2 * Hs, 2 * Ws, w2, b2, c2, out, s);
-    if (rc) return rc;
-    K = c2;
-    Ho = 4 * Hs;
-    Wo = 4 * Ws;
-  }
-  if (final_softmax) return launch_plane_softmax(out, (int64_t)B * K, Ho * Wo, "head_fwd_f32", s);
-  return LPB_OK;
 }

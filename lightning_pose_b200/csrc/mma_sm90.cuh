@@ -152,27 +152,6 @@ __device__ __forceinline__ void for_shifts(F&& f) {
   f(std::integral_constant<int, 3>{});
 }
 
-// One K = 16 step, both operands MN-major (the row layout read transposed: K = rows, M / N = channels):
-// A element (m, k) at a + (m / 8) * sbo_a + 16 k + 2 (m % 8); B element (n, k) at b + (n / 8) * sbo_b + 16 k + 2 (n % 8).
-template <int MT, int NT>
-__device__ __forceinline__ void kstep_mn(float (&acc)[MT][NT][4], uint32_t a, uint32_t sbo_a, uint32_t b, uint32_t sbo_b, int lane) {
-  static_assert(NT % 2 == 0, "n8 tiles are loaded in pairs");
-  uint32_t af[MT][4];
-#pragma unroll
-  for (int mt = 0; mt < MT; ++mt)
-    ldsm_x4_t(af[mt], a + (uint32_t)(2 * mt + ((lane >> 3) & 1)) * sbo_a + (uint32_t)((lane >> 4) * 8 + (lane & 7)) * 16);
-#pragma unroll
-  for (int np = 0; np < NT / 2; ++np) {
-    uint32_t bf[4];
-    ldsm_x4_t(bf, b + (uint32_t)(2 * np + (lane >> 4)) * sbo_b + (uint32_t)(((lane >> 3) & 1) * 8 + (lane & 7)) * 16);
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
-      mma_bf16(acc[mt][2 * np], af[mt], bf[0], bf[1]);
-      mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
-    }
-  }
-}
-
 // n8 tile `nt` of the 32 rows of m16 tiles M0, M0 + 1 -> v[0..7] = D(16 M0 + lane, 8 nt + 0..7).  A lone last tile
 // (M0 + 1 == MT) fills lanes 16..31 with copies of its rows, which the caller ignores.
 template <int M0, int MT, int NT>

@@ -31,20 +31,17 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(_lib.lib, s), f"{s} declared in lpb200.h but not exported by liblpb200.so"
     assert sorted(_lib.SIGNATURES) == syms, "ctypes signature table out of sync with the header"
-    assert _lib.lib.lpb_version() >= 100
+    assert _lib.lib.lpb_version() >= 200
     assert _lib.lib.lpb_build_arch() == b"sm_90a"
 
 
-def test_entry_points_validate_arguments_without_gpu():
+def test_decode_and_target_entries_validate_arguments_without_gpu():
     from lightning_pose_b200 import _lib
 
     rc = _lib.lib.lpb_decode_fwd(None, 1, 8, 8, 2, 1000.0, None, None, None, None, None)
     assert rc == -1 and b"null pointer" in _lib.lib.lpb_last_error()
     rc = _lib.lib.lpb_decode_prepare(8, 8, 7)
     assert rc == -1 and b"bad shape" in _lib.lib.lpb_last_error()
-    n = ctypes.c_size_t(0)
-    assert _lib.lib.lpb_head_workspace_bytes(2, 2048, 12, 12, 17, 17, ctypes.byref(n)) == 0
-    assert n.value == 2 * 17 * 48 * 48 * 4
     with pytest.raises(_lib.LpbError):
         _lib.check(_lib.lib.lpb_generate_heatmaps(None, None, 1, 1.0, 1.0, 4, 4, 1.25, None, None))
 
@@ -210,7 +207,7 @@ def test_reference_arm_does_not_import_the_product():
         assert res.stdout.strip().splitlines()[-1] == "reference"
 
 
-def test_round2_entry_points_validate_arguments_without_gpu():
+def test_round2_and_ws_backward_entries_validate_arguments_without_gpu():
     """Every entry added in round 2 rejects null / malformed arguments with an error code (never a crash), and the
     shape planner works without a device (callers size buffers with it)."""
     import ctypes as C
@@ -230,13 +227,13 @@ def test_round2_entry_points_validate_arguments_without_gpu():
     assert L.lpb_head_bwd_bf16_workspace_bytes(2, 384, 16, 16, 17, 0, C.byref(n)) == 0 and n.value > 0
     for rc in (
         L.lpb_convt_fwd_f32(None, 1, 4, 4, 4, 1, None, None, 2, None, None),
-        L.lpb_convt_bwd_f32(None, None, 1, 4, 4, 4, 1, None, 2, None, None, None, None),
+        L.lpb_convt_bwd_f32_ws(None, None, 1, 4, 4, 4, 1, None, 2, None, None, None, None, 0, None),
         L.lpb_plane_softmax_f32(None, 1, 16, None),
         L.lpb_temporal_heatmap_loss_bwd(None, None, None, 4, 2, 8, 8, 0, None, 0.1, None, None, None),
         L.lpb_keypoints_mask_oob(None, 4, 64.0, 64.0, None, None),
         L.lpb_crnn_prepare(None, None, None, None, 5, 16, None, None, None),
         L.lpb_crnn_combine_fwd(None, None, None, 1, 5, 5, 8, 8, None, None, None, None, None, None),
-        L.lpb_crnn_combine_bwd(None, None, None, None, 1, 5, 5, 8, 8, None, None, None, None, None, None, None, None, None, None, None),
+        L.lpb_crnn_combine_bwd_ws(None, None, None, None, 1, 5, 5, 8, 8, None, None, None, None, None, None, None, None, None, None, None, 0, None),
         L.lpb_context_gather(None, 4, 64, 5, None, None),
         L.lpb_frames_normalize(None, 1, 8, 8, 8, 8, None, None, 0, 0, None, None),
         L.lpb_pack_predictions(None, None, 1, 2, None, 4, None, 0, None),

@@ -7,8 +7,6 @@ static plus dynamic memory passes the device's opt-in limit.
 - Between 200 KB (a former hand-written cap) and the device limit: the plane softmax forward and backward and
   ``upsample2x``.
 - Past the device limit: LPB_ERR_UNSUPPORTED (-3) naming the entry, and the stream stays usable."""
-import ctypes
-
 import pytest
 import torch
 
@@ -128,30 +126,6 @@ def test_fp32_head_at_96x128(ops):
     for i, d in enumerate(deconvs, 1):
         got[f"dw{i}"], got[f"db{i}"] = d.weight.grad, d.bias.grad
     check_grads_f32(got, {k: v for k, v in ref.items() if k != "dfeat"}, gnorm, "fp32 head 96x128")
-
-
-@pytest.mark.parametrize("hw,channels,softmax", [((12, 16), (17, 17), True), ((12, 16), (17, 17), False),
-                                                 ((6, 8), (17,), True), ((6, 8), (17,), False)],
-                         ids=["2deconv_96x128_softmax", "2deconv_96x128_logits", "1deconv_softmax", "1deconv_logits"])
-def test_head_fwd_f32_entry_equals_layerwise_route(ops, hw, channels, softmax):
-    """lpb_head_fwd_f32 and ops.head_forward_f32 (one convolution launch per layer, then the plane softmax) run the same
-    launches, so their heatmaps are bit-identical."""
-    from lightning_pose_b200._lib import check, lib
-
-    b, c, (h, w) = 2, 512, hw
-    head = make_head(c, channels, seed=61)
-    ws, bs = head_params(head)
-    feats = features(b, c, h, w, 62, torch.float32)
-    want = ops.head_forward_f32(feats, ws, bs, final_softmax=softmax)
-    c1, c2 = channels[0], (channels[1] if len(channels) > 1 else 0)
-    n = ctypes.c_size_t()
-    check(lib.lpb_head_workspace_bytes(b, c, h, w, c1, c2, ctypes.byref(n)))
-    ws_buf = torch.empty(max(1, n.value), dtype=torch.uint8, device="cuda")
-    out = torch.empty_like(want)
-    w2, b2 = (ws[1], bs[1]) if c2 else (None, None)
-    check(lib.lpb_head_fwd_f32(ops._ptr(feats), b, c, h, w, ops._ptr(ws[0]), ops._ptr(bs[0]), c1, ops._ptr(w2), ops._ptr(b2), c2,
-                               int(softmax), ops._ptr(out), ops._ptr(ws_buf), ops._stream()))
-    assert torch.equal(out, want)
 
 
 def test_unsup_losses_at_48_kib(ops):
