@@ -287,6 +287,47 @@ int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targets* mse, co
                               int B, int C, int H, int W, const float* w1, int c1, const float* w2, int c2, int feature_layout,
                               void* dfeat, float* dw1, float* db1, float* dw2, float* db2, void* workspace, void* stream);
 
+/* Three-deconv heads on the 16-bit tensor-core kernels: downsample_factor 1 on a stride-32 backbone
+ * (n_layers = log2(stride) - downsample_factor - 1 = 3, lightning_pose/models/heads/heatmap.py:192-193; the forward
+ * :203-212 and its autograd).  features [B, C, H, W] -> PixelShuffle(2) -> deconv (C/4 -> c1) -> deconv (c1 -> c2) ->
+ * deconv (c2 -> c3) [-> spatial softmax], heatmaps out [B, c3, 16H, 16W] fp32.  One entry per operation: the size query,
+ * the forward and the backward.  The kernels are those of the one- and two-deconv entries above, with a third banded
+ * layer between them (forward) and a third weight gradient and layer data gradient (backward).
+ * Shapes served (LPB_ERR_UNSUPPORTED otherwise, in all three entries; the head then runs the fp32 kernels):
+ *   narrow channels: c1, c2 <= 19 (room for the constant-one bias channel in each mid activation), c3 <= 20;
+ *   C % 128 == 0, W in {4, 8, 12, 16}, H * W % 8 == 0, and H even to train; feature_layout LPB_FEATURES_NCHW or
+ *   LPB_FEATURES_NHWC (channels-last, read and written in place, as the _layout entries above).
+ * lpb_head3_query needs no GPU.  It fills `sizes` (all zero when it fails):
+ *   plan         1: the whole-frame first layer ("fast path", saved_xs optional for inference), 0: the banded first
+ *                layer (saved_xs REQUIRED by the forward)
+ *   fwd_workspace, saved   bytes of the forward's workspace and saved_xs
+ *   bwd_workspace, bwd_workspace_targets   train != 0 only: the backward's workspace without / with keypoint targets.
+ * lpb_head3_fwd: operand LPB_OUT_BF16 or LPB_OUT_F16 (the features' element type; fp16 is inference only); band_max
+ *   NULL or, with final_softmax = 1, the per-band maxima as lpb_head_fwd_bf16_band_max writes them, for an
+ *   h x w = 16H x 16W heatmap (lpb_head_band_max_dims(16 H, 16 W)); the heatmaps are the same bits either way.
+ *   saved_xs and workspace must stay alive until lpb_head3_bwd.
+ * lpb_head3_bwd: the gradient sources as in lpb_head_bwd_bf16_targets (g_out, mse, probs, the decode windows; mse and
+ *   g_out not both); dfeat [B, C, H, W] bf16 in feature_layout or NULL; dw1 [C/4, c1, 3, 3], db1 [c1], dw2 [c1, c2, 3, 3],
+ *   db2 [c2], dw3 [c2, c3, 3, 3], db3 [c3] fp32, overwritten.  Every gradient is a fixed-order sum: two identical calls give
+ *   identical bits.  workspace: bwd_workspace (or bwd_workspace_targets with mse) bytes.
+ * Alignment as in the entries above: features, saved_xs, workspaces, dfeat, g_out, probs, win_meta and g_overflow 16
+ * bytes, out 8, band_max 4 (LPB_ERR_INVALID otherwise, before anything is queued). */
+typedef struct lpb_head3_sizes {
+  int plan;
+  size_t fwd_workspace;
+  size_t saved;
+  size_t bwd_workspace;
+  size_t bwd_workspace_targets;
+} lpb_head3_sizes;
+int lpb_head3_query(int B, int C, int H, int W, int c1, int c2, int c3, int feature_layout, int train, lpb_head3_sizes* sizes);
+int lpb_head3_fwd(const void* features, int operand, int feature_layout, int B, int C, int H, int W, const float* w1,
+                  const float* b1, int c1, const float* w2, const float* b2, int c2, const float* w3, const float* b3, int c3,
+                  int final_softmax, float* out, uint32_t* band_max, void* saved_xs, void* workspace, void* stream);
+int lpb_head3_bwd(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win, const int32_t* win_meta,
+                  const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int feature_layout, int B, int C,
+                  int H, int W, const float* w1, int c1, const float* w2, int c2, const float* w3, int c3, void* dfeat,
+                  float* dw1, float* db1, float* dw2, float* db2, float* dw3, float* db3, void* workspace, void* stream);
+
 /* ---- coordinate remap -------------------------------------------------------------------------
  * replaces undo_affine_transform_batch + model_to_frame_batch
  *   lightning_pose/data/utils.py:142-234, lightning_pose/data/bboxes.py:74-105,222-288

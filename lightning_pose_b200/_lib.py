@@ -43,6 +43,18 @@ class MseTargets(C.Structure):
     ]
 
 
+class Head3Sizes(C.Structure):
+    """mirror of ``lpb_head3_sizes`` (include/lpb200.h)."""
+
+    _fields_ = [
+        ("plan", C.c_int),
+        ("fwd_workspace", C.c_size_t),
+        ("saved", C.c_size_t),
+        ("bwd_workspace", C.c_size_t),
+        ("bwd_workspace_targets", C.c_size_t),
+    ]
+
+
 _P, _I, _L, _F, _Z = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
 
 # symbol -> (restype, argtypes); this table is also what tests/test_abi.py checks against the header
@@ -85,6 +97,10 @@ SIGNATURES = {
     "lpb_head_bwd_bf16_workspace_bytes_targets": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(_Z)]),
     "lpb_head_bwd_bf16_targets": (C.c_int, [_P, C.POINTER(MseTargets), _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P, _P,
                                             _P, _P, _P, _P]),
+    "lpb_head3_query": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(Head3Sizes)]),
+    "lpb_head3_fwd": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
+    "lpb_head3_bwd": (C.c_int, [_P, C.POINTER(MseTargets), _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P,
+                                _P, _P, _P, _P, _P, _P]),
     "lpb_remap_keypoints": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
     "lpb_remap_keypoints_bwd": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _L, _F, _F, _P, _P]),
     "lpb_crnn_prepare": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P]),

@@ -39,7 +39,7 @@ template <typename T>
 __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ PrepJobs J) {
   const long long tid0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
+  for (int j = 0; j < 3; ++j) {
     if (!J.fpack[j].out) continue;
     const float* w = J.fpack[j].w;
     const float* bias = J.fpack[j].bias;
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
     }
   }
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
+  for (int j = 0; j < 3; ++j) {
     if (!J.dpack[j].out) continue;
     const float* w = J.dpack[j].w;
     const int Cin = J.dpack[j].Cin, Cout = J.dpack[j].Cout, rpt = J.dpack[j].rows_per_tile, tch = J.dpack[j].tile_ch;
@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
     }
   }
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
+  for (int j = 0; j < 3; ++j) {
     if (!J.pads[j].buf) continue;
     const RowLayout L = J.pads[j].L;
     const int body0 = L.lead, body1 = L.lead + L.Hi * L.Pp;
@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(256) head_prep_kernel(const __grid_constant__ 
     }
   }
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
+  for (int j = 0; j < 6; ++j) {
     if (!J.zero[j].p) continue;
     for (long long i = tid0; i < J.zero[j].n; i += nthr) J.zero[j].p[i] = 0.f;
   }
@@ -549,18 +549,21 @@ extern "C" int lpb_head_bf16_workspace_bytes(int B, int C, int H, int W, int c1,
   return LPB_OK;
 }
 
-// lpb_head_fwd_bf16 (T = __nv_bfloat16) and lpb_head_fwd_f16 (T = __half): one plan, one workspace layout, one kernel
-// sequence; T is the element type of the features, the packed weights and the mid activations.
+// lpb_head_fwd_bf16 (T = __nv_bfloat16) and lpb_head_fwd_f16 (T = __half), and lpb_head3_fwd (c3 > 0): one plan, one
+// workspace layout, one kernel sequence; T is the element type of the features, the packed weights and the mid
+// activations.  A three-deconv head is the two-deconv sequence with its layer 2 writing mid activations (mid2) instead
+// of planes, and a third banded launch over mid2 for the planes or the softmax.
 template <typename T>
 static int head_fwd(const void* features, int B, int C, int H, int W, const float* w1, const float* b1, int c1, const float* w2,
                     const float* b2, int c2, int final_softmax, int feature_layout, float* out, void* saved_xs, void* workspace,
-                    void* stream, uint32_t* band_max = nullptr) {
+                    void* stream, uint32_t* band_max = nullptr, const float* w3 = nullptr, const float* b3 = nullptr, int c3 = 0) {
   using namespace lpb;
   const char* name = head_fwd_name<T>;
   LPB_REQUIRE(feature_layout == LPB_FEATURES_NCHW || feature_layout == LPB_FEATURES_NHWC, "%s: unknown feature layout %d", name, feature_layout);
-  const bool nhwc = feature_layout == LPB_FEATURES_NHWC;
+  const bool nhwc = feature_layout == LPB_FEATURES_NHWC, three = c3 > 0;
   LPB_REQUIRE(features && w1 && b1 && out && workspace, "%s: null pointer", name);
   LPB_REQUIRE(c2 == 0 || (w2 && b2), "%s: a two-deconv head needs w2 and b2", name);
+  LPB_REQUIRE(!three || (c2 > 0 && w3 && b3), "%s: a three-deconv head needs w2, b2, w3 and b3", name);
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1, "%s: bad feature shape C=%d H=%d W=%d", name, C, H, W);
   LPB_REQUIRE((H * W) % 8 == 0, "%s: H*W must be a multiple of 8 (got %d)", name, H * W);
   LPB_REQUIRE(head_narrow(c1, c2) || head_wide(c1, c2), "%s: channel counts %d/%d outside this build's set (lpb200.h)", name, c1, c2);
@@ -585,13 +588,15 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
     set_error("%s: cannot encode the feature tensor map", name);
     return LPB_ERR_INVALID;
   }
-  const int nst = C / 4 / HEAD_KSTAGE, nst2 = head_mid_stages(c1);
+  const int nst = C / 4 / HEAD_KSTAGE, nst2 = head_mid_stages(c1), nst3 = three ? head_mid_stages(c2) : 0;
   unsigned char* ws = static_cast<unsigned char*>(workspace);
-  const RowLayout Lxs = make_row_layout(2 * H, 2 * W), Lmid = make_row_layout(4 * H, 4 * W);
-  const HeadFwdLayout wl = head_fwd_layout(B, C, H, W, c1, c2);
+  const RowLayout Lxs = make_row_layout(2 * H, 2 * W), Lmid = make_row_layout(4 * H, 4 * W), Lmid2 = make_row_layout(8 * H, 8 * W);
+  const HeadFwdLayout wl = head_fwd_layout(B, C, H, W, c1, c2, c3);
   T* wp1 = reinterpret_cast<T*>(ws + wl.w1);
   T* wp2 = reinterpret_cast<T*>(ws + wl.w2);
+  T* wp3 = reinterpret_cast<T*>(ws + wl.w3);
   T* mid = reinterpret_cast<T*>(ws + wl.mid);
+  T* mid2 = reinterpret_cast<T*>(ws + wl.mid2);
   float* partials = reinterpret_cast<float*>(ws + wl.partials);
   {
     // one launch: both operand packs + the pad rows of the fresh row-layout buffers (k1a writes every row of the saved
@@ -601,8 +606,12 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
     // layer 2: bias rides on the constant-one channel c1 of the mid activations (only needed without softmax:
     // a per-plane constant does not change a softmax)
     if (c2 > 0) {
-      jobs.fpack[1] = {w2, final_softmax ? nullptr : b2, c1, c2, nst2, head_groups(c2), wp2};
+      jobs.fpack[1] = {w2, final_softmax && !three ? nullptr : b2, c1, c2, nst2, head_groups(c2), wp2};
       jobs.pads[0] = {mid, Lmid, (long long)B * 4 * nst2};
+    }
+    if (three) {  // layer 3 likewise, its bias on the constant-one channel c2 of mid2
+      jobs.fpack[2] = {w3, final_softmax ? nullptr : b3, c2, c3, nst3, 1, wp3};
+      jobs.pads[1] = {mid2, Lmid2, (long long)B * 4 * nst3};
     }
     launch_head_prep<T>(jobs, sms, s);
   }
@@ -662,21 +671,37 @@ static int head_fwd(const void* features, int B, int C, int H, int W, const floa
     const int items = B * k1.G;
     kern<<<items < sms ? items : sms, K1A_THREADS, s1, s>>>(pa);
   }
-  // ---- layer 2 of a two-deconv head, on both paths: the banded kernel over the mid activations ----
-  ConvtRowsParams<T> p2{};
-  p2.X = mid;
-  p2.L = Lmid;
-  p2.wpk = wp2;
-  p2.bias = nullptr;  // folded into the GEMM through the ones channel (see the pack above)
-  p2.nst = nst2;
-  p2.B = B;
-  p2.cout = c2;
-  p2.out = out;
-  p2.partials = partials;
-  p2.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
-  p2.band_max = final_softmax ? band_max : nullptr;
-  const int rc = launch_convt_rows(p2, sms, s);
+  // ---- the layers after the first, on both paths: the banded kernel over the mid activations; the bias is folded into
+  // the GEMM through the ones channel (see the packs above).  `next` null: the head's last layer (planes or softmax);
+  // otherwise the layer writes the next one's mid activations.
+  auto banded_layer = [&](const T* X, RowLayout L, const T* wpk, int nstg, int cout, T* next, RowLayout Lnext, int next_kc) {
+    ConvtRowsParams<T> p{};
+    p.X = X;
+    p.L = L;
+    p.wpk = wpk;
+    p.bias = nullptr;
+    p.nst = nstg;
+    p.B = B;
+    p.cout = cout;
+    p.out = out;
+    p.partials = partials;
+    if (next) {
+      p.mode = CONVT_ROWS_MID;
+      p.mid = next;
+      p.Lout = Lnext;
+      p.mid_kc = next_kc;
+    } else {
+      p.mode = final_softmax ? CONVT_ROWS_SOFTMAX : CONVT_ROWS_PLANES;
+      p.band_max = final_softmax ? band_max : nullptr;
+    }
+    return launch_convt_rows(p, sms, s);
+  };
+  int rc = three ? banded_layer(mid, Lmid, wp2, nst2, c2, mid2, Lmid2, 4 * nst3) : banded_layer(mid, Lmid, wp2, nst2, c2, nullptr, RowLayout{}, 0);
   if (rc != LPB_OK) return rc;
+  if (three) {
+    rc = banded_layer(mid2, Lmid2, wp3, nst3, c3, nullptr, RowLayout{}, 0);
+    if (rc != LPB_OK) return rc;
+  }
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }
@@ -730,4 +755,28 @@ extern "C" int lpb_head_fwd_f16(const void* features, int B, int C, int H, int W
                                 const float* w2, const float* b2, int c2, int final_softmax, float* out, void* saved_xs,
                                 void* workspace, void* stream) {
   return lpb_head_fwd_f16_layout(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, LPB_FEATURES_NCHW, out, saved_xs, workspace, stream);
+}
+
+// ---- three-deconv heads (lpb200.h lpb_head3_fwd; the size query is with the backward's, head_bwd_bf16.cu) -------------
+extern "C" int lpb_head3_fwd(const void* features, int operand, int feature_layout, int B, int C, int H, int W, const float* w1,
+                             const float* b1, int c1, const float* w2, const float* b2, int c2, const float* w3, const float* b3, int c3,
+                             int final_softmax, float* out, uint32_t* band_max, void* saved_xs, void* workspace, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(operand == LPB_OUT_BF16 || operand == LPB_OUT_F16, "head3_fwd: operand type %d is neither LPB_OUT_BF16 nor LPB_OUT_F16", operand);
+  LPB_REQUIRE(feature_layout == LPB_FEATURES_NCHW || feature_layout == LPB_FEATURES_NHWC, "head3_fwd: unknown feature layout %d", feature_layout);
+  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 1 && c3 >= 1, "head3_fwd: bad shape");
+  LPB_REQUIRE(!band_max || final_softmax, "head3_fwd: band maxima are written by the softmax; final_softmax must be 1");
+  const char* why = nullptr;
+  if (!head3_covered(H, W, c1, c2, c3, false, &why)) {
+    set_error("head3_fwd: %dx%d features, channels %d/%d/%d: %s", H, W, c1, c2, c3, why);
+    return LPB_ERR_UNSUPPORTED;
+  }
+  int plan = 0;
+  LPB_TRY(lpb_head_bf16_plan_layout(C, H, W, c1, c2, feature_layout, &plan));
+  LPB_REQUIRE(plan || saved_xs, "head3_fwd: this shape takes the banded kernels (lpb_head3_query plan = 0): pass saved_xs");
+  if (operand == LPB_OUT_F16)
+    return head_fwd<__half>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, feature_layout, out, saved_xs, workspace, stream,
+                            band_max, w3, b3, c3);
+  return head_fwd<__nv_bfloat16>(features, B, C, H, W, w1, b1, c1, w2, b2, c2, final_softmax, feature_layout, out, saved_xs, workspace,
+                                 stream, band_max, w3, b3, c3);
 }

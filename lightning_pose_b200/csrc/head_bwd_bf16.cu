@@ -1172,13 +1172,16 @@ static int head_bwd_covers(const char* who, int H, int W, int c1, int c2, int fe
 // group of c2 / c1, and two fp32 buffers follow the narrow layout: dmid [B][c1][4H * 4W] (the mid activations' gradient,
 // summed over the c2 groups, two-deconv heads) and acc32 [B][C][H * W] (the d features of the c1 groups before the last,
 // when c1 has more than one group).  Narrow heads have one group everywhere and neither buffer.
+// Three-deconv heads (c3 > 0, narrow: head_narrow3) append [W3 dgrad pack][G3 (8H x 8W grid)][layer-3 wgrad partials]
+// [layer-3 b2d bias partials] to the two-deconv layout; every other head has none of them.
 // With keypoint targets, the per-plane target factors (mse_fac_stride floats per output plane) come last.
 struct HeadBwdLayout {
-  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, dmid, acc32, fac, total;
+  size_t wp1, wp2, G2, G1, ddot, part1, part2, part_db1, part_cs, dmid, acc32, wp3, G3, part3, part_db2, fac, total;
 };
-static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2, bool targets) {
+static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2, bool targets, int c3 = 0) {
   const int C4 = C / 4;
-  const bool two = c2 > 0, wide = head_wide(c1, c2);
+  const bool two = c2 > 0, wide = head_wide(c1, c2), three = two && c3 > 0;
+  const int kout = three ? c3 : two ? c2 : c1;  // planes of the head's output
   const int g1 = head_groups(c1), g2 = two ? head_groups(c2) : 1, nst2 = two ? head_mid_stages(c1) : 1;
   HeadBwdLayout l{};
   l.wp1 = 0;
@@ -1186,7 +1189,7 @@ static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2,
   l.G2 = l.wp2 + (size_t)(two ? g1 * g2 : 1) * 4 * HEAD_KC * 32 * 16;
   l.G1 = l.G2 + (two ? (size_t)B * g2 * HEAD_KC * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
   l.ddot = l.G1 + (size_t)B * g1 * HEAD_KC * make_row_layout(2 * H, 2 * W).rows * 16;
-  l.part1 = l.ddot + (((size_t)B * (two ? c2 : c1) * 4 + 255) & ~(size_t)255);
+  l.part1 = l.ddot + (((size_t)B * kout * 4 + 255) & ~(size_t)255);
   const size_t part1_end = l.part1 + (size_t)wgrad_max_slots(C4 / 8) * wgrad_part_stride(C4, c1) * sizeof(float);
   if (two) {
     l.part2 = part1_end;
@@ -1202,10 +1205,17 @@ static HeadBwdLayout head_bwd_layout(int B, int C, int H, int W, int c1, int c2,
     l.acc32 = l.dmid + (two ? (size_t)B * c1 * 16 * H * W * sizeof(float) : 0);
     l.total = l.acc32 + (g1 > 1 ? (size_t)B * C * H * W * sizeof(float) : 0);
   }
+  if (three) {
+    l.wp3 = (l.total + 255) & ~(size_t)255;
+    l.G3 = l.wp3 + (size_t)4 * HEAD_KC * 32 * 16;
+    l.part3 = l.G3 + (size_t)B * HEAD_KC * make_row_layout(8 * H, 8 * W).rows * 16;
+    l.part_db2 = l.part3 + (size_t)wgrad_max_slots(4 * head_mid_stages(c2)) * wgrad_part_stride(c2, c3) * sizeof(float);
+    l.total = l.part_db2 + (size_t)B2D_MAX_CTAS * 4 * HEAD_CLS * sizeof(float);
+  }
   if (targets) {
-    const int up = two ? 8 : 4;  // output grid: (up H) x (up W)
+    const int up = three ? 16 : two ? 8 : 4;  // output grid: (up H) x (up W)
     l.fac = (l.total + 255) & ~(size_t)255;
-    l.total = l.fac + (size_t)B * (two ? c2 : c1) * mse_fac_stride(up * H, up * W) * sizeof(float);
+    l.total = l.fac + (size_t)B * kout * mse_fac_stride(up * H, up * W) * sizeof(float);
   }
   return l;
 }
@@ -1246,15 +1256,19 @@ extern "C" int lpb_head_bwd_bf16_layout(const float* g_out, const float* probs, 
                                    feature_layout, dfeat, dw1, db1, dw2, db2, workspace, stream);
 }
 
-extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win,
-                                         const int32_t* win_meta, const float* g_overflow, const void* saved_xs,
-                                         const void* fwd_workspace, int B, int C, int H, int W, const float* w1, int c1,
-                                         const float* w2, int c2, int feature_layout, void* dfeat, float* dw1, float* db1,
-                                         float* dw2, float* db2, void* workspace, void* stream) {
+// lpb_head_bwd_bf16_targets (c3 = 0) and lpb_head3_bwd (c3 > 0, a narrow three-deconv head).  A third layer runs ahead of
+// the two-deconv sequence: the front end writes G3 on the 8H x 8W grid, the layer-3 weight gradient reads mid2, and b2d
+// takes G3 to G2 (the mid2 gradient, whose column sums are db2); from G2 on, the two-deconv kernels run unchanged.
+static int head_bwd(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win, const int32_t* win_meta,
+                    const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int B, int C, int H, int W,
+                    const float* w1, int c1, const float* w2, int c2, int feature_layout, void* dfeat, float* dw1, float* db1,
+                    float* dw2, float* db2, void* workspace, void* stream, const float* w3 = nullptr, int c3 = 0,
+                    float* dw3 = nullptr, float* db3 = nullptr) {
   using namespace lpb;
-  const bool two = c2 > 0, nhwc = feature_layout == LPB_FEATURES_NHWC;
+  const bool two = c2 > 0, three = c3 > 0, nhwc = feature_layout == LPB_FEATURES_NHWC;
   LPB_REQUIRE(saved_xs && fwd_workspace && w1 && dw1 && db1 && workspace, "head_bwd_bf16: null pointer");
   LPB_REQUIRE(!two || (w2 && dw2 && db2), "head_bwd_bf16: a two-deconv head needs w2, dw2, db2");
+  LPB_REQUIRE(!three || (two && w3 && dw3 && db3), "head_bwd_bf16: a three-deconv head needs w2, w3, dw2, db2, dw3, db3");
   LPB_REQUIRE(g_out || mse || win, "head_bwd_bf16: neither a dense gradient nor decode windows given");
   if (mse) {
     LPB_REQUIRE(!g_out, "head_bwd_bf16: keypoint targets stand for the dense gradient; g_out must be null");
@@ -1265,6 +1279,10 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
   LPB_REQUIRE(!win || (win_meta && g_overflow), "head_bwd_bf16: windows need their meta and overflow buffers");
   LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1, "head_bwd_bf16: bad shape C=%d H=%d W=%d c1=%d", C, H, W, c1);
   if (const int rc = head_bwd_covers("head_bwd_bf16", H, W, c1, c2, feature_layout); rc != LPB_OK) return rc;
+  if (const char* why = nullptr; three && !head3_covered(H, W, c1, c2, c3, true, &why)) {
+    set_error("head_bwd_bf16: three-deconv head %dx%d with %d/%d/%d channels: %s", H, W, c1, c2, c3, why);
+    return LPB_ERR_UNSUPPORTED;
+  }
   {
     // read or written with 16-byte vectors (g_out, probs, g_overflow: float4 plane dots; win_meta: int4; dfeat: uint4 or
     // TMA stores) or bulk copies (saved_xs, fwd_workspace, workspace)
@@ -1273,14 +1291,18 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
     for (const auto& b : bufs) LPB_REQUIRE(aligned_to(b.p, 16), "head_bwd_bf16: %s must be 16-byte aligned", b.name);
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int C4 = C / 4, Hi1 = 2 * H, Wi1 = 2 * W, Hi2 = 4 * H, Wi2 = 4 * W;
-  const int kout = two ? c2 : c1;
+  const int C4 = C / 4, Hi1 = 2 * H, Wi1 = 2 * W, Hi2 = 4 * H, Wi2 = 4 * W, Hi3 = 8 * H, Wi3 = 8 * W;
+  const int kout = three ? c3 : two ? c2 : c1;
   if (B == 0) {
     LPB_CUDA(cudaMemsetAsync(dw1, 0, sizeof(float) * (size_t)C4 * c1 * 9, s));
     LPB_CUDA(cudaMemsetAsync(db1, 0, sizeof(float) * c1, s));
     if (two) {
       LPB_CUDA(cudaMemsetAsync(dw2, 0, sizeof(float) * (size_t)c1 * c2 * 9, s));
       LPB_CUDA(cudaMemsetAsync(db2, 0, sizeof(float) * c2, s));
+    }
+    if (three) {
+      LPB_CUDA(cudaMemsetAsync(dw3, 0, sizeof(float) * (size_t)c2 * c3 * 9, s));
+      LPB_CUDA(cudaMemsetAsync(db3, 0, sizeof(float) * c3, s));
     }
     return LPB_OK;
   }
@@ -1292,10 +1314,10 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
   DeviceLimits dev;
   LPB_TRY(device_limits(&dev));
   const int sms = dev.sms;
-  const RowLayout L2 = make_row_layout(Hi2, Wi2), L1 = make_row_layout(Hi1, Wi1);
+  const RowLayout L3 = make_row_layout(Hi3, Wi3), L2 = make_row_layout(Hi2, Wi2), L1 = make_row_layout(Hi1, Wi1);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   const int ntile1 = (C4 + 127) / 128;
-  const HeadBwdLayout wl = head_bwd_layout(B, C, H, W, c1, c2, mse != nullptr);
+  const HeadBwdLayout wl = head_bwd_layout(B, C, H, W, c1, c2, mse != nullptr, c3);
   __nv_bfloat16* wp1 = reinterpret_cast<__nv_bfloat16*>(ws + wl.wp1);
   __nv_bfloat16* wp2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.wp2);
   __nv_bfloat16* G2 = reinterpret_cast<__nv_bfloat16*>(ws + wl.G2);
@@ -1309,9 +1331,15 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
   float* part_cs = two && !wide ? nullptr : reinterpret_cast<float*>(ws + wl.part_cs);
   float* dmid = wide && two ? reinterpret_cast<float*>(ws + wl.dmid) : nullptr;
   float* acc32 = wide && g1 > 1 ? reinterpret_cast<float*>(ws + wl.acc32) : nullptr;
+  __nv_bfloat16* wp3 = three ? reinterpret_cast<__nv_bfloat16*>(ws + wl.wp3) : nullptr;
+  __nv_bfloat16* G3 = three ? reinterpret_cast<__nv_bfloat16*>(ws + wl.G3) : nullptr;
+  float* part3 = three ? reinterpret_cast<float*>(ws + wl.part3) : nullptr;
+  float* part_db2 = three ? reinterpret_cast<float*>(ws + wl.part_db2) : nullptr;
+  const int nst3 = three ? head_mid_stages(c2) : 0;
   // the forward pass's mid activations
-  const __nv_bfloat16* mid =
-      reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + head_fwd_layout(B, C, H, W, c1, c2).mid);
+  const HeadFwdLayout fl = head_fwd_layout(B, C, H, W, c1, c2, c3);
+  const __nv_bfloat16* mid = reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + fl.mid);
+  const __nv_bfloat16* mid2 = reinterpret_cast<const __nv_bfloat16*>(static_cast<const unsigned char*>(fwd_workspace) + fl.mid2);
 
   {
     // one launch: gradient accumulators zeroed, both data-gradient operand packs, pad rows of G2 / G1
@@ -1328,13 +1356,19 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
       jobs.zero[2] = {dw2, (long long)c1 * c2 * 9};
       jobs.zero[3] = {db2, (long long)c2};
     }
+    if (three) {
+      jobs.dpack[2] = {w3, c2, c3, 1, 32, 32, 1, wp3};
+      jobs.pads[2] = {G3, L3, (long long)B * HEAD_KC};
+      jobs.zero[4] = {dw3, (long long)c2 * c3 * 9};
+      jobs.zero[5] = {db3, (long long)c3};
+    }
     launch_head_prep(jobs, sms, s);
   }
   {
-    // gradient front end on the head's OUTPUT grid: G2 for a two-deconv head, G1 for a one-deconv head
-    const int Hio = two ? Hi2 : Hi1, Wio = two ? Wi2 : Wi1;
-    __nv_bfloat16* Gout = two ? G2 : G1;
-    const RowLayout Lo = two ? L2 : L1;
+    // gradient front end on the head's OUTPUT grid: G3 / G2 / G1 for a three- / two- / one-deconv head
+    const int Hio = three ? Hi3 : two ? Hi2 : Hi1, Wio = three ? Wi3 : two ? Wi2 : Wi1;
+    __nv_bfloat16* Gout = three ? G3 : two ? G2 : G1;
+    const RowLayout Lo = three ? L3 : two ? L2 : L1;
     G2Src src{};
     src.g_out = g_out;
     src.probs = probs;
@@ -1370,28 +1404,48 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
       else launch_g2_build<false, false>(src, B, kout, Hio, Wio, Gout, Lo, s);
     }
   }
-  if (two) {
-    // layer 2: weight + bias gradient (bias from the all-ones channel c1 of mid), then data gradient -> G1 (+ db1)
-    const int rc = launch_wgrad(mid, G2, dw2, db2, part2, B, Hi2, Wi2, 4 * nst2, c1, c2, c1, sms, s);
-    if (rc != LPB_OK) return rc;
+  // b2d over a (Hi x Wi) gradient grid Gin: the data gradient at the layer's input, written as the gradient rows Gnext
+  // of the layer before (grid Lnext) with the bias-gradient partials of that layer's cmid channels in db_part
+  int grid = B < 2 * sms ? B : 2 * sms;
+  if (grid > B2D_MAX_CTAS) grid = B2D_MAX_CTAS;  // the bias partials' workspace
+  auto b2d_params = [&](const __nv_bfloat16* Gin, RowLayout Lin, const __nv_bfloat16* wpk, __nv_bfloat16* Gnext, RowLayout Lnext, int Hi, int Wi,
+                        int cmid, float* db_part, size_t* smem) {
     B2dParams p{};
-    p.G2 = G2;
-    p.wpk = wp2;
-    p.G1 = G1;
-    p.L2 = L2;
-    p.L1 = L1;
-    p.db1_part = part_db1;
+    p.G2 = Gin;
+    p.wpk = wpk;
+    p.G1 = Gnext;
+    p.L2 = Lin;
+    p.L1 = Lnext;
+    p.db1_part = db_part;
     p.B = B;
-    p.Hi = Hi2;
-    p.Wi = Wi2;
-    p.c1 = c1;
-    p.R2 = (B2D_TILES * 128) / (Wi2 + 1);
-    if (p.R2 > Hi2) p.R2 = Hi2;
-    const int rows_alloc = (Wi2 + 2 + B2D_TILES * 128 + 7) & ~7;
-    const size_t smem = (size_t)HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 32 * 16 + 64;
+    p.Hi = Hi;
+    p.Wi = Wi;
+    p.c1 = cmid;
+    p.R2 = (B2D_TILES * 128) / (Wi + 1);
+    if (p.R2 > Hi) p.R2 = Hi;
+    const int rows_alloc = (Wi + 2 + B2D_TILES * 128 + 7) & ~7;
+    *smem = (size_t)HEAD_KC * rows_alloc * 16 + (size_t)4 * HEAD_KC * 32 * 16 + 64;
+    return p;
+  };
+  if (three) {
+    // layer 3: weight + bias gradient (bias from the all-ones channel c2 of mid2), then data gradient -> G2 (+ db2)
+    const int rc = launch_wgrad(mid2, G3, dw3, db3, part3, B, Hi3, Wi3, 4 * nst3, c2, c3, c2, sms, s);
+    if (rc != LPB_OK) return rc;
+    size_t smem = 0;
+    const B2dParams p = b2d_params(G3, L3, wp3, G2, L2, Hi3, Wi3, c2, part_db2, &smem);
+    LPB_REQUIRE(smem <= HEAD_STAGE_SMEM_BUDGET && p.R2 >= 1, "head_bwd_bf16: layer-3 width %d too large", Wi3);
+    LPB_TRY(set_dynamic_smem(b2d_dgrad_kernel<false>, smem, "head_bwd_bf16"));
+    b2d_dgrad_kernel<false><<<grid, B2D_THREADS, smem, s>>>(p);
+    reduce_partials<1>(part_db2, grid * 4, HEAD_CLS, c2, db2, sms, s);
+  }
+  if (two) {
+    // layer 2: weight gradient and, for a two-deconv head, the bias gradient (from the all-ones channel c1 of mid; a
+    // three-deconv head has db2 from layer 3's b2d), then data gradient -> G1 (+ db1)
+    const int rc = launch_wgrad(mid, G2, dw2, three ? nullptr : db2, part2, B, Hi2, Wi2, 4 * nst2, c1, c2, c1, sms, s);
+    if (rc != LPB_OK) return rc;
+    size_t smem = 0;
+    B2dParams p = b2d_params(G2, L2, wp2, G1, L1, Hi2, Wi2, c1, part_db1, &smem);
     LPB_REQUIRE(smem <= HEAD_STAGE_SMEM_BUDGET && p.R2 >= 1, "head_bwd_bf16: layer-2 width %d too large", Wi2);
-    int grid = B < 2 * sms ? B : 2 * sms;
-    if (grid > B2D_MAX_CTAS) grid = B2D_MAX_CTAS;  // the bias partials' workspace
     if (!wide) {
       LPB_TRY(set_dynamic_smem(b2d_dgrad_kernel<false>, smem, "head_bwd_bf16"));
       b2d_dgrad_kernel<false><<<grid, B2D_THREADS, smem, s>>>(p);
@@ -1500,4 +1554,47 @@ extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targe
   }
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
+}
+
+extern "C" int lpb_head_bwd_bf16_targets(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win,
+                                         const int32_t* win_meta, const float* g_overflow, const void* saved_xs,
+                                         const void* fwd_workspace, int B, int C, int H, int W, const float* w1, int c1,
+                                         const float* w2, int c2, int feature_layout, void* dfeat, float* dw1, float* db1,
+                                         float* dw2, float* db2, void* workspace, void* stream) {
+  return head_bwd(g_out, mse, probs, win, win_meta, g_overflow, saved_xs, fwd_workspace, B, C, H, W, w1, c1, w2, c2, feature_layout, dfeat,
+                  dw1, db1, dw2, db2, workspace, stream);
+}
+
+// ---- three-deconv heads (lpb200.h) -----------------------------------------------------------------------------------
+extern "C" int lpb_head3_query(int B, int C, int H, int W, int c1, int c2, int c3, int feature_layout, int train, lpb_head3_sizes* sizes) {
+  using namespace lpb;
+  LPB_REQUIRE(sizes, "head3_query: null pointer");
+  LPB_REQUIRE(feature_layout == LPB_FEATURES_NCHW || feature_layout == LPB_FEATURES_NHWC, "head3_query: unknown feature layout %d", feature_layout);
+  LPB_REQUIRE(B >= 0 && C >= 128 && C % 128 == 0 && H >= 1 && W >= 1 && c1 >= 1 && c2 >= 1 && c3 >= 1, "head3_query: bad shape");
+  memset(sizes, 0, sizeof(*sizes));
+  const char* why = nullptr;
+  if (!head3_covered(H, W, c1, c2, c3, train != 0, &why)) {
+    set_error("head3_query: %dx%d features, channels %d/%d/%d: %s", H, W, c1, c2, c3, why);
+    return LPB_ERR_UNSUPPORTED;
+  }
+  LPB_TRY(lpb_head_bf16_plan_layout(C, H, W, c1, c2, feature_layout, &sizes->plan));
+  sizes->fwd_workspace = head_fwd_layout(B, C, H, W, c1, c2, c3).total;
+  LPB_TRY(lpb_head_bf16_saved_bytes(B, C, H, W, &sizes->saved));
+  if (train) {
+    LPB_TRY(head_bwd_covers("head3_query", H, W, c1, c2, feature_layout));
+    sizes->bwd_workspace = head_bwd_layout(B, C, H, W, c1, c2, false, c3).total;
+    sizes->bwd_workspace_targets = head_bwd_layout(B, C, H, W, c1, c2, true, c3).total;
+  }
+  return LPB_OK;
+}
+
+extern "C" int lpb_head3_bwd(const float* g_out, const lpb_mse_targets* mse, const float* probs, const float* win, const int32_t* win_meta,
+                             const float* g_overflow, const void* saved_xs, const void* fwd_workspace, int feature_layout, int B, int C,
+                             int H, int W, const float* w1, int c1, const float* w2, int c2, const float* w3, int c3, void* dfeat, float* dw1,
+                             float* db1, float* dw2, float* db2, float* dw3, float* db3, void* workspace, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(w2 && w3 && dw2 && db2 && dw3 && db3, "head3_bwd: null pointer");
+  LPB_REQUIRE(c1 >= 1 && c2 >= 1 && c3 >= 1, "head3_bwd: bad channel counts %d/%d/%d", c1, c2, c3);
+  return head_bwd(g_out, mse, probs, win, win_meta, g_overflow, saved_xs, fwd_workspace, B, C, H, W, w1, c1, w2, c2, feature_layout, dfeat,
+                  dw1, db1, dw2, db2, workspace, stream, w3, c3, dw3, db3);
 }

@@ -89,18 +89,23 @@ __host__ __device__ constexpr bool head_wide(int c1, int c2) {
   return c2 == 0 ? c1 > HEAD_CLS && c1 <= HEAD_MAX_CH : c1 >= 1 && c1 <= HEAD_MAX_CH && c2 > HEAD_CLS && c2 <= HEAD_MAX_CH;
 }
 static_assert(head_groups(HEAD_CLS) == 1 && head_mid_stages(HEAD_CLS - 1) == 1, "narrow heads: one group, one mid stage");
+// Three-deconv heads (downsample factor 1 on a stride-32 backbone) the 16-bit kernels serve: narrow only, every layer one
+// keypoint group, and room for the constant-one channel in both mid activations (c1, c2 < HEAD_CLS).
+__host__ __device__ constexpr bool head_narrow3(int c1, int c2, int c3) {
+  return c1 >= 1 && c1 < HEAD_CLS && c2 >= 1 && c2 < HEAD_CLS && c3 >= 1 && c3 <= HEAD_CLS;
+}
 
 struct PrepJobs {
   // forward operand packs: W[Cin][Cout][3][3] -> B[group][stage][shift][kchunk][80][8] of the launch's operand type T
-  // (head_bf16.cu)
-  struct { const float* w; const float* bias; int Cin, Cout, nstages, ngroups; void* out; } fpack[2];
+  // (head_bf16.cu); one per deconv (three-deconv heads use the third)
+  struct { const float* w; const float* bias; int Cin, Cout, nstages, ngroups; void* out; } fpack[3];
   // data-gradient operand packs: -> [kgroup][tile][shift][kchunk][rows_per_tile][8]    (head_bwd_bf16.cu): K is one
   // keypoint group of the layer's output channels (kgroups of them), row r of tile t is input channel tile_ch t + r
   // (rows r >= tile_ch are zero); always bf16
-  struct { const float* w; int Cin, Cout, ntiles, rows_per_tile, tile_ch, kgroups; __nv_bfloat16* out; } dpack[2];
+  struct { const float* w; int Cin, Cout, ntiles, rows_per_tile, tile_ch, kgroups; __nv_bfloat16* out; } dpack[3];
   // pad rows of row-layout buffers of 2-byte elements (zero in either type)
-  struct { void* buf; RowLayout L; long long nslabs; } pads[2];
-  struct { float* p; long long n; } zero[4];
+  struct { void* buf; RowLayout L; long long nslabs; } pads[3];
+  struct { float* p; long long n; } zero[6];
 };
 
 template <typename T = __nv_bfloat16>

@@ -69,23 +69,51 @@ inline size_t convt_rows_partials_bytes(int B, int ngroups, int Hi, int Wi) {
   return (size_t)B * ngroups * convt_rows_bands(Hi, Wi) * HEAD_CLS * 2 * sizeof(float);
 }
 
-// Byte offsets into the forward's workspace (lpb_head_fwd_bf16): [packed w1][packed w2][mid activations][split-softmax
-// statistics of the last layer].  mid (padded row layout, channel c1 the constant one, 4 * head_mid_stages(c1) K-chunks)
-// exists for two-deconv heads only; one w2 stage is reserved for one-deconv heads as well.  Packs and statistics hold
-// one block per keypoint group.  The backward reads mid from here.
+// Byte offsets into the forward's workspace (lpb_head_fwd_bf16, lpb_head3_fwd): [packed w1][packed w2][packed w3][mid
+// activations][mid2][split-softmax statistics of the last layer].  mid (padded row layout, channel c1 the constant one,
+// 4 * head_mid_stages(c1) K-chunks) exists for two- and three-deconv heads; mid2 (8H x 8W, channel c2 the constant one)
+// and the w3 pack for three-deconv heads only (c3 > 0; narrow, head_narrow3), and for every other head the layout is
+// the two-layer one.  One w2 stage is reserved for one-deconv heads as well.  Packs and statistics hold one block per
+// keypoint group.  The backward reads mid and mid2 from here.
 struct HeadFwdLayout {
-  size_t w1, w2, mid, partials, total;
+  size_t w1, w2, w3, mid, mid2, partials, total;
 };
-inline HeadFwdLayout head_fwd_layout(int B, int C, int H, int W, int c1, int c2) {
+inline HeadFwdLayout head_fwd_layout(int B, int C, int H, int W, int c1, int c2, int c3 = 0) {
   HeadFwdLayout l;
+  const bool three = c2 > 0 && c3 > 0;
   const int nst2 = c2 > 0 ? head_mid_stages(c1) : 1, g1 = head_groups(c1), g2 = c2 > 0 ? head_groups(c2) : 1;
+  const int nst3 = three ? head_mid_stages(c2) : 0;
   l.w1 = 0;
   l.w2 = (size_t)g1 * (C / 4 / HEAD_KSTAGE) * HEAD_BSTAGE_BYTES;
-  l.mid = l.w2 + (size_t)g2 * nst2 * HEAD_BSTAGE_BYTES;
-  l.partials = l.mid + (c2 > 0 ? (size_t)B * 4 * nst2 * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
-  const size_t part = c2 > 0 ? convt_rows_partials_bytes(B, g2, 4 * H, 4 * W) : convt_rows_partials_bytes(B, g1, 2 * H, 2 * W);
+  l.w3 = l.w2 + (size_t)g2 * nst2 * HEAD_BSTAGE_BYTES;
+  l.mid = l.w3 + (size_t)nst3 * HEAD_BSTAGE_BYTES;
+  l.mid2 = l.mid + (c2 > 0 ? (size_t)B * 4 * nst2 * make_row_layout(4 * H, 4 * W).rows * 16 : 0);
+  l.partials = l.mid2 + (three ? (size_t)B * 4 * nst3 * make_row_layout(8 * H, 8 * W).rows * 16 : 0);
+  const size_t part = three    ? convt_rows_partials_bytes(B, 1, 8 * H, 8 * W)
+                      : c2 > 0 ? convt_rows_partials_bytes(B, g2, 4 * H, 4 * W)
+                               : convt_rows_partials_bytes(B, g1, 2 * H, 2 * W);
   l.total = l.partials + ((part + 255) & ~(size_t)255);
   return l;
+}
+
+// The three-deconv heads the 16-bit kernels serve, forward and backward alike (lpb200.h lpb_head3_query): narrow
+// channels (head_narrow3), feature widths W in {4, 8, 12, 16} -- the backward's data-gradient widths whose layer-3 input
+// (8W + 1 raster rows per image row) fits one band of the banded kernel -- H * W a multiple of 8, and H even to train.
+// True when covered; otherwise `why` names the first rule the shape breaks.
+inline bool head3_covered(int H, int W, int c1, int c2, int c3, bool train, const char** why) {
+  if (!head_narrow3(c1, c2, c3)) {
+    *why = "channel counts outside the narrow three-deconv set (c1, c2 <= 19, c3 <= 20)";
+    return false;
+  }
+  if (!(W == 4 || W == 8 || W == 12 || W == 16) || 8 * W + 1 > CR_BAND_ROWS) {
+    *why = "feature width outside {4, 8, 12, 16}";
+    return false;
+  }
+  if (H < 1 || (H * W) % 8 != 0 || (train && H % 2 != 0)) {
+    *why = train ? "feature height must be even to train" : "H * W must be a multiple of 8";
+    return false;
+  }
+  return true;
 }
 
 }  // namespace lpb

@@ -72,7 +72,7 @@ class _HeadFunction(torch.autograd.Function):
     """Fused head, optionally with the soft-argmax decode riding along (``decode = (ds, temperature)``).
 
     Forward: bf16 tensor-core head for bf16 features and, when no backward follows, fp16 tensor-core head for fp16
-    features (one- or two-deconv heads inside its tiling), the fp32 (3xTF32 tensor-core) kernels otherwise (+ decode
+    features (one-, two- and three-deconv heads inside its tiling), the fp32 (3xTF32 tensor-core) kernels otherwise (+ decode
     kernel).  Backward: native in both cases.  On the tensor-core path the gradient
     w.r.t. the heatmaps is never materialised for the decode branch: the sparse decode windows, a dense heatmap-loss
     gradient if there is one, and the softmax backward are all folded into the kernel that writes the
@@ -142,11 +142,13 @@ class _HeadFunction(torch.autograd.Function):
             windows = None
             if g_xy is not None:
                 windows = ops.decode_backward_windows(out, stats, g_xy.contiguous().float(), int(ctx.decode[0]), float(ctx.decode[1]))
-            dfeat, dw1, db1, dw2, db2 = ops.head_backward_bf16(
-                g, ctx.saved, tuple(features.shape), weights[0], weights[1] if n == 2 else None, need_dfeat=need_dfeat,
+            grads = ops.head_backward_bf16(
+                g, ctx.saved, tuple(features.shape), weights[0], weights[1] if n >= 2 else None, need_dfeat=need_dfeat,
                 probs=out if ctx.final_softmax else None, windows=windows, layout=ctx.layout, mse=mse,
+                w3=weights[2] if n == 3 else None,
             )
-            dws, dbs = ([dw1, dw2], [db1, db2]) if n == 2 else ([dw1], [db1])
+            dfeat = grads[0]
+            dws, dbs = list(grads[1::2][:n]), list(grads[2::2][:n])
             return (dfeat, None, None, None, *[d.to(w.dtype) for d, w in zip(dws, weights)], *[d.to(b.dtype) for d, b in zip(dbs, biases)])
         # fp32 path: dense decode gradient, softmax backward, then the deconvs' own backward kernels, last layer first
         if g_xy is not None:

@@ -14,7 +14,7 @@ import torch
 
 import torch.utils._pytree
 
-from ._lib import MseTargets, PcaDesc, check, lib
+from ._lib import Head3Sizes, MseTargets, PcaDesc, check, lib
 
 __all__ = [
     "decode_softargmax",
@@ -25,6 +25,7 @@ __all__ = [
     "head_forward",
     "head_forward_f32",
     "head_bf16_supported",
+    "head3_supported",
     "convt_forward_f32",
     "convt_backward_f32",
     "head_backward_bf16",
@@ -260,23 +261,41 @@ def head_bf16_supported(shape, channels, train: bool, layout: int = FEATURES_NCH
     return not train or lib.lpb_head_bwd_bf16_workspace_bytes_layout(b, c, h, w, c1, c2, layout, C.byref(nbytes)) == 0
 
 
+def _head3_sizes(shape, channels, train: bool, layout: int) -> tuple[int, Head3Sizes]:
+    """``lpb_head3_query``'s return code and sizes for a three-deconv head (c1, c2, c3) on features of ``shape``."""
+    b, c, h, w = shape
+    sizes = Head3Sizes()
+    return lib.lpb_head3_query(b, c, h, w, *channels, layout, int(train), C.byref(sizes)), sizes
+
+
+def head3_supported(shape, channels, train: bool, layout: int = FEATURES_NCHW) -> bool:
+    """``head_bf16_supported`` for three-deconv heads (``downsample_factor=1`` on a stride-32 backbone): whether the
+    tensor-core kernels cover feature shape (B, C, H, W) with deconv output channels (c1, c2, c3) in memory format
+    ``layout``, to train (``train``) or to predict.  The library owns the rule (``lpb_head3_query``, no GPU needed)."""
+    if len(channels) != 3:
+        return False
+    return _head3_sizes(tuple(shape), [int(x) for x in channels], train, layout)[0] == 0
+
+
 def head_16_operand(features, channels, train: bool):
     """``(features as the 16-bit head reads them, layout)`` or None when the tensor-core kernels do not cover the head.
 
     Channels-last features are read in place where the kernels take them.  Where only the NCHW kernels cover the shape
-    (training at W = 32), and for every tensor that is neither format, this is the NCHW copy."""
+    (training at W = 32), and for every tensor that is neither format, this is the NCHW copy.  Three-deconv heads are
+    asked of ``head3_supported``, every other head of ``head_bf16_supported``."""
+    supported = head3_supported if len(channels) == 3 else head_bf16_supported
     layout = feature_layout(features)
-    if layout == FEATURES_NHWC and head_bf16_supported(tuple(features.shape), channels, train, FEATURES_NHWC):
+    if layout == FEATURES_NHWC and supported(tuple(features.shape), channels, train, FEATURES_NHWC):
         return features, FEATURES_NHWC
-    if head_bf16_supported(tuple(features.shape), channels, train):
+    if supported(tuple(features.shape), channels, train):
         return features.contiguous(), FEATURES_NCHW
     return None
 
 
 def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=False, layout=FEATURES_NCHW):
-    """tensor-core path (one- or two-deconv heads) on 16-bit features: bf16 (``lpb_head_fwd_bf16``) or fp16
-    (``lpb_head_fwd_f16``), the weights rounded to the features' dtype on the device; the caller checks
-    ``head_bf16_supported`` first.  Both share the plan and the buffer sizes.  ``layout``: the memory format ``f`` is
+    """tensor-core path (one-, two- or three-deconv heads) on 16-bit features: bf16 (``lpb_head_fwd_bf16``) or fp16
+    (``lpb_head_fwd_f16``), and ``lpb_head3_fwd`` for three deconvs, the weights rounded to the features' dtype on the
+    device; the caller checks ``head_16_operand`` first.  Both dtypes share the plan and the buffer sizes.  ``layout``: the memory format ``f`` is
     dense in (``FEATURES_NCHW``: contiguous; ``FEATURES_NHWC``: channels-last, read in place).
 
     ``train=True`` (bf16 only: there is no fp16 backward) returns ``(out, saved)`` where ``saved`` carries what
@@ -293,26 +312,41 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
     n = len(weights)
     w1 = _cuda_f32(weights[0], "weight")
     b1 = _cuda_f32(biases[0], "bias")
-    w2 = _cuda_f32(weights[1], "weight") if n == 2 else None
-    b2 = _cuda_f32(biases[1], "bias") if n == 2 else None
-    c1, c2 = w1.shape[1], (w2.shape[1] if n == 2 else 0)
-    plan = C.c_int(0)
-    check(lib.lpb_head_bf16_plan_layout(c, h, w, c1, c2, layout, C.byref(plan)))
+    w2 = _cuda_f32(weights[1], "weight") if n >= 2 else None
+    b2 = _cuda_f32(biases[1], "bias") if n >= 2 else None
+    w3 = _cuda_f32(weights[2], "weight") if n == 3 else None
+    b3 = _cuda_f32(biases[2], "bias") if n == 3 else None
+    c1, c2, c3 = w1.shape[1], (w2.shape[1] if n >= 2 else 0), (w3.shape[1] if n == 3 else 0)
     nbytes = C.c_size_t(0)
-    check(lib.lpb_head_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)))
-    ws = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
-    up = 8 if n == 2 else 4
-    out = torch.empty((b, c2 if n == 2 else c1, up * h, up * w), device=f.device, dtype=torch.float32)
+    if n == 3:
+        rc, sizes = _head3_sizes((b, c, h, w), (c1, c2, c3), train, layout)
+        check(rc)
+        plan, ws_bytes, xs_bytes = sizes.plan, sizes.fwd_workspace, sizes.saved
+    else:
+        plan_c = C.c_int(0)
+        check(lib.lpb_head_bf16_plan_layout(c, h, w, c1, c2, layout, C.byref(plan_c)))
+        check(lib.lpb_head_bf16_workspace_bytes(b, c, h, w, c1, c2, C.byref(nbytes)))
+        plan, ws_bytes = plan_c.value, nbytes.value
+    ws = torch.empty((ws_bytes,), device=f.device, dtype=torch.uint8)
+    up = {1: 4, 2: 8, 3: 16}[n]
+    out = torch.empty((b, (c1, c2, c3)[n - 1], up * h, up * w), device=f.device, dtype=torch.float32)
     xs = None
-    if train or plan.value == 0:  # row-layout copy of the shuffled features: the banded path's operand / the wgrad's input
-        check(lib.lpb_head_bf16_saved_bytes(b, c, h, w, C.byref(nbytes)))
-        xs = torch.empty((nbytes.value,), device=f.device, dtype=torch.uint8)
+    if train or plan == 0:  # row-layout copy of the shuffled features: the banded path's operand / the wgrad's input
+        if n != 3:
+            check(lib.lpb_head_bf16_saved_bytes(b, c, h, w, C.byref(nbytes)))
+            xs_bytes = nbytes.value
+        xs = torch.empty((xs_bytes,), device=f.device, dtype=torch.uint8)
     hints = None
     with torch.cuda.device(f.device):
         if want_hints and final_softmax:
             rows, nbands = C.c_int(0), C.c_int(0)
             check(lib.lpb_head_band_max_dims(out.shape[2], out.shape[3], C.byref(rows), C.byref(nbands)))
             hints = BandMax(torch.empty((b, out.shape[1], nbands.value, 8), device=f.device, dtype=torch.int32), rows.value, nbands.value)
+        if n == 3:
+            check(lib.lpb_head3_fwd(_ptr(f), _OPERAND_16[f.dtype], layout, b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, _ptr(w3),
+                                    _ptr(b3), c3, int(bool(final_softmax)), _ptr(out), _ptr(hints.bits if hints is not None else None), _ptr(xs),
+                                    _ptr(ws), _stream()))
+        elif want_hints and final_softmax:
             check(_HEAD_FWD_16_BAND_MAX[f.dtype](_ptr(f), b, c, h, w, _ptr(w1), _ptr(b1), c1, _ptr(w2), _ptr(b2), c2, layout, _ptr(out),
                                                  _ptr(hints.bits), _ptr(xs), _ptr(ws), _stream()))
         else:
@@ -326,6 +360,7 @@ def _head_forward_16(f, weights, biases, final_softmax, train=False, want_hints=
 
 _HEAD_FWD_16 = {torch.bfloat16: lib.lpb_head_fwd_bf16_layout, torch.float16: lib.lpb_head_fwd_f16_layout}
 _HEAD_FWD_16_BAND_MAX = {torch.bfloat16: lib.lpb_head_fwd_bf16_band_max, torch.float16: lib.lpb_head_fwd_f16_band_max}
+_OPERAND_16 = {torch.bfloat16: 1, torch.float16: 2}  # LPB_OUT_BF16, LPB_OUT_F16 (lpb200.h)
 _head_forward_bf16 = _head_forward_16  # the name bench.py and the bf16 tests call
 
 
@@ -343,9 +378,10 @@ def decode_backward_windows(heatmaps, stats, grad_xy, ds, temperature):
     return win, meta, overflow
 
 
-def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None, layout=FEATURES_NCHW, mse=None):
-    """Gradients of the bf16 head: returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None).  ``dfeat`` is dense in
-    ``layout``, the memory format the forward read the features in.
+def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=None, windows=None, layout=FEATURES_NCHW, mse=None, w3=None):
+    """Gradients of the bf16 head: returns (dfeat bf16 | None, dw1, db1, dw2 | None, db2 | None), and for a three-deconv
+    head (``w3`` given, ``lpb_head3_bwd``) also dw3, db3.  ``dfeat`` is dense in ``layout``, the memory format the
+    forward read the features in.
 
     ``g_out``: dense gradient w.r.t. the head output or None; ``probs``: the head output when it ends in the
     spatial softmax (its backward is fused in), None for a logits head; ``windows``: result of
@@ -361,10 +397,16 @@ def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=
         raise ValueError("head_backward_bf16: `mse` stands for the dense gradient of a loss on `probs`")
     w1 = _cuda_f32(w1, "w1")
     w2 = _cuda_f32(w2, "w2") if w2 is not None else None
+    w3 = _cuda_f32(w3, "w3") if w3 is not None else None
     c1, c2 = w1.shape[1], (w2.shape[1] if w2 is not None else 0)
     dev = w1.device
     nbytes = C.c_size_t(0)
-    check(lib.lpb_head_bwd_bf16_workspace_bytes_targets(b, c, h, w, c1, c2, layout, int(mse is not None), C.byref(nbytes)))
+    if w3 is not None:
+        rc, sizes = _head3_sizes((b, c, h, w), (c1, c2, w3.shape[1]), True, layout)
+        check(rc)
+        nbytes.value = sizes.bwd_workspace_targets if mse is not None else sizes.bwd_workspace
+    else:
+        check(lib.lpb_head_bwd_bf16_workspace_bytes_targets(b, c, h, w, c1, c2, layout, int(mse is not None), C.byref(nbytes)))
     ws = torch.empty((nbytes.value,), device=dev, dtype=torch.uint8)
     fmt = torch.channels_last if layout == FEATURES_NHWC else torch.contiguous_format
     dfeat = torch.empty((b, c, h, w), device=dev, dtype=torch.bfloat16, memory_format=fmt) if need_dfeat else None
@@ -374,6 +416,15 @@ def head_backward_bf16(g_out, saved, feat_shape, w1, w2, need_dfeat=True, probs=
     db2 = torch.empty((c2,), device=dev, dtype=torch.float32) if w2 is not None else None
     win, meta, ov = windows if windows is not None else (None, None, None)
     targets = C.byref(mse.targets()) if mse is not None else None
+    if w3 is not None:
+        c3 = w3.shape[1]
+        dw3 = torch.empty_like(w3)
+        db3 = torch.empty((c3,), device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            check(lib.lpb_head3_bwd(_ptr(g), targets, _ptr(probs), _ptr(win), _ptr(meta), _ptr(ov), _ptr(xs), _ptr(fws), layout, b, c, h, w, _ptr(w1),
+                                    c1, _ptr(w2), c2, _ptr(w3), c3, _ptr(dfeat), _ptr(dw1), _ptr(db1), _ptr(dw2), _ptr(db2), _ptr(dw3), _ptr(db3),
+                                    _ptr(ws), _stream()))
+        return dfeat, dw1, db1, dw2, db2, dw3, db3
     with torch.cuda.device(dev):
         check(lib.lpb_head_bwd_bf16_targets(_ptr(g), targets, _ptr(probs), _ptr(win), _ptr(meta), _ptr(ov), _ptr(xs), _ptr(fws), b, c, h, w, _ptr(w1), c1,
                                             _ptr(w2), c2, layout, _ptr(dfeat), _ptr(dw1), _ptr(db1), _ptr(dw2), _ptr(db2), _ptr(ws), _stream()))
@@ -450,7 +501,7 @@ def head_forward(features, weights, biases, final_softmax=True):
     """PixelShuffle(2) + ConvTranspose2d stack + spatial softmax; forward only.
 
     bf16 and fp16 features take the 16-bit tensor-core kernels (operands in the features' dtype, fp32 accumulate, fp32
-    heatmaps) when the head is a one- or two-deconv head the tiling covers; everything else takes the full-precision
+    heatmaps) when the head is a one-, two- or three-deconv head the tiling covers; everything else takes the full-precision
     kernels (3xTF32 on the tensor cores, any depth and keypoint count).  Training uses
     ``HeatmapHead`` which adds the backward.
     """
