@@ -405,6 +405,32 @@ int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V, int F, co
                                int out_w, const float* mean3, const float* std3, int layout, int out_format, void* out,
                                void* stream);
 
+/* ---- ragged video ingest: a chunk of frames from videos of several sizes, in one launch ----------------------------
+ * the reference's directory prediction (one reader per video, each resizing from its own size to resize_dims,
+ * lightning_pose/data/video/dali.py:155, opencv.py:209-212) over one frame stream.
+ * arena: F slots of slot_bytes each (DEVICE, 16-byte aligned, slot_bytes a positive multiple of 16); frame f is uint8
+ * [H, W, 3] with packed rows at arena + f * slot_bytes (64-bit offsets).  videos [n_videos][3] (DEVICE int64, 8-byte
+ * aligned): first global row, H, W of each video of the list, back to back; videos_host is the same table on the host,
+ * checked here: video 0 starts at row 0, first rows increase, every H * W * 3 <= slot_bytes.  Frame f has global row
+ * *cursor + f (DEVICE int64, read, never advanced) and the size of the video holding that row; rows past the last
+ * video's first row belong to it, so the padding of a list's last chunk takes the last video's size.  No argument
+ * depends on the chunk: one captured graph serves every mix of sizes.
+ * lpb_frames_normalize_ragged: out as lpb_frames_normalize (layout, out_format, mean3 / std3 HOST arrays); every output
+ * image is bit-identical to lpb_frames_normalize on that frame alone (a frame already at out_h x out_w is copied and
+ * normalised).  boxes_out [F, 4] fp32: [0, 0, H, W], the whole frame, for lpb_remap_keypoints.
+ * lpb_frames_crop_normalize_ragged: lpb_frames_crop_normalize (in_f32 = 0) with each frame's own size: box row
+ * min(*cursor + f, n_boxes - 1); each frame's output and clamped box are bit-identical to lpb_frames_crop_normalize on
+ * its own video alone.
+ * F <= 65535, out_h * out_w < 2^31.  Null pointers, an empty table or one the host copy refuses, a misaligned arena or
+ * table: LPB_ERR_INVALID.  F = 0 is a no-op. */
+int lpb_frames_normalize_ragged(const uint8_t* arena, int64_t slot_bytes, int F, const int64_t* cursor, const int64_t* videos,
+                                const int64_t* videos_host, int n_videos, int out_h, int out_w, const float* mean3,
+                                const float* std3, int layout, int out_format, void* out, float* boxes_out, void* stream);
+int lpb_frames_crop_normalize_ragged(const uint8_t* arena, int64_t slot_bytes, int F, const int64_t* cursor,
+                                     const int64_t* videos, const int64_t* videos_host, int n_videos, const float* boxes,
+                                     int64_t n_boxes, int out_h, int out_w, const float* mean3, const float* std3, int layout,
+                                     int out_format, void* out, float* boxes_out, void* stream);
+
 /* ---- augmented video ingest: the unlabeled branch's DALI augmentation ----------------------------------------
  * replaces  lightning_pose/data/video/dali.py:154-192  (training.imgaug "dlc" / "dlc-top-down") in front of the
  * normalisation of lpb_frames_normalize, one view, one draw per call.  Per frame of frames_u8 [F, H, W, 3]:

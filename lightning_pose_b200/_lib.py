@@ -112,6 +112,10 @@ SIGNATURES = {
     "lpb_context_gather_bwd": (C.c_int, [_P, _L, _L, _I, _I, _P, _P]),
     "lpb_frames_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
     "lpb_frames_normalize_views": (C.c_int, [C.POINTER(_P), _I, _I, C.POINTER(_I), C.POINTER(_I), _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P]),
+    "lpb_frames_normalize_ragged": (C.c_int, [_P, _L, _I, _P, _P, _P, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I,
+                                              _P, _P, _P]),
+    "lpb_frames_crop_normalize_ragged": (C.c_int, [_P, _L, _I, _P, _P, _P, _I, _P, _L, _I, _I, C.POINTER(C.c_float),
+                                                   C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
     "lpb_frames_augment_normalize": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
     "lpb_frames_crop_resize_cv2": (C.c_int, [_P, _I, _I, _I, _P, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _I, _I, _P, _P, _P]),
     "lpb_patch_mask_select": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _L, C.c_double, C.c_double, _P, _P]),

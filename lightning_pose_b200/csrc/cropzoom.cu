@@ -28,6 +28,10 @@ struct CropParams {
   int64_t n_boxes, row0;
   int F, H, W, OH, OW;
   float scale[3], shift[3];  // out = px * scale + shift (uint8 input only)
+  // ragged arena (uint8 input only): frame f in slot f, its size from the video table at row *cursor + f
+  const int64_t* videos;     // [n_videos][3]: first row, H, W
+  int64_t slot_bytes;
+  int n_videos;
 };
 
 // Python's int() of a float: truncation toward zero.  Clamped first so that the conversion is defined; far outside any
@@ -37,33 +41,47 @@ __device__ __forceinline__ long long trunc_ll(float v) { return (long long)fminf
 // Clamp of crop_and_resize_frames (data/bboxes.py:321-326) for frame f.  Two deliberate divergences, where the reference
 // raises: an origin at or past the far edge is clamped to the last pixel (a one-pixel crop), and a row holding a NaN or
 // an infinity is the whole frame.
-__device__ __forceinline__ void crop_box(const CropParams& P, int f, int& x1, int& y1, int& x2, int& y2) {
+// frame f of H x W pixels.
+__device__ __forceinline__ void crop_box(const CropParams& P, int f, int H, int W, int& x1, int& y1, int& x2, int& y2) {
   int64_t r = (P.cursor ? *P.cursor : P.row0) + f;
   r = r < 0 ? 0 : (r > P.n_boxes - 1 ? P.n_boxes - 1 : r);  // past the end: the final row (dali.py:355-361)
   const float bx = P.boxes[r * 4 + 0], by = P.boxes[r * 4 + 1], bh = P.boxes[r * 4 + 2], bw = P.boxes[r * 4 + 3];
   if (!(isfinite(bx) && isfinite(by) && isfinite(bh) && isfinite(bw))) {
-    x1 = 0, y1 = 0, x2 = P.W, y2 = P.H;
+    x1 = 0, y1 = 0, x2 = W, y2 = H;
     return;
   }
   const long long xi = trunc_ll(bx), yi = trunc_ll(by);
-  const long long xa = min(max(0LL, xi), (long long)P.W - 1), ya = min(max(0LL, yi), (long long)P.H - 1);
+  const long long xa = min(max(0LL, xi), (long long)W - 1), ya = min(max(0LL, yi), (long long)H - 1);
   x1 = (int)xa, y1 = (int)ya;
-  x2 = (int)max(xa + 1, min((long long)P.W, xi + trunc_ll(bw)));  // far edge from the UNclamped origin
-  y2 = (int)max(ya + 1, min((long long)P.H, yi + trunc_ll(bh)));
+  x2 = (int)max(xa + 1, min((long long)W, xi + trunc_ll(bw)));  // far edge from the UNclamped origin
+  y2 = (int)max(ya + 1, min((long long)H, yi + trunc_ll(bh)));
 }
 
+// channel c of pixel (y, x) of one H x W frame at img: fp32 [3, H, W] or uint8 [H, W, 3]
 template <bool IN_F32>
-__device__ __forceinline__ float load_px(const CropParams& P, int f, int c, int y, int x) {
-  if (IN_F32) return static_cast<const float*>(P.in)[(((size_t)f * 3 + c) * P.H + y) * P.W + x];
-  return (float)static_cast<const uint8_t*>(P.in)[(((size_t)f * P.H + y) * P.W + x) * 3 + c];
+__device__ __forceinline__ float load_px(const void* img, int H, int W, int c, int y, int x) {
+  if (IN_F32) return static_cast<const float*>(img)[((size_t)c * H + y) * W + x];
+  return (float)static_cast<const uint8_t*>(img)[((size_t)y * W + x) * 3 + c];
 }
 
-// grid (x-blocks, F): each block computes its frame's box, then strides over that frame's output pixels.
-template <bool IN_F32, int LAYOUT, int FMT>
+// grid (x-blocks, F): each block computes its frame's box, then strides over that frame's output pixels.  RAGGED: the
+// frame is slot f of a uint8 arena and its size that of its video (ragged_video at row *cursor + f).
+template <bool IN_F32, int LAYOUT, int FMT, bool RAGGED = false>
 __global__ void __launch_bounds__(256) crop_kernel(const __grid_constant__ CropParams P) {
   const int f = blockIdx.y;
+  int H = P.H, W = P.W;
+  const void* img;
+  if (RAGGED) {
+    const int vid = ragged_video(P.videos, P.n_videos, *P.cursor + f);
+    H = (int)P.videos[3 * vid + 1], W = (int)P.videos[3 * vid + 2];
+    img = static_cast<const uint8_t*>(P.in) + (size_t)f * P.slot_bytes;
+  } else if (IN_F32) {
+    img = static_cast<const float*>(P.in) + (size_t)f * 3 * H * W;
+  } else {
+    img = static_cast<const uint8_t*>(P.in) + (size_t)f * H * W * 3;
+  }
   int x1, y1, x2, y2;
-  crop_box(P, f, x1, y1, x2, y2);
+  crop_box(P, f, H, W, x1, y1, x2, y2);
   const int ch = y2 - y1, cw = x2 - x1;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     float* b = P.boxes_out + (size_t)f * 4;
@@ -83,8 +101,8 @@ __global__ void __launch_bounds__(256) crop_kernel(const __grid_constant__ CropP
     float v[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float a = load_px<IN_F32>(P, f, c, y1 + ya, x1 + xa), b = load_px<IN_F32>(P, f, c, y1 + ya, x1 + xb);
-      const float d = load_px<IN_F32>(P, f, c, y1 + yb, x1 + xa), e = load_px<IN_F32>(P, f, c, y1 + yb, x1 + xb);
+      const float a = load_px<IN_F32>(img, H, W, c, y1 + ya, x1 + xa), b = load_px<IN_F32>(img, H, W, c, y1 + ya, x1 + xb);
+      const float d = load_px<IN_F32>(img, H, W, c, y1 + yb, x1 + xa), e = load_px<IN_F32>(img, H, W, c, y1 + yb, x1 + xb);
       v[c] = __fadd_rn(__fmul_rn(ly0, __fadd_rn(__fmul_rn(lx0, a), __fmul_rn(lx1, b))),
                        __fmul_rn(ly1, __fadd_rn(__fmul_rn(lx0, d), __fmul_rn(lx1, e))));
       if (!IN_F32) v[c] = fmaf(v[c], P.scale[c], P.shift[c]);
@@ -201,6 +219,7 @@ extern "C" int lpb_frames_crop_normalize(const void* frames, int in_f32, int F, 
   p.in = frames, p.boxes = boxes, p.cursor = cursor, p.out = out, p.boxes_out = boxes_out;
   p.n_boxes = n_boxes, p.row0 = row0;
   p.F = F, p.H = H, p.W = W, p.OH = out_h, p.OW = out_w;
+  p.videos = nullptr, p.slot_bytes = 0, p.n_videos = 0;
   for (int c = 0; c < 3; ++c) {  // mean3 / std3 are HOST arrays, as for lpb_frames_normalize
     p.scale[c] = 1.f, p.shift[c] = 0.f;
     if (in_f32) continue;
@@ -219,6 +238,41 @@ extern "C" int lpb_frames_crop_normalize(const void* frames, int in_f32, int F, 
       case 2: crop_kernel<true, 0, FMT><<<grid, 256, 0, s>>>(p); break;
       default: crop_kernel<true, 1, FMT><<<grid, 256, 0, s>>>(p); break;
     }
+  });
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_frames_crop_normalize_ragged(const uint8_t* arena, int64_t slot_bytes, int F, const int64_t* cursor,
+                                                const int64_t* videos, const int64_t* videos_host, int n_videos,
+                                                const float* boxes, int64_t n_boxes, int out_h, int out_w, const float* mean3,
+                                                const float* std3, int layout, int out_format, void* out, float* boxes_out,
+                                                void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(arena && cursor && videos && videos_host && boxes && mean3 && std3 && out && boxes_out,
+              "frames_crop_normalize_ragged: null pointer");
+  LPB_REQUIRE(out_h >= 1 && out_w >= 1 && (int64_t)out_h * out_w < (1LL << 31) && n_boxes >= 1 && (layout == 0 || layout == 1),
+              "frames_crop_normalize_ragged: bad shape/layout");
+  LPB_REQUIRE(valid_out_format(out_format), "frames_crop_normalize_ragged: unknown output format %d", out_format);
+  LPB_TRY(check_ragged("frames_crop_normalize_ragged", arena, slot_bytes, F, videos, videos_host, n_videos));
+  CropParams p;
+  for (int c = 0; c < 3; ++c) {  // HOST arrays, as for lpb_frames_normalize
+    LPB_REQUIRE(std3[c] > 0.f, "frames_crop_normalize_ragged: std must be positive");
+    p.scale[c] = 1.0f / (255.0f * std3[c]);
+    p.shift[c] = -mean3[c] / std3[c];
+  }
+  if (F == 0) return LPB_OK;
+  p.in = arena, p.boxes = boxes, p.cursor = cursor, p.out = out, p.boxes_out = boxes_out;
+  p.n_boxes = n_boxes, p.row0 = 0;
+  p.F = F, p.H = 0, p.W = 0, p.OH = out_h, p.OW = out_w;
+  p.videos = videos, p.slot_bytes = slot_bytes, p.n_videos = n_videos;
+  const int64_t px_blocks = ((int64_t)out_h * out_w + 255) / 256;
+  dim3 grid((unsigned)(px_blocks < 64 ? px_blocks : 64), (unsigned)F);  // the grid of lpb_frames_crop_normalize
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  with_out_format(out_format, [&](auto fc) {
+    constexpr int FMT = decltype(fc)::value;
+    if (layout == 0) crop_kernel<false, 0, FMT, true><<<grid, 256, 0, s>>>(p);
+    else crop_kernel<false, 1, FMT, true><<<grid, 256, 0, s>>>(p);
   });
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;

@@ -110,6 +110,49 @@ __global__ void __launch_bounds__(256) ingest_views_kernel(const __grid_constant
   }
 }
 
+// ---- ragged ingest: a chunk whose frames come from videos of several sizes, in one launch ---------------------------
+// Frame f sits at the start of slot f of the arena (slot_bytes apart, rows packed).  Its global row *cursor + f names
+// its video in the device table (ragged_video), which gives H and W; the ratios are the ones lpb_frames_normalize
+// computes on the host (IEEE division, the same on both sides), so every output image is that entry's bits for the frame
+// alone.  Nothing but the cursor's value depends on the chunk, so one captured graph serves every mix of sizes.
+// grid (x-blocks, F): each block looks its frame's video up once, then strides over that frame's output pixels.
+struct IngestRaggedParams {
+  const uint8_t* arena;
+  const int64_t* videos;  // [n_videos][3]: first row, H, W
+  const int64_t* cursor;
+  void* out;
+  float* boxes_out;       // [F, 4]: 0, 0, H, W
+  int64_t slot_bytes;
+  int n_videos, OH, OW;
+  float scale[3], shift[3];
+};
+
+template <int LAYOUT, int FMT>
+__global__ void __launch_bounds__(256) ingest_ragged_kernel(const __grid_constant__ IngestRaggedParams P) {
+  const int f = blockIdx.y;
+  const int vid = ragged_video(P.videos, P.n_videos, *P.cursor + f);
+  const int H = (int)P.videos[3 * vid + 1], W = (int)P.videos[3 * vid + 2];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    float* b = P.boxes_out + (size_t)f * 4;
+    b[0] = 0.f, b[1] = 0.f, b[2] = (float)H, b[3] = (float)W;
+  }
+  const bool resize = H != P.OH || W != P.OW;
+  const float ry = (float)H / (float)P.OH, rx = (float)W / (float)P.OW;
+  const uint8_t* img = P.arena + (size_t)f * P.slot_bytes;
+  const int npx = P.OH * P.OW;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < npx; i += gridDim.x * blockDim.x) {
+    const int y = i / P.OW, x = i - y * P.OW;
+    float v[3];
+    if (resize)
+      resized_pixel<true>(img, H, W, ry, rx, y, x, v);
+    else
+      resized_pixel<false>(img, H, W, 0.f, 0.f, y, x, v);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = fmaf(v[c], P.scale[c], P.shift[c]);
+    store_pixel<LAYOUT, FMT>(P.out, P.OH, P.OW, f, y, x, v);
+  }
+}
+
 // ---- augmented ingest: the DALI video augmentation of dali.py:156-178 ---------------------------------------------
 // Per output pixel (f, y, x) of one view, with M = [A | t] the rotate-scale matrix (source -> destination, (x, y)):
 //   warp     the resized image sampled bilinearly at  M^-1 (x + 0.5, y + 0.5) - 0.5, taps outside it read 0.
@@ -417,6 +460,39 @@ extern "C" int lpb_frames_normalize_views(const uint8_t* const* frames_u8, int V
     constexpr int FMT = decltype(fc)::value;
     if (layout == 0) ingest_views_kernel<0, FMT><<<(unsigned)blocks, 256, 0, s>>>(p);
     else ingest_views_kernel<1, FMT><<<(unsigned)blocks, 256, 0, s>>>(p);
+  });
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_frames_normalize_ragged(const uint8_t* arena, int64_t slot_bytes, int F, const int64_t* cursor,
+                                           const int64_t* videos, const int64_t* videos_host, int n_videos, int out_h,
+                                           int out_w, const float* mean3, const float* std3, int layout, int out_format,
+                                           void* out, float* boxes_out, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(arena && cursor && videos && videos_host && mean3 && std3 && out && boxes_out, "frames_normalize_ragged: null pointer");
+  LPB_REQUIRE(out_h >= 1 && out_w >= 1 && (int64_t)out_h * out_w < (1LL << 31) && (layout == 0 || layout == 1),
+              "frames_normalize_ragged: bad shape/layout");
+  LPB_REQUIRE(valid_out_format(out_format), "frames_normalize_ragged: unknown output format %d", out_format);
+  LPB_TRY(check_ragged("frames_normalize_ragged", arena, slot_bytes, F, videos, videos_host, n_videos));
+  IngestRaggedParams p;
+  for (int c = 0; c < 3; ++c) {  // HOST arrays, as for lpb_frames_normalize
+    LPB_REQUIRE(std3[c] > 0.f, "frames_normalize_ragged: std must be positive");
+    p.scale[c] = 1.0f / (255.0f * std3[c]);
+    p.shift[c] = -mean3[c] / std3[c];
+  }
+  if (F == 0) return LPB_OK;
+  p.arena = arena, p.videos = videos, p.cursor = cursor, p.out = out, p.boxes_out = boxes_out;
+  p.slot_bytes = slot_bytes;
+  p.n_videos = n_videos, p.OH = out_h, p.OW = out_w;
+  // about as many CTAs as lpb_frames_normalize launches, split over the frames
+  const int64_t px_blocks = ((int64_t)out_h * out_w + 255) / 256, per_frame = (132 * 32 + F - 1) / F;
+  dim3 grid((unsigned)(px_blocks < per_frame ? px_blocks : per_frame), (unsigned)F);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  with_out_format(out_format, [&](auto fc) {
+    constexpr int FMT = decltype(fc)::value;
+    if (layout == 0) ingest_ragged_kernel<0, FMT><<<grid, 256, 0, s>>>(p);
+    else ingest_ragged_kernel<1, FMT><<<grid, 256, 0, s>>>(p);
   });
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;

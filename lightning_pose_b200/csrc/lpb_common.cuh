@@ -84,6 +84,42 @@ inline void with_out_format(int fmt, F&& f) {
   else f(std::integral_constant<int, LPB_OUT_F32>{});
 }
 
+// ---- ragged frame arena of the ingest entries (lpb_frames_normalize_ragged, lpb_frames_crop_normalize_ragged) ---------
+// The video of global stream row r: the last entry of videos [n][3] (first row, H, W) whose first row is <= r.  Rows
+// past the list's end fall in the last video.  A binary search over a table of a few dozen entries, read through L1.
+__device__ __forceinline__ int ragged_video(const int64_t* videos, int n, int64_t r) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (videos[3 * mid] <= r) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Host checks of an arena and its video table, shared by both ragged entries: the arena and slot_bytes 16-byte
+// aligned, the device table 8-byte aligned, and in the host copy video 0 starting at row 0, first rows increasing and
+// every frame within a slot.
+inline int check_ragged(const char* entry, const uint8_t* arena, int64_t slot_bytes, int F, const int64_t* videos,
+                        const int64_t* videos_host, int n_videos) {
+  LPB_REQUIRE(aligned_to(arena, 16) && aligned_to(videos, 8), "%s: the arena must be 16-byte aligned and the table 8-byte aligned",
+              entry);
+  LPB_REQUIRE(slot_bytes >= 16 && slot_bytes % 16 == 0, "%s: slot_bytes %lld is not a positive multiple of 16", entry,
+              (long long)slot_bytes);
+  LPB_REQUIRE(F >= 0 && F <= 65535, "%s: F = %d outside 0..65535", entry, F);
+  LPB_REQUIRE(n_videos >= 1, "%s: the video table is empty", entry);
+  for (int v = 0; v < n_videos; ++v) {
+    const int64_t row0 = videos_host[3 * v], h = videos_host[3 * v + 1], w = videos_host[3 * v + 2];
+    LPB_REQUIRE(v == 0 ? row0 == 0 : row0 > videos_host[3 * (v - 1)],
+                "%s: video %d starts at row %lld; video 0 starts at row 0 and each later one after it", entry, v, (long long)row0);
+    LPB_REQUIRE(h >= 1 && w >= 1 && h <= INT32_MAX / 3 && w <= INT32_MAX / 3, "%s: video %d has frame size %lld x %lld",
+                entry, v, (long long)h, (long long)w);
+    LPB_REQUIRE(h * w * 3 <= slot_bytes, "%s: video %d's %lld x %lld frames (%lld bytes) do not fit a %lld-byte slot", entry, v,
+                (long long)h, (long long)w, (long long)(h * w * 3), (long long)slot_bytes);
+  }
+  return LPB_OK;
+}
+
 // ---- device helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll

@@ -784,6 +784,63 @@ def frames_normalize_views(views_u8, size, mean=IMAGENET_MEAN, std=IMAGENET_STD,
     return out
 
 
+def ragged_videos(lengths, sizes) -> torch.Tensor:
+    """(n, 3) int64 host table (first row, H, W) of videos of ``lengths`` frames and ``sizes`` (H, W), back to back:
+    the video table of the ragged ingest entries (copy it to the device for their ``videos``)."""
+    lengths, sizes = [int(n) for n in lengths], [(int(h), int(w)) for h, w in sizes]
+    if len(lengths) != len(sizes):
+        raise ValueError(f"{len(lengths)} videos but {len(sizes)} frame sizes")
+    rows, row0 = [], 0
+    for n, (h, w) in zip(lengths, sizes):
+        rows.append((row0, h, w))
+        row0 += n
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 3)
+
+
+def ragged_slot_bytes(sizes) -> int:
+    """Bytes of one arena slot: the largest uint8 (H, W, 3) frame of ``sizes``, rounded up to 16."""
+    return -(-max(int(h) * int(w) * 3 for h, w in sizes) // 16) * 16
+
+
+def _ragged(arena, slot_bytes: int, frames: int, cursor, videos, videos_host) -> torch.Tensor:
+    """Checks the arena arguments shared by the ragged ingests; returns the host table, contiguous."""
+    if not isinstance(arena, torch.Tensor) or not arena.is_cuda:
+        raise RuntimeError("lpb200: `arena` must be a CUDA tensor (this package has no CPU fallback)")
+    if arena.dtype != torch.uint8 or not arena.is_contiguous() or arena.numel() < int(frames) * int(slot_bytes):
+        raise ValueError(f"arena must be a contiguous uint8 tensor of at least {int(frames)} slots of {int(slot_bytes)} bytes; "
+                         f"got {tuple(arena.shape)} {arena.dtype}")
+    if not isinstance(cursor, torch.Tensor) or cursor.device != arena.device or cursor.dtype != torch.int64 or cursor.numel() != 1:
+        raise ValueError("cursor must be a one-element int64 tensor on the arena's device")
+    host = videos_host.contiguous()
+    if (not isinstance(videos, torch.Tensor) or videos.device != arena.device or videos.dtype != torch.int64
+            or not videos.is_contiguous() or videos.dim() != 2 or videos.shape[1] != 3 or host.is_cuda
+            or host.dtype != torch.int64 or host.shape != videos.shape):
+        raise ValueError("videos must be an (n, 3) int64 tensor on the arena's device and videos_host its (n, 3) int64 host copy")
+    return host
+
+
+def frames_normalize_ragged(arena, slot_bytes: int, frames: int, cursor, videos, videos_host, size, mean=IMAGENET_MEAN,
+                            std=IMAGENET_STD, channels_last=False, dtype=torch.float32):
+    """A chunk of ``frames`` uint8 frames from videos of several sizes -> normalised (F, 3, h, w) [or (F, h, w, 3)]
+    fp32 / bf16 / fp16 and their (F, 4) boxes [0, 0, H, W], one launch (``lpb_frames_normalize_ragged``).
+
+    Frame f sits at the start of slot f of ``arena`` (uint8, ``slot_bytes`` per slot, ``ragged_slot_bytes``), rows
+    packed; its size is that of the video of ``videos`` (the device copy of ``videos_host``, ``ragged_videos``) holding
+    global row ``cursor + f``, read on the device, so a captured graph serves every mix of sizes.  Each image is
+    bit-identical to ``frames_normalize`` of that frame alone."""
+    host = _ragged(arena, slot_bytes, frames, cursor, videos, videos_host)
+    fmt, f, dev = _out_format(dtype), int(frames), arena.device
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((f, oh, ow, 3) if channels_last else (f, 3, oh, ow), device=dev, dtype=dtype)
+    boxes = torch.empty((f, 4), device=dev, dtype=torch.float32)
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(dev):
+        check(lib.lpb_frames_normalize_ragged(_ptr(arena), int(slot_bytes), f, _ptr(cursor), _ptr(videos), _ptr(host),
+                                              videos.shape[0], oh, ow, m3, s3, int(bool(channels_last)), fmt, _ptr(out),
+                                              _ptr(boxes), _stream()))
+    return out, boxes
+
+
 # training.imgaug "dlc" draw ranges (lightning_pose/data/video/dali.py:160-175) by column of the augment kernel's
 # params: angle (degrees), sx and sy, brightness and contrast, shot-noise factor
 DLC_PARAM_RANGES = ((slice(0, 1), -10.0, 10.0), (slice(1, 3), 0.8, 1.2), (slice(3, 5), 0.75, 1.25), (slice(5, 6), 0.0, 10.0))
@@ -932,6 +989,26 @@ def frames_crop_normalize(frames, bboxes, size, cursor=None, row0: int = 0, mean
     with torch.cuda.device(x.device):
         check(lib.lpb_frames_crop_normalize(_ptr(x), in_f32, f, h, w, _ptr(b), b.shape[0], _ptr(cursor), int(row0), oh, ow, m3, s3,
                                             int(bool(channels_last)), fmt, _ptr(out), _ptr(boxes_out), _stream()))
+    return out, boxes_out
+
+
+def frames_crop_normalize_ragged(arena, slot_bytes: int, frames: int, cursor, videos, videos_host, bboxes, size,
+                                 mean=IMAGENET_MEAN, std=IMAGENET_STD, channels_last=False, dtype=torch.float32):
+    """``frames_crop_normalize`` of uint8 frames from videos of several sizes, in the arena of
+    ``frames_normalize_ragged``: frame f is cropped to box row min(cursor + f, N - 1) of ``bboxes`` and clamped to its
+    own video's size.  Each frame's output and clamped box are bit-identical to ``frames_crop_normalize`` on its own
+    video alone.  Returns (frames (F, 3, h, w) [or (F, h, w, 3)], clamped boxes (F, 4) fp32)."""
+    host = _ragged(arena, slot_bytes, frames, cursor, videos, videos_host)
+    fmt, f, dev = _out_format(dtype), int(frames), arena.device
+    b = _bbox_table(bboxes, "bboxes")
+    oh, ow = int(size[0]), int(size[1])
+    out = torch.empty((f, oh, ow, 3) if channels_last else (f, 3, oh, ow), device=dev, dtype=dtype)
+    boxes_out = torch.empty((f, 4), device=dev, dtype=torch.float32)
+    m3, s3 = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(dev):
+        check(lib.lpb_frames_crop_normalize_ragged(_ptr(arena), int(slot_bytes), f, _ptr(cursor), _ptr(videos), _ptr(host),
+                                                   videos.shape[0], _ptr(b), b.shape[0], oh, ow, m3, s3,
+                                                   int(bool(channels_last)), fmt, _ptr(out), _ptr(boxes_out), _stream()))
     return out, boxes_out
 
 

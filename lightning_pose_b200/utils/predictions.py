@@ -20,14 +20,16 @@ The gathered table equals the one-GPU table bit for bit.
 A list of videos (``n_frames=[N_0, N_1, ...]``, ``litpose predict <model_dir> <video_dir>``) is one frame stream: the
 videos sit back to back in one table and in one chunk sequence, a chunk may hold the end of one video and the start of
 the next, and only the last chunk of the whole list is padded.  ``video_tables()`` gives each video's rows, equal to
-the table a one-video predictor gives that video.
+the table a one-video predictor gives that video.  With ``frame_sizes`` the videos may differ in frame size: each chunk's
+frames are copied into a slot arena and normalised by one launch that reads every frame's size on the device
+(``segment_chunks`` cuts the videos into such chunks).
 """
 from __future__ import annotations
 
 import bisect
 import numbers
 import operator
-from typing import Callable, Iterable, Sequence
+from typing import Callable, Iterable, Iterator, Sequence
 
 import numpy as np
 import torch
@@ -35,7 +37,7 @@ import torch
 from lightning_pose_b200 import ops
 
 __all__ = ["BatchedPredictor", "FramePredictor", "PredictionHandler", "make_dlc_pandas_index", "frame_range_for_rank",
-           "shard_feed_range", "context_edge_fill", "fill_context_edges"]
+           "shard_feed_range", "context_edge_fill", "fill_context_edges", "segment_chunks"]
 
 
 def frame_range_for_rank(n_frames: int, rank: int, world: int) -> tuple[int, int]:
@@ -64,6 +66,41 @@ def _video_starts(lengths: Sequence[int]) -> list[int]:
     for n in lengths:
         starts.append(starts[-1] + int(n))
     return starts
+
+
+def _chunk_segments(row: int, chunk: int, starts: Sequence[int]) -> list[tuple[int, int]]:
+    """(video, frames) of each run of one video in the chunk of ``chunk`` rows from global row ``row`` of a list whose
+    videos start at ``starts`` (``_video_starts``), in stream order.  Rows past the list's end belong to the last video,
+    as in the ragged ingest's lookup."""
+    out, r, end, last = [], row, row + chunk, len(starts) - 2
+    while r < end:
+        v = min(bisect.bisect_right(starts, r) - 1, last)
+        stop = end if v == last else min(end, starts[v + 1])
+        out.append((v, stop - r))
+        r = stop
+    return out
+
+
+def segment_chunks(videos: Sequence[torch.Tensor], chunk: int,
+                   feed_range: tuple[int, int] | None = None) -> Iterator[list[torch.Tensor]]:
+    """The chunks of a list of uint8 (N_i, H_i, W_i, 3) videos that a ``BatchedPredictor`` built with ``frame_sizes``
+    is fed: frames [lo, hi) of the concatenated stream (``feed_range``, default the whole list) in chunks of ``chunk``,
+    each chunk a list of (t_j, H, W, 3) segments, one per video it touches.  Segments are slices of the videos; rows at
+    or past ``hi`` are zero frames of their video's size (past the list's end, of the last video's size), the padding
+    of the last chunk."""
+    lengths = [int(v.shape[0]) for v in videos]
+    starts = _video_starts(lengths)
+    lo, hi = feed_range if feed_range is not None else (0, starts[-1])
+    for row in range(lo, lo + -(-(hi - lo) // chunk) * chunk, chunk):
+        segs, r = [], row
+        for v, t in _chunk_segments(row, chunk, starts):
+            a = r - starts[v]
+            seg = videos[v][a : a + max(0, min(t, hi - r, lengths[v] - a))]
+            if seg.shape[0] < t:
+                seg = torch.cat([seg, seg.new_zeros((t - seg.shape[0], *videos[v].shape[1:]))])
+            segs.append(seg)
+            r += t
+        yield segs
 
 
 def _context_window_index(start: int, chunk: int, lengths: Sequence[int]) -> list[list[int]]:
@@ -352,13 +389,23 @@ class BatchedPredictor:
     the tensor form (a feature when the caller streams features), or with uint8 views and in crop mode a zero frame.
     Each video's rows then equal the table of a one-video predictor fed that video with ``pad`` as its padding.  Shards
     split the concatenated rows (``shard_feed_range`` and ``context_edge_fill`` take the list of lengths).
+
+    Videos of several frame sizes (``frame_sizes=[(H_0, W_0), ...]``, one per video, one view; in crop mode in place of
+    ``frame_hw``): a chunk is a list of uint8 (t_j, H_j, W_j, 3) segments in stream order, one per video the chunk
+    touches (rows past the list's end, the last chunk's padding, belong to the last video), ``sum t_j`` = T:
+    ``segment_chunks`` cuts them.  ``feed`` copies each segment into its slots of a T-slot arena (``slot_bytes`` each,
+    the largest frame rounded up to 16), then one launch inside the chunk normalises (``ops.frames_normalize_ragged``) or
+    crops (``ops.frames_crop_normalize_ragged``) every frame at its own size, read from a device table of (first row,
+    H, W) per video at the cursor, and writes its box; the bodies are unchanged.  One capture serves every mix of
+    sizes.  A context list's padding frame is a zero frame.
     """
 
     def __init__(self, head, num_keypoints: int, n_frames: int | Sequence[int], chunk: int, image_hw: tuple[int, int],
                  features_of: Callable[[torch.Tensor], torch.Tensor] | None = None, device=None, use_graph: bool = True,
                  sub_chunk: int | None = None, bboxes: torch.Tensor | None = None, frame_hw: tuple[int, int] | None = None,
                  crop_dtype: torch.dtype = torch.float32, crop_channels_last: bool = False, num_views: int = 1,
-                 shard: tuple[int, int] = (0, 1), pad: torch.Tensor | None = None) -> None:
+                 shard: tuple[int, int] = (0, 1), pad: torch.Tensor | None = None,
+                 frame_sizes: Sequence[tuple[int, int]] | None = None) -> None:
         from lightning_pose_b200.models.heads.heatmap_mhcrnn import HeatmapMHCRNNHead
         from lightning_pose_b200.models.heads.regression import LinearRegressionHead
 
@@ -418,12 +465,17 @@ class BatchedPredictor:
         if bboxes is not None:
             if self.num_views > 1:
                 raise ValueError("bbox cropping is not supported for multiview models")
-            if frame_hw is None or features_of is None:
+            if (frame_hw is None and frame_sizes is None) or features_of is None:
                 raise ValueError("crop mode needs frame_hw (the full frame size) and features_of (frames -> features)")
+            if frame_hw is not None and frame_sizes is not None:
+                raise ValueError("frame_sizes gives every video's frame size; drop frame_hw")
             self.bboxes = ops._bbox_table(bboxes, "bboxes")
             if self.bboxes.shape[0] != self.n_frames:
                 raise ValueError(f"bboxes has {self.bboxes.shape[0]} rows but the video has {self.n_frames} frames")
-            self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
+            self.frame_hw = (int(frame_hw[0]), int(frame_hw[1])) if frame_sizes is None else None
+        self.frame_sizes = None  # per-video frame sizes: the slot arena, its video table and the next chunk's first row
+        if frame_sizes is not None:
+            self._init_ragged(frame_sizes, features_of)
         if self.regression:  # the likelihood column
             self._zero_conf = torch.zeros((self.chunk, self.k), dtype=torch.float32, device=self.device)
         if self.context:  # the halo buffers; the maps' are sized by the first chunk's maps
@@ -441,6 +493,26 @@ class BatchedPredictor:
                 # the padding frame's maps are needed when a video has R = N - 1 (computed at the first feed)
                 self._pad = (None if not any(r == n - 1 for _, n, r in self._segments_host.tolist()) else
                              pad if pad is not None else False)
+
+    def _init_ragged(self, frame_sizes, features_of) -> None:
+        """Checks ``frame_sizes``; builds the T-slot arena, the (first row, H, W) video table on the host and the device,
+        and the host row of the next chunk."""
+        videos = self.lengths if self.lengths is not None else [self.n_frames]
+        sizes = [tuple(operator.index(s) for s in hw) for hw in frame_sizes]
+        if len(sizes) != len(videos) or any(len(hw) != 2 or min(hw) < 1 for hw in sizes):
+            raise ValueError(f"frame_sizes must hold one (H >= 1, W >= 1) per video: {len(videos)} videos; got {sizes}")
+        if self.num_views > 1:
+            raise ValueError("per-video frame sizes are single-view (multi-view videos would need a size per video and view)")
+        if features_of is None:
+            raise ValueError("uint8 frames of frame_sizes need features_of (frames -> features)")
+        self.frame_sizes = sizes
+        self._starts = _video_starts(videos)
+        self._videos_host = ops.ragged_videos(videos, sizes)
+        self._videos = self._videos_host.to(self.device)
+        self.slot_bytes = ops.ragged_slot_bytes(sizes)
+        self._arena = torch.zeros(self.chunk * self.slot_bytes, dtype=torch.uint8, device=self.device)
+        self._row = self.feed_range[0]
+
     def _whole_frames(self, sizes: list[tuple[int, int]]) -> torch.Tensor:
         """(T, 4 V) boxes [0, 0, h, w] of whole frames of the views' ``sizes``."""
         row = [float(s) for h, w in sizes for s in (0, 0, h, w)]
@@ -481,6 +553,9 @@ class BatchedPredictor:
         elif form == "crop":
             x, _ = ops.frames_crop_normalize(torch.zeros_like(xs[0]), self.bboxes, self.image_hw, row0=0,
                                              channels_last=self.crop_channels_last, dtype=self.crop_dtype)
+        elif form in ("ragged", "crop_ragged"):  # a zero arena at a row past the list's end: the last video's size
+            past_end = torch.full((1,), self.n_frames, dtype=torch.int64, device=self.device)
+            x, _ = self._ingest_ragged(form, torch.zeros_like(self._arena), past_end)
         else:
             x = ops.frames_normalize_views([torch.zeros_like(v) for v in xs[:-1]], self.image_hw,
                                            channels_last=self.crop_channels_last, dtype=self.crop_dtype)
@@ -496,6 +571,8 @@ class BatchedPredictor:
         """A chunk as fed -> (its form, its checked tensors): "crop" (frames,), "views" (*views, boxes) or
         "tensor" (x, boxes)."""
         t, v = self.chunk, self.num_views
+        if self.frame_sizes is not None:
+            return self._segments_in(x, bbox)
         if self.bboxes is not None:
             if bbox is not None:
                 raise ValueError("crop mode takes its boxes from the `bboxes` table given at construction")
@@ -535,9 +612,42 @@ class BatchedPredictor:
             raise ValueError(f"bbox must be ({t}, {4 * v}); got {tuple(bbox.shape)}")
         return "tensor", (x, bbox)
 
+    def _segments_in(self, x, bbox) -> tuple[str, tuple[torch.Tensor, ...]]:
+        """A chunk of a ``frame_sizes`` predictor: its segments checked against the videos the chunk at the host row
+        touches -> ("ragged" or "crop_ragged", (arena,)).  The segments are copied into the arena by ``feed``."""
+        if bbox is not None:
+            raise ValueError("segments take their boxes from frame_sizes (or, in crop mode, the bboxes table)")
+        if not isinstance(x, (list, tuple)) or not all(isinstance(s, torch.Tensor) for s in x):
+            raise ValueError("with frame_sizes a chunk is a list of uint8 (t, H, W, 3) segments, one per video it touches")
+        for seg in x:
+            if seg.dtype != torch.uint8 or seg.dim() != 4 or seg.shape[-1] != 3:
+                raise ValueError(f"each segment must be uint8 (t, H, W, 3); got {tuple(seg.shape)} {seg.dtype}")
+        want = [(t, *self.frame_sizes[v]) for v, t in _chunk_segments(self._row, self.chunk, self._starts)]
+        got = [tuple(int(d) for d in seg.shape[:3]) for seg in x]
+        if got != want:
+            raise ValueError(f"the chunk from row {self._row} holds segments (frames, H, W) {want}, in this order; got {got}")
+        return ("crop_ragged" if self.bboxes is not None else "ragged"), (self._arena,)
+
+    def _fill_arena(self, segments) -> None:
+        """Segment j's frames into their slots: one strided copy per segment."""
+        slots, f0 = self._arena.view(self.chunk, self.slot_bytes), 0
+        for seg in segments:
+            t, size = seg.shape[0], seg[0].numel()
+            slots[f0 : f0 + t, :size].copy_(seg.reshape(t, size), non_blocking=True)
+            f0 += t
+
+    def _ingest_ragged(self, form: str, arena: torch.Tensor, cursor: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+        args = (arena, self.slot_bytes, self.chunk, cursor, self._videos, self._videos_host)
+        kw = {"channels_last": self.crop_channels_last, "dtype": self.crop_dtype}
+        if form == "crop_ragged":
+            return ops.frames_crop_normalize_ragged(*args, self.bboxes, self.image_hw, **kw)
+        return ops.frames_normalize_ragged(*args, self.image_hw, **kw)
+
     def _ingest(self, form: str, xs) -> tuple[torch.Tensor, torch.Tensor]:
         """A chunk's tensors -> (the (T V, ...) batch for ``features_of``, the (T, 4 V) boxes)."""
-        if form == "crop":  # crop to the rows at the cursor BEFORE the table writer advances it
+        if form in ("ragged", "crop_ragged"):  # at the rows of the cursor, before the table writer advances it
+            x, bbox = self._ingest_ragged(form, xs[0], self.cursor)
+        elif form == "crop":  # crop to the rows at the cursor BEFORE the table writer advances it
             x, bbox = ops.frames_crop_normalize(xs[0], self.bboxes, self.image_hw, cursor=self.cursor,
                                                 channels_last=self.crop_channels_last, dtype=self.crop_dtype)
         elif form == "views":
@@ -601,7 +711,7 @@ class BatchedPredictor:
                 buf[:halo].copy_(tail.clone() if t < halo else tail)
 
     def _capture(self, form: str, xs) -> None:
-        self._static = [x.clone() for x in xs]
+        self._static = [x if form in ("ragged", "crop_ragged") else x.clone() for x in xs]  # the arena is its own
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
@@ -621,6 +731,9 @@ class BatchedPredictor:
         """Process the next chunk: a tensor with an optional ``bbox``, V uint8 views, or in crop mode uint8 full frames
         (the forms of the class docstring)."""
         form, xs = self._inputs(x, bbox)
+        if self.frame_sizes is not None:
+            self._fill_arena(x)
+            self._row += self.chunk
         if self.context and self._pad is not None and self._pad is not True:
             if self._pad is False and form == "tensor":
                 raise ValueError("a video of this list has R = N - 1 rows, so its frame N - 2 is predicted from the "
@@ -636,7 +749,8 @@ class BatchedPredictor:
         if got != self._captured:  # a replay would cast or mis-read it
             raise ValueError(f"the chunk's graph was captured for {self._captured}; this chunk is {got}")
         for dst, src in zip(self._static, xs):
-            dst.copy_(src, non_blocking=True)
+            if dst is not src:
+                dst.copy_(src, non_blocking=True)
         self._graph.replay()
 
     def run(self, chunks: Iterable[torch.Tensor | tuple[torch.Tensor, torch.Tensor] | Sequence[torch.Tensor]]) -> torch.Tensor:
