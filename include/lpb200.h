@@ -603,6 +603,33 @@ int lpb_pack_context_predictions_segments(const float* kp_sf, const float* conf_
                                           int64_t* cursor, const int64_t* segments, const int64_t* segments_host,
                                           int n_segments, int64_t step, int32_t* window_index, void* stream);
 
+/* ---- a live stream with context (MHCRNN) models: one new frame per call --------------------------------------------
+ * replaces the five-frame window of Model.predict_frame  lightning_pose/api/model.py:360-509 (every call ingests and runs
+ * the backbone on all T = 5 frames) for a stream that pushes one frame per call: each frame's model-space data stays on
+ * the device in a ring of LPB_CONTEXT_RING_SLOTS slots, slot t mod 5 holding stream frame t.  count: device int64, the
+ * frames pushed so far; read by both entries, advanced only by lpb_context_ring_select, so one captured graph (push ->
+ * lpb_crnn_combine_fwd -> decode -> select) serves every call.
+ *
+ * lpb_context_ring_push: with c = *count, copies this frame's W_f / W_b maps wf, wb [K][H][W] (UpsamplingCRNN's
+ *   per-frame deconv outputs, heads/heatmap_mhcrnn.py:268-316) to ring_wf / ring_wb [5][K][H][W] slot c mod 5, its
+ *   single-frame decode kp_sf [2K], conf_sf [K] to ring_kp [5][2K], ring_conf [5][K], and its box bbox [4]
+ *   ([x, y, h, w], as lpb_frames_crop_resize_cv2 writes it) to ring_box [5][4]; writes window_index [1][5] =
+ *   [(c - 4) mod 5, ..., c mod 5], the frames c - 4 .. c in time order, as lpb_crnn_combine_fwd reads it.  wf, wb,
+ *   ring_wf and ring_wb 16-byte aligned; H and W even.
+ * lpb_context_ring_select: with c = *count, frame c - 2 (the centre of the window): per keypoint the multi-frame
+ *   decode kp_mf [2K], conf_mf [K] where conf_mf > the ring's conf_sf of slot (c - 2) mod 5, else that slot's kp_sf (a
+ *   NaN keeps sf; torch.gt, models/heatmap_tracker_mhcrnn.py:214-220), mapped model -> frame with that slot's own box
+ *   (model_to_frame_batch's centre-frame rows bbox[2:-2], data/bboxes.py:94-104, lpb_remap_keypoints' operation order):
+ *   out [K][3] = (x, y, confidence).  Then *count = c + 1.  The result is meaningful once c >= 4. */
+#define LPB_CONTEXT_RING_SLOTS 5
+#define LPB_CONTEXT_RING_MAX_K 65536
+int lpb_context_ring_push(const float* wf, const float* wb, const float* kp_sf, const float* conf_sf, const float* bbox,
+                          int K, int H, int W, float* ring_wf, float* ring_wb, float* ring_kp, float* ring_conf,
+                          float* ring_box, const int64_t* count, int32_t* window_index, void* stream);
+int lpb_context_ring_select(const float* ring_kp, const float* ring_conf, const float* ring_box, const float* kp_mf,
+                            const float* conf_mf, int K, float model_height, float model_width, float* out,
+                            int64_t* count, void* stream);
+
 /* ---- optimizer step (the tail of a training step) ---------------------------------------------------
  * replaces torch.optim.Adam / AdamW as configured by configure_optimizers  lightning_pose/models/base.py:458-477
  * (no amsgrad).  One launch over up to 16 fp32 tensors; params / grads / exp_avg / exp_avg_sq / numel are HOST arrays

@@ -126,6 +126,8 @@ SIGNATURES = {
     "lpb_pack_predictions": (C.c_int, [_P, _P, _I, _I, _P, _L, _P, _L, _P]),
     "lpb_pack_context_predictions": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _F, _F, _P, _L, _P, _L, _L, _P]),
     "lpb_pack_context_predictions_segments": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _F, _F, _P, _L, _P, _P, _P, _I, _L, _P, _P]),
+    "lpb_context_ring_push": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "lpb_context_ring_select": (C.c_int, [_P, _P, _P, _P, _P, _I, _F, _F, _P, _P, _P]),
     "lpb_adam_step": (C.c_int, [_I, _P, _P, _P, _P, _P, _P, _P, _F, _P, C.c_double, C.c_double, _F, _F, _I, _P]),
     "lpb_plane_softmax_bwd": (C.c_int, [_P, _P, _L, _I, _P, _P]),
     "lpb_heatmap_loss_fwd": (C.c_int, [_P, _P, _L, _I, _I, _I, _P, _P, _P]),

@@ -154,6 +154,59 @@ __global__ void advance_cursor_windows_kernel(int64_t* cursor, int64_t n, int32_
   if (threadIdx.x == 0) *cursor = c;
 }
 
+// ---- a live stream of one frame per call (FramePredictor.push_frame) ----------------------------------------------
+// Model.predict_frame  lightning_pose/api/model.py:360-509 on frames t - 4 .. t, with each frame's maps, single-frame
+// decode and box computed once and kept in a ring (see lpb200.h).  Slot s holds stream frame t with t mod 5 = s;
+// count = the frames pushed so far.
+__device__ __forceinline__ int ring_slot(int64_t t) {
+  const int64_t s = t % LPB_CONTEXT_RING_SLOTS;
+  return (int)(s < 0 ? s + LPB_CONTEXT_RING_SLOTS : s);
+}
+
+// grid-stride float4 copies of the frame's two maps into slot c mod 5; block 0 also stores the single-frame decode and
+// the box, and writes the window [(c - 4) mod 5, ..., c mod 5]
+__global__ void context_ring_push_kernel(const float4* __restrict__ wf, const float4* __restrict__ wb, int64_t map_vec,
+                                         const float* __restrict__ kp_sf, const float* __restrict__ conf_sf,
+                                         const float* __restrict__ bbox, int K, float4* __restrict__ ring_wf,
+                                         float4* __restrict__ ring_wb, float* __restrict__ ring_kp,
+                                         float* __restrict__ ring_conf, float* __restrict__ ring_box,
+                                         const int64_t* __restrict__ count, int32_t* __restrict__ window) {
+  const int64_t c = *count;
+  const int s = ring_slot(c);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < map_vec; i += stride) {
+    ring_wf[s * map_vec + i] = __ldg(wf + i);
+    ring_wb[s * map_vec + i] = __ldg(wb + i);
+  }
+  if (blockIdx.x != 0) return;
+  for (int i = threadIdx.x; i < 2 * K; i += blockDim.x) ring_kp[(size_t)s * 2 * K + i] = kp_sf[i];
+  for (int i = threadIdx.x; i < K; i += blockDim.x) ring_conf[(size_t)s * K + i] = conf_sf[i];
+  if (threadIdx.x < 4) ring_box[s * 4 + threadIdx.x] = bbox[threadIdx.x];
+  if (threadIdx.x < LPB_CONTEXT_RING_SLOTS) window[threadIdx.x] = ring_slot(c - 4 + threadIdx.x);
+}
+
+// one block: frame c - 2's selection and remap (the rule and operation order of pack_context_kernel), then count += 1
+__global__ void context_ring_select_kernel(const float* __restrict__ ring_kp, const float* __restrict__ ring_conf,
+                                           const float* __restrict__ ring_box, const float* __restrict__ kp_mf,
+                                           const float* __restrict__ conf_mf, int K, float inv_mh, float inv_mw,
+                                           float* __restrict__ out, int64_t* count) {
+  const int64_t c = *count;
+  const int s = ring_slot(c - 2);
+  const float* kp_sf = ring_kp + (size_t)s * 2 * K;
+  const float* bb = ring_box + s * 4;  // [x, y, h, w] of frame c - 2
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    const float csf = ring_conf[(size_t)s * K + k], cmf = conf_mf[k];
+    const bool mf = cmf > csf;  // a NaN keeps sf
+    const float* src = mf ? kp_mf : kp_sf;
+    const float x = src[2 * k], y = src[2 * k + 1];
+    out[3 * k] = (x * inv_mw) * bb[3] + bb[0];
+    out[3 * k + 1] = (y * inv_mh) * bb[2] + bb[1];
+    out[3 * k + 2] = mf ? cmf : csf;
+  }
+  __syncthreads();  // every thread has read the count
+  if (threadIdx.x == 0) *count = c + 1;
+}
+
 }  // namespace lpb
 
 extern "C" int lpb_pack_predictions(const float* keypoints, const float* confidences, int n_frames, int K, float* table,
@@ -236,6 +289,50 @@ extern "C" int lpb_pack_context_predictions_segments(const float* kp_sf, const f
     advance_cursor_windows_kernel<<<1, 256, 0, s>>>(cursor, n_frames, window_index, step, segments, n_segments, n_rows);
   else
     advance_cursor_kernel<<<1, 1, 0, s>>>(cursor, n_frames);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_context_ring_push(const float* wf, const float* wb, const float* kp_sf, const float* conf_sf,
+                                     const float* bbox, int K, int H, int W, float* ring_wf, float* ring_wb,
+                                     float* ring_kp, float* ring_conf, float* ring_box, const int64_t* count,
+                                     int32_t* window_index, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(wf && wb && kp_sf && conf_sf && bbox && ring_wf && ring_wb && ring_kp && ring_conf && ring_box && count &&
+                  window_index,
+              "context_ring_push: null pointer");
+  LPB_REQUIRE(aligned_to(wf, 16) && aligned_to(wb, 16) && aligned_to(ring_wf, 16) && aligned_to(ring_wb, 16) &&
+                  aligned_to(kp_sf, 4) && aligned_to(conf_sf, 4) && aligned_to(bbox, 4) && aligned_to(ring_kp, 4) &&
+                  aligned_to(ring_conf, 4) && aligned_to(ring_box, 4) && aligned_to(count, 8) &&
+                  aligned_to(window_index, 4),
+              "context_ring_push: misaligned pointer (maps 16 bytes, count 8, the rest 4)");
+  LPB_REQUIRE(K >= 1 && K <= LPB_CONTEXT_RING_MAX_K, "context_ring_push: bad K=%d (1 .. %d)", K, LPB_CONTEXT_RING_MAX_K);
+  LPB_REQUIRE(H >= 2 && W >= 2 && H % 2 == 0 && W % 2 == 0,
+              "context_ring_push: maps must be (K, H, W) with even H, W >= 2 (got H=%d W=%d)", H, W);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int64_t map_vec = (int64_t)K * H * W / 4;  // H, W even: a whole number of float4
+  const int64_t blocks = (map_vec + 255) / 256;
+  context_ring_push_kernel<<<(unsigned)(blocks < 1024 ? blocks : 1024), 256, 0, s>>>(
+      reinterpret_cast<const float4*>(wf), reinterpret_cast<const float4*>(wb), map_vec, kp_sf, conf_sf, bbox, K,
+      reinterpret_cast<float4*>(ring_wf), reinterpret_cast<float4*>(ring_wb), ring_kp, ring_conf, ring_box, count,
+      window_index);
+  LPB_CUDA(cudaGetLastError());
+  return LPB_OK;
+}
+
+extern "C" int lpb_context_ring_select(const float* ring_kp, const float* ring_conf, const float* ring_box,
+                                       const float* kp_mf, const float* conf_mf, int K, float model_height,
+                                       float model_width, float* out, int64_t* count, void* stream) {
+  using namespace lpb;
+  LPB_REQUIRE(ring_kp && ring_conf && ring_box && kp_mf && conf_mf && out && count, "context_ring_select: null pointer");
+  LPB_REQUIRE(aligned_to(ring_kp, 4) && aligned_to(ring_conf, 4) && aligned_to(ring_box, 4) && aligned_to(kp_mf, 4) &&
+                  aligned_to(conf_mf, 4) && aligned_to(out, 4) && aligned_to(count, 8),
+              "context_ring_select: misaligned pointer (count 8 bytes, the rest 4)");
+  LPB_REQUIRE(K >= 1 && K <= LPB_CONTEXT_RING_MAX_K, "context_ring_select: bad K=%d (1 .. %d)", K, LPB_CONTEXT_RING_MAX_K);
+  LPB_REQUIRE(model_height > 0.f && model_width > 0.f, "context_ring_select: bad model dims");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  context_ring_select_kernel<<<1, 256, 0, s>>>(ring_kp, ring_conf, ring_box, kp_mf, conf_mf, K, 1.0f / model_height,
+                                               1.0f / model_width, out, count);
   LPB_CUDA(cudaGetLastError());
   return LPB_OK;
 }

@@ -1129,6 +1129,55 @@ def pack_context_predictions_segments(kp_sf, conf_sf, kp_mf, conf_mf, bbox, mode
     return table
 
 
+CONTEXT_RING_SLOTS = 5  # LPB_CONTEXT_RING_SLOTS (include/lpb200.h)
+
+
+def _ring_buffer(t, shape, name: str, dtype=torch.float32) -> None:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise RuntimeError(f"lpb200: `{name}` must be a CUDA tensor (this package has no CPU fallback)")
+    if t.dtype != dtype or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name} must be a contiguous {dtype} {tuple(shape)} tensor; got {tuple(t.shape)} {t.dtype}")
+
+
+def context_ring_push(wf, wb, kp_sf, conf_sf, bbox, ring_wf, ring_wb, ring_kp, ring_conf, ring_box, count, window_index):
+    """One frame's W_f / W_b maps (1, K, H, W), single-frame decode (1, 2K) / (1, K) and box (1, 4) into slot
+    ``count mod 5`` of the ring (``ring_wf`` / ``ring_wb`` (5, K, H, W), ``ring_kp`` (5, 2K), ``ring_conf`` (5, K),
+    ``ring_box`` (5, 4)), and the (1, 5) int32 ``window_index`` of frames count - 4 .. count for ``crnn_combine`` over the
+    ring (``lpb_context_ring_push``).  ``count`` (one-element int64) is read, not advanced.  Mutates the ring and
+    ``window_index``."""
+    wf, wb, kp_sf, conf_sf, bbox = (_cuda_f32(t, n) for t, n in ((wf, "wf"), (wb, "wb"), (kp_sf, "kp_sf"),
+                                                                   (conf_sf, "conf_sf"), (bbox, "bbox")))
+    k, h, w = wf.shape[1:] if wf.dim() == 4 else (0, 0, 0)
+    r = CONTEXT_RING_SLOTS
+    for t, shape, name in ((wf, (1, k, h, w), "wf"), (wb, (1, k, h, w), "wb"), (kp_sf, (1, 2 * k), "kp_sf"),
+                           (conf_sf, (1, k), "conf_sf"), (bbox, (1, 4), "bbox"), (ring_wf, (r, k, h, w), "ring_wf"),
+                           (ring_wb, (r, k, h, w), "ring_wb"), (ring_kp, (r, 2 * k), "ring_kp"),
+                           (ring_conf, (r, k), "ring_conf"), (ring_box, (r, 4), "ring_box")):
+        _ring_buffer(t, shape, name)
+    _ring_buffer(count, (1,), "count", torch.int64)
+    _ring_buffer(window_index, (1, r), "window_index", torch.int32)
+    with torch.cuda.device(wf.device):
+        check(lib.lpb_context_ring_push(_ptr(wf), _ptr(wb), _ptr(kp_sf), _ptr(conf_sf), _ptr(bbox), k, h, w, _ptr(ring_wf),
+                                        _ptr(ring_wb), _ptr(ring_kp), _ptr(ring_conf), _ptr(ring_box), _ptr(count),
+                                        _ptr(window_index), _stream()))
+
+
+def context_ring_select(ring_kp, ring_conf, ring_box, kp_mf, conf_mf, model_height, model_width, out, count):
+    """Frame count - 2 of the ring: per keypoint the more confident of its single-frame decode (ring slot
+    ``(count - 2) mod 5``) and the multi-frame decode ``kp_mf`` (1, 2K) / ``conf_mf`` (1, K) (a NaN keeps single-frame),
+    mapped to the frame with that slot's box, into ``out`` (K, 3); then ``count`` += 1 (``lpb_context_ring_select``)."""
+    kp_mf, conf_mf = _cuda_f32(kp_mf, "kp_mf"), _cuda_f32(conf_mf, "conf_mf")
+    r, k = CONTEXT_RING_SLOTS, ring_conf.shape[-1]
+    for t, shape, name in ((ring_kp, (r, 2 * k), "ring_kp"), (ring_conf, (r, k), "ring_conf"), (ring_box, (r, 4), "ring_box"),
+                           (kp_mf, (1, 2 * k), "kp_mf"), (conf_mf, (1, k), "conf_mf"), (out, (k, 3), "out")):
+        _ring_buffer(t, shape, name)
+    _ring_buffer(count, (1,), "count", torch.int64)
+    with torch.cuda.device(out.device):
+        check(lib.lpb_context_ring_select(_ptr(ring_kp), _ptr(ring_conf), _ptr(ring_box), _ptr(kp_mf), _ptr(conf_mf), k,
+                                          float(model_height), float(model_width), _ptr(out), _ptr(count), _stream()))
+    return out
+
+
 def plane_softmax_backward(probs: torch.Tensor, grad_probs: torch.Tensor) -> torch.Tensor:
     p = _cuda_f32(probs, "probs")
     g = _cuda_f32(grad_probs, "grad_probs")

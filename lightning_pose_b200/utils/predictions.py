@@ -800,6 +800,10 @@ class BatchedPredictor:
         return [self.table[:, w * v : w * (v + 1)] for v in range(self.num_views)]
 
 
+_NO_STREAM = ("push_frame streams context (MHCRNN) models; a single-frame or regression model predicts each frame on its "
+              "own with predict_frame")
+
+
 class FramePredictor:
     """One frame in, its keypoints out, with one CUDA-graph replay per call: the reference's ``Model.predict_frame``
     (``lightning_pose/api/model.py:298-509``) for loops that need each answer before the next camera frame.
@@ -830,6 +834,20 @@ class FramePredictor:
     device frame is copied into the graph's input buffer on the device.  A call is: write the staging buffers, replay,
     synchronise once, return copies.  ``launches_per_call`` counts the captured kernels.  ``use_graph=False`` runs the
     same body eagerly.
+
+    A live stream with a context model: ``push_frame(frame_rgb, bbox=None)`` takes ONE uint8 (H, W, 3) frame (the input
+    rules of the single-frame form) and its own optional box, and returns ``{"keypoints", "confidence", "frame"}`` for
+    stream frame t - 2, t counting the pushes since the last ``reset_stream()`` from 0 (``None`` values for the first
+    four).  Each push ingests, runs ``features_of``, the single-frame head and decode and the W_f / W_b maps on its frame
+    alone, and keeps them with the frame's box in slot t mod 5 of a device ring (``ops.context_ring_push``); the
+    recurrence then reads slots t - 4 .. t in time order, and ``ops.context_ring_select`` keeps per keypoint the more
+    confident of frame t - 2's single-frame and multi-frame predictions and maps them with frame t - 2's own box.  With
+    one box for all frames this is ``predict_frame(frames[t - 4 : t + 1], bbox)``; with a box per frame it is the video
+    crop-mode rule (each frame cropped to its own box, the centre frame's box remapping).  A device counter drives the
+    ring, so one captured graph (``launches_per_push`` kernels) serves every push.  The push graph is captured per input
+    form like ``predict_frame``'s and apart from it: ``predict_frame`` calls between pushes leave the stream alone, and a
+    new frame shape or source recaptures the push graph and keeps the stream (the ring holds model-space data only).
+    Single-frame and regression heads, and a (5, H, W, 3) stack, raise ``ValueError``.
     """
 
     CONTEXT_FRAMES = 5
@@ -857,13 +875,28 @@ class FramePredictor:
         self._table = torch.zeros((self.CONTEXT_FRAMES if self.context else 1, 3 * self.k), dtype=torch.float32, device=self.device)
         self._ones = torch.ones((1, self.k), dtype=torch.float32, device=self.device)  # a regression head's confidence
         self._box = torch.zeros(4, dtype=torch.int32, device=self.device)
-        self._pin_box = torch.zeros(4, dtype=torch.int32).pin_memory()
-        self._pin_out = torch.zeros((self.k, 3), dtype=torch.float32).pin_memory()
+        self._pin_box = self._pin_out = None  # pinned staging of the box and the result, made at the first call
         self._key = self._graph = self._frames = self._pin_frames = None
         self.launches_per_call = None
+        # push_frame's stream (context heads): its own input form and graph, and the ring of the last five frames'
+        # model-space data, slot t mod 5 holding stream frame t; the maps' slots are sized by the first push
+        self._push_key = self._push_graph = self._push_frames = self._push_pin_frames = None
+        self.launches_per_push = None
+        self._pushed = 0  # frames pushed since the last reset: the host's copy of ``_ring_count``
+        if self.context:
+            r, k, dev = ops.CONTEXT_RING_SLOTS, self.k, self.device
+            self._ring_count = torch.zeros(1, dtype=torch.int64, device=dev)
+            self._ring_kp = torch.zeros((r, 2 * k), dtype=torch.float32, device=dev)
+            self._ring_cf = torch.zeros((r, k), dtype=torch.float32, device=dev)
+            self._ring_box = torch.zeros((r, 4), dtype=torch.float32, device=dev)
+            self._ring_wf = self._ring_wb = None
+            self._window = torch.zeros((1, r), dtype=torch.int32, device=dev)
+            self._push_row = torch.zeros((self.k, 3), dtype=torch.float32, device=dev)
 
-    def _check(self, frame_rgb, bbox) -> tuple[np.ndarray | torch.Tensor, tuple[int, int, int, int]]:
-        """The reference's input checks (api/model.py:353-407) -> (frames (F, H, W, 3), box [x, y, w, h])."""
+    def _check(self, frame_rgb, bbox, stack: bool | None = None) -> tuple[np.ndarray | torch.Tensor, tuple[int, int, int, int]]:
+        """The reference's input checks (api/model.py:353-407) -> (frames (F, H, W, 3), box [x, y, w, h]).  ``stack``:
+        whether a (5, H, W, 3) stack is expected (default: for a context model) rather than one (H, W, 3) frame."""
+        stack = self.context if stack is None else stack
         if isinstance(frame_rgb, torch.Tensor):
             if frame_rgb.dtype != torch.uint8:
                 raise ValueError(f"frame_rgb must be uint8, got {frame_rgb.dtype}")
@@ -880,13 +913,13 @@ class FramePredictor:
             raise ValueError(f"frame_rgb must be (H, W, 3) or (T, H, W, 3), got shape {shape}")
         if int(np.prod(shape)) == 0:
             raise ValueError("frame_rgb is empty")
-        if self.context and len(shape) == 3:
+        if stack and len(shape) == 3:
             raise ValueError(f"a context model requires frame_rgb of shape ({self.CONTEXT_FRAMES}, H, W, 3); got a single frame "
                              f"{shape}. Use BatchedPredictor for video input.")
-        if self.context and shape[0] != self.CONTEXT_FRAMES:
+        if stack and shape[0] != self.CONTEXT_FRAMES:
             raise ValueError(f"a context model takes {self.CONTEXT_FRAMES} frames, the context length of its labeled batches; "
                              f"got {shape[0]}")
-        if not self.context and len(shape) == 4:
+        if not stack and len(shape) == 4:
             raise ValueError(f"a single-frame model takes one (H, W, 3) frame; got shape {shape}")
         h, w = shape[-3], shape[-2]
         if bbox is None:
@@ -938,23 +971,36 @@ class FramePredictor:
         """Buffers (and with ``use_graph`` the graph) of an input form: (host?, frame shape)."""
         self._key, self._graph = key, None
         from_host, shape = key
-        self._frames = torch.zeros(shape, dtype=torch.uint8, device=self.device)
-        self._pin_frames = torch.zeros(shape, dtype=torch.uint8).pin_memory() if from_host else None
-        if not self.use_graph:
-            return
+        self._frames, self._pin_frames = self._staging(key)
+        if self.use_graph:
+            self._graph = self._captured(lambda: self._call(from_host))
+            self.launches_per_call = _graph_kernel_count(self._graph)
+            self._graph.instantiate()
+
+    def _staging(self, key) -> tuple[torch.Tensor, torch.Tensor | None]:
+        """The device input buffer of an input form (host?, frame shape) and, for host frames, its pinned staging
+        buffer; the box and result staging buffers at the first call."""
+        from_host, shape = key
+        if self._pin_out is None:
+            self._pin_box = torch.zeros(4, dtype=torch.int32).pin_memory()
+            self._pin_out = torch.zeros((self.k, 3), dtype=torch.float32).pin_memory()
+        return (torch.zeros(shape, dtype=torch.uint8, device=self.device),
+                torch.zeros(shape, dtype=torch.uint8).pin_memory() if from_host else None)
+
+    def _captured(self, call: Callable[[], None]) -> torch.cuda.CUDAGraph:
+        """Two warm-up runs of ``call`` (per-shape tables, allocator pools), then its capture, not yet instantiated: kept
+        so that its kernel nodes can be counted."""
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
-            for _ in range(2):  # warm-up: per-shape tables, allocator pools
-                self._call(from_host)
+            for _ in range(2):
+                call()
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph(keep_graph=True)  # kept so that its kernel nodes can be counted
+        graph = torch.cuda.CUDAGraph(keep_graph=True)
         with torch.cuda.graph(graph):
-            self._call(from_host)
-        self.launches_per_call = _graph_kernel_count(graph)
-        graph.instantiate()
-        self._graph = graph
+            call()
+        return graph
 
     def predict_frame(self, frame_rgb, bbox: tuple[int, int, int, int] | None = None) -> dict[str, np.ndarray]:
         """The reference's ``predict_frame``: ``{"keypoints": (K, 2), "confidence": (K,)}`` float32, frame pixels."""
@@ -975,3 +1021,93 @@ class FramePredictor:
         torch.cuda.current_stream(self.device).synchronize()
         out = self._pin_out.numpy()
         return {"keypoints": out[:, :2].copy(), "confidence": out[:, 2].copy()}
+
+    # ---- a live stream: one new frame per call ------------------------------------------------------------------
+    def _push_body(self) -> torch.Tensor:
+        """One pushed frame: ingest -> features -> single-frame head and decode, W_f / W_b maps -> ring slot; the
+        recurrence over the ring's frames t - 4 .. t -> decode -> selection and remap of frame t - 2 (returned, (K, 3)
+        on the device)."""
+        head, mf = self.head, self.head.head_mf
+        x, bbox = ops.frames_crop_resize_cv2(self._push_frames, self.image_hw, self._box, self.mean, self.std,
+                                             channels_last=self.channels_last, dtype=self.dtype)
+        if self.channels_last:
+            x = x.permute(0, 3, 1, 2)
+        # contiguous: the layout HeatmapMHCRNNHead.forward gives predict_frame's features, so the head runs the same kernels
+        feats = self.features_of(x).contiguous()
+        kp_sf, cf_sf = head.run_subpixelmaxima(head.head_sf(feats))
+        wf, wb = mf._maps(feats)
+        if self._ring_wf is None:
+            self._ring_wf = torch.zeros((ops.CONTEXT_RING_SLOTS, *wf.shape[1:]), dtype=torch.float32, device=self.device)
+            self._ring_wb = torch.zeros_like(self._ring_wf)
+        ops.context_ring_push(wf, wb, kp_sf, cf_sf, bbox, self._ring_wf, self._ring_wb, self._ring_kp, self._ring_cf,
+                              self._ring_box, self._ring_count, self._window)
+        hf = (mf.H_f[0].weight, mf.H_f[0].bias, mf.H_f[1].weight, mf.H_f[1].bias)
+        hb = (mf.H_b[0].weight, mf.H_b[0].bias, mf.H_b[1].weight, mf.H_b[1].bias)
+        kp_mf, cf_mf = head.run_subpixelmaxima(ops.plane_softmax(ops.crnn_combine(self._ring_wf, self._ring_wb, self._window, hf, hb)))
+        return ops.context_ring_select(self._ring_kp, self._ring_cf, self._ring_box, kp_mf, cf_mf, *self.image_hw,
+                                       self._push_row, self._ring_count)
+
+    @torch.no_grad()
+    def _push_call(self, from_host: bool) -> None:
+        """One push's device work on the current stream: staging -> device, the body, result -> pinned buffer."""
+        if from_host:
+            self._push_frames.copy_(self._push_pin_frames, non_blocking=True)
+        self._box.copy_(self._pin_box, non_blocking=True)
+        self._pin_out.copy_(self._push_body(), non_blocking=True)
+
+    def _ring_state(self) -> list[torch.Tensor]:
+        return [t for t in (self._ring_count, self._ring_kp, self._ring_cf, self._ring_box, self._ring_wf, self._ring_wb,
+                            self._window) if t is not None]
+
+    def _prepare_push(self, key) -> None:
+        """Buffers (and with ``use_graph`` the graph) of a push input form: (host?, (1, H, W, 3)).  The warm-up runs
+        advance the ring, so the stream's state is saved before and put back after them."""
+        self._push_key, self._push_graph = key, None
+        from_host, _ = key
+        self._push_frames, self._push_pin_frames = self._staging(key)
+        if not self.use_graph:
+            return
+        saved = [(t, t.clone()) for t in self._ring_state()]
+        graph = self._captured(lambda: self._push_call(from_host))
+        for dst, src in saved:  # maps the first warm-up allocates exist only at t = 0 and are written before they are read
+            dst.copy_(src)
+        self.launches_per_push = _graph_kernel_count(graph)
+        graph.instantiate()
+        self._push_graph = graph
+
+    def push_frame(self, frame_rgb, bbox: tuple[int, int, int, int] | None = None) -> dict:
+        """Stream frame t of a context model in, the prediction of frame t - 2 out (t counts the pushes since the last
+        ``reset_stream``): ``{"keypoints": (K, 2), "confidence": (K,), "frame": t - 2}``, what ``predict_frame`` returns
+        for frames t - 4 .. t when they share one box; ``None`` values for the first four pushes."""
+        if not self.context:
+            raise ValueError(_NO_STREAM)
+        ndim = frame_rgb.ndim if hasattr(frame_rgb, "ndim") else np.ndim(frame_rgb)
+        if ndim == 4:
+            raise ValueError("push_frame takes one (H, W, 3) frame per call; predict_frame takes a (5, H, W, 3) stack")
+        frames, box = self._check(frame_rgb, bbox, stack=False)
+        from_host = not isinstance(frames, torch.Tensor)
+        shape = (1, *frames.shape)
+        if self._push_key != (from_host, shape):
+            self._prepare_push((from_host, shape))
+        self._pin_box.numpy()[:] = box
+        if from_host:
+            np.copyto(self._push_pin_frames.numpy(), frames.reshape(shape))
+        else:
+            self._push_frames.copy_(frames.reshape(shape))
+        if self._push_graph is not None:
+            self._push_graph.replay()
+        else:
+            self._push_call(from_host)
+        torch.cuda.current_stream(self.device).synchronize()
+        t, self._pushed = self._pushed, self._pushed + 1
+        if t < self.CONTEXT_FRAMES - 1:
+            return {"keypoints": None, "confidence": None, "frame": None}
+        out = self._pin_out.numpy()
+        return {"keypoints": out[:, :2].copy(), "confidence": out[:, 2].copy(), "frame": t - 2}
+
+    def reset_stream(self) -> None:
+        """Start a new stream: the next push is its frame 0."""
+        if not self.context:
+            raise ValueError(_NO_STREAM)
+        self._ring_count.zero_()
+        self._pushed = 0
